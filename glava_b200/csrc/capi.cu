@@ -534,12 +534,13 @@ glava_b200* glava_b200_new(const glava_b200_params* params, int batch, int devic
     r->sizereq.store(0);
     { const char* e = getenv("GLAVA_B200_TAP_KU"); r->tap_ku = e ? atoi(e) : 8; }
     r->fused_k5 = getenv("GLAVA_B200_FUSED_K5") != nullptr;
-    // Launch structure of the lazy pipeline-B update (DESIGN 4.1): wherever the need-list K5 runs as its own kernel (auto:
-    // setbufsize >= 8192) the R16 state update does too, and at 8192 the FFT passes run out of place with 256 threads —
-    // the measured optima (tools/variant_sweep.sh).  GLAVA_B200_SPLIT_EPI / _SPEC_OOP / _SPEC_T override.
+    // Launch structure of the lazy pipeline-B update (DESIGN 4.1): wherever the need-list K5 runs as its own kernel (auto: an
+    // FFT size >= 4096, or taps too large for shared memory: build_tables) the R16 state update does too, and at an FFT size
+    // of 8192 the FFT passes run out of place with 256 threads — the measured optima (tools/variant_sweep.sh).  The FFT size
+    // is the one the kernels run at, r->p.n = setbufsize / setbufscale.  GLAVA_B200_SPLIT_EPI / _SPEC_OOP / _SPEC_T override.
     { const char* e = getenv("GLAVA_B200_SPLIT_EPI"); r->split_epilogue = e ? atoi(e) != 0 : true; }
-    { const char* e = getenv("GLAVA_B200_SPEC_OOP"); r->spec_oop = e ? atoi(e) : (params->n == 8192 ? 1 : 0); }
-    { const char* e = getenv("GLAVA_B200_SPEC_T"); r->spec_t = e ? atoi(e) : (params->n == 8192 ? 256 : 0); }
+    { const char* e = getenv("GLAVA_B200_SPEC_OOP"); r->spec_oop = e ? atoi(e) : (r->p.n == 8192 ? 1 : 0); }
+    { const char* e = getenv("GLAVA_B200_SPEC_T"); r->spec_t = e ? atoi(e) : (r->p.n == 8192 ? 256 : 0); }
     r->no_texmm = getenv("GLAVA_B200_NO_TEXMM") != nullptr;
     r->no_coltab = getenv("GLAVA_B200_NO_COLTAB") != nullptr;
     r->kcounter = 0; r->d_scaled[0] = r->d_scaled[1] = nullptr; r->d_key[0] = r->d_key[1] = r->d_key[2] = nullptr;

@@ -47,6 +47,20 @@ static int device_sm_count() {
     return n > 0 ? n : 132;                              // H100 SXM
 }
 
+// grid.y is limited to 65535 and a batch is not (glava_b200_new takes any batch >= 1): a launcher whose y axis counts planes,
+// streams or groups of planes launches slices of at most that many rows, each told its first row (launch_raster chunks its
+// batch axis the same way).  `launch(y0, rows)` enqueues one slice.
+constexpr int GRID_Y_MAX = 65535;
+template <class Launch>
+static cudaError_t launch_y_slices(int rows, Launch launch) {
+    for (int y0 = 0; y0 < rows; y0 += GRID_Y_MAX) {
+        launch(y0, (unsigned) min(GRID_Y_MAX, rows - y0));
+        const cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return e;
+    }
+    return cudaSuccess;
+}
+
 // ---------------------------------------------------------------------------------------------
 // spectrum kernel
 constexpr int spec_default_threads(int log2n) {
@@ -531,11 +545,11 @@ int launch_spectrum(const glava_b200_params& p, const SpectrumArgs& a, bool is_f
 #define K5_XT 128
 __global__ void __launch_bounds__(K5_XT)
 k5_planes_kernel(const uint16_t* __restrict__ in, uint16_t* __restrict__ out, int n, int count,
-                 const __grid_constant__ glava_b200_params p) {
+                 const __grid_constant__ glava_b200_params p, int y0) {
     uint16_t* seg = reinterpret_cast<uint16_t*>(glb_smem);           // [K5_S][span]
     const SmoothParams sp = smooth_params(p);
     const int x0 = blockIdx.x * K5_XT, x1 = min(n, x0 + K5_XT);
-    const int pl0 = blockIdx.y * K5_S, npl = min(K5_S, count - pl0);
+    const int pl0 = (y0 + (int) blockIdx.y) * K5_S, npl = min(K5_S, count - pl0);
     // input index range any tap of this block's texels can touch (scale_audio is increasing)
     const float fn = (float) n;
     const float lo_f = scale_audio(sp, g_clamp(((float) x0 + 0.5f) / fn - sp.smooth_factor, 0.0f, 1.0f)) * fn;
@@ -574,11 +588,11 @@ static_assert(K5_S == K5_S_PLANES && K5_XT == K5_BLOCK, "K5 table layout and ker
 template <bool AVG_ONLY, int S>
 __global__ void __launch_bounds__(K5_BLOCK)
 k5_table_kernel(const uint16_t* __restrict__ in, uint16_t* __restrict__ out, int n, int count, const K5Table tb,
-                const SmoothParams sp, int plane_stride, int plane_offset) {
+                const SmoothParams sp, int plane_stride, int plane_offset, int y0) {
     float* seg = reinterpret_cast<float*>(glb_smem);                  // [S][span] texels as float
     const int4 d = __ldg(tb.blk + blockIdx.x);
     const int base = d.x, taps = d.y, lo = d.z, span = d.w;
-    const int pl0 = blockIdx.y * S, npl = min(S, count - pl0);
+    const int pl0 = (y0 + (int) blockIdx.y) * S, npl = min(S, count - pl0);
     for (int i = threadIdx.x; i < S * span; i += K5_BLOCK) {
         const int pl = i / span, k = i - pl * span;
         seg[i] = pl < npl ? from16(in[((size_t) (pl0 + pl) * plane_stride + plane_offset) * n + lo + k]) : 0.0f;
@@ -619,9 +633,10 @@ static int launch_k5_table_t(const glava_b200_params& p, const uint16_t* d_in, u
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
         if (e != cudaSuccess) return fail(GLAVA_B200_ECUDA, "cudaFuncSetAttribute(k5 table): %s", cudaGetErrorString(e));
     }
-    dim3 grid((tb.count + K5_BLOCK - 1) / K5_BLOCK, (count + S - 1) / S);
-    kern<<<grid, K5_BLOCK, smem, st>>>(d_in, d_out, p.n, count, tb, sp, plane_stride, plane_offset);
-    cudaError_t e = cudaGetLastError();
+    const unsigned gx = (tb.count + K5_BLOCK - 1) / K5_BLOCK;
+    cudaError_t e = launch_y_slices((count + S - 1) / S, [&](int y0, unsigned rows) {
+        kern<<<dim3(gx, rows), K5_BLOCK, smem, st>>>(d_in, d_out, p.n, count, tb, sp, plane_stride, plane_offset, y0);
+    });
     if (e != cudaSuccess) return fail(GLAVA_B200_ECUDA, "smooth (table) kernel launch: %s", cudaGetErrorString(e));
     return 0;
 }
@@ -661,9 +676,10 @@ int launch_smooth_only(const glava_b200_params& p, const uint16_t* d_in, uint16_
         cudaError_t e = cudaFuncSetAttribute(k5_planes_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
         if (e != cudaSuccess) return fail(GLAVA_B200_ECUDA, "cudaFuncSetAttribute(k5): %s", cudaGetErrorString(e));
     }
-    dim3 grid((p.n + K5_XT - 1) / K5_XT, (count + K5_S - 1) / K5_S);
-    k5_planes_kernel<<<grid, K5_XT, smem, (cudaStream_t) stream>>>(d_in, d_out, p.n, count, p);
-    cudaError_t e = cudaGetLastError();
+    const unsigned gx = (p.n + K5_XT - 1) / K5_XT;
+    cudaError_t e = launch_y_slices((count + K5_S - 1) / K5_S, [&](int y0, unsigned rows) {
+        k5_planes_kernel<<<dim3(gx, rows), K5_XT, smem, (cudaStream_t) stream>>>(d_in, d_out, p.n, count, p, y0);
+    });
     if (e != cudaSuccess) return fail(GLAVA_B200_ECUDA, "smooth kernel launch: %s", cudaGetErrorString(e));
     return 0;
 }
@@ -682,8 +698,8 @@ int launch_smooth_only(const glava_b200_params& p, const uint16_t* d_in, uint16_
 // Arithmetic = the in-kernel epilogue's (gravity_b, newest-first weighted average), bit for bit.
 template <int FT>
 __global__ void __launch_bounds__(128)
-epilogue_b_kernel(const __grid_constant__ SpectrumArgs a, int n, int bins, int F, float diff) {
-    const int plane = blockIdx.y, g8 = blockIdx.x * blockDim.x + threadIdx.x;
+epilogue_b_kernel(const __grid_constant__ SpectrumArgs a, int n, int bins, int F, float diff, int y0) {
+    const int plane = y0 + (int) blockIdx.y, g8 = blockIdx.x * blockDim.x + threadIdx.x;
     const int n0 = g8 * 8;
     if (n0 >= bins) return;
     const uint32_t um = a.umask ? __ldg(a.umask + (plane >> 1)) : 0x80000000u;
@@ -736,18 +752,19 @@ epilogue_b_kernel(const __grid_constant__ SpectrumArgs a, int n, int bins, int F
 int launch_epilogue_b(const glava_b200_params& p, const SpectrumArgs& a, int bins, void* stream) {
     const int planes = a.batch * 2, F = p.avg_frames;
     const float diff = p.gravity_step * (1.0f / p.ur);
-    dim3 grid((bins / 8 + 127) / 128, planes);
+    const unsigned gx = (bins / 8 + 127) / 128;
     cudaStream_t st = (cudaStream_t) stream;
-#define GLB_EPI(FT) epilogue_b_kernel<FT><<<grid, 128, 0, st>>>(a, p.n, bins, F, diff)
-    switch (F) {
-        case 5: GLB_EPI(5); break;                              // shipped default (smooth_parameters.glsl:56)
-        case 6: GLB_EPI(6); break;                              // compiled-in default (render.c:912)
-        case 3: GLB_EPI(3); break;
-        case 4: GLB_EPI(4); break;
-        default: GLB_EPI(0); break;
-    }
+    cudaError_t e = launch_y_slices(planes, [&](int y0, unsigned rows) {
+#define GLB_EPI(FT) epilogue_b_kernel<FT><<<dim3(gx, rows), 128, 0, st>>>(a, p.n, bins, F, diff, y0)
+        switch (F) {
+            case 5: GLB_EPI(5); break;                          // shipped default (smooth_parameters.glsl:56)
+            case 6: GLB_EPI(6); break;                          // compiled-in default (render.c:912)
+            case 3: GLB_EPI(3); break;
+            case 4: GLB_EPI(4); break;
+            default: GLB_EPI(0); break;
+        }
 #undef GLB_EPI
-    cudaError_t e = cudaGetLastError();
+    });
     if (e != cudaSuccess) return fail(GLAVA_B200_ECUDA, "epilogue kernel launch: %s", cudaGetErrorString(e));
     return 0;
 }
@@ -968,8 +985,8 @@ int launch_k5_need(const glava_b200_params& p, const uint16_t* d_av, float* d_av
 template <bool FLOAT_IN>
 __global__ void fifo_ingest_kernel(const void* __restrict__ chunks, int frames, int n, int channels,
                                    const float* __restrict__ src_l, const float* __restrict__ src_r,
-                                   float* __restrict__ dst_l, float* __restrict__ dst_r) {
-    const int s = blockIdx.y;
+                                   float* __restrict__ dst_l, float* __restrict__ dst_r, int y0) {
+    const int s = y0 + (int) blockIdx.y;
     const size_t base = (size_t) s * n;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         float l, r;
@@ -993,11 +1010,13 @@ __global__ void fifo_ingest_kernel(const void* __restrict__ chunks, int frames, 
 }
 int launch_fifo_ingest(const glava_b200_params& p, const void* d_chunks, bool float_in, int frames, const float* src_l, const float* src_r,
                        float* dst_l, float* dst_r, int batch, void* stream) {
-    dim3 grid((p.n + 1023) / 1024, batch);
+    const unsigned gx = (p.n + 1023) / 1024;
     const int chans = (p.mirror_input || p.channels == 1) ? 1 : 2;       // the AUDIO side's mono mix (setmirror), not the shader's _CHANNELS
-    if (float_in) fifo_ingest_kernel<true><<<grid, 256, 0, (cudaStream_t) stream>>>(d_chunks, frames, p.n, chans, src_l, src_r, dst_l, dst_r);
-    else fifo_ingest_kernel<false><<<grid, 256, 0, (cudaStream_t) stream>>>(d_chunks, frames, p.n, chans, src_l, src_r, dst_l, dst_r);
-    cudaError_t e = cudaGetLastError();
+    cudaStream_t st = (cudaStream_t) stream;
+    cudaError_t e = launch_y_slices(batch, [&](int y0, unsigned rows) {
+        if (float_in) fifo_ingest_kernel<true><<<dim3(gx, rows), 256, 0, st>>>(d_chunks, frames, p.n, chans, src_l, src_r, dst_l, dst_r, y0);
+        else fifo_ingest_kernel<false><<<dim3(gx, rows), 256, 0, st>>>(d_chunks, frames, p.n, chans, src_l, src_r, dst_l, dst_r, y0);
+    });
     if (e != cudaSuccess) return fail(GLAVA_B200_ECUDA, "fifo ingest kernel launch: %s", cudaGetErrorString(e));
     return 0;
 }

@@ -7,23 +7,56 @@ import pytest
 import glava_b200 as g
 from oracle.oracle import OracleChannel, params_from
 from tests import emul
+from tests.pcm import EDGE_SIGNALS, edge_signal, fft_magnitude_error, fft_ramp
 
 
 def _tex(n, seed):
     return (np.random.default_rng(seed).random(n) ** 2 * 65535).astype(np.uint16)
 
 
-@pytest.mark.parametrize("n", [256, 512, 1024, 2048, 4096, 8192, 16384])
+FFT_SIZES = [256, 512, 1024, 2048, 4096, 8192, 16384]
+
+
+def transform_fft_numpy(x):
+    """render.c:783-847 in float64 with numpy: window macro cos(TWOPI*i/N - 1) with TWOPI = 6.28318530718 (render.c:660,794),
+    the windowed sample rounded to float, the packed (N/2)-point complex transform, |Re| and |Im| interleaved, log, ramp"""
+    n = x.shape[0]
+    i = np.arange(n, dtype=np.float64)
+    xw = (x.astype(np.float64) * (0.53836 - 0.46164 * np.cos(6.28318530718 * i / n - 1))).astype(np.float32).astype(np.float64)
+    z = np.fft.fft(xw[0::2] + 1j * xw[1::2])
+    mag = np.empty(n); mag[0::2] = np.abs(z.real); mag[1::2] = np.abs(z.imag)
+    return np.log(mag + 1) / 3 * fft_ramp(n)
+
+
+@pytest.mark.parametrize("n", FFT_SIZES)
+def test_oracle_fft_f64_is_render_c_transform(orc_pm, n, built):
+    """anchor: the oracle's float64 evaluation equals an independent numpy restatement of transform_fft"""
+    op = params_from(g.default_params("bars", n=n))
+    for kind in ("noise", "impulse_last", "tone_half_bin"):
+        x = edge_signal(kind, n)
+        want = transform_fft_numpy(x)
+        assert np.abs(orc_pm.fft_f64(op, x) - want).max() <= 1e-12 * max(want.max(), 1.0), kind
+
+
+@pytest.mark.parametrize("n", FFT_SIZES)
 def test_stockham_fft_vs_reference_restatement(orc_pm, n, built):
+    """every edge signal (tests/pcm.py): silence gives exact zeros, everything else is within 2e-6 of the peak |X| of
+    exact arithmetic (and, for noise, of the peak output)"""
     p = g.default_params("bars", n=n); op = params_from(p)
-    x = (np.random.default_rng(n).standard_normal(n) * 0.2).astype(np.float32)
-    got = emul.fft(x)
-    f32 = orc_pm.fft_f32(op, x); f64 = orc_pm.fft_f64(op, x)
-    # north_star tolerance: 1e-5 of peak against render.c's transform.  The reference's own float
-    # twiddle recurrence is 1.2e-5 / 1.6e-5 away from exact arithmetic at N = 8192 / 16384 (SURVEY §7),
-    # so above 4096 the bar is 1e-5 against the float64 evaluation and 2.5e-5 against the float32 one.
-    assert np.abs(got - f64).max() / f64.max() <= 2e-6
-    assert np.abs(got - f32).max() / f32.max() <= (1e-5 if n <= 4096 else 2.5e-5)
+    for signal in EDGE_SIGNALS:
+        x = edge_signal(signal, n)
+        got = emul.fft(x)
+        f32 = orc_pm.fft_f32(op, x); f64 = orc_pm.fft_f64(op, x)
+        if signal == "silence":
+            assert not got.any() and not f64.any()
+            continue
+        # north_star tolerance: 1e-5 of peak against render.c's transform.  The reference's own float
+        # twiddle recurrence is 1.2e-5 / 1.6e-5 away from exact arithmetic at N = 8192 / 16384 (SURVEY §7),
+        # so above 4096 the bar is 1e-5 against the float64 evaluation and 2.5e-5 against the float32 one.
+        assert fft_magnitude_error(got, f64) <= 2e-6, signal
+        if signal == "noise":
+            assert np.abs(got - f64).max() / f64.max() <= 2e-6
+            assert np.abs(got - f32).max() / f32.max() <= (1e-5 if n <= 4096 else 2.5e-5)
 
 
 @pytest.mark.parametrize("accel", [0, 1])
