@@ -13,9 +13,9 @@ There is no CPU fallback: constructing a Renderer without the CUDA library or wi
 raises.
 """
 from .api import (Params, Color, Renderer, GlavaError, default_params, load_config, lib, lib_path,
-                  MODULES, pinned_empty, Pipe, ShardedRenderer)
+                  MODULES, pinned_empty, Pipe, ShardedRenderer, stream_state_bytes, STATE_HEADER_BYTES)
 from . import audio
 from .synth import synth_pcm_int16, fifo_to_float, StreamRings
 
 __all__ = ["audio", "Params", "Color", "Renderer", "GlavaError", "default_params", "load_config", "lib",
-           "lib_path", "MODULES", "pinned_empty", "Pipe", "ShardedRenderer", "synth_pcm_int16", "fifo_to_float", "StreamRings"]
+           "lib_path", "MODULES", "pinned_empty", "Pipe", "ShardedRenderer", "stream_state_bytes", "STATE_HEADER_BYTES", "synth_pcm_int16", "fifo_to_float", "StreamRings"]

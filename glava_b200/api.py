@@ -208,6 +208,14 @@ def lib():
     L.glava_b200_pipe_bind.argtypes = [vp, i32, C.POINTER(cp), C.POINTER(cp), C.POINTER(C.c_float)]
     L.glava_b200_pipe_apply.argtypes = [vp, vp]
     L.glava_b200_pipe_free.argtypes = [vp]
+    L.glava_b200_stream_state_bytes.restype = C.c_size_t
+    L.glava_b200_stream_state_bytes.argtypes = [C.POINTER(Params)]
+    L.glava_b200_reset_streams.argtypes = [vp, vp]
+    L.glava_b200_save_streams.argtypes = [vp, vp, i32, vp]
+    L.glava_b200_load_streams.argtypes = [vp, vp, i32, vp]
+    L.glava_b200_sharded_reset_streams.argtypes = [vp, vp]
+    L.glava_b200_sharded_save_streams.argtypes = [vp, vp, i32, vp]
+    L.glava_b200_sharded_load_streams.argtypes = [vp, vp, i32, vp]
     _lib = L
     # errors surface as Python exceptions; keep stderr quiet
     _quiet = C.CFUNCTYPE(None, cp)(lambda msg: None)
@@ -229,6 +237,47 @@ def default_params(module="bars", **overrides):
             v = type(getattr(p, k))(*v)
         setattr(p, k, v)
     return p
+
+
+STATE_HEADER_BYTES = 4096        # GLAVA_B200_STATE_HEADER_BYTES
+
+
+def stream_state_bytes(params):
+    """bytes of one stream's state blob for renderers created with `params` (glava_b200_stream_state_bytes); raises while
+    keyframe interpolation is active"""
+    n = lib().glava_b200_stream_state_bytes(C.byref(params))
+    if n == 0:
+        raise GlavaError(lib().glava_b200_last_error().decode(errors="replace"))
+    return int(n)
+
+
+class _StreamState:
+    """reset_streams / save_streams / load_streams over the handle's C entry points (self._fn: their names)"""
+
+    def _stream_list(self, streams):
+        s = np.ascontiguousarray(np.asarray(streams, dtype=np.int64).reshape(-1), dtype=np.int32)
+        assert s.ndim == 1
+        return s
+
+    def reset_streams(self, mask):
+        """streams with mask[s] != 0 start fresh: from their next update on, what a new batch-1 renderer renders"""
+        m = np.ascontiguousarray(np.asarray(mask) != 0, dtype=np.uint8)
+        assert m.shape == (self.batch,), m.shape
+        _check(self._fn[0](self._h, m.ctypes.data))
+
+    def save_streams(self, streams):
+        """-> uint8 [len(streams)][stream_state_bytes] blobs of the listed streams' state"""
+        s = self._stream_list(streams)
+        out = np.empty((s.shape[0], stream_state_bytes(self.params)), np.uint8)
+        _check(self._fn[1](self._h, s.ctypes.data, s.shape[0], out.ctypes.data))
+        return out
+
+    def load_streams(self, streams, blobs):
+        """put blobs from save_streams (same effective parameters, any renderer) into the listed streams"""
+        s = self._stream_list(streams)
+        b = np.ascontiguousarray(blobs, dtype=np.uint8)
+        assert b.shape == (s.shape[0], stream_state_bytes(self.params)), b.shape
+        _check(self._fn[2](self._h, s.ctypes.data, s.shape[0], b.ctypes.data))
 
 
 def _cstr_array(items):
@@ -314,8 +363,12 @@ def pinned_empty(shape, dtype, device=None):
     return np.frombuffer(buf, dtype=dtype).reshape(shape)
 
 
-class Renderer:
+class Renderer(_StreamState):
     """Batched renderer handle: the role of struct glava_renderer (render.h:8-30)."""
+
+    @property
+    def _fn(self):
+        return self._L.glava_b200_reset_streams, self._L.glava_b200_save_streams, self._L.glava_b200_load_streams
 
     def __init__(self, params, batch=1, device=0):
         self._L = lib()
@@ -527,9 +580,15 @@ class Renderer:
         except Exception: pass
 
 
-class ShardedRenderer:
+class ShardedRenderer(_StreamState):
     """One handle for a batch spread over several GPUs of a node (glava_b200_new_sharded): contiguous stream blocks, one
-    worker thread per device, no inter-device traffic.  devices: list of CUDA ordinals (may repeat), or None = all visible."""
+    worker thread per device, no inter-device traffic.  devices: list of CUDA ordinals (may repeat), or None = all visible.
+    reset_streams / save_streams / load_streams take global stream indices."""
+
+    @property
+    def _fn(self):
+        return (self._L.glava_b200_sharded_reset_streams, self._L.glava_b200_sharded_save_streams,
+                self._L.glava_b200_sharded_load_streams)
 
     def __init__(self, params, batch, devices=None):
         self._L = lib()

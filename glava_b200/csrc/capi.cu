@@ -8,6 +8,7 @@
 #include "raster_core.h"
 #include "chain_core.h"
 #include "tables.h"
+#include "stream_state_core.h"
 
 #include <cuda_runtime.h>
 
@@ -113,6 +114,11 @@ struct glava_b200 {
     bool desync;
     std::vector<uint32_t> cursor;          // [batch] modified updates of that stream so far, mod avg_frames (valid once desync)
     uint32_t* h_umask[4]; uint32_t* d_umask[4]; cudaEvent_t ev_umask[4]; int umask_cur;
+    // per-stream state I/O (glava_b200_save_streams / _load_streams / _reset_streams): two device staging halves, each
+    // [chunk table: int stream[k], uint32 cursor[k]][blob segments of k streams], allocated on first use; the tables go up
+    // from pinned host buffers.  ev_sst_copied[i]: the H2D copies into half i are done; ev_sst_free[i]: its kernel and D2H
+    // copies are done
+    void* d_sst[2]; int* h_sst[2]; cudaEvent_t ev_sst_copied[2], ev_sst_free[2]; int sst_cur, sst_streams; size_t sst_table;
     uint64_t launches;
     std::vector<void*> allocs;
     // optional per-kernel device timing (glava_b200_set_timing): events around each launch
@@ -563,6 +569,8 @@ glava_b200* glava_b200_new(const glava_b200_params* params, int batch, int devic
     r->updates = 0; r->launches = 0; r->timing = false;
     r->desync = false; r->umask_cur = 0; r->async_input = false; r->last_in = -1; r->ev_input = nullptr;
     for (int i = 0; i < 4; ++i) { r->h_umask[i] = nullptr; r->d_umask[i] = nullptr; r->ev_umask[i] = nullptr; }
+    for (int i = 0; i < 2; ++i) { r->d_sst[i] = nullptr; r->h_sst[i] = nullptr; r->ev_sst_copied[i] = r->ev_sst_free[i] = nullptr; }
+    r->sst_cur = 0; r->sst_streams = 0; r->sst_table = 0;
     if (build(r) != 0) { glava_b200_destroy(r); return nullptr; }
     return r;
 }
@@ -585,6 +593,13 @@ void glava_b200_destroy(glava_b200* r) {
         if (r->ev_umask[i]) cudaEventDestroy(r->ev_umask[i]);
     }
     if (r->ev_input) cudaEventDestroy(r->ev_input);
+    if (r->copy_stream) cudaStreamSynchronize(r->copy_stream);
+    for (int i = 0; i < 2; ++i) {
+        if (r->d_sst[i]) cudaFree(r->d_sst[i]);
+        if (r->h_sst[i]) cudaFreeHost(r->h_sst[i]);
+        if (r->ev_sst_copied[i]) cudaEventDestroy(r->ev_sst_copied[i]);
+        if (r->ev_sst_free[i]) cudaEventDestroy(r->ev_sst_free[i]);
+    }
     if (r->copy_stream) cudaStreamDestroy(r->copy_stream);
     if (r->out_stream) { cudaStreamSynchronize(r->out_stream); cudaStreamDestroy(r->out_stream); }
     for (int i = 0; i < 2; ++i) {
@@ -1219,6 +1234,230 @@ int glava_b200_transform_smooth(glava_b200* r, float* planes, int count) {
     } while (0);
     cudaFree(d);
     return rc;
+}
+
+}  // extern "C"
+
+// ---- lifetime of individual streams: reset, save, load (DESIGN.md §4.8) ---------------------------------------------------
+static_assert(GLB_STATE_HEADER_BYTES == GLAVA_B200_STATE_HEADER_BYTES, "one header size");
+static_assert(sizeof(StateHeader) + sizeof(glava_b200_params) <= GLB_STATE_HEADER_BYTES, "header holds the parameters");
+static const size_t kStateStageBytes = (size_t) 16 << 20;   // blob segments per staging half (two halves)
+enum { SS_SAVE = 0, SS_LOAD = 1, SS_RESET = 2 };
+
+static StateLayout state_layout(const glava_b200_params& p, int n_in) {
+    StateLayout L;
+    L.n = p.n; L.n_in = n_in; L.F = p.avg_frames; L.esz = p.accel_fft ? 2 : 4;
+    L.chans = p.module == GLAVA_B200_MOD_WAVE ? 1 : 2;
+    return L;
+}
+
+// The parameters a blob records and is checked against: the effective ones, fb_slots zeroed (it sizes no stream's state)
+static void state_params(const glava_b200* r, glava_b200_params* out) {
+    memset(out, 0, sizeof(*out));
+    memcpy(out, &r->p, sizeof(*out));
+    out->fb_slots = 0;
+}
+
+static int state_unavailable(const char* who) {
+    return fail(GLAVA_B200_EINVAL, "%s: not available with keyframe interpolation active (setinterpolate): the keyframe rotation "
+                                   "is per renderer", who);
+}
+
+static int state_check_streams(const glava_b200* r, const int* streams, int count, const char* who) {
+    if (count < 0 || (count > 0 && !streams)) return fail(GLAVA_B200_EINVAL, "%s: bad arguments", who);
+    std::vector<char> seen((size_t) r->batch, 0);
+    for (int i = 0; i < count; ++i) {
+        const int s = streams[i];
+        if (s < 0 || s >= r->batch) return fail(GLAVA_B200_EINVAL, "%s: stream %d out of range (batch %d)", who, s, r->batch);
+        if (seen[(size_t) s]) return fail(GLAVA_B200_EINVAL, "%s: stream %d listed twice", who, s);
+        seen[(size_t) s] = 1;
+    }
+    return 0;
+}
+
+namespace glb {
+int state_check_blobs(const glava_b200* r, const void* const* blobs, int count, const char* who) {
+    const StateLayout L = state_layout(r->p, r->n_in);
+    glava_b200_params want;
+    state_params(r, &want);
+    for (int i = 0; i < count; ++i) {
+        if (!blobs[i]) return fail(GLAVA_B200_EINVAL, "%s: blob %d is null", who, i);
+        StateHeader h;
+        memcpy(&h, blobs[i], sizeof(h));
+        if (h.magic != GLB_STATE_MAGIC) return fail(GLAVA_B200_EINVAL, "%s: blob %d is not a stream state (bad magic)", who, i);
+        if (h.version != GLB_STATE_VERSION)
+            return fail(GLAVA_B200_EINVAL, "%s: blob %d has format version %u, this library reads %u", who, i, h.version, GLB_STATE_VERSION);
+        if (h.header_bytes != GLB_STATE_HEADER_BYTES || h.params_bytes != sizeof(glava_b200_params) || h.blob_bytes != ss_blob_bytes(L))
+            return fail(GLAVA_B200_EINVAL, "%s: blob %d has the wrong size (%llu bytes, this renderer's streams take %zu)", who, i,
+                        (unsigned long long) h.blob_bytes, ss_blob_bytes(L));
+        if (memcmp((const char*) blobs[i] + sizeof(StateHeader), &want, sizeof(want)) != 0)
+            return fail(GLAVA_B200_EINVAL, "%s: blob %d was saved from a renderer with other parameters", who, i);
+    }
+    return 0;
+}
+}  // namespace glb
+
+// device staging, allocated on first use: halves of up to kStateStageBytes of segments plus the chunk table
+static int state_staging(glava_b200* r, const StateLayout& L) {
+    if (r->d_sst[0]) return 0;
+    const size_t seg = ss_segment_bytes(L);
+    size_t k = kStateStageBytes / seg;
+    if (k < 1) k = 1;
+    if (k > (size_t) r->batch) k = (size_t) r->batch;
+    r->sst_streams = (int) k;
+    r->sst_table = (k * 8 + 255) / 256 * 256;
+    for (int i = 0; i < 2; ++i) {
+        CU(cudaMalloc(&r->d_sst[i], r->sst_table + k * seg));
+        CU(cudaHostAlloc((void**) &r->h_sst[i], k * 8, cudaHostAllocDefault));
+        CU(cudaEventCreateWithFlags(&r->ev_sst_copied[i], cudaEventDisableTiming));
+        CU(cudaEventCreateWithFlags(&r->ev_sst_free[i], cudaEventDisableTiming));
+    }
+    return 0;
+}
+
+// Save / load / reset of the listed streams in chunks of at most sst_streams.  Kernels and D2H copies run on spec_stream
+// (where every update reads and writes this state, in issue order); the H2D copies of load and reset run on copy_stream, so
+// the host waits for copies only, never for earlier kernels.  Reset and load write the texture half the last raster may still
+// read: spec_stream waits for that raster on the device.
+static int state_io(glava_b200* r, int op, const int* streams, int count, void* const* out, const void* const* in) {
+    const StateLayout L = state_layout(r->p, r->n_in);
+    const size_t seg = ss_segment_bytes(L), blob = ss_blob_bytes(L);
+    int rc;
+    if (count == 0) return 0;
+    if ((rc = state_staging(r, L)) != 0) return rc;
+    StatePtrs P;
+    P.gravity = (char*) (r->p.accel_fft ? (void*) r->d_gr_store : (void*) r->d_applied);
+    P.ring = (char*) (r->p.accel_fft ? (void*) r->d_ring_u : (void*) r->d_ring_f);
+    P.spec = (char*) r->d_spec; P.tex = (char*) tex_half(r, r->tex_cur); P.av = (char*) r->d_av;
+    P.fifo[0] = (char*) r->d_ring[r->ring_cur][0]; P.fifo[1] = (char*) r->d_ring[r->ring_cur][1];
+    CU(cudaStreamWaitEvent(r->spec_stream, r->ev_raster_done[r->tex_cur], 0));
+    const uint32_t F = (uint32_t) r->p.avg_frames;
+    int last = -1;
+    for (int c0 = 0; c0 < count; c0 += r->sst_streams) {
+        const int k = r->sst_cur, cnt = count - c0 < r->sst_streams ? count - c0 : r->sst_streams;
+        r->sst_cur ^= 1; last = k;
+        CU(cudaEventSynchronize(r->ev_sst_copied[k]));          // the last table copy out of h_sst[k] (two chunks ago)
+        int* tab = r->h_sst[k];
+        for (int i = 0; i < cnt; ++i) {
+            const int s = streams[c0 + i];
+            tab[i] = s;
+            tab[cnt + i] = (int) (r->desync ? r->cursor[(size_t) s] : (uint32_t) (r->updates % (unsigned long long) F));
+        }
+        char* d_tab = (char*) r->d_sst[k];
+        char* d_seg = d_tab + r->sst_table;
+        cudaStream_t up = op == SS_SAVE ? r->spec_stream : r->copy_stream;
+        if (op != SS_SAVE) CU(cudaStreamWaitEvent(up, r->ev_sst_free[k], 0));
+        CU(cudaMemcpyAsync(d_tab, tab, (size_t) cnt * 8, cudaMemcpyHostToDevice, up));
+        if (op == SS_LOAD) {
+            // runs of blobs adjacent in host memory go up as one strided copy each
+            for (int i = 0; i < cnt;) {
+                int j = i + 1;
+                while (j < cnt && (const char*) in[c0 + j] == (const char*) in[c0 + j - 1] + blob) ++j;
+                CU(cudaMemcpy2DAsync(d_seg + (size_t) i * seg, seg, (const char*) in[c0 + i] + GLB_STATE_HEADER_BYTES, blob, seg,
+                                     (size_t) (j - i), cudaMemcpyHostToDevice, up));
+                i = j;
+            }
+        }
+        CU(cudaEventRecord(r->ev_sst_copied[k], up));
+        if (op != SS_SAVE) CU(cudaStreamWaitEvent(r->spec_stream, r->ev_sst_copied[k], 0));
+        if (op == SS_SAVE) rc = launch_state_pack(L, P, (const int*) d_tab, cnt, d_seg, r->spec_stream);
+        else rc = launch_state_unpack(L, P, (const int*) d_tab, cnt, op == SS_LOAD ? d_seg : nullptr, r->spec_stream);
+        if (rc) return rc;
+        ++r->launches;
+        if (op == SS_SAVE) {
+            for (int i = 0; i < cnt;) {
+                int j = i + 1;
+                while (j < cnt && (char*) out[c0 + j] == (char*) out[c0 + j - 1] + blob) ++j;
+                CU(cudaMemcpy2DAsync((char*) out[c0 + i] + GLB_STATE_HEADER_BYTES, blob, d_seg + (size_t) i * seg, seg, seg,
+                                     (size_t) (j - i), cudaMemcpyDeviceToHost, r->spec_stream));
+                i = j;
+            }
+        }
+        CU(cudaEventRecord(r->ev_sst_free[k], r->spec_stream));
+    }
+    if (last < 0) return 0;
+    if (op == SS_SAVE) {
+        CU(cudaEventSynchronize(r->ev_sst_free[last]));
+    } else {
+        // a raster-only update after this call waits for ev_spec_done[tex_cur]: move it behind the new texture contents
+        CU(cudaEventRecord(r->ev_spec_done[r->tex_cur], r->spec_stream));
+        if (op == SS_LOAD) CU(cudaEventSynchronize(r->ev_sst_copied[last]));   // copy_stream runs in order: every blob is consumed
+    }
+    return 0;
+}
+
+namespace glb {
+int state_save_ptrs(glava_b200* r, const int* streams, int count, void* const* blobs) {
+    const char* who = "glava_b200_save_streams";
+    if (r->interp_on) return state_unavailable(who);
+    int rc = state_check_streams(r, streams, count, who);
+    if (rc) return rc;
+    for (int i = 0; i < count; ++i) if (!blobs[i]) return fail(GLAVA_B200_EINVAL, "%s: null blob", who);
+    CU(cudaSetDevice(r->device));
+    const StateLayout L = state_layout(r->p, r->n_in);
+    StateHeader h;
+    memset(&h, 0, sizeof(h));
+    h.magic = GLB_STATE_MAGIC; h.version = GLB_STATE_VERSION; h.header_bytes = GLB_STATE_HEADER_BYTES;
+    h.params_bytes = sizeof(glava_b200_params); h.blob_bytes = ss_blob_bytes(L);
+    glava_b200_params q;
+    state_params(r, &q);
+    for (int i = 0; i < count; ++i) {
+        char* b = (char*) blobs[i];
+        memset(b, 0, GLB_STATE_HEADER_BYTES);
+        memcpy(b, &h, sizeof(h));
+        memcpy(b + sizeof(h), &q, sizeof(q));
+    }
+    return state_io(r, SS_SAVE, streams, count, blobs, nullptr);
+}
+int state_load_ptrs(glava_b200* r, const int* streams, int count, const void* const* blobs) {
+    const char* who = "glava_b200_load_streams";
+    if (r->interp_on) return state_unavailable(who);
+    int rc = state_check_streams(r, streams, count, who);
+    if (rc) return rc;
+    if ((rc = state_check_blobs(r, blobs, count, who)) != 0) return rc;
+    CU(cudaSetDevice(r->device));
+    return state_io(r, SS_LOAD, streams, count, nullptr, blobs);
+}
+}  // namespace glb
+
+extern "C" {
+
+size_t glava_b200_stream_state_bytes(const glava_b200_params* p) {
+    clear_error();
+    if (!p) { fail(GLAVA_B200_EINVAL, "glava_b200_stream_state_bytes: null argument"); return 0; }
+    if (validate_params(p) != 0) return 0;
+    glava_b200 probe; probe.p_user = *p; derive(&probe);
+    if (probe.interp_on) { state_unavailable("glava_b200_stream_state_bytes"); return 0; }
+    return ss_blob_bytes(state_layout(probe.p, probe.n_in));
+}
+
+int glava_b200_reset_streams(glava_b200* r, const uint8_t* mask) {
+    clear_error();
+    if (!r || !mask) return fail(GLAVA_B200_EINVAL, "glava_b200_reset_streams: null argument");
+    if (r->interp_on) return state_unavailable("glava_b200_reset_streams");
+    std::vector<int> list;
+    for (int s = 0; s < r->batch; ++s) if (mask[s]) list.push_back(s);
+    if (list.empty()) return 0;
+    CU(cudaSetDevice(r->device));
+    return state_io(r, SS_RESET, list.data(), (int) list.size(), nullptr, nullptr);
+}
+
+int glava_b200_save_streams(glava_b200* r, const int* streams, int count, void* blobs) {
+    clear_error();
+    if (!r || (count > 0 && !blobs)) return fail(GLAVA_B200_EINVAL, "glava_b200_save_streams: null argument");
+    const size_t bytes = ss_blob_bytes(state_layout(r->p, r->n_in));
+    std::vector<void*> ptrs(count > 0 ? (size_t) count : 0);
+    for (size_t i = 0; i < ptrs.size(); ++i) ptrs[i] = (char*) blobs + i * bytes;
+    return state_save_ptrs(r, streams, count, ptrs.data());
+}
+
+int glava_b200_load_streams(glava_b200* r, const int* streams, int count, const void* blobs) {
+    clear_error();
+    if (!r || (count > 0 && !blobs)) return fail(GLAVA_B200_EINVAL, "glava_b200_load_streams: null argument");
+    const size_t bytes = ss_blob_bytes(state_layout(r->p, r->n_in));
+    std::vector<const void*> ptrs(count > 0 ? (size_t) count : 0);
+    for (size_t i = 0; i < ptrs.size(); ++i) ptrs[i] = (const char*) blobs + i * bytes;
+    return state_load_ptrs(r, streams, count, ptrs.data());
 }
 
 }  // extern "C"

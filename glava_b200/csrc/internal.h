@@ -154,6 +154,16 @@ int launch_transform_smooth(float* d_planes, int n, const void* d_tab, int asz, 
                             const uint32_t* d_umask = nullptr, int mask_shift = 1);   // d_umask: SpectrumArgs::umask, planes of unmodified
                             // streams are skipped; stream of plane i = i >> mask_shift (1: interleaved [batch*2] planes, 0: one channel's [batch])
 int launch_upload(const float* d_s, const float* d_e, float mod, uint16_t* d_out, size_t total, void* stream);
+// stream_state_kernels.cu: per-stream state <-> blob-ordered staging (stream_state_core.h); d_table = int stream[count]
+// followed by uint32 cursor[count]; d_in == nullptr zeroes the streams' state
+struct StateLayout; struct StatePtrs;
+int launch_state_pack(const StateLayout& L, const StatePtrs& P, const int* d_table, int count, void* d_out, void* stream);
+int launch_state_unpack(const StateLayout& L, const StatePtrs& P, const int* d_table, int count, const void* d_in, void* stream);
+// capi.cu, for sharded.cpp: the blob checks of glava_b200_load_streams (nothing is touched), and save / load with one
+// host pointer per listed stream (the blobs of one shard's streams are not contiguous in the caller's array)
+int state_check_blobs(const glava_b200* r, const void* const* blobs, int count, const char* who);
+int state_save_ptrs(glava_b200* r, const int* streams, int count, void* const* blobs);
+int state_load_ptrs(glava_b200* r, const int* streams, int count, const void* const* blobs);
 
 }  // namespace glb
 

@@ -8,6 +8,7 @@
 // stream-indexed read-backs.  Host code only: every device operation goes through the single-device C ABI (capi.cu).
 #include "internal.h"
 
+#include <algorithm>
 #include <condition_variable>
 #include <functional>
 #include <string>
@@ -195,6 +196,78 @@ const void* glava_b200_sharded_frame_device(glava_b200_sharded* g, int stream, i
     if (device) *device = s->device;
     return glava_b200_frame_device(s->r, stream - s->first);
 }
+// Per-stream state (DESIGN.md §4.8), global stream indices: reset by each shard's slice of the mask; save and load group the
+// listed streams per shard and run every shard's part at once.  Indices and blobs are checked for the whole call before any
+// shard starts, so a rejected call touches no shard.
+int glava_b200_sharded_reset_streams(glava_b200_sharded* g, const uint8_t* mask) {
+    clear_error();
+    if (!g || !mask) return fail(GLAVA_B200_EINVAL, "glava_b200_sharded_reset_streams: null argument");
+    if (glava_b200_stream_state_bytes(&g->p) == 0) return GLAVA_B200_EINVAL;
+    return broadcast(g, [=](Shard& s) { return glava_b200_reset_streams(s.r, mask + s.first); });
+}
+
+// split `streams` into per-shard local index lists and blob pointers (blob i at base + i * bytes)
+static int group_streams(glava_b200_sharded* g, const int* streams, int count, const char* base, size_t bytes, const char* who,
+                         std::vector<std::vector<int>>* idx, std::vector<std::vector<const char*>>* ptr) {
+    if (count < 0 || (count > 0 && (!streams || !base))) return fail(GLAVA_B200_EINVAL, "%s: bad arguments", who);
+    idx->assign(g->shards.size(), {}); ptr->assign(g->shards.size(), {});
+    std::vector<char> seen((size_t) g->batch, 0);
+    for (int i = 0; i < count; ++i) {
+        const int s = streams[i];
+        if (s < 0 || s >= g->batch) return fail(GLAVA_B200_EINVAL, "%s: stream %d out of range (batch %d)", who, s, g->batch);
+        if (seen[(size_t) s]) return fail(GLAVA_B200_EINVAL, "%s: stream %d listed twice", who, s);
+        seen[(size_t) s] = 1;
+        for (size_t k = 0; k < g->shards.size(); ++k) {
+            const Shard* sh = g->shards[k];
+            if (s >= sh->first && s < sh->first + sh->count) {
+                (*idx)[k].push_back(s - sh->first); (*ptr)[k].push_back(base + (size_t) i * bytes);
+                break;
+            }
+        }
+    }
+    return 0;
+}
+
+int glava_b200_sharded_save_streams(glava_b200_sharded* g, const int* streams, int count, void* blobs) {
+    clear_error();
+    const char* who = "glava_b200_sharded_save_streams";
+    if (!g) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
+    const size_t bytes = glava_b200_stream_state_bytes(&g->p);
+    if (!bytes) return GLAVA_B200_EINVAL;
+    std::vector<std::vector<int>> idx; std::vector<std::vector<const char*>> ptr;
+    int rc = group_streams(g, streams, count, (const char*) blobs, bytes, who, &idx, &ptr);
+    if (rc) return rc;
+    return broadcast(g, [&](Shard& s) {
+        const size_t k = (size_t) (std::find(g->shards.begin(), g->shards.end(), &s) - g->shards.begin());
+        if (idx[k].empty()) return 0;
+        std::vector<void*> out(ptr[k].size());
+        for (size_t i = 0; i < out.size(); ++i) out[i] = (void*) ptr[k][i];
+        return state_save_ptrs(s.r, idx[k].data(), (int) idx[k].size(), out.data());
+    });
+}
+
+int glava_b200_sharded_load_streams(glava_b200_sharded* g, const int* streams, int count, const void* blobs) {
+    clear_error();
+    const char* who = "glava_b200_sharded_load_streams";
+    if (!g) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
+    const size_t bytes = glava_b200_stream_state_bytes(&g->p);
+    if (!bytes) return GLAVA_B200_EINVAL;
+    std::vector<std::vector<int>> idx; std::vector<std::vector<const char*>> ptr;
+    int rc = group_streams(g, streams, count, (const char*) blobs, bytes, who, &idx, &ptr);
+    if (rc) return rc;
+    for (size_t k = 0; k < g->shards.size(); ++k) {
+        if (ptr[k].empty()) continue;
+        std::vector<const void*> in(ptr[k].begin(), ptr[k].end());
+        if ((rc = state_check_blobs(g->shards[k]->r, in.data(), (int) in.size(), who)) != 0) return rc;
+    }
+    return broadcast(g, [&](Shard& s) {
+        const size_t k = (size_t) (std::find(g->shards.begin(), g->shards.end(), &s) - g->shards.begin());
+        if (idx[k].empty()) return 0;
+        std::vector<const void*> in(ptr[k].begin(), ptr[k].end());
+        return state_load_ptrs(s.r, idx[k].data(), (int) idx[k].size(), in.data());
+    });
+}
+
 int glava_b200_sharded_textures(glava_b200_sharded* g, uint16_t* out_l, uint16_t* out_r) {
     clear_error();
     if (!g) return fail(GLAVA_B200_EINVAL, "null argument");

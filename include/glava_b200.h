@@ -351,6 +351,38 @@ int  glava_b200_sharded_readback(glava_b200_sharded* s, int stream, uint8_t* rgb
 const void* glava_b200_sharded_frame_device(glava_b200_sharded* s, int stream, int* device);
 int  glava_b200_sharded_textures(glava_b200_sharded* s, uint16_t* out_l, uint16_t* out_r);
 
+/* ---- lifetime of individual streams: reset, save and load (DESIGN.md §4.8) -------------------------------------------
+ * A stream's state is what its next update reads besides its new audio: gravity store and average ring, the latest
+ * spectrum, the texture the next raster reads, the pre-smoothing texture and the device FIFO ring.
+ *   glava_b200_stream_state_bytes  bytes of one stream's blob for renderers created with `p`:
+ *                                  GLAVA_B200_STATE_HEADER_BYTES + chans * ((1 + F) * n * esz + 8 * n + 4 * setbufsize),
+ *                                  n = setbufsize / setbufscale, F = setavgframes, esz = 2 under setaccelfft (pipeline B) and
+ *                                  4 otherwise (an appended "smooth" transform clears setaccelfft), chans = 1 for wave, else 2.
+ *                                  0 (with the error set) when keyframe interpolation is active or `p` is invalid.
+ *   glava_b200_reset_streams       every stream with mask[s] != 0 becomes stream 0 of a newly created renderer: from its next
+ *                                  update on it renders what a fresh batch-1 renderer fed the same calls renders.  Its
+ *                                  framebuffer slot keeps the old frame until then.  Does not wait for the device.
+ *   glava_b200_save_streams        writes the state of streams[0 .. count) into `blobs` (HOST, count * bytes; pinned memory
+ *                                  from glava_b200_host_alloc copies at the PCIe rate).  Returns once the blobs are complete.
+ *   glava_b200_load_streams        puts blobs saved from a renderer with the same effective parameters (fb_slots aside) into
+ *                                  streams[0 .. count) of this one, whatever its batch, device, update count or ring cursors:
+ *                                  each slot then continues exactly as the saved stream would have.  Returns once the blobs
+ *                                  have been consumed, like glava_b200_update; does not wait for earlier updates.
+ * All three are ordered with the handle's updates like any other call.  GLAVA_B200_EINVAL, with nothing touched, for
+ * stream indices out of range or repeated, a blob of other parameters, magic, version or size, and while keyframe
+ * interpolation is active (the keyframe rotation belongs to the renderer, as for uneven masks).  The format is not
+ * stable across library versions: the version field rejects a mismatch.
+ * The sharded forms take global stream indices (mask: [batch] in global order); a stream moves between shards by a
+ * save on one and a load on the other. */
+#define GLAVA_B200_STATE_HEADER_BYTES 4096
+size_t glava_b200_stream_state_bytes(const glava_b200_params* p);
+int glava_b200_reset_streams(glava_b200* r, const uint8_t* mask /* [batch], non-zero = reset */);
+int glava_b200_save_streams(glava_b200* r, const int* streams, int count, void* blobs /* HOST, count * bytes */);
+int glava_b200_load_streams(glava_b200* r, const int* streams, int count, const void* blobs);
+int glava_b200_sharded_reset_streams(glava_b200_sharded* s, const uint8_t* mask /* [batch], global order */);
+int glava_b200_sharded_save_streams(glava_b200_sharded* s, const int* streams, int count, void* blobs);
+int glava_b200_sharded_load_streams(glava_b200_sharded* s, const int* streams, int count, const void* blobs);
+
 /* Stage-wise entry points (used by the parity tests; same kernels as the fused path). */
 int glava_b200_smooth_pass(glava_b200* r, const uint16_t* in, uint16_t* out, int count);      /* K5 on HOST [count][n] */
 int glava_b200_raster_textures(glava_b200* r, const uint16_t* tex_l, const uint16_t* tex_r);  /* HOST [batch][n] -> raster */
