@@ -497,7 +497,7 @@ static int build(glava_b200* r) {
     }
     ALLOC(r->d_tex, 2 * planes * n * 2, true);
     ALLOC(r->d_av, planes * n * 2, true);
-    ALLOC(r->d_texmm, planes * GLB_TEXMM_STRIDE * sizeof(uint32_t), true);          // double-buffered: spectrum i+1 writes one half while raster i reads the other
+    ALLOC(r->d_texmm, planes * GLB_TEXMM_STRIDE * sizeof(uint32_t), true);          // one buffer: texmm_kernel fills it on the raster stream right before the circle raster reads it
     ALLOC(r->d_rowtab, (size_t) p.h * 8, true);
     if (p.module == GLAVA_B200_MOD_GRAPH || p.module == GLAVA_B200_MOD_WAVE)          // (the module of a handle never changes: reconfigure refuses)
         ALLOC(r->d_coltab, (size_t) r->batch * GLB_COLTAB_PLANES * p.w * sizeof(float), true);

@@ -769,6 +769,8 @@ int launch_raster(const glava_b200_params& p, const RasterArgs& a, void* stream,
     if (const char* e = getenv("GLAVA_B200_GW_MINB")) minb = atoi(e) == 5 ? 5 : 4;
     if (const char* e = getenv("GLAVA_B200_ROWS")) { int v = atoi(e); if (v > 0) rows = v; }
     if (const char* e = getenv("GLAVA_B200_BX")) { int v = atoi(e); if (v >= 32 && v <= 256 && v % 32 == 0) bx = v; }
+    // bars / graph / wave are __launch_bounds__(256); generic and both radial kernels take at most 128 threads
+    if (!(fast_bars || fast_graph || fast_wave) && bx > 128) bx = 128;
     if (rows > p.h) rows = p.h;
     // z dimension limit 65535: chunk the batch
     // one launch covers at most `slots` streams (and at most the grid z limit): with a framebuffer

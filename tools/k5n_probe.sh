@@ -9,4 +9,4 @@ echo "== sweep default"; python tools/sweep_configs.py bars:4096:1920x1080 bars:
 echo "== sweep 4096 3k"; GLAVA_B200_K5_SPLIT=1 python tools/sweep_configs.py bars:4096:1920x1080 bars:4096:1280x720 bars:2048:1280x720 2>&1 | cut -c1-200
 echo "== sweep 4096 3k oop128"; GLAVA_B200_K5_SPLIT=1 GLAVA_B200_SPEC_OOP=1 GLAVA_B200_SPEC_T=128 python tools/sweep_configs.py bars:4096:1920x1080 bars:4096:1280x720 bars:2048:1280x720 2>&1 | cut -c1-200
 echo "== circle tests"; python -m pytest tests/test_gpu_raster.py tests/test_glsl_golden.py tests/test_llvmpipe_golden.py -m gpu -q -k "circle or raster" 2>&1 | tail -4
-echo "== circle sweep (tile cull on / off)"; python tools/sweep_configs.py circle:4096:1920x1080 2>&1 | cut -c1-330; GLAVA_B200_NO_CTILE=1 python tools/sweep_configs.py circle:4096:1920x1080 2>&1 | cut -c1-330
+echo "== circle sweep (tile cull off / on)"; python tools/sweep_configs.py circle:4096:1920x1080 2>&1 | cut -c1-330; GLAVA_B200_CTILE=1 python tools/sweep_configs.py circle:4096:1920x1080 2>&1 | cut -c1-330
