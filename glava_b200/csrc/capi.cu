@@ -791,7 +791,7 @@ static int run_update(glava_b200* r, const float* d_l, const float* d_r, int mod
         a.av_out = (split_k5 || split_lazy) ? r->d_av : nullptr;
         a.av_t_len = split_lazy ? r->av_t_len : 0;
         // three-kernel form of the lazy pipeline-B update: transform_fft only in the plane-per-CTA kernel, the R16 state
-        // update as an elementwise kernel, K5 on (texel, stream) pairs.  (F = 1 has no ring: in-kernel form.)
+        // update as an elementwise kernel, K5 on (texel, stream) pairs.  Every F: at F = 1 epilogue_b_kernel<0> keeps no ring.
         const int epi8 = ((r->epi_n + 7) / 8) * 8;
         const bool split_epi = split_lazy && is_fft && p.accel_fft && r->split_epilogue && epi8 > 0 && epi8 <= p.n && F >= 1;
         a.fft_only = split_epi ? 1 : 0;

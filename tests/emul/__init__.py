@@ -27,12 +27,14 @@ def lib():
         L.emul_chan_free.argtypes = [vp]
         L.emul_chan_update.argtypes = [vp, vp, vp, i32, vp, vp]
         L.emul_smooth.argtypes = [vp, vp, vp]
+        L.emul_smooth_at.argtypes = [vp, vp, vp, i32, vp]
         L.emul_raster.argtypes = [vp, vp, vp, vp, i32, i32]
         L.emul_raster_fast.argtypes = [vp, vp, vp, vp]
         L.emul_eval_color.argtypes = [vp, C.c_float, vp]
         L.emul_lazy_k5.argtypes = [vp, i32, i32, vp, vp, vp]
         L.emul_lazy_epi_n.argtypes = [vp]
         L.emul_k5_table.argtypes = [vp, vp, vp]
+        L.emul_table_sizes.argtypes = [vp, i32, i32, i32, vp]
         L.emul_bufscale.argtypes = [vp, i32, i32, vp]
         L.emul_transform_smooth.argtypes = [vp, i32, C.c_float, C.c_float]
         L.emul_upload.argtypes = [vp, vp, i32, C.c_float, C.c_float, i32, vp]
@@ -68,6 +70,15 @@ def smooth(params, tex):
     t = np.ascontiguousarray(tex, dtype=np.uint16)
     out = np.empty_like(t)
     lib().emul_smooth(C.addressof(params), t.ctypes.data, out.ctypes.data)
+    return out
+
+
+def smooth_at(params, tex, idx):
+    """smooth(params, tex)[idx] without computing the other texels"""
+    t = np.ascontiguousarray(tex, dtype=np.uint16)
+    ix = np.ascontiguousarray(idx, dtype=np.int32)
+    out = np.empty(ix.shape[0], np.uint16)
+    lib().emul_smooth_at(C.addressof(params), t.ctypes.data, ix.ctypes.data, ix.shape[0], out.ctypes.data)
     return out
 
 
@@ -119,6 +130,19 @@ def lazy_k5(p, chan, path, av):
 
 def lazy_epi_n(p):
     return lib().emul_lazy_epi_n(C.byref(p))
+
+
+TABLE_SIZES = ("need", "need_count", "blob", "tap_bytes", "epi_n", "max_rows", "nblk", "k5_span", "k5_ent_bytes",
+               "planes_span", "spec_smem")
+
+
+def table_sizes(p, target_rows=-105, texels_per_block=16, full=True):
+    """the table sizes build_tables and launch_smooth_only choose the K5 launch structure from (emul.cpp emul_table_sizes);
+    target_rows / texels_per_block as GLAVA_B200_K5N_ROWS / _TPB, defaults as build_tables; full=False skips the
+    full-plane table (k5_span, k5_ent_bytes read 0)"""
+    out = np.zeros(len(TABLE_SIZES), np.int64)
+    lib().emul_table_sizes(C.byref(p), target_rows, texels_per_block, 1 if full else 0, out.ctypes.data)
+    return dict(zip(TABLE_SIZES, out.tolist()))
 
 
 def k5_table(p, tex):

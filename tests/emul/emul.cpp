@@ -161,6 +161,11 @@ void emul_smooth(const glava_b200_params* p, const uint16_t* in, uint16_t* out) 
     SmoothParams sp = smooth_params(*p);
     for (int x = 0; x < p->n; ++x) out[x] = (uint16_t) smooth_pass_texel(sp, in, p->n, x);
 }
+// the same pass at the texels idx[0 .. count) only: out[k] = texel idx[k]
+void emul_smooth_at(const glava_b200_params* p, const uint16_t* in, const int* idx, int count, uint16_t* out) {
+    SmoothParams sp = smooth_params(*p);
+    for (int k = 0; k < count; ++k) out[k] = (uint16_t) smooth_pass_texel(sp, in, p->n, idx[k]);
+}
 
 // one compiled colour expression at X (the interpreter the kernels run: raster_core.h eval_color_prog)
 void emul_eval_color(const glava_b200_color_prog* prog, float x, float out[4]) {
@@ -326,6 +331,44 @@ int emul_lazy_epi_n(const glava_b200_params* pp) {
     LazyTables t;
     build_lazy_tables(*pp, lists, &t);
     return t.epi_n;
+}
+// The sizes capi.cu build_tables / build_k5_table and spectrum_kernels.cu launch_smooth_only choose the K5 launch structure
+// from, computed by the same tables.h builders (out[0] = 0 when the module has no need-list):
+//   [0] need-list present  [1] entries per channel  [2] texel-major blob bytes per channel  [3] tap-table bytes
+//   [4] epi_n  [5] build_need_blocks max_rows (target_rows, texels_per_block as GLAVA_B200_K5N_ROWS / _TPB)  [6] its nblk
+//   [7] build_k5_table_host max_span  [8] its entry bytes  [9] k5_planes_kernel's widest staged span (launch_smooth_only)
+//   [10] spectrum_kernel's in-place shared memory (SpecCfg<log2 n>::SMEM, spectrum_smem_bytes)
+//   ([7], [8] only with `full`: the full table takes seconds to build for wide windows at n = 16384)
+void emul_table_sizes(const glava_b200_params* pp, int target_rows, int texels_per_block, int full, long long* out) {
+    const glava_b200_params& p = *pp;
+    for (int i = 0; i < 11; ++i) out[i] = 0;
+    std::vector<int> lists[2];
+    if (build_need_list(p, lists)) {
+        LazyTables t;
+        build_lazy_tables(p, lists, &t);
+        NeedBlocks nb;
+        build_need_blocks(t, p.n, target_rows, texels_per_block, &nb);
+        out[0] = 1; out[1] = (long long) t.cnt; out[2] = (long long) t.blob; out[3] = (long long) (t.tab.size() * sizeof(TapEntry));
+        out[4] = t.epi_n; out[5] = nb.max_rows; out[6] = nb.nblk;
+    }
+    if (full) {
+        K5TableHost k;
+        build_k5_table_host(p, &k);
+        out[7] = k.max_span; out[8] = (long long) (k.ent.size() * sizeof(K5Ent));
+    }
+    const SmoothParams sp = smooth_params(p);
+    const float fn = (float) p.n;
+    int span = 0;
+    for (int x0 = 0; x0 < p.n; x0 += K5_BLOCK) {
+        const int x1 = (x0 + K5_BLOCK < p.n) ? x0 + K5_BLOCK : p.n;
+        const float lo_f = scale_audio(sp, g_clamp(((float) x0 + 0.5f) / fn - sp.smooth_factor, 0.0f, 1.0f)) * fn;
+        const float hi_f = scale_audio(sp, g_clamp(((float) (x1 - 1) + 0.5f) / fn + sp.smooth_factor, 0.0f, 1.0f)) * fn;
+        int lo = (int) floorf(lo_f) - 2, hi = (int) ceilf(hi_f) + 3;
+        lo = lo < 0 ? 0 : lo; hi = hi > p.n ? p.n : hi;
+        if (hi - lo > span) span = hi - lo;
+    }
+    out[9] = span;
+    out[10] = (long long) (((fft_padded_size(p.n / 2) * 8 + 15) / 16) * 16 + p.n * 2 + 16);
 }
 // full-plane K5 of one plane through the per-block table, as k5_table_kernel does it (float staging, padded uniform loop)
 void emul_k5_table(const glava_b200_params* pp, const uint16_t* in, uint16_t* out) {

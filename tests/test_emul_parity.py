@@ -6,7 +6,7 @@ import pytest
 
 import glava_b200 as g
 from oracle.oracle import OracleChannel, params_from
-from tests import emul
+from tests import emul, spectrum_cases
 from tests.pcm import EDGE_SIGNALS, edge_signal, fft_magnitude_error, fft_ramp
 
 
@@ -257,7 +257,11 @@ def test_need_list_covers_the_join_channels_middle_taps(built):
 
 
 def test_update_chain_random_parameters(orc_pm, built):
-    """product spectrum arithmetic vs the (reference-pinned) oracle over random parameters, both pipelines"""
+    """product spectrum arithmetic vs the (reference-pinned) oracle over random parameters, both pipelines: random bars
+    configurations at n <= 2048, then the shared case list (tests/spectrum_cases.py) — every size to 16384 in both
+    pipelines, every F, the spectrum and smoothing knobs, all modules, setbufscale, the post chain, with silent and masked
+    updates.  Stream 0, the texels each case's launch structure defines (for the widest windows a strided subset, see
+    texel_sets).  The GPU tier (tests/test_gpu_spectrum_params.py) checks the kernels against the same expectations."""
     rng = np.random.default_rng(77)
     for trial in range(24):
         n = int(rng.choice([256, 1024, 2048]))
@@ -275,3 +279,11 @@ def test_update_chain_random_parameters(orc_pm, built):
         peak = max(np.abs(s0).max(), 1e-30)
         assert np.abs(s0 - s1).max() / peak <= 1e-5, (trial, n)
         assert np.abs(t0.astype(int) - t1.astype(int)).max() <= 2, (trial, n)
+    for case in spectrum_cases.build_cases():
+        k = case.kernel_params()
+        wave = k.module == g.MODULES.index("wave")
+        host, want = spectrum_cases.host_stream(case, 0), spectrum_cases.oracle_stream(orc_pm, case, 0)
+        tol = 1e-5 if k.n <= 4096 else 2.5e-5
+        for ch in ((0,) if wave else (0, 1)):
+            assert spectrum_cases.spectrum_error(case, host[0][ch], want[0][ch]) <= tol, (case.id, ch)
+            assert np.abs(host[1][ch].astype(int) - want[1][ch].astype(int)).max(initial=0) <= 2, (case.id, ch)
