@@ -108,6 +108,9 @@ struct glava_b200 {
     uint16_t* d_gr_store; uint16_t* d_ring_u; uint16_t* d_tex;
     uint16_t* d_av;             // pre-smoothing textures [batch*2][n] (full-plane K5 runs as its own kernel)
     uint8_t* d_fb;
+    // dirty-row marks of the framebuffer slots (RasterArgs::marks) and the launch structure that last wrote them
+    // (launch_raster; 0 = none: the next bars / graph / wave launch stores every row)
+    uint32_t* d_marks; int mark_key;
     unsigned long long updates;
     // per-stream `modified` masks (glava_b200_update_masked): once streams have advanced unevenly, every stream has its
     // own average-ring cursor; words {bit 31 = modified, low bits = cursor} go to the device through a small pinned ring
@@ -137,6 +140,11 @@ static void derive(glava_b200* r) {
     const float fr = r->p.fr > 0.0f ? r->p.fr : r->p.ur;
     r->interp_on = r->p.interpolate && !(r->p.accel_fft && is_fft) && (r->p.ur / fr) <= 0.9f;
     r->post_chain = r->p.transform_smooth == 1 || r->interp_on;
+}
+
+// dirty-row marks: one word per (slot, row, 128-pixel strip), so that any band height finds its band's word at its first row
+static size_t mark_bytes(const glava_b200_params& p, int slots) {
+    return (size_t) slots * p.h * ((p.w + 127) / 128) * sizeof(uint32_t);
 }
 
 static int dev_alloc(glava_b200* r, void** out, size_t bytes, bool zero) {
@@ -505,6 +513,8 @@ static int build(glava_b200* r) {
     size_t frame = (size_t) p.w * p.h * 4;
     r->slots = (p.fb_slots > 0 && p.fb_slots < r->batch) ? p.fb_slots : r->batch;
     ALLOC(r->d_fb, frame * r->slots, true);
+    ALLOC(r->d_marks, mark_bytes(p, r->slots), true);          // empty marks: the framebuffer starts all 0
+    r->mark_key = 0;
 #undef ALLOC
     // window LUT: render.c:660 macro as expanded at render.c:794 — cos(TWOPI*i/N - 1), double
     std::vector<double> w(n);
@@ -562,6 +572,7 @@ glava_b200* glava_b200_new(const glava_b200_params* params, int batch, int devic
     r->d_ctile = nullptr; r->ctile_nx = r->ctile_count = 0;
     r->d_geo = nullptr; r->geo_box[0] = r->geo_box[1] = r->geo_box[2] = r->geo_box[3] = 0;
     r->d_spec = r->d_applied = r->d_ring_f = nullptr; r->d_gr_store = r->d_ring_u = r->d_tex = nullptr; r->d_av = nullptr; r->d_texmm = nullptr; r->d_coltab = nullptr; r->d_fb = nullptr;
+    r->d_marks = nullptr; r->mark_key = 0;
     for (int i = 0; i < 2; ++i) { r->d_pcm[i][0] = r->d_pcm[i][1] = nullptr; r->ev_copied[i] = r->ev_free[i] = nullptr; }
     r->stage_cur = 0; r->copy_stream = nullptr;
     r->out_stream = nullptr; r->d_stage[0] = r->d_stage[1] = nullptr; r->stage_bytes = 0; r->out_cur = 0;
@@ -668,14 +679,16 @@ static int apply_resize(glava_b200* r, int w, int h) {
     int rc = validate_params(&q);
     if (rc) return rc;
     if ((rc = sync_all(r)) != 0) return rc;
-    dev_free(r, r->d_fb); dev_free(r, r->d_rowtab); dev_free(r, r->d_coltab);
-    r->d_fb = nullptr; r->d_rowtab = nullptr; r->d_coltab = nullptr;
+    dev_free(r, r->d_fb); dev_free(r, r->d_marks); dev_free(r, r->d_rowtab); dev_free(r, r->d_coltab);
+    r->d_fb = nullptr; r->d_marks = nullptr; r->d_rowtab = nullptr; r->d_coltab = nullptr;
+    r->mark_key = 0;
     r->p_user = q;
     derive(r);
     if ((rc = dev_alloc(r, (void**) &r->d_rowtab, (size_t) q.h * 8, true)) != 0) return rc;
     if ((q.module == GLAVA_B200_MOD_GRAPH || q.module == GLAVA_B200_MOD_WAVE) &&
         (rc = dev_alloc(r, (void**) &r->d_coltab, (size_t) r->batch * GLB_COLTAB_PLANES * q.w * sizeof(float), true)) != 0) return rc;
     if ((rc = dev_alloc(r, (void**) &r->d_fb, (size_t) q.w * q.h * 4 * r->slots, true)) != 0) return rc;
+    if ((rc = dev_alloc(r, (void**) &r->d_marks, mark_bytes(q, r->slots), true)) != 0) return rc;
     return build_tables(r);
 }
 
@@ -865,6 +878,7 @@ static int run_update(glava_b200* r, const float* d_l, const float* d_r, int mod
     ra.geo = r->d_geo; ra.gx0 = r->geo_box[0]; ra.gy0 = r->geo_box[1]; ra.gw = r->geo_box[2]; ra.gh = r->geo_box[3];
     ra.texmm = nullptr; ra.ctile = nullptr; ra.ctile_zero = nullptr; ra.ctile_nx = 0;
     ra.coltab = r->no_coltab ? nullptr : r->d_coltab;
+    ra.marks = r->d_marks; ra.marks_valid = 0;            // launch_raster decides from r->mark_key
     // params.shader_pre_smoothed: the module's stage-1 shader believes something else about its textures than what the
     // K5 pass did.  Only the raster launch sees that belief (as its smooth_pass); everything before it follows the real one.
     glava_b200_params pr_store;
@@ -881,7 +895,7 @@ static int run_update(glava_b200* r, const float* d_l, const float* d_r, int mod
     }
     if (r->timing && (rc = timing_mark(r->ev_ras, r->stream)) != 0) return rc;
     int raster_launches = 0;
-    if ((rc = launch_raster(*pr, ra, r->stream, &raster_launches)) != 0) return rc;
+    if ((rc = launch_raster(*pr, ra, r->stream, &raster_launches, &r->mark_key)) != 0) return rc;
     if (r->timing && (rc = timing_mark(r->ev_ras, r->stream)) != 0) return rc;
     CU(cudaEventRecord(r->ev_raster_done[b], r->stream));
     r->launches += (uint64_t) raster_launches;

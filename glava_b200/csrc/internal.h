@@ -94,6 +94,11 @@ struct RasterArgs {
     // graph / wave: per-stream column table [batch][GLB_COLTAB_PLANES][w] floats, scratch that launch_raster fills on the
     // raster stream right before the module kernel (graph: plane 0 = column height; wave: WaveCol's five fields); may be null
     float* coltab;
+    // bars / graph / wave: dirty-row marks (raster_core.h dirty_pack), [slots][h][(w + 127) / 128] words, a band's word at
+    // its first row.  marks_valid = 0: the words do not describe the framebuffer (another kernel or band height wrote it
+    // last); the kernel then stores every zero row and writes fresh marks.  launch_raster sets it.
+    uint32_t* marks;
+    int       marks_valid;
 };
 #define GLB_COLTAB_PLANES 5
 #define GLB_CIRCLE_NB 128                         // texel buckets per plane (n / 128 texels each)
@@ -134,7 +139,9 @@ int launch_k5_need_smem(const glava_b200_params& p, const uint16_t* d_av, uint16
 // pipeline B epilogue as its own elementwise kernel: spec (transform_fft output) -> upload quantisation, K1 - K4 on the R16
 // state, pre-smoothing texels into av_out (leading `bins` of every plane; bins is a multiple of 8)
 int launch_epilogue_b(const glava_b200_params& p, const SpectrumArgs& a, int bins, void* stream);
-int launch_raster(const glava_b200_params& p, const RasterArgs& a, void* stream, int* launched = nullptr);   // *launched += kernels launched
+// *launched += kernels launched.  *mark_key: the renderer's record of which launch structure last wrote a.marks (0: none,
+// or a kernel that keeps no marks wrote the framebuffer since); read and updated here.  Null: every launch stores every row.
+int launch_raster(const glava_b200_params& p, const RasterArgs& a, void* stream, int* launched = nullptr, int* mark_key = nullptr);
 int launch_bars_rowtab(const glava_b200_params& p, void* d_rowtab, void* stream);
 // geometry cache of the polar modules: box = {x0, y0, w, h}; returns bytes needed when d_geo == nullptr
 size_t polar_geo_box(const glava_b200_params& p, int box[4]);

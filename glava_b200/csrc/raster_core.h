@@ -679,6 +679,19 @@ GLB_HD uint32_t test_px(const glava_b200_params& p) {
     return premultiply8(px);                                                // test/3.frag
 }
 
+// ================================= dirty-row marks (bars, graph, wave) ============================
+// Every framebuffer slot keeps one word per (row band, 128-pixel warp strip) of the raster launch that last wrote it:
+// rows [lo, hi) of the band may be non-zero in memory, every other row of the band is 0 (lo = low 16 bits, hi = high
+// 16 bits; h <= 16384, validate_params).  A kernel stores a zero row only where it falls inside the old interval — a row
+// that is 0 in memory and 0 in the new frame needs no store — and then records the rows it stored non-zero content in.
+GLB_HD uint32_t dirty_pack(int lo, int hi) { return lo < hi ? ((uint32_t) lo | ((uint32_t) hi << 16)) : 0u; }
+// Zero rows [za, zb) of a band, old mark `old` -> the rows [*a, *b) of them that must be stored (*a == *b: none).
+GLB_HD void dirty_zero_span(uint32_t old, int za, int zb, int* a, int* b) {
+    const int lo = (int) (old & 0xffffu), hi = (int) (old >> 16);
+    const int s = za > lo ? za : lo, e = zb < hi ? zb : hi;
+    *a = s; *b = e > s ? e : s;
+}
+
 // generic per-pixel dispatcher
 GLB_HD_NOINLINE uint32_t module_px(const glava_b200_params& p, const AudioTex& t, int x, int y) {
     switch (p.module) {

@@ -45,6 +45,22 @@ __device__ __forceinline__ void zero_rows(uint32_t* fb, int x, int w, int ya, in
     }
 }
 
+// Dirty-row mark of the warp that owns the 128-pixel strip of quad x in the band starting at row y0 (RasterArgs::marks).
+// Only lane 0 reads and writes it, and no other warp touches it.
+__device__ __forceinline__ uint32_t* mark_word(const RasterArgs& a, const glava_b200_params& p, int stream, int x, int y0) {
+    return a.marks + ((size_t) (stream % a.slots) * p.h + y0) * ((p.w + 127) >> 7) + (x >> 7);
+}
+// the rows of [y0, y1) that may be non-zero in memory, as a mark; without valid marks, all of them
+__device__ __forceinline__ uint32_t mark_load(const RasterArgs& a, const uint32_t* m, int y0, int y1, unsigned lanes) {
+    if (!a.marks_valid) return dirty_pack(y0, y1);
+    uint32_t v = 0u;
+    if ((threadIdx.x & 31) == 0) v = *m;
+    return __shfl_sync(lanes, v, 0);
+}
+__device__ __forceinline__ void mark_store(uint32_t* m, int lo, int hi) {
+    if ((threadIdx.x & 31) == 0) *m = dirty_pack(lo, hi);
+}
+
 // generic: every pixel through module_px() — reference semantics with no hoisting; also the
 // fallback for option combinations the specialised kernels do not cover.
 __global__ void __launch_bounds__(128)
@@ -120,6 +136,7 @@ __global__ void __launch_bounds__(256)
 raster_bars_kernel(const __grid_constant__ RasterArgs a, const __grid_constant__ glava_b200_params p, int rows_per_cta) {
     const int stream = a.stream0 + blockIdx.z;
     const int x = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
+    if ((x & ~127) >= p.w) return;                                        // the whole warp is right of the frame
     const bool valid = x < p.w;
     const AudioTex t = make_tex(p, a.tex, stream);
     const uint2* __restrict__ rowtab = reinterpret_cast<const uint2*>(a.rowtab);
@@ -143,11 +160,15 @@ raster_bars_kernel(const __grid_constant__ RasterArgs a, const __grid_constant__
     int f0, f1, z0, z1;
     if (!p.bars_flip) { f0 = y0; f1 = min(y1, tmax); z0 = max(y0, tmax); z1 = y1; }
     else              { z0 = y0; z1 = min(y1, p.h - tmax); f0 = max(y0, p.h - tmax); f1 = y1; }
-    {
-        uint4* ptr = base + (size_t) z0 * stride;
+    uint32_t* const mark = mark_word(a, p, stream, x, y0);
+    {   // of the zero rows, only those the previous frame in this slot may have left non-zero
+        int s0, s1;
+        dirty_zero_span(mark_load(a, mark, y0, y1, 0xffffffffu), z0, z1, &s0, &s1);
+        uint4* ptr = base + (size_t) s0 * stride;
         const uint4 zero = make_uint4(0u, 0u, 0u, 0u);
-        for (int y = z0; y < z1; ++y, ptr += stride) if (valid) __stcs(ptr, zero);
+        for (int y = s0; y < s1; ++y, ptr += stride) if (valid) __stcs(ptr, zero);
     }
+    mark_store(mark, f0, f1);
     {
         uint4* ptr = base + (size_t) f0 * stride;
         for (int y = f0; y < f1; ++y, ptr += stride) {
@@ -244,7 +265,8 @@ raster_graph_kernel(const __grid_constant__ RasterArgs a, const __grid_constant_
         }
     };
 
-    if (p.graph_invert > 0) { full_rows(y0, y1); return; }
+    uint32_t* const mark = mark_word(a, p, stream, x, y0);     // lane 0 is active: lanes past the right edge returned
+    if (p.graph_invert > 0) { full_rows(y0, y1); mark_store(mark, y0, y1); return; }
 
     // thread bounds: rows >= E are empty for all 4 pixels; rows < F (and >= 1, < h-1) are interior for all 4
     int E = 0, F = p.h;
@@ -254,10 +276,8 @@ raster_graph_kernel(const __grid_constant__ RasterArgs a, const __grid_constant_
         E = max(E, graph_first_row(hi[k], -1, p.h));                 // (y-1)+1.5 > hi  <=> 3x3 empty
         F = min(F, inner_x[k] ? graph_first_row(lo[k], +1, p.h) : 0); // (y+1)+1.5 <= lo <=> 3x3 filled
     }
-    {
-        const unsigned m = __activemask();
-        E = __reduce_max_sync(m, E); F = __reduce_min_sync(m, F);
-    }
+    const unsigned lanes = __activemask();
+    E = __reduce_max_sync(lanes, E); F = __reduce_min_sync(lanes, F);
     const int b1 = min(y1, max(y0, 1));
     const int b2 = max(b1, min(y1, min(F, p.h - 1)));
     const int b3 = max(b2, min(y1, E));
@@ -270,7 +290,10 @@ raster_graph_kernel(const __grid_constant__ RasterArgs a, const __grid_constant_
         } else full_rows(y, y + 1);
     }
     full_rows(b2, b3);
-    zero_rows(fb, x, p.w, b3, y1);
+    int s0, s1;
+    dirty_zero_span(mark_load(a, mark, y0, y1, lanes), b3, y1, &s0, &s1);
+    zero_rows(fb, x, p.w, s0, s1);
+    mark_store(mark, y0, b3);
 }
 
 // wave: 6 column descriptors in registers
@@ -311,11 +334,15 @@ raster_wave_kernel(const __grid_constant__ RasterArgs a, const __grid_constant__
     float lo4 = fminf(fminf(ylo[0], ylo[1]), fminf(ylo[2], ylo[3])), hi4 = fmaxf(fmaxf(yhi[0], yhi[1]), fmaxf(yhi[2], yhi[3]));
     lo4 = fminf(fmaxf(lo4, -1.0f), 1.0e6f); hi4 = fminf(fmaxf(hi4, -1.0f), 1.0e6f);
     int ra = min(y1, max(y0, (int) floorf(lo4))), rb = max(ra, min(y1, (int) ceilf(hi4) + 1));
-    {   // make the split warp-uniform (lanes past the right edge have already returned)
-        const unsigned m = __activemask();
-        ra = __reduce_min_sync(m, ra); rb = __reduce_max_sync(m, rb);
-    }
-    zero_rows(fb, x, p.w, y0, ra);
+    // make the split warp-uniform (lanes past the right edge have already returned)
+    const unsigned lanes = __activemask();
+    ra = __reduce_min_sync(lanes, ra); rb = __reduce_max_sync(lanes, rb);
+    // zero rows on both sides of the line: store those the previous frame in this slot may have left non-zero
+    uint32_t* const mark = mark_word(a, p, stream, x, y0);
+    const uint32_t old = mark_load(a, mark, y0, y1, lanes);
+    int s0, s1;
+    dirty_zero_span(old, y0, ra, &s0, &s1);
+    zero_rows(fb, x, p.w, s0, s1);
     for (int y = ra; y < rb; ++y) {
         const float fy = (float) y;
         uint32_t px[4];
@@ -327,7 +354,9 @@ raster_wave_kernel(const __grid_constant__ RasterArgs a, const __grid_constant__
         }
         store4(fb + (size_t) y * p.w, x, p.w, px);
     }
-    zero_rows(fb, x, p.w, rb, y1);
+    dirty_zero_span(old, rb, y1, &s0, &s1);
+    zero_rows(fb, x, p.w, s0, s1);
+    mark_store(mark, ra, rb);
 }
 
 // circle: stage 1 (polar line test) is evaluated once per pixel of a tile + 1-pixel halo into shared
@@ -745,7 +774,7 @@ static int pick_block_x(int quads) {       // threads per row-segment: prefer an
     return 128;
 }
 
-int launch_raster(const glava_b200_params& p, const RasterArgs& a, void* stream, int* launched) {
+int launch_raster(const glava_b200_params& p, const RasterArgs& a, void* stream, int* launched, int* mark_key) {
     cudaStream_t st = (cudaStream_t) stream;
     const int quads = (p.w + 3) / 4;
     // The specialised kernels assume native opacity (a fragment left at vec4(0) stores 0, whole zero rows / discs are skipped);
@@ -758,12 +787,14 @@ int launch_raster(const glava_b200_params& p, const RasterArgs& a, void* stream,
                             && !(p.radial_bar_outline_width > 0.0f);      // the cache holds two values per pixel, the end cap needs three
     int bx = (fast_bars || fast_graph || fast_wave) ? pick_block_x(quads) : 128;
     if (bx > 256) bx = 256;
-    // rows per CTA.  bars: on an H100 SXM (400 W limit), 1080p x 1024 streams with the spectrum kernel co-running, 68 / 135 / 270
-    // rows and 96 / 160 threads per CTA were within 1 % of each other (~360 k frames/s).  graph / wave pay a per-thread column
+    // rows per CTA.  bars: with the dirty-row marks a band above the bars stores nothing but still pays the per-column set-up, so
+    // taller bands win.  On an H100 SXM (700 W limit), 1080p x 1024 streams, bench steps: 135 / 270 / 360 / 540 / 1080 rows gave
+    // 3.60 / 4.66 / 4.81 / 4.87 / 4.94 M frames/s (tools/tune_raster.py); 540 keeps two bands per column for small batches, and
+    // 96 / 160 / 256 threads per CTA were within 0.2 % there.  graph / wave pay a per-thread column
     // set-up, so whole columns without the column table; with it (a.coltab) their set-up is six loads and short bands win
     // (tools/gw_tune.py sweeps them); radial-from-cache 45.
     const bool coltab = a.coltab && (fast_graph || fast_wave);
-    int rows = fast_bars ? 135 : ((fast_graph || fast_wave) ? (coltab ? (fast_wave ? 16 : 30) : 720) : (geo_radial ? 45 : 8));
+    int rows = fast_bars ? 540 : ((fast_graph || fast_wave) ? (coltab ? (fast_wave ? 16 : 30) : 720) : (geo_radial ? 45 : 8));
     // development overrides for tuning sweeps (tools/tune_raster.py); unset in normal use
     int minb = 4;                                     // graph / wave with the column table: <= 64 registers (4 CTAs of 256; measured ahead) or 48 (5)
     if (const char* e = getenv("GLAVA_B200_GW_MINB")) minb = atoi(e) == 5 ? 5 : 4;
@@ -772,13 +803,22 @@ int launch_raster(const glava_b200_params& p, const RasterArgs& a, void* stream,
     // bars / graph / wave are __launch_bounds__(256); generic and both radial kernels take at most 128 threads
     if (!(fast_bars || fast_graph || fast_wave) && bx > 128) bx = 128;
     if (rows > p.h) rows = p.h;
+    // Dirty-row marks.  Their layout depends on the kernel's band height, and a kernel that keeps none (generic, radial, circle)
+    // can leave non-zero pixels anywhere: they describe the framebuffer only if the previous launch was the same kernel at the
+    // same `rows`.  GLAVA_B200_FULL_STORE=1 (read at every launch) stores every zero row anyway, for same-process A/B timing.
+    const bool keeps_marks = fast_bars || fast_graph || fast_wave;
+    const int key = keeps_marks ? ((fast_bars ? 1 : (fast_graph ? 2 : 3)) | (rows << 2)) : 0;
+    if (keeps_marks && !a.marks) return fail(GLAVA_B200_EINVAL, "raster launch: no dirty-row marks for the bars / graph / wave kernel");
+    const char* full_store = getenv("GLAVA_B200_FULL_STORE");
+    const int marks_valid = (mark_key && key != 0 && *mark_key == key && !(full_store && atoi(full_store) != 0)) ? 1 : 0;
+    if (mark_key) *mark_key = 0;                      // until every launch below is enqueued
     // z dimension limit 65535: chunk the batch
     // one launch covers at most `slots` streams (and at most the grid z limit): with a framebuffer
     // ring (fb_slots < batch) two streams of one launch must never share a slot, and launches on
     // the same stream are ordered, so slot s % slots ends up holding the highest stream mapped to it.
     const int chunk = a.slots < 32768 ? (a.slots > 0 ? a.slots : 1) : 32768;
     for (int s0 = 0; s0 < a.batch; s0 += chunk) {
-        RasterArgs b = a; b.stream0 = a.stream0 + s0;
+        RasterArgs b = a; b.stream0 = a.stream0 + s0; b.marks_valid = marks_valid;
         int nz = a.batch - s0 < chunk ? a.batch - s0 : chunk;
         dim3 grid((quads + bx - 1) / bx, (p.h + rows - 1) / rows, nz);
         if (coltab) {
@@ -812,6 +852,7 @@ int launch_raster(const glava_b200_params& p, const RasterArgs& a, void* stream,
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return fail(GLAVA_B200_ECUDA, "raster kernel launch: %s", cudaGetErrorString(e));
     }
+    if (mark_key) *mark_key = key;
     return 0;
 }
 

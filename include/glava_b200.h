@@ -319,7 +319,10 @@ void* glava_b200_cuda_stream(const glava_b200* r);                              
  *                              consumer stream after the frame without a host round trip (glava_tex hands out the GL
  *                              texture id; here the "texture" is glava_b200_frame_device / _framebuffer_device)
  *   glava_b200_framebuffer_ipc cudaIpcMemHandle_t (64 bytes) of the framebuffer array, for a consumer in another
- *                              process (the OBS-plugin situation, glava-obs/entry.c:141-214) */
+ *                              process (the OBS-plugin situation, glava-obs/entry.c:141-214)
+ * The framebuffer is READ-ONLY for consumers, through these pointers and through the IPC mapping alike: the bars, graph
+ * and wave rasters skip storing rows that they themselves left at zero in that slot, so a pixel written from outside can
+ * survive into later frames.  Copy a frame out before modifying it. */
 int   glava_b200_sizereq(glava_b200* r, int w, int h);
 int   glava_b200_wait_frame(glava_b200* r);
 void* glava_b200_frame_event(const glava_b200* r);
