@@ -8,6 +8,7 @@
 #include "raster_core.h"
 #include "chain_core.h"
 #include "tables.h"
+#include "spectrum_plan.h"
 #include "stream_state_core.h"
 
 #include <cuda_runtime.h>
@@ -55,77 +56,84 @@ bool has_error() { return g_has_error; }
 
 using namespace glb;
 
+// The tables build_tables derives from the parameters (audio-independent), freed and rebuilt together on reconfigure and
+// resize.  Device pointers are owned through glava_b200::allocs; null / 0 where the configuration has none.
+struct ConfigTables {
+    int* need = nullptr; int need_count = 0;                  // lazy K5 need-list [2][need_count]
+    TapEntry* tap_tab = nullptr; int* tap_cnt = nullptr; float* tap_wsum = nullptr; int tap_max = 0;   // its taps, tap-major
+    unsigned char* csr = nullptr; int csr_bytes = 0, csr_idx_off = 0, csr_off_off = 0;   // the same taps, texel-major
+    void* need_blk = nullptr; int need_nblk = 0, need_max_rows = 0;   // k5_need_smem_kernel: blocks of sampled texels
+    float* av_t = nullptr;                                    // k5_need_kernel: transposed pre-smoothing texels
+    K5Table k5 = {}; void* k5_blk = nullptr; void* k5_ent = nullptr; void* k5_wsum = nullptr;   // full-plane K5 tap table
+    void* geo = nullptr; int geo_box[4] = { 0, 0, 0, 0 };     // polar geometry cache (radial / circle), see raster_kernels.cu
+    void* ctile = nullptr; int ctile_nx = 0, ctile_count = 0; // circle: per-tile texel reference ranges (launch_circle_tiles)
+};
+
 struct glava_b200 {
     glava_b200_params p;        // EFFECTIVE parameters the kernels run with: n = setbufsize / setbufscale, accel_fft
                                 // cleared when a transform follows "fft" (render.c:2143-2154)
     glava_b200_params p_user;   // as given (glava_b200_get_params)
-    int n_in;                   // setbufsize: floats per channel the caller hands to glava_b200_update
-    bool post_chain;            // transform_smooth and / or keyframe lerp: the spectrum kernel stops at the float chain
+    int n_in = 0;               // setbufsize: floats per channel the caller hands to glava_b200_update
+    bool post_chain = false;    // transform_smooth and / or keyframe lerp: the spectrum kernel stops at the float chain
                                 // result; upload + K5 run as separate kernels
-    bool interp_on;             // keyframe interpolation active (render.c:1761-1763, 2161-2168)
-    int  kcounter;              // frames since the last modified update (render.c:2380-2383)
-    float* d_scaled[2];         // bufscale output [batch][n] x {l, r}
-    float* d_key[3]; int key_start, key_end;   // keyframe buffers [batch*2][n] (start, end, the one being written)
-    float* d_spec_cur;          // latest post-transform buffer (glava_b200_spectrum)
-    void* d_ts_tab; int ts_asz, ts_lim;        // transform_smooth {smin, smax} table
-    std::atomic<unsigned long long> sizereq;   // pending glava_b200_sizereq: (1 << 63) | w << 32 | h, 0 = none
-    int tap_ku; bool fused_k5, no_texmm;       // environment knobs, read once at creation (DESIGN 6.2)
-    int batch, device, slots;
-    cudaStream_t stream;        // raster kernels, read-backs (the stream glava_b200_cuda_stream returns)
-    cudaStream_t spec_stream;   // spectrum kernels + FIFO ingest, lowest priority: the latency-bound spectrum
-                                // kernel of update i+1 runs under the HBM-bound raster kernel of update i
-    int    tex_cur;             // which half of d_tex the latest spectrum wrote / the raster reads
-    cudaEvent_t ev_spec_done[2], ev_raster_done[2];
+    bool interp_on = false;     // keyframe interpolation active (render.c:1761-1763, 2161-2168)
+    int  kcounter = 0;          // frames since the last modified update (render.c:2380-2383)
+    float* d_scaled[2] = {};    // bufscale output [batch][n] x {l, r}
+    float* d_key[3] = {}; int key_start = 0, key_end = 1;   // keyframe buffers [batch*2][n] (start, end, the one being written)
+    float* d_spec_cur = nullptr;   // latest post-transform buffer (glava_b200_spectrum)
+    void* d_ts_tab = nullptr; int ts_asz = 0, ts_lim = 0;   // transform_smooth {smin, smax} table
+    std::atomic<unsigned long long> sizereq{0};   // pending glava_b200_sizereq: (1 << 63) | w << 32 | h, 0 = none
+    bool no_texmm = false, no_coltab = false;     // GLAVA_B200_NO_TEXMM, _NO_COLTAB, read once at creation (DESIGN 6.2)
+    int batch = 0, device = 0, slots = 0;
+    cudaStream_t stream = nullptr;        // raster kernels, read-backs (the stream glava_b200_cuda_stream returns)
+    cudaStream_t spec_stream = nullptr;   // spectrum kernels + FIFO ingest, lowest priority: the latency-bound spectrum
+                                          // kernel of update i+1 runs under the HBM-bound raster kernel of update i
+    int    tex_cur = 0;         // which half of d_tex the latest spectrum wrote / the raster reads
+    cudaEvent_t ev_spec_done[2] = {}, ev_raster_done[2] = {};
     // inputs
-    float* d_pcm[2][2];         // H2D staging for glava_b200_update, double-buffered  [2][batch][n] x {l, r}
-    int    stage_cur;
-    cudaEvent_t ev_input;       // glava_b200_input_event
-    bool   async_input; int last_in;   // glava_b200_set_async_input: update() does not wait for its H2D copy
-    cudaStream_t copy_stream;   // H2D of update i+1 overlaps the kernels of update i
+    float* d_pcm[2][2] = {};    // H2D staging for glava_b200_update, double-buffered  [2][batch][n] x {l, r}
+    int    stage_cur = 0;
+    cudaEvent_t ev_input = nullptr;   // glava_b200_input_event
+    bool   async_input = false; int last_in = -1;   // glava_b200_set_async_input: update() does not wait for its H2D copy
+    cudaStream_t copy_stream = nullptr;   // H2D of update i+1 overlaps the kernels of update i
     // asynchronous frame read-back: D2D into a staging frame on the raster stream (microseconds), D2H from there on its
     // own stream — the PCIe copy of frame i runs under raster i+1 instead of in front of it
-    cudaStream_t out_stream; uint8_t* d_stage[2]; size_t stage_bytes; int out_cur;
-    cudaEvent_t ev_stage_ready[2], ev_stage_free[2];
-    cudaEvent_t ev_copied[2], ev_free[2];
-    float* d_ring[2][2];        // FIFO rings, ping-pong                      [2][batch][n] x {l, r}
-    int    ring_cur;
-    void* d_chunks; size_t chunks_cap;
+    cudaStream_t out_stream = nullptr; uint8_t* d_stage[2] = {}; size_t stage_bytes = 0; int out_cur = 0;
+    cudaEvent_t ev_stage_ready[2] = {}, ev_stage_free[2] = {};
+    cudaEvent_t ev_copied[2] = {}, ev_free[2] = {};
+    float* d_ring[2][2] = {};   // FIFO rings, ping-pong                      [2][batch][n] x {l, r}
+    int    ring_cur = 0;
+    void* d_chunks = nullptr; size_t chunks_cap = 0;
     // constants
-    double* d_window; float* d_twiddle; void* d_rowtab; int* d_need; int need_count;
-    TapEntry* d_tap_tab; int* d_tap_cnt; float* d_tap_wsum; int tap_max; int epi_n;
-    K5Table k5; void* d_k5_blk; void* d_k5_ent; void* d_k5_wsum;   // full-plane K5 tap table (null: evaluate taps in the kernel)
-    // need-list K5 as its own kernel (one table per channel): the serial per-texel sums run at full occupancy on
-    // (texel, plane) pairs instead of on a sixth of the threads of one spectrum CTA
-    void* d_need_blk; int need_nblk, need_max_rows;    // need-list K5 out of shared memory: blocks of sampled texels (tables.h build_need_blocks)
-    bool k5_split_lazy, csr_in_smem, split_epilogue; int av_t_len; float* d_av_t; int spec_oop, spec_t;   // need-list K5 as its own kernel (k5_need_smem_kernel; k5_need_kernel + transposed copy as the fall-back)
-    unsigned char* d_csr; int csr_bytes, csr_idx_off, csr_off_off;   // the same taps, texel-major, for the shared-memory path
-    void* d_geo; int geo_box[4];   // polar geometry cache (radial / circle), see raster_kernels.cu
-    void* d_ctile; int ctile_nx, ctile_count;   // circle: per-tile texel reference ranges (launch_circle_tiles)
-    float* d_coltab; bool no_coltab;   // graph / wave: per-stream column table (launch_raster fills it), GLAVA_B200_NO_COLTAB
-    uint32_t* d_texmm;             // circle: per-plane {min, max} of the sampled texture, refreshed before each raster
+    double* d_window = nullptr; float* d_twiddle = nullptr; void* d_rowtab = nullptr;
+    ConfigTables tab;           // build_tables
+    SpectrumPlan plan;          // launch structure of the spectrum update (spectrum_plan.h), chosen by build_tables
+    float* d_coltab = nullptr;  // graph / wave: per-stream column table (launch_raster fills it), GLAVA_B200_NO_COLTAB
+    uint32_t* d_texmm = nullptr;   // circle: per-plane {min, max} of the sampled texture, refreshed before each raster
     // state + outputs
-    float* d_spec; float* d_applied; float* d_ring_f;
-    uint16_t* d_gr_store; uint16_t* d_ring_u; uint16_t* d_tex;
-    uint16_t* d_av;             // pre-smoothing textures [batch*2][n] (full-plane K5 runs as its own kernel)
-    uint8_t* d_fb;
+    float* d_spec = nullptr; float* d_applied = nullptr; float* d_ring_f = nullptr;
+    uint16_t* d_gr_store = nullptr; uint16_t* d_ring_u = nullptr; uint16_t* d_tex = nullptr;
+    uint16_t* d_av = nullptr;   // pre-smoothing textures [batch*2][n] (full-plane K5 runs as its own kernel)
+    uint8_t* d_fb = nullptr;
     // dirty-row marks of the framebuffer slots (RasterArgs::marks) and the launch structure that last wrote them
     // (launch_raster; 0 = none: the next bars / graph / wave launch stores every row)
-    uint32_t* d_marks; int mark_key;
-    unsigned long long updates;
+    uint32_t* d_marks = nullptr; int mark_key = 0;
+    unsigned long long updates = 0;
     // per-stream `modified` masks (glava_b200_update_masked): once streams have advanced unevenly, every stream has its
     // own average-ring cursor; words {bit 31 = modified, low bits = cursor} go to the device through a small pinned ring
-    bool desync;
+    bool desync = false;
     std::vector<uint32_t> cursor;          // [batch] modified updates of that stream so far, mod avg_frames (valid once desync)
-    uint32_t* h_umask[4]; uint32_t* d_umask[4]; cudaEvent_t ev_umask[4]; int umask_cur;
+    uint32_t* h_umask[4] = {}; uint32_t* d_umask[4] = {}; cudaEvent_t ev_umask[4] = {}; int umask_cur = 0;
     // per-stream state I/O (glava_b200_save_streams / _load_streams / _reset_streams): two device staging halves, each
     // [chunk table: int stream[k], uint32 cursor[k]][blob segments of k streams], allocated on first use; the tables go up
     // from pinned host buffers.  ev_sst_copied[i]: the H2D copies into half i are done; ev_sst_free[i]: its kernel and D2H
     // copies are done
-    void* d_sst[2]; int* h_sst[2]; cudaEvent_t ev_sst_copied[2], ev_sst_free[2]; int sst_cur, sst_streams; size_t sst_table;
-    uint64_t launches;
+    void* d_sst[2] = {}; int* h_sst[2] = {}; cudaEvent_t ev_sst_copied[2] = {}, ev_sst_free[2] = {};
+    int sst_cur = 0, sst_streams = 0; size_t sst_table = 0;
+    uint64_t launches = 0;
     std::vector<void*> allocs;
     // optional per-kernel device timing (glava_b200_set_timing): events around each launch
-    bool timing;
+    bool timing = false;
     std::vector<cudaEvent_t> ev_spec; // pairs around each spectrum launch (spec_stream)
     std::vector<cudaEvent_t> ev_ras;  // pairs around each raster launch (stream)
 };
@@ -292,56 +300,25 @@ static void dev_free(glava_b200* r, void* ptr) {
     cudaFree(ptr);
 }
 
-// Upload a K5 tap table (tables.h) for k5_table_kernel; slots = {blk, ent, wsum, out} device pointers owned by the handle.
-static int upload_k5_table(glava_b200* r, const K5TableHost& t, K5Table* out, void** slots, bool with_out) {
-    static_assert(sizeof(K5Blk) == sizeof(int4) && sizeof(K5Ent) == sizeof(int2), "table records are read as int4 / int2");
-    int rc;
-    if ((rc = dev_alloc(r, &slots[0], t.blk.size() * sizeof(K5Blk), false)) != 0) return rc;
-    if ((rc = dev_alloc(r, &slots[1], (t.ent.empty() ? 1 : t.ent.size()) * sizeof(K5Ent), false)) != 0) return rc;
-    if ((rc = dev_alloc(r, &slots[2], t.wsum.size() * sizeof(float), false)) != 0) return rc;
-    CU(cudaMemcpyAsync(slots[0], t.blk.data(), t.blk.size() * sizeof(K5Blk), cudaMemcpyHostToDevice, r->stream));
-    if (!t.ent.empty()) CU(cudaMemcpyAsync(slots[1], t.ent.data(), t.ent.size() * sizeof(K5Ent), cudaMemcpyHostToDevice, r->stream));
-    CU(cudaMemcpyAsync(slots[2], t.wsum.data(), t.wsum.size() * sizeof(float), cudaMemcpyHostToDevice, r->stream));
-    if (with_out) {
-        if ((rc = dev_alloc(r, &slots[3], (t.out.empty() ? 1 : t.out.size()) * sizeof(int), false)) != 0) return rc;
-        if (!t.out.empty()) CU(cudaMemcpyAsync(slots[3], t.out.data(), t.out.size() * sizeof(int), cudaMemcpyHostToDevice, r->stream));
-    }
-    CU(cudaStreamSynchronize(r->stream));
-    out->blk = (const int4*) slots[0]; out->ent = (const int2*) slots[1]; out->wsum = (const float*) slots[2];
-    out->out = with_out ? (const int*) slots[3] : nullptr;
-    out->count = (int) t.out.size(); out->max_span = t.max_span;
-    out->smem_bytes = K5_S_PLANES * t.max_span * (int) sizeof(float);
+// A new device allocation owned by the handle, filled from host memory.
+static int dev_upload(glava_b200* r, void** out, const void* src, size_t bytes) {
+    int rc = dev_alloc(r, out, bytes, false);
+    if (rc) return rc;
+    if (bytes) CU(cudaMemcpyAsync(*out, src, bytes, cudaMemcpyHostToDevice, r->stream));
     return 0;
 }
 
-// Full-plane K5 (every texel wanted: lazy_smooth = 0, circle, the optional-stage path): the taps of ALL n output
-// texels (tables.h build_k5_table_host), uploaded for k5_table_kernel.
-static int build_k5_table(glava_b200* r) {
-    K5TableHost t;
-    build_k5_table_host(r->p, &t);
-    if ((size_t) 2 * t.max_span * sizeof(float) > 200 * 1024 || t.ent.size() * sizeof(K5Ent) > ((size_t) 256 << 20)) return 0;   // keep the in-kernel evaluation
-    void* slots[4] = { nullptr, nullptr, nullptr, nullptr };
-    int rc = upload_k5_table(r, t, &r->k5, slots, false);
-    r->d_k5_blk = slots[0]; r->d_k5_ent = slots[1]; r->d_k5_wsum = slots[2];
-    return rc;
-}
-
-// Everything derived from the parameters that does not depend on the audio: the lazy-K5 need-list and tap
-// table, the bars / graph row-colour table, the polar geometry cache.  Called at creation and again by
-// glava_b200_reconfigure (the analogue of a `--pipe` uniform update, render.c:1846-2005).
+// Everything derived from the parameters that does not depend on the audio: the launch structure of the spectrum update
+// (spectrum_plan.h) and the K5 tables it reads, the bars / graph row-colour table, the polar geometry cache.  Called at
+// creation and again by glava_b200_reconfigure (the analogue of a `--pipe` uniform update, render.c:1846-2005) and on resize.
 static int build_tables(glava_b200* r) {
     const glava_b200_params& p = r->p;
     int rc;
-    dev_free(r, r->d_need); dev_free(r, r->d_tap_tab); dev_free(r, r->d_tap_cnt); dev_free(r, r->d_tap_wsum); dev_free(r, r->d_geo);
-    dev_free(r, r->d_k5_blk); dev_free(r, r->d_k5_ent); dev_free(r, r->d_k5_wsum);
-    r->d_k5_blk = r->d_k5_ent = r->d_k5_wsum = nullptr; memset(&r->k5, 0, sizeof(r->k5));
-    dev_free(r, r->d_csr); r->d_csr = nullptr; r->csr_bytes = r->csr_idx_off = r->csr_off_off = 0;
-    dev_free(r, r->d_av_t); r->d_av_t = nullptr;
-    dev_free(r, r->d_need_blk); r->d_need_blk = nullptr; r->need_nblk = r->need_max_rows = 0;
-    dev_free(r, r->d_ctile); r->d_ctile = nullptr; r->ctile_nx = r->ctile_count = 0;
-    r->k5_split_lazy = false; r->csr_in_smem = false; r->av_t_len = 0;
-    r->d_need = nullptr; r->need_count = 0; r->d_tap_tab = nullptr; r->d_tap_cnt = nullptr; r->d_tap_wsum = nullptr;
-    r->tap_max = 0; r->epi_n = 0; r->d_geo = nullptr; r->geo_box[0] = r->geo_box[1] = r->geo_box[2] = r->geo_box[3] = 0;
+    ConfigTables& tb = r->tab;
+    for (void* d : { (void*) tb.need, (void*) tb.tap_tab, (void*) tb.tap_cnt, (void*) tb.tap_wsum, (void*) tb.csr, tb.need_blk,
+                     (void*) tb.av_t, tb.k5_blk, tb.k5_ent, tb.k5_wsum, tb.geo, tb.ctile })
+        dev_free(r, d);
+    tb = ConfigTables();
     if (p.transform_smooth) {
         // transform_smooth's sampling window of output t (render.c:700-707) depends on t and the parameters only:
         // evaluated once on the host (chain_core.h), with the same libm calls and types as the reference
@@ -351,78 +328,63 @@ static int build_tables(glava_b200* r) {
         CU(cudaMemcpyAsync(r->d_ts_tab, tab.data(), (size_t) sz * sizeof(SmoothWin), cudaMemcpyHostToDevice, r->stream));
         CU(cudaStreamSynchronize(r->stream));
     }
-    if (p.lazy_smooth && !r->post_chain) {
-        std::vector<int> lists[2];
-        if (build_need_list(p, lists)) {
-            // need-list, K5 tap table (tap-major, for the L2 path) and its texel-major blob (tables.h)
-            LazyTables t;
-            build_lazy_tables(p, lists, &t);
-            if ((rc = dev_alloc(r, (void**) &r->d_need, t.need.size() * sizeof(int), false)) != 0) return rc;
-            CU(cudaMemcpyAsync(r->d_need, t.need.data(), t.need.size() * sizeof(int), cudaMemcpyHostToDevice, r->stream));
-            CU(cudaStreamSynchronize(r->stream));
-            r->need_count = (int) t.cnt;
-            r->epi_n = getenv("GLAVA_B200_NO_EPI_PRUNE") ? 0 : t.epi_n;
-            if (t.tab.size() * sizeof(TapEntry) <= (size_t) 64 << 20 && !getenv("GLAVA_B200_NO_TAPTAB")) {
-                if ((rc = dev_alloc(r, (void**) &r->d_tap_tab, t.tab.size() * sizeof(TapEntry), false)) != 0) return rc;
-                if ((rc = dev_alloc(r, (void**) &r->d_tap_cnt, t.tcnt.size() * sizeof(int), false)) != 0) return rc;
-                if ((rc = dev_alloc(r, (void**) &r->d_tap_wsum, t.wsum.size() * sizeof(float), false)) != 0) return rc;
-                CU(cudaMemcpyAsync(r->d_tap_tab, t.tab.data(), t.tab.size() * sizeof(TapEntry), cudaMemcpyHostToDevice, r->stream));
-                CU(cudaMemcpyAsync(r->d_tap_cnt, t.tcnt.data(), t.tcnt.size() * sizeof(int), cudaMemcpyHostToDevice, r->stream));
-                CU(cudaMemcpyAsync(r->d_tap_wsum, t.wsum.data(), t.wsum.size() * sizeof(float), cudaMemcpyHostToDevice, r->stream));
-                CU(cudaStreamSynchronize(r->stream));
-                r->tap_max = (int) t.tap_max;
-                // When one channel's blob is small enough for two CTAs per SM to hold it in shared memory next to the FFT
-                // buffers, the kernel's serial per-texel sums read their taps from there (no L2 round trips on the chain).
-                const int base = spectrum_smem_bytes(p.n);
-                const bool fits = base > 0 && base + t.blob <= (size_t) 112 * 1024 && !getenv("GLAVA_B200_NO_SMEM_TAPS");
-                if ((rc = dev_alloc(r, (void**) &r->d_csr, t.csr.size(), false)) != 0) return rc;
-                CU(cudaMemcpyAsync(r->d_csr, t.csr.data(), t.csr.size(), cudaMemcpyHostToDevice, r->stream));
-                CU(cudaStreamSynchronize(r->stream));
-                r->csr_bytes = (int) t.blob; r->csr_idx_off = (int) t.idx_off; r->csr_off_off = (int) t.off_off;
-                r->csr_in_smem = fits;
-                // Need-list K5 as its own kernel (k5_need_smem_kernel / k5_need_kernel, lanes = streams): default whenever the taps do not fit shared
-                // memory next to the FFT, and from setbufsize 4096 up anyway; GLAVA_B200_K5_SPLIT=1 / 0 forces it on / off.
-                const char* ks = getenv("GLAVA_B200_K5_SPLIT");
-                r->k5_split_lazy = ks ? atoi(ks) != 0 : (!fits || p.n >= 4096);
-                r->av_t_len = t.epi_n > 0 ? t.epi_n : p.n;
-                if (r->k5_split_lazy) {
-                    // blocks of sampled texels for the shared-memory form; GLAVA_B200_K5N_SMEM=0 keeps the L2 form (k5_need_kernel)
-                    NeedBlocks nb;
-                    int target = -105, tpb = 16;         // tile rows: 105 % of the tallest window (tables.h), or an absolute number / -per cent
-                    if (const char* e = getenv("GLAVA_B200_K5N_ROWS")) { const int v = atoi(e); if (v >= 32 || v < 0) target = v; }
-                    if (const char* e = getenv("GLAVA_B200_K5N_TPB")) { const int v = atoi(e); if (v >= 1) tpb = v; }
-                    build_need_blocks(t, p.n, target, tpb, &nb);
-                    const char* ke = getenv("GLAVA_B200_K5N_SMEM");
-                    if (nb.nblk > 0 && (size_t) nb.max_rows * 33 * sizeof(float) <= (size_t) 200 * 1024 && !(ke && atoi(ke) == 0)) {
-                        if ((rc = dev_alloc(r, &r->d_need_blk, nb.blk.size() * sizeof(int), false)) != 0) return rc;
-                        CU(cudaMemcpyAsync(r->d_need_blk, nb.blk.data(), nb.blk.size() * sizeof(int), cudaMemcpyHostToDevice, r->stream));
-                        CU(cudaStreamSynchronize(r->stream));
-                        r->need_nblk = nb.nblk; r->need_max_rows = nb.max_rows;
-                    } else if ((rc = dev_alloc(r, (void**) &r->d_av_t, (size_t) 2 * r->av_t_len * r->batch * sizeof(float), true)) != 0) return rc;
-                }
-            }
-        }
+    int sm_count = 0;
+    if (cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, r->device) != cudaSuccess || sm_count <= 0) {
+        cudaGetLastError(); sm_count = 132;                        // H100 SXM
     }
-    if (p.smooth_pass && (!r->d_need || r->post_chain) && !getenv("GLAVA_B200_NO_K5_TABLE")) {
-        if ((rc = build_k5_table(r)) != 0) return rc;
+    SpectrumTables host;
+    const SpectrumKnobs knobs = spectrum_knobs([](const char* name) -> const char* { return getenv(name); });
+    r->plan = plan_spectrum(p, r->post_chain, r->batch, sm_count, knobs, &host);
+    const SpectrumPlan& pl = r->plan;
+    const LazyTables& lt = host.lazy;
+    if (pl.need_list) {
+        if ((rc = dev_upload(r, (void**) &tb.need, lt.need.data(), lt.need.size() * sizeof(int))) != 0) return rc;
+        tb.need_count = (int) lt.cnt;
+    }
+    if (pl.tap_table) {
+        // tap-major for the L2 path, texel-major blob per channel for the shared-memory path and the need-list kernels
+        if ((rc = dev_upload(r, (void**) &tb.tap_tab, lt.tab.data(), lt.tab.size() * sizeof(TapEntry))) != 0 ||
+            (rc = dev_upload(r, (void**) &tb.tap_cnt, lt.tcnt.data(), lt.tcnt.size() * sizeof(int))) != 0 ||
+            (rc = dev_upload(r, (void**) &tb.tap_wsum, lt.wsum.data(), lt.wsum.size() * sizeof(float))) != 0 ||
+            (rc = dev_upload(r, (void**) &tb.csr, lt.csr.data(), lt.csr.size())) != 0) return rc;
+        tb.tap_max = (int) lt.tap_max;
+        tb.csr_bytes = (int) lt.blob; tb.csr_idx_off = (int) lt.idx_off; tb.csr_off_off = (int) lt.off_off;
+    }
+    if (pl.k5 == K5Form::NEED_SMEM) {
+        const NeedBlocks& nb = host.blocks;
+        if ((rc = dev_upload(r, &tb.need_blk, nb.blk.data(), nb.blk.size() * sizeof(int))) != 0) return rc;
+        tb.need_nblk = nb.nblk; tb.need_max_rows = nb.max_rows;
+    } else if (pl.k5 == K5Form::NEED_L2) {
+        if ((rc = dev_alloc(r, (void**) &tb.av_t, (size_t) 2 * pl.av_t_len * r->batch * sizeof(float), true)) != 0) return rc;
+    }
+    if (pl.full_table) {
+        // the taps of ALL n output texels (tables.h build_k5_table_host) for k5_table_kernel
+        static_assert(sizeof(K5Blk) == sizeof(int4) && sizeof(K5Ent) == sizeof(int2), "table records are read as int4 / int2");
+        const K5TableHost& kt = host.full;
+        if ((rc = dev_upload(r, &tb.k5_blk, kt.blk.data(), kt.blk.size() * sizeof(K5Blk))) != 0 ||
+            (rc = dev_upload(r, &tb.k5_ent, kt.ent.data(), kt.ent.size() * sizeof(K5Ent))) != 0 ||
+            (rc = dev_upload(r, &tb.k5_wsum, kt.wsum.data(), kt.wsum.size() * sizeof(float))) != 0) return rc;
+        tb.k5.blk = (const int4*) tb.k5_blk; tb.k5.ent = (const int2*) tb.k5_ent; tb.k5.wsum = (const float*) tb.k5_wsum;
+        tb.k5.out = nullptr; tb.k5.count = (int) kt.out.size(); tb.k5.max_span = kt.max_span;
+        tb.k5.smem_bytes = K5_S_PLANES * kt.max_span * (int) sizeof(float);
     }
     if (p.module == GLAVA_B200_MOD_BARS || p.module == GLAVA_B200_MOD_GRAPH) { if ((rc = launch_bars_rowtab(p, r->d_rowtab, r->stream)) != 0) return rc; ++r->launches; }
     // polar modules: cache the audio-independent per-pixel geometry (circle: only when the module samples a
     // pre-smoothed texture, i.e. smooth_audio() is a single texelFetch)
     if (p.module == GLAVA_B200_MOD_RADIAL || (p.module == GLAVA_B200_MOD_CIRCLE && p.smooth_pass)) {
-        const size_t bytes = polar_geo_box(p, r->geo_box);
+        const size_t bytes = polar_geo_box(p, tb.geo_box);
         if (bytes > 0 && bytes <= ((size_t) 512 << 20) && !getenv("GLAVA_B200_NO_GEO")) {
-            if ((rc = dev_alloc(r, &r->d_geo, bytes, false)) != 0) return rc;
-            if ((rc = launch_polar_geo(p, r->d_geo, r->geo_box, r->stream)) != 0) return rc;
+            if ((rc = dev_alloc(r, &tb.geo, bytes, false)) != 0) return rc;
+            if ((rc = launch_polar_geo(p, tb.geo, tb.geo_box, r->stream)) != 0) return rc;
             ++r->launches;
             // per-tile annulus from bucketed texture min / max (DESIGN 4.2): off by default, GLAVA_B200_CTILE=1 enables it (the
             // curve's halo keeps most tiles of the annulus alive and every live tile pays the bucket reduction)
             if (p.module == GLAVA_B200_MOD_CIRCLE && getenv("GLAVA_B200_CTILE")) {
                 int ntx = 0, nty = 0;
-                const size_t tb = circle_tile_bytes(p, &ntx, &nty);
-                if ((rc = dev_alloc(r, &r->d_ctile, tb, false)) != 0) return rc;
-                if ((rc = launch_circle_tiles(p, r->d_geo, r->geo_box, r->d_ctile, r->stream)) != 0) return rc;
-                r->ctile_nx = ntx; r->ctile_count = ntx * nty;
+                const size_t tile_bytes = circle_tile_bytes(p, &ntx, &nty);
+                if ((rc = dev_alloc(r, &tb.ctile, tile_bytes, false)) != 0) return rc;
+                if ((rc = launch_circle_tiles(p, tb.geo, tb.geo_box, tb.ctile, r->stream)) != 0) return rc;
+                tb.ctile_nx = ntx; tb.ctile_count = ntx * nty;
                 r->launches += 2;
             }
         }
@@ -547,41 +509,8 @@ glava_b200* glava_b200_new(const glava_b200_params* params, int batch, int devic
     glava_b200* r = new glava_b200();
     r->p_user = *params; r->batch = batch; r->device = device;
     derive(r);
-    r->sizereq.store(0);
-    { const char* e = getenv("GLAVA_B200_TAP_KU"); r->tap_ku = e ? atoi(e) : 8; }
-    r->fused_k5 = getenv("GLAVA_B200_FUSED_K5") != nullptr;
-    // Launch structure of the lazy pipeline-B update (DESIGN 4.1): wherever the need-list K5 runs as its own kernel (auto: an
-    // FFT size >= 4096, or taps too large for shared memory: build_tables) the R16 state update does too, and at an FFT size
-    // of 8192 the FFT passes run out of place with 256 threads — the measured optima (tools/variant_sweep.sh).  The FFT size
-    // is the one the kernels run at, r->p.n = setbufsize / setbufscale.  GLAVA_B200_SPLIT_EPI / _SPEC_OOP / _SPEC_T override.
-    { const char* e = getenv("GLAVA_B200_SPLIT_EPI"); r->split_epilogue = e ? atoi(e) != 0 : true; }
-    { const char* e = getenv("GLAVA_B200_SPEC_OOP"); r->spec_oop = e ? atoi(e) : (r->p.n == 8192 ? 1 : 0); }
-    { const char* e = getenv("GLAVA_B200_SPEC_T"); r->spec_t = e ? atoi(e) : (r->p.n == 8192 ? 256 : 0); }
     r->no_texmm = getenv("GLAVA_B200_NO_TEXMM") != nullptr;
     r->no_coltab = getenv("GLAVA_B200_NO_COLTAB") != nullptr;
-    r->kcounter = 0; r->d_scaled[0] = r->d_scaled[1] = nullptr; r->d_key[0] = r->d_key[1] = r->d_key[2] = nullptr;
-    r->key_start = 0; r->key_end = 1; r->d_spec_cur = nullptr; r->d_ts_tab = nullptr; r->ts_asz = r->ts_lim = 0;
-    r->stream = nullptr; r->spec_stream = nullptr; r->tex_cur = 0; r->ring_cur = 0;
-    for (int i = 0; i < 2; ++i) { r->ev_spec_done[i] = nullptr; r->ev_raster_done[i] = nullptr; } r->d_chunks = nullptr; r->chunks_cap = 0;
-    r->d_window = nullptr; r->d_twiddle = nullptr; r->d_rowtab = nullptr; r->d_need = nullptr; r->need_count = 0;
-    r->d_tap_tab = nullptr; r->d_tap_cnt = nullptr; r->d_tap_wsum = nullptr; r->tap_max = 0; r->epi_n = 0;
-    r->d_csr = nullptr; r->csr_bytes = r->csr_idx_off = r->csr_off_off = 0;
-    r->d_k5_blk = r->d_k5_ent = r->d_k5_wsum = nullptr; memset(&r->k5, 0, sizeof(r->k5));
-    r->k5_split_lazy = false; r->csr_in_smem = false; r->av_t_len = 0; r->d_av_t = nullptr;
-    r->d_need_blk = nullptr; r->need_nblk = r->need_max_rows = 0;
-    r->d_ctile = nullptr; r->ctile_nx = r->ctile_count = 0;
-    r->d_geo = nullptr; r->geo_box[0] = r->geo_box[1] = r->geo_box[2] = r->geo_box[3] = 0;
-    r->d_spec = r->d_applied = r->d_ring_f = nullptr; r->d_gr_store = r->d_ring_u = r->d_tex = nullptr; r->d_av = nullptr; r->d_texmm = nullptr; r->d_coltab = nullptr; r->d_fb = nullptr;
-    r->d_marks = nullptr; r->mark_key = 0;
-    for (int i = 0; i < 2; ++i) { r->d_pcm[i][0] = r->d_pcm[i][1] = nullptr; r->ev_copied[i] = r->ev_free[i] = nullptr; }
-    r->stage_cur = 0; r->copy_stream = nullptr;
-    r->out_stream = nullptr; r->d_stage[0] = r->d_stage[1] = nullptr; r->stage_bytes = 0; r->out_cur = 0;
-    for (int i = 0; i < 2; ++i) { r->ev_stage_ready[i] = nullptr; r->ev_stage_free[i] = nullptr; }
-    r->updates = 0; r->launches = 0; r->timing = false;
-    r->desync = false; r->umask_cur = 0; r->async_input = false; r->last_in = -1; r->ev_input = nullptr;
-    for (int i = 0; i < 4; ++i) { r->h_umask[i] = nullptr; r->d_umask[i] = nullptr; r->ev_umask[i] = nullptr; }
-    for (int i = 0; i < 2; ++i) { r->d_sst[i] = nullptr; r->h_sst[i] = nullptr; r->ev_sst_copied[i] = r->ev_sst_free[i] = nullptr; }
-    r->sst_cur = 0; r->sst_streams = 0; r->sst_table = 0;
     if (build(r) != 0) { glava_b200_destroy(r); return nullptr; }
     return r;
 }
@@ -778,14 +707,21 @@ static int run_update(glava_b200* r, const float* d_l, const float* d_r, int mod
         a.pcm_l = d_l; a.pcm_r = d_r; a.window = r->d_window; a.twiddle = r->d_twiddle;
         a.spec = chain_out; a.skip_tex = r->post_chain ? 1 : 0; a.applied = r->d_applied; a.ring_f = r->d_ring_f;
         a.gr_store = r->d_gr_store; a.ring_u = r->d_ring_u; a.tex = tex_half(r, b);
-        const bool split_lazy = r->k5_split_lazy && p.lazy_smooth && r->d_need && !r->post_chain && p.smooth_pass;
-        a.need = (p.lazy_smooth && r->d_need && !split_lazy) ? r->d_need : nullptr; a.need_count = r->need_count;
-        a.tap_tab = a.need ? r->d_tap_tab : nullptr; a.tap_cnt = r->d_tap_cnt; a.tap_wsum = r->d_tap_wsum; a.tap_max = r->tap_max;
-        a.epi_n = (a.need || split_lazy) ? r->epi_n : 0;
-        a.tap_ku = r->tap_ku;
-        a.csr = (a.need && a.tap_tab && r->csr_in_smem) ? r->d_csr : nullptr; a.csr_bytes = r->csr_bytes; a.csr_idx_off = r->csr_idx_off; a.csr_off_off = r->csr_off_off;
+        // the launch structure build_tables chose (spectrum_plan.h)
+        const SpectrumPlan& pl = r->plan;
+        const ConfigTables& tb = r->tab;
+        const bool need_in_kernel = pl.k5 == K5Form::TAPS_SMEM || pl.k5 == K5Form::TAPS_L2 || pl.k5 == K5Form::TAPS_DIRECT;
+        const bool need_kernel = pl.k5 == K5Form::NEED_SMEM || pl.k5 == K5Form::NEED_L2;
+        // full-plane smoothing (every texel wanted): the spectrum kernel exports the pre-smoothing texture and
+        // a second kernel smooths all planes, sharing the tap weights between planes
+        const bool planes_kernel = !r->post_chain && (pl.k5 == K5Form::FULL_TABLE || pl.k5 == K5Form::FULL_PLANES);
+        a.need = need_in_kernel ? tb.need : nullptr; a.need_count = tb.need_count;
+        a.tap_tab = a.need ? tb.tap_tab : nullptr; a.tap_cnt = tb.tap_cnt; a.tap_wsum = tb.tap_wsum; a.tap_max = tb.tap_max;
+        a.epi_n = pl.epi_n;
+        a.tap_ku = pl.tap_ku;
+        a.csr = pl.k5 == K5Form::TAPS_SMEM ? tb.csr : nullptr; a.csr_bytes = tb.csr_bytes; a.csr_idx_off = tb.csr_idx_off; a.csr_off_off = tb.csr_off_off;
         a.batch = r->batch; a.update = r->updates;
-        a.variant_oop = r->spec_oop; a.variant_t = r->spec_t;
+        a.variant_oop = pl.fft_oop; a.variant_t = pl.fft_t;
         a.umask = nullptr; a.tex_prev = tex_half(r, r->tex_cur);
         if (mask || r->desync) { if ((rc = stage_umask(r, mask, &a.umask)) != 0) return rc; }
         const int F = p.avg_frames;
@@ -798,36 +734,29 @@ static int run_update(glava_b200* r, const float* d_l, const float* d_r, int mod
         a.avg_b_windowed = (p.avg_window && F != 2) ? 1 : 0;
         const bool is_fft = p.module != GLAVA_B200_MOD_WAVE;
         if (r->timing && (rc = timing_mark(r->ev_spec, r->spec_stream)) != 0) return rc;
-        // full-plane smoothing (every texel wanted): the spectrum kernel exports the pre-smoothing texture and
-        // a second kernel smooths all planes, sharing the tap weights between planes
-        const bool split_k5 = p.smooth_pass && !a.need && !r->post_chain && !r->fused_k5 && !split_lazy;
-        a.av_out = (split_k5 || split_lazy) ? r->d_av : nullptr;
-        a.av_t_len = split_lazy ? r->av_t_len : 0;
+        a.av_out = (planes_kernel || need_kernel) ? r->d_av : nullptr;
+        a.av_t_len = need_kernel ? pl.av_t_len : 0;
         // three-kernel form of the lazy pipeline-B update: transform_fft only in the plane-per-CTA kernel, the R16 state
         // update as an elementwise kernel, K5 on (texel, stream) pairs.  Every F: at F = 1 epilogue_b_kernel<0> keeps no ring.
-        const int epi8 = ((r->epi_n + 7) / 8) * 8;
-        const bool split_epi = split_lazy && is_fft && p.accel_fft && r->split_epilogue && epi8 > 0 && epi8 <= p.n && F >= 1;
-        a.fft_only = split_epi ? 1 : 0;
-        if (split_epi) a.epi_n = epi8;
-        if ((rc = launch_spectrum(p, a, is_fft, r->spec_stream)) != 0) return rc;
-        if (split_epi) {
-            if ((rc = launch_epilogue_b(p, a, epi8, r->spec_stream)) != 0) return rc;
+        a.fft_only = pl.split_epilogue ? 1 : 0;
+        if ((rc = launch_spectrum(p, a, is_fft, pl.spec_grid, pl.spec_resident, r->spec_stream)) != 0) return rc;
+        if (pl.split_epilogue) {
+            if ((rc = launch_epilogue_b(p, a, pl.epi_n, r->spec_stream)) != 0) return rc;
             ++r->launches;
         }
-        if (split_lazy) {
-            if (r->d_need_blk) {
-                if ((rc = launch_k5_need_smem(p, r->d_av, a.tex, r->batch, is_fft ? 2 : 1, r->d_csr, r->csr_bytes, r->csr_idx_off, r->csr_off_off,
-                                              r->d_need, r->d_tap_wsum, r->need_count, r->d_need_blk, r->need_nblk, r->need_max_rows, r->spec_stream)) != 0) return rc;
-                r->launches += 1;
-            } else {
-                if ((rc = launch_k5_need(p, r->d_av, r->d_av_t, r->av_t_len, a.tex, r->batch, is_fft ? 2 : 1, r->d_csr, r->csr_bytes, r->csr_idx_off,
-                                         r->csr_off_off, r->d_need, r->d_tap_wsum, r->need_count, r->spec_stream)) != 0) return rc;
-                r->launches += 2;
-            }
+        if (pl.k5 == K5Form::NEED_SMEM) {
+            if ((rc = launch_k5_need_smem(p, r->d_av, a.tex, r->batch, is_fft ? 2 : 1, tb.csr, tb.csr_bytes, tb.csr_idx_off, tb.csr_off_off,
+                                          tb.need, tb.tap_wsum, tb.need_count, tb.need_blk, tb.need_nblk, tb.need_max_rows, pl.k5n_warps,
+                                          r->spec_stream)) != 0) return rc;
+            r->launches += 1;
+        } else if (pl.k5 == K5Form::NEED_L2) {
+            if ((rc = launch_k5_need(p, r->d_av, tb.av_t, pl.av_t_len, a.tex, r->batch, is_fft ? 2 : 1, tb.csr, tb.csr_bytes, tb.csr_idx_off,
+                                     tb.csr_off_off, tb.need, tb.tap_wsum, tb.need_count, pl.k5n_s, pl.k5n_warps, r->spec_stream)) != 0) return rc;
+            r->launches += 2;
         }
-        if (split_k5) {
+        if (planes_kernel) {
             // wave uses plane 0 of each stream only; smoothing the (zero) odd planes too keeps the launch simple
-            if ((rc = launch_smooth_only(p, r->d_av, a.tex, r->batch * 2, r->spec_stream, &r->k5)) != 0) return rc;
+            if ((rc = launch_smooth_only(p, r->d_av, a.tex, r->batch * 2, r->spec_stream, &tb.k5)) != 0) return rc;
             ++r->launches;
         }
         if (r->post_chain && p.transform_smooth == 1) {                     // render.c:694-718, after the module's chain
@@ -857,7 +786,7 @@ static int run_update(glava_b200* r, const float* d_l, const float* d_r, int mod
         if (rc) return rc;
         ++r->launches;
         if (p.smooth_pass) {
-            if ((rc = launch_smooth_only(p, r->d_av, tex_half(r, b), planes, r->spec_stream, &r->k5)) != 0) return rc;
+            if ((rc = launch_smooth_only(p, r->d_av, tex_half(r, b), planes, r->spec_stream, &r->tab.k5)) != 0) return rc;
             ++r->launches;
         }
         if (modified && r->timing && (rc = timing_mark(r->ev_spec, r->spec_stream)) != 0) return rc;
@@ -875,7 +804,7 @@ static int run_update(glava_b200* r, const float* d_l, const float* d_r, int mod
     ra.tex = tex_half(r, b); ra.fb = r->d_fb;
     ra.rowtab = (p.module == GLAVA_B200_MOD_BARS || p.module == GLAVA_B200_MOD_GRAPH) ? r->d_rowtab : nullptr;
     ra.batch = r->batch; ra.slots = r->slots; ra.stream0 = 0;
-    ra.geo = r->d_geo; ra.gx0 = r->geo_box[0]; ra.gy0 = r->geo_box[1]; ra.gw = r->geo_box[2]; ra.gh = r->geo_box[3];
+    ra.geo = r->tab.geo; ra.gx0 = r->tab.geo_box[0]; ra.gy0 = r->tab.geo_box[1]; ra.gw = r->tab.geo_box[2]; ra.gh = r->tab.geo_box[3];
     ra.texmm = nullptr; ra.ctile = nullptr; ra.ctile_zero = nullptr; ra.ctile_nx = 0;
     ra.coltab = r->no_coltab ? nullptr : r->d_coltab;
     ra.marks = r->d_marks; ra.marks_valid = 0;            // launch_raster decides from r->mark_key
@@ -891,7 +820,7 @@ static int run_update(glava_b200* r, const float* d_l, const float* d_r, int mod
         if ((rc = launch_texmm(p, ra.tex, r->d_texmm, r->batch * 2, r->stream)) != 0) return rc;
         ++r->launches;
         ra.texmm = r->d_texmm;
-        if (r->d_ctile) { ra.ctile = (const int4*) r->d_ctile; ra.ctile_zero = (const int*) ((const int4*) r->d_ctile + r->ctile_count); ra.ctile_nx = r->ctile_nx; }
+        if (r->tab.ctile) { ra.ctile = (const int4*) r->tab.ctile; ra.ctile_zero = (const int*) ((const int4*) r->tab.ctile + r->tab.ctile_count); ra.ctile_nx = r->tab.ctile_nx; }
     }
     if (r->timing && (rc = timing_mark(r->ev_ras, r->stream)) != 0) return rc;
     int raster_launches = 0;
@@ -1207,7 +1136,7 @@ int glava_b200_smooth_pass(glava_b200* r, const uint16_t* in, uint16_t* out, int
     int rc = 0;
     do {
         if (cudaMemcpyAsync(d_in, in, bytes, cudaMemcpyHostToDevice, r->stream) != cudaSuccess) { rc = fail(GLAVA_B200_ECUDA, "H2D copy failed"); break; }
-        if ((rc = launch_smooth_only(r->p, d_in, d_out, count, r->stream, &r->k5)) != 0) break;
+        if ((rc = launch_smooth_only(r->p, d_in, d_out, count, r->stream, &r->tab.k5)) != 0) break;
         ++r->launches;
         if (cudaMemcpyAsync(out, d_out, bytes, cudaMemcpyDeviceToHost, r->stream) != cudaSuccess) { rc = fail(GLAVA_B200_ECUDA, "D2H copy failed"); break; }
         cudaError_t se = cudaStreamSynchronize(r->stream);

@@ -105,7 +105,8 @@ struct RasterArgs {
 #define GLB_TEXMM_STRIDE (2 + 2 * GLB_CIRCLE_NB)  // u32 per plane
 
 // ---- kernel launchers (spectrum_kernels.cu, raster_kernels.cu); `stream` is a cudaStream_t passed as void* ------------------
-int launch_spectrum(const glava_b200_params& p, const SpectrumArgs& a, bool is_fft, void* stream);
+// grid, resident: SpectrumPlan::spec_grid, ::spec_resident (spectrum_plan.h)
+int launch_spectrum(const glava_b200_params& p, const SpectrumArgs& a, bool is_fft, int grid, int resident, void* stream);
 // Full-plane K5 tap table (built once per parameter set, capi.cu): for every block of K5_BLOCK output texels the taps of
 // all its texels, tap-major and padded to the block's longest sum with zero-weight entries, so a warp's loads coalesce
 // and the tap loop is uniform.
@@ -121,21 +122,21 @@ struct K5Table {
 #ifndef K5_BLOCK
 #define K5_BLOCK 128
 #endif
-#define K5_S_PLANES 8        // planes that share one tap (K5_S in spectrum_kernels.cu)
 // planes handled: plane(i) = i * plane_stride + plane_offset for i in [0, count) — stride 2 / offset ch walks one channel's
 // planes of the interleaved [batch][2] layout (need-list tables differ per channel)
 int launch_smooth_only(const glava_b200_params& p, const uint16_t* d_in, uint16_t* d_out, int count, void* stream,
                        const K5Table* table = nullptr, int plane_stride = 1, int plane_offset = 0);
 // need-list K5, lanes = streams (d_av [batch*2][n] u16 as exported by the spectrum kernel -> transposed float d_av_t): csr = the texel-major tap blobs of SpectrumArgs (per channel float w[] | u16 idx[] | int off[]),
-// need / wsum = [2][need_count]; av_t as exported by the spectrum kernel; writes tex[(stream * 2 + ch) * n + need[k]]
+// need / wsum = [2][need_count]; av_t as exported by the spectrum kernel; writes tex[(stream * 2 + ch) * n + need[k]];
+// S streams per lane, wpc warps per CTA (SpectrumPlan::k5n_s, ::k5n_warps)
 int launch_k5_need(const glava_b200_params& p, const uint16_t* d_av, float* d_av_t, int av_t_len, uint16_t* d_tex, int batch, int channels,
                    const unsigned char* d_csr, int csr_bytes, int csr_idx_off, int csr_off_off, const int* d_need,
-                   const float* d_wsum, int need_count, void* stream);
+                   const float* d_wsum, int need_count, int S, int wpc, void* stream);
 // the same need-list K5 from shared-memory tiles over blocks of sampled texels (tables.h build_need_blocks); reads the
 // [plane][bin] R16 texture directly
 int launch_k5_need_smem(const glava_b200_params& p, const uint16_t* d_av, uint16_t* d_tex, int batch, int channels,
                         const unsigned char* d_csr, int csr_bytes, int csr_idx_off, int csr_off_off, const int* d_need,
-                        const float* d_wsum, int need_count, const void* d_blocks, int nblk, int max_rows, void* stream);
+                        const float* d_wsum, int need_count, const void* d_blocks, int nblk, int max_rows, int wpc, void* stream);
 // pipeline B epilogue as its own elementwise kernel: spec (transform_fft output) -> upload quantisation, K1 - K4 on the R16
 // state, pre-smoothing texels into av_out (leading `bins` of every plane; bins is a multiple of 8)
 int launch_epilogue_b(const glava_b200_params& p, const SpectrumArgs& a, int bins, void* stream);
@@ -152,7 +153,6 @@ size_t circle_tile_bytes(const glava_b200_params& p, int* ntx, int* nty);
 int launch_circle_tiles(const glava_b200_params& p, const void* d_geo, const int box[4], void* d_tiles, void* stream);
 int launch_fifo_ingest(const glava_b200_params& p, const void* d_chunks, bool float_in, int frames, const float* src_l, const float* src_r,
                        float* dst_l, float* dst_r, int batch, void* stream);
-int spectrum_smem_bytes(int n);
 int spectrum_threads(int n);
 // chain_kernels.cu: optional stages of rd_update (bufscale, transform_smooth, keyframe lerp + R16 upload)
 int launch_bufscale(const float* in_l, const float* in_r, float* out_l, float* out_r, int batch, int n_in, int k,

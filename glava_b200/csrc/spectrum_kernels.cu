@@ -12,10 +12,10 @@
 // Compiled with --fmad=false: results are bit-identical to the host build of the *_core.h maths.
 #include "internal.h"
 #include "raster_core.h"
+#include "spectrum_plan.h"
 
 #include <cuda_runtime.h>
 
-#include <cstdlib>
 #include <type_traits>
 
 namespace glb {
@@ -39,12 +39,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         "{\n .reg .pred p;\n WAIT_%=:\n"
         " mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
         " @p bra DONE_%=;\n bra WAIT_%=;\n DONE_%=:\n}\n" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-
-static int device_sm_count() {
-    int dev = 0, n = 0;
-    if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    return n > 0 ? n : 132;                              // H100 SXM
 }
 
 // grid.y is limited to 65535 and a batch is not (glava_b200_new takes any batch >= 1): a launcher whose y axis counts planes,
@@ -74,14 +68,13 @@ constexpr int spec_default_threads(int log2n) {
 template <int LOG2N, int TT = 0, bool OOP = false> struct SpecCfg {
     static constexpr int N = 1 << LOG2N, M = N / 2;
     static constexpr int T = TT > 0 ? TT : spec_default_threads(LOG2N);
-    static constexpr int BUF_CPX = fft_padded_size(M);
-    static constexpr int BUF_BYTES = ((BUF_CPX * 8 + 15) / 16) * 16;
-    // in place:     cpx buffer (also the raw-PCM staging area, N floats = M cpx) | u16 av[N] | mbarriers
+    static constexpr int BUF_BYTES = spectrum_buf_bytes(N);
+    // in place:     cpx buffer (also the raw-PCM staging area, N floats = M cpx) | u16 av[N] | mbarriers (spectrum_plan.h)
     // out of place: buffer A (PCM lands here) | buffer B | mbarriers; av[N] lives in whichever buffer the result is NOT in
     static constexpr int OFF_B   = BUF_BYTES;
     static constexpr int OFF_AV  = BUF_BYTES;
-    static constexpr int OFF_BAR = OOP ? 2 * BUF_BYTES : OFF_AV + N * 2;
-    static constexpr int SMEM    = OFF_BAR + 16;
+    static constexpr int SMEM    = OOP ? 2 * BUF_BYTES + 16 : spectrum_smem_bytes(N);
+    static constexpr int OFF_BAR = SMEM - 16;
     static constexpr bool RESULT_IN_B = OOP && (fft_pass_count(M) % 2 == 1);
     // resident CTAs per SM the register allocation must allow: the kernel waits on memory a lot (TMA load,
     // state loads), so occupancy is worth more than the last registers (128 regs -> 2 CTAs/SM was measured)
@@ -465,70 +458,48 @@ int spectrum_threads(int n) {
         case 16384: return SpecCfg<14>::T;  default: return -1;
     }
 }
-int spectrum_smem_bytes(int n) {
-    switch (n) {
-        case 256:   return SpecCfg<8>::SMEM;   case 512:   return SpecCfg<9>::SMEM;
-        case 1024:  return SpecCfg<10>::SMEM;  case 2048:  return SpecCfg<11>::SMEM;
-        case 4096:  return SpecCfg<12>::SMEM;  case 8192:  return SpecCfg<13>::SMEM;
-        case 16384: return SpecCfg<14>::SMEM;  default: return -1;
-    }
-}
-
 template <int LOG2N, bool IS_FFT, int TT = 0, bool OOP = false>
-static int launch_spectrum_t(const glava_b200_params& p, const SpectrumArgs& a, cudaStream_t st) {
+static int launch_spectrum_t(const glava_b200_params& p, const SpectrumArgs& a, int grid, int resident, cudaStream_t st) {
     using C = SpecCfg<LOG2N, TT, OOP>;
     auto kern = spectrum_kernel<LOG2N, IS_FFT, TT, OOP>;
     // Residency cap (tuning aid, off): the kernel co-runs with the raster kernel (capi.cu run_update) and
     // at full occupancy (5 CTAs x 256 threads x 48 registers per SM) takes most of the register file.
-    // Requesting more dynamic shared memory than needed caps it at `cap` CTAs per SM; off, because the
+    // Requesting more dynamic shared memory than needed caps it at `resident` CTAs per SM; off, because the
     // stretched spectrum kernel (and the L1 it takes from the raster kernel) costs more than it frees.
     int smem_req = C::SMEM + (a.csr ? a.csr_bytes : 0);          // + the K5 tap table of one channel (shared-memory K5 path)
-    {
-        static int cap = -1;
-        if (cap < 0) { cap = 0; if (const char* e = getenv("GLAVA_B200_SPEC_RESIDENT")) cap = atoi(e); }
-        if (cap > 0) { int want = (227 * 1024) / cap - 1024; if (want > smem_req) smem_req = want; }
-        if (smem_req > 227 * 1024) smem_req = 227 * 1024;
-    }
+    if (resident > 0) { int want = (227 * 1024) / resident - 1024; if (want > smem_req) smem_req = want; }
+    if (smem_req > 227 * 1024) smem_req = 227 * 1024;
     if (smem_req > 48 * 1024) {
         // per-device function attribute: set on every launch (handles on several devices may live in one process)
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_req);
         if (e != cudaSuccess) return fail(GLAVA_B200_ECUDA, "cudaFuncSetAttribute(spectrum): %s", cudaGetErrorString(e));
     }
-    // Persistent grid: a few CTAs per SM.  Small on purpose — this kernel is latency bound and is meant
-    // to run UNDER the HBM-bound raster kernel of the previous update (capi.cu run_update) without taking
-    // its occupancy away.  GLAVA_B200_SPEC_CTAS_PER_SM overrides (0 = one CTA per work unit).
-    const int sm_count = device_sm_count();
-    // Global-memory tap table: one CTA per unit.  Shared-memory tap table: a persistent grid at the kernel's residency
-    // (2 CTAs per SM) loads the table once per CTA and lets the TMA engine prefetch the next unit's PCM during K5.
-    int per_sm = a.csr ? 2 : 0;
-    if (const char* e = getenv("GLAVA_B200_SPEC_CTAS_PER_SM")) per_sm = atoi(e);
-    const int units = IS_FFT ? a.batch * 2 : a.batch;
-    int grid = (per_sm > 0 && sm_count * per_sm < units) ? sm_count * per_sm : units;
-    if (a.csr && IS_FFT && grid < units && (grid & 1)) ++grid;      // even stride: a persistent CTA stays on one channel (one tap-table load)
     kern<<<grid, C::T, smem_req, st>>>(a, p);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(GLAVA_B200_ECUDA, "spectrum kernel launch: %s", cudaGetErrorString(e));
     return 0;
 }
 
-// Variant selection: default = the measured-best one per size; GLAVA_B200_SPEC_OOP=0|1 and GLAVA_B200_SPEC_T=128|256|512
-// override it for tuning sweeps (tools/spec_probe.py).
+// Variant selection (spectrum_plan.h): default = the measured-best one per size; GLAVA_B200_SPEC_OOP=0|1 and
+// GLAVA_B200_SPEC_T=128|256|512 override it for tuning sweeps (tools/spec_probe.py).
 template <int L>
-static int launch_spectrum_fft(const glava_b200_params& p, const SpectrumArgs& a, cudaStream_t st, int oop, int tsel) {
+static int launch_spectrum_fft(const glava_b200_params& p, const SpectrumArgs& a, int grid, int resident, cudaStream_t st,
+                               int oop, int tsel) {
     if (oop) {
-        if (tsel == 128) return launch_spectrum_t<L, true, 128, true>(p, a, st);
-        if (tsel == 512) { if constexpr (L >= 13) return launch_spectrum_t<L, true, 512, true>(p, a, st); }
-        if (tsel == 1024) { if constexpr (L >= 14) return launch_spectrum_t<L, true, 1024, true>(p, a, st); }
-        return launch_spectrum_t<L, true, 256, true>(p, a, st);
+        if (tsel == 128) return launch_spectrum_t<L, true, 128, true>(p, a, grid, resident, st);
+        if (tsel == 512) { if constexpr (L >= 13) return launch_spectrum_t<L, true, 512, true>(p, a, grid, resident, st); }
+        if (tsel == 1024) { if constexpr (L >= 14) return launch_spectrum_t<L, true, 1024, true>(p, a, grid, resident, st); }
+        return launch_spectrum_t<L, true, 256, true>(p, a, grid, resident, st);
     }
-    if (tsel == 256) { if constexpr (L >= 13) return launch_spectrum_t<L, true, 256, false>(p, a, st); }
-    return launch_spectrum_t<L, true, 0, false>(p, a, st);
+    if (tsel == 256) { if constexpr (L >= 13) return launch_spectrum_t<L, true, 256, false>(p, a, grid, resident, st); }
+    return launch_spectrum_t<L, true, 0, false>(p, a, grid, resident, st);
 }
 
-int launch_spectrum(const glava_b200_params& p, const SpectrumArgs& a, bool is_fft, void* stream) {
+int launch_spectrum(const glava_b200_params& p, const SpectrumArgs& a, bool is_fft, int grid, int resident, void* stream) {
     cudaStream_t st = (cudaStream_t) stream;
-    const int tsel = a.variant_t, oop = a.variant_oop;          // chosen per handle at creation (capi.cu)
-#define GLB_CASE(L) case (1 << L): return is_fft ? launch_spectrum_fft<L>(p, a, st, oop, tsel) : launch_spectrum_t<L, false>(p, a, st);
+    const int tsel = a.variant_t, oop = a.variant_oop;
+#define GLB_CASE(L) case (1 << L): return is_fft ? launch_spectrum_fft<L>(p, a, grid, resident, st, oop, tsel) \
+                                                 : launch_spectrum_t<L, false>(p, a, grid, resident, st);
     switch (p.n) {
         GLB_CASE(8) GLB_CASE(9) GLB_CASE(10) GLB_CASE(11) GLB_CASE(12) GLB_CASE(13) GLB_CASE(14)
         default: return fail(GLAVA_B200_EINVAL, "unsupported setbufsize %d", p.n);
@@ -644,34 +615,23 @@ static int launch_k5_table_t(const glava_b200_params& p, const uint16_t* d_in, u
 int launch_smooth_only(const glava_b200_params& p, const uint16_t* d_in, uint16_t* d_out, int count, void* stream,
                        const K5Table* table, int plane_stride, int plane_offset) {
     if (table && table->blk) {
-        // planes per CTA share every tap's index / weight load: as many as the staged spans leave room for
+        // planes per CTA share every tap's index / weight load (spectrum_plan.h k5_table_planes)
         const bool avg = smooth_params(p).sample_mode == 0;
         cudaStream_t st = (cudaStream_t) stream;
-        const size_t per_plane = (size_t) table->max_span * sizeof(float);
-        if (8 * per_plane <= 200 * 1024)
-            return avg ? launch_k5_table_t<true, 8>(p, d_in, d_out, count, st, *table, plane_stride, plane_offset)
-                       : launch_k5_table_t<false, 8>(p, d_in, d_out, count, st, *table, plane_stride, plane_offset);
-        if (4 * per_plane <= 200 * 1024)
-            return avg ? launch_k5_table_t<true, 4>(p, d_in, d_out, count, st, *table, plane_stride, plane_offset)
-                       : launch_k5_table_t<false, 4>(p, d_in, d_out, count, st, *table, plane_stride, plane_offset);
-        return avg ? launch_k5_table_t<true, 2>(p, d_in, d_out, count, st, *table, plane_stride, plane_offset)
-                   : launch_k5_table_t<false, 2>(p, d_in, d_out, count, st, *table, plane_stride, plane_offset);
+        switch (k5_table_planes(table->max_span)) {
+            case 8: return avg ? launch_k5_table_t<true, 8>(p, d_in, d_out, count, st, *table, plane_stride, plane_offset)
+                               : launch_k5_table_t<false, 8>(p, d_in, d_out, count, st, *table, plane_stride, plane_offset);
+            case 4: return avg ? launch_k5_table_t<true, 4>(p, d_in, d_out, count, st, *table, plane_stride, plane_offset)
+                               : launch_k5_table_t<false, 4>(p, d_in, d_out, count, st, *table, plane_stride, plane_offset);
+            default: return avg ? launch_k5_table_t<true, 2>(p, d_in, d_out, count, st, *table, plane_stride, plane_offset)
+                                : launch_k5_table_t<false, 2>(p, d_in, d_out, count, st, *table, plane_stride, plane_offset);
+        }
     }
     if (plane_stride != 1 || plane_offset != 0) return fail(GLAVA_B200_EINVAL, "smooth pass: strided planes need a tap table");
-    // worst-case span: the last block's taps, bounded by the whole plane
-    const SmoothParams sp = smooth_params(p);
-    const float fn = (float) p.n;
-    int span = 0;
-    for (int x0 = 0; x0 < p.n; x0 += K5_XT) {
-        const int x1 = (x0 + K5_XT < p.n) ? x0 + K5_XT : p.n;
-        const float lo_f = scale_audio(sp, g_clamp(((float) x0 + 0.5f) / fn - sp.smooth_factor, 0.0f, 1.0f)) * fn;
-        const float hi_f = scale_audio(sp, g_clamp(((float) (x1 - 1) + 0.5f) / fn + sp.smooth_factor, 0.0f, 1.0f)) * fn;
-        int lo = (int) floorf(lo_f) - 2, hi = (int) ceilf(hi_f) + 3;
-        lo = lo < 0 ? 0 : lo; hi = hi > p.n ? p.n : hi;
-        if (hi - lo > span) span = hi - lo;
-    }
-    const size_t smem = (size_t) K5_S * (span > 0 ? span : 1) * sizeof(uint16_t);
-    if (smem > 200 * 1024) return fail(GLAVA_B200_EINVAL, "smooth pass: tap span %d too large for shared memory", span);
+    const int span = k5_planes_span(p);
+    const std::string refusal = k5_planes_refusal(span);
+    if (!refusal.empty()) return fail(GLAVA_B200_EINVAL, "%s", refusal.c_str());
+    const size_t smem = k5_planes_smem(span);
     if (smem > 48 * 1024) {
         cudaError_t e = cudaFuncSetAttribute(k5_planes_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
         if (e != cudaSuccess) return fail(GLAVA_B200_ECUDA, "cudaFuncSetAttribute(k5): %s", cudaGetErrorString(e));
@@ -790,7 +750,6 @@ av_transpose_kernel(const uint16_t* __restrict__ av, float* __restrict__ av_t, i
     }
 }
 
-#define K5N_WARPS 4
 template <int MODE, int S, int D>
 __global__ void __launch_bounds__(512)
 k5_need_kernel(const float* __restrict__ av_t, int av_t_len, uint16_t* __restrict__ tex, int n, int batch, int channels,
@@ -918,13 +877,11 @@ k5_need_smem_kernel(const uint16_t* __restrict__ av, uint16_t* __restrict__ tex,
 
 int launch_k5_need_smem(const glava_b200_params& p, const uint16_t* d_av, uint16_t* d_tex, int batch, int channels,
                         const unsigned char* d_csr, int csr_bytes, int csr_idx_off, int csr_off_off, const int* d_need,
-                        const float* d_wsum, int need_count, const void* d_blocks, int nblk, int max_rows, void* stream) {
+                        const float* d_wsum, int need_count, const void* d_blocks, int nblk, int max_rows, int wpc, void* stream) {
     const SmoothParams sp = smooth_params(p);
     cudaStream_t st = (cudaStream_t) stream;
     if (nblk <= 0) return 0;
     const size_t smem = (size_t) max_rows * 33 * sizeof(float);
-    int wpc = 16;
-    if (const char* e = getenv("GLAVA_B200_K5N_WARPS")) { const int v = atoi(e); if (v >= 1 && v <= 16) wpc = v; }
     dim3 grid((unsigned) nblk, (unsigned) ((batch + 31) / 32), (unsigned) channels);
     cudaError_t e;
     if (sp.sample_mode == 0) {
@@ -944,7 +901,7 @@ int launch_k5_need_smem(const glava_b200_params& p, const uint16_t* d_av, uint16
 
 int launch_k5_need(const glava_b200_params& p, const uint16_t* d_av, float* d_av_t, int av_t_len, uint16_t* d_tex, int batch, int channels,
                    const unsigned char* d_csr, int csr_bytes, int csr_idx_off, int csr_off_off, const int* d_need,
-                   const float* d_wsum, int need_count, void* stream) {
+                   const float* d_wsum, int need_count, int S, int wpc, void* stream) {
     const SmoothParams sp = smooth_params(p);
     cudaStream_t st = (cudaStream_t) stream;
     {
@@ -953,16 +910,11 @@ int launch_k5_need(const glava_b200_params& p, const uint16_t* d_av, float* d_av
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return fail(GLAVA_B200_ECUDA, "transpose kernel launch: %s", cudaGetErrorString(e));
     }
-    // streams per lane: 4 sums share every tap broadcast once the batch is large enough to still fill the device;
-    // with few sampled texels (radial: ~90 per channel) two streams per lane do not fill it: one stream per lane there
-    int S = (batch >= 256 && (long long) channels * need_count * ((batch + 63) / 64) >= device_sm_count() * 24) ? 2 : 1;
-    if (const char* e = getenv("GLAVA_B200_K5N_S")) { const int v = atoi(e); if (v == 1 || v == 2 || v == 4) S = v; }
+    // S streams per lane share every tap broadcast (spectrum_plan.h chooses S from the batch)
     const int groups = (batch + 32 * S - 1) / (32 * S);
     const long long warps = (long long) channels * need_count * groups;
     // warps per CTA = consecutive texels of one stream group: their tap windows overlap almost entirely, so the more of them
     // share an SM's L1 the fewer reads go to L2 (the kernel moves 4 bytes per tap and lane: L2 bandwidth is its bound)
-    int wpc = K5N_WARPS;
-    if (const char* e = getenv("GLAVA_B200_K5N_WARPS")) { const int v = atoi(e); if (v >= 1 && v <= 16) wpc = v; }
     const unsigned grid = (unsigned) ((warps + wpc - 1) / wpc);
     if (grid == 0) return 0;
 #define GLB_K5N(M, SS, DD) k5_need_kernel<M, SS, DD><<<grid, wpc * 32, 0, st>>>(d_av_t, av_t_len, d_tex, p.n, batch, channels, d_csr, csr_bytes, \

@@ -35,6 +35,7 @@ def lib():
         L.emul_lazy_epi_n.argtypes = [vp]
         L.emul_k5_table.argtypes = [vp, vp, vp]
         L.emul_table_sizes.argtypes = [vp, i32, i32, i32, vp]
+        L.emul_spectrum_plan.argtypes = [vp, i32, i32, i32, vp, vp, i32, vp, vp, i32]
         L.emul_bufscale.argtypes = [vp, i32, i32, vp]
         L.emul_transform_smooth.argtypes = [vp, i32, C.c_float, C.c_float]
         L.emul_upload.argtypes = [vp, vp, i32, C.c_float, C.c_float, i32, vp]
@@ -143,6 +144,29 @@ def table_sizes(p, target_rows=-105, texels_per_block=16, full=True):
     out = np.zeros(len(TABLE_SIZES), np.int64)
     lib().emul_table_sizes(C.byref(p), target_rows, texels_per_block, 1 if full else 0, out.ctypes.data)
     return dict(zip(TABLE_SIZES, out.tolist()))
+
+
+PLAN_FIELDS = ("need_list", "tap_table", "full_table", "split_epilogue", "epi_n", "av_t_len", "k5", "tap_ku", "table_planes",
+               "k5n_s", "k5n_warps", "fft_oop", "fft_t", "spec_grid", "spec_resident")
+K5_FORMS = ("none", "taps_smem", "taps_l2", "taps_direct", "need_smem", "need_l2", "full_table", "full_planes", "fused")
+
+
+def spectrum_plan(p, post_chain, batch, sm_count, env):
+    """the launch structure the library chooses (spectrum_plan.h plan_spectrum) for the effective parameters p under the
+    environment overrides env ({"K5_SPLIT": "1", ...}, names without GLAVA_B200_) -> dict of PLAN_FIELDS (k5 as a K5_FORMS
+    name) and "refusal" (None: none)"""
+    names = [("GLAVA_B200_" + k).encode() for k in env]
+    values = [str(v).encode() for v in env.values()]
+    n = max(len(names), 1)
+    name_arr = (C.c_char_p * n)(*names); value_arr = (C.c_char_p * n)(*values)
+    out = np.zeros(len(PLAN_FIELDS), np.int64)
+    refusal = C.create_string_buffer(256)
+    lib().emul_spectrum_plan(C.byref(p), int(post_chain), batch, sm_count, name_arr, value_arr, len(names), out.ctypes.data,
+                             refusal, len(refusal))
+    plan = dict(zip(PLAN_FIELDS, out.tolist()))
+    plan["k5"] = K5_FORMS[plan["k5"]]
+    plan["refusal"] = refusal.value.decode() or None
+    return plan
 
 
 def k5_table(p, tex):

@@ -7,6 +7,7 @@
 #include "../../glava_b200/csrc/raster_core.h"
 #include "../../glava_b200/csrc/chain_core.h"
 #include "../../glava_b200/csrc/tables.h"
+#include "../../glava_b200/csrc/spectrum_plan.h"
 
 #include <cmath>
 #include <cstring>
@@ -332,12 +333,12 @@ int emul_lazy_epi_n(const glava_b200_params* pp) {
     build_lazy_tables(*pp, lists, &t);
     return t.epi_n;
 }
-// The sizes capi.cu build_tables / build_k5_table and spectrum_kernels.cu launch_smooth_only choose the K5 launch structure
-// from, computed by the same tables.h builders (out[0] = 0 when the module has no need-list):
+// The sizes spectrum_plan.h chooses the K5 launch structure from, computed by the same tables.h builders (out[0] = 0 when
+// the module has no need-list):
 //   [0] need-list present  [1] entries per channel  [2] texel-major blob bytes per channel  [3] tap-table bytes
 //   [4] epi_n  [5] build_need_blocks max_rows (target_rows, texels_per_block as GLAVA_B200_K5N_ROWS / _TPB)  [6] its nblk
-//   [7] build_k5_table_host max_span  [8] its entry bytes  [9] k5_planes_kernel's widest staged span (launch_smooth_only)
-//   [10] spectrum_kernel's in-place shared memory (SpecCfg<log2 n>::SMEM, spectrum_smem_bytes)
+//   [7] build_k5_table_host max_span  [8] its entry bytes  [9] k5_planes_kernel's widest staged span (k5_planes_span)
+//   [10] spectrum_kernel's in-place shared memory (spectrum_smem_bytes)
 //   ([7], [8] only with `full`: the full table takes seconds to build for wide windows at n = 16384)
 void emul_table_sizes(const glava_b200_params* pp, int target_rows, int texels_per_block, int full, long long* out) {
     const glava_b200_params& p = *pp;
@@ -356,19 +357,25 @@ void emul_table_sizes(const glava_b200_params* pp, int target_rows, int texels_p
         build_k5_table_host(p, &k);
         out[7] = k.max_span; out[8] = (long long) (k.ent.size() * sizeof(K5Ent));
     }
-    const SmoothParams sp = smooth_params(p);
-    const float fn = (float) p.n;
-    int span = 0;
-    for (int x0 = 0; x0 < p.n; x0 += K5_BLOCK) {
-        const int x1 = (x0 + K5_BLOCK < p.n) ? x0 + K5_BLOCK : p.n;
-        const float lo_f = scale_audio(sp, g_clamp(((float) x0 + 0.5f) / fn - sp.smooth_factor, 0.0f, 1.0f)) * fn;
-        const float hi_f = scale_audio(sp, g_clamp(((float) (x1 - 1) + 0.5f) / fn + sp.smooth_factor, 0.0f, 1.0f)) * fn;
-        int lo = (int) floorf(lo_f) - 2, hi = (int) ceilf(hi_f) + 3;
-        lo = lo < 0 ? 0 : lo; hi = hi > p.n ? p.n : hi;
-        if (hi - lo > span) span = hi - lo;
-    }
-    out[9] = span;
-    out[10] = (long long) (((fft_padded_size(p.n / 2) * 8 + 15) / 16) * 16 + p.n * 2 + 16);
+    out[9] = k5_planes_span(p);
+    out[10] = spectrum_smem_bytes(p.n);
+}
+// The launch structure the library chooses (spectrum_plan.h plan_spectrum) for the effective parameters `pp`, with the
+// environment overrides names[i] = values[i] (full GLAVA_B200_* names): out[] = { need_list, tap_table, full_table,
+// split_epilogue, epi_n, av_t_len, k5 (K5Form), tap_ku, table_planes, k5n_s, k5n_warps, fft_oop, fft_t, spec_grid,
+// spec_resident }, the refusal text into refusal[refusal_len].
+void emul_spectrum_plan(const glava_b200_params* pp, int post_chain, int batch, int sm_count, const char* const* names,
+                        const char* const* values, int count, long long* out, char* refusal, int refusal_len) {
+    const SpectrumKnobs k = spectrum_knobs([&](const char* name) -> const char* {
+        for (int i = 0; i < count; ++i) if (!strcmp(names[i], name)) return values[i];
+        return nullptr;
+    });
+    SpectrumTables t;
+    const SpectrumPlan pl = plan_spectrum(*pp, post_chain != 0, batch, sm_count, k, &t);
+    const long long v[] = { pl.need_list, pl.tap_table, pl.full_table, pl.split_epilogue, pl.epi_n, pl.av_t_len, (long long) pl.k5,
+                            pl.tap_ku, pl.table_planes, pl.k5n_s, pl.k5n_warps, pl.fft_oop, pl.fft_t, pl.spec_grid, pl.spec_resident };
+    for (size_t i = 0; i < sizeof(v) / sizeof(v[0]); ++i) out[i] = v[i];
+    snprintf(refusal, (size_t) refusal_len, "%s", pl.refusal.c_str());
 }
 // full-plane K5 of one plane through the per-block table, as k5_table_kernel does it (float staging, padded uniform loop)
 void emul_k5_table(const glava_b200_params* pp, const uint16_t* in, uint16_t* out) {
