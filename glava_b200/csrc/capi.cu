@@ -9,6 +9,7 @@
 #include "chain_core.h"
 #include "tables.h"
 #include "spectrum_plan.h"
+#include "raster_plan.h"
 #include "stream_state_core.h"
 
 #include <cuda_runtime.h>
@@ -65,7 +66,8 @@ struct ConfigTables {
     void* need_blk = nullptr; int need_nblk = 0, need_max_rows = 0;   // k5_need_smem_kernel: blocks of sampled texels
     float* av_t = nullptr;                                    // k5_need_kernel: transposed pre-smoothing texels
     K5Table k5 = {}; void* k5_blk = nullptr; void* k5_ent = nullptr; void* k5_wsum = nullptr;   // full-plane K5 tap table
-    void* geo = nullptr; int geo_box[4] = { 0, 0, 0, 0 };     // polar geometry cache (radial / circle), see raster_kernels.cu
+    RasterTables raster;                                      // which raster tables exist (raster_plan.h), the cache's box
+    void* geo = nullptr;                                      // polar geometry cache (radial / circle), see raster_kernels.cu
     void* ctile = nullptr; int ctile_nx = 0, ctile_count = 0; // circle: per-tile texel reference ranges (launch_circle_tiles)
 };
 
@@ -83,7 +85,6 @@ struct glava_b200 {
     float* d_spec_cur = nullptr;   // latest post-transform buffer (glava_b200_spectrum)
     void* d_ts_tab = nullptr; int ts_asz = 0, ts_lim = 0;   // transform_smooth {smin, smax} table
     std::atomic<unsigned long long> sizereq{0};   // pending glava_b200_sizereq: (1 << 63) | w << 32 | h, 0 = none
-    bool no_texmm = false, no_coltab = false;     // GLAVA_B200_NO_TEXMM, _NO_COLTAB, read once at creation (DESIGN 6.2)
     int batch = 0, device = 0, slots = 0;
     cudaStream_t stream = nullptr;        // raster kernels, read-backs (the stream glava_b200_cuda_stream returns)
     cudaStream_t spec_stream = nullptr;   // spectrum kernels + FIFO ingest, lowest priority: the latency-bound spectrum
@@ -108,7 +109,7 @@ struct glava_b200 {
     double* d_window = nullptr; float* d_twiddle = nullptr; void* d_rowtab = nullptr;
     ConfigTables tab;           // build_tables
     SpectrumPlan plan;          // launch structure of the spectrum update (spectrum_plan.h), chosen by build_tables
-    float* d_coltab = nullptr;  // graph / wave: per-stream column table (launch_raster fills it), GLAVA_B200_NO_COLTAB
+    float* d_coltab = nullptr;  // graph / wave: per-stream column table (launch_raster fills it)
     uint32_t* d_texmm = nullptr;   // circle: per-plane {min, max} of the sampled texture, refreshed before each raster
     // state + outputs
     float* d_spec = nullptr; float* d_applied = nullptr; float* d_ring_f = nullptr;
@@ -116,7 +117,7 @@ struct glava_b200 {
     uint16_t* d_av = nullptr;   // pre-smoothing textures [batch*2][n] (full-plane K5 runs as its own kernel)
     uint8_t* d_fb = nullptr;
     // dirty-row marks of the framebuffer slots (RasterArgs::marks) and the launch structure that last wrote them
-    // (launch_raster; 0 = none: the next bars / graph / wave launch stores every row)
+    // (RasterPlan::mark_key; 0 = none: the next bars / graph / wave launch stores every row)
     uint32_t* d_marks = nullptr; int mark_key = 0;
     unsigned long long updates = 0;
     // per-stream `modified` masks (glava_b200_update_masked): once streams have advanced unevenly, every stream has its
@@ -369,28 +370,37 @@ static int build_tables(glava_b200* r) {
         tb.k5.smem_bytes = K5_S_PLANES * kt.max_span * (int) sizeof(float);
     }
     if (p.module == GLAVA_B200_MOD_BARS || p.module == GLAVA_B200_MOD_GRAPH) { if ((rc = launch_bars_rowtab(p, r->d_rowtab, r->stream)) != 0) return rc; ++r->launches; }
-    // polar modules: cache the audio-independent per-pixel geometry (circle: only when the module samples a
-    // pre-smoothed texture, i.e. smooth_audio() is a single texelFetch)
-    if (p.module == GLAVA_B200_MOD_RADIAL || (p.module == GLAVA_B200_MOD_CIRCLE && p.smooth_pass)) {
-        const size_t bytes = polar_geo_box(p, tb.geo_box);
-        if (bytes > 0 && bytes <= ((size_t) 512 << 20) && !getenv("GLAVA_B200_NO_GEO")) {
-            if ((rc = dev_alloc(r, &tb.geo, bytes, false)) != 0) return rc;
-            if ((rc = launch_polar_geo(p, tb.geo, tb.geo_box, r->stream)) != 0) return rc;
-            ++r->launches;
-            // per-tile annulus from bucketed texture min / max (DESIGN 4.2): off by default, GLAVA_B200_CTILE=1 enables it (the
-            // curve's halo keeps most tiles of the annulus alive and every live tile pays the bucket reduction)
-            if (p.module == GLAVA_B200_MOD_CIRCLE && getenv("GLAVA_B200_CTILE")) {
-                int ntx = 0, nty = 0;
-                const size_t tile_bytes = circle_tile_bytes(p, &ntx, &nty);
-                if ((rc = dev_alloc(r, &tb.ctile, tile_bytes, false)) != 0) return rc;
-                if ((rc = launch_circle_tiles(p, tb.geo, tb.geo_box, tb.ctile, r->stream)) != 0) return rc;
-                tb.ctile_nx = ntx; tb.ctile_count = ntx * nty;
-                r->launches += 2;
-            }
-        }
+    // polar modules: the audio-independent per-pixel geometry; recorded in tb.raster once every table it names exists
+    const RasterTables rt = raster_tables(p, raster_knobs([](const char* name) -> const char* { return getenv(name); }));
+    if (rt.geo) {
+        if ((rc = dev_alloc(r, &tb.geo, rt.geo_bytes, false)) != 0) return rc;
+        if ((rc = launch_polar_geo(p, tb.geo, rt.box, r->stream)) != 0) return rc;
+        ++r->launches;
     }
+    if (rt.ctile) {
+        int ntx = 0, nty = 0;
+        const size_t tile_bytes = circle_tile_bytes(p, &ntx, &nty);
+        if ((rc = dev_alloc(r, &tb.ctile, tile_bytes, false)) != 0) return rc;
+        if ((rc = launch_circle_tiles(p, tb.geo, rt.box, tb.ctile, r->stream)) != 0) return rc;
+        tb.ctile_nx = ntx; tb.ctile_count = ntx * nty;
+        r->launches += 2;
+    }
+    tb.raster = rt;
     CU(cudaStreamSynchronize(r->stream));
     return 0;
+}
+
+// The buffers sized by the frame: row table, column table (graph / wave; the module of a handle never changes: reconfigure
+// refuses), framebuffers [slots][h][w] RGBA8 and their dirty-row marks.  At creation and on a resize.
+static int alloc_frame_buffers(glava_b200* r) {
+    const glava_b200_params& p = r->p;
+    int rc;
+    r->mark_key = 0;
+    if ((rc = dev_alloc(r, &r->d_rowtab, (size_t) p.h * 8, true)) != 0) return rc;
+    if ((p.module == GLAVA_B200_MOD_GRAPH || p.module == GLAVA_B200_MOD_WAVE) &&
+        (rc = dev_alloc(r, (void**) &r->d_coltab, (size_t) r->batch * GLB_COLTAB_PLANES * p.w * sizeof(float), true)) != 0) return rc;
+    if ((rc = dev_alloc(r, (void**) &r->d_fb, (size_t) p.w * p.h * 4 * r->slots, true)) != 0) return rc;
+    return dev_alloc(r, (void**) &r->d_marks, mark_bytes(p, r->slots), true);    // empty marks: the framebuffer starts all 0
 }
 
 static int build(glava_b200* r) {
@@ -468,15 +478,8 @@ static int build(glava_b200* r) {
     ALLOC(r->d_tex, 2 * planes * n * 2, true);
     ALLOC(r->d_av, planes * n * 2, true);
     ALLOC(r->d_texmm, planes * GLB_TEXMM_STRIDE * sizeof(uint32_t), true);          // one buffer: texmm_kernel fills it on the raster stream right before the circle raster reads it
-    ALLOC(r->d_rowtab, (size_t) p.h * 8, true);
-    if (p.module == GLAVA_B200_MOD_GRAPH || p.module == GLAVA_B200_MOD_WAVE)          // (the module of a handle never changes: reconfigure refuses)
-        ALLOC(r->d_coltab, (size_t) r->batch * GLB_COLTAB_PLANES * p.w * sizeof(float), true);
-    // framebuffers: [slots][h][w] RGBA8
-    size_t frame = (size_t) p.w * p.h * 4;
     r->slots = (p.fb_slots > 0 && p.fb_slots < r->batch) ? p.fb_slots : r->batch;
-    ALLOC(r->d_fb, frame * r->slots, true);
-    ALLOC(r->d_marks, mark_bytes(p, r->slots), true);          // empty marks: the framebuffer starts all 0
-    r->mark_key = 0;
+    if ((rc = alloc_frame_buffers(r)) != 0) return rc;
 #undef ALLOC
     // window LUT: render.c:660 macro as expanded at render.c:794 — cos(TWOPI*i/N - 1), double
     std::vector<double> w(n);
@@ -509,8 +512,6 @@ glava_b200* glava_b200_new(const glava_b200_params* params, int batch, int devic
     glava_b200* r = new glava_b200();
     r->p_user = *params; r->batch = batch; r->device = device;
     derive(r);
-    r->no_texmm = getenv("GLAVA_B200_NO_TEXMM") != nullptr;
-    r->no_coltab = getenv("GLAVA_B200_NO_COLTAB") != nullptr;
     if (build(r) != 0) { glava_b200_destroy(r); return nullptr; }
     return r;
 }
@@ -610,14 +611,9 @@ static int apply_resize(glava_b200* r, int w, int h) {
     if ((rc = sync_all(r)) != 0) return rc;
     dev_free(r, r->d_fb); dev_free(r, r->d_marks); dev_free(r, r->d_rowtab); dev_free(r, r->d_coltab);
     r->d_fb = nullptr; r->d_marks = nullptr; r->d_rowtab = nullptr; r->d_coltab = nullptr;
-    r->mark_key = 0;
     r->p_user = q;
     derive(r);
-    if ((rc = dev_alloc(r, (void**) &r->d_rowtab, (size_t) q.h * 8, true)) != 0) return rc;
-    if ((q.module == GLAVA_B200_MOD_GRAPH || q.module == GLAVA_B200_MOD_WAVE) &&
-        (rc = dev_alloc(r, (void**) &r->d_coltab, (size_t) r->batch * GLB_COLTAB_PLANES * q.w * sizeof(float), true)) != 0) return rc;
-    if ((rc = dev_alloc(r, (void**) &r->d_fb, (size_t) q.w * q.h * 4 * r->slots, true)) != 0) return rc;
-    if ((rc = dev_alloc(r, (void**) &r->d_marks, mark_bytes(q, r->slots), true)) != 0) return rc;
+    if ((rc = alloc_frame_buffers(r)) != 0) return rc;
     return build_tables(r);
 }
 
@@ -800,34 +796,31 @@ static int run_update(glava_b200* r, const float* d_l, const float* d_r, int mod
     if (!raster_only) r->kcounter = modified ? 0 : r->kcounter + 1;           // render.c:2380-2383
     const int b = r->tex_cur;
     CU(cudaStreamWaitEvent(r->stream, r->ev_spec_done[b], 0));
+    // the raster pass (raster_plan.h); its knobs are read at every pass
+    const RasterKnobs knobs = raster_knobs([](const char* name) -> const char* { return getenv(name); });
+    const glava_b200_params view = raster_view(p);
+    const ConfigTables& tb = r->tab;
+    const RasterPlan pl = plan_raster(view, tb.raster, r->batch, r->slots, knobs);
     RasterArgs ra;
     ra.tex = tex_half(r, b); ra.fb = r->d_fb;
-    ra.rowtab = (p.module == GLAVA_B200_MOD_BARS || p.module == GLAVA_B200_MOD_GRAPH) ? r->d_rowtab : nullptr;
+    ra.rowtab = pl.rowtab ? r->d_rowtab : nullptr;
     ra.batch = r->batch; ra.slots = r->slots; ra.stream0 = 0;
-    ra.geo = r->tab.geo; ra.gx0 = r->tab.geo_box[0]; ra.gy0 = r->tab.geo_box[1]; ra.gw = r->tab.geo_box[2]; ra.gh = r->tab.geo_box[3];
-    ra.texmm = nullptr; ra.ctile = nullptr; ra.ctile_zero = nullptr; ra.ctile_nx = 0;
-    ra.coltab = r->no_coltab ? nullptr : r->d_coltab;
-    ra.marks = r->d_marks; ra.marks_valid = 0;            // launch_raster decides from r->mark_key
-    // params.shader_pre_smoothed: the module's stage-1 shader believes something else about its textures than what the
-    // K5 pass did.  Only the raster launch sees that belief (as its smooth_pass); everything before it follows the real one.
-    glava_b200_params pr_store;
-    const glava_b200_params* pr = &p;
-    if (p.shader_pre_smoothed) {
-        pr_store = p; pr_store.smooth_pass = p.shader_pre_smoothed == 1 ? 1 : 0; pr = &pr_store;
-        if (p.module == GLAVA_B200_MOD_CIRCLE) ra.geo = nullptr;          // the circle cache is laid out for the consistent case
-    }
-    if (p.module == GLAVA_B200_MOD_CIRCLE && ra.geo && !r->no_texmm) {
-        if ((rc = launch_texmm(p, ra.tex, r->d_texmm, r->batch * 2, r->stream)) != 0) return rc;
-        ++r->launches;
-        ra.texmm = r->d_texmm;
-        if (r->tab.ctile) { ra.ctile = (const int4*) r->tab.ctile; ra.ctile_zero = (const int*) ((const int4*) r->tab.ctile + r->tab.ctile_count); ra.ctile_nx = r->tab.ctile_nx; }
-    }
+    ra.geo = pl.geo ? tb.geo : nullptr;
+    ra.gx0 = tb.raster.box[0]; ra.gy0 = tb.raster.box[1]; ra.gw = tb.raster.box[2]; ra.gh = tb.raster.box[3];
+    ra.texmm = pl.texmm ? r->d_texmm : nullptr;
+    ra.ctile = pl.ctile ? (const int4*) tb.ctile : nullptr;
+    ra.ctile_zero = pl.ctile ? (const int*) ((const int4*) tb.ctile + tb.ctile_count) : nullptr;
+    ra.ctile_nx = pl.ctile ? tb.ctile_nx : 0;
+    ra.coltab = pl.coltab ? r->d_coltab : nullptr;
+    ra.marks = r->d_marks; ra.marks_valid = raster_marks_valid(pl, r->mark_key, knobs) ? 1 : 0;
+    if (pl.texmm && (rc = launch_texmm(p, ra.tex, r->d_texmm, r->batch * 2, r->stream)) != 0) return rc;
+    r->mark_key = 0;                                      // until every launch of the pass is enqueued
     if (r->timing && (rc = timing_mark(r->ev_ras, r->stream)) != 0) return rc;
-    int raster_launches = 0;
-    if ((rc = launch_raster(*pr, ra, r->stream, &raster_launches, &r->mark_key)) != 0) return rc;
+    if ((rc = launch_raster(view, pl, ra, r->stream)) != 0) return rc;
+    r->mark_key = pl.mark_key;
     if (r->timing && (rc = timing_mark(r->ev_ras, r->stream)) != 0) return rc;
     CU(cudaEventRecord(r->ev_raster_done[b], r->stream));
-    r->launches += (uint64_t) raster_launches;
+    r->launches += (uint64_t) pl.launches;
     return 0;
 }
 

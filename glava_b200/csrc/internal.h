@@ -96,7 +96,7 @@ struct RasterArgs {
     float* coltab;
     // bars / graph / wave: dirty-row marks (raster_core.h dirty_pack), [slots][h][(w + 127) / 128] words, a band's word at
     // its first row.  marks_valid = 0: the words do not describe the framebuffer (another kernel or band height wrote it
-    // last); the kernel then stores every zero row and writes fresh marks.  launch_raster sets it.
+    // last); the kernel then stores every zero row and writes fresh marks.  run_update sets it (raster_plan.h raster_marks_valid).
     uint32_t* marks;
     int       marks_valid;
 };
@@ -140,13 +140,12 @@ int launch_k5_need_smem(const glava_b200_params& p, const uint16_t* d_av, uint16
 // pipeline B epilogue as its own elementwise kernel: spec (transform_fft output) -> upload quantisation, K1 - K4 on the R16
 // state, pre-smoothing texels into av_out (leading `bins` of every plane; bins is a multiple of 8)
 int launch_epilogue_b(const glava_b200_params& p, const SpectrumArgs& a, int bins, void* stream);
-// *launched += kernels launched.  *mark_key: the renderer's record of which launch structure last wrote a.marks (0: none,
-// or a kernel that keeps no marks wrote the framebuffer since); read and updated here.  Null: every launch stores every row.
-int launch_raster(const glava_b200_params& p, const RasterArgs& a, void* stream, int* launched = nullptr, int* mark_key = nullptr);
+// the raster kernels of one pass (raster_plan.h plan_raster; texmm_kernel aside); p: the raster view (raster_view)
+struct RasterPlan;
+int launch_raster(const glava_b200_params& p, const RasterPlan& plan, const RasterArgs& a, void* stream);
 int launch_bars_rowtab(const glava_b200_params& p, void* d_rowtab, void* stream);
-// geometry cache of the polar modules: box = {x0, y0, w, h}; returns bytes needed when d_geo == nullptr
-size_t polar_geo_box(const glava_b200_params& p, int box[4]);
 int launch_texmm(const glava_b200_params& p, const uint16_t* d_tex, uint32_t* d_out, int planes, void* stream);
+// geometry cache of the polar modules over box = {x0, y0, w, h} (raster_plan.h polar_geo_box)
 int launch_polar_geo(const glava_b200_params& p, void* d_geo, const int box[4], void* stream);
 // circle: the per-tile texel reference ranges from the finished cache; d_tiles = int4[ntx * nty] followed by int[ntx * nty]
 size_t circle_tile_bytes(const glava_b200_params& p, int* ntx, int* nty);

@@ -6,10 +6,9 @@
 // Compiled with --fmad=false: results are bit-identical to the host build of the *_core.h maths.
 #include "internal.h"
 #include "raster_core.h"
+#include "raster_plan.h"
 
 #include <cuda_runtime.h>
-
-#include <cstdlib>
 
 namespace glb {
 
@@ -567,28 +566,7 @@ int launch_texmm(const glava_b200_params& p, const uint16_t* d_tex, uint32_t* d_
     return 0;
 }
 
-// ---- polar geometry cache ------------------------------------------------------------------------
-// radial and circle spend almost all their arithmetic (atan, sqrt, sin, mod, colour ramp, blending,
-// premultiply) on quantities that depend on the pixel position and the parameters only.  They are
-// evaluated ONCE per renderer over the bounding box of the disc that can be non-zero (the same core
-// functions, so nothing changes numerically) and every frame of every stream reuses them out of L2.
-size_t polar_geo_box(const glava_b200_params& p, int box[4]) {
-    float reach, cx, cy;
-    if (p.module == GLAVA_B200_MOD_RADIAL) { reach = radial_reach(p); cx = (float) (p.w / 2) - p.radial_off_x; cy = (float) (p.h / 2) - p.radial_off_y; }
-    else if (p.module == GLAVA_B200_MOD_CIRCLE) { reach = circle_reach(p); cx = (float) (p.w / 2); cy = (float) (p.h / 2); }
-    else { box[0] = box[1] = box[2] = box[3] = 0; return 0; }
-    const int wpad = (p.w + 3) & ~3;
-    int x0 = (int) floorf(cx - reach) - 3, x1 = (int) ceilf(cx + reach) + 4;
-    int y0 = (int) floorf(cy - reach) - 3, y1 = (int) ceilf(cy + reach) + 4;
-    x0 = x0 < 0 ? 0 : (x0 & ~3); x1 = x1 > wpad ? wpad : ((x1 + 3) & ~3);
-    y0 = y0 < 0 ? 0 : y0; y1 = y1 > p.h ? p.h : y1;
-    if (x1 <= x0 || y1 <= y0) { box[0] = box[1] = box[2] = box[3] = 0; return 0; }
-    box[0] = x0; box[1] = y0; box[2] = x1 - x0; box[3] = y1 - y0;
-    // radial: [full 16 B/px][{lit, dR} 8 B/px][class code 1 B/px]; circle: 16 B/px
-    const size_t px = (size_t) box[2] * box[3];
-    return p.module == GLAVA_B200_MOD_RADIAL ? px * 25 : px * 16;
-}
-
+// ---- polar geometry cache (raster_plan.h polar_geo_box) -----------------------------------------------------------------
 __global__ void polar_geo_kernel(int4* __restrict__ geo, int gx0, int gy0, int gw, int gh, const __grid_constant__ glava_b200_params p) {
     const int bx = blockIdx.x * blockDim.x + threadIdx.x, by = blockIdx.y;
     if (bx >= gw || by >= gh) return;
@@ -685,7 +663,6 @@ int launch_circle_tiles(const glava_b200_params& p, const void* d_geo, const int
 
 // radial from the geometry cache: per pixel one 16-byte load, one compare against the bar's height
 // (160 heights per stream, in shared memory), one select.
-#define RADIAL_MAX_BARS 1024
 __global__ void __launch_bounds__(128)
 raster_radial_geo_kernel(const __grid_constant__ RasterArgs a, const __grid_constant__ glava_b200_params p, int rows_per_cta) {
     __shared__ float vflat[RADIAL_MAX_BARS + 4];        // bar heights, index side * nk + k (== class code - 1)
@@ -768,91 +745,48 @@ raster_radial_geo_kernel(const __grid_constant__ RasterArgs a, const __grid_cons
     }
 }
 
-static int pick_block_x(int quads) {       // threads per row-segment: prefer an exact tiling of w/4
-    static const int cand[] = { 96, 160, 128, 192, 256, 64 };
-    for (int c : cand) if (quads % c == 0) return c;
-    return 128;
-}
-
-int launch_raster(const glava_b200_params& p, const RasterArgs& a, void* stream, int* launched, int* mark_key) {
+int launch_raster(const glava_b200_params& p, const RasterPlan& pl, const RasterArgs& a, void* stream) {
     cudaStream_t st = (cudaStream_t) stream;
+    if (pl.mark_key && !a.marks) return fail(GLAVA_B200_EINVAL, "raster launch: no dirty-row marks for the bars / graph / wave kernel");
     const int quads = (p.w + 3) / 4;
-    // The specialised kernels assume native opacity (a fragment left at vec4(0) stores 0, whole zero rows / discs are skipped);
-    // with GL blending (premultiply_alpha == 0) every stage output is blended over the clear colour: generic kernel.
-    const bool native = p.premultiply_alpha != 0;
-    const bool fast_bars  = native && p.module == GLAVA_B200_MOD_BARS && !p.bars_mirror_yx && a.rowtab && (p.w & 3) == 0;
-    const bool fast_graph = native && p.module == GLAVA_B200_MOD_GRAPH && a.rowtab && !p.graph_join_channels && !p.graph_anti_alias;
-    const bool fast_wave  = native && p.module == GLAVA_B200_MOD_WAVE;
-    const bool geo_radial = native && p.module == GLAVA_B200_MOD_RADIAL && a.geo && p.radial_nbars <= RADIAL_MAX_BARS
-                            && !(p.radial_bar_outline_width > 0.0f);      // the cache holds two values per pixel, the end cap needs three
-    int bx = (fast_bars || fast_graph || fast_wave) ? pick_block_x(quads) : 128;
-    if (bx > 256) bx = 256;
-    // rows per CTA.  bars: with the dirty-row marks a band above the bars stores nothing but still pays the per-column set-up, so
-    // taller bands win.  On an H100 SXM (700 W limit), 1080p x 1024 streams, bench steps: 135 / 270 / 360 / 540 / 1080 rows gave
-    // 3.60 / 4.66 / 4.81 / 4.87 / 4.94 M frames/s (tools/tune_raster.py); 540 keeps two bands per column for small batches, and
-    // 96 / 160 / 256 threads per CTA were within 0.2 % there.  graph / wave pay a per-thread column
-    // set-up, so whole columns without the column table; with it (a.coltab) their set-up is six loads and short bands win
-    // (tools/gw_tune.py sweeps them); radial-from-cache 45.
-    const bool coltab = a.coltab && (fast_graph || fast_wave);
-    int rows = fast_bars ? 540 : ((fast_graph || fast_wave) ? (coltab ? (fast_wave ? 16 : 30) : 720) : (geo_radial ? 45 : 8));
-    // development overrides for tuning sweeps (tools/tune_raster.py); unset in normal use
-    int minb = 4;                                     // graph / wave with the column table: <= 64 registers (4 CTAs of 256; measured ahead) or 48 (5)
-    if (const char* e = getenv("GLAVA_B200_GW_MINB")) minb = atoi(e) == 5 ? 5 : 4;
-    if (const char* e = getenv("GLAVA_B200_ROWS")) { int v = atoi(e); if (v > 0) rows = v; }
-    if (const char* e = getenv("GLAVA_B200_BX")) { int v = atoi(e); if (v >= 32 && v <= 256 && v % 32 == 0) bx = v; }
-    // bars / graph / wave are __launch_bounds__(256); generic and both radial kernels take at most 128 threads
-    if (!(fast_bars || fast_graph || fast_wave) && bx > 128) bx = 128;
-    if (rows > p.h) rows = p.h;
-    // Dirty-row marks.  Their layout depends on the kernel's band height, and a kernel that keeps none (generic, radial, circle)
-    // can leave non-zero pixels anywhere: they describe the framebuffer only if the previous launch was the same kernel at the
-    // same `rows`.  GLAVA_B200_FULL_STORE=1 (read at every launch) stores every zero row anyway, for same-process A/B timing.
-    const bool keeps_marks = fast_bars || fast_graph || fast_wave;
-    const int key = keeps_marks ? ((fast_bars ? 1 : (fast_graph ? 2 : 3)) | (rows << 2)) : 0;
-    if (keeps_marks && !a.marks) return fail(GLAVA_B200_EINVAL, "raster launch: no dirty-row marks for the bars / graph / wave kernel");
-    const char* full_store = getenv("GLAVA_B200_FULL_STORE");
-    const int marks_valid = (mark_key && key != 0 && *mark_key == key && !(full_store && atoi(full_store) != 0)) ? 1 : 0;
-    if (mark_key) *mark_key = 0;                      // until every launch below is enqueued
-    // z dimension limit 65535: chunk the batch
-    // one launch covers at most `slots` streams (and at most the grid z limit): with a framebuffer
-    // ring (fb_slots < batch) two streams of one launch must never share a slot, and launches on
-    // the same stream are ordered, so slot s % slots ends up holding the highest stream mapped to it.
-    const int chunk = a.slots < 32768 ? (a.slots > 0 ? a.slots : 1) : 32768;
-    for (int s0 = 0; s0 < a.batch; s0 += chunk) {
-        RasterArgs b = a; b.stream0 = a.stream0 + s0; b.marks_valid = marks_valid;
-        int nz = a.batch - s0 < chunk ? a.batch - s0 : chunk;
-        dim3 grid((quads + bx - 1) / bx, (p.h + rows - 1) / rows, nz);
-        if (coltab) {
-            dim3 tg((p.w + 127) / 128, nz);
-            if (fast_wave) column_table_kernel<true><<<tg, 128, 0, st>>>(b, p);
-            else column_table_kernel<false><<<tg, 128, 0, st>>>(b, p);
-            if (launched) ++*launched;
-        }
-        if (launched) ++*launched;
-        if (fast_bars) raster_bars_kernel<<<grid, bx, 0, st>>>(b, p, rows);
-        else if (fast_graph) {
-            if (!coltab) raster_graph_kernel<false, 1><<<grid, bx, 0, st>>>(b, p, rows);
-            else if (minb == 5) raster_graph_kernel<true, 5><<<grid, bx, 0, st>>>(b, p, rows);
-            else raster_graph_kernel<true, 4><<<grid, bx, 0, st>>>(b, p, rows);
-        }
-        else if (fast_wave) {
-            if (!coltab) raster_wave_kernel<false, 1><<<grid, bx, 0, st>>>(b, p, rows);
-            else if (minb == 5) raster_wave_kernel<true, 5><<<grid, bx, 0, st>>>(b, p, rows);
-            else raster_wave_kernel<true, 4><<<grid, bx, 0, st>>>(b, p, rows);
-        }
-        else if (geo_radial) raster_radial_geo_kernel<<<grid, bx, 0, st>>>(b, p, rows);
-        else if (native && p.module == GLAVA_B200_MOD_RADIAL) raster_radial_kernel<<<grid, bx, 0, st>>>(b, p, rows);
-        else if (native && p.module == GLAVA_B200_MOD_CIRCLE) {
-            int tiles = 16;                                   // 128 rows per CTA
-            if (const char* e = getenv("GLAVA_B200_CIRCLE_TILES")) { int v = atoi(e); if (v > 0) tiles = v; }
+    for (int s0 = 0; s0 < a.batch; s0 += pl.chunk) {
+        RasterArgs b = a; b.stream0 = a.stream0 + s0;
+        const int nz = a.batch - s0 < pl.chunk ? a.batch - s0 : pl.chunk;
+        const dim3 grid((quads + pl.bx - 1) / pl.bx, (p.h + pl.rows - 1) / pl.rows, nz);
+        const dim3 tg((p.w + 127) / 128, nz);                  // column_table_kernel: a thread per column
+        switch (pl.kernel) {
+        case RasterKernel::GENERIC: raster_generic_kernel<<<grid, pl.bx, 0, st>>>(b, p, pl.rows); break;
+        case RasterKernel::BARS: raster_bars_kernel<<<grid, pl.bx, 0, st>>>(b, p, pl.rows); break;
+        case RasterKernel::GRAPH: raster_graph_kernel<false, 1><<<grid, pl.bx, 0, st>>>(b, p, pl.rows); break;
+        case RasterKernel::GRAPH_TAB4:
+            column_table_kernel<false><<<tg, 128, 0, st>>>(b, p);
+            raster_graph_kernel<true, 4><<<grid, pl.bx, 0, st>>>(b, p, pl.rows);
+            break;
+        case RasterKernel::GRAPH_TAB5:
+            column_table_kernel<false><<<tg, 128, 0, st>>>(b, p);
+            raster_graph_kernel<true, 5><<<grid, pl.bx, 0, st>>>(b, p, pl.rows);
+            break;
+        case RasterKernel::WAVE: raster_wave_kernel<false, 1><<<grid, pl.bx, 0, st>>>(b, p, pl.rows); break;
+        case RasterKernel::WAVE_TAB4:
+            column_table_kernel<true><<<tg, 128, 0, st>>>(b, p);
+            raster_wave_kernel<true, 4><<<grid, pl.bx, 0, st>>>(b, p, pl.rows);
+            break;
+        case RasterKernel::WAVE_TAB5:
+            column_table_kernel<true><<<tg, 128, 0, st>>>(b, p);
+            raster_wave_kernel<true, 5><<<grid, pl.bx, 0, st>>>(b, p, pl.rows);
+            break;
+        case RasterKernel::RADIAL: raster_radial_kernel<<<grid, pl.bx, 0, st>>>(b, p, pl.rows); break;
+        case RasterKernel::RADIAL_GEO: raster_radial_geo_kernel<<<grid, pl.bx, 0, st>>>(b, p, pl.rows); break;
+        case RasterKernel::CIRCLE: {
             const int ntile_y = (p.h + CIRCLE_TH - 1) / CIRCLE_TH;
-            dim3 cgrid((p.w + CIRCLE_TW - 1) / CIRCLE_TW, (ntile_y + tiles - 1) / tiles, nz);
-            raster_circle_kernel<<<cgrid, 256, 0, st>>>(b, p, tiles);
+            const dim3 cgrid((p.w + CIRCLE_TW - 1) / CIRCLE_TW, (ntile_y + pl.circle_tiles - 1) / pl.circle_tiles, nz);
+            raster_circle_kernel<<<cgrid, pl.bx, 0, st>>>(b, p, pl.circle_tiles);
+            break;
         }
-        else raster_generic_kernel<<<grid, bx, 0, st>>>(b, p, rows);
+        }
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return fail(GLAVA_B200_ECUDA, "raster kernel launch: %s", cudaGetErrorString(e));
     }
-    if (mark_key) *mark_key = key;
     return 0;
 }
 

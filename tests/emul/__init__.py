@@ -36,6 +36,7 @@ def lib():
         L.emul_k5_table.argtypes = [vp, vp, vp]
         L.emul_table_sizes.argtypes = [vp, i32, i32, i32, vp]
         L.emul_spectrum_plan.argtypes = [vp, i32, i32, i32, vp, vp, i32, vp, vp, i32]
+        L.emul_raster_plan.argtypes = [vp, i32, i32, vp, vp, i32, i32, vp]
         L.emul_bufscale.argtypes = [vp, i32, i32, vp]
         L.emul_transform_smooth.argtypes = [vp, i32, C.c_float, C.c_float]
         L.emul_upload.argtypes = [vp, vp, i32, C.c_float, C.c_float, i32, vp]
@@ -151,21 +152,43 @@ PLAN_FIELDS = ("need_list", "tap_table", "full_table", "split_epilogue", "epi_n"
 K5_FORMS = ("none", "taps_smem", "taps_l2", "taps_direct", "need_smem", "need_l2", "full_table", "full_planes", "fused")
 
 
+def _env_arrays(env):
+    """env ({"K5_SPLIT": "1", ...}, names without GLAVA_B200_) -> (names, values, count) for the C side"""
+    names = [("GLAVA_B200_" + k).encode() for k in env]
+    values = [str(v).encode() for v in env.values()]
+    n = max(len(names), 1)
+    return (C.c_char_p * n)(*names), (C.c_char_p * n)(*values), len(names)
+
+
 def spectrum_plan(p, post_chain, batch, sm_count, env):
     """the launch structure the library chooses (spectrum_plan.h plan_spectrum) for the effective parameters p under the
     environment overrides env ({"K5_SPLIT": "1", ...}, names without GLAVA_B200_) -> dict of PLAN_FIELDS (k5 as a K5_FORMS
     name) and "refusal" (None: none)"""
-    names = [("GLAVA_B200_" + k).encode() for k in env]
-    values = [str(v).encode() for v in env.values()]
-    n = max(len(names), 1)
-    name_arr = (C.c_char_p * n)(*names); value_arr = (C.c_char_p * n)(*values)
     out = np.zeros(len(PLAN_FIELDS), np.int64)
     refusal = C.create_string_buffer(256)
-    lib().emul_spectrum_plan(C.byref(p), int(post_chain), batch, sm_count, name_arr, value_arr, len(names), out.ctypes.data,
+    lib().emul_spectrum_plan(C.byref(p), int(post_chain), batch, sm_count, *_env_arrays(env), out.ctypes.data,
                              refusal, len(refusal))
     plan = dict(zip(PLAN_FIELDS, out.tolist()))
     plan["k5"] = K5_FORMS[plan["k5"]]
     plan["refusal"] = refusal.value.decode() or None
+    return plan
+
+
+RASTER_PLAN_FIELDS = ("kernel", "bx", "rows", "minb", "circle_tiles", "coltab", "texmm", "ctile", "rowtab", "geo", "chunk",
+                      "mark_key", "launches", "marks_valid")
+RASTER_KERNELS = ("generic", "bars", "graph", "graph_tab4", "graph_tab5", "wave", "wave_tab4", "wave_tab5", "radial",
+                  "radial_geo", "circle")
+
+
+def raster_plan(p, batch, slots, env, last_key=0):
+    """the raster pass the library plans (raster_plan.h) for the effective parameters p, `batch` streams and `slots`
+    framebuffer slots under the environment overrides env (names without GLAVA_B200_, set when the tables are built and at
+    the launch) -> dict of RASTER_PLAN_FIELDS (kernel as a RASTER_KERNELS name); marks_valid: whether a launch whose
+    renderer last recorded `last_key` may trust its dirty-row marks"""
+    out = np.zeros(len(RASTER_PLAN_FIELDS), np.int64)
+    lib().emul_raster_plan(C.byref(p), batch, slots, *_env_arrays(env), last_key, out.ctypes.data)
+    plan = dict(zip(RASTER_PLAN_FIELDS, out.tolist()))
+    plan["kernel"] = RASTER_KERNELS[plan["kernel"]]
     return plan
 
 

@@ -8,6 +8,7 @@
 #include "../../glava_b200/csrc/chain_core.h"
 #include "../../glava_b200/csrc/tables.h"
 #include "../../glava_b200/csrc/spectrum_plan.h"
+#include "../../glava_b200/csrc/raster_plan.h"
 
 #include <cmath>
 #include <cstring>
@@ -174,18 +175,18 @@ void emul_eval_color(const glava_b200_color_prog* prog, float x, float out[4]) {
     out[0] = r.r; out[1] = r.g; out[2] = r.b; out[3] = r.a;
 }
 
-// per-pixel reference semantics (raster_generic_kernel)
+// per-pixel reference semantics (raster_generic_kernel), on the parameters the raster launch sees
 void emul_raster(const glava_b200_params* pp, const uint16_t* tl, const uint16_t* tr, uint8_t* out, int y0, int y1) {
-    const glava_b200_params& p = *pp;
-    AudioTex t; t.l = tl; t.r = tr; t.n = p.n; t.pre_smoothed = p.shader_pre_smoothed ? (p.shader_pre_smoothed == 1) : p.smooth_pass;   /* capi.cu run_update: the raster launch's view */ t.sp = smooth_params(p);
+    const glava_b200_params p = raster_view(*pp);
+    AudioTex t; t.l = tl; t.r = tr; t.n = p.n; t.pre_smoothed = p.smooth_pass; t.sp = smooth_params(p);
     uint32_t* dst = reinterpret_cast<uint32_t*>(out);
     for (int y = y0; y < y1; ++y) for (int x = 0; x < p.w; ++x) dst[(size_t) y * p.w + x] = module_px(p, t, x, y);
 }
 
 // hoisted evaluation exactly as raster_bars_kernel / raster_graph_kernel / raster_wave_kernel do it
 int emul_raster_fast(const glava_b200_params* pp, const uint16_t* tl, const uint16_t* tr, uint8_t* out) {
-    const glava_b200_params& p = *pp;
-    AudioTex t; t.l = tl; t.r = tr; t.n = p.n; t.pre_smoothed = p.shader_pre_smoothed ? (p.shader_pre_smoothed == 1) : p.smooth_pass;   /* capi.cu run_update: the raster launch's view */ t.sp = smooth_params(p);
+    const glava_b200_params p = raster_view(*pp);
+    AudioTex t; t.l = tl; t.r = tr; t.n = p.n; t.pre_smoothed = p.smooth_pass; t.sp = smooth_params(p);
     uint32_t* dst = reinterpret_cast<uint32_t*>(out);
     if (p.module == GLAVA_B200_MOD_BARS && !p.bars_mirror_yx) {
         std::vector<BarsCol> col(p.w);
@@ -376,6 +377,21 @@ void emul_spectrum_plan(const glava_b200_params* pp, int post_chain, int batch, 
                             pl.tap_ku, pl.table_planes, pl.k5n_s, pl.k5n_warps, pl.fft_oop, pl.fft_t, pl.spec_grid, pl.spec_resident };
     for (size_t i = 0; i < sizeof(v) / sizeof(v[0]); ++i) out[i] = v[i];
     snprintf(refusal, (size_t) refusal_len, "%s", pl.refusal.c_str());
+}
+// The raster pass the library plans (raster_plan.h) for the effective parameters `pp`, `batch` streams and `slots`
+// framebuffer slots, with the environment overrides names[i] = values[i] (full GLAVA_B200_* names) both when the tables
+// are built and at the launch: out[] = { kernel (RasterKernel), bx, rows, minb, circle_tiles, coltab, texmm, ctile, rowtab,
+// geo, chunk, mark_key, launches, marks_valid (raster_marks_valid against last_key) }.
+void emul_raster_plan(const glava_b200_params* pp, int batch, int slots, const char* const* names, const char* const* values,
+                      int count, int last_key, long long* out) {
+    const RasterKnobs k = raster_knobs([&](const char* name) -> const char* {
+        for (int i = 0; i < count; ++i) if (!strcmp(names[i], name)) return values[i];
+        return nullptr;
+    });
+    const RasterPlan pl = plan_raster(raster_view(*pp), raster_tables(*pp, k), batch, slots, k);
+    const long long v[] = { (long long) pl.kernel, pl.bx, pl.rows, pl.minb, pl.circle_tiles, pl.coltab, pl.texmm, pl.ctile,
+                            pl.rowtab, pl.geo, pl.chunk, pl.mark_key, pl.launches, raster_marks_valid(pl, last_key, k) };
+    for (size_t i = 0; i < sizeof(v) / sizeof(v[0]); ++i) out[i] = v[i];
 }
 // full-plane K5 of one plane through the per-block table, as k5_table_kernel does it (float staging, padded uniform loop)
 void emul_k5_table(const glava_b200_params* pp, const uint16_t* in, uint16_t* out) {

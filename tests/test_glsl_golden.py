@@ -60,7 +60,7 @@ def test_product_arithmetic_equals_the_reference_shader_frames(orc_pm, gold, cas
     assert _lsb(got, want) <= 1 and (got != want).any(axis=2).sum() <= 0.002 * want.shape[0] * want.shape[1], case
     if module in ("bars", "graph", "wave", "circle") and not p.bars_mirror_yx and p.premultiply_alpha and not p.graph_join_channels and not p.graph_anti_alias:
         assert np.array_equal(emul.raster(p, tl, tr, fast=True), got)                      # the kernels' hoisted evaluation (native
-                                                                                           # opacity only: launch_raster's rule)
+                                                                                           # opacity only: plan_raster's rule)
 
 
 def _native_cases():

@@ -1,8 +1,9 @@
-"""-m gpu: every launch form of launch_raster, bit for bit against the oracle.
+"""-m gpu: every launch form of the raster pass, bit for bit against the oracle.
 
-launch_raster picks one of ten kernels and template instantiations and takes its tile shape from the environment
-(GLAVA_B200_ROWS, _BX, _GW_MINB, _CIRCLE_TILES at every launch; _NO_COLTAB, _NO_TEXMM, _NO_GEO, _CTILE at renderer creation;
-DESIGN 6.2).  The row band moves the warp-uniform splits of the specialised kernels (bars z0/z1/f0/f1, graph b1/b2/b3, wave
+raster_plan.h plan_raster picks one of eleven kernels and template instantiations and takes its tile shape from the
+environment (GLAVA_B200_ROWS, _BX, _GW_MINB, _CIRCLE_TILES, _NO_COLTAB, _NO_TEXMM at every launch; _NO_GEO, _CTILE when the
+tables are built; DESIGN 6.2); launch_raster executes the plan.  tests/test_raster_plan.py checks which plan each variant
+gets on the host; here every variant's pass must issue the plan's launches.  The row band moves the warp-uniform splits of the specialised kernels (bars z0/z1/f0/f1, graph b1/b2/b3, wave
 ra/rb, radial_geo band_live), and those splits exist only in the kernels.  Each case computes the oracle's frames once and
 runs every variant on them through raster_textures.  The textures reach the edges: silence, saturation, single spikes at
 texel 0 and n - 1, height ramps whose columns take every row value from 0 to h (bars, graph), lines that leave the frame
@@ -15,6 +16,7 @@ import pytest
 
 import glava_b200 as g
 from oracle.oracle import params_from
+from tests import emul
 
 pytestmark = pytest.mark.gpu
 
@@ -213,7 +215,9 @@ def _render(p, tl, tr, env, monkeypatch):
     for k, v in env.items():
         monkeypatch.setenv("GLAVA_B200_" + k, str(v))
     with g.Renderer(p, batch=tl.shape[0]) as r:
+        before = r.launch_count
         r.raster_textures(tl, tr)
+        assert r.launch_count - before == emul.raster_plan(p, tl.shape[0], tl.shape[0], env)["launches"], env
         return [r.readback(s) for s in range(tl.shape[0])]
 
 

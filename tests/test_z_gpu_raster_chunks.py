@@ -3,13 +3,15 @@
 launch_raster covers at most 32768 streams (grid z) or `fb_slots` streams per launch, whichever is fewer, and starts each
 launch at stream0 > 0.  The column table (graph / wave), the per-stream texture min / max (circle) and the framebuffer slot
 are all indexed by the global stream; the geometry cache (radial / circle) is shared.  Probe streams on both sides of the
-chunk boundary must equal the oracle on the same textures.  Tiny frames and parameters that light pixels inside them keep
+chunk boundary must equal the oracle on the same textures, and each pass must issue the launches raster_plan.h plans for it
+(one set per chunk).  Tiny frames and parameters that light pixels inside them keep
 the host side small: on an H100 the device holds about 1.5 GB during the 32771-stream cases, CUDA context included."""
 import numpy as np
 import pytest
 
 import glava_b200 as g
 from oracle.oracle import params_from
+from tests import emul
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900)]
 
@@ -21,6 +23,13 @@ SMALL_PARAMS = {
     "circle": dict(circle_radius=8.0, circle_amplify=12.0),
     "test": dict(),
 }
+
+
+def _raster(r, p, batch, slots, tl, tr):
+    """r.raster_textures(tl, tr), checking the pass's launch count against the plan"""
+    before = r.launch_count
+    r.raster_textures(tl, tr)
+    assert r.launch_count - before == emul.raster_plan(p, batch, slots, {})["launches"], (g.MODULES[p.module], batch, slots)
 
 
 def _textures(n, batch, seed, wave=False):
@@ -41,7 +50,7 @@ def test_raster_past_the_stream_chunk(orc_pm, module, built):
     p = g.default_params(module, n=n, w=32, h=24, **SMALL_PARAMS[module]); op = params_from(p)
     tl, tr = _textures(n, batch, 7, wave=module == "wave")
     with g.Renderer(p, batch=batch) as r:
-        r.raster_textures(tl, tr)
+        _raster(r, p, batch, batch, tl, tr)
         for s in (0, 1, 32767, 32768, 32769, batch - 1):
             got = r.readback(s)
             assert got.any(), (module, s)
@@ -60,7 +69,7 @@ def test_framebuffer_ring(orc_pm, module, slots, built):
     rng = np.random.default_rng(slots)
     lb = ((rng.random((batch, n), np.float32) - 0.5) * 0.4); rb = ((rng.random((batch, n), np.float32) - 0.5) * 0.4)
     with g.Renderer(p, batch=batch) as r:
-        r.raster_textures(tl, tr)
+        _raster(r, p, batch, slots, tl, tr)
         for j, s in enumerate(tops):
             got = r.readback(j)
             assert got.any(), (module, s)

@@ -1,6 +1,6 @@
 """-m gpu: setopacity other than "native" (premultiply_alpha = 0).  The reference then draws every module stage with
 GL_BLEND, glBlendFunc(GL_SRC_ALPHA, GL_ONE_MINUS_SRC_ALPHA), over the target glClear'd to the `setbg` colour and skips the
-premultiply stages (render.c:1467-1470, 1700, 2028).  Kernels (the generic per-pixel path: launch_raster's rule) against
+premultiply stages (render.c:1467-1470, 1700, 2028).  Kernels (the generic per-pixel path: plan_raster's rule) against
 frames computed from the reference's shader text with that blend state (tests/golden/glsl_golden.npz, *_blend cases),
 against the oracle, and against the host build of the same arithmetic."""
 import json
@@ -55,7 +55,7 @@ def test_full_size_non_native_frame(orc_pm, built):
 
 
 def test_radial_bar_outline_through_the_per_pixel_kernel(orc_pm, built):
-    """BAR_OUTLINE_WIDTH > 0 (deprecated, radial.glsl:33-36): three values per pixel, so launch_raster leaves the geometry
+    """BAR_OUTLINE_WIDTH > 0 (deprecated, radial.glsl:33-36): three values per pixel, so plan_raster leaves the geometry
     cache for the per-pixel radial kernel"""
     from tests import emul
     z = np.load(os.path.join(GOLDEN, "glsl_golden.npz"))
