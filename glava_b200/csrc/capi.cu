@@ -60,12 +60,7 @@ using namespace glb;
 // The tables build_tables derives from the parameters (audio-independent), freed and rebuilt together on reconfigure and
 // resize.  Device pointers are owned through glava_b200::allocs; null / 0 where the configuration has none.
 struct ConfigTables {
-    int* need = nullptr; int need_count = 0;                  // lazy K5 need-list [2][need_count]
-    TapEntry* tap_tab = nullptr; int* tap_cnt = nullptr; float* tap_wsum = nullptr; int tap_max = 0;   // its taps, tap-major
-    unsigned char* csr = nullptr; int csr_bytes = 0, csr_idx_off = 0, csr_off_off = 0;   // the same taps, texel-major
-    void* need_blk = nullptr; int need_nblk = 0, need_max_rows = 0;   // k5_need_smem_kernel: blocks of sampled texels
-    float* av_t = nullptr;                                    // k5_need_kernel: transposed pre-smoothing texels
-    K5Table k5 = {}; void* k5_blk = nullptr; void* k5_ent = nullptr; void* k5_wsum = nullptr;   // full-plane K5 tap table
+    SpectrumDevTables spec;                                   // the K5 tables the spectrum plan names (internal.h)
     RasterTables raster;                                      // which raster tables exist (raster_plan.h), the cache's box
     void* geo = nullptr;                                      // polar geometry cache (radial / circle), see raster_kernels.cu
     void* ctile = nullptr; int ctile_nx = 0, ctile_count = 0; // circle: per-tile texel reference ranges (launch_circle_tiles)
@@ -316,8 +311,9 @@ static int build_tables(glava_b200* r) {
     const glava_b200_params& p = r->p;
     int rc;
     ConfigTables& tb = r->tab;
-    for (void* d : { (void*) tb.need, (void*) tb.tap_tab, (void*) tb.tap_cnt, (void*) tb.tap_wsum, (void*) tb.csr, tb.need_blk,
-                     (void*) tb.av_t, tb.k5_blk, tb.k5_ent, tb.k5_wsum, tb.geo, tb.ctile })
+    SpectrumDevTables& st = tb.spec;
+    for (void* d : { (void*) st.need, (void*) st.tap_tab, (void*) st.tap_cnt, (void*) st.tap_wsum, (void*) st.csr, st.need_blk,
+                     (void*) st.av_t, (void*) st.k5.blk, (void*) st.k5.ent, (void*) st.k5.wsum, tb.geo, tb.ctile })
         dev_free(r, d);
     tb = ConfigTables();
     if (p.transform_smooth) {
@@ -339,35 +335,34 @@ static int build_tables(glava_b200* r) {
     const SpectrumPlan& pl = r->plan;
     const LazyTables& lt = host.lazy;
     if (pl.need_list) {
-        if ((rc = dev_upload(r, (void**) &tb.need, lt.need.data(), lt.need.size() * sizeof(int))) != 0) return rc;
-        tb.need_count = (int) lt.cnt;
+        if ((rc = dev_upload(r, (void**) &st.need, lt.need.data(), lt.need.size() * sizeof(int))) != 0) return rc;
+        st.need_count = (int) lt.cnt;
     }
     if (pl.tap_table) {
         // tap-major for the L2 path, texel-major blob per channel for the shared-memory path and the need-list kernels
-        if ((rc = dev_upload(r, (void**) &tb.tap_tab, lt.tab.data(), lt.tab.size() * sizeof(TapEntry))) != 0 ||
-            (rc = dev_upload(r, (void**) &tb.tap_cnt, lt.tcnt.data(), lt.tcnt.size() * sizeof(int))) != 0 ||
-            (rc = dev_upload(r, (void**) &tb.tap_wsum, lt.wsum.data(), lt.wsum.size() * sizeof(float))) != 0 ||
-            (rc = dev_upload(r, (void**) &tb.csr, lt.csr.data(), lt.csr.size())) != 0) return rc;
-        tb.tap_max = (int) lt.tap_max;
-        tb.csr_bytes = (int) lt.blob; tb.csr_idx_off = (int) lt.idx_off; tb.csr_off_off = (int) lt.off_off;
+        if ((rc = dev_upload(r, (void**) &st.tap_tab, lt.tab.data(), lt.tab.size() * sizeof(TapEntry))) != 0 ||
+            (rc = dev_upload(r, (void**) &st.tap_cnt, lt.tcnt.data(), lt.tcnt.size() * sizeof(int))) != 0 ||
+            (rc = dev_upload(r, (void**) &st.tap_wsum, lt.wsum.data(), lt.wsum.size() * sizeof(float))) != 0 ||
+            (rc = dev_upload(r, (void**) &st.csr, lt.csr.data(), lt.csr.size())) != 0) return rc;
+        st.tap_max = (int) lt.tap_max;
+        st.csr_bytes = (int) lt.blob; st.csr_idx_off = (int) lt.idx_off; st.csr_off_off = (int) lt.off_off;
     }
     if (pl.k5 == K5Form::NEED_SMEM) {
         const NeedBlocks& nb = host.blocks;
-        if ((rc = dev_upload(r, &tb.need_blk, nb.blk.data(), nb.blk.size() * sizeof(int))) != 0) return rc;
-        tb.need_nblk = nb.nblk; tb.need_max_rows = nb.max_rows;
+        if ((rc = dev_upload(r, &st.need_blk, nb.blk.data(), nb.blk.size() * sizeof(int))) != 0) return rc;
+        st.need_nblk = nb.nblk; st.need_max_rows = nb.max_rows;
     } else if (pl.k5 == K5Form::NEED_L2) {
-        if ((rc = dev_alloc(r, (void**) &tb.av_t, (size_t) 2 * pl.av_t_len * r->batch * sizeof(float), true)) != 0) return rc;
+        if ((rc = dev_alloc(r, (void**) &st.av_t, (size_t) 2 * pl.av_t_len * r->batch * sizeof(float), true)) != 0) return rc;
     }
     if (pl.full_table) {
         // the taps of ALL n output texels (tables.h build_k5_table_host) for k5_table_kernel
         static_assert(sizeof(K5Blk) == sizeof(int4) && sizeof(K5Ent) == sizeof(int2), "table records are read as int4 / int2");
         const K5TableHost& kt = host.full;
-        if ((rc = dev_upload(r, &tb.k5_blk, kt.blk.data(), kt.blk.size() * sizeof(K5Blk))) != 0 ||
-            (rc = dev_upload(r, &tb.k5_ent, kt.ent.data(), kt.ent.size() * sizeof(K5Ent))) != 0 ||
-            (rc = dev_upload(r, &tb.k5_wsum, kt.wsum.data(), kt.wsum.size() * sizeof(float))) != 0) return rc;
-        tb.k5.blk = (const int4*) tb.k5_blk; tb.k5.ent = (const int2*) tb.k5_ent; tb.k5.wsum = (const float*) tb.k5_wsum;
-        tb.k5.out = nullptr; tb.k5.count = (int) kt.out.size(); tb.k5.max_span = kt.max_span;
-        tb.k5.smem_bytes = K5_S_PLANES * kt.max_span * (int) sizeof(float);
+        if ((rc = dev_upload(r, (void**) &st.k5.blk, kt.blk.data(), kt.blk.size() * sizeof(K5Blk))) != 0 ||
+            (rc = dev_upload(r, (void**) &st.k5.ent, kt.ent.data(), kt.ent.size() * sizeof(K5Ent))) != 0 ||
+            (rc = dev_upload(r, (void**) &st.k5.wsum, kt.wsum.data(), kt.wsum.size() * sizeof(float))) != 0) return rc;
+        st.k5.out = nullptr; st.k5.count = (int) kt.out.size(); st.k5.max_span = kt.max_span;
+        st.k5.smem_bytes = K5_S_PLANES * kt.max_span * (int) sizeof(float);
     }
     if (p.module == GLAVA_B200_MOD_BARS || p.module == GLAVA_B200_MOD_GRAPH) { if ((rc = launch_bars_rowtab(p, r->d_rowtab, r->stream)) != 0) return rc; ++r->launches; }
     // polar modules: the audio-independent per-pixel geometry; recorded in tb.raster once every table it names exists
@@ -671,6 +666,9 @@ static int run_update(glava_b200* r, const float* d_l, const float* d_r, int mod
     const bool new_tex = !raster_only && (modified || r->interp_on);   // an interpolated frame has a new texture without new audio
     const int planes = r->batch * 2;
     const size_t total = (size_t) planes * p.n;
+    // a K5 form the plan refuses (spectrum_plan.h) fails every update with a new texture before it enqueues anything or
+    // changes any state
+    if (new_tex && !r->plan.refusal.empty()) return fail(GLAVA_B200_EINVAL, "%s", r->plan.refusal.c_str());
     if (new_tex) CU(cudaStreamWaitEvent(r->spec_stream, r->ev_raster_done[r->tex_cur ^ 1], 0));
     if (modified && r->p_user.bufscale > 1) {
         const int chans = p.module == GLAVA_B200_MOD_WAVE ? 1 : 2;
@@ -702,22 +700,8 @@ static int run_update(glava_b200* r, const float* d_l, const float* d_r, int mod
         memset(&a, 0, sizeof(a));
         a.pcm_l = d_l; a.pcm_r = d_r; a.window = r->d_window; a.twiddle = r->d_twiddle;
         a.spec = chain_out; a.skip_tex = r->post_chain ? 1 : 0; a.applied = r->d_applied; a.ring_f = r->d_ring_f;
-        a.gr_store = r->d_gr_store; a.ring_u = r->d_ring_u; a.tex = tex_half(r, b);
-        // the launch structure build_tables chose (spectrum_plan.h)
-        const SpectrumPlan& pl = r->plan;
-        const ConfigTables& tb = r->tab;
-        const bool need_in_kernel = pl.k5 == K5Form::TAPS_SMEM || pl.k5 == K5Form::TAPS_L2 || pl.k5 == K5Form::TAPS_DIRECT;
-        const bool need_kernel = pl.k5 == K5Form::NEED_SMEM || pl.k5 == K5Form::NEED_L2;
-        // full-plane smoothing (every texel wanted): the spectrum kernel exports the pre-smoothing texture and
-        // a second kernel smooths all planes, sharing the tap weights between planes
-        const bool planes_kernel = !r->post_chain && (pl.k5 == K5Form::FULL_TABLE || pl.k5 == K5Form::FULL_PLANES);
-        a.need = need_in_kernel ? tb.need : nullptr; a.need_count = tb.need_count;
-        a.tap_tab = a.need ? tb.tap_tab : nullptr; a.tap_cnt = tb.tap_cnt; a.tap_wsum = tb.tap_wsum; a.tap_max = tb.tap_max;
-        a.epi_n = pl.epi_n;
-        a.tap_ku = pl.tap_ku;
-        a.csr = pl.k5 == K5Form::TAPS_SMEM ? tb.csr : nullptr; a.csr_bytes = tb.csr_bytes; a.csr_idx_off = tb.csr_idx_off; a.csr_off_off = tb.csr_off_off;
+        a.gr_store = r->d_gr_store; a.ring_u = r->d_ring_u; a.tex = tex_half(r, b); a.av_out = r->d_av;
         a.batch = r->batch; a.update = r->updates;
-        a.variant_oop = pl.fft_oop; a.variant_t = pl.fft_t;
         a.umask = nullptr; a.tex_prev = tex_half(r, r->tex_cur);
         if (mask || r->desync) { if ((rc = stage_umask(r, mask, &a.umask)) != 0) return rc; }
         const int F = p.avg_frames;
@@ -728,33 +712,10 @@ static int run_update(glava_b200* r, const float* d_l, const float* d_r, int mod
             a.avg_w_b[f] = 0.53836f - (0.46164f * cosf(6.28318530718f * (float) f / (float) F - 1.0f));
         }
         a.avg_b_windowed = (p.avg_window && F != 2) ? 1 : 0;
-        const bool is_fft = p.module != GLAVA_B200_MOD_WAVE;
         if (r->timing && (rc = timing_mark(r->ev_spec, r->spec_stream)) != 0) return rc;
-        a.av_out = (planes_kernel || need_kernel) ? r->d_av : nullptr;
-        a.av_t_len = need_kernel ? pl.av_t_len : 0;
-        // three-kernel form of the lazy pipeline-B update: transform_fft only in the plane-per-CTA kernel, the R16 state
-        // update as an elementwise kernel, K5 on (texel, stream) pairs.  Every F: at F = 1 epilogue_b_kernel<0> keeps no ring.
-        a.fft_only = pl.split_epilogue ? 1 : 0;
-        if ((rc = launch_spectrum(p, a, is_fft, pl.spec_grid, pl.spec_resident, r->spec_stream)) != 0) return rc;
-        if (pl.split_epilogue) {
-            if ((rc = launch_epilogue_b(p, a, pl.epi_n, r->spec_stream)) != 0) return rc;
-            ++r->launches;
-        }
-        if (pl.k5 == K5Form::NEED_SMEM) {
-            if ((rc = launch_k5_need_smem(p, r->d_av, a.tex, r->batch, is_fft ? 2 : 1, tb.csr, tb.csr_bytes, tb.csr_idx_off, tb.csr_off_off,
-                                          tb.need, tb.tap_wsum, tb.need_count, tb.need_blk, tb.need_nblk, tb.need_max_rows, pl.k5n_warps,
-                                          r->spec_stream)) != 0) return rc;
-            r->launches += 1;
-        } else if (pl.k5 == K5Form::NEED_L2) {
-            if ((rc = launch_k5_need(p, r->d_av, tb.av_t, pl.av_t_len, a.tex, r->batch, is_fft ? 2 : 1, tb.csr, tb.csr_bytes, tb.csr_idx_off,
-                                     tb.csr_off_off, tb.need, tb.tap_wsum, tb.need_count, pl.k5n_s, pl.k5n_warps, r->spec_stream)) != 0) return rc;
-            r->launches += 2;
-        }
-        if (planes_kernel) {
-            // wave uses plane 0 of each stream only; smoothing the (zero) odd planes too keeps the launch simple
-            if ((rc = launch_smooth_only(p, r->d_av, a.tex, r->batch * 2, r->spec_stream, &tb.k5)) != 0) return rc;
-            ++r->launches;
-        }
+        // in the launch structure build_tables chose (spectrum_plan.h)
+        if ((rc = launch_spectrum_update(p, r->plan, r->tab.spec, a, r->spec_stream)) < 0) return rc;
+        r->launches += (uint64_t) rc;
         if (r->post_chain && p.transform_smooth == 1) {                     // render.c:694-718, after the module's chain
             if ((rc = launch_transform_smooth(chain_out, p.n, r->d_ts_tab, r->ts_asz, r->ts_lim, planes, r->spec_stream, a.umask)) != 0) return rc;
             ++r->launches;
@@ -764,7 +725,7 @@ static int run_update(glava_b200* r, const float* d_l, const float* d_r, int mod
             CU(cudaEventRecord(r->ev_spec_done[b], r->spec_stream));
             r->tex_cur = b;
         }
-        ++r->launches; ++r->updates;
+        ++r->updates;
         r->d_spec_cur = chain_out;
     }
     if (r->post_chain && new_tex) {
@@ -782,7 +743,7 @@ static int run_update(glava_b200* r, const float* d_l, const float* d_r, int mod
         if (rc) return rc;
         ++r->launches;
         if (p.smooth_pass) {
-            if ((rc = launch_smooth_only(p, r->d_av, tex_half(r, b), planes, r->spec_stream, &r->tab.k5)) != 0) return rc;
+            if ((rc = launch_k5_full(p, r->plan, r->tab.spec.k5, r->d_av, tex_half(r, b), planes, r->spec_stream)) != 0) return rc;
             ++r->launches;
         }
         if (modified && r->timing && (rc = timing_mark(r->ev_spec, r->spec_stream)) != 0) return rc;
@@ -1121,6 +1082,9 @@ int glava_b200_smooth_pass(glava_b200* r, const uint16_t* in, uint16_t* out, int
     clear_error();
     if (!r || !in || !out || count < 1) return fail(GLAVA_B200_EINVAL, "glava_b200_smooth_pass: bad arguments");
     CU(cudaSetDevice(r->device));
+    // the renderer's whole-plane table when it has one, else k5_planes_kernel where its spans fit shared memory
+    const std::string refusal = r->plan.full_table ? std::string() : k5_planes_refusal(k5_planes_span(r->p));
+    if (!refusal.empty()) return fail(GLAVA_B200_EINVAL, "%s", refusal.c_str());
     size_t bytes = (size_t) count * r->p.n * 2;
     uint16_t* d_in = nullptr; uint16_t* d_out = nullptr;
     CU(cudaMalloc((void**) &d_in, bytes));
@@ -1129,7 +1093,7 @@ int glava_b200_smooth_pass(glava_b200* r, const uint16_t* in, uint16_t* out, int
     int rc = 0;
     do {
         if (cudaMemcpyAsync(d_in, in, bytes, cudaMemcpyHostToDevice, r->stream) != cudaSuccess) { rc = fail(GLAVA_B200_ECUDA, "H2D copy failed"); break; }
-        if ((rc = launch_smooth_only(r->p, d_in, d_out, count, r->stream, &r->tab.k5)) != 0) break;
+        if ((rc = launch_k5_full(r->p, r->plan, r->tab.spec.k5, d_in, d_out, count, r->stream)) != 0) break;
         ++r->launches;
         if (cudaMemcpyAsync(out, d_out, bytes, cudaMemcpyDeviceToHost, r->stream) != cudaSuccess) { rc = fail(GLAVA_B200_ECUDA, "D2H copy failed"); break; }
         cudaError_t se = cudaStreamSynchronize(r->stream);

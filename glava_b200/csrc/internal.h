@@ -69,7 +69,7 @@ struct SpectrumArgs {
     // texture is carried from `tex_prev` (the half of the double buffer the previous raster read) into `tex`.
     int variant_oop, variant_t; // kernel variant: out-of-place passes, threads per CTA (0 = the size's default)
     int fft_only;               // 1: stop after transform_fft — `spec` (the leading epi_n bins) is all this launch produces; gravity /
-                                // average run as epilogue_b_kernel, K5 as k5_need_smem_kernel / k5_need_kernel (capi.cu run_update)
+                                // average run as epilogue_b_kernel, K5 as k5_need_smem_kernel / k5_need_kernel (launch_spectrum_update)
     int av_t_len;               // > 0: av_out receives only the leading av_t_len bins (need-list K5 as its own kernel downstream)
     const uint32_t* umask;      // [batch]
     const uint16_t* tex_prev;   // [batch*2][n]
@@ -104,9 +104,6 @@ struct RasterArgs {
 #define GLB_CIRCLE_NB 128                         // texel buckets per plane (n / 128 texels each)
 #define GLB_TEXMM_STRIDE (2 + 2 * GLB_CIRCLE_NB)  // u32 per plane
 
-// ---- kernel launchers (spectrum_kernels.cu, raster_kernels.cu); `stream` is a cudaStream_t passed as void* ------------------
-// grid, resident: SpectrumPlan::spec_grid, ::spec_resident (spectrum_plan.h)
-int launch_spectrum(const glava_b200_params& p, const SpectrumArgs& a, bool is_fft, int grid, int resident, void* stream);
 // Full-plane K5 tap table (built once per parameter set, capi.cu): for every block of K5_BLOCK output texels the taps of
 // all its texels, tap-major and padded to the block's longest sum with zero-weight entries, so a warp's loads coalesce
 // and the tap loop is uniform.
@@ -122,24 +119,30 @@ struct K5Table {
 #ifndef K5_BLOCK
 #define K5_BLOCK 128
 #endif
-// planes handled: plane(i) = i * plane_stride + plane_offset for i in [0, count) — stride 2 / offset ch walks one channel's
-// planes of the interleaved [batch][2] layout (need-list tables differ per channel)
-int launch_smooth_only(const glava_b200_params& p, const uint16_t* d_in, uint16_t* d_out, int count, void* stream,
-                       const K5Table* table = nullptr, int plane_stride = 1, int plane_offset = 0);
-// need-list K5, lanes = streams (d_av [batch*2][n] u16 as exported by the spectrum kernel -> transposed float d_av_t): csr = the texel-major tap blobs of SpectrumArgs (per channel float w[] | u16 idx[] | int off[]),
-// need / wsum = [2][need_count]; av_t as exported by the spectrum kernel; writes tex[(stream * 2 + ch) * n + need[k]];
-// S streams per lane, wpc warps per CTA (SpectrumPlan::k5n_s, ::k5n_warps)
-int launch_k5_need(const glava_b200_params& p, const uint16_t* d_av, float* d_av_t, int av_t_len, uint16_t* d_tex, int batch, int channels,
-                   const unsigned char* d_csr, int csr_bytes, int csr_idx_off, int csr_off_off, const int* d_need,
-                   const float* d_wsum, int need_count, int S, int wpc, void* stream);
-// the same need-list K5 from shared-memory tiles over blocks of sampled texels (tables.h build_need_blocks); reads the
-// [plane][bin] R16 texture directly
-int launch_k5_need_smem(const glava_b200_params& p, const uint16_t* d_av, uint16_t* d_tex, int batch, int channels,
-                        const unsigned char* d_csr, int csr_bytes, int csr_idx_off, int csr_off_off, const int* d_need,
-                        const float* d_wsum, int need_count, const void* d_blocks, int nblk, int max_rows, int wpc, void* stream);
-// pipeline B epilogue as its own elementwise kernel: spec (transform_fft output) -> upload quantisation, K1 - K4 on the R16
-// state, pre-smoothing texels into av_out (leading `bins` of every plane; bins is a multiple of 8)
-int launch_epilogue_b(const glava_b200_params& p, const SpectrumArgs& a, int bins, void* stream);
+// The spectrum path's device tables (capi.cu build_tables uploads the ones the plan names and owns them; null / 0 elsewhere)
+struct SpectrumDevTables {
+    int* need = nullptr; int need_count = 0;                  // lazy K5 need-list [2][need_count]
+    TapEntry* tap_tab = nullptr; int* tap_cnt = nullptr; float* tap_wsum = nullptr; int tap_max = 0;   // its taps, tap-major
+    // the same taps as one texel-major blob per channel (float w[] | u16 idx[] | int off[]), SpectrumArgs::csr
+    unsigned char* csr = nullptr; int csr_bytes = 0, csr_idx_off = 0, csr_off_off = 0;
+    void* need_blk = nullptr; int need_nblk = 0, need_max_rows = 0;   // k5_need_smem_kernel: blocks of sampled texels
+    float* av_t = nullptr;                                    // k5_need_kernel: transposed pre-smoothing texels
+    K5Table k5 = {};                                          // whole-plane K5 tap table (blk null: none)
+};
+
+// ---- kernel launchers (spectrum_kernels.cu, raster_kernels.cu); `stream` is a cudaStream_t passed as void* ------------------
+struct SpectrumPlan;
+// The spectrum-stream kernels of one modified update in the launch structure `plan` names (spectrum_plan.h): spectrum_kernel,
+// then epilogue_b_kernel, then the need-list K5 kernel(s), then the whole-plane K5 unless a post chain follows (a.skip_tex:
+// it runs after the upload).  `a` carries the per-update buffers and values, av_out = the pre-smoothing texture buffer; the
+// launcher sets every field the plan decides.  Returns the number of kernels launched, or a negative error code.
+int launch_spectrum_update(const glava_b200_params& p, const SpectrumPlan& plan, const SpectrumDevTables& tables,
+                           const SpectrumArgs& a, void* stream);
+// Whole-plane K5 over `count` R16 planes d_in -> d_out: k5_table_kernel from `table` with plan.table_planes planes per CTA
+// when the plan has that table (plan.full_table; under K5Form::FULL_TABLE), else k5_planes_kernel (FULL_PLANES), whose
+// refusal the caller checks (SpectrumPlan::refusal, k5_planes_refusal)
+int launch_k5_full(const glava_b200_params& p, const SpectrumPlan& plan, const K5Table& table, const uint16_t* d_in,
+                   uint16_t* d_out, int count, void* stream);
 // the raster kernels of one pass (raster_plan.h plan_raster; texmm_kernel aside); p: the raster view (raster_view)
 struct RasterPlan;
 int launch_raster(const glava_b200_params& p, const RasterPlan& plan, const RasterArgs& a, void* stream);

@@ -495,8 +495,9 @@ static int launch_spectrum_fft(const glava_b200_params& p, const SpectrumArgs& a
     return launch_spectrum_t<L, true, 0, false>(p, a, grid, resident, st);
 }
 
-int launch_spectrum(const glava_b200_params& p, const SpectrumArgs& a, bool is_fft, int grid, int resident, void* stream) {
-    cudaStream_t st = (cudaStream_t) stream;
+static int launch_spectrum(const glava_b200_params& p, const SpectrumPlan& pl, const SpectrumArgs& a, cudaStream_t st) {
+    const bool is_fft = p.module != GLAVA_B200_MOD_WAVE;
+    const int grid = pl.spec_grid, resident = pl.spec_resident;
     const int tsel = a.variant_t, oop = a.variant_oop;
 #define GLB_CASE(L) case (1 << L): return is_fft ? launch_spectrum_fft<L>(p, a, grid, resident, st, oop, tsel) \
                                                  : launch_spectrum_t<L, false>(p, a, grid, resident, st);
@@ -596,7 +597,7 @@ k5_table_kernel(const uint16_t* __restrict__ in, uint16_t* __restrict__ out, int
 
 template <bool AVG_ONLY, int S>
 static int launch_k5_table_t(const glava_b200_params& p, const uint16_t* d_in, uint16_t* d_out, int count, cudaStream_t st,
-                             const K5Table& tb, int plane_stride, int plane_offset) {
+                             const K5Table& tb) {
     const SmoothParams sp = smooth_params(p);
     auto kern = k5_table_kernel<AVG_ONLY, S>;
     const int smem = S * tb.max_span * (int) sizeof(float);
@@ -606,39 +607,35 @@ static int launch_k5_table_t(const glava_b200_params& p, const uint16_t* d_in, u
     }
     const unsigned gx = (tb.count + K5_BLOCK - 1) / K5_BLOCK;
     cudaError_t e = launch_y_slices((count + S - 1) / S, [&](int y0, unsigned rows) {
-        kern<<<dim3(gx, rows), K5_BLOCK, smem, st>>>(d_in, d_out, p.n, count, tb, sp, plane_stride, plane_offset, y0);
+        kern<<<dim3(gx, rows), K5_BLOCK, smem, st>>>(d_in, d_out, p.n, count, tb, sp, 1, 0, y0);   // every plane in order
     });
     if (e != cudaSuccess) return fail(GLAVA_B200_ECUDA, "smooth (table) kernel launch: %s", cudaGetErrorString(e));
     return 0;
 }
 
-int launch_smooth_only(const glava_b200_params& p, const uint16_t* d_in, uint16_t* d_out, int count, void* stream,
-                       const K5Table* table, int plane_stride, int plane_offset) {
-    if (table && table->blk) {
-        // planes per CTA share every tap's index / weight load (spectrum_plan.h k5_table_planes)
+int launch_k5_full(const glava_b200_params& p, const SpectrumPlan& pl, const K5Table& table, const uint16_t* d_in,
+                   uint16_t* d_out, int count, void* stream) {
+    cudaStream_t st = (cudaStream_t) stream;
+    if (pl.full_table) {
+        // planes per CTA share every tap's index / weight load
         const bool avg = smooth_params(p).sample_mode == 0;
-        cudaStream_t st = (cudaStream_t) stream;
-        switch (k5_table_planes(table->max_span)) {
-            case 8: return avg ? launch_k5_table_t<true, 8>(p, d_in, d_out, count, st, *table, plane_stride, plane_offset)
-                               : launch_k5_table_t<false, 8>(p, d_in, d_out, count, st, *table, plane_stride, plane_offset);
-            case 4: return avg ? launch_k5_table_t<true, 4>(p, d_in, d_out, count, st, *table, plane_stride, plane_offset)
-                               : launch_k5_table_t<false, 4>(p, d_in, d_out, count, st, *table, plane_stride, plane_offset);
-            default: return avg ? launch_k5_table_t<true, 2>(p, d_in, d_out, count, st, *table, plane_stride, plane_offset)
-                                : launch_k5_table_t<false, 2>(p, d_in, d_out, count, st, *table, plane_stride, plane_offset);
+        switch (pl.table_planes) {
+            case 8: return avg ? launch_k5_table_t<true, 8>(p, d_in, d_out, count, st, table)
+                               : launch_k5_table_t<false, 8>(p, d_in, d_out, count, st, table);
+            case 4: return avg ? launch_k5_table_t<true, 4>(p, d_in, d_out, count, st, table)
+                               : launch_k5_table_t<false, 4>(p, d_in, d_out, count, st, table);
+            default: return avg ? launch_k5_table_t<true, 2>(p, d_in, d_out, count, st, table)
+                                : launch_k5_table_t<false, 2>(p, d_in, d_out, count, st, table);
         }
     }
-    if (plane_stride != 1 || plane_offset != 0) return fail(GLAVA_B200_EINVAL, "smooth pass: strided planes need a tap table");
-    const int span = k5_planes_span(p);
-    const std::string refusal = k5_planes_refusal(span);
-    if (!refusal.empty()) return fail(GLAVA_B200_EINVAL, "%s", refusal.c_str());
-    const size_t smem = k5_planes_smem(span);
+    const size_t smem = k5_planes_smem(k5_planes_span(p));
     if (smem > 48 * 1024) {
         cudaError_t e = cudaFuncSetAttribute(k5_planes_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
         if (e != cudaSuccess) return fail(GLAVA_B200_ECUDA, "cudaFuncSetAttribute(k5): %s", cudaGetErrorString(e));
     }
     const unsigned gx = (p.n + K5_XT - 1) / K5_XT;
     cudaError_t e = launch_y_slices((count + K5_S - 1) / K5_S, [&](int y0, unsigned rows) {
-        k5_planes_kernel<<<dim3(gx, rows), K5_XT, smem, (cudaStream_t) stream>>>(d_in, d_out, p.n, count, p, y0);
+        k5_planes_kernel<<<dim3(gx, rows), K5_XT, smem, st>>>(d_in, d_out, p.n, count, p, y0);
     });
     if (e != cudaSuccess) return fail(GLAVA_B200_ECUDA, "smooth kernel launch: %s", cudaGetErrorString(e));
     return 0;
@@ -709,11 +706,11 @@ epilogue_b_kernel(const __grid_constant__ SpectrumArgs a, int n, int bins, int F
     *reinterpret_cast<uint4*>(a.av_out + base) = tex;
 }
 
-int launch_epilogue_b(const glava_b200_params& p, const SpectrumArgs& a, int bins, void* stream) {
-    const int planes = a.batch * 2, F = p.avg_frames;
+// over the leading SpectrumPlan::epi_n bins of every plane (a multiple of 8)
+static int launch_epilogue_b(const glava_b200_params& p, const SpectrumPlan& pl, const SpectrumArgs& a, cudaStream_t st) {
+    const int planes = a.batch * 2, F = p.avg_frames, bins = pl.epi_n;
     const float diff = p.gravity_step * (1.0f / p.ur);
     const unsigned gx = (bins / 8 + 127) / 128;
-    cudaStream_t st = (cudaStream_t) stream;
     cudaError_t e = launch_y_slices(planes, [&](int y0, unsigned rows) {
 #define GLB_EPI(FT) epilogue_b_kernel<FT><<<dim3(gx, rows), 128, 0, st>>>(a, p.n, bins, F, diff, y0)
         switch (F) {
@@ -875,50 +872,45 @@ k5_need_smem_kernel(const uint16_t* __restrict__ av, uint16_t* __restrict__ tex,
     }
 }
 
-int launch_k5_need_smem(const glava_b200_params& p, const uint16_t* d_av, uint16_t* d_tex, int batch, int channels,
-                        const unsigned char* d_csr, int csr_bytes, int csr_idx_off, int csr_off_off, const int* d_need,
-                        const float* d_wsum, int need_count, const void* d_blocks, int nblk, int max_rows, int wpc, void* stream) {
+// the need-list K5 kernels read the pre-smoothing texture a.av_out and write the sampled texels of a.tex
+static int launch_k5_need_smem(const glava_b200_params& p, const SpectrumPlan& pl, const SpectrumDevTables& tb,
+                               const SpectrumArgs& a, cudaStream_t st) {
     const SmoothParams sp = smooth_params(p);
-    cudaStream_t st = (cudaStream_t) stream;
-    if (nblk <= 0) return 0;
-    const size_t smem = (size_t) max_rows * 33 * sizeof(float);
-    dim3 grid((unsigned) nblk, (unsigned) ((batch + 31) / 32), (unsigned) channels);
+    if (tb.need_nblk <= 0) return 0;
+    const size_t smem = (size_t) tb.need_max_rows * 33 * sizeof(float);
+    const int channels = p.module != GLAVA_B200_MOD_WAVE ? 2 : 1;
+    dim3 grid((unsigned) tb.need_nblk, (unsigned) ((a.batch + 31) / 32), (unsigned) channels);
+    auto kern = sp.sample_mode == 0 ? k5_need_smem_kernel<0> : k5_need_smem_kernel<1>;
     cudaError_t e;
-    if (sp.sample_mode == 0) {
-        if ((e = cudaFuncSetAttribute(k5_need_smem_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem)) != cudaSuccess)
-            return fail(GLAVA_B200_ECUDA, "need-list smooth kernel shared memory %zu: %s", smem, cudaGetErrorString(e));
-        k5_need_smem_kernel<0><<<grid, wpc * 32, smem, st>>>(d_av, d_tex, p.n, batch, d_csr, csr_bytes, csr_idx_off, csr_off_off, d_need, d_wsum,
-                                                             need_count, reinterpret_cast<const int4*>(d_blocks), nblk, sp);
-    } else {
-        if ((e = cudaFuncSetAttribute(k5_need_smem_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem)) != cudaSuccess)
-            return fail(GLAVA_B200_ECUDA, "need-list smooth kernel shared memory %zu: %s", smem, cudaGetErrorString(e));
-        k5_need_smem_kernel<1><<<grid, wpc * 32, smem, st>>>(d_av, d_tex, p.n, batch, d_csr, csr_bytes, csr_idx_off, csr_off_off, d_need, d_wsum,
-                                                             need_count, reinterpret_cast<const int4*>(d_blocks), nblk, sp);
-    }
+    if ((e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem)) != cudaSuccess)
+        return fail(GLAVA_B200_ECUDA, "need-list smooth kernel shared memory %zu: %s", smem, cudaGetErrorString(e));
+    kern<<<grid, pl.k5n_warps * 32, smem, st>>>(a.av_out, a.tex, p.n, a.batch, tb.csr, tb.csr_bytes, tb.csr_idx_off, tb.csr_off_off,
+                                                tb.need, tb.tap_wsum, tb.need_count, reinterpret_cast<const int4*>(tb.need_blk),
+                                                tb.need_nblk, sp);
     if ((e = cudaGetLastError()) != cudaSuccess) return fail(GLAVA_B200_ECUDA, "need-list smooth kernel launch: %s", cudaGetErrorString(e));
     return 0;
 }
 
-int launch_k5_need(const glava_b200_params& p, const uint16_t* d_av, float* d_av_t, int av_t_len, uint16_t* d_tex, int batch, int channels,
-                   const unsigned char* d_csr, int csr_bytes, int csr_idx_off, int csr_off_off, const int* d_need,
-                   const float* d_wsum, int need_count, int S, int wpc, void* stream) {
+static int launch_k5_need(const glava_b200_params& p, const SpectrumPlan& pl, const SpectrumDevTables& tb, const SpectrumArgs& a,
+                          cudaStream_t st) {
     const SmoothParams sp = smooth_params(p);
-    cudaStream_t st = (cudaStream_t) stream;
+    const int batch = a.batch, channels = p.module != GLAVA_B200_MOD_WAVE ? 2 : 1, av_t_len = pl.av_t_len;
     {
         dim3 tg((av_t_len + 31) / 32, (batch + 31) / 32, channels);
-        av_transpose_kernel<<<tg, 256, 0, st>>>(d_av, d_av_t, p.n, av_t_len, batch);
+        av_transpose_kernel<<<tg, 256, 0, st>>>(a.av_out, tb.av_t, p.n, av_t_len, batch);
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return fail(GLAVA_B200_ECUDA, "transpose kernel launch: %s", cudaGetErrorString(e));
     }
     // S streams per lane share every tap broadcast (spectrum_plan.h chooses S from the batch)
+    const int S = pl.k5n_s, wpc = pl.k5n_warps;
     const int groups = (batch + 32 * S - 1) / (32 * S);
-    const long long warps = (long long) channels * need_count * groups;
+    const long long warps = (long long) channels * tb.need_count * groups;
     // warps per CTA = consecutive texels of one stream group: their tap windows overlap almost entirely, so the more of them
     // share an SM's L1 the fewer reads go to L2 (the kernel moves 4 bytes per tap and lane: L2 bandwidth is its bound)
     const unsigned grid = (unsigned) ((warps + wpc - 1) / wpc);
     if (grid == 0) return 0;
-#define GLB_K5N(M, SS, DD) k5_need_kernel<M, SS, DD><<<grid, wpc * 32, 0, st>>>(d_av_t, av_t_len, d_tex, p.n, batch, channels, d_csr, csr_bytes, \
-                                                                                  csr_idx_off, csr_off_off, d_need, d_wsum, need_count, sp)
+#define GLB_K5N(M, SS, DD) k5_need_kernel<M, SS, DD><<<grid, wpc * 32, 0, st>>>(tb.av_t, av_t_len, a.tex, p.n, batch, channels, tb.csr, \
+                                                 tb.csr_bytes, tb.csr_idx_off, tb.csr_off_off, tb.need, tb.tap_wsum, tb.need_count, sp)
 #define GLB_K5N_M(SS, DD) do { if (sp.sample_mode == 0) GLB_K5N(0, SS, DD); else GLB_K5N(1, SS, DD); } while (0)
     if (S == 4) GLB_K5N_M(4, 8);
     else if (S == 2) GLB_K5N_M(2, 8);
@@ -928,6 +920,37 @@ int launch_k5_need(const glava_b200_params& p, const uint16_t* d_av, float* d_av
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(GLAVA_B200_ECUDA, "need-list smooth kernel launch: %s", cudaGetErrorString(e));
     return 0;
+}
+
+int launch_spectrum_update(const glava_b200_params& p, const SpectrumPlan& pl, const SpectrumDevTables& tb, const SpectrumArgs& in,
+                           void* stream) {
+    cudaStream_t st = (cudaStream_t) stream;
+    const bool need_in_kernel = pl.k5 == K5Form::TAPS_SMEM || pl.k5 == K5Form::TAPS_L2 || pl.k5 == K5Form::TAPS_DIRECT;
+    const bool need_kernel = pl.k5 == K5Form::NEED_SMEM || pl.k5 == K5Form::NEED_L2;
+    // full-plane smoothing (every texel wanted): the spectrum kernel exports the pre-smoothing texture and a second kernel
+    // smooths all planes, sharing the tap weights between planes
+    const bool full_kernel = !in.skip_tex && (pl.k5 == K5Form::FULL_TABLE || pl.k5 == K5Form::FULL_PLANES);
+    SpectrumArgs a = in;
+    a.need = need_in_kernel ? tb.need : nullptr; a.need_count = tb.need_count;
+    a.tap_tab = need_in_kernel ? tb.tap_tab : nullptr; a.tap_cnt = tb.tap_cnt; a.tap_wsum = tb.tap_wsum; a.tap_max = tb.tap_max;
+    a.tap_ku = pl.tap_ku;
+    a.epi_n = pl.epi_n;
+    a.csr = pl.k5 == K5Form::TAPS_SMEM ? tb.csr : nullptr; a.csr_bytes = tb.csr_bytes; a.csr_idx_off = tb.csr_idx_off; a.csr_off_off = tb.csr_off_off;
+    a.variant_oop = pl.fft_oop; a.variant_t = pl.fft_t;
+    a.av_out = (full_kernel || need_kernel) ? in.av_out : nullptr;
+    a.av_t_len = need_kernel ? pl.av_t_len : 0;
+    // three-kernel form of the lazy pipeline-B update: transform_fft only in the plane-per-CTA kernel, the R16 state update as
+    // an elementwise kernel, K5 on (texel, stream) pairs.  Every F: at F = 1 epilogue_b_kernel<0> keeps no ring.
+    a.fft_only = pl.split_epilogue ? 1 : 0;
+    int rc;
+    if ((rc = launch_spectrum(p, pl, a, st)) != 0) return rc;
+    if (pl.split_epilogue && (rc = launch_epilogue_b(p, pl, a, st)) != 0) return rc;
+    if (pl.k5 == K5Form::NEED_SMEM && (rc = launch_k5_need_smem(p, pl, tb, a, st)) != 0) return rc;
+    if (pl.k5 == K5Form::NEED_L2 && (rc = launch_k5_need(p, pl, tb, a, st)) != 0) return rc;
+    // wave uses plane 0 of each stream only; smoothing the (zero) odd planes too keeps the launch simple
+    if (full_kernel && (rc = launch_k5_full(p, pl, tb.k5, a.av_out, a.tex, a.batch * 2, stream)) != 0) return rc;
+    // NEED_L2: av_transpose_kernel + k5_need_kernel
+    return 1 + pl.split_epilogue + (pl.k5 == K5Form::NEED_SMEM) + 2 * (pl.k5 == K5Form::NEED_L2) + full_kernel;
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -6,8 +6,8 @@
 // av_transpose_kernel + k5_need_kernel) or as a whole-plane kernel (k5_table_kernel, k5_planes_kernel); the FFT pass
 // variant; the persistent grid.  plan_spectrum makes every one of these choices from the effective parameters, the
 // environment overrides (SpectrumKnobs) and the sizes of the host tables (tables.h).  capi.cu build_tables stores the plan
-// on the handle and uploads the tables it names; run_update executes it.  No CUDA here: tests/emul compiles the same
-// decision for the host test tier.
+// on the handle and uploads the tables it names; spectrum_kernels.cu launch_spectrum_update executes it, run_update calls
+// that once per modified update.  No CUDA here: tests/emul compiles the same decision for the host test tier.
 #ifndef GLB_SPECTRUM_PLAN_H
 #define GLB_SPECTRUM_PLAN_H
 
@@ -133,13 +133,13 @@ struct SpectrumPlan {
     int  av_t_len = 0;             // need-list kernels: leading bins of the pre-smoothing texture they read
     K5Form k5 = K5Form::NONE;      // where K5 runs; with a post chain the whole-plane forms follow the upload
     int  tap_ku = 8;               // SpectrumArgs::tap_ku
-    int  table_planes = 0;         // FULL_TABLE: planes per k5_table_kernel CTA
+    int  table_planes = 0;         // full_table: planes per k5_table_kernel CTA (FULL_TABLE, glava_b200_smooth_pass)
     int  k5n_s = 0;                // NEED_L2: streams per lane
     int  k5n_warps = 0;            // NEED_SMEM, NEED_L2: warps per CTA
     int  fft_oop = 0, fft_t = 0;   // FFT pass variant: out of place, threads per CTA (0: the size's default)
     int  spec_grid = 0;            // spectrum_kernel CTAs (fewer than work units: persistent)
     int  spec_resident = 0;        // resident spectrum CTAs per SM it is capped at (0: no cap)
-    std::string refusal;           // non-empty: the K5 launch refuses every update with this error
+    std::string refusal;           // non-empty: every update with a new texture fails with this error before it enqueues anything
 };
 
 // The host tables a plan is computed from, each built the first time the decision reads it (the whole-plane table takes
@@ -205,9 +205,10 @@ inline SpectrumPlan plan_spectrum(const glava_b200_params& p, bool post_chain, i
         if (!k.no_k5_table) {
             build_k5_table_host(p, &t->full);
             pl.full_table = 2 * t->full.max_span * sizeof(float) <= K5_SMEM_MAX && t->full.ent.size() * sizeof(K5Ent) <= (size_t) 256 << 20;
+            if (pl.full_table) pl.table_planes = k5_table_planes(t->full.max_span);
         }
         if (k.fused_k5 && !post_chain) pl.k5 = K5Form::FUSED;
-        else if (pl.full_table) { pl.k5 = K5Form::FULL_TABLE; pl.table_planes = k5_table_planes(t->full.max_span); }
+        else if (pl.full_table) pl.k5 = K5Form::FULL_TABLE;
         else { pl.k5 = K5Form::FULL_PLANES; pl.refusal = k5_planes_refusal(k5_planes_span(p)); }
     }
     // Persistent grid: a few CTAs per SM.  Small on purpose: the kernel is latency bound and is meant to run UNDER the

@@ -139,7 +139,7 @@ TABLE_SIZES = ("need", "need_count", "blob", "tap_bytes", "epi_n", "max_rows", "
 
 
 def table_sizes(p, target_rows=-105, texels_per_block=16, full=True):
-    """the table sizes build_tables and launch_smooth_only choose the K5 launch structure from (emul.cpp emul_table_sizes);
+    """the table sizes plan_spectrum chooses the K5 launch structure from (emul.cpp emul_table_sizes);
     target_rows / texels_per_block as GLAVA_B200_K5N_ROWS / _TPB, defaults as build_tables; full=False skips the
     full-plane table (k5_span, k5_ent_bytes read 0)"""
     out = np.zeros(len(TABLE_SIZES), np.int64)

@@ -19,14 +19,17 @@ from tests import spectrum_cases as sc
 CASES = sc.build_cases()
 
 
-def _run(monkeypatch, case, env):
+def _renderer(monkeypatch, case, env):
     for k in sc.ENV_KEYS:
         monkeypatch.delenv("GLAVA_B200_" + k, raising=False)
     for k, v in env.items():
         monkeypatch.setenv("GLAVA_B200_" + k, v)
-    p = case.params()
+    return g.Renderer(case.params(), batch=case.batch)
+
+
+def _run(monkeypatch, case, env):
     wave = case.module == "wave"
-    with g.Renderer(p, batch=case.batch) as r:
+    with _renderer(monkeypatch, case, env) as r:
         for t, m in enumerate(sc.masks(case)):
             pcm = [sc.stream_pcm(case, t, s) for s in range(case.batch)]
             lb = np.stack([x[0] for x in pcm]); rb = np.stack([x[1] for x in pcm])
@@ -80,8 +83,16 @@ def test_spectrum_parameters_in_every_launch_structure(orc_pm, monkeypatch, case
     for env in case.envs:
         structure, want_launches, refused = sc.launch_structure(case, env)
         if refused:
-            with pytest.raises(g.GlavaError, match=refused):
-                _run(monkeypatch, case, env)
+            with _renderer(monkeypatch, case, env) as r:
+                spec0, count0 = r.spectrum(), r.launch_count
+                lb, rb = sc.stream_pcm(case, 0, 0)
+                assert lb.any()
+                with pytest.raises(g.GlavaError, match=refused):
+                    r.update(np.tile(lb, (case.batch, 1)), None if wave else np.tile(rb, (case.batch, 1)), True)
+                # the refused update enqueued nothing and changed no state
+                assert r.launch_count == count0, (env, r.launch_count, count0)
+                for a, b in zip(r.spectrum(), spec0):
+                    assert np.array_equal(a, b, equal_nan=True), (env, "spectrum after the refused update")
             continue
         got = _run(monkeypatch, case, env)
         assert got[3] == want_launches, (env, structure, got[3], want_launches)
