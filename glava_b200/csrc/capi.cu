@@ -11,6 +11,7 @@
 #include "spectrum_plan.h"
 #include "raster_plan.h"
 #include "stream_state_core.h"
+#include "cuda_owner.h"
 
 #include <cuda_runtime.h>
 
@@ -57,107 +58,142 @@ bool has_error() { return g_has_error; }
 
 using namespace glb;
 
-// The tables build_tables derives from the parameters (audio-independent), freed and rebuilt together on reconfigure and
-// resize.  Device pointers are owned through glava_b200::allocs; null / 0 where the configuration has none.
+// Everything build_tables derives from the parameters alone (audio-independent), released and rebuilt together on every
+// reconfigure and resize: the launch structure of the spectrum update and the tables it reads, the row table, the polar
+// geometry cache and circle tiles, the transform_smooth window table.  The raw pointers are views of `bufs`; null / 0
+// where the configuration has none.
 struct ConfigTables {
+    SpectrumPlan plan;                                        // launch structure of the spectrum update (spectrum_plan.h)
     SpectrumDevTables spec;                                   // the K5 tables the spectrum plan names (internal.h)
     RasterTables raster;                                      // which raster tables exist (raster_plan.h), the cache's box
+    void* rowtab = nullptr;                                   // bars / graph row colours, [h] {fill, outline} RGBA8 pairs
     void* geo = nullptr;                                      // polar geometry cache (radial / circle), see raster_kernels.cu
     void* ctile = nullptr; int ctile_nx = 0, ctile_count = 0; // circle: per-tile texel reference ranges (launch_circle_tiles)
+    void* ts_tab = nullptr; int ts_asz = 0, ts_lim = 0;       // transform_smooth {smin, smax} table
+    std::vector<DevBuf<>> bufs;
 };
 
-struct glava_b200 {
-    glava_b200_params p;        // EFFECTIVE parameters the kernels run with: n = setbufsize / setbufscale, accel_fft
-                                // cleared when a transform follows "fft" (render.c:2143-2154)
-    glava_b200_params p_user;   // as given (glava_b200_get_params)
-    int n_in = 0;               // setbufsize: floats per channel the caller hands to glava_b200_update
-    bool post_chain = false;    // transform_smooth and / or keyframe lerp: the spectrum kernel stops at the float chain
+// The buffers sized by the frame, replaced on a resize: column table (graph / wave; the module of a handle never changes:
+// reconfigure refuses), framebuffers [slots][h][w] RGBA8 and their dirty-row marks
+struct FrameBuffers {
+    DevBuf<float> coltab;       // graph / wave: per-stream column table (launch_raster fills it)
+    DevBuf<uint8_t> fb;
+    DevBuf<uint32_t> marks;     // dirty-row marks of the framebuffer slots (RasterArgs::marks)
+};
+
+// The effective parameters and mode flags of a parameter set
+struct Derived {
+    glava_b200_params p;        // n = setbufsize / setbufscale, accel_fft cleared when a transform follows "fft" (render.c:2143-2154)
+    int n_in;                   // setbufsize: floats per channel the caller hands to glava_b200_update
+    bool interp_on;             // keyframe interpolation active (render.c:1761-1763, 2161-2168)
+    bool post_chain;            // transform_smooth and / or keyframe lerp: the spectrum kernel stops at the float chain
                                 // result; upload + K5 run as separate kernels
-    bool interp_on = false;     // keyframe interpolation active (render.c:1761-1763, 2161-2168)
+};
+
+static Derived derive(const glava_b200_params& user) {
+    Derived d;
+    d.p = user;
+    d.n_in = user.n;
+    d.p.n = user.n / user.bufscale;
+    const bool is_fft = d.p.module != GLAVA_B200_MOD_WAVE;
+    if (d.p.transform_smooth == 1 && is_fft) d.p.accel_fft = 0;           // (2 = "smooth" before "fft": applied to the PCM)
+    const float fr = d.p.fr > 0.0f ? d.p.fr : d.p.ur;
+    d.interp_on = d.p.interpolate && !(d.p.accel_fft && is_fft) && (d.p.ur / fr) <= 0.9f;
+    d.post_chain = d.p.transform_smooth == 1 || d.interp_on;
+    return d;
+}
+
+// Every member that holds a CUDA resource owns it; glava_b200_destroy synchronises the streams before the destructors run.
+struct glava_b200 {
+    glava_b200_params p;        // EFFECTIVE parameters the kernels run with (Derived::p)
+    glava_b200_params p_user;   // as given at the last successful build (glava_b200_get_params)
+    int n_in = 0;
+    bool post_chain = false;
+    bool interp_on = false;
     int  kcounter = 0;          // frames since the last modified update (render.c:2380-2383)
-    float* d_scaled[2] = {};    // bufscale output [batch][n] x {l, r}
-    float* d_key[3] = {}; int key_start = 0, key_end = 1;   // keyframe buffers [batch*2][n] (start, end, the one being written)
+    DevBuf<float> d_scaled[2];  // bufscale output [batch][n] x {l, r}
+    DevBuf<float> d_key[3]; int key_start = 0, key_end = 1;   // keyframe buffers [batch*2][n] (start, end, the one being written)
     float* d_spec_cur = nullptr;   // latest post-transform buffer (glava_b200_spectrum)
-    void* d_ts_tab = nullptr; int ts_asz = 0, ts_lim = 0;   // transform_smooth {smin, smax} table
     std::atomic<unsigned long long> sizereq{0};   // pending glava_b200_sizereq: (1 << 63) | w << 32 | h, 0 = none
     int batch = 0, device = 0, slots = 0;
-    cudaStream_t stream = nullptr;        // raster kernels, read-backs (the stream glava_b200_cuda_stream returns)
+    Stream stream;                        // raster kernels, read-backs (the stream glava_b200_cuda_stream returns)
+    Stream own_spec_stream;               // spec_stream unless GLAVA_B200_NO_OVERLAP makes it `stream`
     cudaStream_t spec_stream = nullptr;   // spectrum kernels + FIFO ingest, lowest priority: the latency-bound spectrum
                                           // kernel of update i+1 runs under the HBM-bound raster kernel of update i
     int    tex_cur = 0;         // which half of d_tex the latest spectrum wrote / the raster reads
-    cudaEvent_t ev_spec_done[2] = {}, ev_raster_done[2] = {};
+    Event ev_spec_done[2], ev_raster_done[2];
     // inputs
-    float* d_pcm[2][2] = {};    // H2D staging for glava_b200_update, double-buffered  [2][batch][n] x {l, r}
+    DevBuf<float> d_pcm[2][2];  // H2D staging for glava_b200_update, double-buffered  [2][batch][n] x {l, r}
     int    stage_cur = 0;
-    cudaEvent_t ev_input = nullptr;   // glava_b200_input_event
+    Event ev_input;             // glava_b200_input_event
     bool   async_input = false; int last_in = -1;   // glava_b200_set_async_input: update() does not wait for its H2D copy
-    cudaStream_t copy_stream = nullptr;   // H2D of update i+1 overlaps the kernels of update i
+    Stream copy_stream;         // H2D of update i+1 overlaps the kernels of update i
     // asynchronous frame read-back: D2D into a staging frame on the raster stream (microseconds), D2H from there on its
     // own stream — the PCIe copy of frame i runs under raster i+1 instead of in front of it
-    cudaStream_t out_stream = nullptr; uint8_t* d_stage[2] = {}; size_t stage_bytes = 0; int out_cur = 0;
-    cudaEvent_t ev_stage_ready[2] = {}, ev_stage_free[2] = {};
-    cudaEvent_t ev_copied[2] = {}, ev_free[2] = {};
-    float* d_ring[2][2] = {};   // FIFO rings, ping-pong                      [2][batch][n] x {l, r}
+    Stream out_stream; DevBuf<uint8_t> d_stage[2]; size_t stage_bytes = 0; int out_cur = 0;
+    Event ev_stage_ready[2], ev_stage_free[2];
+    Event ev_copied[2], ev_free[2];
+    DevBuf<float> d_ring[2][2]; // FIFO rings, ping-pong                      [2][batch][n] x {l, r}
     int    ring_cur = 0;
-    void* d_chunks = nullptr; size_t chunks_cap = 0;
+    DevBuf<> d_chunks; size_t chunks_cap = 0;
     // constants
-    double* d_window = nullptr; float* d_twiddle = nullptr; void* d_rowtab = nullptr;
+    DevBuf<double> d_window; DevBuf<float> d_twiddle;
+    bool built = false;         // tab and frame hold a complete build for p (false after a failed reconfigure or resize)
     ConfigTables tab;           // build_tables
-    SpectrumPlan plan;          // launch structure of the spectrum update (spectrum_plan.h), chosen by build_tables
-    float* d_coltab = nullptr;  // graph / wave: per-stream column table (launch_raster fills it)
-    uint32_t* d_texmm = nullptr;   // circle: per-plane {min, max} of the sampled texture, refreshed before each raster
+    FrameBuffers frame;
+    DevBuf<uint32_t> d_texmm;   // circle: per-plane {min, max} of the sampled texture, refreshed before each raster
     // state + outputs
-    float* d_spec = nullptr; float* d_applied = nullptr; float* d_ring_f = nullptr;
-    uint16_t* d_gr_store = nullptr; uint16_t* d_ring_u = nullptr; uint16_t* d_tex = nullptr;
-    uint16_t* d_av = nullptr;   // pre-smoothing textures [batch*2][n] (full-plane K5 runs as its own kernel)
-    uint8_t* d_fb = nullptr;
-    // dirty-row marks of the framebuffer slots (RasterArgs::marks) and the launch structure that last wrote them
-    // (RasterPlan::mark_key; 0 = none: the next bars / graph / wave launch stores every row)
-    uint32_t* d_marks = nullptr; int mark_key = 0;
+    DevBuf<float> d_spec;
+    DevBuf<char> d_state;       // gravity + average state: the two views below, one allocation
+    float* d_applied = nullptr; float* d_ring_f = nullptr; uint16_t* d_gr_store = nullptr; uint16_t* d_ring_u = nullptr;
+    DevBuf<uint16_t> d_tex;
+    DevBuf<uint16_t> d_av;      // pre-smoothing textures [batch*2][n] (full-plane K5 runs as its own kernel)
+    // the launch structure that last wrote the dirty-row marks (RasterPlan::mark_key; 0 = none: the next bars / graph / wave
+    // launch stores every row)
+    int mark_key = 0;
     unsigned long long updates = 0;
     // per-stream `modified` masks (glava_b200_update_masked): once streams have advanced unevenly, every stream has its
     // own average-ring cursor; words {bit 31 = modified, low bits = cursor} go to the device through a small pinned ring
     bool desync = false;
     std::vector<uint32_t> cursor;          // [batch] modified updates of that stream so far, mod avg_frames (valid once desync)
-    uint32_t* h_umask[4] = {}; uint32_t* d_umask[4] = {}; cudaEvent_t ev_umask[4] = {}; int umask_cur = 0;
+    PinnedBuf<uint32_t> h_umask[4]; DevBuf<uint32_t> d_umask[4]; Event ev_umask[4]; int umask_cur = 0;
     // per-stream state I/O (glava_b200_save_streams / _load_streams / _reset_streams): two device staging halves, each
     // [chunk table: int stream[k], uint32 cursor[k]][blob segments of k streams], allocated on first use; the tables go up
     // from pinned host buffers.  ev_sst_copied[i]: the H2D copies into half i are done; ev_sst_free[i]: its kernel and D2H
     // copies are done
-    void* d_sst[2] = {}; int* h_sst[2] = {}; cudaEvent_t ev_sst_copied[2] = {}, ev_sst_free[2] = {};
+    DevBuf<char> d_sst[2]; PinnedBuf<int> h_sst[2]; Event ev_sst_copied[2], ev_sst_free[2];
     int sst_cur = 0, sst_streams = 0; size_t sst_table = 0;
     uint64_t launches = 0;
-    std::vector<void*> allocs;
     // optional per-kernel device timing (glava_b200_set_timing): events around each launch
     bool timing = false;
-    std::vector<cudaEvent_t> ev_spec; // pairs around each spectrum launch (spec_stream)
-    std::vector<cudaEvent_t> ev_ras;  // pairs around each raster launch (stream)
+    std::vector<Event> ev_spec; // pairs around each spectrum launch (spec_stream)
+    std::vector<Event> ev_ras;  // pairs around each raster launch (stream)
 };
-
-// effective parameters and mode flags from the user's parameters
-static void derive(glava_b200* r) {
-    r->p = r->p_user;
-    r->n_in = r->p_user.n;
-    r->p.n = r->p_user.n / r->p_user.bufscale;
-    const bool is_fft = r->p.module != GLAVA_B200_MOD_WAVE;
-    if (r->p.transform_smooth == 1 && is_fft) r->p.accel_fft = 0;           // (2 = "smooth" before "fft": applied to the PCM)
-    const float fr = r->p.fr > 0.0f ? r->p.fr : r->p.ur;
-    r->interp_on = r->p.interpolate && !(r->p.accel_fft && is_fft) && (r->p.ur / fr) <= 0.9f;
-    r->post_chain = r->p.transform_smooth == 1 || r->interp_on;
-}
 
 // dirty-row marks: one word per (slot, row, 128-pixel strip), so that any band height finds its band's word at its first row
 static size_t mark_bytes(const glava_b200_params& p, int slots) {
     return (size_t) slots * p.h * ((p.w + 127) / 128) * sizeof(uint32_t);
 }
 
-static int dev_alloc(glava_b200* r, void** out, size_t bytes, bool zero) {
-    if (bytes == 0) bytes = 16;
-    cudaError_t e = cudaMalloc(out, bytes);
-    if (e != cudaSuccess)
-        return fail(GLAVA_B200_ECUDA, "cudaMalloc(%zu bytes): %s", bytes, cudaGetErrorString(e));
-    r->allocs.push_back(*out);
-    if (zero) CU(cudaMemsetAsync(*out, 0, bytes, r->stream));
+// A device buffer of `bytes`, zero-filled on `st`
+template <typename T>
+static int alloc_zeroed(DevBuf<T>& b, size_t bytes, cudaStream_t st) {
+    int rc = b.alloc(bytes);
+    if (rc) return rc;
+    CU(cudaMemsetAsync(b, 0, bytes ? bytes : 16, st));
+    return 0;
+}
+
+// A new device buffer of `bytes` owned by `tb`, *view pointing at it: filled from host memory `src` on `st`, zero-filled
+// (`zero`), or left for a kernel to fill
+template <typename T>
+static int table_buf(ConfigTables& tb, T** view, size_t bytes, cudaStream_t st, const void* src, bool zero = false) {
+    DevBuf<> b;
+    int rc = zero ? alloc_zeroed(b, bytes, st) : b.alloc(bytes);
+    if (rc) return rc;
+    if (src && bytes) CU(cudaMemcpyAsync(b, src, bytes, cudaMemcpyHostToDevice, st));
+    *view = (T*) b.get();
+    tb.bufs.push_back(std::move(b));
     return 0;
 }
 
@@ -266,6 +302,7 @@ void* glava_b200_host_alloc_on(size_t bytes, int device) {
     }
     void* p = nullptr;
     if (cudaHostAlloc(&p, bytes, cudaHostAllocPortable) != cudaSuccess) {
+        cudaGetLastError();
         fail(GLAVA_B200_ECUDA, "cudaHostAlloc(%zu) failed", bytes);
         return nullptr;
     }
@@ -290,40 +327,20 @@ void glava_b200_host_free(void* p) {
 
 }  // extern "C"
 
-static void dev_free(glava_b200* r, void* ptr) {
-    if (!ptr) return;
-    for (size_t i = 0; i < r->allocs.size(); ++i) if (r->allocs[i] == ptr) { r->allocs.erase(r->allocs.begin() + i); break; }
-    cudaFree(ptr);
-}
-
-// A new device allocation owned by the handle, filled from host memory.
-static int dev_upload(glava_b200* r, void** out, const void* src, size_t bytes) {
-    int rc = dev_alloc(r, out, bytes, false);
-    if (rc) return rc;
-    if (bytes) CU(cudaMemcpyAsync(*out, src, bytes, cudaMemcpyHostToDevice, r->stream));
-    return 0;
-}
-
-// Everything derived from the parameters that does not depend on the audio: the launch structure of the spectrum update
-// (spectrum_plan.h) and the K5 tables it reads, the bars / graph row-colour table, the polar geometry cache.  Called at
-// creation and again by glava_b200_reconfigure (the analogue of a `--pipe` uniform update, render.c:1846-2005) and on resize.
-static int build_tables(glava_b200* r) {
-    const glava_b200_params& p = r->p;
+// Everything derived from the parameters that does not depend on the audio (ConfigTables), built into `tb` for the
+// parameters of `d`.  Its kernels run on the handle's stream.
+static int build_tables(glava_b200* r, const Derived& d, ConfigTables& tb) {
+    const glava_b200_params& p = d.p;
+    cudaStream_t st = r->stream;
     int rc;
-    ConfigTables& tb = r->tab;
-    SpectrumDevTables& st = tb.spec;
-    for (void* d : { (void*) st.need, (void*) st.tap_tab, (void*) st.tap_cnt, (void*) st.tap_wsum, (void*) st.csr, st.need_blk,
-                     (void*) st.av_t, (void*) st.k5.blk, (void*) st.k5.ent, (void*) st.k5.wsum, tb.geo, tb.ctile })
-        dev_free(r, d);
-    tb = ConfigTables();
+    SpectrumDevTables& sd = tb.spec;
     if (p.transform_smooth) {
         // transform_smooth's sampling window of output t (render.c:700-707) depends on t and the parameters only:
         // evaluated once on the host (chain_core.h), with the same libm calls and types as the reference
         const int sz = p.n;
-        std::vector<SmoothWin> tab;
-        r->ts_asz = transform_smooth_windows(sz, p.smooth_distance, p.smooth_ratio, &tab, &r->ts_lim);
-        CU(cudaMemcpyAsync(r->d_ts_tab, tab.data(), (size_t) sz * sizeof(SmoothWin), cudaMemcpyHostToDevice, r->stream));
-        CU(cudaStreamSynchronize(r->stream));
+        std::vector<SmoothWin> win;
+        tb.ts_asz = transform_smooth_windows(sz, p.smooth_distance, p.smooth_ratio, &win, &tb.ts_lim);
+        if ((rc = table_buf(tb, &tb.ts_tab, (size_t) sz * sizeof(SmoothWin), st, win.data())) != 0) return rc;
     }
     int sm_count = 0;
     if (cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, r->device) != cudaSuccess || sm_count <= 0) {
@@ -331,78 +348,108 @@ static int build_tables(glava_b200* r) {
     }
     SpectrumTables host;
     const SpectrumKnobs knobs = spectrum_knobs([](const char* name) -> const char* { return getenv(name); });
-    r->plan = plan_spectrum(p, r->post_chain, r->batch, sm_count, knobs, &host);
-    const SpectrumPlan& pl = r->plan;
+    tb.plan = plan_spectrum(p, d.post_chain, r->batch, sm_count, knobs, &host);
+    const SpectrumPlan& pl = tb.plan;
     const LazyTables& lt = host.lazy;
     if (pl.need_list) {
-        if ((rc = dev_upload(r, (void**) &st.need, lt.need.data(), lt.need.size() * sizeof(int))) != 0) return rc;
-        st.need_count = (int) lt.cnt;
+        if ((rc = table_buf(tb, &sd.need, lt.need.size() * sizeof(int), st, lt.need.data())) != 0) return rc;
+        sd.need_count = (int) lt.cnt;
     }
     if (pl.tap_table) {
         // tap-major for the L2 path, texel-major blob per channel for the shared-memory path and the need-list kernels
-        if ((rc = dev_upload(r, (void**) &st.tap_tab, lt.tab.data(), lt.tab.size() * sizeof(TapEntry))) != 0 ||
-            (rc = dev_upload(r, (void**) &st.tap_cnt, lt.tcnt.data(), lt.tcnt.size() * sizeof(int))) != 0 ||
-            (rc = dev_upload(r, (void**) &st.tap_wsum, lt.wsum.data(), lt.wsum.size() * sizeof(float))) != 0 ||
-            (rc = dev_upload(r, (void**) &st.csr, lt.csr.data(), lt.csr.size())) != 0) return rc;
-        st.tap_max = (int) lt.tap_max;
-        st.csr_bytes = (int) lt.blob; st.csr_idx_off = (int) lt.idx_off; st.csr_off_off = (int) lt.off_off;
+        if ((rc = table_buf(tb, &sd.tap_tab, lt.tab.size() * sizeof(TapEntry), st, lt.tab.data())) != 0 ||
+            (rc = table_buf(tb, &sd.tap_cnt, lt.tcnt.size() * sizeof(int), st, lt.tcnt.data())) != 0 ||
+            (rc = table_buf(tb, &sd.tap_wsum, lt.wsum.size() * sizeof(float), st, lt.wsum.data())) != 0 ||
+            (rc = table_buf(tb, &sd.csr, lt.csr.size(), st, lt.csr.data())) != 0) return rc;
+        sd.tap_max = (int) lt.tap_max;
+        sd.csr_bytes = (int) lt.blob; sd.csr_idx_off = (int) lt.idx_off; sd.csr_off_off = (int) lt.off_off;
     }
     if (pl.k5 == K5Form::NEED_SMEM) {
         const NeedBlocks& nb = host.blocks;
-        if ((rc = dev_upload(r, &st.need_blk, nb.blk.data(), nb.blk.size() * sizeof(int))) != 0) return rc;
-        st.need_nblk = nb.nblk; st.need_max_rows = nb.max_rows;
+        if ((rc = table_buf(tb, &sd.need_blk, nb.blk.size() * sizeof(int), st, nb.blk.data())) != 0) return rc;
+        sd.need_nblk = nb.nblk; sd.need_max_rows = nb.max_rows;
     } else if (pl.k5 == K5Form::NEED_L2) {
-        if ((rc = dev_alloc(r, (void**) &st.av_t, (size_t) 2 * pl.av_t_len * r->batch * sizeof(float), true)) != 0) return rc;
+        if ((rc = table_buf(tb, &sd.av_t, (size_t) 2 * pl.av_t_len * r->batch * sizeof(float), st, nullptr, true)) != 0) return rc;
     }
     if (pl.full_table) {
         // the taps of ALL n output texels (tables.h build_k5_table_host) for k5_table_kernel
         static_assert(sizeof(K5Blk) == sizeof(int4) && sizeof(K5Ent) == sizeof(int2), "table records are read as int4 / int2");
         const K5TableHost& kt = host.full;
-        if ((rc = dev_upload(r, (void**) &st.k5.blk, kt.blk.data(), kt.blk.size() * sizeof(K5Blk))) != 0 ||
-            (rc = dev_upload(r, (void**) &st.k5.ent, kt.ent.data(), kt.ent.size() * sizeof(K5Ent))) != 0 ||
-            (rc = dev_upload(r, (void**) &st.k5.wsum, kt.wsum.data(), kt.wsum.size() * sizeof(float))) != 0) return rc;
-        st.k5.out = nullptr; st.k5.count = (int) kt.out.size(); st.k5.max_span = kt.max_span;
-        st.k5.smem_bytes = K5_S_PLANES * kt.max_span * (int) sizeof(float);
+        if ((rc = table_buf(tb, &sd.k5.blk, kt.blk.size() * sizeof(K5Blk), st, kt.blk.data())) != 0 ||
+            (rc = table_buf(tb, &sd.k5.ent, kt.ent.size() * sizeof(K5Ent), st, kt.ent.data())) != 0 ||
+            (rc = table_buf(tb, &sd.k5.wsum, kt.wsum.size() * sizeof(float), st, kt.wsum.data())) != 0) return rc;
+        sd.k5.out = nullptr; sd.k5.count = (int) kt.out.size(); sd.k5.max_span = kt.max_span;
+        sd.k5.smem_bytes = K5_S_PLANES * kt.max_span * (int) sizeof(float);
     }
-    if (p.module == GLAVA_B200_MOD_BARS || p.module == GLAVA_B200_MOD_GRAPH) { if ((rc = launch_bars_rowtab(p, r->d_rowtab, r->stream)) != 0) return rc; ++r->launches; }
-    // polar modules: the audio-independent per-pixel geometry; recorded in tb.raster once every table it names exists
+    if ((rc = table_buf(tb, &tb.rowtab, (size_t) p.h * 8, st, nullptr, true)) != 0) return rc;
+    if (p.module == GLAVA_B200_MOD_BARS || p.module == GLAVA_B200_MOD_GRAPH) { if ((rc = launch_bars_rowtab(p, tb.rowtab, st)) != 0) return rc; ++r->launches; }
+    // polar modules: the audio-independent per-pixel geometry
     const RasterTables rt = raster_tables(p, raster_knobs([](const char* name) -> const char* { return getenv(name); }));
     if (rt.geo) {
-        if ((rc = dev_alloc(r, &tb.geo, rt.geo_bytes, false)) != 0) return rc;
-        if ((rc = launch_polar_geo(p, tb.geo, rt.box, r->stream)) != 0) return rc;
+        if ((rc = table_buf(tb, &tb.geo, rt.geo_bytes, st, nullptr)) != 0) return rc;
+        if ((rc = launch_polar_geo(p, tb.geo, rt.box, st)) != 0) return rc;
         ++r->launches;
     }
     if (rt.ctile) {
         int ntx = 0, nty = 0;
         const size_t tile_bytes = circle_tile_bytes(p, &ntx, &nty);
-        if ((rc = dev_alloc(r, &tb.ctile, tile_bytes, false)) != 0) return rc;
-        if ((rc = launch_circle_tiles(p, tb.geo, rt.box, tb.ctile, r->stream)) != 0) return rc;
+        if ((rc = table_buf(tb, &tb.ctile, tile_bytes, st, nullptr)) != 0) return rc;
+        if ((rc = launch_circle_tiles(p, tb.geo, rt.box, tb.ctile, st)) != 0) return rc;
         tb.ctile_nx = ntx; tb.ctile_count = ntx * nty;
         r->launches += 2;
     }
     tb.raster = rt;
-    CU(cudaStreamSynchronize(r->stream));
+    CU(cudaStreamSynchronize(st));
     return 0;
 }
 
-// The buffers sized by the frame: row table, column table (graph / wave; the module of a handle never changes: reconfigure
-// refuses), framebuffers [slots][h][w] RGBA8 and their dirty-row marks.  At creation and on a resize.
-static int alloc_frame_buffers(glava_b200* r) {
-    const glava_b200_params& p = r->p;
+static int alloc_frame_buffers(glava_b200* r, const glava_b200_params& p, FrameBuffers& f) {
     int rc;
-    r->mark_key = 0;
-    if ((rc = dev_alloc(r, &r->d_rowtab, (size_t) p.h * 8, true)) != 0) return rc;
     if ((p.module == GLAVA_B200_MOD_GRAPH || p.module == GLAVA_B200_MOD_WAVE) &&
-        (rc = dev_alloc(r, (void**) &r->d_coltab, (size_t) r->batch * GLB_COLTAB_PLANES * p.w * sizeof(float), true)) != 0) return rc;
-    if ((rc = dev_alloc(r, (void**) &r->d_fb, (size_t) p.w * p.h * 4 * r->slots, true)) != 0) return rc;
-    return dev_alloc(r, (void**) &r->d_marks, mark_bytes(p, r->slots), true);    // empty marks: the framebuffer starts all 0
+        (rc = alloc_zeroed(f.coltab, (size_t) r->batch * GLB_COLTAB_PLANES * p.w * sizeof(float), r->stream)) != 0) return rc;
+    if ((rc = alloc_zeroed(f.fb, (size_t) p.w * p.h * 4 * r->slots, r->stream)) != 0) return rc;
+    return alloc_zeroed(f.marks, mark_bytes(p, r->slots), r->stream);    // empty marks: the framebuffer starts all 0
 }
 
-static int build(glava_b200* r) {
+static int sync_all(glava_b200* r) {
+    CU(cudaStreamSynchronize(r->spec_stream));
+    CU(cudaStreamSynchronize(r->stream));
+    if (r->out_stream.get()) CU(cudaStreamSynchronize(r->out_stream));
+    return 0;
+}
+
+// The one path that builds the renderer for the user parameters `q`: at creation, on glava_b200_reconfigure and on a resize.
+// It releases what the new parameters replace first — the tables, and the frame buffers when the geometry changes or they
+// are missing — so that a rebuild never holds two sets at once, then builds, and commits parameters, flags, tables and
+// plan together once everything has succeeded.  On failure the renderer is unbuilt: it holds no tables, keeps the
+// parameters of its last successful build, and refuses to run (frame_ready) until a rebuild succeeds.
+static int rebuild(glava_b200* r, const glava_b200_params& q) {
+    int rc = validate_params(&q);
+    if (rc) return rc;
+    const Derived d = derive(q);
+    if ((rc = sync_all(r)) != 0) return rc;
+    const bool new_frame = !r->built || !r->frame.fb.get() || q.w != r->p_user.w || q.h != r->p_user.h;
+    r->built = false;
+    r->tab = ConfigTables();
+    if (new_frame) r->frame = FrameBuffers();
+    FrameBuffers f;
+    ConfigTables tb;
+    if (new_frame && (rc = alloc_frame_buffers(r, d.p, f)) != 0) return rc;
+    if ((rc = build_tables(r, d, tb)) != 0) return rc;
+    r->p_user = q; r->p = d.p; r->n_in = d.n_in; r->interp_on = d.interp_on; r->post_chain = d.post_chain;
+    r->tab = std::move(tb);
+    if (new_frame) { r->frame = std::move(f); r->mark_key = 0; }
+    r->built = true;
+    return 0;
+}
+
+// The per-stream state, inputs and constants, sized by parameters that never change on a live renderer
+static int build_state(glava_b200* r) {
     const glava_b200_params& p = r->p;
     const size_t n = (size_t) p.n, planes = (size_t) r->batch * 2, F = (size_t) p.avg_frames;
     CU(cudaSetDevice(r->device));
-    CU(cudaStreamCreateWithFlags(&r->stream, cudaStreamNonBlocking));
+    int rc;
+    if ((rc = r->stream.create(0)) != 0) return rc;
     {
         int lo = 0, hi = 0;
         CU(cudaDeviceGetStreamPriorityRange(&lo, &hi));
@@ -413,41 +460,40 @@ static int build(glava_b200* r) {
         int prio = lo;
         if (pr && !strcmp(pr, "high")) prio = hi; else if (pr && !strcmp(pr, "equal")) prio = 0;
         if (getenv("GLAVA_B200_NO_OVERLAP")) r->spec_stream = r->stream;   // tuning aid: serialise spectrum and raster
-        else CU(cudaStreamCreateWithPriority(&r->spec_stream, cudaStreamNonBlocking, prio));
+        else {
+            if ((rc = r->own_spec_stream.create(prio)) != 0) return rc;
+            r->spec_stream = r->own_spec_stream;
+        }
     }
-    for (int i = 0; i < 2; ++i) {
-        CU(cudaEventCreateWithFlags(&r->ev_spec_done[i], cudaEventDisableTiming));
-        CU(cudaEventCreateWithFlags(&r->ev_raster_done[i], cudaEventDisableTiming));
-    }
-    int rc;
-#define ALLOC(ptr, bytes, zero) if ((rc = dev_alloc(r, (void**) &(ptr), (bytes), (zero))) != 0) return rc
-    CU(cudaStreamCreateWithFlags(&r->copy_stream, cudaStreamNonBlocking));
+    for (int i = 0; i < 2; ++i)
+        if ((rc = r->ev_spec_done[i].create()) != 0 || (rc = r->ev_raster_done[i].create()) != 0) return rc;
+    cudaStream_t st = r->stream;
+#define ALLOC(buf, bytes) if ((rc = alloc_zeroed((buf), (bytes), st)) != 0) return rc
+    if ((rc = r->copy_stream.create(0)) != 0) return rc;
     const size_t n_in = (size_t) r->n_in;
     for (int i = 0; i < 2; ++i) {
-        ALLOC(r->d_pcm[i][0], (size_t) r->batch * n_in * 4, true); ALLOC(r->d_pcm[i][1], (size_t) r->batch * n_in * 4, true);
-        CU(cudaEventCreateWithFlags(&r->ev_copied[i], cudaEventDisableTiming));
-        CU(cudaEventCreateWithFlags(&r->ev_free[i], cudaEventDisableTiming));
+        ALLOC(r->d_pcm[i][0], (size_t) r->batch * n_in * 4); ALLOC(r->d_pcm[i][1], (size_t) r->batch * n_in * 4);
+        if ((rc = r->ev_copied[i].create()) != 0 || (rc = r->ev_free[i].create()) != 0) return rc;
     }
-    for (int i = 0; i < 2; ++i) for (int c = 0; c < 2; ++c) ALLOC(r->d_ring[i][c], (size_t) r->batch * n_in * 4, true);
-    if (r->p_user.bufscale > 1 || r->p_user.transform_smooth == 2) { ALLOC(r->d_scaled[0], (size_t) r->batch * n * 4, true); ALLOC(r->d_scaled[1], (size_t) r->batch * n * 4, true); }
+    for (int i = 0; i < 2; ++i) for (int c = 0; c < 2; ++c) ALLOC(r->d_ring[i][c], (size_t) r->batch * n_in * 4);
+    if (r->p_user.bufscale > 1 || r->p_user.transform_smooth == 2) { ALLOC(r->d_scaled[0], (size_t) r->batch * n * 4); ALLOC(r->d_scaled[1], (size_t) r->batch * n * 4); }
     if (r->interp_on) {
-        for (int i = 0; i < 3; ++i) ALLOC(r->d_key[i], planes * n * 4, true);      // keyframes start at 0 (render.c:1681 calloc)
+        for (int i = 0; i < 3; ++i) ALLOC(r->d_key[i], planes * n * 4);      // keyframes start at 0 (render.c:1681 calloc)
         r->key_start = 0; r->key_end = 1;
     }
-    if (r->p.transform_smooth) ALLOC(r->d_ts_tab, n * sizeof(int2), true);
-    ALLOC(r->d_window, n * 8, false); ALLOC(r->d_twiddle, n * 4, false);
-    ALLOC(r->d_spec, planes * n * 4, true);
+    if ((rc = r->d_window.alloc(n * 8)) != 0 || (rc = r->d_twiddle.alloc(n * 4)) != 0) return rc;
+    ALLOC(r->d_spec, planes * n * 4);
     r->d_spec_cur = r->d_spec;
     // gravity + average state: ONE allocation, so a single L2 access-policy window can cover it (below)
-    char* state = nullptr; size_t state_bytes = 0;
+    size_t state_bytes = 0;
     if (p.accel_fft) {
         state_bytes = planes * n * 2 * (1 + F);
-        ALLOC(state, state_bytes, true);
-        r->d_gr_store = (uint16_t*) state; r->d_ring_u = (uint16_t*) (state + planes * n * 2);
+        ALLOC(r->d_state, state_bytes);
+        r->d_gr_store = (uint16_t*) r->d_state.get(); r->d_ring_u = (uint16_t*) ((char*) r->d_state + planes * n * 2);
     } else {
         state_bytes = planes * n * 4 * (1 + F);
-        ALLOC(state, state_bytes, true);
-        r->d_applied = (float*) state; r->d_ring_f = (float*) (state + planes * n * 4);
+        ALLOC(r->d_state, state_bytes);
+        r->d_applied = (float*) r->d_state.get(); r->d_ring_f = (float*) ((char*) r->d_state + planes * n * 4);
     }
     // EXPERIMENT, off by default (GLAVA_B200_L2_PERSIST=1): pin the spectrum kernel's read-modify-write
     // state in the 50 MB L2 with a persisting access window, so that its DRAM reads do not get mixed into
@@ -461,7 +507,7 @@ static int build(glava_b200* r) {
             cudaStreamAttrValue attr;
             memset(&attr, 0, sizeof(attr));
             size_t win = state_bytes < (size_t) prop.accessPolicyMaxWindowSize ? state_bytes : (size_t) prop.accessPolicyMaxWindowSize;
-            attr.accessPolicyWindow.base_ptr = state;
+            attr.accessPolicyWindow.base_ptr = r->d_state;
             attr.accessPolicyWindow.num_bytes = win;
             attr.accessPolicyWindow.hitRatio = win > 0 ? (float) ((double) want / (double) win) : 0.0f;
             if (attr.accessPolicyWindow.hitRatio > 1.0f) attr.accessPolicyWindow.hitRatio = 1.0f;
@@ -470,16 +516,15 @@ static int build(glava_b200* r) {
             if (cudaStreamSetAttribute(r->spec_stream, cudaStreamAttributeAccessPolicyWindow, &attr) != cudaSuccess) cudaGetLastError();
         }
     }
-    ALLOC(r->d_tex, 2 * planes * n * 2, true);
-    ALLOC(r->d_av, planes * n * 2, true);
-    ALLOC(r->d_texmm, planes * GLB_TEXMM_STRIDE * sizeof(uint32_t), true);          // one buffer: texmm_kernel fills it on the raster stream right before the circle raster reads it
-    r->slots = (p.fb_slots > 0 && p.fb_slots < r->batch) ? p.fb_slots : r->batch;
-    if ((rc = alloc_frame_buffers(r)) != 0) return rc;
+    ALLOC(r->d_tex, 2 * planes * n * 2);
+    ALLOC(r->d_av, planes * n * 2);
+    ALLOC(r->d_texmm, planes * GLB_TEXMM_STRIDE * sizeof(uint32_t));          // one buffer: texmm_kernel fills it on the raster stream right before the circle raster reads it
 #undef ALLOC
+    r->slots = (p.fb_slots > 0 && p.fb_slots < r->batch) ? p.fb_slots : r->batch;
     // window LUT: render.c:660 macro as expanded at render.c:794 — cos(TWOPI*i/N - 1), double
     std::vector<double> w(n);
     for (size_t i = 0; i < n; ++i) w[i] = 0.53836 - (0.46164 * cos(6.28318530718 * (double) i / (double) n - 1));
-    CU(cudaMemcpyAsync(r->d_window, w.data(), n * 8, cudaMemcpyHostToDevice, r->stream));
+    CU(cudaMemcpyAsync(r->d_window, w.data(), n * 8, cudaMemcpyHostToDevice, st));
     // twiddles exp(-2*pi*i*k/M), M = n/2, evaluated in double
     const size_t M = n / 2;
     std::vector<float> tw(2 * M);
@@ -487,10 +532,8 @@ static int build(glava_b200* r) {
         double ang = -2.0 * M_PI * (double) k / (double) M;
         tw[2 * k] = (float) cos(ang); tw[2 * k + 1] = (float) sin(ang);
     }
-    CU(cudaMemcpyAsync(r->d_twiddle, tw.data(), n * 4, cudaMemcpyHostToDevice, r->stream));
-    CU(cudaStreamSynchronize(r->stream));
-    if ((rc = build_tables(r)) != 0) return rc;
-    CU(cudaStreamSynchronize(r->stream));
+    CU(cudaMemcpyAsync(r->d_twiddle, tw.data(), n * 4, cudaMemcpyHostToDevice, st));
+    CU(cudaStreamSynchronize(st));
     return 0;
 }
 
@@ -505,45 +548,18 @@ glava_b200* glava_b200_new(const glava_b200_params* params, int batch, int devic
     }
     if (device < 0 || device >= ndev) { fail(GLAVA_B200_EINVAL, "device %d out of range (%d devices)", device, ndev); return nullptr; }
     glava_b200* r = new glava_b200();
-    r->p_user = *params; r->batch = batch; r->device = device;
-    derive(r);
-    if (build(r) != 0) { glava_b200_destroy(r); return nullptr; }
+    r->batch = batch; r->device = device;
+    const Derived d = derive(*params);
+    r->p_user = *params; r->p = d.p; r->n_in = d.n_in; r->interp_on = d.interp_on; r->post_chain = d.post_chain;
+    if (build_state(r) != 0 || rebuild(r, *params) != 0) { glava_b200_destroy(r); return nullptr; }
     return r;
 }
 
 void glava_b200_destroy(glava_b200* r) {
     if (!r) return;
     cudaSetDevice(r->device);
-    if (r->spec_stream) cudaStreamSynchronize(r->spec_stream);
-    if (r->stream) cudaStreamSynchronize(r->stream);
-    for (cudaEvent_t e : r->ev_spec) cudaEventDestroy(e);
-    for (cudaEvent_t e : r->ev_ras) cudaEventDestroy(e);
-    for (int i = 0; i < 2; ++i) { if (r->ev_spec_done[i]) cudaEventDestroy(r->ev_spec_done[i]); if (r->ev_raster_done[i]) cudaEventDestroy(r->ev_raster_done[i]); }
-    if (r->spec_stream && r->spec_stream != r->stream) cudaStreamDestroy(r->spec_stream);
-    for (void* p : r->allocs) cudaFree(p);
-    if (r->d_chunks) cudaFree(r->d_chunks);
-    for (int i = 0; i < 2; ++i) { if (r->ev_copied[i]) cudaEventDestroy(r->ev_copied[i]); if (r->ev_free[i]) cudaEventDestroy(r->ev_free[i]); }
-    for (int i = 0; i < 4; ++i) {
-        if (r->h_umask[i]) cudaFreeHost(r->h_umask[i]);
-        if (r->d_umask[i]) cudaFree(r->d_umask[i]);
-        if (r->ev_umask[i]) cudaEventDestroy(r->ev_umask[i]);
-    }
-    if (r->ev_input) cudaEventDestroy(r->ev_input);
-    if (r->copy_stream) cudaStreamSynchronize(r->copy_stream);
-    for (int i = 0; i < 2; ++i) {
-        if (r->d_sst[i]) cudaFree(r->d_sst[i]);
-        if (r->h_sst[i]) cudaFreeHost(r->h_sst[i]);
-        if (r->ev_sst_copied[i]) cudaEventDestroy(r->ev_sst_copied[i]);
-        if (r->ev_sst_free[i]) cudaEventDestroy(r->ev_sst_free[i]);
-    }
-    if (r->copy_stream) cudaStreamDestroy(r->copy_stream);
-    if (r->out_stream) { cudaStreamSynchronize(r->out_stream); cudaStreamDestroy(r->out_stream); }
-    for (int i = 0; i < 2; ++i) {
-        if (r->d_stage[i]) cudaFree(r->d_stage[i]);
-        if (r->ev_stage_ready[i]) cudaEventDestroy(r->ev_stage_ready[i]);
-        if (r->ev_stage_free[i]) cudaEventDestroy(r->ev_stage_free[i]);
-    }
-    if (r->stream) cudaStreamDestroy(r->stream);
+    for (cudaStream_t s : { r->spec_stream, r->stream.get(), r->copy_stream.get(), r->out_stream.get() })
+        if (s) cudaStreamSynchronize(s);
     delete r;
 }
 
@@ -553,19 +569,14 @@ int glava_b200_reconfigure(glava_b200* r, const glava_b200_params* params) {
     int rc = validate_params(params);
     if (rc) return rc;
     const glava_b200_params& o = r->p_user;
-    glava_b200 probe; probe.p_user = *params; derive(&probe);
     if (params->n != o.n || params->w != o.w || params->h != o.h || params->module != o.module || params->accel_fft != o.accel_fft ||
         params->avg_frames != o.avg_frames || params->fb_slots != o.fb_slots || params->bufscale != o.bufscale ||
-        params->transform_smooth != o.transform_smooth || probe.interp_on != r->interp_on)
+        params->transform_smooth != o.transform_smooth || derive(*params).interp_on != r->interp_on)
         return fail(GLAVA_B200_EINVAL, "glava_b200_reconfigure: setbufsize, setbufscale, geometry, module, setaccelfft, setavgframes, "
                                        "fb_slots, the \"smooth\" transform and whether interpolation is active size the device "
                                        "state and cannot change on a live renderer; create a new one");
     CU(cudaSetDevice(r->device));
-    CU(cudaStreamSynchronize(r->spec_stream));
-    CU(cudaStreamSynchronize(r->stream));
-    r->p_user = *params;
-    derive(r);
-    return build_tables(r);
+    return rebuild(r, *params);
 }
 
 int glava_b200_get_params(const glava_b200* r, glava_b200_params* out) {
@@ -575,41 +586,35 @@ int glava_b200_get_params(const glava_b200* r, glava_b200_params* out) {
 int glava_b200_batch(const glava_b200* r) { return r ? r->batch : 0; }
 const char* glava_b200_module_name(const glava_b200* r) { return r ? module_name(r->p.module) : "?"; }
 int glava_b200_spectrum_size(const glava_b200* r) { return r ? r->p.n : 0; }
-const void* glava_b200_framebuffer_device(const glava_b200* r) { return r ? r->d_fb : nullptr; }
+const void* glava_b200_framebuffer_device(const glava_b200* r) { return r ? r->frame.fb.get() : nullptr; }
 void* glava_b200_cuda_stream(const glava_b200* r) { return r ? (void*) r->stream : nullptr; }
 uint64_t glava_b200_launch_count(const glava_b200* r) { return r ? r->launches : 0; }
 
-static int timing_mark(std::vector<cudaEvent_t>& v, cudaStream_t st) {
-    cudaEvent_t e;
-    CU(cudaEventCreate(&e));
+static int timing_mark(std::vector<Event>& v, cudaStream_t st) {
+    Event e;
+    int rc = e.create(cudaEventDefault);
+    if (rc) return rc;
     CU(cudaEventRecord(e, st));
-    v.push_back(e);
+    v.push_back(std::move(e));
     return 0;
 }
 
 static uint16_t* tex_half(glava_b200* r, int b) { return r->d_tex + (size_t) b * r->batch * 2 * r->p.n; }
-static int sync_all(glava_b200* r) {
-    CU(cudaStreamSynchronize(r->spec_stream));
-    CU(cudaStreamSynchronize(r->stream));
-    if (r->out_stream) CU(cudaStreamSynchronize(r->out_stream));
-    return 0;
-}
-
 // Runtime resize (render.c:1811-1830 resizes the stage FBOs when the framebuffer size changed; offscreen consumers ask
-// through glava_sizereq, glava.c:263-267).  Spectrum state is untouched; the framebuffers and every table that depends
-// on the geometry (row colours, polar geometry cache, lazy-K5 need-list) are rebuilt.
-static int apply_resize(glava_b200* r, int w, int h) {
-    glava_b200_params q = r->p_user;
-    q.w = w; q.h = h;
-    int rc = validate_params(&q);
-    if (rc) return rc;
-    if ((rc = sync_all(r)) != 0) return rc;
-    dev_free(r, r->d_fb); dev_free(r, r->d_marks); dev_free(r, r->d_rowtab); dev_free(r, r->d_coltab);
-    r->d_fb = nullptr; r->d_marks = nullptr; r->d_rowtab = nullptr; r->d_coltab = nullptr;
-    r->p_user = q;
-    derive(r);
-    if ((rc = alloc_frame_buffers(r)) != 0) return rc;
-    return build_tables(r);
+// through glava_sizereq, glava.c:263-267), applied at the start of a frame (render.c:1811-1815).  Spectrum state is
+// untouched; the framebuffers and every table (row colours, polar geometry cache, lazy-K5 need-list) are rebuilt.  Then a
+// renderer that a failed reconfigure or resize left unbuilt refuses to run, before anything is enqueued.
+static int unbuilt() {
+    return fail(GLAVA_B200_ECUDA, "the renderer has no tables: a reconfigure or resize failed and must be repeated");
+}
+static int frame_ready(glava_b200* r) {
+    if (unsigned long long req = r->sizereq.exchange(0)) {
+        glava_b200_params q = r->p_user;
+        q.w = (int) ((req >> 32) & 0x7fffffffu); q.h = (int) (req & 0xffffffffu);
+        int rc = rebuild(r, q);
+        if (rc) return rc;
+    }
+    return r->built ? 0 : unbuilt();
 }
 
 // One update = spectrum kernel on spec_stream (if modified) + raster kernel on stream.
@@ -626,10 +631,10 @@ static int stage_umask(glava_b200* r, const uint8_t* mask, const uint32_t** d_ou
         r->desync = true;
     }
     const int k = r->umask_cur;
-    if (!r->h_umask[k]) {
-        CU(cudaHostAlloc((void**) &r->h_umask[k], (size_t) r->batch * 4, cudaHostAllocDefault));
-        CU(cudaMalloc((void**) &r->d_umask[k], (size_t) r->batch * 4));
-        CU(cudaEventCreateWithFlags(&r->ev_umask[k], cudaEventDisableTiming));
+    if (!r->ev_umask[k].get()) {                              // created last: the slot is complete
+        int rc;
+        if ((rc = r->h_umask[k].alloc((size_t) r->batch * 4)) != 0 || (rc = r->d_umask[k].alloc((size_t) r->batch * 4)) != 0 ||
+            (rc = r->ev_umask[k].create()) != 0) return rc;
     } else {
         CU(cudaEventSynchronize(r->ev_umask[k]));               // the copy that last read this pinned buffer (4 updates ago)
     }
@@ -658,17 +663,14 @@ static int run_update(glava_b200* r, const float* d_l, const float* d_r, int mod
             return fail(GLAVA_B200_EINVAL, "per-stream modified masks are not available with keyframe interpolation active "
                                            "(setinterpolate): the keyframe rotation is per renderer; update the streams in lock step");
     } else mask = nullptr;
-    if (unsigned long long req = r->sizereq.exchange(0)) {                  // render.c:1811-1815: at the start of a frame
-        if ((rc = apply_resize(r, (int) ((req >> 32) & 0x7fffffffu), (int) (req & 0xffffffffu))) != 0) return rc;
-    }
-    if (!r->d_fb) return fail(GLAVA_B200_ECUDA, "renderer has no framebuffer (a resize failed)");
+    if ((rc = frame_ready(r)) != 0) return rc;
     const glava_b200_params& p = r->p;
     const bool new_tex = !raster_only && (modified || r->interp_on);   // an interpolated frame has a new texture without new audio
     const int planes = r->batch * 2;
     const size_t total = (size_t) planes * p.n;
     // a K5 form the plan refuses (spectrum_plan.h) fails every update with a new texture before it enqueues anything or
     // changes any state
-    if (new_tex && !r->plan.refusal.empty()) return fail(GLAVA_B200_EINVAL, "%s", r->plan.refusal.c_str());
+    if (new_tex && !r->tab.plan.refusal.empty()) return fail(GLAVA_B200_EINVAL, "%s", r->tab.plan.refusal.c_str());
     if (new_tex) CU(cudaStreamWaitEvent(r->spec_stream, r->ev_raster_done[r->tex_cur ^ 1], 0));
     if (modified && r->p_user.bufscale > 1) {
         const int chans = p.module == GLAVA_B200_MOD_WAVE ? 1 : 2;
@@ -684,7 +686,7 @@ static int run_update(glava_b200* r, const float* d_l, const float* d_r, int mod
         const float* src[2] = { d_l, d_r };
         for (int c = 0; c < chans; ++c) {
             if (src[c] != r->d_scaled[c]) CU(cudaMemcpyAsync(r->d_scaled[c], src[c], (size_t) r->batch * p.n * 4, cudaMemcpyDeviceToDevice, r->spec_stream));
-            if ((rc = launch_transform_smooth(r->d_scaled[c], p.n, r->d_ts_tab, r->ts_asz, r->ts_lim, r->batch, r->spec_stream, nullptr, 0)) != 0) return rc;
+            if ((rc = launch_transform_smooth(r->d_scaled[c], p.n, r->tab.ts_tab, r->tab.ts_asz, r->tab.ts_lim, r->batch, r->spec_stream, nullptr, 0)) != 0) return rc;
             ++r->launches;
         }
         d_l = r->d_scaled[0]; d_r = chans == 2 ? r->d_scaled[1] : r->d_scaled[0];
@@ -714,10 +716,10 @@ static int run_update(glava_b200* r, const float* d_l, const float* d_r, int mod
         a.avg_b_windowed = (p.avg_window && F != 2) ? 1 : 0;
         if (r->timing && (rc = timing_mark(r->ev_spec, r->spec_stream)) != 0) return rc;
         // in the launch structure build_tables chose (spectrum_plan.h)
-        if ((rc = launch_spectrum_update(p, r->plan, r->tab.spec, a, r->spec_stream)) < 0) return rc;
+        if ((rc = launch_spectrum_update(p, r->tab.plan, r->tab.spec, a, r->spec_stream)) < 0) return rc;
         r->launches += (uint64_t) rc;
         if (r->post_chain && p.transform_smooth == 1) {                     // render.c:694-718, after the module's chain
-            if ((rc = launch_transform_smooth(chain_out, p.n, r->d_ts_tab, r->ts_asz, r->ts_lim, planes, r->spec_stream, a.umask)) != 0) return rc;
+            if ((rc = launch_transform_smooth(chain_out, p.n, r->tab.ts_tab, r->tab.ts_asz, r->tab.ts_lim, planes, r->spec_stream, a.umask)) != 0) return rc;
             ++r->launches;
         }
         if (!r->post_chain) {
@@ -743,7 +745,7 @@ static int run_update(glava_b200* r, const float* d_l, const float* d_r, int mod
         if (rc) return rc;
         ++r->launches;
         if (p.smooth_pass) {
-            if ((rc = launch_k5_full(p, r->plan, r->tab.spec.k5, r->d_av, tex_half(r, b), planes, r->spec_stream)) != 0) return rc;
+            if ((rc = launch_k5_full(p, r->tab.plan, r->tab.spec.k5, r->d_av, tex_half(r, b), planes, r->spec_stream)) != 0) return rc;
             ++r->launches;
         }
         if (modified && r->timing && (rc = timing_mark(r->ev_spec, r->spec_stream)) != 0) return rc;
@@ -763,17 +765,17 @@ static int run_update(glava_b200* r, const float* d_l, const float* d_r, int mod
     const ConfigTables& tb = r->tab;
     const RasterPlan pl = plan_raster(view, tb.raster, r->batch, r->slots, knobs);
     RasterArgs ra;
-    ra.tex = tex_half(r, b); ra.fb = r->d_fb;
-    ra.rowtab = pl.rowtab ? r->d_rowtab : nullptr;
+    ra.tex = tex_half(r, b); ra.fb = r->frame.fb;
+    ra.rowtab = pl.rowtab ? tb.rowtab : nullptr;
     ra.batch = r->batch; ra.slots = r->slots; ra.stream0 = 0;
     ra.geo = pl.geo ? tb.geo : nullptr;
     ra.gx0 = tb.raster.box[0]; ra.gy0 = tb.raster.box[1]; ra.gw = tb.raster.box[2]; ra.gh = tb.raster.box[3];
-    ra.texmm = pl.texmm ? r->d_texmm : nullptr;
+    ra.texmm = pl.texmm ? (const uint32_t*) r->d_texmm : nullptr;
     ra.ctile = pl.ctile ? (const int4*) tb.ctile : nullptr;
     ra.ctile_zero = pl.ctile ? (const int*) ((const int4*) tb.ctile + tb.ctile_count) : nullptr;
     ra.ctile_nx = pl.ctile ? tb.ctile_nx : 0;
-    ra.coltab = pl.coltab ? r->d_coltab : nullptr;
-    ra.marks = r->d_marks; ra.marks_valid = raster_marks_valid(pl, r->mark_key, knobs) ? 1 : 0;
+    ra.coltab = pl.coltab ? (float*) r->frame.coltab : nullptr;
+    ra.marks = r->frame.marks; ra.marks_valid = raster_marks_valid(pl, r->mark_key, knobs) ? 1 : 0;
     if (pl.texmm && (rc = launch_texmm(p, ra.tex, r->d_texmm, r->batch * 2, r->stream)) != 0) return rc;
     r->mark_key = 0;                                      // until every launch of the pass is enqueued
     if (r->timing && (rc = timing_mark(r->ev_ras, r->stream)) != 0) return rc;
@@ -799,6 +801,8 @@ static int update_host(glava_b200* r, const float* lb, const float* rb, size_t b
     if (modified && !rb && r->p.module != GLAVA_B200_MOD_WAVE)
         return fail(GLAVA_B200_EINVAL, "glava_b200_update: module '%s' reads both channels, rb is null", module_name(r->p.module));
     CU(cudaSetDevice(r->device));
+    int rc = frame_ready(r);
+    if (rc) return rc;
     size_t bytes = (size_t) r->batch * bsz * 4;
     const int b = r->stage_cur;
     if (modified) {
@@ -812,8 +816,7 @@ static int update_host(glava_b200* r, const float* lb, const float* rb, size_t b
         CU(cudaEventRecord(r->ev_copied[b], r->copy_stream));
         CU(cudaStreamWaitEvent(r->spec_stream, r->ev_copied[b], 0));
     }
-    int rc = run_update(r, r->d_pcm[b][0], r->d_pcm[b][1], modified, false, mask);
-    if (rc) return rc;
+    if ((rc = run_update(r, r->d_pcm[b][0], r->d_pcm[b][1], modified, false, mask)) != 0) return rc;
     if (modified) {
         CU(cudaEventRecord(r->ev_free[b], r->spec_stream));
         r->stage_cur = b ^ 1;
@@ -876,7 +879,7 @@ int glava_b200_update_device_after(glava_b200* r, const float* d_lb, const float
 }
 void* glava_b200_input_event(glava_b200* r) {
     if (!r) return nullptr;
-    if (!r->ev_input) { if (cudaEventCreateWithFlags(&r->ev_input, cudaEventDisableTiming) != cudaSuccess) { cudaGetLastError(); return nullptr; } }
+    if (!r->ev_input.get() && r->ev_input.create() != 0) return nullptr;
     cudaSetDevice(r->device);
     cudaEventRecord(r->ev_input, r->spec_stream);          // after everything enqueued so far on the reading stream
     return (void*) r->ev_input;
@@ -901,9 +904,9 @@ static int ingest(glava_b200* r, const void* chunks, bool float_in, int frames, 
     size_t bytes = (size_t) r->batch * frames * 2 * (float_in ? sizeof(float) : sizeof(int16_t));
     if (bytes > r->chunks_cap) {
         CU(cudaStreamSynchronize(r->spec_stream));
-        if (r->d_chunks) cudaFree(r->d_chunks);
-        r->d_chunks = nullptr; r->chunks_cap = 0;
-        CU(cudaMalloc((void**) &r->d_chunks, bytes));
+        r->chunks_cap = 0;
+        int rc = r->d_chunks.alloc(bytes);
+        if (rc) return rc;
         r->chunks_cap = bytes;
     }
     // ordered with the spectrum kernels (they read the rings): same stream
@@ -940,15 +943,15 @@ int glava_b200_wait_frame(glava_b200* r) {
 }
 void* glava_b200_frame_event(const glava_b200* r) { return r ? (void*) r->ev_raster_done[r->tex_cur] : nullptr; }
 const void* glava_b200_frame_device(const glava_b200* r, int stream) {
-    if (!r || stream < 0 || stream >= r->batch || !r->d_fb) return nullptr;
-    return r->d_fb + (size_t) r->p.w * r->p.h * 4 * (size_t) (stream % r->slots);
+    if (!r || stream < 0 || stream >= r->batch || !r->frame.fb) return nullptr;
+    return r->frame.fb + (size_t) r->p.w * r->p.h * 4 * (size_t) (stream % r->slots);
 }
 int glava_b200_framebuffer_ipc(glava_b200* r, void* handle, size_t handle_bytes) {
     clear_error();
     if (!r || !handle || handle_bytes < sizeof(cudaIpcMemHandle_t)) return fail(GLAVA_B200_EINVAL, "glava_b200_framebuffer_ipc: need a %zu-byte buffer", sizeof(cudaIpcMemHandle_t));
     CU(cudaSetDevice(r->device));
     cudaIpcMemHandle_t h;
-    CU(cudaIpcGetMemHandle(&h, r->d_fb));
+    CU(cudaIpcGetMemHandle(&h, r->frame.fb));
     memcpy(handle, &h, sizeof(h));
     return 0;
 }
@@ -957,8 +960,6 @@ int glava_b200_set_timing(glava_b200* r, int enable) {
     if (!r) return fail(GLAVA_B200_EINVAL, "null argument");
     CU(cudaSetDevice(r->device));
     int rc0 = sync_all(r); if (rc0) return rc0;
-    for (cudaEvent_t e : r->ev_spec) cudaEventDestroy(e);
-    for (cudaEvent_t e : r->ev_ras) cudaEventDestroy(e);
     r->ev_spec.clear(); r->ev_ras.clear();
     r->timing = enable != 0;
     return 0;
@@ -1009,7 +1010,7 @@ int glava_b200_readback(glava_b200* r, int stream, uint8_t* rgba) {
     if (!r || !rgba || stream < 0 || stream >= r->batch) return fail(GLAVA_B200_EINVAL, "glava_b200_readback: bad arguments");
     CU(cudaSetDevice(r->device));
     size_t frame = (size_t) r->p.w * r->p.h * 4;
-    CU(cudaMemcpyAsync(rgba, r->d_fb + frame * (size_t) (stream % r->slots), frame, cudaMemcpyDeviceToHost, r->stream));
+    CU(cudaMemcpyAsync(rgba, r->frame.fb + frame * (size_t) (stream % r->slots), frame, cudaMemcpyDeviceToHost, r->stream));
     CU(cudaStreamSynchronize(r->stream));
     return 0;
 }
@@ -1019,25 +1020,24 @@ int glava_b200_readback_async(glava_b200* r, int stream, uint8_t* rgba) {
     if (!r || !rgba || stream < 0 || stream >= r->batch) return fail(GLAVA_B200_EINVAL, "glava_b200_readback_async: bad arguments");
     CU(cudaSetDevice(r->device));
     const size_t frame = (size_t) r->p.w * r->p.h * 4;
-    if (!r->out_stream) {
-        CU(cudaStreamCreateWithFlags(&r->out_stream, cudaStreamNonBlocking));
-        for (int i = 0; i < 2; ++i) {
-            CU(cudaEventCreateWithFlags(&r->ev_stage_ready[i], cudaEventDisableTiming));
-            CU(cudaEventCreateWithFlags(&r->ev_stage_free[i], cudaEventDisableTiming));
-        }
+    int rc;
+    if (!r->ev_stage_free[1].get()) {                      // created last: the read-back stream and its events are complete
+        if ((rc = r->out_stream.create(0)) != 0) return rc;
+        for (int i = 0; i < 2; ++i)
+            if ((rc = r->ev_stage_ready[i].create()) != 0 || (rc = r->ev_stage_free[i].create()) != 0) return rc;
     }
     if (r->stage_bytes != frame) {                       // first use, or the geometry changed (glava_b200_sizereq)
         CU(cudaStreamSynchronize(r->out_stream));
-        for (int i = 0; i < 2; ++i) { if (r->d_stage[i]) cudaFree(r->d_stage[i]); r->d_stage[i] = nullptr; }
         r->stage_bytes = 0;
-        for (int i = 0; i < 2; ++i) CU(cudaMalloc((void**) &r->d_stage[i], frame));
+        for (int i = 0; i < 2; ++i) { r->d_stage[i].reset(); }
+        for (int i = 0; i < 2; ++i) if ((rc = r->d_stage[i].alloc(frame)) != 0) return rc;
         r->stage_bytes = frame;
     }
     const int i = r->out_cur;
     // the frame is snapshotted on the raster stream (ordered after the raster that produced it, before the next one
     // overwrites the slot); the slow PCIe leg then runs from the snapshot on its own stream
     CU(cudaStreamWaitEvent(r->stream, r->ev_stage_free[i], 0));
-    CU(cudaMemcpyAsync(r->d_stage[i], r->d_fb + frame * (size_t) (stream % r->slots), frame, cudaMemcpyDeviceToDevice, r->stream));
+    CU(cudaMemcpyAsync(r->d_stage[i], r->frame.fb + frame * (size_t) (stream % r->slots), frame, cudaMemcpyDeviceToDevice, r->stream));
     CU(cudaEventRecord(r->ev_stage_ready[i], r->stream));
     CU(cudaStreamWaitEvent(r->out_stream, r->ev_stage_ready[i], 0));
     CU(cudaMemcpyAsync(rgba, r->d_stage[i], frame, cudaMemcpyDeviceToHost, r->out_stream));
@@ -1050,7 +1050,7 @@ int glava_b200_readback_async(glava_b200* r, int stream, uint8_t* rgba) {
 // on a separate stream): an event recorded on glava_b200_cuda_stream() after this call covers them.
 int glava_b200_readback_fence(glava_b200* r) {
     if (!r) return fail(GLAVA_B200_EINVAL, "null argument");
-    if (!r->out_stream) return 0;
+    if (!r->ev_stage_free[1].get()) return 0;
     CU(cudaSetDevice(r->device));
     for (int i = 0; i < 2; ++i) CU(cudaStreamWaitEvent(r->stream, r->ev_stage_free[i], 0));
     return 0;
@@ -1081,32 +1081,29 @@ int glava_b200_textures(glava_b200* r, uint16_t* out_l, uint16_t* out_r) {
 int glava_b200_smooth_pass(glava_b200* r, const uint16_t* in, uint16_t* out, int count) {
     clear_error();
     if (!r || !in || !out || count < 1) return fail(GLAVA_B200_EINVAL, "glava_b200_smooth_pass: bad arguments");
+    if (!r->built) return unbuilt();
     CU(cudaSetDevice(r->device));
     // the renderer's whole-plane table when it has one, else k5_planes_kernel where its spans fit shared memory
-    const std::string refusal = r->plan.full_table ? std::string() : k5_planes_refusal(k5_planes_span(r->p));
+    const std::string refusal = r->tab.plan.full_table ? std::string() : k5_planes_refusal(k5_planes_span(r->p));
     if (!refusal.empty()) return fail(GLAVA_B200_EINVAL, "%s", refusal.c_str());
-    size_t bytes = (size_t) count * r->p.n * 2;
-    uint16_t* d_in = nullptr; uint16_t* d_out = nullptr;
-    CU(cudaMalloc((void**) &d_in, bytes));
-    cudaError_t e = cudaMalloc((void**) &d_out, bytes);
-    if (e != cudaSuccess) { cudaFree(d_in); return fail(GLAVA_B200_ECUDA, "cudaMalloc: %s", cudaGetErrorString(e)); }
-    int rc = 0;
-    do {
-        if (cudaMemcpyAsync(d_in, in, bytes, cudaMemcpyHostToDevice, r->stream) != cudaSuccess) { rc = fail(GLAVA_B200_ECUDA, "H2D copy failed"); break; }
-        if ((rc = launch_k5_full(r->p, r->plan, r->tab.spec.k5, d_in, d_out, count, r->stream)) != 0) break;
-        ++r->launches;
-        if (cudaMemcpyAsync(out, d_out, bytes, cudaMemcpyDeviceToHost, r->stream) != cudaSuccess) { rc = fail(GLAVA_B200_ECUDA, "D2H copy failed"); break; }
-        cudaError_t se = cudaStreamSynchronize(r->stream);
-        if (se != cudaSuccess) rc = fail(GLAVA_B200_ECUDA, "smooth pass: %s", cudaGetErrorString(se));
-    } while (0);
-    cudaFree(d_in); cudaFree(d_out);
-    return rc;
+    const size_t bytes = (size_t) count * r->p.n * 2;
+    DevBuf<uint16_t> d_in, d_out;
+    int rc;
+    if ((rc = d_in.alloc(bytes)) != 0 || (rc = d_out.alloc(bytes)) != 0) return rc;
+    CU(cudaMemcpyAsync(d_in, in, bytes, cudaMemcpyHostToDevice, r->stream));
+    if ((rc = launch_k5_full(r->p, r->tab.plan, r->tab.spec.k5, d_in, d_out, count, r->stream)) != 0) return rc;
+    ++r->launches;
+    CU(cudaMemcpyAsync(out, d_out, bytes, cudaMemcpyDeviceToHost, r->stream));
+    CU(cudaStreamSynchronize(r->stream));
+    return 0;
 }
 
 int glava_b200_raster_textures(glava_b200* r, const uint16_t* tex_l, const uint16_t* tex_r) {
     clear_error();
     if (!r || !tex_l) return fail(GLAVA_B200_EINVAL, "glava_b200_raster_textures: null argument");
     CU(cudaSetDevice(r->device));
+    int rc = frame_ready(r);
+    if (rc) return rc;
     const size_t row = (size_t) r->p.n * 2;
     CU(cudaStreamSynchronize(r->spec_stream));
     char* dst = (char*) tex_half(r, r->tex_cur);
@@ -1119,21 +1116,18 @@ int glava_b200_transform_smooth(glava_b200* r, float* planes, int count) {
     clear_error();
     if (!r || !planes || count < 1) return fail(GLAVA_B200_EINVAL, "glava_b200_transform_smooth: bad arguments");
     if (!r->p.transform_smooth) return fail(GLAVA_B200_EINVAL, "glava_b200_transform_smooth: the renderer was not created with transform_smooth");
+    if (!r->built) return unbuilt();
     CU(cudaSetDevice(r->device));
     const size_t bytes = (size_t) count * r->p.n * 4;
-    float* d = nullptr;
-    CU(cudaMalloc((void**) &d, bytes));
-    int rc = 0;
-    do {
-        if (cudaMemcpyAsync(d, planes, bytes, cudaMemcpyHostToDevice, r->stream) != cudaSuccess) { rc = fail(GLAVA_B200_ECUDA, "H2D copy failed"); break; }
-        if ((rc = launch_transform_smooth(d, r->p.n, r->d_ts_tab, r->ts_asz, r->ts_lim, count, r->stream)) != 0) break;
-        ++r->launches;
-        if (cudaMemcpyAsync(planes, d, bytes, cudaMemcpyDeviceToHost, r->stream) != cudaSuccess) { rc = fail(GLAVA_B200_ECUDA, "D2H copy failed"); break; }
-        cudaError_t se = cudaStreamSynchronize(r->stream);
-        if (se != cudaSuccess) rc = fail(GLAVA_B200_ECUDA, "transform_smooth: %s", cudaGetErrorString(se));
-    } while (0);
-    cudaFree(d);
-    return rc;
+    DevBuf<float> d;
+    int rc = d.alloc(bytes);
+    if (rc) return rc;
+    CU(cudaMemcpyAsync(d, planes, bytes, cudaMemcpyHostToDevice, r->stream));
+    if ((rc = launch_transform_smooth(d, r->p.n, r->tab.ts_tab, r->tab.ts_asz, r->tab.ts_lim, count, r->stream)) != 0) return rc;
+    ++r->launches;
+    CU(cudaMemcpyAsync(planes, d, bytes, cudaMemcpyDeviceToHost, r->stream));
+    CU(cudaStreamSynchronize(r->stream));
+    return 0;
 }
 
 }  // extern "C"
@@ -1199,19 +1193,17 @@ int state_check_blobs(const glava_b200* r, const void* const* blobs, int count, 
 
 // device staging, allocated on first use: halves of up to kStateStageBytes of segments plus the chunk table
 static int state_staging(glava_b200* r, const StateLayout& L) {
-    if (r->d_sst[0]) return 0;
+    if (r->ev_sst_free[1].get()) return 0;                   // created last: both halves are complete
     const size_t seg = ss_segment_bytes(L);
     size_t k = kStateStageBytes / seg;
     if (k < 1) k = 1;
     if (k > (size_t) r->batch) k = (size_t) r->batch;
     r->sst_streams = (int) k;
     r->sst_table = (k * 8 + 255) / 256 * 256;
-    for (int i = 0; i < 2; ++i) {
-        CU(cudaMalloc(&r->d_sst[i], r->sst_table + k * seg));
-        CU(cudaHostAlloc((void**) &r->h_sst[i], k * 8, cudaHostAllocDefault));
-        CU(cudaEventCreateWithFlags(&r->ev_sst_copied[i], cudaEventDisableTiming));
-        CU(cudaEventCreateWithFlags(&r->ev_sst_free[i], cudaEventDisableTiming));
-    }
+    int rc;
+    for (int i = 0; i < 2; ++i)
+        if ((rc = r->d_sst[i].alloc(r->sst_table + k * seg)) != 0 || (rc = r->h_sst[i].alloc(k * 8)) != 0 ||
+            (rc = r->ev_sst_copied[i].create()) != 0 || (rc = r->ev_sst_free[i].create()) != 0) return rc;
     return 0;
 }
 
@@ -1228,8 +1220,8 @@ static int state_io(glava_b200* r, int op, const int* streams, int count, void* 
     StatePtrs P;
     P.gravity = (char*) (r->p.accel_fft ? (void*) r->d_gr_store : (void*) r->d_applied);
     P.ring = (char*) (r->p.accel_fft ? (void*) r->d_ring_u : (void*) r->d_ring_f);
-    P.spec = (char*) r->d_spec; P.tex = (char*) tex_half(r, r->tex_cur); P.av = (char*) r->d_av;
-    P.fifo[0] = (char*) r->d_ring[r->ring_cur][0]; P.fifo[1] = (char*) r->d_ring[r->ring_cur][1];
+    P.spec = (char*) r->d_spec.get(); P.tex = (char*) tex_half(r, r->tex_cur); P.av = (char*) r->d_av.get();
+    P.fifo[0] = (char*) r->d_ring[r->ring_cur][0].get(); P.fifo[1] = (char*) r->d_ring[r->ring_cur][1].get();
     CU(cudaStreamWaitEvent(r->spec_stream, r->ev_raster_done[r->tex_cur], 0));
     const uint32_t F = (uint32_t) r->p.avg_frames;
     int last = -1;
@@ -1326,9 +1318,9 @@ size_t glava_b200_stream_state_bytes(const glava_b200_params* p) {
     clear_error();
     if (!p) { fail(GLAVA_B200_EINVAL, "glava_b200_stream_state_bytes: null argument"); return 0; }
     if (validate_params(p) != 0) return 0;
-    glava_b200 probe; probe.p_user = *p; derive(&probe);
-    if (probe.interp_on) { state_unavailable("glava_b200_stream_state_bytes"); return 0; }
-    return ss_blob_bytes(state_layout(probe.p, probe.n_in));
+    const Derived d = derive(*p);
+    if (d.interp_on) { state_unavailable("glava_b200_stream_state_bytes"); return 0; }
+    return ss_blob_bytes(state_layout(d.p, d.n_in));
 }
 
 int glava_b200_reset_streams(glava_b200* r, const uint8_t* mask) {

@@ -223,7 +223,9 @@ void glava_b200_destroy(glava_b200* r);
 
 /* Live parameter update — the analogue of a `--pipe` uniform write (render.c:1846-2005): colours, AMPLIFY,
  * gradient, smoothing parameters ... take effect from the next update.  Everything that sizes device state
- * (setbufsize, geometry, module, setaccelfft, setavgframes, fb_slots) must be unchanged. */
+ * (setbufsize, geometry, module, setaccelfft, setavgframes, fb_slots) must be unchanged.  Invalid parameters leave the
+ * renderer as it was.  If building the new tables fails (out of memory), the renderer keeps its previous parameters but
+ * has no tables: every update fails until a reconfigure or resize succeeds. */
 int  glava_b200_reconfigure(glava_b200* r, const glava_b200_params* params);
 int  glava_b200_get_params(const glava_b200* r, glava_b200_params* out);
 int  glava_b200_pipe_apply(glava_b200_pipe* p, glava_b200* r);   /* see glava_b200_pipe_new */
@@ -313,7 +315,10 @@ void* glava_b200_cuda_stream(const glava_b200* r);                              
 /* Offscreen hand-off — the analogues of glava_sizereq / glava_wait / glava_tex (glava.h:22-24, glava.c:244-267) for a
  * consumer (compositor, encoder) that takes frames straight from HBM:
  *   glava_b200_sizereq         thread-safe resize request, applied at the start of the next update (render.c:1811-1830);
- *                              spectrum state is kept, framebuffers and geometry tables are rebuilt
+ *                              spectrum state is kept, framebuffers and geometry tables are rebuilt.  An invalid
+ *                              geometry fails that update and changes nothing; one whose buffers cannot be allocated
+ *                              fails it, keeps the old parameters and leaves the renderer refusing updates until a
+ *                              reconfigure or resize succeeds
  *   glava_b200_wait_frame      host-blocks until the latest frame is complete (glava_wait)
  *   glava_b200_frame_event     cudaEvent_t recorded after the latest raster: cudaStreamWaitEvent(consumer, ev) orders a
  *                              consumer stream after the frame without a host round trip (glava_tex hands out the GL

@@ -1,0 +1,167 @@
+// fakecuda.cpp — TEST INFRASTRUCTURE: the CUDA runtime calls of capi.cu and the kernel launchers it calls, on the host.
+//
+// tests/fakecuda/__init__.py compiles capi.cu and config.cpp with g++ against this file.  Host memory stands in for device
+// and pinned memory; copies and kernels do nothing.  The runtime half counts the live buffers, pinned buffers, events and
+// streams, fails the k-th resource creation on request, and records every error for cudaGetLastError as the runtime does
+// (until read).  One device, 132 SMs, no PCI bus id.  The launcher half checks that every table the launch structure names
+// exists, and reports a pending runtime error as its launch failure, as the real launchers' post-launch check does.
+#include <cuda_runtime.h>
+
+#include "../../glava_b200/csrc/internal.h"
+#include "../../glava_b200/csrc/spectrum_plan.h"
+#include "../../glava_b200/csrc/raster_plan.h"
+
+#include <cstdlib>
+#include <set>
+#include <string>
+
+namespace {
+enum Kind { BUF, PINNED, EVENT, STREAM, KINDS };
+std::set<void*> g_live[KINDS];
+long g_creations = 0, g_fail_at = -1;
+cudaError_t g_last = cudaSuccess;
+long g_launches = 0, g_violations = 0, g_stale = 0, g_reached = 0;
+std::string g_violation;
+
+cudaError_t record(cudaError_t e) {
+    if (e != cudaSuccess) g_last = e;
+    return e;
+}
+cudaError_t create(Kind k, void** out, size_t bytes) {
+    *out = nullptr;
+    if (g_creations++ == g_fail_at) return record(k == BUF || k == PINNED ? cudaErrorMemoryAllocation : cudaErrorLaunchOutOfResources);
+    void* p = calloc(1, bytes ? bytes : 1);
+    g_live[k].insert(p);
+    *out = p;
+    return cudaSuccess;
+}
+cudaError_t destroy(Kind k, void* p, bool null_ok) {
+    if (!p && null_ok) return cudaSuccess;
+    if (!g_live[k].erase(p)) return record(cudaErrorInvalidValue);
+    free(p);
+    return cudaSuccess;
+}
+cudaError_t handle(Kind k, const void* p) { return g_live[k].count(const_cast<void*>(p)) ? cudaSuccess : record(cudaErrorInvalidResourceHandle); }
+cudaError_t stream_ok(cudaStream_t s) { return s ? handle(STREAM, s) : cudaSuccess; }
+
+// which tables the launches have used, for the test to check that a configuration reaches what it is meant to
+enum Reached { R_NEED = 1, R_TAPS = 2, R_FULL = 4, R_NEED_SMEM = 8, R_NEED_L2 = 16, R_GEO = 32, R_CTILE = 64, R_COLTAB = 128,
+               R_TSMOOTH = 256 };
+
+int launched(const char* what, bool tables_ok, long reached = 0) {
+    ++g_launches;
+    g_reached |= reached;
+    if (!tables_ok) {
+        if (!g_violations) g_violation = what;
+        ++g_violations;
+    }
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) {
+        ++g_stale;
+        return glb::fail(GLAVA_B200_ECUDA, "%s launch: %s", what, cudaGetErrorString(e));
+    }
+    return 0;
+}
+}  // namespace
+
+// ---- the runtime -------------------------------------------------------------------------------------------------------
+extern "C" {
+const char* cudaGetErrorString(cudaError_t e) { return e == cudaSuccess ? "no error" : e == cudaErrorMemoryAllocation ? "out of memory" : "fake error"; }
+cudaError_t cudaGetLastError(void) { const cudaError_t e = g_last; g_last = cudaSuccess; return e; }
+cudaError_t cudaGetDeviceCount(int* count) { *count = 1; return cudaSuccess; }
+cudaError_t cudaGetDevice(int* device) { *device = 0; return cudaSuccess; }
+cudaError_t cudaSetDevice(int device) { return device == 0 ? cudaSuccess : record(cudaErrorInvalidDevice); }
+cudaError_t cudaDeviceGetAttribute(int* value, enum cudaDeviceAttr attr, int) {
+    *value = attr == cudaDevAttrMultiProcessorCount ? 132 : 0;
+    return cudaSuccess;
+}
+cudaError_t cudaGetDeviceProperties(struct cudaDeviceProp* prop, int) { *prop = cudaDeviceProp(); prop->multiProcessorCount = 132; return cudaSuccess; }
+cudaError_t cudaDeviceGetPCIBusId(char*, int, int) { return record(cudaErrorNotSupported); }
+cudaError_t cudaDeviceGetStreamPriorityRange(int* least, int* greatest) { *least = 0; *greatest = -5; return cudaSuccess; }
+cudaError_t cudaDeviceSetLimit(enum cudaLimit, size_t) { return cudaSuccess; }
+
+cudaError_t cudaMalloc(void** p, size_t bytes) { return create(BUF, p, bytes); }
+cudaError_t cudaFree(void* p) { return destroy(BUF, p, true); }
+cudaError_t cudaHostAlloc(void** p, size_t bytes, unsigned int) { return create(PINNED, p, bytes); }
+cudaError_t cudaFreeHost(void* p) { return destroy(PINNED, p, true); }
+cudaError_t cudaHostRegister(void*, size_t, unsigned int) { return record(cudaErrorNotSupported); }
+cudaError_t cudaHostUnregister(void*) { return record(cudaErrorNotSupported); }
+cudaError_t cudaEventCreateWithFlags(cudaEvent_t* e, unsigned int) { return create(EVENT, (void**) e, 1); }
+cudaError_t cudaEventCreate(cudaEvent_t* e) { return create(EVENT, (void**) e, 1); }
+cudaError_t cudaEventDestroy(cudaEvent_t e) { return destroy(EVENT, e, false); }
+cudaError_t cudaStreamCreateWithFlags(cudaStream_t* s, unsigned int) { return create(STREAM, (void**) s, 1); }
+cudaError_t cudaStreamCreateWithPriority(cudaStream_t* s, unsigned int, int) { return create(STREAM, (void**) s, 1); }
+cudaError_t cudaStreamDestroy(cudaStream_t s) { return destroy(STREAM, s, false); }
+
+cudaError_t cudaEventRecord(cudaEvent_t e, cudaStream_t s) { cudaError_t r = handle(EVENT, e); return r ? r : stream_ok(s); }
+cudaError_t cudaEventSynchronize(cudaEvent_t e) { return handle(EVENT, e); }
+cudaError_t cudaEventElapsedTime(float* ms, cudaEvent_t a, cudaEvent_t b) {
+    *ms = 0.0f;
+    cudaError_t r = handle(EVENT, a);
+    return r ? r : handle(EVENT, b);
+}
+cudaError_t cudaStreamWaitEvent(cudaStream_t s, cudaEvent_t e, unsigned int) { cudaError_t r = handle(EVENT, e); return r ? r : stream_ok(s); }
+cudaError_t cudaStreamSynchronize(cudaStream_t s) { return stream_ok(s); }
+cudaError_t cudaStreamSetAttribute(cudaStream_t s, cudaStreamAttrID, const cudaStreamAttrValue*) { return stream_ok(s); }
+cudaError_t cudaMemsetAsync(void* p, int, size_t, cudaStream_t s) { return p ? stream_ok(s) : record(cudaErrorInvalidValue); }
+cudaError_t cudaMemcpyAsync(void* d, const void* src, size_t, enum cudaMemcpyKind, cudaStream_t s) {
+    return d && src ? stream_ok(s) : record(cudaErrorInvalidValue);
+}
+cudaError_t cudaMemcpy2DAsync(void* d, size_t, const void* src, size_t, size_t, size_t, enum cudaMemcpyKind, cudaStream_t s) {
+    return d && src ? stream_ok(s) : record(cudaErrorInvalidValue);
+}
+cudaError_t cudaIpcGetMemHandle(cudaIpcMemHandle_t* h, void* p) { *h = cudaIpcMemHandle_t(); return handle(BUF, p); }
+
+// ---- the test's controls -----------------------------------------------------------------------------------------------
+// fail the k-th resource creation from now on (k < 0: none); counting restarts
+void fake_fail_at(long k) { g_fail_at = k; g_creations = 0; }
+long fake_creations(void) { return g_creations; }
+long fake_live(int kind) { return (long) g_live[kind].size(); }
+long fake_launches(void) { return g_launches; }
+long fake_violations(void) { return g_violations; }
+const char* fake_first_violation(void) { return g_violation.c_str(); }
+long fake_stale(void) { return g_stale; }
+long fake_reached(void) { return g_reached; }
+void fake_clear(void) { g_launches = g_violations = g_stale = g_reached = 0; g_violation.clear(); g_last = cudaSuccess; }
+}  // extern "C"
+
+// ---- the launchers capi.cu calls ---------------------------------------------------------------------------------------
+namespace glb {
+int launch_spectrum_update(const glava_b200_params&, const SpectrumPlan& pl, const SpectrumDevTables& t, const SpectrumArgs& a, void*) {
+    const bool ok = (!pl.need_list || t.need) && (!pl.tap_table || (t.tap_tab && t.csr)) &&
+                    (pl.k5 != K5Form::NEED_SMEM || t.need_blk) && (pl.k5 != K5Form::NEED_L2 || t.av_t) &&
+                    (!pl.full_table || t.k5.blk) && a.spec && a.tex;
+    const long reached = (pl.need_list ? R_NEED : 0) | (pl.tap_table ? R_TAPS : 0) | (pl.full_table ? R_FULL : 0) |
+                         (pl.k5 == K5Form::NEED_SMEM ? R_NEED_SMEM : 0) | (pl.k5 == K5Form::NEED_L2 ? R_NEED_L2 : 0);
+    const int rc = launched("spectrum update", ok, reached);
+    return rc ? rc : 1;
+}
+int launch_k5_full(const glava_b200_params&, const SpectrumPlan& pl, const K5Table& t, const uint16_t* in, uint16_t* out, int, void*) {
+    return launched("whole-plane K5", (!pl.full_table || t.blk) && in && out);
+}
+int launch_raster(const glava_b200_params&, const RasterPlan& pl, const RasterArgs& a, void*) {
+    const bool ok = (!pl.geo || a.geo) && (!pl.ctile || (a.ctile && a.ctile_zero)) && (!pl.coltab || a.coltab) &&
+                    (!pl.rowtab || a.rowtab) && a.fb && a.marks && a.tex;
+    return launched("raster", ok, (pl.geo ? R_GEO : 0) | (pl.ctile ? R_CTILE : 0) | (pl.coltab ? R_COLTAB : 0));
+}
+int launch_bars_rowtab(const glava_b200_params&, void* d_rowtab, void*) { return launched("row table", d_rowtab != nullptr); }
+int launch_texmm(const glava_b200_params&, const uint16_t* tex, uint32_t* out, int, void*) { return launched("texmm", tex && out); }
+int launch_polar_geo(const glava_b200_params&, void* d_geo, const int*, void*) { return launched("polar geometry", d_geo != nullptr); }
+size_t circle_tile_bytes(const glava_b200_params& p, int* ntx, int* nty) {
+    *ntx = (p.w + 127) / 128; *nty = (p.h + 7) / 8;
+    return (size_t) *ntx * *nty * (sizeof(int4) + sizeof(int));
+}
+int launch_circle_tiles(const glava_b200_params&, const void* d_geo, const int*, void* d_tiles, void*) {
+    return launched("circle tiles", d_geo && d_tiles);
+}
+int launch_fifo_ingest(const glava_b200_params&, const void* chunks, bool, int, const float* sl, const float* sr, float* dl, float* dr, int, void*) {
+    return launched("fifo ingest", chunks && sl && sr && dl && dr);
+}
+int launch_bufscale(const float* il, const float*, float* ol, float* orr, int, int, int, int, void*) { return launched("bufscale", il && ol && orr); }
+int launch_transform_smooth(float* planes, int, const void* tab, int, int, int, void*, const uint32_t*, int) {
+    return launched("transform_smooth", planes && tab, R_TSMOOTH);
+}
+int launch_upload(const float* s, const float*, float, uint16_t* out, size_t, void*) { return launched("upload", s && out); }
+int launch_state_pack(const StateLayout&, const StatePtrs&, const int* table, int, void* out, void*) { return launched("state pack", table && out); }
+int launch_state_unpack(const StateLayout&, const StatePtrs&, const int* table, int, const void*, void*) { return launched("state unpack", table != nullptr); }
+}  // namespace glb
