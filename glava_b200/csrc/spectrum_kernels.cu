@@ -76,6 +76,18 @@ template <int LOG2N, int TT = 0, bool OOP = false> struct SpecCfg {
     static constexpr int SMEM    = OOP ? 2 * BUF_BYTES + 16 : spectrum_smem_bytes(N);
     static constexpr int OFF_BAR = SMEM - 16;
     static constexpr bool RESULT_IN_B = OOP && (fft_pass_count(M) % 2 == 1);
+    // Twiddle table (M complex floats) in shared memory, behind the mbarriers, landed by the TMA engine with the CTA's first
+    // PCM load: in place up to N = 4096 (16 KB there), where it fits beside the buffers at the size's residency and a
+    // thread's first pass is one butterfly (its window factors are prefetched before the PCM wait).  At 8192 (out of place,
+    // 3 CTAs/SM by shared memory) the table would cost a resident CTA, at 16384 a thread holds two first-pass butterflies:
+    // there the passes read the table through L1.
+    static constexpr bool TW_SMEM  = !OOP && N <= 4096;
+    static constexpr int  TW_BYTES = TW_SMEM ? M * 8 : 0;
+    static constexpr int  OFF_TW   = SMEM;
+    // fixed dynamic shared memory of the FFT (twiddles) or wave kernel; the K5 tap table follows it
+    static constexpr int  dyn_bytes(bool is_fft) { return SMEM + (is_fft ? TW_BYTES : 0); }
+    static constexpr int  R0 = M >= 8 ? 8 : M, NB0 = M / R0;   // first pass: radix, butterflies (fft_core.h, NS = 1)
+    static_assert(!TW_SMEM || NB0 <= T, "shared-memory twiddle form: one first-pass butterfly per thread");
     // resident CTAs per SM the register allocation must allow: the kernel waits on memory a lot (TMA load,
     // state loads), so occupancy is worth more than the last registers (128 regs -> 2 CTAs/SM was measured)
     static constexpr int SMEM_CTAS = (220 * 1024) / SMEM < 1 ? 1 : (220 * 1024) / SMEM;
@@ -132,23 +144,27 @@ spectrum_kernel(const __grid_constant__ SpectrumArgs a, const __grid_constant__ 
     float*    raw = reinterpret_cast<float*>(glb_smem);
     uint16_t* av  = OOP ? reinterpret_cast<uint16_t*>((IS_FFT && C::RESULT_IN_B) ? bufA : bufB) : reinterpret_cast<uint16_t*>(glb_smem + C::OFF_AV);
     uint64_t* bar = reinterpret_cast<uint64_t*>(glb_smem + C::OFF_BAR);
+    cpx*      twsm = reinterpret_cast<cpx*>(glb_smem + C::OFF_TW);
+    const cpx* const tw = C::TW_SMEM ? twsm : reinterpret_cast<const cpx*>(a.twiddle);
 
     // Persistent CTAs: work unit u = one (stream, channel) plane (wave: one stream, audio_l only,
     // wave/1.frag:7); a CTA walks u = blockIdx.x, + gridDim.x, ...  The PCM ring of the NEXT unit is
     // prefetched by the TMA engine while this unit's smoothing pass runs.
     const int units = IS_FFT ? a.batch * 2 : a.batch;
-    auto issue_load = [&](int u) {                   // one bulk async copy, N*4 bytes, completes on `bar`
+    // one bulk async copy, N*4 bytes, completes on `bar`; the CTA's first one also lands the twiddle table
+    auto issue_load = [&](int u, bool with_tw = false) {
         const int cc = IS_FFT ? u : 2 * u;
         const float* pcm = ((cc & 1) == 0 ? a.pcm_l : a.pcm_r) + (size_t) (cc >> 1) * N;
         // the buffer was last touched through the generic proxy (FFT passes): order those accesses
         // before the async-proxy (TMA) write
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        mbar_expect_tx(bar, N * 4);
+        mbar_expect_tx(bar, N * 4 + (with_tw ? C::TW_BYTES : 0));
         bulk_g2s(raw, pcm, N * 4, bar);
+        if (with_tw) bulk_g2s(twsm, a.twiddle, C::TW_BYTES, bar);
     };
     // K5 tap table of this CTA's channel in shared memory (behind the fixed regions): one more bulk copy, in flight
     // during the FFT and the epilogue
-    unsigned char* tapsm = glb_smem + C::SMEM;
+    unsigned char* tapsm = glb_smem + C::dyn_bytes(IS_FFT);
     uint64_t* bar2 = bar + 1;
     auto issue_tab = [&](int ch) {
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -159,7 +175,7 @@ spectrum_kernel(const __grid_constant__ SpectrumArgs a, const __grid_constant__ 
     };
     if (tid == 0) { mbar_init(bar, 1); mbar_init(bar2, 1); }
     __syncthreads();
-    if (tid == 0 && (int) blockIdx.x < units) issue_load(blockIdx.x);
+    if (tid == 0 && (int) blockIdx.x < units) issue_load(blockIdx.x, IS_FFT && C::TW_SMEM);
     int tab_ch = -1; bool tab_pending = false; uint32_t parity2 = 0;
     if (a.csr && a.need && (int) blockIdx.x < units && !a.skip_tex && p.smooth_pass) {
         tab_ch = IS_FFT ? ((int) blockIdx.x & 1) : 0;
@@ -187,15 +203,29 @@ spectrum_kernel(const __grid_constant__ SpectrumArgs a, const __grid_constant__ 
         if (tid == 0 && u + (int) gridDim.x < units) issue_load(u + gridDim.x);
         continue;
     }
-    if (IS_FFT && p.accel_fft) {
-        // while the PCM load is in flight: pull this plane's gravity / average state (1 + F planes of
-        // u16, HBM-resident) towards L2, so the epilogue's loads after the FFT are L2 hits
+    if (IS_FFT && p.accel_fft && !a.fft_only) {
+        // while the PCM load is in flight: pull the R16 state the pipeline-B epilogue below reads (HBM-resident) towards L2,
+        // so its loads after the FFT are L2 hits: the leading bins it runs over of the gravity plane (s = 0) and of the F - 1
+        // ring slots it averages (s = 1 .. F-1: slot cursor - s).  Not the slot it overwrites, nothing past its bins.  (The
+        // FFT-only form reads no state: epilogue_b_kernel does, after the whole grid.)
+        // (the epilogue rounds epi_n up to a multiple of T: those last few bins are not prefetched)
+        const int lines = (a.epi_n > 0 && a.epi_n < N) ? (a.epi_n * 2 + 127) / 128 : (N * 2) / 128;
         const char* g0 = reinterpret_cast<const char*>(a.gr_store + plane);
         const char* r0 = reinterpret_cast<const char*>(a.ring_u + plane * F);
-        const int lines_g = (N * 2) / 128, lines_r = (N * 2 * F) / 128;   // (whole planes: cheap, and epi_n varies)
-        for (int i = tid; i < lines_g + lines_r; i += T) {
-            const char* ptr = i < lines_g ? g0 + (size_t) i * 128 : r0 + (size_t) (i - lines_g) * 128;
-            asm volatile("prefetch.global.L2 [%0];" ::"l"(ptr));
+        for (int s = 0; s < F; ++s) {
+            int fr = cursor - s; if (fr < 0) fr += F;
+            const char* src = s == 0 ? g0 : r0 + (size_t) fr * N * 2;
+            for (int l = tid; l < lines; l += T) asm volatile("prefetch.global.L2 [%0];" ::"l"(src + (size_t) l * 128));
+        }
+    }
+    if constexpr (IS_FFT && C::TW_SMEM) {
+        // the window factors of this thread's first-pass butterfly (j = tid: points tid + t * NB0) towards L1 before the
+        // wait, so that their L2 latency overlaps the TMA.  (Held in registers instead, 32 of them, they spill under the
+        // 3-CTA register cap at 4096.)
+        if (tid < C::NB0) {
+#pragma unroll
+            for (int t = 0; t < C::R0; ++t)
+                asm volatile("prefetch.global.L1 [%0];" ::"l"(reinterpret_cast<const double2*>(a.window) + tid + t * C::NB0));
         }
     }
     mbar_wait(bar, parity); parity ^= 1u;
@@ -209,8 +239,8 @@ spectrum_kernel(const __grid_constant__ SpectrumArgs a, const __grid_constant__ 
             cpx r = { (float) ((double) v.x * w.x), (float) ((double) v.y * w.y) };
             return r;
         };
-        if constexpr (OOP) run_passes_oop<M, T, 1>(bufA, bufB, first, reinterpret_cast<const cpx*>(a.twiddle), tid);
-        else run_passes<M, T, 1>(buf, first, reinterpret_cast<const cpx*>(a.twiddle), tid);
+        if constexpr (OOP) run_passes_oop<M, T, 1>(bufA, bufB, first, tw, tid);
+        else run_passes<M, T, 1>(buf, first, tw, tid);
 
         if (a.fft_only) {
             // transform_fft's tail only (render.c:842-846); the state update and K5 follow as full-occupancy kernels
@@ -466,7 +496,7 @@ static int launch_spectrum_t(const glava_b200_params& p, const SpectrumArgs& a, 
     // at full occupancy (5 CTAs x 256 threads x 48 registers per SM) takes most of the register file.
     // Requesting more dynamic shared memory than needed caps it at `resident` CTAs per SM; off, because the
     // stretched spectrum kernel (and the L1 it takes from the raster kernel) costs more than it frees.
-    int smem_req = C::SMEM + (a.csr ? a.csr_bytes : 0);          // + the K5 tap table of one channel (shared-memory K5 path)
+    int smem_req = C::dyn_bytes(IS_FFT) + (a.csr ? a.csr_bytes : 0);   // + the K5 tap table of one channel (shared-memory K5 path)
     if (resident > 0) { int want = (227 * 1024) / resident - 1024; if (want > smem_req) smem_req = want; }
     if (smem_req > 227 * 1024) smem_req = 227 * 1024;
     if (smem_req > 48 * 1024) {
@@ -655,10 +685,11 @@ int launch_k5_full(const glava_b200_params& p, const SpectrumPlan& pl, const K5T
 // Arithmetic = the in-kernel epilogue's (gravity_b, newest-first weighted average), bit for bit.
 template <int FT>
 __global__ void __launch_bounds__(128)
-epilogue_b_kernel(const __grid_constant__ SpectrumArgs a, int n, int bins, int F, float diff, int y0) {
-    const int plane = y0 + (int) blockIdx.y, g8 = blockIdx.x * blockDim.x + threadIdx.x;
-    const int n0 = g8 * 8;
-    if (n0 >= bins) return;
+epilogue_b_kernel(const __grid_constant__ SpectrumArgs a, int n, int bins, int F, float diff, int y0, int rows) {
+    // flat index over (plane of this slice, group of 8 bins): only the last CTA of a slice has idle threads
+    const int groups = bins / 8, idx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= rows * groups) return;
+    const int pr = idx / groups, plane = y0 + pr, n0 = (idx - pr * groups) * 8;
     const uint32_t um = a.umask ? __ldg(a.umask + (plane >> 1)) : 0x80000000u;
     if (!(um >> 31)) return;                                   // stream without new audio: state and texels stay
     const int out_idx = a.umask ? (int) (um & 0xffffu) : (int) (a.update % (unsigned long long) F);
@@ -710,9 +741,10 @@ epilogue_b_kernel(const __grid_constant__ SpectrumArgs a, int n, int bins, int F
 static int launch_epilogue_b(const glava_b200_params& p, const SpectrumPlan& pl, const SpectrumArgs& a, cudaStream_t st) {
     const int planes = a.batch * 2, F = p.avg_frames, bins = pl.epi_n;
     const float diff = p.gravity_step * (1.0f / p.ur);
-    const unsigned gx = (bins / 8 + 127) / 128;
+    // slices of at most GRID_Y_MAX planes keep the flat index in int (65535 planes x 2048 groups at 16384)
     cudaError_t e = launch_y_slices(planes, [&](int y0, unsigned rows) {
-#define GLB_EPI(FT) epilogue_b_kernel<FT><<<dim3(gx, rows), 128, 0, st>>>(a, p.n, bins, F, diff, y0)
+        const unsigned gx = (unsigned) (((long long) rows * (bins / 8) + 127) / 128);
+#define GLB_EPI(FT) epilogue_b_kernel<FT><<<gx, 128, 0, st>>>(a, p.n, bins, F, diff, y0, (int) rows)
         switch (F) {
             case 5: GLB_EPI(5); break;                          // shipped default (smooth_parameters.glsl:56)
             case 6: GLB_EPI(6); break;                          // compiled-in default (render.c:912)
