@@ -81,17 +81,20 @@ struct FrameBuffers {
     DevBuf<uint32_t> marks;     // dirty-row marks of the framebuffer slots (RasterArgs::marks)
 };
 
-// The effective parameters and mode flags of a parameter set
+// A parameter set as given, its effective parameters and mode flags, and the transform_average weights of every update
 struct Derived {
+    glava_b200_params user;     // as given (glava_b200_get_params)
     glava_b200_params p;        // n = setbufsize / setbufscale, accel_fft cleared when a transform follows "fft" (render.c:2143-2154)
     int n_in;                   // setbufsize: floats per channel the caller hands to glava_b200_update
     bool interp_on;             // keyframe interpolation active (render.c:1761-1763, 2161-2168)
     bool post_chain;            // transform_smooth and / or keyframe lerp: the spectrum kernel stops at the float chain
                                 // result; upload + K5 run as separate kernels
+    SpectrumArgs spec_args;     // what every update's SpectrumArgs starts from: the transform_average weights, all else 0
 };
 
 static Derived derive(const glava_b200_params& user) {
-    Derived d;
+    Derived d{};
+    d.user = user;
     d.p = user;
     d.n_in = user.n;
     d.p.n = user.n / user.bufscale;
@@ -100,16 +103,20 @@ static Derived derive(const glava_b200_params& user) {
     const float fr = d.p.fr > 0.0f ? d.p.fr : d.p.ur;
     d.interp_on = d.p.interpolate && !(d.p.accel_fft && is_fft) && (d.p.ur / fr) <= 0.9f;
     d.post_chain = d.p.transform_smooth == 1 || d.interp_on;
+    const int F = d.p.avg_frames;
+    for (int f = 0; f < F; ++f) {
+        // pipeline A: window_frame(f, avg_frames - 1) -> cos(TWOPI*f/F - 1), double (render.c:661,766)
+        d.spec_args.avg_w_a[f] = 0.6 - (0.4 * cos(6.28318530718 * (double) f / (double) F - 1));
+        // pipeline B: window(I, _AVG_FRAMES - 1) -> cos(TWOPI*I/F - 1), GLSL float (average_pass.frag:41)
+        d.spec_args.avg_w_b[f] = 0.53836f - (0.46164f * cosf(6.28318530718f * (float) f / (float) F - 1.0f));
+    }
+    d.spec_args.avg_b_windowed = (d.p.avg_window && F != 2) ? 1 : 0;
     return d;
 }
 
 // Every member that holds a CUDA resource owns it; glava_b200_destroy synchronises the streams before the destructors run.
 struct glava_b200 {
-    glava_b200_params p;        // EFFECTIVE parameters the kernels run with (Derived::p)
-    glava_b200_params p_user;   // as given at the last successful build (glava_b200_get_params)
-    int n_in = 0;
-    bool post_chain = false;
-    bool interp_on = false;
+    Derived d;                  // the parameters of the last successful build (rebuild); the kernels run with d.p
     int  kcounter = 0;          // frames since the last modified update (render.c:2380-2383)
     DevBuf<float> d_scaled[2];  // bufscale output [batch][n] x {l, r}
     DevBuf<float> d_key[3]; int key_start = 0, key_end = 1;   // keyframe buffers [batch*2][n] (start, end, the one being written)
@@ -428,7 +435,7 @@ static int rebuild(glava_b200* r, const glava_b200_params& q) {
     if (rc) return rc;
     const Derived d = derive(q);
     if ((rc = sync_all(r)) != 0) return rc;
-    const bool new_frame = !r->built || !r->frame.fb.get() || q.w != r->p_user.w || q.h != r->p_user.h;
+    const bool new_frame = !r->built || !r->frame.fb.get() || q.w != r->d.user.w || q.h != r->d.user.h;
     r->built = false;
     r->tab = ConfigTables();
     if (new_frame) r->frame = FrameBuffers();
@@ -436,16 +443,16 @@ static int rebuild(glava_b200* r, const glava_b200_params& q) {
     ConfigTables tb;
     if (new_frame && (rc = alloc_frame_buffers(r, d.p, f)) != 0) return rc;
     if ((rc = build_tables(r, d, tb)) != 0) return rc;
-    r->p_user = q; r->p = d.p; r->n_in = d.n_in; r->interp_on = d.interp_on; r->post_chain = d.post_chain;
+    r->d = d;
     r->tab = std::move(tb);
     if (new_frame) { r->frame = std::move(f); r->mark_key = 0; }
     r->built = true;
     return 0;
 }
 
-// The per-stream state, inputs and constants, sized by parameters that never change on a live renderer
-static int build_state(glava_b200* r) {
-    const glava_b200_params& p = r->p;
+// The per-stream state, inputs and constants for the parameters of `d`, sized by parameters that never change on a live renderer
+static int build_state(glava_b200* r, const Derived& d) {
+    const glava_b200_params& p = d.p;
     const size_t n = (size_t) p.n, planes = (size_t) r->batch * 2, F = (size_t) p.avg_frames;
     CU(cudaSetDevice(r->device));
     int rc;
@@ -470,14 +477,14 @@ static int build_state(glava_b200* r) {
     cudaStream_t st = r->stream;
 #define ALLOC(buf, bytes) if ((rc = alloc_zeroed((buf), (bytes), st)) != 0) return rc
     if ((rc = r->copy_stream.create(0)) != 0) return rc;
-    const size_t n_in = (size_t) r->n_in;
+    const size_t n_in = (size_t) d.n_in;
     for (int i = 0; i < 2; ++i) {
         ALLOC(r->d_pcm[i][0], (size_t) r->batch * n_in * 4); ALLOC(r->d_pcm[i][1], (size_t) r->batch * n_in * 4);
         if ((rc = r->ev_copied[i].create()) != 0 || (rc = r->ev_free[i].create()) != 0) return rc;
     }
     for (int i = 0; i < 2; ++i) for (int c = 0; c < 2; ++c) ALLOC(r->d_ring[i][c], (size_t) r->batch * n_in * 4);
-    if (r->p_user.bufscale > 1 || r->p_user.transform_smooth == 2) { ALLOC(r->d_scaled[0], (size_t) r->batch * n * 4); ALLOC(r->d_scaled[1], (size_t) r->batch * n * 4); }
-    if (r->interp_on) {
+    if (d.user.bufscale > 1 || d.user.transform_smooth == 2) { ALLOC(r->d_scaled[0], (size_t) r->batch * n * 4); ALLOC(r->d_scaled[1], (size_t) r->batch * n * 4); }
+    if (d.interp_on) {
         for (int i = 0; i < 3; ++i) ALLOC(r->d_key[i], planes * n * 4);      // keyframes start at 0 (render.c:1681 calloc)
         r->key_start = 0; r->key_end = 1;
     }
@@ -549,9 +556,7 @@ glava_b200* glava_b200_new(const glava_b200_params* params, int batch, int devic
     if (device < 0 || device >= ndev) { fail(GLAVA_B200_EINVAL, "device %d out of range (%d devices)", device, ndev); return nullptr; }
     glava_b200* r = new glava_b200();
     r->batch = batch; r->device = device;
-    const Derived d = derive(*params);
-    r->p_user = *params; r->p = d.p; r->n_in = d.n_in; r->interp_on = d.interp_on; r->post_chain = d.post_chain;
-    if (build_state(r) != 0 || rebuild(r, *params) != 0) { glava_b200_destroy(r); return nullptr; }
+    if (build_state(r, derive(*params)) != 0 || rebuild(r, *params) != 0) { glava_b200_destroy(r); return nullptr; }
     return r;
 }
 
@@ -568,10 +573,10 @@ int glava_b200_reconfigure(glava_b200* r, const glava_b200_params* params) {
     if (!r || !params) return fail(GLAVA_B200_EINVAL, "glava_b200_reconfigure: null argument");
     int rc = validate_params(params);
     if (rc) return rc;
-    const glava_b200_params& o = r->p_user;
+    const glava_b200_params& o = r->d.user;
     if (params->n != o.n || params->w != o.w || params->h != o.h || params->module != o.module || params->accel_fft != o.accel_fft ||
         params->avg_frames != o.avg_frames || params->fb_slots != o.fb_slots || params->bufscale != o.bufscale ||
-        params->transform_smooth != o.transform_smooth || derive(*params).interp_on != r->interp_on)
+        params->transform_smooth != o.transform_smooth || derive(*params).interp_on != r->d.interp_on)
         return fail(GLAVA_B200_EINVAL, "glava_b200_reconfigure: setbufsize, setbufscale, geometry, module, setaccelfft, setavgframes, "
                                        "fb_slots, the \"smooth\" transform and whether interpolation is active size the device "
                                        "state and cannot change on a live renderer; create a new one");
@@ -581,11 +586,11 @@ int glava_b200_reconfigure(glava_b200* r, const glava_b200_params* params) {
 
 int glava_b200_get_params(const glava_b200* r, glava_b200_params* out) {
     if (!r || !out) return fail(GLAVA_B200_EINVAL, "null argument");
-    *out = r->p_user; return 0;
+    *out = r->d.user; return 0;
 }
 int glava_b200_batch(const glava_b200* r) { return r ? r->batch : 0; }
-const char* glava_b200_module_name(const glava_b200* r) { return r ? module_name(r->p.module) : "?"; }
-int glava_b200_spectrum_size(const glava_b200* r) { return r ? r->p.n : 0; }
+const char* glava_b200_module_name(const glava_b200* r) { return r ? module_name(r->d.p.module) : "?"; }
+int glava_b200_spectrum_size(const glava_b200* r) { return r ? r->d.p.n : 0; }
 const void* glava_b200_framebuffer_device(const glava_b200* r) { return r ? r->frame.fb.get() : nullptr; }
 void* glava_b200_cuda_stream(const glava_b200* r) { return r ? (void*) r->stream : nullptr; }
 uint64_t glava_b200_launch_count(const glava_b200* r) { return r ? r->launches : 0; }
@@ -599,7 +604,7 @@ static int timing_mark(std::vector<Event>& v, cudaStream_t st) {
     return 0;
 }
 
-static uint16_t* tex_half(glava_b200* r, int b) { return r->d_tex + (size_t) b * r->batch * 2 * r->p.n; }
+static uint16_t* tex_half(glava_b200* r, int b) { return r->d_tex + (size_t) b * r->batch * 2 * r->d.p.n; }
 // Runtime resize (render.c:1811-1830 resizes the stage FBOs when the framebuffer size changed; offscreen consumers ask
 // through glava_sizereq, glava.c:263-267), applied at the start of a frame (render.c:1811-1815).  Spectrum state is
 // untouched; the framebuffers and every table (row colours, polar geometry cache, lazy-K5 need-list) are rebuilt.  Then a
@@ -609,7 +614,7 @@ static int unbuilt() {
 }
 static int frame_ready(glava_b200* r) {
     if (unsigned long long req = r->sizereq.exchange(0)) {
-        glava_b200_params q = r->p_user;
+        glava_b200_params q = r->d.user;
         q.w = (int) ((req >> 32) & 0x7fffffffu); q.h = (int) (req & 0xffffffffu);
         int rc = rebuild(r, q);
         if (rc) return rc;
@@ -617,15 +622,9 @@ static int frame_ready(glava_b200* r) {
     return r->built ? 0 : unbuilt();
 }
 
-// One update = spectrum kernel on spec_stream (if modified) + raster kernel on stream.
-//   spectrum(i) waits for: its input (caller-provided event on spec_stream), spectrum(i-1) (same stream:
-//                          gravity / average state is read-modify-write), raster(i-2) (last reader of the
-//                          texture half it overwrites)
-//   raster(i)   waits for: spectrum(i)
-// so raster(i) and spectrum(i+1) run concurrently: one is HBM-store bound, the other latency bound.
 // Per-stream mask -> device words.  Returns the device array for this update (nullptr: every stream modified in lock step).
 static int stage_umask(glava_b200* r, const uint8_t* mask, const uint32_t** d_out) {
-    const int F = r->p.avg_frames;
+    const int F = r->d.p.avg_frames;
     if (!r->desync) {                                           // first uneven update: every stream starts from the shared cursor
         r->cursor.assign((size_t) r->batch, (uint32_t) (r->updates % (unsigned long long) F));
         r->desync = true;
@@ -650,31 +649,61 @@ static int stage_umask(glava_b200* r, const uint8_t* mask, const uint32_t** d_ou
     return 0;
 }
 
-// `mask` (may be null): one byte per stream, non-zero = that stream has new audio (glava.c:528-537 per renderer).
-static int run_update(glava_b200* r, const float* d_l, const float* d_r, int modified, bool raster_only = false,
-                      const uint8_t* mask = nullptr) {
+// One update's input, as a public entry point received it
+struct UpdateInput {
+    enum Source { HOST, DEVICE, RINGS, TEXTURES } src;
+    const char* who;                  // the public function, for error messages
+    const void* l = nullptr, *r = nullptr;   // HOST / DEVICE: PCM [batch][bsz]; TEXTURES: R16 [batch][n]; r may be null
+    size_t bsz = 0;                   // HOST / DEVICE: floats per stream and channel
+    bool modified = false;            // every stream has new audio
+    const uint8_t* mask = nullptr;    // or: one byte per stream, non-zero = that stream has new audio (glava.c:528-537 per renderer)
+    void* ready = nullptr;            // DEVICE: a cudaEvent_t the PCM is written behind (glava_b200_update_device_after), or null
+};
+
+// Everything an update checks before it enqueues anything, in this order.  A mask leaves here normalised: `modified` says
+// whether any stream has new audio, and a mask that marks none or all of them gives way to the plain form.
+static int check_update(glava_b200* r, UpdateInput& in) {
+    const bool pcm = in.src == UpdateInput::HOST || in.src == UpdateInput::DEVICE;
+    if (pcm && in.bsz != (size_t) r->d.n_in) return fail(GLAVA_B200_EINVAL, "%s: bsz %zu != setbufsize %d", in.who, in.bsz, r->d.n_in);
+    if (in.src == UpdateInput::DEVICE && (((uintptr_t) in.l & 15) || ((uintptr_t) in.r & 15)))
+        return fail(GLAVA_B200_EINVAL, "device PCM pointers must be 16-byte aligned");
+    int cnt = 0;
+    for (int s = 0; in.mask && s < r->batch; ++s) cnt += in.mask[s] ? 1 : 0;
+    if (in.mask) in.modified = cnt > 0;
+    // rd_update always gets both rings (render.h:58); only `wave` ignores rb (wave/1.frag:7 samples audio_l alone).  A masked
+    // update from device pointers asks for d_rb whatever its mask.
+    if (pcm && !in.r && r->d.p.module != GLAVA_B200_MOD_WAVE && (in.modified || (in.mask && in.src == UpdateInput::DEVICE)))
+        return fail(GLAVA_B200_EINVAL, "%s: module '%s' reads both channels, %s is null", in.who, module_name(r->d.p.module),
+                    in.src == UpdateInput::HOST ? "rb" : "d_rb");
+    CU(cudaSetDevice(r->device));
     int rc;
-    if (mask && !raster_only) {
-        int cnt = 0;
-        for (int s = 0; s < r->batch; ++s) cnt += mask[s] ? 1 : 0;
-        modified = cnt > 0;
-        if (cnt == 0 || cnt == r->batch) mask = nullptr;        // nobody / everybody: the plain forms
-        else if (r->interp_on)
-            return fail(GLAVA_B200_EINVAL, "per-stream modified masks are not available with keyframe interpolation active "
-                                           "(setinterpolate): the keyframe rotation is per renderer; update the streams in lock step");
-    } else mask = nullptr;
-    if ((rc = frame_ready(r)) != 0) return rc;
-    const glava_b200_params& p = r->p;
-    const bool new_tex = !raster_only && (modified || r->interp_on);   // an interpolated frame has a new texture without new audio
+    if (in.src == UpdateInput::HOST && (rc = frame_ready(r)) != 0) return rc;     // host input: before the mask
+    if (in.mask && (cnt == 0 || cnt == r->batch)) in.mask = nullptr;               // nobody / everybody: the plain forms
+    if (in.mask && r->d.interp_on)
+        return fail(GLAVA_B200_EINVAL, "per-stream modified masks are not available with keyframe interpolation active "
+                                       "(setinterpolate): the keyframe rotation is per renderer; update the streams in lock step");
+    if (in.src != UpdateInput::HOST && (rc = frame_ready(r)) != 0) return rc;
+    // a K5 form the plan refuses (spectrum_plan.h) fails every update with a new texture
+    const bool new_tex = in.src != UpdateInput::TEXTURES && (in.modified || r->d.interp_on);
+    if (new_tex && !r->tab.plan.refusal.empty()) return fail(GLAVA_B200_EINVAL, "%s", r->tab.plan.refusal.c_str());
+    return 0;
+}
+
+// The keyframe buffer that is neither the start nor the end of the interpolation: the next update's chain result goes there
+static int next_key(const glava_b200* r) { int k = 0; while (k == r->key_start || k == r->key_end) ++k; return k; }
+
+// The spectrum half of an update, on spec_stream, from device PCM [batch][n_in]: the stages in front of the FFT, the spectrum
+// update in the launch structure build_tables chose (spectrum_plan.h), the post chain and the keyframe rotation
+static int enqueue_spectrum(glava_b200* r, const float* d_l, const float* d_r, bool modified, const uint8_t* mask) {
+    const glava_b200_params& p = r->d.p;
+    const bool new_tex = modified || r->d.interp_on;      // an interpolated frame has a new texture without new audio
     const int planes = r->batch * 2;
     const size_t total = (size_t) planes * p.n;
-    // a K5 form the plan refuses (spectrum_plan.h) fails every update with a new texture before it enqueues anything or
-    // changes any state
-    if (new_tex && !r->tab.plan.refusal.empty()) return fail(GLAVA_B200_EINVAL, "%s", r->tab.plan.refusal.c_str());
+    int rc;
     if (new_tex) CU(cudaStreamWaitEvent(r->spec_stream, r->ev_raster_done[r->tex_cur ^ 1], 0));
-    if (modified && r->p_user.bufscale > 1) {
+    if (modified && r->d.user.bufscale > 1) {
         const int chans = p.module == GLAVA_B200_MOD_WAVE ? 1 : 2;
-        if ((rc = launch_bufscale(d_l, d_r, r->d_scaled[0], r->d_scaled[1], r->batch, r->n_in, r->p_user.bufscale, chans, r->spec_stream)) != 0) return rc;
+        if ((rc = launch_bufscale(d_l, d_r, r->d_scaled[0], r->d_scaled[1], r->batch, r->d.n_in, r->d.user.bufscale, chans, r->spec_stream)) != 0) return rc;
         ++r->launches;
         d_l = r->d_scaled[0]; d_r = r->d_scaled[1];
     }
@@ -692,37 +721,24 @@ static int run_update(glava_b200* r, const float* d_l, const float* d_r, int mod
         d_l = r->d_scaled[0]; d_r = chans == 2 ? r->d_scaled[1] : r->d_scaled[0];
     }
     float* chain_out = r->d_spec;                         // where the float chain result of this update goes
-    if (r->interp_on) {
-        int nxt = 0; while (nxt == r->key_start || nxt == r->key_end) ++nxt;
-        chain_out = r->d_key[nxt];
-    }
+    if (r->d.interp_on) chain_out = r->d_key[next_key(r)];
     if (modified) {
         const int b = r->tex_cur ^ 1;
-        SpectrumArgs a;
-        memset(&a, 0, sizeof(a));
+        SpectrumArgs a = r->d.spec_args;
         a.pcm_l = d_l; a.pcm_r = d_r; a.window = r->d_window; a.twiddle = r->d_twiddle;
-        a.spec = chain_out; a.skip_tex = r->post_chain ? 1 : 0; a.applied = r->d_applied; a.ring_f = r->d_ring_f;
+        a.spec = chain_out; a.skip_tex = r->d.post_chain ? 1 : 0; a.applied = r->d_applied; a.ring_f = r->d_ring_f;
         a.gr_store = r->d_gr_store; a.ring_u = r->d_ring_u; a.tex = tex_half(r, b); a.av_out = r->d_av;
         a.batch = r->batch; a.update = r->updates;
         a.umask = nullptr; a.tex_prev = tex_half(r, r->tex_cur);
         if (mask || r->desync) { if ((rc = stage_umask(r, mask, &a.umask)) != 0) return rc; }
-        const int F = p.avg_frames;
-        for (int f = 0; f < F; ++f) {
-            // pipeline A: window_frame(f, avg_frames - 1) -> cos(TWOPI*f/F - 1), double (render.c:661,766)
-            a.avg_w_a[f] = 0.6 - (0.4 * cos(6.28318530718 * (double) f / (double) F - 1));
-            // pipeline B: window(I, _AVG_FRAMES - 1) -> cos(TWOPI*I/F - 1), GLSL float (average_pass.frag:41)
-            a.avg_w_b[f] = 0.53836f - (0.46164f * cosf(6.28318530718f * (float) f / (float) F - 1.0f));
-        }
-        a.avg_b_windowed = (p.avg_window && F != 2) ? 1 : 0;
         if (r->timing && (rc = timing_mark(r->ev_spec, r->spec_stream)) != 0) return rc;
-        // in the launch structure build_tables chose (spectrum_plan.h)
         if ((rc = launch_spectrum_update(p, r->tab.plan, r->tab.spec, a, r->spec_stream)) < 0) return rc;
         r->launches += (uint64_t) rc;
-        if (r->post_chain && p.transform_smooth == 1) {                     // render.c:694-718, after the module's chain
+        if (r->d.post_chain && p.transform_smooth == 1) {                     // render.c:694-718, after the module's chain
             if ((rc = launch_transform_smooth(chain_out, p.n, r->tab.ts_tab, r->tab.ts_asz, r->tab.ts_lim, planes, r->spec_stream, a.umask)) != 0) return rc;
             ++r->launches;
         }
-        if (!r->post_chain) {
+        if (!r->d.post_chain) {
             if (r->timing && (rc = timing_mark(r->ev_spec, r->spec_stream)) != 0) return rc;
             CU(cudaEventRecord(r->ev_spec_done[b], r->spec_stream));
             r->tex_cur = b;
@@ -730,13 +746,13 @@ static int run_update(glava_b200* r, const float* d_l, const float* d_r, int mod
         ++r->updates;
         r->d_spec_cur = chain_out;
     }
-    if (r->post_chain && new_tex) {
+    if (r->d.post_chain && new_tex) {
         // R16 upload of the buffer this frame shows (render.c:2185) and K5 (render.c:2276-2303).  With keyframe
         // interpolation that is the lerp of the two PREVIOUS post-transform buffers (render.c:1792-1809): the
         // update just computed becomes visible one update later (rc.glsl:129-130).
         const int b = r->tex_cur ^ 1;
         uint16_t* dst = p.smooth_pass ? r->d_av : tex_half(r, b);
-        if (r->interp_on) {
+        if (r->d.interp_on) {
             const float mod = keyframe_mod(p.ur, p.fr > 0.0f ? p.fr : p.ur, r->kcounter);   // render.c:1761,1804
             rc = launch_upload(r->d_key[r->key_start], r->d_key[r->key_end], mod, dst, total, r->spec_stream);
         } else {
@@ -751,17 +767,22 @@ static int run_update(glava_b200* r, const float* d_l, const float* d_r, int mod
         if (modified && r->timing && (rc = timing_mark(r->ev_spec, r->spec_stream)) != 0) return rc;
         CU(cudaEventRecord(r->ev_spec_done[b], r->spec_stream));
         r->tex_cur = b;
-        if (r->interp_on && modified) {                                       // render.c:2347-2353: start <- end <- this update
-            int nxt = 0; while (nxt == r->key_start || nxt == r->key_end) ++nxt;
+        if (r->d.interp_on && modified) {                                       // render.c:2347-2353: start <- end <- this update
+            const int nxt = next_key(r);
             r->key_start = r->key_end; r->key_end = nxt;
         }
     }
-    if (!raster_only) r->kcounter = modified ? 0 : r->kcounter + 1;           // render.c:2380-2383
+    r->kcounter = modified ? 0 : r->kcounter + 1;                             // render.c:2380-2383
+    return 0;
+}
+
+// The raster half of an update, on stream: the raster pass of raster_plan.h (knobs read at every pass) over the latest texture
+static int enqueue_raster(glava_b200* r) {
     const int b = r->tex_cur;
+    int rc;
     CU(cudaStreamWaitEvent(r->stream, r->ev_spec_done[b], 0));
-    // the raster pass (raster_plan.h); its knobs are read at every pass
     const RasterKnobs knobs = raster_knobs([](const char* name) -> const char* { return getenv(name); });
-    const glava_b200_params view = raster_view(p);
+    const glava_b200_params view = raster_view(r->d.p);
     const ConfigTables& tb = r->tab;
     const RasterPlan pl = plan_raster(view, tb.raster, r->batch, r->slots, knobs);
     RasterArgs ra;
@@ -776,7 +797,7 @@ static int run_update(glava_b200* r, const float* d_l, const float* d_r, int mod
     ra.ctile_nx = pl.ctile ? tb.ctile_nx : 0;
     ra.coltab = pl.coltab ? (float*) r->frame.coltab : nullptr;
     ra.marks = r->frame.marks; ra.marks_valid = raster_marks_valid(pl, r->mark_key, knobs) ? 1 : 0;
-    if (pl.texmm && (rc = launch_texmm(p, ra.tex, r->d_texmm, r->batch * 2, r->stream)) != 0) return rc;
+    if (pl.texmm && (rc = launch_texmm(r->d.p, ra.tex, r->d_texmm, r->batch * 2, r->stream)) != 0) return rc;
     r->mark_key = 0;                                      // until every launch of the pass is enqueued
     if (r->timing && (rc = timing_mark(r->ev_ras, r->stream)) != 0) return rc;
     if ((rc = launch_raster(view, pl, ra, r->stream)) != 0) return rc;
@@ -787,43 +808,46 @@ static int run_update(glava_b200* r, const float* d_l, const float* d_r, int mod
     return 0;
 }
 
-static int update_host(glava_b200* r, const float* lb, const float* rb, size_t bsz, int modified, const uint8_t* mask);
-
-int glava_b200_update(glava_b200* r, const float* lb, const float* rb, size_t bsz, int modified) {
-    clear_error();
-    if (!r || !lb) return fail(GLAVA_B200_EINVAL, "glava_b200_update: null argument");
-    return update_host(r, lb, rb, bsz, modified, nullptr);
-}
-
-static int update_host(glava_b200* r, const float* lb, const float* rb, size_t bsz, int modified, const uint8_t* mask) {
-    if (bsz != (size_t) r->n_in) return fail(GLAVA_B200_EINVAL, "glava_b200_update: bsz %zu != setbufsize %d", bsz, r->n_in);
-    // rd_update always gets both rings (render.h:58); only `wave` ignores rb (wave/1.frag:7 samples audio_l alone)
-    if (modified && !rb && r->p.module != GLAVA_B200_MOD_WAVE)
-        return fail(GLAVA_B200_EINVAL, "glava_b200_update: module '%s' reads both channels, rb is null", module_name(r->p.module));
-    CU(cudaSetDevice(r->device));
-    int rc = frame_ready(r);
+// One update = the spectrum half on spec_stream (when there is a new texture) + the raster half on stream.
+//   spectrum(i) waits for: its input (caller-provided event on spec_stream), spectrum(i-1) (same stream:
+//                          gravity / average state is read-modify-write), raster(i-2) (last reader of the
+//                          texture half it overwrites)
+//   raster(i)   waits for: spectrum(i)
+// so raster(i) and spectrum(i+1) run concurrently: one is HBM-store bound, the other latency bound.
+static int run_update(glava_b200* r, UpdateInput in) {
+    int rc = check_update(r, in);
     if (rc) return rc;
-    size_t bytes = (size_t) r->batch * bsz * 4;
+    const float* d_l = (const float*) in.l;
+    const float* d_r = in.r ? (const float*) in.r : d_l;
     const int b = r->stage_cur;
-    if (modified) {
-        // Staging buffer b is free once the spectrum kernel that last read it has finished; the copy runs
-        // on its own stream so it overlaps the previous update's kernels.  The call returns after the
-        // copy has completed, so — like rd_update — the caller may reuse lb / rb immediately.
+    const bool staged = in.src == UpdateInput::HOST && in.modified;
+    if (staged) {
+        // into staging buffer b once the kernels that last read it are done; on copy_stream, under the previous update
+        const size_t bytes = (size_t) r->batch * in.bsz * 4;
         CU(cudaStreamWaitEvent(r->copy_stream, r->ev_free[b], 0));
-        CU(cudaMemcpyAsync(r->d_pcm[b][0], lb, bytes, cudaMemcpyHostToDevice, r->copy_stream));
-        if (r->p.module != GLAVA_B200_MOD_WAVE)
-            CU(cudaMemcpyAsync(r->d_pcm[b][1], rb, bytes, cudaMemcpyHostToDevice, r->copy_stream));
+        CU(cudaMemcpyAsync(r->d_pcm[b][0], in.l, bytes, cudaMemcpyHostToDevice, r->copy_stream));
+        if (r->d.p.module != GLAVA_B200_MOD_WAVE) CU(cudaMemcpyAsync(r->d_pcm[b][1], in.r, bytes, cudaMemcpyHostToDevice, r->copy_stream));
         CU(cudaEventRecord(r->ev_copied[b], r->copy_stream));
         CU(cudaStreamWaitEvent(r->spec_stream, r->ev_copied[b], 0));
     }
-    if ((rc = run_update(r, r->d_pcm[b][0], r->d_pcm[b][1], modified, false, mask)) != 0) return rc;
-    if (modified) {
+    if (in.src == UpdateInput::HOST) { d_l = r->d_pcm[b][0]; d_r = r->d_pcm[b][1]; }
+    if (in.src == UpdateInput::RINGS) { d_l = r->d_ring[r->ring_cur][0]; d_r = r->d_ring[r->ring_cur][1]; }
+    if (in.ready) CU(cudaStreamWaitEvent(r->spec_stream, (cudaEvent_t) in.ready, 0));
+    if ((rc = enqueue_spectrum(r, d_l, d_r, in.modified, in.mask)) != 0 || (rc = enqueue_raster(r)) != 0) return rc;
+    if (staged) {
+        // like rd_update, return once lb / rb are consumed (unless glava_b200_set_async_input)
         CU(cudaEventRecord(r->ev_free[b], r->spec_stream));
         r->stage_cur = b ^ 1;
         r->last_in = b;
         if (!r->async_input) CU(cudaEventSynchronize(r->ev_copied[b]));
     }
     return 0;
+}
+
+int glava_b200_update(glava_b200* r, const float* lb, const float* rb, size_t bsz, int modified) {
+    clear_error();
+    if (!r || !lb) return fail(GLAVA_B200_EINVAL, "glava_b200_update: null argument");
+    return run_update(r, { UpdateInput::HOST, "glava_b200_update", lb, rb, bsz, modified != 0 });
 }
 
 // Double-buffer contract for the host rings (instead of rd_update's "consumed on return"): with async input enabled
@@ -845,26 +869,19 @@ int glava_b200_wait_input(glava_b200* r) {
 int glava_b200_update_masked(glava_b200* r, const float* lb, const float* rb, size_t bsz, const uint8_t* modified) {
     clear_error();
     if (!r || !lb || !modified) return fail(GLAVA_B200_EINVAL, "glava_b200_update_masked: null argument");
-    int any = 0;
-    for (int s = 0; s < r->batch; ++s) any |= modified[s];
-    return update_host(r, lb, rb, bsz, any ? 1 : 0, modified);
+    return run_update(r, { UpdateInput::HOST, "glava_b200_update_masked", lb, rb, bsz, true, modified });
 }
 
 int glava_b200_update_device_masked(glava_b200* r, const float* d_lb, const float* d_rb, size_t bsz, const uint8_t* modified) {
     clear_error();
     if (!r || !d_lb || !modified) return fail(GLAVA_B200_EINVAL, "glava_b200_update_device_masked: null argument");
-    if (bsz != (size_t) r->n_in) return fail(GLAVA_B200_EINVAL, "glava_b200_update_device_masked: bsz %zu != setbufsize %d", bsz, r->n_in);
-    if (((uintptr_t) d_lb & 15) || ((uintptr_t) d_rb & 15)) return fail(GLAVA_B200_EINVAL, "device PCM pointers must be 16-byte aligned");
-    if (!d_rb && r->p.module != GLAVA_B200_MOD_WAVE) return fail(GLAVA_B200_EINVAL, "glava_b200_update_device_masked: module '%s' reads both channels, d_rb is null", module_name(r->p.module));
-    CU(cudaSetDevice(r->device));
-    return run_update(r, d_lb, d_rb ? d_rb : d_lb, 1, false, modified);
+    return run_update(r, { UpdateInput::DEVICE, "glava_b200_update_device_masked", d_lb, d_rb, bsz, true, modified });
 }
 
 int glava_b200_update_rings_masked(glava_b200* r, const uint8_t* modified) {
     clear_error();
     if (!r || !modified) return fail(GLAVA_B200_EINVAL, "glava_b200_update_rings_masked: null argument");
-    CU(cudaSetDevice(r->device));
-    return run_update(r, r->d_ring[r->ring_cur][0], r->d_ring[r->ring_cur][1], 1, false, modified);
+    return run_update(r, { UpdateInput::RINGS, "glava_b200_update_rings_masked", nullptr, nullptr, 0, true, modified });
 }
 
 // Ordering of glava_b200_update_device against the caller's own CUDA work.  The spectrum kernel reads d_lb / d_rb on an
@@ -872,10 +889,9 @@ int glava_b200_update_rings_masked(glava_b200* r, const uint8_t* modified) {
 // kernel waits for it on the device; glava_b200_input_event() is recorded after the kernel that last READ the buffers, so
 // the producer can cudaStreamWaitEvent on it before overwriting them.  Both are cudaEvent_t passed as void*.
 int glava_b200_update_device_after(glava_b200* r, const float* d_lb, const float* d_rb, size_t bsz, int modified, void* ready_event) {
-    if (!r) return fail(GLAVA_B200_EINVAL, "null argument");
-    CU(cudaSetDevice(r->device));
-    if (ready_event) CU(cudaStreamWaitEvent(r->spec_stream, (cudaEvent_t) ready_event, 0));
-    return glava_b200_update_device(r, d_lb, d_rb, bsz, modified);
+    clear_error();
+    if (!r || !d_lb) return fail(GLAVA_B200_EINVAL, "glava_b200_update_device_after: null argument");
+    return run_update(r, { UpdateInput::DEVICE, "glava_b200_update_device_after", d_lb, d_rb, bsz, modified != 0, nullptr, ready_event });
 }
 void* glava_b200_input_event(glava_b200* r) {
     if (!r) return nullptr;
@@ -888,18 +904,13 @@ void* glava_b200_input_event(glava_b200* r) {
 int glava_b200_update_device(glava_b200* r, const float* d_lb, const float* d_rb, size_t bsz, int modified) {
     clear_error();
     if (!r || !d_lb) return fail(GLAVA_B200_EINVAL, "glava_b200_update_device: null argument");
-    if (bsz != (size_t) r->n_in) return fail(GLAVA_B200_EINVAL, "glava_b200_update_device: bsz %zu != setbufsize %d", bsz, r->n_in);
-    if (((uintptr_t) d_lb & 15) || ((uintptr_t) d_rb & 15)) return fail(GLAVA_B200_EINVAL, "device PCM pointers must be 16-byte aligned");
-    if (modified && !d_rb && r->p.module != GLAVA_B200_MOD_WAVE)
-        return fail(GLAVA_B200_EINVAL, "glava_b200_update_device: module '%s' reads both channels, d_rb is null", module_name(r->p.module));
-    CU(cudaSetDevice(r->device));
-    return run_update(r, d_lb, d_rb ? d_rb : d_lb, modified);
+    return run_update(r, { UpdateInput::DEVICE, "glava_b200_update_device", d_lb, d_rb, bsz, modified != 0 });
 }
 
 static int ingest(glava_b200* r, const void* chunks, bool float_in, int frames, const char* who) {
     clear_error();
     if (!r || !chunks) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
-    if (frames < 1 || frames > r->n_in) return fail(GLAVA_B200_EINVAL, "%s: frames %d out of range", who, frames);
+    if (frames < 1 || frames > r->d.n_in) return fail(GLAVA_B200_EINVAL, "%s: frames %d out of range", who, frames);
     CU(cudaSetDevice(r->device));
     size_t bytes = (size_t) r->batch * frames * 2 * (float_in ? sizeof(float) : sizeof(int16_t));
     if (bytes > r->chunks_cap) {
@@ -912,7 +923,7 @@ static int ingest(glava_b200* r, const void* chunks, bool float_in, int frames, 
     // ordered with the spectrum kernels (they read the rings): same stream
     CU(cudaMemcpyAsync(r->d_chunks, chunks, bytes, cudaMemcpyHostToDevice, r->spec_stream));
     int cur = r->ring_cur, nxt = cur ^ 1;
-    int rc = launch_fifo_ingest(r->p_user, r->d_chunks, float_in, frames, r->d_ring[cur][0], r->d_ring[cur][1],
+    int rc = launch_fifo_ingest(r->d.user, r->d_chunks, float_in, frames, r->d_ring[cur][0], r->d_ring[cur][1],
                                 r->d_ring[nxt][0], r->d_ring[nxt][1], r->batch, r->spec_stream);
     if (rc) return rc;
     ++r->launches;
@@ -925,8 +936,7 @@ int glava_b200_ingest_float(glava_b200* r, const float* chunks, int frames) { re
 int glava_b200_update_rings(glava_b200* r, int modified) {
     clear_error();
     if (!r) return fail(GLAVA_B200_EINVAL, "null argument");
-    CU(cudaSetDevice(r->device));
-    return run_update(r, r->d_ring[r->ring_cur][0], r->d_ring[r->ring_cur][1], modified);
+    return run_update(r, { UpdateInput::RINGS, "glava_b200_update_rings", nullptr, nullptr, 0, modified != 0 });
 }
 
 // ---- offscreen hand-off (glava.h:16-25, glava.c:244-267) -----------------------------------------------------------
@@ -944,7 +954,7 @@ int glava_b200_wait_frame(glava_b200* r) {
 void* glava_b200_frame_event(const glava_b200* r) { return r ? (void*) r->ev_raster_done[r->tex_cur] : nullptr; }
 const void* glava_b200_frame_device(const glava_b200* r, int stream) {
     if (!r || stream < 0 || stream >= r->batch || !r->frame.fb) return nullptr;
-    return r->frame.fb + (size_t) r->p.w * r->p.h * 4 * (size_t) (stream % r->slots);
+    return r->frame.fb + (size_t) r->d.p.w * r->d.p.h * 4 * (size_t) (stream % r->slots);
 }
 int glava_b200_framebuffer_ipc(glava_b200* r, void* handle, size_t handle_bytes) {
     clear_error();
@@ -1009,7 +1019,7 @@ int glava_b200_readback(glava_b200* r, int stream, uint8_t* rgba) {
     clear_error();
     if (!r || !rgba || stream < 0 || stream >= r->batch) return fail(GLAVA_B200_EINVAL, "glava_b200_readback: bad arguments");
     CU(cudaSetDevice(r->device));
-    size_t frame = (size_t) r->p.w * r->p.h * 4;
+    size_t frame = (size_t) r->d.p.w * r->d.p.h * 4;
     CU(cudaMemcpyAsync(rgba, r->frame.fb + frame * (size_t) (stream % r->slots), frame, cudaMemcpyDeviceToHost, r->stream));
     CU(cudaStreamSynchronize(r->stream));
     return 0;
@@ -1019,7 +1029,7 @@ int glava_b200_readback_async(glava_b200* r, int stream, uint8_t* rgba) {
     clear_error();
     if (!r || !rgba || stream < 0 || stream >= r->batch) return fail(GLAVA_B200_EINVAL, "glava_b200_readback_async: bad arguments");
     CU(cudaSetDevice(r->device));
-    const size_t frame = (size_t) r->p.w * r->p.h * 4;
+    const size_t frame = (size_t) r->d.p.w * r->d.p.h * 4;
     int rc;
     if (!r->ev_stage_free[1].get()) {                      // created last: the read-back stream and its events are complete
         if ((rc = r->out_stream.create(0)) != 0) return rc;
@@ -1058,7 +1068,7 @@ int glava_b200_readback_fence(glava_b200* r) {
 
 static int planes_to_host(glava_b200* r, const void* d, size_t elem, void* out_l, void* out_r) {
     // device layout [batch][2][n] -> two host arrays [batch][n]
-    const size_t row = (size_t) r->p.n * elem;
+    const size_t row = (size_t) r->d.p.n * elem;
     CU(cudaStreamSynchronize(r->spec_stream));
     if (out_l) CU(cudaMemcpy2DAsync(out_l, row, d, 2 * row, row, (size_t) r->batch, cudaMemcpyDeviceToHost, r->stream));
     if (out_r) CU(cudaMemcpy2DAsync(out_r, row, (const char*) d + row, 2 * row, row, (size_t) r->batch, cudaMemcpyDeviceToHost, r->stream));
@@ -1084,14 +1094,14 @@ int glava_b200_smooth_pass(glava_b200* r, const uint16_t* in, uint16_t* out, int
     if (!r->built) return unbuilt();
     CU(cudaSetDevice(r->device));
     // the renderer's whole-plane table when it has one, else k5_planes_kernel where its spans fit shared memory
-    const std::string refusal = r->tab.plan.full_table ? std::string() : k5_planes_refusal(k5_planes_span(r->p));
+    const std::string refusal = r->tab.plan.full_table ? std::string() : k5_planes_refusal(k5_planes_span(r->d.p));
     if (!refusal.empty()) return fail(GLAVA_B200_EINVAL, "%s", refusal.c_str());
-    const size_t bytes = (size_t) count * r->p.n * 2;
+    const size_t bytes = (size_t) count * r->d.p.n * 2;
     DevBuf<uint16_t> d_in, d_out;
     int rc;
     if ((rc = d_in.alloc(bytes)) != 0 || (rc = d_out.alloc(bytes)) != 0) return rc;
     CU(cudaMemcpyAsync(d_in, in, bytes, cudaMemcpyHostToDevice, r->stream));
-    if ((rc = launch_k5_full(r->p, r->tab.plan, r->tab.spec.k5, d_in, d_out, count, r->stream)) != 0) return rc;
+    if ((rc = launch_k5_full(r->d.p, r->tab.plan, r->tab.spec.k5, d_in, d_out, count, r->stream)) != 0) return rc;
     ++r->launches;
     CU(cudaMemcpyAsync(out, d_out, bytes, cudaMemcpyDeviceToHost, r->stream));
     CU(cudaStreamSynchronize(r->stream));
@@ -1101,29 +1111,29 @@ int glava_b200_smooth_pass(glava_b200* r, const uint16_t* in, uint16_t* out, int
 int glava_b200_raster_textures(glava_b200* r, const uint16_t* tex_l, const uint16_t* tex_r) {
     clear_error();
     if (!r || !tex_l) return fail(GLAVA_B200_EINVAL, "glava_b200_raster_textures: null argument");
-    CU(cudaSetDevice(r->device));
-    int rc = frame_ready(r);
+    UpdateInput in = { UpdateInput::TEXTURES, "glava_b200_raster_textures", tex_l, tex_r };
+    int rc = check_update(r, in);
     if (rc) return rc;
-    const size_t row = (size_t) r->p.n * 2;
+    const size_t row = (size_t) r->d.p.n * 2;
     CU(cudaStreamSynchronize(r->spec_stream));
     char* dst = (char*) tex_half(r, r->tex_cur);
     CU(cudaMemcpy2DAsync(dst, 2 * row, tex_l, row, row, (size_t) r->batch, cudaMemcpyHostToDevice, r->stream));
     if (tex_r) CU(cudaMemcpy2DAsync(dst + row, 2 * row, tex_r, row, row, (size_t) r->batch, cudaMemcpyHostToDevice, r->stream));
-    return run_update(r, nullptr, nullptr, 0, true);
+    return enqueue_raster(r);
 }
 
 int glava_b200_transform_smooth(glava_b200* r, float* planes, int count) {
     clear_error();
     if (!r || !planes || count < 1) return fail(GLAVA_B200_EINVAL, "glava_b200_transform_smooth: bad arguments");
-    if (!r->p.transform_smooth) return fail(GLAVA_B200_EINVAL, "glava_b200_transform_smooth: the renderer was not created with transform_smooth");
+    if (!r->d.p.transform_smooth) return fail(GLAVA_B200_EINVAL, "glava_b200_transform_smooth: the renderer was not created with transform_smooth");
     if (!r->built) return unbuilt();
     CU(cudaSetDevice(r->device));
-    const size_t bytes = (size_t) count * r->p.n * 4;
+    const size_t bytes = (size_t) count * r->d.p.n * 4;
     DevBuf<float> d;
     int rc = d.alloc(bytes);
     if (rc) return rc;
     CU(cudaMemcpyAsync(d, planes, bytes, cudaMemcpyHostToDevice, r->stream));
-    if ((rc = launch_transform_smooth(d, r->p.n, r->tab.ts_tab, r->tab.ts_asz, r->tab.ts_lim, count, r->stream)) != 0) return rc;
+    if ((rc = launch_transform_smooth(d, r->d.p.n, r->tab.ts_tab, r->tab.ts_asz, r->tab.ts_lim, count, r->stream)) != 0) return rc;
     ++r->launches;
     CU(cudaMemcpyAsync(planes, d, bytes, cudaMemcpyDeviceToHost, r->stream));
     CU(cudaStreamSynchronize(r->stream));
@@ -1148,7 +1158,7 @@ static StateLayout state_layout(const glava_b200_params& p, int n_in) {
 // The parameters a blob records and is checked against: the effective ones, fb_slots zeroed (it sizes no stream's state)
 static void state_params(const glava_b200* r, glava_b200_params* out) {
     memset(out, 0, sizeof(*out));
-    memcpy(out, &r->p, sizeof(*out));
+    memcpy(out, &r->d.p, sizeof(*out));
     out->fb_slots = 0;
 }
 
@@ -1171,7 +1181,7 @@ static int state_check_streams(const glava_b200* r, const int* streams, int coun
 
 namespace glb {
 int state_check_blobs(const glava_b200* r, const void* const* blobs, int count, const char* who) {
-    const StateLayout L = state_layout(r->p, r->n_in);
+    const StateLayout L = state_layout(r->d.p, r->d.n_in);
     glava_b200_params want;
     state_params(r, &want);
     for (int i = 0; i < count; ++i) {
@@ -1212,18 +1222,18 @@ static int state_staging(glava_b200* r, const StateLayout& L) {
 // the host waits for copies only, never for earlier kernels.  Reset and load write the texture half the last raster may still
 // read: spec_stream waits for that raster on the device.
 static int state_io(glava_b200* r, int op, const int* streams, int count, void* const* out, const void* const* in) {
-    const StateLayout L = state_layout(r->p, r->n_in);
+    const StateLayout L = state_layout(r->d.p, r->d.n_in);
     const size_t seg = ss_segment_bytes(L), blob = ss_blob_bytes(L);
     int rc;
     if (count == 0) return 0;
     if ((rc = state_staging(r, L)) != 0) return rc;
     StatePtrs P;
-    P.gravity = (char*) (r->p.accel_fft ? (void*) r->d_gr_store : (void*) r->d_applied);
-    P.ring = (char*) (r->p.accel_fft ? (void*) r->d_ring_u : (void*) r->d_ring_f);
+    P.gravity = (char*) (r->d.p.accel_fft ? (void*) r->d_gr_store : (void*) r->d_applied);
+    P.ring = (char*) (r->d.p.accel_fft ? (void*) r->d_ring_u : (void*) r->d_ring_f);
     P.spec = (char*) r->d_spec.get(); P.tex = (char*) tex_half(r, r->tex_cur); P.av = (char*) r->d_av.get();
     P.fifo[0] = (char*) r->d_ring[r->ring_cur][0].get(); P.fifo[1] = (char*) r->d_ring[r->ring_cur][1].get();
     CU(cudaStreamWaitEvent(r->spec_stream, r->ev_raster_done[r->tex_cur], 0));
-    const uint32_t F = (uint32_t) r->p.avg_frames;
+    const uint32_t F = (uint32_t) r->d.p.avg_frames;
     int last = -1;
     for (int c0 = 0; c0 < count; c0 += r->sst_streams) {
         const int k = r->sst_cur, cnt = count - c0 < r->sst_streams ? count - c0 : r->sst_streams;
@@ -1281,12 +1291,12 @@ static int state_io(glava_b200* r, int op, const int* streams, int count, void* 
 namespace glb {
 int state_save_ptrs(glava_b200* r, const int* streams, int count, void* const* blobs) {
     const char* who = "glava_b200_save_streams";
-    if (r->interp_on) return state_unavailable(who);
+    if (r->d.interp_on) return state_unavailable(who);
     int rc = state_check_streams(r, streams, count, who);
     if (rc) return rc;
     for (int i = 0; i < count; ++i) if (!blobs[i]) return fail(GLAVA_B200_EINVAL, "%s: null blob", who);
     CU(cudaSetDevice(r->device));
-    const StateLayout L = state_layout(r->p, r->n_in);
+    const StateLayout L = state_layout(r->d.p, r->d.n_in);
     StateHeader h;
     memset(&h, 0, sizeof(h));
     h.magic = GLB_STATE_MAGIC; h.version = GLB_STATE_VERSION; h.header_bytes = GLB_STATE_HEADER_BYTES;
@@ -1303,7 +1313,7 @@ int state_save_ptrs(glava_b200* r, const int* streams, int count, void* const* b
 }
 int state_load_ptrs(glava_b200* r, const int* streams, int count, const void* const* blobs) {
     const char* who = "glava_b200_load_streams";
-    if (r->interp_on) return state_unavailable(who);
+    if (r->d.interp_on) return state_unavailable(who);
     int rc = state_check_streams(r, streams, count, who);
     if (rc) return rc;
     if ((rc = state_check_blobs(r, blobs, count, who)) != 0) return rc;
@@ -1326,7 +1336,7 @@ size_t glava_b200_stream_state_bytes(const glava_b200_params* p) {
 int glava_b200_reset_streams(glava_b200* r, const uint8_t* mask) {
     clear_error();
     if (!r || !mask) return fail(GLAVA_B200_EINVAL, "glava_b200_reset_streams: null argument");
-    if (r->interp_on) return state_unavailable("glava_b200_reset_streams");
+    if (r->d.interp_on) return state_unavailable("glava_b200_reset_streams");
     std::vector<int> list;
     for (int s = 0; s < r->batch; ++s) if (mask[s]) list.push_back(s);
     if (list.empty()) return 0;
@@ -1337,7 +1347,7 @@ int glava_b200_reset_streams(glava_b200* r, const uint8_t* mask) {
 int glava_b200_save_streams(glava_b200* r, const int* streams, int count, void* blobs) {
     clear_error();
     if (!r || (count > 0 && !blobs)) return fail(GLAVA_B200_EINVAL, "glava_b200_save_streams: null argument");
-    const size_t bytes = ss_blob_bytes(state_layout(r->p, r->n_in));
+    const size_t bytes = ss_blob_bytes(state_layout(r->d.p, r->d.n_in));
     std::vector<void*> ptrs(count > 0 ? (size_t) count : 0);
     for (size_t i = 0; i < ptrs.size(); ++i) ptrs[i] = (char*) blobs + i * bytes;
     return state_save_ptrs(r, streams, count, ptrs.data());
@@ -1346,7 +1356,7 @@ int glava_b200_save_streams(glava_b200* r, const int* streams, int count, void* 
 int glava_b200_load_streams(glava_b200* r, const int* streams, int count, const void* blobs) {
     clear_error();
     if (!r || (count > 0 && !blobs)) return fail(GLAVA_B200_EINVAL, "glava_b200_load_streams: null argument");
-    const size_t bytes = ss_blob_bytes(state_layout(r->p, r->n_in));
+    const size_t bytes = ss_blob_bytes(state_layout(r->d.p, r->d.n_in));
     std::vector<const void*> ptrs(count > 0 ? (size_t) count : 0);
     for (size_t i = 0; i < ptrs.size(); ++i) ptrs[i] = (const char*) blobs + i * bytes;
     return state_load_ptrs(r, streams, count, ptrs.data());

@@ -66,7 +66,7 @@ GLB_HD float gravity_a(float b, float* applied, float g) {
     return a;
 }
 // transform_average weight (render.c:661,766): window_frame(f, avg_frames - 1) expands to
-// 0.6 - 0.4*cos(TWOPI*f/F - 1), double.  Host-computed LUT, see make_avg_weights_a().
+// 0.6 - 0.4*cos(TWOPI*f/F - 1), double.  Host-computed LUT, once per build: derive() in capi.cu.
 
 // ---- pipeline B (R16 GL passes) ------------------------------------------------------------------
 // K1 + K2: GL_MAX blend into gr_store then gravity_pass.frag:8, render.c:2199-2228

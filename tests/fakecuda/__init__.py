@@ -34,6 +34,7 @@ def lib():
         L = C.CDLL(so)
         shutil.rmtree(out)                                            # stays mapped
         L.fake_first_violation.restype = C.c_char_p
+        L.fake_trace.restype = C.c_char_p
         for f in ("fake_creations", "fake_live", "fake_launches", "fake_violations", "fake_stale", "fake_reached"):
             getattr(L, f).restype = C.c_long
         L.fake_fail_at.argtypes = [C.c_long]

@@ -41,6 +41,11 @@ class Fake:
             "glava_b200_default_params": (i32, [P, C.c_char_p]), "glava_b200_new": (vp, [P, i32, i32]),
             "glava_b200_destroy": (None, [vp]), "glava_b200_reconfigure": (i32, [vp, P]), "glava_b200_get_params": (i32, [vp, P]),
             "glava_b200_update": (i32, [vp, vp, vp, C.c_size_t, i32]), "glava_b200_update_masked": (i32, [vp, vp, vp, C.c_size_t, vp]),
+            "glava_b200_update_device": (i32, [vp, vp, vp, C.c_size_t, i32]),
+            "glava_b200_update_device_masked": (i32, [vp, vp, vp, C.c_size_t, vp]),
+            "glava_b200_update_device_after": (i32, [vp, vp, vp, C.c_size_t, i32, vp]),
+            "glava_b200_update_rings_masked": (i32, [vp, vp]),
+            "glava_b200_set_async_input": (i32, [vp, i32]), "glava_b200_wait_input": (i32, [vp]),
             "glava_b200_ingest_fifo": (i32, [vp, vp, i32]), "glava_b200_update_rings": (i32, [vp, i32]),
             "glava_b200_reset_streams": (i32, [vp, vp]), "glava_b200_save_streams": (i32, [vp, vp, i32, vp]),
             "glava_b200_load_streams": (i32, [vp, vp, i32, vp]), "glava_b200_stream_state_bytes": (C.c_size_t, [P]),
