@@ -13,9 +13,11 @@ There is no CPU fallback: constructing a Renderer without the CUDA library or wi
 raises.
 """
 from .api import (Params, Color, Renderer, GlavaError, default_params, load_config, lib, lib_path,
-                  MODULES, pinned_empty, Pipe, ShardedRenderer, stream_state_bytes, STATE_HEADER_BYTES)
+                  MODULES, pinned_empty, Pipe, ShardedRenderer, stream_state_bytes, STATE_HEADER_BYTES,
+                  StreamStyle, stream_style, style_params, STYLE_AMPLIFY, STYLE_FG, STYLE_BG)
 from . import audio
 from .synth import synth_pcm_int16, fifo_to_float, StreamRings
 
 __all__ = ["audio", "Params", "Color", "Renderer", "GlavaError", "default_params", "load_config", "lib",
-           "lib_path", "MODULES", "pinned_empty", "Pipe", "ShardedRenderer", "stream_state_bytes", "STATE_HEADER_BYTES", "synth_pcm_int16", "fifo_to_float", "StreamRings"]
+           "lib_path", "MODULES", "pinned_empty", "Pipe", "ShardedRenderer", "stream_state_bytes", "STATE_HEADER_BYTES",
+           "StreamStyle", "stream_style", "style_params", "STYLE_AMPLIFY", "STYLE_FG", "STYLE_BG", "synth_pcm_int16", "fifo_to_float", "StreamRings"]

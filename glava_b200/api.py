@@ -104,6 +104,14 @@ class Params(C.Structure):
         return q
 
 
+class StreamStyle(C.Structure):
+    """glava_b200_stream_style: what one stream overrides of the renderer's look (`set`: STYLE_* bits)"""
+    _fields_ = [("set", C.c_uint32), ("amplify", C.c_float), ("fg", Color), ("bg", C.c_float * 4)]
+
+
+STYLE_AMPLIFY, STYLE_FG, STYLE_BG = 1, 2, 4
+
+
 _lib = None
 
 
@@ -216,6 +224,11 @@ def lib():
     L.glava_b200_sharded_reset_streams.argtypes = [vp, vp]
     L.glava_b200_sharded_save_streams.argtypes = [vp, vp, i32, vp]
     L.glava_b200_sharded_load_streams.argtypes = [vp, vp, i32, vp]
+    L.glava_b200_style_params.argtypes = [C.POINTER(Params), C.POINTER(StreamStyle), C.POINTER(Params)]
+    L.glava_b200_parse_hex_color.argtypes = [C.c_char_p, C.POINTER(C.c_float)]
+    for f in ("glava_b200_set_stream_styles", "glava_b200_get_stream_styles", "glava_b200_sharded_set_stream_styles",
+              "glava_b200_sharded_get_stream_styles"):
+        getattr(L, f).argtypes = [vp, vp, i32, vp]
     _lib = L
     # errors surface as Python exceptions; keep stderr quiet
     _quiet = C.CFUNCTYPE(None, cp)(lambda msg: None)
@@ -302,6 +315,76 @@ def load_config(paths=None, entry="rc.glsl", requests=None, force_module=None, b
     return p
 
 
+def _rgba(value):
+    """a colour as floats: "#rrggbb[aa]" through the library's own parser (glava_b200_parse_hex_color: the rounding of a
+    `--pipe` bind), or 4 numbers"""
+    if isinstance(value, str):
+        out = (C.c_float * 4)()
+        _check(lib().glava_b200_parse_hex_color(value.strip().encode(), out))
+        return tuple(out)
+    v = tuple(float(x) for x in value)
+    assert len(v) == 4, value
+    return v
+
+
+def stream_style(style):
+    """a StreamStyle from a StreamStyle, None (no style) or a dict such as
+    {"amplify": 450, "fg": "#ff8000", "bg": (0.1, 0.1, 0.1, 1)}; fg may also be a Color (mode 0: a gradient)"""
+    if isinstance(style, StreamStyle):
+        return style
+    s = StreamStyle()
+    if not style:
+        return s
+    unknown = set(style) - {"amplify", "fg", "bg"}
+    if unknown:
+        raise ValueError(f"unknown stream style fields {sorted(unknown)}")
+    if style.get("amplify") is not None:
+        s.set |= STYLE_AMPLIFY
+        s.amplify = float(style["amplify"])
+    if style.get("fg") is not None:
+        s.set |= STYLE_FG
+        fg = style["fg"]
+        if isinstance(fg, Color):
+            C.memmove(C.byref(s.fg), C.byref(fg), C.sizeof(Color))
+        else:
+            c = _rgba(fg)
+            s.fg.mode = 1
+            s.fg.lo = (C.c_float * 4)(*c)
+            s.fg.hi = (C.c_float * 4)(*c)
+    if style.get("bg") is not None:
+        s.set |= STYLE_BG
+        s.bg = (C.c_float * 4)(*_rgba(style["bg"]))
+    return s
+
+
+def style_params(params, style):
+    """`params` with the stream style applied (glava_b200_style_params): what a batch-1 renderer needs to render what a
+    stream of that style renders"""
+    out = Params()
+    s = stream_style(style)
+    _check(lib().glava_b200_style_params(C.byref(params), C.byref(s), C.byref(out)))
+    return out
+
+
+class _StreamStyles:
+    """set_stream_styles / get_stream_styles over the handle's C entry points (self._style_fn: set, get)"""
+
+    def set_stream_styles(self, streams, styles):
+        """give streams[i] the look styles[i] (StreamStyle, dict or None = the renderer's own) from the next raster pass on"""
+        s = np.ascontiguousarray(np.asarray(streams, dtype=np.int64).reshape(-1), dtype=np.int32)
+        styles = list(styles)
+        assert len(styles) == s.shape[0], (len(styles), s.shape)
+        arr = (StreamStyle * max(len(styles), 1))(*[stream_style(x) for x in styles])
+        _check(self._style_fn[0](self._h, s.ctypes.data, s.shape[0], arr))
+
+    def get_stream_styles(self, streams):
+        """-> [StreamStyle] of the listed streams (set == 0: none)"""
+        s = np.ascontiguousarray(np.asarray(streams, dtype=np.int64).reshape(-1), dtype=np.int32)
+        arr = (StreamStyle * max(s.shape[0], 1))()
+        _check(self._style_fn[1](self._h, s.ctypes.data, s.shape[0], arr))
+        return [arr[i] for i in range(s.shape[0])]
+
+
 class Pipe:
     """live `--pipe NAME[:TYPE]` binds fed with stdin text (glava.c:338-411, render.c:1846-2100)"""
 
@@ -363,8 +446,12 @@ def pinned_empty(shape, dtype, device=None):
     return np.frombuffer(buf, dtype=dtype).reshape(shape)
 
 
-class Renderer(_StreamState):
+class Renderer(_StreamState, _StreamStyles):
     """Batched renderer handle: the role of struct glava_renderer (render.h:8-30)."""
+
+    @property
+    def _style_fn(self):
+        return self._L.glava_b200_set_stream_styles, self._L.glava_b200_get_stream_styles
 
     @property
     def _fn(self):
@@ -580,10 +667,14 @@ class Renderer(_StreamState):
         except Exception: pass
 
 
-class ShardedRenderer(_StreamState):
+class ShardedRenderer(_StreamState, _StreamStyles):
     """One handle for a batch spread over several GPUs of a node (glava_b200_new_sharded): contiguous stream blocks, one
     worker thread per device, no inter-device traffic.  devices: list of CUDA ordinals (may repeat), or None = all visible.
     reset_streams / save_streams / load_streams take global stream indices."""
+
+    @property
+    def _style_fn(self):
+        return self._L.glava_b200_sharded_set_stream_styles, self._L.glava_b200_sharded_get_stream_styles
 
     @property
     def _fn(self):

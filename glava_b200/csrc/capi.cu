@@ -70,6 +70,9 @@ struct ConfigTables {
     void* geo = nullptr;                                      // polar geometry cache (radial / circle), see raster_kernels.cu
     void* ctile = nullptr; int ctile_nx = 0, ctile_count = 0; // circle: per-tile texel reference ranges (launch_circle_tiles)
     void* ts_tab = nullptr; int ts_asz = 0, ts_lim = 0;       // transform_smooth {smin, smax} table
+    // stream styles (DESIGN 4.9), when any stream has one: the style slot of every stream [batch] and the slots' records
+    // (RasterArgs::style_of / styles); rowtab then holds a table per slot, geo a radial cache per distinct (fg, bg)
+    const int* style_of = nullptr; const StyleSlot* styles = nullptr;
     std::vector<DevBuf<>> bufs;
 };
 
@@ -158,6 +161,8 @@ struct glava_b200 {
     // the launch structure that last wrote the dirty-row marks (RasterPlan::mark_key; 0 = none: the next bars / graph / wave
     // launch stores every row)
     int mark_key = 0;
+    // per-stream styles as set (glava_b200_set_stream_styles), [batch]; empty: no stream has one
+    std::vector<glava_b200_stream_style> styles;
     unsigned long long updates = 0;
     // per-stream `modified` masks (glava_b200_update_masked): once streams have advanced unevenly, every stream has its
     // own average-ring cursor; words {bit 31 = modified, low bits = cursor} go to the device through a small pinned ring
@@ -334,9 +339,105 @@ void glava_b200_host_free(void* p) {
 
 }  // extern "C"
 
+// ---- stream styles (DESIGN 4.9) ------------------------------------------------------------------------------------------
+// The fields a style replaces (glava_b200_stream_style), and the refusals that do not need validate_params
+static int style_fields(const glava_b200_params& base, const glava_b200_stream_style& s, glava_b200_params* q) {
+    auto bad = [](const char* why) { return fail(GLAVA_B200_EINVAL, "stream style: %s", why); };
+    if (s.set & ~(GLAVA_B200_STYLE_AMPLIFY | GLAVA_B200_STYLE_FG | GLAVA_B200_STYLE_BG)) return bad("unknown bits in `set`");
+    *q = base;
+    if (!s.set) return 0;
+    const int m = base.module;
+    if (m == GLAVA_B200_MOD_TEST) return bad("the test module has no AMPLIFY, @fg or @bg");
+    if (s.set & GLAVA_B200_STYLE_AMPLIFY) {
+        if (!std::isfinite(s.amplify)) return bad("amplify must be finite");
+        *style_amplify_field(*q) = s.amplify;
+    }
+    if (s.set & GLAVA_B200_STYLE_FG) {
+        if (s.fg.mode != 0 && s.fg.mode != 1) return bad("fg must be a constant (mode 1) or a gradient (mode 0)");
+        if ((m == GLAVA_B200_MOD_CIRCLE || m == GLAVA_B200_MOD_WAVE) && s.fg.mode != 1)
+            return bad("circle / wave take a constant fg (mode 1)");
+        if (m == GLAVA_B200_MOD_BARS && !(s.set & GLAVA_B200_STYLE_BG) && base.bars_outline_mode == 2)
+            return bad("fg without bg on bars whose BAR_OUTLINE is an expression (it was compiled against the renderer's COLOR)");
+        // a constant, as the config reader stores a constant COLOR: hi = lo, the gradient stays
+        auto take = [&](glava_b200_color* c, glava_b200_color_prog* prog) {
+            const float g = c->gradient;
+            *c = s.fg;
+            if (c->mode == 1) { memcpy(c->hi, c->lo, sizeof(c->hi)); c->gradient = g; }
+            prog->n_ops = 0;
+        };
+        switch (m) {
+            case GLAVA_B200_MOD_BARS: take(&q->bars_color, &q->bars_color_prog); break;
+            case GLAVA_B200_MOD_RADIAL: take(&q->radial_color, &q->radial_color_prog); break;
+            case GLAVA_B200_MOD_GRAPH: take(&q->graph_color, &q->graph_color_prog); break;
+            case GLAVA_B200_MOD_CIRCLE: memcpy(q->circle_outline, s.fg.lo, sizeof(q->circle_outline)); break;
+            case GLAVA_B200_MOD_WAVE: memcpy(q->wave_base_color, s.fg.lo, sizeof(q->wave_base_color)); break;
+        }
+    }
+    if (s.set & GLAVA_B200_STYLE_BG) {
+        const size_t c4 = 4 * sizeof(float);
+        switch (m) {
+            case GLAVA_B200_MOD_BARS: q->bars_outline_mode = 1; memcpy(q->bars_outline, s.bg, c4); break;
+            case GLAVA_B200_MOD_RADIAL: memcpy(q->radial_outline, s.bg, c4); memcpy(q->radial_bar_outline, s.bg, c4); break;
+            case GLAVA_B200_MOD_GRAPH: memcpy(q->graph_outline, s.bg, c4); break;
+            case GLAVA_B200_MOD_WAVE: memcpy(q->wave_outline, s.bg, c4); break;
+            case GLAVA_B200_MOD_CIRCLE: return bad("circle has no @bg");
+        }
+    }
+    return 0;
+}
+
+}  // extern "C"
+
+namespace glb {
+int style_apply(const glava_b200_params& base, const glava_b200_stream_style& s, glava_b200_params* out) {
+    glava_b200_params q;
+    int rc = style_fields(base, s, &q);
+    if (rc) return rc;
+    if ((rc = validate_params(&q)) != 0) return rc;
+    *out = q;
+    return 0;
+}
+}  // namespace glb
+
+extern "C" {
+
+// A style with only what it sets, so that equal looks compare equal byte for byte (a constant fg: lo alone)
+static glava_b200_stream_style style_key(const glava_b200_stream_style& s, uint32_t fields) {
+    glava_b200_stream_style k;
+    memset(&k, 0, sizeof(k));
+    k.set = s.set & fields;
+    if (k.set & GLAVA_B200_STYLE_AMPLIFY) k.amplify = s.amplify;
+    if (k.set & GLAVA_B200_STYLE_FG) {
+        k.fg.mode = s.fg.mode;
+        memcpy(k.fg.lo, s.fg.lo, sizeof(k.fg.lo));
+        if (s.fg.mode != 1) { memcpy(k.fg.hi, s.fg.hi, sizeof(k.fg.hi)); k.fg.gradient = s.fg.gradient; }
+    }
+    if (k.set & GLAVA_B200_STYLE_BG) memcpy(k.bg, s.bg, sizeof(k.bg));
+    return k;
+}
+static int style_find(const std::vector<glava_b200_stream_style>& keys, const glava_b200_stream_style& k) {
+    for (size_t i = 0; i < keys.size(); ++i) if (!memcmp(&keys[i], &k, sizeof(k))) return (int) i;
+    return -1;
+}
+
+extern "C" int glava_b200_parse_hex_color(const char* text, float rgba[4]) {
+    clear_error();
+    if (!text || !rgba) return fail(GLAVA_B200_EINVAL, "glava_b200_parse_hex_color: null argument");
+    float c[4];
+    if (text[0] != '#' || !parse_hex_color(text, c, true)) return fail(GLAVA_B200_EINVAL, "'%s' is not a #rrggbb[aa] colour", text);
+    memcpy(rgba, c, sizeof(c));
+    return 0;
+}
+
+extern "C" int glava_b200_style_params(const glava_b200_params* base, const glava_b200_stream_style* s, glava_b200_params* out) {
+    clear_error();
+    if (!base || !s || !out) return fail(GLAVA_B200_EINVAL, "glava_b200_style_params: null argument");
+    return style_apply(*base, *s, out);
+}
+
 // Everything derived from the parameters that does not depend on the audio (ConfigTables), built into `tb` for the
-// parameters of `d`.  Its kernels run on the handle's stream.
-static int build_tables(glava_b200* r, const Derived& d, ConfigTables& tb) {
+// parameters of `d` and the stream styles `styles` ([batch], or empty).  Its kernels run on the handle's stream.
+static int build_tables(glava_b200* r, const Derived& d, const std::vector<glava_b200_stream_style>& styles, ConfigTables& tb) {
     const glava_b200_params& p = d.p;
     cudaStream_t st = r->stream;
     int rc;
@@ -388,14 +489,63 @@ static int build_tables(glava_b200* r, const Derived& d, ConfigTables& tb) {
         sd.k5.out = nullptr; sd.k5.count = (int) kt.out.size(); sd.k5.max_span = kt.max_span;
         sd.k5.smem_bytes = K5_S_PLANES * kt.max_span * (int) sizeof(float);
     }
-    if ((rc = table_buf(tb, &tb.rowtab, (size_t) p.h * 8, st, nullptr, true)) != 0) return rc;
-    if (p.module == GLAVA_B200_MOD_BARS || p.module == GLAVA_B200_MOD_GRAPH) { if ((rc = launch_bars_rowtab(p, tb.rowtab, st)) != 0) return rc; ++r->launches; }
-    // polar modules: the audio-independent per-pixel geometry
-    const RasterTables rt = raster_tables(p, raster_knobs([](const char* name) -> const char* { return getenv(name); }));
-    if (rt.geo) {
-        if ((rc = table_buf(tb, &tb.geo, rt.geo_bytes, st, nullptr)) != 0) return rc;
-        if ((rc = launch_polar_geo(p, tb.geo, rt.box, st)) != 0) return rc;
+    // Style slots: slot 0 is the renderer's own look, every distinct style of `styles` one more slot (sp: its effective
+    // parameters); radial keeps a geometry cache per distinct (fg, bg) pair of the slots (geo_of)
+    std::vector<glava_b200_params> sp(1, p);
+    std::vector<int> slot_of, geo_of(1, 0);
+    if (!styles.empty()) {
+        const uint32_t colours = GLAVA_B200_STYLE_FG | GLAVA_B200_STYLE_BG;
+        std::vector<glava_b200_stream_style> keys(1, style_key(styles[0], 0)), pairs(1, style_key(styles[0], 0));
+        slot_of.assign((size_t) r->batch, 0);
+        for (int s = 0; s < r->batch; ++s) {
+            const glava_b200_stream_style k = style_key(styles[(size_t) s], ~0u);
+            int slot = style_find(keys, k);
+            if (slot < 0) {
+                glava_b200_params q;
+                if ((rc = style_fields(p, k, &q)) != 0) return rc;
+                const glava_b200_stream_style pk = style_key(k, colours);
+                int g = style_find(pairs, pk);
+                if (g < 0) { g = (int) pairs.size(); pairs.push_back(pk); }
+                slot = (int) keys.size(); keys.push_back(k); sp.push_back(q); geo_of.push_back(g);
+            }
+            slot_of[(size_t) s] = slot;
+        }
+    }
+    const int nslots = (int) sp.size();
+    int ngeo = 0;
+    for (int g : geo_of) ngeo = g + 1 > ngeo ? g + 1 : ngeo;
+    const glava_b200_params reach = style_reach_params(p, sp.data(), nslots);
+    const RasterTables rt = raster_tables(reach, raster_knobs([](const char* name) -> const char* { return getenv(name); }), nslots, ngeo);
+    const bool rows = p.module == GLAVA_B200_MOD_BARS || p.module == GLAVA_B200_MOD_GRAPH;
+    if ((rc = table_buf(tb, &tb.rowtab, (size_t) nslots * p.h * 8, st, nullptr, true)) != 0) return rc;
+    for (int k = 0; rows && k < nslots; ++k) {
+        if ((rc = launch_bars_rowtab(sp[(size_t) k], (char*) tb.rowtab + (size_t) k * p.h * 8, st)) != 0) return rc;
         ++r->launches;
+    }
+    // polar modules: the audio-independent per-pixel geometry (radial: of every (fg, bg) pair, in the slots' common box)
+    if (rt.geo) {
+        if ((rc = table_buf(tb, &tb.geo, rt.geo_bytes * rt.geo_caches, st, nullptr)) != 0) return rc;
+        for (int g = 0; g < rt.geo_caches; ++g) {
+            int k = 0;
+            while (geo_of[(size_t) k] != g) ++k;
+            if ((rc = launch_polar_geo(sp[(size_t) k], (char*) tb.geo + (size_t) g * rt.geo_bytes, rt.box, st)) != 0) return rc;
+            ++r->launches;
+        }
+    }
+    if (nslots > 1) {
+        std::vector<StyleSlot> rec((size_t) nslots);
+        for (int k = 0; k < nslots; ++k) {
+            rec[(size_t) k].p = raster_view(sp[(size_t) k]);
+            rec[(size_t) k].rowtab = (const char*) tb.rowtab + (size_t) k * p.h * 8;
+            rec[(size_t) k].geo = !rt.geo ? nullptr
+                                : (const char*) tb.geo + (p.module == GLAVA_B200_MOD_RADIAL ? (size_t) geo_of[(size_t) k] * rt.geo_bytes : 0);
+        }
+        StyleSlot* d_rec = nullptr; int* d_of = nullptr;
+        if ((rc = table_buf(tb, &d_rec, rec.size() * sizeof(StyleSlot), st, rec.data())) != 0 ||
+            (rc = table_buf(tb, &d_of, slot_of.size() * sizeof(int), st, slot_of.data())) != 0) return rc;
+        tb.styles = d_rec; tb.style_of = d_of;
+        // the host copies of `rec` and `slot_of` must outlive the uploads
+        CU(cudaStreamSynchronize(st));
     }
     if (rt.ctile) {
         int ntx = 0, nty = 0;
@@ -430,9 +580,18 @@ static int sync_all(glava_b200* r) {
 // are missing — so that a rebuild never holds two sets at once, then builds, and commits parameters, flags, tables and
 // plan together once everything has succeeded.  On failure the renderer is unbuilt: it holds no tables, keeps the
 // parameters of its last successful build, and refuses to run (frame_ready) until a rebuild succeeds.
-static int rebuild(glava_b200* r, const glava_b200_params& q) {
+static int rebuild(glava_b200* r, const glava_b200_params& q, const std::vector<glava_b200_stream_style>& styles) {
     int rc = validate_params(&q);
     if (rc) return rc;
+    // every style must suit the new parameters (style_params of them is what its stream renders)
+    std::vector<glava_b200_stream_style> seen;
+    for (const glava_b200_stream_style& s : styles) {
+        const glava_b200_stream_style k = style_key(s, ~0u);
+        if (!k.set || style_find(seen, k) >= 0) continue;
+        glava_b200_params tmp;
+        if ((rc = style_apply(q, s, &tmp)) != 0) return rc;
+        seen.push_back(k);
+    }
     const Derived d = derive(q);
     if ((rc = sync_all(r)) != 0) return rc;
     const bool new_frame = !r->built || !r->frame.fb.get() || q.w != r->d.user.w || q.h != r->d.user.h;
@@ -442,7 +601,7 @@ static int rebuild(glava_b200* r, const glava_b200_params& q) {
     FrameBuffers f;
     ConfigTables tb;
     if (new_frame && (rc = alloc_frame_buffers(r, d.p, f)) != 0) return rc;
-    if ((rc = build_tables(r, d, tb)) != 0) return rc;
+    if ((rc = build_tables(r, d, styles, tb)) != 0) return rc;
     r->d = d;
     r->tab = std::move(tb);
     if (new_frame) { r->frame = std::move(f); r->mark_key = 0; }
@@ -556,7 +715,7 @@ glava_b200* glava_b200_new(const glava_b200_params* params, int batch, int devic
     if (device < 0 || device >= ndev) { fail(GLAVA_B200_EINVAL, "device %d out of range (%d devices)", device, ndev); return nullptr; }
     glava_b200* r = new glava_b200();
     r->batch = batch; r->device = device;
-    if (build_state(r, derive(*params)) != 0 || rebuild(r, *params) != 0) { glava_b200_destroy(r); return nullptr; }
+    if (build_state(r, derive(*params)) != 0 || rebuild(r, *params, r->styles) != 0) { glava_b200_destroy(r); return nullptr; }
     return r;
 }
 
@@ -581,7 +740,7 @@ int glava_b200_reconfigure(glava_b200* r, const glava_b200_params* params) {
                                        "fb_slots, the \"smooth\" transform and whether interpolation is active size the device "
                                        "state and cannot change on a live renderer; create a new one");
     CU(cudaSetDevice(r->device));
-    return rebuild(r, *params);
+    return rebuild(r, *params, r->styles);
 }
 
 int glava_b200_get_params(const glava_b200* r, glava_b200_params* out) {
@@ -616,7 +775,7 @@ static int frame_ready(glava_b200* r) {
     if (unsigned long long req = r->sizereq.exchange(0)) {
         glava_b200_params q = r->d.user;
         q.w = (int) ((req >> 32) & 0x7fffffffu); q.h = (int) (req & 0xffffffffu);
-        int rc = rebuild(r, q);
+        int rc = rebuild(r, q, r->styles);
         if (rc) return rc;
     }
     return r->built ? 0 : unbuilt();
@@ -785,7 +944,7 @@ static int enqueue_raster(glava_b200* r) {
     const glava_b200_params view = raster_view(r->d.p);
     const ConfigTables& tb = r->tab;
     const RasterPlan pl = plan_raster(view, tb.raster, r->batch, r->slots, knobs);
-    RasterArgs ra;
+    RasterPass ra = {};
     ra.tex = tex_half(r, b); ra.fb = r->frame.fb;
     ra.rowtab = pl.rowtab ? tb.rowtab : nullptr;
     ra.batch = r->batch; ra.slots = r->slots; ra.stream0 = 0;
@@ -797,6 +956,7 @@ static int enqueue_raster(glava_b200* r) {
     ra.ctile_nx = pl.ctile ? tb.ctile_nx : 0;
     ra.coltab = pl.coltab ? (float*) r->frame.coltab : nullptr;
     ra.marks = r->frame.marks; ra.marks_valid = raster_marks_valid(pl, r->mark_key, knobs) ? 1 : 0;
+    if (pl.styled) { ra.styles.style_of = tb.style_of; ra.styles.styles = tb.styles; }
     if (pl.texmm && (rc = launch_texmm(r->d.p, ra.tex, r->d_texmm, r->batch * 2, r->stream)) != 0) return rc;
     r->mark_key = 0;                                      // until every launch of the pass is enqueued
     if (r->timing && (rc = timing_mark(r->ev_ras, r->stream)) != 0) return rc;
@@ -1360,6 +1520,42 @@ int glava_b200_load_streams(glava_b200* r, const int* streams, int count, const 
     std::vector<const void*> ptrs(count > 0 ? (size_t) count : 0);
     for (size_t i = 0; i < ptrs.size(); ++i) ptrs[i] = (const char*) blobs + i * bytes;
     return state_load_ptrs(r, streams, count, ptrs.data());
+}
+
+}  // extern "C"
+
+// ---- stream styles (DESIGN 4.9) ------------------------------------------------------------------------------------------
+extern "C" {
+
+int glava_b200_set_stream_styles(glava_b200* r, const int* streams, int count, const glava_b200_stream_style* styles) {
+    clear_error();
+    const char* who = "glava_b200_set_stream_styles";
+    if (!r || (count > 0 && !styles)) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
+    int rc = state_check_streams(r, streams, count, who);
+    if (rc) return rc;
+    std::vector<glava_b200_stream_style> next = r->styles;
+    if (next.empty()) next.assign((size_t) r->batch, style_key(glava_b200_stream_style{}, 0));
+    for (int i = 0; i < count; ++i) next[(size_t) streams[i]] = styles[i];
+    bool any = false;
+    for (const glava_b200_stream_style& s : next) any |= s.set != 0;
+    if (!any) next.clear();
+    CU(cudaSetDevice(r->device));
+    if ((rc = rebuild(r, r->d.user, next)) != 0) return rc;     // refuses an invalid style before it touches anything
+    r->styles = std::move(next);
+    return 0;
+}
+
+int glava_b200_get_stream_styles(const glava_b200* r, const int* streams, int count, glava_b200_stream_style* out) {
+    clear_error();
+    const char* who = "glava_b200_get_stream_styles";
+    if (!r || (count > 0 && !out)) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
+    int rc = state_check_streams(r, streams, count, who);
+    if (rc) return rc;
+    for (int i = 0; i < count; ++i) {
+        if (r->styles.empty()) memset(&out[i], 0, sizeof(out[i]));
+        else out[i] = r->styles[(size_t) streams[i]];
+    }
+    return 0;
 }
 
 }  // extern "C"

@@ -23,6 +23,7 @@ bool parse_hex_components(const char* s, float* out[4]);
 int  load_config(glava_b200_params* out, const char* const* paths, const char* entry,
                  const char* const* requests, const char* force_module, const char* const* binds);
 int  validate_params(const glava_b200_params* p);
+int  style_apply(const glava_b200_params& base, const glava_b200_stream_style& s, glava_b200_params* out);   // capi.cu
 
 #define GLB_MAX_AVG_FRAMES 16
 
@@ -100,6 +101,24 @@ struct RasterArgs {
     uint32_t* marks;
     int       marks_valid;
 };
+// Stream styles (DESIGN 4.9): the style slot of every stream [batch] and the slots' records [style slots] (slot 0: the
+// renderer's own look).  A parameter of the styled kernel instantiations only, after the others: RasterArgs keeps its
+// layout, so the plain kernels keep their parameter offsets and machine code.
+struct RasterStyles {
+    const int* style_of;
+    const struct StyleSlot* styles;
+};
+// What capi.cu hands launch_raster: the kernels' RasterArgs and, for the styled instantiations, the style slots
+struct RasterPass : RasterArgs {
+    RasterStyles styles;
+};
+// One style slot as the styled raster kernels see it: the raster view of the styled parameters and the slot's tables
+// (bars / graph row table, radial geometry cache; circle: the one cache).  Copied whole into shared memory by every CTA.
+struct alignas(16) StyleSlot {
+    glava_b200_params p;
+    const void* rowtab;
+    const void* geo;
+};
 #define GLB_COLTAB_PLANES 5
 #define GLB_CIRCLE_NB 128                         // texel buckets per plane (n / 128 texels each)
 #define GLB_TEXMM_STRIDE (2 + 2 * GLB_CIRCLE_NB)  // u32 per plane
@@ -145,6 +164,7 @@ int launch_k5_full(const glava_b200_params& p, const SpectrumPlan& plan, const K
                    uint16_t* d_out, int count, void* stream);
 // the raster kernels of one pass (raster_plan.h plan_raster; texmm_kernel aside); p: the raster view (raster_view)
 struct RasterPlan;
+// A styled plan (plan.styled) reads the style slots from the RasterPass `a` is then part of.
 int launch_raster(const glava_b200_params& p, const RasterPlan& plan, const RasterArgs& a, void* stream);
 int launch_bars_rowtab(const glava_b200_params& p, void* d_rowtab, void* stream);
 int launch_texmm(const glava_b200_params& p, const uint16_t* d_tex, uint32_t* d_out, int planes, void* stream);

@@ -60,11 +60,44 @@ __device__ __forceinline__ void mark_store(uint32_t* m, int lo, int hi) {
     if ((threadIdx.x & 31) == 0) *m = dirty_pack(lo, hi);
 }
 
+// Stream styles (DESIGN 4.9).  Every raster kernel has a plain and a styled twin.  The styled one copies its stream's
+// StyleSlot (parameters and tables of the slot) into dynamic shared memory once per CTA, before any thread leaves, and reads
+// everything through it; the plain one reads the kernel parameter and RasterArgs' tables as it always has.  Most pairs are
+// two instantiations of one body.  The plain circle, radial-from-cache and column-less wave kernels keep their own text:
+// instantiated from a shared body they compile to other machine code (register allocation, extra branches and
+// instructions; tools/sass_diff.py), and the plain path must stay what it was.  Their styled twins repeat that code with the
+// slot's reads; tests/test_gpu_stream_styles.py holds each twin to the plain kernel of a batch-1 renderer, frame by frame.
+template <bool STYLED>
+__device__ __forceinline__ const StyleSlot* stream_style(const RasterStyles& sa, int stream) {
+    if constexpr (!STYLED) return nullptr;
+    else {
+        extern __shared__ int4 style_smem[];
+        const int4* src = reinterpret_cast<const int4*>(sa.styles + __ldg(sa.style_of + stream));
+        for (int i = threadIdx.x; i < (int) (sizeof(StyleSlot) / sizeof(int4)); i += blockDim.x) style_smem[i] = __ldg(src + i);
+        __syncthreads();
+        return reinterpret_cast<const StyleSlot*>(style_smem);
+    }
+}
+template <bool STYLED>
+__device__ __forceinline__ const glava_b200_params& style_params_of(const StyleSlot* s, const glava_b200_params& p) {
+    if constexpr (STYLED) return s->p;
+    else return p;
+}
+#define GLB_STYLED_PAIR(body, bounds, name, styled_name)                                                                        \
+    __global__ void bounds name(const __grid_constant__ RasterArgs a, const __grid_constant__ glava_b200_params p, int n) {    \
+        body<false>(a, p, n, RasterStyles{});                                                                                  \
+    }                                                                                                                           \
+    __global__ void bounds styled_name(const __grid_constant__ RasterArgs a, const __grid_constant__ glava_b200_params p, int n, \
+                                       const __grid_constant__ RasterStyles sa) {                                              \
+        body<true>(a, p, n, sa);                                                                                                \
+    }
+
 // generic: every pixel through module_px() — reference semantics with no hoisting; also the
 // fallback for option combinations the specialised kernels do not cover.
-__global__ void __launch_bounds__(128)
-raster_generic_kernel(const __grid_constant__ RasterArgs a, const __grid_constant__ glava_b200_params p, int rows_per_cta) {
+template <bool STYLED>
+__device__ __forceinline__ void generic_body(const RasterArgs& a, const glava_b200_params& pk, int rows_per_cta, const RasterStyles& sa) {
     const int stream = a.stream0 + blockIdx.z;
+    const glava_b200_params& p = style_params_of<STYLED>(stream_style<STYLED>(sa, stream), pk);
     const AudioTex t = make_tex(p, a.tex, stream);
     uint32_t* fb = reinterpret_cast<uint32_t*>(a.fb) + (size_t) (stream % a.slots) * p.w * p.h;
     const int x = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
@@ -95,9 +128,10 @@ raster_generic_kernel(const __grid_constant__ RasterArgs a, const __grid_constan
         store4(fb + (size_t) y * p.w, x, p.w, px);
     }
 }
+GLB_STYLED_PAIR(generic_body, __launch_bounds__(128), raster_generic_kernel, raster_generic_styled_kernel)
 
 // bars (default orientation): column state in registers, row colours from a per-renderer table
-__global__ void bars_rowtab_kernel(uint2* __restrict__ tab, const __grid_constant__ glava_b200_params p) {
+__device__ __forceinline__ void bars_rowtab_body(uint2* __restrict__ tab, const glava_b200_params& p) {
     int y = blockIdx.x * blockDim.x + threadIdx.x;
     if (y >= p.h) return;
     if (p.module == GLAVA_B200_MOD_GRAPH) {
@@ -111,13 +145,15 @@ __global__ void bars_rowtab_kernel(uint2* __restrict__ tab, const __grid_constan
     BarsRow r = bars_row(p, d);
     tab[y] = make_uint2(r.fill, r.outl);
 }
+__global__ void bars_rowtab_kernel(uint2* __restrict__ tab, const __grid_constant__ glava_b200_params p) {
+    bars_rowtab_body(tab, p);
+}
 int launch_bars_rowtab(const glava_b200_params& p, void* d_rowtab, void* stream) {
     bars_rowtab_kernel<<<(p.h + 127) / 128, 128, 0, (cudaStream_t) stream>>>(reinterpret_cast<uint2*>(d_rowtab), p);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(GLAVA_B200_ECUDA, "bars rowtab kernel launch: %s", cudaGetErrorString(e));
     return 0;
 }
-
 // Rows are addressed by t = distance from the bars' base line (t = y, or h-1-y with FLIP), for which
 // d = t + 0.5 exactly in float.  `d < lim` / `d <= lim` are monotone in t, so each column's two float
 // compares per pixel collapse into two integer row thresholds computed once (and corrected with the
@@ -131,14 +167,16 @@ __device__ __forceinline__ int bars_rows_below(float lim, bool inclusive, int h)
 }
 
 // requires w % 4 == 0 (128-bit row alignment) and MIRROR_YX == 0
-__global__ void __launch_bounds__(256)
-raster_bars_kernel(const __grid_constant__ RasterArgs a, const __grid_constant__ glava_b200_params p, int rows_per_cta) {
+template <bool STYLED>
+__device__ __forceinline__ void bars_body(const RasterArgs& a, const glava_b200_params& pk, int rows_per_cta, const RasterStyles& sa) {
     const int stream = a.stream0 + blockIdx.z;
+    const StyleSlot* const sty = stream_style<STYLED>(sa, stream);
+    const glava_b200_params& p = style_params_of<STYLED>(sty, pk);
     const int x = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
     if ((x & ~127) >= p.w) return;                                        // the whole warp is right of the frame
     const bool valid = x < p.w;
     const AudioTex t = make_tex(p, a.tex, stream);
-    const uint2* __restrict__ rowtab = reinterpret_cast<const uint2*>(a.rowtab);
+    const uint2* __restrict__ rowtab = reinterpret_cast<const uint2*>(STYLED ? sty->rowtab : a.rowtab);
     const bool has_outline = p.bars_outline_width > 0.0f;
     int ya[4], yb[4]; bool inner[4];
     int tmax = 0;
@@ -180,6 +218,7 @@ raster_bars_kernel(const __grid_constant__ RasterArgs a, const __grid_constant__
         }
     }
 }
+GLB_STYLED_PAIR(bars_body, __launch_bounds__(256), raster_bars_kernel, raster_bars_styled_kernel)
 
 // graph: heights of 6 columns in registers, row colours from a per-renderer table.  Pixels whose whole
 // 3x3 neighbourhood is filled (or empty) skip the stencil — exact, because then avg.a is exactly the
@@ -200,11 +239,11 @@ __device__ __forceinline__ int graph_first_row(float lim, int off, int h) {
 // graph/1.frag:84-114; wave: wave/1.frag:17-31).  One thread per (stream, column) evaluates it once per update into the
 // column table; the raster kernels then start with six coalesced loads instead of six dependent texture samples per
 // thread and ROW BAND — which had forced whole-column CTAs (1080p: 2560 CTAs of 720 / 360 rows, under two waves).
-template <bool WAVE>
-__global__ void __launch_bounds__(128)
-column_table_kernel(const __grid_constant__ RasterArgs a, const __grid_constant__ glava_b200_params p) {
+template <bool WAVE, bool STYLED>
+__device__ __forceinline__ void column_table_body(const RasterArgs& a, const glava_b200_params& pk, const RasterStyles& sa) {
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
     const int stream = a.stream0 + blockIdx.y;
+    const glava_b200_params& p = style_params_of<STYLED>(stream_style<STYLED>(sa, stream), pk);
     if (x >= p.w) return;
     const AudioTex t = make_tex(p, a.tex, stream);
     float* ct = a.coltab + (size_t) stream * GLB_COLTAB_PLANES * p.w;
@@ -213,11 +252,23 @@ column_table_kernel(const __grid_constant__ RasterArgs a, const __grid_constant_
         ct[x] = c.s; ct[p.w + x] = c.dmin; ct[2 * p.w + x] = c.dmax; ct[3 * p.w + x] = c.thick; ct[4 * p.w + x] = __uint_as_float(c.color);
     } else ct[x] = graph_height(p, t, x);
 }
+template <bool WAVE>
+__global__ void __launch_bounds__(128)
+column_table_kernel(const __grid_constant__ RasterArgs a, const __grid_constant__ glava_b200_params p) {
+    column_table_body<WAVE, false>(a, p, RasterStyles{});
+}
+template <bool WAVE>
+__global__ void __launch_bounds__(128)
+column_table_styled_kernel(const __grid_constant__ RasterArgs a, const __grid_constant__ glava_b200_params p,
+                           const __grid_constant__ RasterStyles sa) {
+    column_table_body<WAVE, true>(a, p, sa);
+}
 
-template <bool TAB, int MINB>
-__global__ void __launch_bounds__(256, MINB)
-raster_graph_kernel(const __grid_constant__ RasterArgs a, const __grid_constant__ glava_b200_params p, int rows_per_cta) {
+template <bool TAB, bool STYLED>
+__device__ __forceinline__ void graph_body(const RasterArgs& a, const glava_b200_params& pk, int rows_per_cta, const RasterStyles& sa) {
     const int stream = a.stream0 + blockIdx.z;
+    const StyleSlot* const sty = stream_style<STYLED>(sa, stream);
+    const glava_b200_params& p = style_params_of<STYLED>(sty, pk);
     const int x = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
     if (x >= p.w) return;
     const AudioTex t = make_tex(p, a.tex, stream);
@@ -237,7 +288,7 @@ raster_graph_kernel(const __grid_constant__ RasterArgs a, const __grid_constant_
         inner_x[k] = (x + k - 1 >= 0) && (x + k + 1 < p.w);
     }
     const int y0 = blockIdx.y * rows_per_cta, y1 = min(p.h, y0 + rows_per_cta);
-    const uint2* __restrict__ rowtab = reinterpret_cast<const uint2*>(a.rowtab);   // [h] {graph_row(y), rows y-1..y+1 opaque}
+    const uint2* __restrict__ rowtab = reinterpret_cast<const uint2*>(STYLED ? sty->rowtab : a.rowtab);   // [h] {graph_row(y), rows y-1..y+1 opaque}
 
     auto full_rows = [&](int ya, int yb) {             // reference evaluation with per-pixel shortcuts
         for (int y = ya; y < yb; ++y) {
@@ -293,6 +344,17 @@ raster_graph_kernel(const __grid_constant__ RasterArgs a, const __grid_constant_
     dirty_zero_span(mark_load(a, mark, y0, y1, lanes), b3, y1, &s0, &s1);
     zero_rows(fb, x, p.w, s0, s1);
     mark_store(mark, y0, b3);
+}
+template <bool TAB, int MINB>
+__global__ void __launch_bounds__(256, MINB)
+raster_graph_kernel(const __grid_constant__ RasterArgs a, const __grid_constant__ glava_b200_params p, int rows_per_cta) {
+    graph_body<TAB, false>(a, p, rows_per_cta, RasterStyles{});
+}
+template <bool TAB, int MINB>
+__global__ void __launch_bounds__(256, MINB)
+raster_graph_styled_kernel(const __grid_constant__ RasterArgs a, const __grid_constant__ glava_b200_params p, int rows_per_cta,
+                         const __grid_constant__ RasterStyles sa) {
+    graph_body<TAB, true>(a, p, rows_per_cta, sa);
 }
 
 // wave: 6 column descriptors in registers
@@ -356,6 +418,74 @@ raster_wave_kernel(const __grid_constant__ RasterArgs a, const __grid_constant__
     dirty_zero_span(old, rb, y1, &s0, &s1);
     zero_rows(fb, x, p.w, s0, s1);
     mark_store(mark, ra, rb);
+}
+// styled twin (DESIGN 4.9): the same code reading its stream's style slot
+template <bool TAB>
+__device__ __forceinline__ void wave_styled_body(const RasterArgs& a, int rows_per_cta, const RasterStyles& sa) {
+    const int stream = a.stream0 + blockIdx.z;
+    const glava_b200_params& p = stream_style<true>(sa, stream)->p;
+    const int x = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
+    if (x >= p.w) return;
+    const AudioTex t = make_tex(p, a.tex, stream);
+    uint32_t* fb = reinterpret_cast<uint32_t*>(a.fb) + (size_t) (stream % a.slots) * p.w * p.h;
+    WaveCol c[6];
+#pragma unroll
+    for (int k = 0; k < 6; ++k) {
+        int xc = x - 1 + k;
+        xc = xc < 0 ? 0 : (xc >= p.w ? p.w - 1 : xc);   // clamped columns are masked by wave_px_cols
+        if (TAB) {
+            const float* __restrict__ ct = a.coltab + (size_t) stream * GLB_COLTAB_PLANES * p.w + xc;
+            c[k].s = __ldg(ct); c[k].dmin = __ldg(ct + p.w); c[k].dmax = __ldg(ct + 2 * p.w); c[k].thick = __ldg(ct + 3 * p.w);
+            c[k].color = __float_as_uint(__ldg(ct + 4 * p.w));
+        } else c[k] = wave_column(p, t, xc);
+    }
+    // rows where any of a pixel's three columns can be lit (+-1 row for the stencil), conservative
+    float ylo[4], yhi[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        float l = 3.0e38f, h = -3.0e38f;
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+            const WaveCol& w = c[k + j];
+            l = fminf(l, fminf(w.s - w.thick, w.s + w.dmin));
+            h = fmaxf(h, fmaxf(w.s + w.thick, w.s + w.dmax));
+        }
+        ylo[k] = l - 2.0f; yhi[k] = h + 2.0f;
+    }
+    const int y0 = blockIdx.y * rows_per_cta, y1 = min(p.h, y0 + rows_per_cta);
+    // rows outside [ra, rb) are 0 for every pixel of this thread: run them as a bare zero-store loop
+    float lo4 = fminf(fminf(ylo[0], ylo[1]), fminf(ylo[2], ylo[3])), hi4 = fmaxf(fmaxf(yhi[0], yhi[1]), fmaxf(yhi[2], yhi[3]));
+    lo4 = fminf(fmaxf(lo4, -1.0f), 1.0e6f); hi4 = fminf(fmaxf(hi4, -1.0f), 1.0e6f);
+    int ra = min(y1, max(y0, (int) floorf(lo4))), rb = max(ra, min(y1, (int) ceilf(hi4) + 1));
+    // make the split warp-uniform (lanes past the right edge have already returned)
+    const unsigned lanes = __activemask();
+    ra = __reduce_min_sync(lanes, ra); rb = __reduce_max_sync(lanes, rb);
+    // zero rows on both sides of the line: store those the previous frame in this slot may have left non-zero
+    uint32_t* const mark = mark_word(a, p, stream, x, y0);
+    const uint32_t old = mark_load(a, mark, y0, y1, lanes);
+    int s0, s1;
+    dirty_zero_span(old, y0, ra, &s0, &s1);
+    zero_rows(fb, x, p.w, s0, s1);
+    for (int y = ra; y < rb; ++y) {
+        const float fy = (float) y;
+        uint32_t px[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            if (fy < ylo[k] || fy > yhi[k] || x + k >= p.w) { px[k] = 0u; continue; }
+            const WaveCol c3[3] = { c[k], c[k + 1], c[k + 2] };
+            px[k] = wave_px_cols(p, c3, x + k, y);
+        }
+        store4(fb + (size_t) y * p.w, x, p.w, px);
+    }
+    dirty_zero_span(old, rb, y1, &s0, &s1);
+    zero_rows(fb, x, p.w, s0, s1);
+    mark_store(mark, ra, rb);
+}
+template <bool TAB, int MINB>
+__global__ void __launch_bounds__(256, MINB)
+raster_wave_styled_kernel(const __grid_constant__ RasterArgs a, const __grid_constant__ glava_b200_params, int rows_per_cta,
+                         const __grid_constant__ RasterStyles sa) {
+    wave_styled_body<TAB>(a, rows_per_cta, sa);
 }
 
 // circle: stage 1 (polar line test) is evaluated once per pixel of a tile + 1-pixel halo into shared
@@ -507,12 +637,162 @@ raster_circle_kernel(const __grid_constant__ RasterArgs a, const __grid_constant
         if (!tile_dead) __syncthreads();             // the tile is rewritten by the next iteration
     }
 }
-
+// styled twin (DESIGN 4.9): the same code reading its stream's style slot
+__device__ __forceinline__ void circle_styled_body(const RasterArgs& a, int tiles_per_cta, const RasterStyles& sa) {
+    __shared__ uint32_t tile[CIRCLE_TH + 2][CIRCLE_TW + 2];
+    const int stream = a.stream0 + blockIdx.z;
+    const glava_b200_params& p = stream_style<true>(sa, stream)->p;   // the cache is the slots' one
+    const AudioTex t = make_tex(p, a.tex, stream);
+    uint32_t* fb = reinterpret_cast<uint32_t*>(a.fb) + (size_t) (stream % a.slots) * p.w * p.h;
+    const int tx0 = blockIdx.x * CIRCLE_TW;
+    const float cx = (float) (p.w / 2), cy = (float) (p.h / 2);
+    // Static bounds of the annulus that can be lit, tightened per stream: a pixel is lit only if
+    // d - C_RADIUS lies within [min(v) - C_LINE/2, max(v) + C_LINE/2] (circle/1.frag:72-80; v = AMPLIFY * texel over
+    // the three fetched texels, 0 for out-of-range fetches), so the stream's texel range bounds its annulus.
+    float reach = circle_reach(p);
+    float inner = p.circle_radius - p.circle_line / 2.0f - 2.0f;
+    if (a.texmm) {
+        const uint32_t* mm = a.texmm + (size_t) stream * 2 * GLB_TEXMM_STRIDE;     // plane l, then plane r: {min, max} first
+        const float f0 = from16(min(__ldg(mm + 0), __ldg(mm + GLB_TEXMM_STRIDE))) * p.circle_amplify;
+        const float f1 = from16(max(__ldg(mm + 1), __ldg(mm + GLB_TEXMM_STRIDE + 1))) * p.circle_amplify;
+        const float vlo = fminf(fminf(f0, f1), 0.0f), vhi = fmaxf(fmaxf(f0, f1), 0.0f);
+        const float hl3 = fabsf(p.circle_line) / 2.0f + 3.0f;
+        reach = fminf(reach, p.circle_radius + vhi + hl3);
+        if (!p.circle_fill) inner = fmaxf(inner, p.circle_radius + vlo - hl3);
+    }
+    const float bx0 = (float) (tx0 - 1) - cx, bx1 = (float) (tx0 + CIRCLE_TW) - cx;
+    const float nx = (bx0 > 0.0f) ? bx0 : ((bx1 < 0.0f) ? -bx1 : 0.0f);
+    const float fxm = fmaxf(fabsf(bx0), fabsf(bx1));
+    // 256 threads: 32 quads per row x 8 rows
+    const int qx = threadIdx.x & 31, qy = threadIdx.x >> 5;
+    const int x = tx0 + qx * 4;
+    const CircleConsts cc = circle_consts(p);
+    // whole CTA region (its 128 columns x tiles_per_cta*8 rows, + halo) outside the disc: bare zero-store loop
+    {
+        const int Y0 = blockIdx.y * tiles_per_cta * CIRCLE_TH, Y1 = min(p.h, Y0 + tiles_per_cta * CIRCLE_TH);
+        const float cb0 = (float) (Y0 - 1) - cy, cb1 = (float) Y1 - cy;
+        const float cny = (cb0 > 0.0f) ? cb0 : ((cb1 < 0.0f) ? -cb1 : 0.0f);
+        if (nx * nx + cny * cny > reach * reach && (p.w & 3) == 0) {
+            if (x < p.w) {
+                const int stride = p.w >> 2;
+                uint4* ptr = reinterpret_cast<uint4*>(fb) + (size_t) (Y0 + qy) * stride + (x >> 2);
+                const uint4 zero = make_uint4(0u, 0u, 0u, 0u);
+                for (int y = Y0 + qy; y < Y1; y += CIRCLE_TH, ptr += (size_t) CIRCLE_TH * stride) __stcs(ptr, zero);
+            }
+            return;
+        }
+    }
+    // a CTA walks `tiles_per_cta` vertically adjacent 128x8 tiles (a tile per CTA is too little work:
+    // most tiles are outside the annulus and only store 4 KB of zeros)
+    for (int it = 0; it < tiles_per_cta; ++it) {
+        const int ty0 = (blockIdx.y * tiles_per_cta + it) * CIRCLE_TH;
+        if (ty0 >= p.h) break;
+        // distance range of the tile (+halo) from the centre
+        const float by0 = (float) (ty0 - 1) - cy, by1 = (float) (ty0 + CIRCLE_TH) - cy;
+        const float ny = (by0 > 0.0f) ? by0 : ((by1 < 0.0f) ? -by1 : 0.0f);
+        const float fym = fmaxf(fabsf(by0), fabsf(by1));
+        bool tile_dead = (nx * nx + ny * ny > reach * reach) || (inner > 0.0f && fxm * fxm + fym * fym < inner * inner);
+        if (!tile_dead && a.ctile && a.texmm) {
+            // the curve inside THIS tile's angular range: min / max over the texel buckets its cells can reference.  Every warp
+            // reduces the same few buckets (no barrier; the outcome is CTA-uniform by construction)
+            const int ti = (blockIdx.y * tiles_per_cta + it) * a.ctile_nx + blockIdx.x;
+            const int4 tr = __ldg(a.ctile + ti);
+            const int lane = threadIdx.x & 31, bs = t.n / GLB_CIRCLE_NB;
+            const uint32_t* ml = a.texmm + (size_t) stream * 2 * GLB_TEXMM_STRIDE + 2;
+            const uint32_t* mr = ml + GLB_TEXMM_STRIDE;
+            uint32_t lo = 65535u, hi = 0u;
+            bool any = __ldg(a.ctile_zero + ti) != 0;
+            if (any) lo = 0u;                                   // an out-of-range reference reads 0
+            if (tr.y >= tr.x) { any = true; for (int b = tr.x / bs + lane; b <= tr.y / bs; b += 32) { lo = min(lo, __ldg(ml + 2 * b)); hi = max(hi, __ldg(ml + 2 * b + 1)); } }
+            if (tr.w >= tr.z) { any = true; for (int b = tr.z / bs + lane; b <= tr.w / bs; b += 32) { lo = min(lo, __ldg(mr + 2 * b)); hi = max(hi, __ldg(mr + 2 * b + 1)); } }
+#pragma unroll
+            for (int k = 16; k > 0; k >>= 1) { lo = min(lo, __shfl_xor_sync(0xffffffffu, lo, k)); hi = max(hi, __shfl_xor_sync(0xffffffffu, hi, k)); }
+            if (!any) tile_dead = true;                         // no cell of the tile (or its halo) can be lit
+            else {
+                if (hi < lo) hi = lo;
+                const float g0 = from16(lo) * p.circle_amplify, g1 = from16(hi) * p.circle_amplify;
+                const float tlo = fminf(g0, g1), thi = fmaxf(g0, g1);
+                const float hl3 = fabsf(p.circle_line) / 2.0f + 3.0f;
+                const float dnear = sqrtf(nx * nx + ny * ny) - p.circle_radius, dfar = sqrtf(fxm * fxm + fym * fym) - p.circle_radius;
+                if (dnear > thi + hl3 || (!p.circle_fill && dfar < tlo - hl3)) tile_dead = true;
+            }
+        }
+        if (!tile_dead) {
+            // (batching the geometry loads of a thread's 5-6 cells ahead of the dependent texel fetches costs
+            // registers and halves the resident warps; the live tiles are bound by instruction issue, not by the two
+            // dependent L2 round trips.)
+            if (a.geo) {
+                // cached geometry: a cell is either outside the cache box (0) or a 16-byte entry with three
+                // texel references + d; entries that cannot be lit carry e0 = -1.  No per-cell float culling,
+                // no transcendental, constants hoisted (the kernel is instruction bound).
+                const int4* __restrict__ geo = reinterpret_cast<const int4*>(a.geo);
+                int ly = threadIdx.x / (CIRCLE_TW + 2), lx = threadIdx.x - ly * (CIRCLE_TW + 2);
+                for (; ly < CIRCLE_TH + 2; ) {
+                    const int bxi = tx0 + lx - 1 - a.gx0, byi = ty0 + ly - 1 - a.gy0;
+                    uint32_t v = 0u;
+                    if (bxi >= 0 && byi >= 0 && bxi < a.gw && byi < a.gh) {
+                        const float dx = (float) (tx0 + lx - 1) - cx, dy = (float) (ty0 + ly - 1) - cy;
+                        const float d2 = dx * dx + dy * dy;
+                        if (d2 <= reach * reach && !(inner > 0.0f && d2 < inner * inner)) {   // per-stream annulus
+                            const int4 e = __ldg(geo + (size_t) byi * a.gw + bxi);
+                            CircleGeo g; g.dR = __int_as_float(e.x); g.e0 = e.y; g.e1 = e.z; g.e2 = e.w;
+                            v = circle_stage1_c(cc, t.l, t.r, t.n, g);
+                        }
+                    }
+                    tile[ly][lx] = v;
+                    lx += 256 - (CIRCLE_TW + 2); ly += 1;               // advance by 256 cells: 256 = 130 + 126
+                    if (lx >= CIRCLE_TW + 2) { lx -= CIRCLE_TW + 2; ly += 1; }
+                }
+            } else
+            for (int i = threadIdx.x; i < (CIRCLE_TH + 2) * (CIRCLE_TW + 2); i += blockDim.x) {
+                const int ly = i / (CIRCLE_TW + 2), lx = i - ly * (CIRCLE_TW + 2);
+                const int gx = tx0 + lx - 1, gy = ty0 + ly - 1;
+                uint32_t v = 0u;
+                if (gx >= 0 && gy >= 0 && gx < p.w && gy < p.h) {
+                    const float dx = (float) gx - cx, dy = (float) gy - cy;
+                    const float d2 = dx * dx + dy * dy;
+                    if (d2 <= reach * reach && !(inner > 0.0f && d2 < inner * inner)) v = circle_stage1(p, t, gx, gy);
+                }
+                tile[ly][lx] = v;
+            }
+            __syncthreads();
+        }
+        const int y = ty0 + qy;
+        if (tile_dead) {
+            if (x < p.w && y < p.h) { const uint32_t px[4] = { 0u, 0u, 0u, 0u }; store4(fb + (size_t) y * p.w, x, p.w, px); }
+        } else if (y < p.h) {
+            // live tile: a lane takes the pixels qx, qx + 32, qx + 64, qx + 96 of its row, so that the 7 tile reads per pixel
+            // are CONSECUTIVE across the warp.  With 4 adjacent pixels per lane (one 128-bit store) every one of those reads
+            // was a 4-way bank conflict, and the kernel is issue bound; four coalesced 4-byte stores per lane cost far less than that.
+            uint32_t* row = fb + (size_t) y * p.w;
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const int cx = qx + 32 * k, gx = tx0 + cx;
+                if (gx >= p.w) continue;
+                const int lx = cx + 1, ly = qy + 1;
+                // circle/2.frag's "- 1" taps at column 0 / row 0 read column 0 / row 0 (int(-0.5) = 0, see circle_px)
+                const int lxm = (gx > 0) ? lx - 1 : lx, lym = (y > 0) ? ly - 1 : ly;
+                const uint32_t own = tile[ly][lx];
+                const uint32_t nb[6] = { tile[ly][lx + 1], tile[ly + 1][lx + 1], tile[ly + 1][lx],
+                                         tile[ly][lxm], tile[lym][lxm], tile[lym][lx] };
+                const uint32_t v = ((own | nb[0] | nb[1] | nb[2] | nb[3] | nb[4] | nb[5]) == 0u) ? 0u : circle_finish(p, own, nb);
+                __stcs(row + gx, v);
+            }
+        }
+        if (!tile_dead) __syncthreads();             // the tile is rewritten by the next iteration
+    }
+}
+__global__ void __launch_bounds__(256, 5)
+raster_circle_styled_kernel(const __grid_constant__ RasterArgs a, const __grid_constant__ glava_b200_params, int tiles_per_cta,
+                            const __grid_constant__ RasterStyles sa) {
+    circle_styled_body(a, tiles_per_cta, sa);
+}
 // radial: per-pixel polar maths (radial/1.frag + premultiply) with disc culling; same arithmetic as
 // raster_generic_kernel but without the module switch (no spills).
-__global__ void __launch_bounds__(128)
-raster_radial_kernel(const __grid_constant__ RasterArgs a, const __grid_constant__ glava_b200_params p, int rows_per_cta) {
+template <bool STYLED>
+__device__ __forceinline__ void radial_body(const RasterArgs& a, const glava_b200_params& pk, int rows_per_cta, const RasterStyles& sa) {
     const int stream = a.stream0 + blockIdx.z;
+    const glava_b200_params& p = style_params_of<STYLED>(stream_style<STYLED>(sa, stream), pk);
     const int x = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
     if (x >= p.w) return;
     const AudioTex t = make_tex(p, a.tex, stream);
@@ -534,6 +814,7 @@ raster_radial_kernel(const __grid_constant__ RasterArgs a, const __grid_constant
         store4(fb + (size_t) y * p.w, x, p.w, px);
     }
 }
+GLB_STYLED_PAIR(radial_body, __launch_bounds__(128), raster_radial_kernel, raster_radial_styled_kernel)
 
 // per-plane {min, max} of the R16 texture the module samples (circle: bounds the stream's annulus), followed by the
 // {min, max} of GLB_CIRCLE_NB buckets of n / GLB_CIRCLE_NB consecutive texels (bounds a TILE's annulus: a tile's cells
@@ -744,46 +1025,158 @@ raster_radial_geo_kernel(const __grid_constant__ RasterArgs a, const __grid_cons
         store4(fb + (size_t) y * p.w, x, p.w, px);
     }
 }
+// styled twin (DESIGN 4.9): the same code reading its stream's style slot and its colours' cache
+__device__ __forceinline__ void radial_geo_styled_body(const RasterArgs& a, int rows_per_cta, const RasterStyles& sa) {
+    __shared__ float vflat[RADIAL_MAX_BARS + 4];        // bar heights, index side * nk + k (== class code - 1)
+    __shared__ float vmax_s;                             // tallest bar of this stream
+    const int stream = a.stream0 + blockIdx.z;
+    const StyleSlot* const sty = stream_style<true>(sa, stream);
+    const glava_b200_params& p = sty->p;
+    const AudioTex t = make_tex(p, a.tex, stream);
+    const int nk = p.radial_nbars / 2 + 2;               // k = int(|idx| / section) <= NBARS / 2 (+1 for rounding)
+    const int y0 = blockIdx.y * rows_per_cta, y1 = min(p.h, y0 + rows_per_cta);
+    const bool band_live = (y1 > a.gy0) && (y0 < a.gy0 + a.gh);
+    if (band_live) {
+        for (int i = threadIdx.x; i < 2 * nk; i += blockDim.x) {
+            const int side = i / nk, k = i - side * nk;
+            vflat[i] = radial_bar_value(p, t, (side << 16) | k);
+        }
+        __syncthreads();
+        if (threadIdx.x < 32) {                          // tallest bar: nothing beyond C_RADIUS + vmax can be lit
+            float m = 0.0f;
+            for (int i = threadIdx.x; i < 2 * nk; i += 32) m = fmaxf(m, vflat[i]);
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+            if (threadIdx.x == 0) vmax_s = m;
+        }
+        __syncthreads();
+    }
+    const int x = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
+    if (x >= p.w) return;
+    // per-stream reach: a bar pixel is lit only if d - C_RADIUS <= v <= vmax; beyond that (and beyond the ring) the
+    // frame is 0 for THIS stream, so those quads skip the geometry loads (typical spectra reach a third of AMPLIFY)
+    const float rcull = band_live ? p.radial_radius + fmaxf(fmaxf(vmax_s, 0.0f), fabsf(p.radial_line)) + 2.0f : 0.0f;
+    const float ccx = (float) (p.w / 2) - p.radial_off_x, ccy = (float) (p.h / 2) - p.radial_off_y;
+    float qdx; {
+        const float dxa = (float) x - ccx, dxb = (float) (x + 4) - ccx;          // pixel centres are at +0.5: [x, x+4) covers them
+        qdx = (dxa > 0.0f) ? dxa : ((dxb < 0.0f) ? -dxb : 0.0f);
+        qdx = fmaxf(qdx - 1.0f, 0.0f);
+    }
+    uint32_t* fb = reinterpret_cast<uint32_t*>(a.fb) + (size_t) (stream % a.slots) * p.w * p.h;
+    const size_t npx = (size_t) a.gw * a.gh;
+    const int4* __restrict__ geo = reinterpret_cast<const int4*>(sty->geo);   // full entries (the slot's colours)
+    const int2* __restrict__ bar8 = reinterpret_cast<const int2*>(geo + npx);               // {lit, dR}
+    const unsigned char* __restrict__ code = reinterpret_cast<const unsigned char*>(bar8 + npx);
+    const int bxi = x - a.gx0;
+    const bool col_live = bxi >= 0 && bxi < a.gw;        // gx0, gw multiples of 4: the quad is inside or outside as a whole
+    // One row per trip on purpose: batching the loads of 4 rows (more memory-level parallelism per warp)
+    // raises the register count enough to halve the resident warps, and even the pure zero-store rows
+    // outside the box need the occupancy.
+    for (int y = y0; y < y1; ++y) {
+        uint32_t px[4] = { 0u, 0u, 0u, 0u };
+        const int byi = y - a.gy0;
+        const float qdy = fmaxf(fabsf((float) y + 0.5f - ccy) - 1.0f, 0.0f);
+        if (col_live && byi >= 0 && byi < a.gh && qdx * qdx + qdy * qdy <= rcull * rcull) {
+            const size_t at = (size_t) byi * a.gw + bxi;
+            // codes and {lit, dR} are fetched together (independent addresses): one L2 round trip per
+            // row instead of two dependent ones — the row loop is latency x occupancy bound
+            const uint32_t codes = __ldg(reinterpret_cast<const uint32_t*>(code + at));       // 4 pixels
+            const int4 e01 = __ldg(reinterpret_cast<const int4*>(bar8 + at));                 // pixels 0, 1
+            const int4 e23 = __ldg(reinterpret_cast<const int4*>(bar8 + at) + 1);             // pixels 2, 3
+            if (codes != 0u) {
+                const int2 e8[4] = { make_int2(e01.x, e01.y), make_int2(e01.z, e01.w), make_int2(e23.x, e23.y), make_int2(e23.z, e23.w) };
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    const uint32_t c = (codes >> (8 * k)) & 255u;
+                    if (c == 0u) continue;
+                    if (c != 255u) {
+                        const int2 e = e8[k];
+                        if (__int_as_float(e.y) <= vflat[c - 1u]) px[k] = (uint32_t) e.x;
+                    } else {
+                        const int4 e = __ldg(geo + at + k);            // {lit, unlit, dR, bar}
+                        uint32_t v = (uint32_t) e.y;
+                        if (e.w >= 0) {
+                            const int kk = e.w & 0xffff;
+                            const float vb = kk < nk ? vflat[(e.w >> 16) * nk + kk] : radial_bar_value(p, t, e.w);
+                            if (__int_as_float(e.z) <= vb) v = (uint32_t) e.x;
+                        }
+                        px[k] = v;
+                    }
+                }
+            }
+        }
+        store4(fb + (size_t) y * p.w, x, p.w, px);
+    }
+}
+__global__ void __launch_bounds__(128)
+raster_radial_geo_styled_kernel(const __grid_constant__ RasterArgs a, const __grid_constant__ glava_b200_params, int rows_per_cta,
+                                const __grid_constant__ RasterStyles sa) {
+    radial_geo_styled_body(a, rows_per_cta, sa);
+}
+
+// One launch of a plain kernel or of its styled twin (the style slots as the last parameter, room for a slot's copy as
+// dynamic shared memory)
+template <bool S>
+static void launch_one(void (*plain)(RasterArgs, glava_b200_params, int), void (*styled)(RasterArgs, glava_b200_params, int, RasterStyles),
+                       dim3 grid, int threads, cudaStream_t st, const RasterArgs& b, const glava_b200_params& p, const RasterStyles& sa, int n) {
+    if constexpr (S) styled<<<grid, threads, sizeof(StyleSlot), st>>>(b, p, n, sa);
+    else plain<<<grid, threads, 0, st>>>(b, p, n);
+}
+template <bool S>
+static void launch_one(void (*plain)(RasterArgs, glava_b200_params), void (*styled)(RasterArgs, glava_b200_params, RasterStyles),
+                       dim3 grid, int threads, cudaStream_t st, const RasterArgs& b, const glava_b200_params& p, const RasterStyles& sa) {
+    if constexpr (S) styled<<<grid, threads, sizeof(StyleSlot), st>>>(b, p, sa);
+    else plain<<<grid, threads, 0, st>>>(b, p);
+}
+// The kernels of one chunk of streams, plain (S = false) or styled
+template <bool S>
+static void launch_chunk(const glava_b200_params& p, const RasterPlan& pl, const RasterArgs& b, const RasterStyles& sa, int nz, cudaStream_t st) {
+    const int quads = (p.w + 3) / 4;
+    const dim3 grid((quads + pl.bx - 1) / pl.bx, (p.h + pl.rows - 1) / pl.rows, nz);
+    const dim3 tg((p.w + 127) / 128, nz);                  // column_table_kernel: a thread per column
+    const int r = pl.rows;
+    switch (pl.kernel) {
+    case RasterKernel::GENERIC: launch_one<S>(raster_generic_kernel, raster_generic_styled_kernel, grid, pl.bx, st, b, p, sa, r); break;
+    case RasterKernel::BARS: launch_one<S>(raster_bars_kernel, raster_bars_styled_kernel, grid, pl.bx, st, b, p, sa, r); break;
+    case RasterKernel::GRAPH: launch_one<S>(raster_graph_kernel<false, 1>, raster_graph_styled_kernel<false, 1>, grid, pl.bx, st, b, p, sa, r); break;
+    case RasterKernel::GRAPH_TAB4:
+        launch_one<S>(column_table_kernel<false>, column_table_styled_kernel<false>, tg, 128, st, b, p, sa);
+        launch_one<S>(raster_graph_kernel<true, 4>, raster_graph_styled_kernel<true, 4>, grid, pl.bx, st, b, p, sa, r);
+        break;
+    case RasterKernel::GRAPH_TAB5:
+        launch_one<S>(column_table_kernel<false>, column_table_styled_kernel<false>, tg, 128, st, b, p, sa);
+        launch_one<S>(raster_graph_kernel<true, 5>, raster_graph_styled_kernel<true, 5>, grid, pl.bx, st, b, p, sa, r);
+        break;
+    case RasterKernel::WAVE: launch_one<S>(raster_wave_kernel<false, 1>, raster_wave_styled_kernel<false, 1>, grid, pl.bx, st, b, p, sa, r); break;
+    case RasterKernel::WAVE_TAB4:
+        launch_one<S>(column_table_kernel<true>, column_table_styled_kernel<true>, tg, 128, st, b, p, sa);
+        launch_one<S>(raster_wave_kernel<true, 4>, raster_wave_styled_kernel<true, 4>, grid, pl.bx, st, b, p, sa, r);
+        break;
+    case RasterKernel::WAVE_TAB5:
+        launch_one<S>(column_table_kernel<true>, column_table_styled_kernel<true>, tg, 128, st, b, p, sa);
+        launch_one<S>(raster_wave_kernel<true, 5>, raster_wave_styled_kernel<true, 5>, grid, pl.bx, st, b, p, sa, r);
+        break;
+    case RasterKernel::RADIAL: launch_one<S>(raster_radial_kernel, raster_radial_styled_kernel, grid, pl.bx, st, b, p, sa, r); break;
+    case RasterKernel::RADIAL_GEO: launch_one<S>(raster_radial_geo_kernel, raster_radial_geo_styled_kernel, grid, pl.bx, st, b, p, sa, r); break;
+    case RasterKernel::CIRCLE: {
+        const int ntile_y = (p.h + CIRCLE_TH - 1) / CIRCLE_TH;
+        const dim3 cgrid((p.w + CIRCLE_TW - 1) / CIRCLE_TW, (ntile_y + pl.circle_tiles - 1) / pl.circle_tiles, nz);
+        launch_one<S>(raster_circle_kernel, raster_circle_styled_kernel, cgrid, pl.bx, st, b, p, sa, pl.circle_tiles);
+        break;
+    }
+    }
+}
 
 int launch_raster(const glava_b200_params& p, const RasterPlan& pl, const RasterArgs& a, void* stream) {
     cudaStream_t st = (cudaStream_t) stream;
+    const RasterStyles sa = pl.styled ? static_cast<const RasterPass&>(a).styles : RasterStyles{};
     if (pl.mark_key && !a.marks) return fail(GLAVA_B200_EINVAL, "raster launch: no dirty-row marks for the bars / graph / wave kernel");
-    const int quads = (p.w + 3) / 4;
+    if (pl.styled && (!sa.style_of || !sa.styles)) return fail(GLAVA_B200_EINVAL, "raster launch: no style slots for the styled kernels");
     for (int s0 = 0; s0 < a.batch; s0 += pl.chunk) {
         RasterArgs b = a; b.stream0 = a.stream0 + s0;
         const int nz = a.batch - s0 < pl.chunk ? a.batch - s0 : pl.chunk;
-        const dim3 grid((quads + pl.bx - 1) / pl.bx, (p.h + pl.rows - 1) / pl.rows, nz);
-        const dim3 tg((p.w + 127) / 128, nz);                  // column_table_kernel: a thread per column
-        switch (pl.kernel) {
-        case RasterKernel::GENERIC: raster_generic_kernel<<<grid, pl.bx, 0, st>>>(b, p, pl.rows); break;
-        case RasterKernel::BARS: raster_bars_kernel<<<grid, pl.bx, 0, st>>>(b, p, pl.rows); break;
-        case RasterKernel::GRAPH: raster_graph_kernel<false, 1><<<grid, pl.bx, 0, st>>>(b, p, pl.rows); break;
-        case RasterKernel::GRAPH_TAB4:
-            column_table_kernel<false><<<tg, 128, 0, st>>>(b, p);
-            raster_graph_kernel<true, 4><<<grid, pl.bx, 0, st>>>(b, p, pl.rows);
-            break;
-        case RasterKernel::GRAPH_TAB5:
-            column_table_kernel<false><<<tg, 128, 0, st>>>(b, p);
-            raster_graph_kernel<true, 5><<<grid, pl.bx, 0, st>>>(b, p, pl.rows);
-            break;
-        case RasterKernel::WAVE: raster_wave_kernel<false, 1><<<grid, pl.bx, 0, st>>>(b, p, pl.rows); break;
-        case RasterKernel::WAVE_TAB4:
-            column_table_kernel<true><<<tg, 128, 0, st>>>(b, p);
-            raster_wave_kernel<true, 4><<<grid, pl.bx, 0, st>>>(b, p, pl.rows);
-            break;
-        case RasterKernel::WAVE_TAB5:
-            column_table_kernel<true><<<tg, 128, 0, st>>>(b, p);
-            raster_wave_kernel<true, 5><<<grid, pl.bx, 0, st>>>(b, p, pl.rows);
-            break;
-        case RasterKernel::RADIAL: raster_radial_kernel<<<grid, pl.bx, 0, st>>>(b, p, pl.rows); break;
-        case RasterKernel::RADIAL_GEO: raster_radial_geo_kernel<<<grid, pl.bx, 0, st>>>(b, p, pl.rows); break;
-        case RasterKernel::CIRCLE: {
-            const int ntile_y = (p.h + CIRCLE_TH - 1) / CIRCLE_TH;
-            const dim3 cgrid((p.w + CIRCLE_TW - 1) / CIRCLE_TW, (ntile_y + pl.circle_tiles - 1) / pl.circle_tiles, nz);
-            raster_circle_kernel<<<cgrid, pl.bx, 0, st>>>(b, p, pl.circle_tiles);
-            break;
-        }
-        }
+        if (pl.styled) launch_chunk<true>(p, pl, b, sa, nz, st);
+        else launch_chunk<false>(p, pl, b, sa, nz, st);
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return fail(GLAVA_B200_ECUDA, "raster kernel launch: %s", cudaGetErrorString(e));
     }

@@ -76,17 +76,24 @@ inline size_t polar_geo_box(const glava_b200_params& p, int box[4]) {
 struct RasterTables {
     bool   geo = false;            // the polar geometry cache
     int    box[4] = { 0, 0, 0, 0 };  // its box (polar_geo_box)
-    size_t geo_bytes = 0;
+    size_t geo_bytes = 0;          // of one cache
     bool   ctile = false;          // circle: the per-tile texel reference ranges (launch_circle_tiles), built from the cache
+    int    style_slots = 1;        // style slots (DESIGN 4.9); more than slot 0 ("no override") selects the styled kernels
+    int    geo_caches = 1;         // radial: one cache per distinct (fg, bg) pair of the slots; circle: always one
 };
 
-// p: the effective parameters (not the raster view: the tables follow what the K5 pass really did).
-inline RasterTables raster_tables(const glava_b200_params& p, const RasterKnobs& k) {
+// p: the effective parameters (not the raster view: the tables follow what the K5 pass really did), with the largest
+// |AMPLIFY| of the style slots (style_reach_params), so that the box holds every slot's disc.  style_slots / geo_caches:
+// the slots and the radial caches they need; all caches together stay within the 512 MiB of a single one, else the
+// per-pixel radial kernel runs, as for a box that is too big.
+inline RasterTables raster_tables(const glava_b200_params& p, const RasterKnobs& k, int style_slots = 1, int geo_caches = 1) {
     RasterTables t;
+    t.style_slots = style_slots;
+    t.geo_caches = p.module == GLAVA_B200_MOD_RADIAL ? geo_caches : 1;
     // circle: only when the module samples a pre-smoothed texture, i.e. smooth_audio() is a single texelFetch
     if (p.module == GLAVA_B200_MOD_RADIAL || (p.module == GLAVA_B200_MOD_CIRCLE && p.smooth_pass)) {
         const size_t bytes = polar_geo_box(p, t.box);
-        t.geo = bytes > 0 && bytes <= ((size_t) 512 << 20) && !k.no_geo;
+        t.geo = bytes > 0 && bytes * (size_t) t.geo_caches <= ((size_t) 512 << 20) && !k.no_geo;
         t.geo_bytes = t.geo ? bytes : 0;
         // per-tile annulus from bucketed texture min / max (DESIGN 4.2): off by default, GLAVA_B200_CTILE=1 enables it (the
         // curve's halo keeps most tiles of the annulus alive and every live tile pays the bucket reduction)
@@ -132,6 +139,7 @@ struct RasterPlan {
     int  chunk = 1;             // streams per launch
     int  mark_key = 0;          // the dirty-row marks' layout the kernel reads and writes (0: it keeps none)
     int  launches = 0;          // kernel launches of the pass, texmm_kernel included
+    bool styled = false;        // the styled instantiation of the kernels (RasterArgs::style_of / styles are passed)
 };
 
 // threads per row-segment: prefer an exact tiling of w / 4
@@ -187,7 +195,35 @@ inline RasterPlan plan_raster(const glava_b200_params& v, const RasterTables& t,
     // s % slots ends up holding the highest stream mapped to it.
     pl.chunk = slots < 32768 ? (slots > 0 ? slots : 1) : 32768;
     pl.launches = (pl.texmm ? 1 : 0) + ((batch + pl.chunk - 1) / pl.chunk) * (pl.coltab ? 2 : 1);
+    // Styles change no choice above: every kernel reads its stream's slot once per CTA in its styled instantiation, which
+    // keeps the marks of the plain one (zero rows do not depend on colours, and AMPLIFY only moves the rows a frame writes)
+    pl.styled = t.style_slots > 1;
     return pl;
+}
+
+// The module's AMPLIFY field (graph: VSCALE), what a style's `amplify` replaces; nullptr for the test module
+inline float* style_amplify_field(glava_b200_params& p) {
+    switch (p.module) {
+        case GLAVA_B200_MOD_BARS: return &p.bars_amplify;
+        case GLAVA_B200_MOD_RADIAL: return &p.radial_amplify;
+        case GLAVA_B200_MOD_CIRCLE: return &p.circle_amplify;
+        case GLAVA_B200_MOD_GRAPH: return &p.graph_vscale;
+        case GLAVA_B200_MOD_WAVE: return &p.wave_amplify;
+        default: return nullptr;
+    }
+}
+
+// What the polar box is built for: p with the largest |AMPLIFY| of the slots' parameters sp[0 .. slots)
+inline glava_b200_params style_reach_params(const glava_b200_params& p, const glava_b200_params* sp, int slots) {
+    glava_b200_params q = p;
+    float* a = style_amplify_field(q);
+    if (!a) return q;
+    for (int i = 0; i < slots; ++i) {
+        glava_b200_params s = sp[i];
+        const float v = *style_amplify_field(s);
+        if (fabsf(v) > fabsf(*a)) *a = v;
+    }
+    return q;
 }
 
 // Whether the marks describe the framebuffer: the renderer's record `last_key` of the launch that last wrote them (0: none,

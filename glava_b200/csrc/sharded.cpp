@@ -268,6 +268,45 @@ int glava_b200_sharded_load_streams(glava_b200_sharded* g, const int* streams, i
     });
 }
 
+// Per-stream styles (DESIGN 4.9), global stream indices.  Indices and styles are checked for the whole call before any
+// shard starts, so a rejected call touches no shard.
+int glava_b200_sharded_set_stream_styles(glava_b200_sharded* g, const int* streams, int count, const glava_b200_stream_style* styles) {
+    clear_error();
+    const char* who = "glava_b200_sharded_set_stream_styles";
+    if (!g || (count > 0 && !styles)) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
+    std::vector<std::vector<int>> idx; std::vector<std::vector<const char*>> ptr;
+    int rc = group_streams(g, streams, count, (const char*) styles, sizeof(glava_b200_stream_style), who, &idx, &ptr);
+    if (rc) return rc;
+    for (int i = 0; i < count; ++i) {
+        glava_b200_params q;
+        if ((rc = glava_b200_style_params(&g->p, &styles[i], &q)) != 0) return rc;
+    }
+    return broadcast(g, [&](Shard& s) {
+        const size_t k = (size_t) (std::find(g->shards.begin(), g->shards.end(), &s) - g->shards.begin());
+        if (idx[k].empty()) return 0;
+        std::vector<glava_b200_stream_style> st(ptr[k].size());
+        for (size_t i = 0; i < st.size(); ++i) st[i] = *(const glava_b200_stream_style*) ptr[k][i];
+        return glava_b200_set_stream_styles(s.r, idx[k].data(), (int) idx[k].size(), st.data());
+    });
+}
+
+int glava_b200_sharded_get_stream_styles(const glava_b200_sharded* g, const int* streams, int count, glava_b200_stream_style* out) {
+    clear_error();
+    const char* who = "glava_b200_sharded_get_stream_styles";
+    if (!g || (count > 0 && !out)) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
+    glava_b200_sharded* gg = const_cast<glava_b200_sharded*>(g);
+    std::vector<std::vector<int>> idx; std::vector<std::vector<const char*>> ptr;
+    int rc = group_streams(gg, streams, count, (const char*) out, sizeof(glava_b200_stream_style), who, &idx, &ptr);
+    if (rc) return rc;
+    for (size_t k = 0; k < g->shards.size(); ++k) {
+        if (idx[k].empty()) continue;
+        std::vector<glava_b200_stream_style> st(idx[k].size());
+        if ((rc = glava_b200_get_stream_styles(g->shards[k]->r, idx[k].data(), (int) idx[k].size(), st.data())) != 0) return rc;
+        for (size_t i = 0; i < st.size(); ++i) *(glava_b200_stream_style*) ptr[k][i] = st[i];
+    }
+    return 0;
+}
+
 int glava_b200_sharded_textures(glava_b200_sharded* g, uint16_t* out_l, uint16_t* out_r) {
     clear_error();
     if (!g) return fail(GLAVA_B200_EINVAL, "null argument");

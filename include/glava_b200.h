@@ -173,6 +173,22 @@ typedef struct {
                                         rings stay mono.  0 with channels == 1 is treated as 1 (older callers set only channels) */
 } glava_b200_params;
 
+/* Stream style: what one stream of a batch overrides of the renderer's look — the `AMPLIFY` (graph: `VSCALE`) and the
+ * `@fg` / `@bg` colour binds the shipped module configs route their colours through, i.e. what `--pipe fg / bg` binds
+ * give one GLava instance (glava.c:421-436).  `set` is a mask of GLAVA_B200_STYLE_*; a field outside it is ignored.
+ *   amplify  bars_amplify / radial_amplify / circle_amplify / graph_vscale / wave_amplify
+ *   fg       bars_color, radial_color, graph_color (mode 0 or 1; the module's colour program is dropped);
+ *            circle_outline, wave_base_color = fg.lo (mode 1 only).  Mode 1 takes lo, as a constant macro does (hi = lo,
+ *            the gradient is kept)
+ *   bg       bars: bars_outline_mode = 1, bars_outline = bg; radial: radial_outline and radial_bar_outline;
+ *            graph_outline; wave_outline.  circle has no `@bg`
+ * The test module has no style.  fg mode 2, a non-finite amplify, bg on circle, fg without bg on bars whose outline is an
+ * expression (bars_outline_mode 2) and anything validation refuses are GLAVA_B200_EINVAL. */
+#define GLAVA_B200_STYLE_AMPLIFY 1u
+#define GLAVA_B200_STYLE_FG      2u
+#define GLAVA_B200_STYLE_BG      4u
+typedef struct { uint32_t set; float amplify; glava_b200_color fg; float bg[4]; } glava_b200_stream_style;
+
 typedef struct glava_b200 glava_b200;    /* plays the role of struct glava_renderer (render.h:8-30) */
 
 /* Fatal-error hook, the analogue of the `glava_abort` fn-ptr (glava.h:17). NULL restores the default. */
@@ -390,6 +406,31 @@ int glava_b200_load_streams(glava_b200* r, const int* streams, int count, const 
 int glava_b200_sharded_reset_streams(glava_b200_sharded* s, const uint8_t* mask /* [batch], global order */);
 int glava_b200_sharded_save_streams(glava_b200_sharded* s, const int* streams, int count, void* blobs);
 int glava_b200_sharded_load_streams(glava_b200_sharded* s, const int* streams, int count, const void* blobs);
+
+/* ---- per-stream looks (DESIGN.md §4.9) --------------------------------------------------------------------------------
+ *   glava_b200_style_params       `base` with the style `s` applied (see glava_b200_stream_style): what a batch-1 renderer
+ *                                 needs to render what a stream of that style renders.  GLAVA_B200_EINVAL for a style
+ *                                 the module cannot take or parameters that fail validation.
+ *   glava_b200_set_stream_styles  gives streams[i] the style styles[i]; a style with set == 0 returns the stream to the
+ *                                 renderer's own look.  From the next raster pass on (a modified = 0 update re-rasters the
+ *                                 old spectrum in the new look), stream s renders, byte for byte, what a batch-1 renderer
+ *                                 created with glava_b200_style_params(current parameters, style of s) renders when fed
+ *                                 the same calls.  Textures and spectra do not depend on styles.  Out-of-range or repeated
+ *                                 indices and any invalid style are GLAVA_B200_EINVAL with nothing changed.  The tables are
+ *                                 rebuilt as on glava_b200_reconfigure, with its out-of-memory behaviour.
+ *   glava_b200_get_stream_styles  the styles of streams[0 .. count), as set (set == 0: none)
+ * Styles belong to the stream slot: glava_b200_reconfigure and glava_b200_sizereq keep them (an unstyled field follows the
+ * new parameters; a reconfigure that would make a style invalid is refused), reset / save / load of streams leave them
+ * alone.  The sharded forms take global stream indices; they check every index and style before any shard starts, but a
+ * shard whose table rebuild then fails (out of memory) is left as glava_b200_set_stream_styles leaves it, while the shards
+ * that succeeded keep their new styles: after such a failure, read the styles back or set them again. */
+int glava_b200_style_params(const glava_b200_params* base, const glava_b200_stream_style* s, glava_b200_params* out);
+/* "#rrggbb" / "#rrggbbaa" -> RGBA floats, rounded as a `--pipe` bind of that text is (GLAVA_B200_EINVAL: not such a colour) */
+int glava_b200_parse_hex_color(const char* text, float rgba[4]);
+int glava_b200_set_stream_styles(glava_b200* r, const int* streams, int count, const glava_b200_stream_style* styles);
+int glava_b200_get_stream_styles(const glava_b200* r, const int* streams, int count, glava_b200_stream_style* out);
+int glava_b200_sharded_set_stream_styles(glava_b200_sharded* s, const int* streams, int count, const glava_b200_stream_style* styles);
+int glava_b200_sharded_get_stream_styles(const glava_b200_sharded* s, const int* streams, int count, glava_b200_stream_style* out);
 
 /* Stage-wise entry points (used by the parity tests; same kernels as the fused path). */
 int glava_b200_smooth_pass(glava_b200* r, const uint16_t* in, uint16_t* out, int count);      /* K5 on HOST [count][n] */
