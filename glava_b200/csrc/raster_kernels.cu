@@ -62,11 +62,15 @@ __device__ __forceinline__ void mark_store(uint32_t* m, int lo, int hi) {
 
 // Stream styles (DESIGN 4.9).  Every raster kernel has a plain and a styled twin.  The styled one copies its stream's
 // StyleSlot (parameters and tables of the slot) into dynamic shared memory once per CTA, before any thread leaves, and reads
-// everything through it; the plain one reads the kernel parameter and RasterArgs' tables as it always has.  Most pairs are
-// two instantiations of one body.  The plain circle, radial-from-cache and column-less wave kernels keep their own text:
-// instantiated from a shared body they compile to other machine code (register allocation, extra branches and
-// instructions; tools/sass_diff.py), and the plain path must stay what it was.  Their styled twins repeat that code with the
-// slot's reads; tests/test_gpu_stream_styles.py holds each twin to the plain kernel of a batch-1 renderer, frame by frame.
+// everything through it; the plain one reads the kernel parameter and RasterArgs' tables as it always has.  Six pairs share
+// one body: five instantiate a body template, and both radial-from-cache kernels call radial_geo_body with their
+// parameters and cache (the kernel's or the slot's).  The plain circle and
+// wave kernels keep their own text, because the plain path must stay what it was: moved into a __forceinline__ body that
+// takes the chosen `p` as an argument, they compile to other machine code under nvcc 12.9 (tools/sass_diff.py):
+// raster_wave_kernel<false, 1> 2968 -> 3040 instructions, raster_circle_kernel 3968 in another schedule.  Passing `a` by
+// value, __restrict__ on `a` / `p`, internal linkage and a body instance per kernel do not change that (DESIGN 4.9).  Their
+// styled twins repeat that code with the slot's reads; tests/test_gpu_stream_styles.py holds each twin to the plain kernel
+// of a batch-1 renderer, frame by frame.
 template <bool STYLED>
 __device__ __forceinline__ const StyleSlot* stream_style(const RasterStyles& sa, int stream) {
     if constexpr (!STYLED) return nullptr;
@@ -944,8 +948,10 @@ int launch_circle_tiles(const glava_b200_params& p, const void* d_geo, const int
 
 // radial from the geometry cache: per pixel one 16-byte load, one compare against the bar's height
 // (160 heights per stream, in shared memory), one select.
-__global__ void __launch_bounds__(128)
-raster_radial_geo_kernel(const __grid_constant__ RasterArgs a, const __grid_constant__ glava_b200_params p, int rows_per_cta) {
+// `geo_cache` is a.geo (plain) or the slot's cache (styled).  `a` is taken by value: taken by reference, the plain kernel
+// compiles to other machine code (DESIGN 4.9).
+__device__ __forceinline__ void radial_geo_body(const RasterArgs a, const glava_b200_params& p, const void* geo_cache,
+                                                int rows_per_cta) {
     __shared__ float vflat[RADIAL_MAX_BARS + 4];        // bar heights, index side * nk + k (== class code - 1)
     __shared__ float vmax_s;                             // tallest bar of this stream
     const int stream = a.stream0 + blockIdx.z;
@@ -981,7 +987,7 @@ raster_radial_geo_kernel(const __grid_constant__ RasterArgs a, const __grid_cons
     }
     uint32_t* fb = reinterpret_cast<uint32_t*>(a.fb) + (size_t) (stream % a.slots) * p.w * p.h;
     const size_t npx = (size_t) a.gw * a.gh;
-    const int4* __restrict__ geo = reinterpret_cast<const int4*>(a.geo);                    // full entries
+    const int4* __restrict__ geo = reinterpret_cast<const int4*>(geo_cache);                // full entries
     const int2* __restrict__ bar8 = reinterpret_cast<const int2*>(geo + npx);               // {lit, dR}
     const unsigned char* __restrict__ code = reinterpret_cast<const unsigned char*>(bar8 + npx);
     const int bxi = x - a.gx0;
@@ -1025,93 +1031,15 @@ raster_radial_geo_kernel(const __grid_constant__ RasterArgs a, const __grid_cons
         store4(fb + (size_t) y * p.w, x, p.w, px);
     }
 }
-// styled twin (DESIGN 4.9): the same code reading its stream's style slot and its colours' cache
-__device__ __forceinline__ void radial_geo_styled_body(const RasterArgs& a, int rows_per_cta, const RasterStyles& sa) {
-    __shared__ float vflat[RADIAL_MAX_BARS + 4];        // bar heights, index side * nk + k (== class code - 1)
-    __shared__ float vmax_s;                             // tallest bar of this stream
-    const int stream = a.stream0 + blockIdx.z;
-    const StyleSlot* const sty = stream_style<true>(sa, stream);
-    const glava_b200_params& p = sty->p;
-    const AudioTex t = make_tex(p, a.tex, stream);
-    const int nk = p.radial_nbars / 2 + 2;               // k = int(|idx| / section) <= NBARS / 2 (+1 for rounding)
-    const int y0 = blockIdx.y * rows_per_cta, y1 = min(p.h, y0 + rows_per_cta);
-    const bool band_live = (y1 > a.gy0) && (y0 < a.gy0 + a.gh);
-    if (band_live) {
-        for (int i = threadIdx.x; i < 2 * nk; i += blockDim.x) {
-            const int side = i / nk, k = i - side * nk;
-            vflat[i] = radial_bar_value(p, t, (side << 16) | k);
-        }
-        __syncthreads();
-        if (threadIdx.x < 32) {                          // tallest bar: nothing beyond C_RADIUS + vmax can be lit
-            float m = 0.0f;
-            for (int i = threadIdx.x; i < 2 * nk; i += 32) m = fmaxf(m, vflat[i]);
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-            if (threadIdx.x == 0) vmax_s = m;
-        }
-        __syncthreads();
-    }
-    const int x = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
-    if (x >= p.w) return;
-    // per-stream reach: a bar pixel is lit only if d - C_RADIUS <= v <= vmax; beyond that (and beyond the ring) the
-    // frame is 0 for THIS stream, so those quads skip the geometry loads (typical spectra reach a third of AMPLIFY)
-    const float rcull = band_live ? p.radial_radius + fmaxf(fmaxf(vmax_s, 0.0f), fabsf(p.radial_line)) + 2.0f : 0.0f;
-    const float ccx = (float) (p.w / 2) - p.radial_off_x, ccy = (float) (p.h / 2) - p.radial_off_y;
-    float qdx; {
-        const float dxa = (float) x - ccx, dxb = (float) (x + 4) - ccx;          // pixel centres are at +0.5: [x, x+4) covers them
-        qdx = (dxa > 0.0f) ? dxa : ((dxb < 0.0f) ? -dxb : 0.0f);
-        qdx = fmaxf(qdx - 1.0f, 0.0f);
-    }
-    uint32_t* fb = reinterpret_cast<uint32_t*>(a.fb) + (size_t) (stream % a.slots) * p.w * p.h;
-    const size_t npx = (size_t) a.gw * a.gh;
-    const int4* __restrict__ geo = reinterpret_cast<const int4*>(sty->geo);   // full entries (the slot's colours)
-    const int2* __restrict__ bar8 = reinterpret_cast<const int2*>(geo + npx);               // {lit, dR}
-    const unsigned char* __restrict__ code = reinterpret_cast<const unsigned char*>(bar8 + npx);
-    const int bxi = x - a.gx0;
-    const bool col_live = bxi >= 0 && bxi < a.gw;        // gx0, gw multiples of 4: the quad is inside or outside as a whole
-    // One row per trip on purpose: batching the loads of 4 rows (more memory-level parallelism per warp)
-    // raises the register count enough to halve the resident warps, and even the pure zero-store rows
-    // outside the box need the occupancy.
-    for (int y = y0; y < y1; ++y) {
-        uint32_t px[4] = { 0u, 0u, 0u, 0u };
-        const int byi = y - a.gy0;
-        const float qdy = fmaxf(fabsf((float) y + 0.5f - ccy) - 1.0f, 0.0f);
-        if (col_live && byi >= 0 && byi < a.gh && qdx * qdx + qdy * qdy <= rcull * rcull) {
-            const size_t at = (size_t) byi * a.gw + bxi;
-            // codes and {lit, dR} are fetched together (independent addresses): one L2 round trip per
-            // row instead of two dependent ones — the row loop is latency x occupancy bound
-            const uint32_t codes = __ldg(reinterpret_cast<const uint32_t*>(code + at));       // 4 pixels
-            const int4 e01 = __ldg(reinterpret_cast<const int4*>(bar8 + at));                 // pixels 0, 1
-            const int4 e23 = __ldg(reinterpret_cast<const int4*>(bar8 + at) + 1);             // pixels 2, 3
-            if (codes != 0u) {
-                const int2 e8[4] = { make_int2(e01.x, e01.y), make_int2(e01.z, e01.w), make_int2(e23.x, e23.y), make_int2(e23.z, e23.w) };
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    const uint32_t c = (codes >> (8 * k)) & 255u;
-                    if (c == 0u) continue;
-                    if (c != 255u) {
-                        const int2 e = e8[k];
-                        if (__int_as_float(e.y) <= vflat[c - 1u]) px[k] = (uint32_t) e.x;
-                    } else {
-                        const int4 e = __ldg(geo + at + k);            // {lit, unlit, dR, bar}
-                        uint32_t v = (uint32_t) e.y;
-                        if (e.w >= 0) {
-                            const int kk = e.w & 0xffff;
-                            const float vb = kk < nk ? vflat[(e.w >> 16) * nk + kk] : radial_bar_value(p, t, e.w);
-                            if (__int_as_float(e.z) <= vb) v = (uint32_t) e.x;
-                        }
-                        px[k] = v;
-                    }
-                }
-            }
-        }
-        store4(fb + (size_t) y * p.w, x, p.w, px);
-    }
+__global__ void __launch_bounds__(128)
+raster_radial_geo_kernel(const __grid_constant__ RasterArgs a, const __grid_constant__ glava_b200_params p, int rows_per_cta) {
+    radial_geo_body(a, p, a.geo, rows_per_cta);
 }
 __global__ void __launch_bounds__(128)
 raster_radial_geo_styled_kernel(const __grid_constant__ RasterArgs a, const __grid_constant__ glava_b200_params, int rows_per_cta,
                                 const __grid_constant__ RasterStyles sa) {
-    radial_geo_styled_body(a, rows_per_cta, sa);
+    const StyleSlot* const sty = stream_style<true>(sa, a.stream0 + blockIdx.z);
+    radial_geo_body(a, sty->p, sty->geo, rows_per_cta);      // the slot's colours' cache
 }
 
 // One launch of a plain kernel or of its styled twin (the style slots as the last parameter, room for a slot's copy as
