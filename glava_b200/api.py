@@ -112,6 +112,18 @@ class StreamStyle(C.Structure):
 STYLE_AMPLIFY, STYLE_FG, STYLE_BG = 1, 2, 4
 
 
+class Export(C.Structure):
+    """glava_b200_export: what one frame export writes — format (EXPORT_RGBA / _BGRA / _NV12), flags (EXPORT_OVER),
+    the RGB8 background of the composite, and the destination's row pitch and NV12 CbCr plane offset (0: pitch * h)"""
+    _fields_ = [("format", C.c_int), ("flags", C.c_uint32), ("background", C.c_uint8 * 4), ("pitch", C.c_size_t),
+                ("uv_offset", C.c_size_t)]
+
+
+EXPORT_RGBA, EXPORT_BGRA, EXPORT_NV12 = 0, 1, 2
+EXPORT_OVER = 1
+EXPORT_FORMATS = {"rgba": EXPORT_RGBA, "bgra": EXPORT_BGRA, "nv12": EXPORT_NV12}
+
+
 _lib = None
 
 
@@ -229,6 +241,9 @@ def lib():
     for f in ("glava_b200_set_stream_styles", "glava_b200_get_stream_styles", "glava_b200_sharded_set_stream_styles",
               "glava_b200_sharded_get_stream_styles"):
         getattr(L, f).argtypes = [vp, vp, i32, vp]
+    L.glava_b200_export_bytes.argtypes = [vp, C.POINTER(Export), C.POINTER(C.c_size_t)]
+    L.glava_b200_export_frames.argtypes = [vp, vp, i32, vp, C.POINTER(Export), vp, vp]
+    L.glava_b200_sharded_export_frames.argtypes = [vp, vp, i32, vp, C.POINTER(Export)]
     _lib = L
     # errors surface as Python exceptions; keep stderr quiet
     _quiet = C.CFUNCTYPE(None, cp)(lambda msg: None)
@@ -385,6 +400,79 @@ class _StreamStyles:
         return [arr[i] for i in range(s.shape[0])]
 
 
+class _FrameExport:
+    """export_frames over the handle's C entry point: destinations as torch tensors (DESIGN 4.10)"""
+
+    def _export_plan(self, streams, fmt, over, background, out, device_of):
+        """-> (stream list, Export, [dst pointers], what to return).  device_of(stream): the CUDA device of a stream's
+        frame.  out: None (allocate), one uint8 tensor [count, rows, ...] whose dim 1 steps by the pitch, or a list of
+        count tensors [rows, ...] with one common pitch; rows = h (RGBA / BGRA) or h * 3 / 2 (NV12)"""
+        import torch
+        s = np.ascontiguousarray(np.asarray(streams, dtype=np.int64).reshape(-1), dtype=np.int32)
+        count = int(s.shape[0])
+        devices = [device_of(int(x)) for x in s]
+        if fmt not in EXPORT_FORMATS:
+            raise ValueError(f"format {fmt!r}: one of {sorted(EXPORT_FORMATS)}")
+        p = self.params
+        nv12 = fmt == "nv12"
+        rows, row_bytes = (p.h * 3 // 2, p.w) if nv12 else (p.h, p.w * 4)
+        desc = Export()
+        desc.format = EXPORT_FORMATS[fmt]
+        desc.flags = EXPORT_OVER if over else 0
+        bg = [int(v) for v in background]
+        assert len(bg) in (3, 4), background
+        desc.background = (C.c_uint8 * 4)(*bg[:3], 0)
+
+        def frame_view(t):
+            return t[:, :row_bytes] if nv12 else t[:, :row_bytes].unflatten(1, (p.w, 4))
+
+        if out is None:
+            pitch = (row_bytes + 15) // 16 * 16
+            if len(set(devices)) <= 1:
+                base = torch.empty((count, rows, pitch), dtype=torch.uint8, device=f"cuda:{devices[0] if devices else 0}")
+                dst = [base.data_ptr() + i * rows * pitch for i in range(count)]
+                result = base[:, :, :row_bytes] if nv12 else base[:, :, :row_bytes].unflatten(2, (p.w, 4))
+            else:
+                bufs = [torch.empty((rows, pitch), dtype=torch.uint8, device=f"cuda:{d}") for d in devices]
+                dst = [b.data_ptr() for b in bufs]
+                result = [frame_view(b) for b in bufs]
+        else:
+            tensors = list(out) if isinstance(out, (list, tuple)) else None
+            if tensors is None:
+                if out.dtype != torch.uint8 or not out.is_cuda or out.dim() < 3 or out.shape[0] != count or out.shape[1] != rows:
+                    raise ValueError(f"out: a uint8 CUDA tensor [{count}, {rows}, ...] (got {out.dtype} {tuple(out.shape)})")
+                pitch = out.stride(1)
+                dst = [out.data_ptr() + i * out.stride(0) for i in range(count)]
+                row = out[0, 0]
+            else:
+                if len(tensors) != count:
+                    raise ValueError(f"out: {count} tensors, got {len(tensors)}")
+                for t in tensors:
+                    if t.dtype != torch.uint8 or not t.is_cuda or t.dim() < 2 or t.shape[0] != rows or t.stride(0) != tensors[0].stride(0):
+                        raise ValueError(f"out: uint8 CUDA tensors [{rows}, ...] with one pitch (got {t.dtype} {tuple(t.shape)})")
+                pitch = tensors[0].stride(0)
+                dst = [t.data_ptr() for t in tensors]
+                row = tensors[0][0]
+            if not row.is_contiguous() or row.numel() < row_bytes:
+                raise ValueError(f"out: every row must hold {row_bytes} contiguous bytes")
+            result = out
+        desc.pitch = pitch
+        desc.uv_offset = pitch * p.h if nv12 else 0
+        return s, desc, (C.c_void_p * max(count, 1))(*dst), result
+
+
+def _event_handle(ev, stream=None):
+    """a cudaEvent_t as an integer (None: none): an integer handle, or a torch.cuda.Event — one that was never recorded is
+    created by recording it on `stream` (None: nothing to wait for)"""
+    if ev is None or isinstance(ev, int):
+        return ev
+    if not ev.cuda_event:
+        if stream is None:
+            return None
+        ev.record(stream)
+    return ev.cuda_event
+
+
 class Pipe:
     """live `--pipe NAME[:TYPE]` binds fed with stdin text (glava.c:338-411, render.c:1846-2100)"""
 
@@ -446,7 +534,7 @@ def pinned_empty(shape, dtype, device=None):
     return np.frombuffer(buf, dtype=dtype).reshape(shape)
 
 
-class Renderer(_StreamState, _StreamStyles):
+class Renderer(_StreamState, _StreamStyles, _FrameExport):
     """Batched renderer handle: the role of struct glava_renderer (render.h:8-30)."""
 
     @property
@@ -636,6 +724,27 @@ class Renderer(_StreamState, _StreamStyles):
     def framebuffer_device(self):
         return self._L.glava_b200_framebuffer_device(self._h)
 
+    def export_frames(self, streams, fmt="rgba", over=False, background=(0, 0, 0), out=None, after=None, done=None):
+        """The current frames of `streams` (repeats allowed) top-down in the caller's device memory (glava_b200_export_frames):
+        fmt "rgba" / "bgra" ([h, w, 4] per frame; over=True composites over `background` as GLava's window shows it) or
+        "nv12" ([h * 3 / 2, w]: Y rows, then interleaved CbCr rows; always composited).  out: see _export_plan; None
+        allocates [count, h, w, 4] / [count, h * 3 / 2, w] (rows padded to a multiple of 16 bytes).  Returns out.
+        after / done: torch.cuda.Event or cudaEvent_t handles — the export waits for `after` on the device and records
+        `done` behind itself.  Left None, the export is ordered after the work already queued on torch's current stream,
+        and that stream waits for the export (the tensors can be used right away)."""
+        import torch
+        s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, lambda stream: self.device)
+        dev = torch.device("cuda", self.device)
+        cur = torch.cuda.current_stream(dev)
+        own = torch.cuda.ExternalStream(self.cuda_stream, device=dev)
+        if after is None:
+            own.wait_stream(cur)
+        _check(self._L.glava_b200_export_frames(self._h, s.ctypes.data, s.shape[0], dst, C.byref(desc),
+                                                _event_handle(after), _event_handle(done, cur)))
+        if done is None:
+            cur.wait_stream(own)
+        return result
+
     @property
     def cuda_stream(self):
         return self._L.glava_b200_cuda_stream(self._h)
@@ -667,7 +776,7 @@ class Renderer(_StreamState, _StreamStyles):
         except Exception: pass
 
 
-class ShardedRenderer(_StreamState, _StreamStyles):
+class ShardedRenderer(_StreamState, _StreamStyles, _FrameExport):
     """One handle for a batch spread over several GPUs of a node (glava_b200_new_sharded): contiguous stream blocks, one
     worker thread per device, no inter-device traffic.  devices: list of CUDA ordinals (may repeat), or None = all visible.
     reset_streams / save_streams / load_streams take global stream indices."""
@@ -735,6 +844,26 @@ class ShardedRenderer(_StreamState, _StreamStyles):
         l = np.empty((self.batch, n), dtype=np.uint16); r = np.empty_like(l)
         _check(self._L.glava_b200_sharded_textures(self._h, l.ctypes.data, r.ctypes.data))
         return l, r
+
+    def export_frames(self, streams, fmt="rgba", over=False, background=(0, 0, 0), out=None):
+        """Renderer.export_frames with global stream indices (glava_b200_sharded_export_frames): each destination on the
+        device of the shard that owns its stream (out None: one tensor when every listed stream lives on one device, else
+        a list of per-frame tensors).  Work queued on torch's current streams of those devices is waited for first; the
+        frames are complete after sync()."""
+        import torch
+        shards = self.shards
+
+        def device_of(stream):
+            for d, first, cnt in shards:
+                if first <= stream < first + cnt:
+                    return d
+            return shards[0][0]
+
+        s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, device_of)
+        for d in sorted({device_of(int(x)) for x in s}):
+            torch.cuda.current_stream(d).synchronize()
+        _check(self._L.glava_b200_sharded_export_frames(self._h, s.ctypes.data, s.shape[0], dst, C.byref(desc)))
+        return result
 
     def close(self):
         if getattr(self, "_h", None):

@@ -175,6 +175,9 @@ struct glava_b200 {
     // copies are done
     DevBuf<char> d_sst[2]; PinnedBuf<int> h_sst[2]; Event ev_sst_copied[2], ev_sst_free[2];
     int sst_cur = 0, sst_streams = 0; size_t sst_table = 0;
+    // state another source file keeps per renderer (export.cpp: the frame export's list buffers), created on its first use
+    // through renderer_view and released by attach_free once the streams are drained (glava_b200_destroy)
+    void* attach = nullptr; void (*attach_free)(void*) = nullptr;
     uint64_t launches = 0;
     // optional per-kernel device timing (glava_b200_set_timing): events around each launch
     bool timing = false;
@@ -724,6 +727,7 @@ void glava_b200_destroy(glava_b200* r) {
     cudaSetDevice(r->device);
     for (cudaStream_t s : { r->spec_stream, r->stream.get(), r->copy_stream.get(), r->out_stream.get() })
         if (s) cudaStreamSynchronize(s);
+    if (r->attach_free) r->attach_free(r->attach);
     delete r;
 }
 
@@ -1559,3 +1563,16 @@ int glava_b200_get_stream_styles(const glava_b200* r, const int* streams, int co
 }
 
 }  // extern "C"
+
+
+// ---- what export.cpp reads of a renderer (DESIGN 4.10) -------------------------------------------------------------------
+namespace glb {
+RendererView renderer_view(glava_b200* r) {
+    RendererView v;
+    v.built = r->built; v.device = r->device; v.batch = r->batch; v.slots = r->slots;
+    v.w = r->d.p.w; v.h = r->d.p.h; v.native = r->d.p.premultiply_alpha != 0; v.mark_key = r->mark_key;
+    v.stream = r->stream; v.fb = r->frame.fb; v.marks = r->frame.marks;
+    v.launches = &r->launches; v.attach = &r->attach; v.attach_free = &r->attach_free;
+    return v;
+}
+}  // namespace glb

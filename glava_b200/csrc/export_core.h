@@ -1,0 +1,105 @@
+// export_core.h — the pixel arithmetic of glava_b200_export_frames (DESIGN 4.10) as __host__ __device__ functions: the
+// composite over an opaque background, RGB -> BT.709 limited-range Y / Cb / Cr in integer fixed point, the 2x2 chroma
+// average, and which framebuffer rows the dirty-row marks say must be read.  export_kernels.cu and the host test tier
+// (tests/test_export_core.py) compile this same code.
+#ifndef GLAVA_B200_EXPORT_CORE_H
+#define GLAVA_B200_EXPORT_CORE_H
+
+#include "raster_core.h"
+
+namespace glb {
+
+// What one export call does to every pixel: the public format, whether it composites, the renderer's opacity
+// (premultiply_alpha != 0: native, the frame is premultiplied over a transparent target) and the background 0x00BBGGRR
+struct ExportFmt {
+    int      format;            // GLAVA_B200_EXPORT_RGBA / _BGRA / _NV12
+    int      over;              // composite (always for NV12)
+    int      native;
+    uint32_t bg;
+};
+
+// ---- composite ---------------------------------------------------------------------------------------------------------
+// The opaque colour GLava's window shows for a stored pixel (R in the low byte).  Native opacity: the premultiplied pixel
+// over `bg`, C = min(255, c + mul_norm8(bg, 255 - a)) per channel, the unorm8 product the blend path uses (raster_core.h).
+// Any other opacity: the window ignores alpha, the colour is as stored.  Alpha becomes 255.
+GLB_HD uint32_t export_over(uint32_t px, uint32_t bg, int native) {
+    if (!native) return px | 0xff000000u;
+    const uint32_t ia = 255u - (px >> 24);
+    uint32_t out = 0xff000000u;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const uint32_t v = ((px >> (8 * c)) & 255u) + mul_norm8((bg >> (8 * c)) & 255u, ia);
+        out |= (v > 255u ? 255u : v) << (8 * c);
+    }
+    return out;
+}
+GLB_HD uint32_t export_swap_rb(uint32_t px) { return (px & 0xff00ff00u) | ((px & 0xffu) << 16) | ((px >> 16) & 0xffu); }
+// one RGBA / BGRA output pixel
+GLB_HD uint32_t export_px(const ExportFmt& f, uint32_t px) {
+    if (f.over) px = export_over(px, f.bg, f.native);
+    return f.format == GLAVA_B200_EXPORT_BGRA ? export_swap_rb(px) : px;
+}
+
+// ---- BT.709, limited range ---------------------------------------------------------------------------------------------
+// Kr = 0.2126, Kb = 0.0722; Y' = Kr R + Kg G + Kb B, Y = 16 + 219/255 Y', Cb = 128 + 224/255 (B - Y') / (2 (1 - Kb)),
+// Cr = 128 + 224/255 (R - Y') / (2 (1 - Kr)).  Coefficients scaled by 2^16 and rounded; the blue coefficient of Cb and the
+// red one of Cr are minus the sum of the other two, so every grey has Cb = Cr = 128 exactly.  Black gives (16, 128, 128),
+// white (235, 128, 128); over all 2^24 colours the result is within 0.503 code values of the float64 formula.
+#define GLB_YUV_SHIFT 16
+#define GLB_YUV_HALF (1 << (GLB_YUV_SHIFT - 1))
+#define GLB_Y_R 11966
+#define GLB_Y_G 40254
+#define GLB_Y_B 4064
+#define GLB_CB_R (-6596)
+#define GLB_CB_G (-22189)
+#define GLB_CB_B (-(GLB_CB_R + GLB_CB_G))
+#define GLB_CR_G (-26145)
+#define GLB_CR_B (-2639)
+#define GLB_CR_R (-(GLB_CR_G + GLB_CR_B))
+GLB_HD uint32_t export_y(uint32_t c) {
+    const int r = (int) (c & 255u), g = (int) ((c >> 8) & 255u), b = (int) ((c >> 16) & 255u);
+    return (uint32_t) ((GLB_Y_R * r + GLB_Y_G * g + GLB_Y_B * b + (16 << GLB_YUV_SHIFT) + GLB_YUV_HALF) >> GLB_YUV_SHIFT);
+}
+// (Cb, Cr) as the two bytes of NV12's interleaved plane: Cb low, Cr high
+GLB_HD uint32_t export_cbcr(uint32_t c) {
+    const int r = (int) (c & 255u), g = (int) ((c >> 8) & 255u), b = (int) ((c >> 16) & 255u);
+    const int cb = (GLB_CB_R * r + GLB_CB_G * g + GLB_CB_B * b + (128 << GLB_YUV_SHIFT) + GLB_YUV_HALF) >> GLB_YUV_SHIFT;
+    const int cr = (GLB_CR_R * r + GLB_CR_G * g + GLB_CR_B * b + (128 << GLB_YUV_SHIFT) + GLB_YUV_HALF) >> GLB_YUV_SHIFT;
+    return (uint32_t) cb | ((uint32_t) cr << 8);
+}
+// The chroma sample of a 2x2 block: the per-channel average (s + 2) >> 2 of its four composited pixels
+GLB_HD uint32_t export_avg4(uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+    uint32_t out = 0;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        const uint32_t s = ((a >> (8 * k)) & 255u) + ((b >> (8 * k)) & 255u) + ((c >> (8 * k)) & 255u) + ((d >> (8 * k)) & 255u);
+        out |= ((s + 2u) >> 2) << (8 * k);
+    }
+    return out;
+}
+// NV12 of a quad of output rows 2j (top) and 2j + 1 (bot): four Y bytes per row, and the (Cb, Cr) pairs of the quad's two
+// 2x2 blocks as one little-endian word (Cb0, Cr0, Cb1, Cr1)
+GLB_HD uint32_t export_nv12_quad(const ExportFmt& f, const uint32_t top[4], const uint32_t bot[4], uint32_t* y_top, uint32_t* y_bot) {
+    uint32_t t[4], b[4];
+    *y_top = 0u; *y_bot = 0u;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        t[k] = export_over(top[k], f.bg, f.native);
+        b[k] = export_over(bot[k], f.bg, f.native);
+        *y_top |= export_y(t[k]) << (8 * k);
+        *y_bot |= export_y(b[k]) << (8 * k);
+    }
+    return export_cbcr(export_avg4(t[0], t[1], b[0], b[1])) | (export_cbcr(export_avg4(t[2], t[3], b[2], b[3])) << 16);
+}
+
+// ---- mark-aware reads ----------------------------------------------------------------------------------------------------
+// When the last raster pass kept dirty-row marks (capi.cu mark_key != 0), slot s of the framebuffer has one word per (band of
+// `rows` rows, 128-pixel strip) at the band's first row (raster_core.h dirty_pack): rows [lo, hi) of the band may be non-zero,
+// every other row of it is 0 in memory.  The export reads a row of a strip only when its band's word says so.
+GLB_HD size_t export_mark_index(int slot, int w, int h, int rows, int y, int strip) {
+    return ((size_t) slot * h + (size_t) (y - y % rows)) * (size_t) ((w + 127) >> 7) + (size_t) strip;
+}
+GLB_HD bool export_row_read(uint32_t mark, int y) { return y >= (int) (mark & 0xffffu) && y < (int) (mark >> 16); }
+
+}  // namespace glb
+#endif

@@ -1,0 +1,106 @@
+// export_kernels.cu — glava_b200_export_frames (capi.cu, DESIGN 4.10): the current frames of a list of streams, flipped
+// top-down and written as RGBA / BGRA (optionally composited) or NV12 into the caller's device buffers.
+//
+// One launch per call.  The list (destination, framebuffer slot) reaches the device in one small copy; the grid is
+// flattened over (listed entry, output row pair, 128-pixel strip) on grid.x only, one warp per item, so any list length
+// and frame size fit.  A thread owns a quad of pixels on both rows of its pair: two 16-byte loads, then two 16-byte
+// streaming stores (RGBA / BGRA) or two 4-byte Y stores and one 4-byte CbCr store (NV12).  With dirty-row marks the warp
+// reads only the rows its strip's band words say may be non-zero (export_core.h); every other row is zero pixels that are
+// never loaded.  Widths that are not a multiple of 4 take a per-pixel tail.
+#include "internal.h"
+#include "export_core.h"
+
+#include <cuda_runtime.h>
+
+namespace glb {
+
+// whether row y of the strip must be read (false: it is all zero in memory)
+__device__ __forceinline__ bool row_read(const ExportArgs& a, int slot, int y, int strip) {
+    if (!a.marks) return true;
+    return export_row_read(__ldg(a.marks + export_mark_index(slot, a.w, a.h, a.mark_rows, y, strip)), y);
+}
+
+// the quad at x of framebuffer row y (pixels past the right edge read as 0)
+__device__ __forceinline__ void load_quad(const ExportArgs& a, const uint32_t* frame, int y, int x, uint32_t px[4]) {
+    const uint32_t* row = frame + (size_t) y * a.w;
+    if ((a.w & 3) == 0) {                                   // rows are 16-byte aligned
+        const uint4 v = __ldcs(reinterpret_cast<const uint4*>(row + x));
+        px[0] = v.x; px[1] = v.y; px[2] = v.z; px[3] = v.w;
+    } else {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) px[k] = x + k < a.w ? __ldcs(row + x + k) : 0u;
+    }
+}
+
+// zpx: what a zero pixel becomes (a quad of zero pixels skips the per-pixel arithmetic)
+__device__ __forceinline__ void store_rgba(const ExportFmt& f, uint8_t* row, int x, int w, const uint32_t in[4], uint32_t zpx) {
+    uint32_t px[4] = { zpx, zpx, zpx, zpx };
+    if ((in[0] | in[1] | in[2] | in[3]) != 0u) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) px[k] = export_px(f, in[k]);
+    }
+    uint32_t* out = reinterpret_cast<uint32_t*>(row) + x;
+    if (x + 4 <= w) __stcs(reinterpret_cast<uint4*>(out), make_uint4(px[0], px[1], px[2], px[3]));   // pitch and dst: multiples of 16
+    else
+        for (int k = 0; k < 4 && x + k < w; ++k) __stcs(out + k, px[k]);
+}
+
+template <typename Index>
+__global__ void __launch_bounds__(256) export_kernel(const __grid_constant__ ExportArgs a) {
+    const ExportFmt f = { a.format, a.over, a.native, a.bg };
+    const Index strips = (Index) ((a.w + 127) >> 7), per = strips * (Index) ((a.h + 1) >> 1);
+    const Index items = (Index) a.count * per;
+    const Index warps = (Index) (((size_t) gridDim.x * blockDim.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    // what zero pixels become: most of a frame is zero rows the marks skip, and most of the rest is zero pixels
+    const uint32_t zero4[4] = { 0u, 0u, 0u, 0u };
+    uint32_t zy, zy1;
+    const uint32_t zuv = export_nv12_quad(f, zero4, zero4, &zy, &zy1), zpx = export_px(f, 0u);
+    for (Index it = (Index) (((size_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5); it < items; it += warps) {
+        const Index k = it / per, rem = it - k * per;
+        const int j = (int) (rem / strips), strip = (int) (rem - (Index) j * strips);
+        const int x = strip * 128 + lane * 4;
+        if (x >= a.w) continue;
+        const ExportEntry* e = a.list + k;
+        uint8_t* const dst = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst)));
+        const int slot = __ldg(&e->slot);
+        const uint32_t* frame = reinterpret_cast<const uint32_t*>(a.fb) + (size_t) slot * a.h * a.w;
+        // output rows 2j and 2j + 1 are framebuffer rows h - 1 - 2j and h - 2 - 2j
+        const int y0 = a.h - 1 - 2 * j, y1 = y0 - 1;
+        uint32_t top[4] = { 0u, 0u, 0u, 0u }, bot[4] = { 0u, 0u, 0u, 0u };
+        if (row_read(a, slot, y0, strip)) load_quad(a, frame, y0, x, top);
+        if (y1 >= 0 && row_read(a, slot, y1, strip)) load_quad(a, frame, y1, x, bot);
+        uint8_t* const r0 = dst + (size_t) (2 * j) * a.pitch;
+        if (a.format == GLAVA_B200_EXPORT_NV12) {           // h even: both rows exist
+            uint32_t yt = zy, yb = zy, uv = zuv;
+            if ((top[0] | top[1] | top[2] | top[3] | bot[0] | bot[1] | bot[2] | bot[3]) != 0u) uv = export_nv12_quad(f, top, bot, &yt, &yb);
+            uint8_t* const pu = dst + a.uv_offset + (size_t) j * a.pitch + x;
+            if (x + 4 <= a.w) {
+                __stcs(reinterpret_cast<uint32_t*>(r0 + x), yt);
+                __stcs(reinterpret_cast<uint32_t*>(r0 + a.pitch + x), yb);
+                __stcs(reinterpret_cast<uint32_t*>(pu), uv);
+            } else {                                        // w even: the last two pixels of a row
+                __stcs(reinterpret_cast<unsigned short*>(r0 + x), (unsigned short) yt);
+                __stcs(reinterpret_cast<unsigned short*>(r0 + a.pitch + x), (unsigned short) yb);
+                __stcs(reinterpret_cast<unsigned short*>(pu), (unsigned short) uv);
+            }
+        } else {
+            store_rgba(f, r0, x, a.w, top, zpx);
+            if (y1 >= 0) store_rgba(f, r0 + a.pitch, x, a.w, bot, zpx);
+        }
+    }
+}
+
+int launch_export(const ExportArgs& a, void* stream) {
+    const uint64_t items = (uint64_t) a.count * (uint64_t) ((a.w + 127) >> 7) * (uint64_t) ((a.h + 1) >> 1);
+    const uint64_t blocks = (items + 7) / 8;                // 8 warps per CTA
+    const unsigned grid = blocks < 132u * 16u ? (unsigned) (blocks ? blocks : 1) : 132u * 16u;   // grid-stride beyond 16 CTAs per SM of an H100 SXM
+    // 32-bit item arithmetic whenever the item count allows (every realistic list: 1024 1080p frames are 8.3 M items)
+    if (items + ((uint64_t) grid << 3) < (1ull << 32)) export_kernel<uint32_t><<<grid, 256, 0, (cudaStream_t) stream>>>(a);
+    else export_kernel<uint64_t><<<grid, 256, 0, (cudaStream_t) stream>>>(a);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(GLAVA_B200_ECUDA, "export kernel launch: %s", cudaGetErrorString(e));
+    return 0;
+}
+
+}  // namespace glb

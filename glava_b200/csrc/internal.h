@@ -188,6 +188,39 @@ int launch_upload(const float* d_s, const float* d_e, float mod, uint16_t* d_out
 struct StateLayout; struct StatePtrs;
 int launch_state_pack(const StateLayout& L, const StatePtrs& P, const int* d_table, int count, void* d_out, void* stream);
 int launch_state_unpack(const StateLayout& L, const StatePtrs& P, const int* d_table, int count, const void* d_in, void* stream);
+// export_kernels.cu: glava_b200_export_frames (DESIGN 4.10), one launch for the whole list.  The list ([count] entries)
+// is in device memory; marks == nullptr (or mark_rows == 0) reads every framebuffer row, else only the rows the marks say
+// may be non-zero (export_core.h)
+struct alignas(16) ExportEntry {
+    uint8_t* dst;               // the caller's destination
+    int      slot;              // framebuffer slot of the listed stream (stream % slots)
+    int      pad;
+};
+struct ExportArgs {
+    const uint8_t*  fb;         // [slots][h][w] RGBA8
+    const uint32_t* marks;      // dirty-row marks of the last raster pass, or nullptr
+    int             mark_rows;  // their band height
+    const ExportEntry* list;
+    int    count, w, h;
+    int    format, over, native;  // export_core.h ExportFmt
+    uint32_t bg;
+    size_t pitch, uv_offset;
+};
+int launch_export(const ExportArgs& a, void* stream);
+// capi.cu, for export.cpp: what the frame export reads of a renderer, and the slot where it keeps its own per-renderer
+// state (*attach, released by *attach_free when the renderer is destroyed)
+struct RendererView {
+    bool built;
+    int  device, batch, slots, w, h, native, mark_key;   // native: premultiply_alpha; mark_key: capi.cu's record of the marks
+    void* stream;                                        // the raster stream (cudaStream_t)
+    const uint8_t* fb; const uint32_t* marks;
+    uint64_t* launches;
+    void** attach; void (**attach_free)(void*);
+};
+RendererView renderer_view(glava_b200* r);
+// export.cpp, for sharded.cpp: every refusal of glava_b200_export_frames that does not depend on the other shards (nothing
+// is enqueued)
+int export_check(glava_b200* r, const int* streams, int count, void* const* dst, const glava_b200_export* desc, const char* who);
 // capi.cu, for sharded.cpp: the blob checks of glava_b200_load_streams (nothing is touched), and save / load with one
 // host pointer per listed stream (the blobs of one shard's streams are not contiguous in the caller's array)
 int state_check_blobs(const glava_b200* r, const void* const* blobs, int count, const char* who);

@@ -350,6 +350,50 @@ void* glava_b200_frame_event(const glava_b200* r);
 const void* glava_b200_frame_device(const glava_b200* r, int stream);
 int   glava_b200_framebuffer_ipc(glava_b200* r, void* handle, size_t handle_bytes);
 
+/* Frame export into the caller's DEVICE buffers (DESIGN.md §4.10), for a consumer that wants frames top-down, opaque or in
+ * NV12 (a compositor's surface, an encoder's input) without writing its own flip / composite / convert pass.
+ *   glava_b200_export_frames   converts the current frame of streams[i] — exactly what glava_b200_readback(streams[i])
+ *                              would return at this point in call order, framebuffer ring included — into dst[i]
+ *                              (a device pointer on the renderer's device; streams may repeat).  Every format is
+ *                              top-down: output row 0 is framebuffer row h - 1.
+ *     GLAVA_B200_EXPORT_RGBA   h rows of w * 4 bytes R,G,B,A, `pitch` bytes apart
+ *     GLAVA_B200_EXPORT_BGRA   the same as B,G,R,A (what compositors and NVENC's ARGB input take)
+ *     GLAVA_B200_EXPORT_NV12   Y plane of h rows x w bytes, then the interleaved CbCr plane of h / 2 rows x w bytes at
+ *                              `uv_offset` (0: pitch * h); BT.709 limited range in 16-bit fixed point (export_core.h),
+ *                              chroma from the per-channel average (s + 2) >> 2 of each composited 2x2 block; w and h even
+ *   GLAVA_B200_EXPORT_OVER     (implied for NV12) the opaque colour GLava's window shows over `background` (RGB8,
+ *                              byte 3 unused): under setopacity "native" (premultiply_alpha) C = min(255, c +
+ *                              mul_norm8(bg, 255 - a)) per channel; under any other opacity the stored colour (the window
+ *                              ignores alpha and the clear colour already stands in for the desktop).  Alpha becomes 255.
+ *                              Without it RGBA / BGRA carry the stored pixels, alpha included.
+ *   dst[i], pitch and uv_offset are multiples of 16, pitch >= the row bytes, uv_offset (when set) >= pitch * h.  An unknown
+ *   format or flag, odd NV12 dimensions, a misaligned or short pitch, a null, host or other-device dst, a stream out of
+ *   range, count < 1 and a renderer a failed rebuild left unbuilt are GLAVA_B200_EINVAL with nothing enqueued.
+ *   The work runs on the handle's stream (glava_b200_cuda_stream) after the latest raster pass and before the next one can
+ *   overwrite a slot, so an update issued right after this call cannot change what it exports.  `after_event` (a
+ *   cudaEvent_t, or NULL): the export waits for it on the device before writing the destinations — it holds back the
+ *   handle's stream, and so the next raster pass, until then.  `done_event` (or NULL) is recorded after the export.
+ *   Returns once the work is enqueued, without a host wait.
+ *   glava_b200_export_bytes    the bytes one destination spans for `desc` on this renderer (pitch * h; NV12: uv_offset +
+ *                              pitch * h / 2), after the same descriptor checks.
+ *   glava_b200_sharded_export_frames  the same with global stream indices, dst[i] on the device of the shard that owns
+ *                              streams[i]; every index and pointer is checked before any shard starts, the shards issue
+ *                              concurrently, and glava_b200_sharded_sync completes the work. */
+#define GLAVA_B200_EXPORT_RGBA 0
+#define GLAVA_B200_EXPORT_BGRA 1
+#define GLAVA_B200_EXPORT_NV12 2
+#define GLAVA_B200_EXPORT_OVER 1u
+typedef struct {
+    int      format;            /* GLAVA_B200_EXPORT_RGBA / _BGRA / _NV12 */
+    uint32_t flags;             /* GLAVA_B200_EXPORT_OVER */
+    uint8_t  background[4];     /* R, G, B of the opaque background the composite uses; byte 3 unused */
+    size_t   pitch;             /* bytes from one output row to the next (both NV12 planes) */
+    size_t   uv_offset;         /* NV12: bytes from dst[i] to the CbCr plane, 0 = pitch * h */
+} glava_b200_export;
+int glava_b200_export_bytes(const glava_b200* r, const glava_b200_export* desc, size_t* bytes);
+int glava_b200_export_frames(glava_b200* r, const int* streams, int count, void* const* dst,
+                             const glava_b200_export* desc, void* after_event, void* done_event);
+
 /* ---- one handle for a batch spread over several GPUs of a node (csrc/sharded.cpp) -------------------------------------
  * The streams of a batch are independent (one GLava process each, in the reference), so the batch is cut into contiguous
  * blocks, one per device — glava_b200_shard_range: counts differ by at most one — and nothing crosses between devices (no
@@ -374,6 +418,8 @@ int  glava_b200_sharded_sync(glava_b200_sharded* s);
 int  glava_b200_sharded_readback(glava_b200_sharded* s, int stream, uint8_t* rgba);
 const void* glava_b200_sharded_frame_device(glava_b200_sharded* s, int stream, int* device);
 int  glava_b200_sharded_textures(glava_b200_sharded* s, uint16_t* out_l, uint16_t* out_r);
+int  glava_b200_sharded_export_frames(glava_b200_sharded* s, const int* streams, int count, void* const* dst,
+                                      const glava_b200_export* desc);   /* global indices; see glava_b200_export_frames */
 
 /* ---- lifetime of individual streams: reset, save and load (DESIGN.md §4.8) -------------------------------------------
  * A stream's state is what its next update reads besides its new audio: gravity store and average ring, the latest
