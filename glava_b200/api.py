@@ -119,6 +119,13 @@ class Export(C.Structure):
                 ("uv_offset", C.c_size_t)]
 
 
+class ExportScale(C.Structure):
+    """glava_b200_export_scale: the source rectangle of a scaled export, top-down (all zero: the whole frame), and the
+    output size"""
+    _fields_ = [("src_x", C.c_int), ("src_y", C.c_int), ("src_w", C.c_int), ("src_h", C.c_int), ("out_w", C.c_int),
+                ("out_h", C.c_int)]
+
+
 EXPORT_RGBA, EXPORT_BGRA, EXPORT_NV12 = 0, 1, 2
 EXPORT_OVER = 1
 EXPORT_FORMATS = {"rgba": EXPORT_RGBA, "bgra": EXPORT_BGRA, "nv12": EXPORT_NV12}
@@ -244,6 +251,9 @@ def lib():
     L.glava_b200_export_bytes.argtypes = [vp, C.POINTER(Export), C.POINTER(C.c_size_t)]
     L.glava_b200_export_frames.argtypes = [vp, vp, i32, vp, C.POINTER(Export), vp, vp]
     L.glava_b200_sharded_export_frames.argtypes = [vp, vp, i32, vp, C.POINTER(Export)]
+    L.glava_b200_export_scaled_bytes.argtypes = [vp, C.POINTER(Export), C.POINTER(ExportScale), C.POINTER(C.c_size_t)]
+    L.glava_b200_export_scaled.argtypes = [vp, vp, i32, vp, vp, C.POINTER(Export), C.POINTER(ExportScale), vp, vp]
+    L.glava_b200_sharded_export_scaled.argtypes = [vp, vp, i32, vp, vp, C.POINTER(Export), C.POINTER(ExportScale)]
     _lib = L
     # errors surface as Python exceptions; keep stderr quiet
     _quiet = C.CFUNCTYPE(None, cp)(lambda msg: None)
@@ -403,35 +413,30 @@ class _StreamStyles:
 class _FrameExport:
     """export_frames over the handle's C entry point: destinations as torch tensors (DESIGN 4.10)"""
 
-    def _export_plan(self, streams, fmt, over, background, out, device_of):
+    def _export_plan(self, streams, fmt, over, background, out, device_of, size=None):
         """-> (stream list, Export, [dst pointers], what to return).  device_of(stream): the CUDA device of a stream's
-        frame.  out: None (allocate), one uint8 tensor [count, rows, ...] whose dim 1 steps by the pitch, or a list of
-        count tensors [rows, ...] with one common pitch; rows = h (RGBA / BGRA) or h * 3 / 2 (NV12)"""
+        frame.  size: (w, h) of each output, None: the frame's.  out: None (allocate), one uint8 tensor [count, rows, ...]
+        whose dim 1 steps by the pitch, or a list of count tensors [rows, ...] with one common pitch; rows = h (RGBA / BGRA)
+        or h * 3 / 2 (NV12)"""
         import torch
         s = np.ascontiguousarray(np.asarray(streams, dtype=np.int64).reshape(-1), dtype=np.int32)
         count = int(s.shape[0])
         devices = [device_of(int(x)) for x in s]
-        if fmt not in EXPORT_FORMATS:
-            raise ValueError(f"format {fmt!r}: one of {sorted(EXPORT_FORMATS)}")
         p = self.params
+        w, h = (p.w, p.h) if size is None else (int(size[0]), int(size[1]))
         nv12 = fmt == "nv12"
-        rows, row_bytes = (p.h * 3 // 2, p.w) if nv12 else (p.h, p.w * 4)
-        desc = Export()
-        desc.format = EXPORT_FORMATS[fmt]
-        desc.flags = EXPORT_OVER if over else 0
-        bg = [int(v) for v in background]
-        assert len(bg) in (3, 4), background
-        desc.background = (C.c_uint8 * 4)(*bg[:3], 0)
+        rows, row_bytes = (h * 3 // 2, w) if nv12 else (h, w * 4)
+        desc = _export_desc(fmt, over, background)
 
         def frame_view(t):
-            return t[:, :row_bytes] if nv12 else t[:, :row_bytes].unflatten(1, (p.w, 4))
+            return t[:, :row_bytes] if nv12 else t[:, :row_bytes].unflatten(1, (w, 4))
 
         if out is None:
             pitch = (row_bytes + 15) // 16 * 16
             if len(set(devices)) <= 1:
                 base = torch.empty((count, rows, pitch), dtype=torch.uint8, device=f"cuda:{devices[0] if devices else 0}")
                 dst = [base.data_ptr() + i * rows * pitch for i in range(count)]
-                result = base[:, :, :row_bytes] if nv12 else base[:, :, :row_bytes].unflatten(2, (p.w, 4))
+                result = base[:, :, :row_bytes] if nv12 else base[:, :, :row_bytes].unflatten(2, (w, 4))
             else:
                 bufs = [torch.empty((rows, pitch), dtype=torch.uint8, device=f"cuda:{d}") for d in devices]
                 dst = [b.data_ptr() for b in bufs]
@@ -457,8 +462,29 @@ class _FrameExport:
                 raise ValueError(f"out: every row must hold {row_bytes} contiguous bytes")
             result = out
         desc.pitch = pitch
-        desc.uv_offset = pitch * p.h if nv12 else 0
+        desc.uv_offset = pitch * h if nv12 else 0
         return s, desc, (C.c_void_p * max(count, 1))(*dst), result
+
+
+def _export_desc(fmt, over, background):
+    """the Export descriptor of a format name, the composite flag and an RGB(A) background (pitch and uv_offset 0)"""
+    if fmt not in EXPORT_FORMATS:
+        raise ValueError(f"format {fmt!r}: one of {sorted(EXPORT_FORMATS)}")
+    desc = Export()
+    desc.format = EXPORT_FORMATS[fmt]
+    desc.flags = EXPORT_OVER if over else 0
+    bg = [int(v) for v in background]
+    assert len(bg) in (3, 4), background
+    desc.background = (C.c_uint8 * 4)(*bg[:3], 0)
+    return desc
+
+
+def _export_scale(size, crop):
+    """the ExportScale of an output size (w, h) and a crop (x, y, w, h) in top-down coordinates (None: the whole frame)"""
+    sc = ExportScale()
+    sc.src_x, sc.src_y, sc.src_w, sc.src_h = (0, 0, 0, 0) if crop is None else (int(v) for v in crop)
+    sc.out_w, sc.out_h = (int(v) for v in size)
+    return sc
 
 
 def _event_handle(ev, stream=None):
@@ -732,17 +758,70 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
         after / done: torch.cuda.Event or cudaEvent_t handles — the export waits for `after` on the device and records
         `done` behind itself.  Left None, the export is ordered after the work already queued on torch's current stream,
         and that stream waits for the export (the tensors can be used right away)."""
-        import torch
         s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, lambda stream: self.device)
+        self._ordered(lambda a, d: self._L.glava_b200_export_frames(self._h, s.ctypes.data, s.shape[0], dst, C.byref(desc), a, d),
+                      after, done)
+        return result
+
+    def _ordered(self, call, after, done):
+        """call(after_event, done_event) on the handle's stream, ordered against torch's current stream as export_frames
+        describes"""
+        import torch
         dev = torch.device("cuda", self.device)
         cur = torch.cuda.current_stream(dev)
         own = torch.cuda.ExternalStream(self.cuda_stream, device=dev)
         if after is None:
             own.wait_stream(cur)
-        _check(self._L.glava_b200_export_frames(self._h, s.ctypes.data, s.shape[0], dst, C.byref(desc),
-                                                _event_handle(after), _event_handle(done, cur)))
+        _check(call(_event_handle(after), _event_handle(done, cur)))
         if done is None:
             cur.wait_stream(own)
+
+    def export_scaled(self, streams, size, crop=None, fmt="rgba", over=False, background=(0, 0, 0), out=None, after=None,
+                      done=None):
+        """export_frames of a source rectangle shrunk to size = (w, h) by the exact area average (glava_b200_export_scaled):
+        crop = (x, y, w, h) in top-down coordinates (y = 0 is the top row), None: the whole frame.  Downscale only; NV12
+        needs an even w and h.  Shapes, out, after and done as export_frames, with the output size in place of the frame's."""
+        s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, lambda stream: self.device, size)
+        sc = _export_scale(size, crop)
+        self._ordered(lambda a, d: self._L.glava_b200_export_scaled(self._h, s.ctypes.data, s.shape[0], dst, None, C.byref(desc),
+                                                                    C.byref(sc), a, d), after, done)
+        return result
+
+    def export_mosaic(self, streams, cols, tile, fmt="nv12", background=(0, 0, 0), out=None):
+        """The frames of `streams` shrunk to tile = (w, h) and laid out row-major, `cols` tiles per row, in one picture, by
+        one export_scaled call with a destination (and for NV12 a chroma destination) per tile.  Returns [H * 3 / 2, W]
+        for NV12 (Y rows, then CbCr rows) or [H, W, 4], W = cols * w, H = rows * h: one surface to hand to an encoder.
+        Tiles start at multiples of 16 bytes, so w is a multiple of 16 (NV12) or 4 (RGBA / BGRA).  out: a uint8 CUDA
+        tensor [H * 3 / 2 or H, pitch] whose rows hold W (NV12) or W * 4 contiguous bytes; tiles past the last stream keep
+        its bytes (out None: black).  Ordered against torch's current stream as export_frames without events."""
+        import torch
+        s = np.ascontiguousarray(np.asarray(streams, dtype=np.int64).reshape(-1), dtype=np.int32)
+        count, cols = int(s.shape[0]), int(cols)
+        tw, th = (int(v) for v in tile)
+        if count < 1 or cols < 1:
+            raise ValueError("export_mosaic: at least one stream and one column")
+        desc = _export_desc(fmt, False, background)
+        nv12, px = fmt == "nv12", 1 if fmt == "nv12" else 4
+        W, H = cols * tw, (count + cols - 1) // cols * th
+        rows = H * 3 // 2 if nv12 else H
+        if out is None:
+            base = torch.empty((rows, (W * px + 15) // 16 * 16), dtype=torch.uint8, device=f"cuda:{self.device}")
+            if count % cols:                                  # black where no stream lands
+                base[:H].fill_(16 if nv12 else 0)
+                base[H:].fill_(128)
+            result = base[:, :W] if nv12 else base[:, :W * 4].unflatten(1, (W, 4))
+        else:
+            if (out.dtype != torch.uint8 or not out.is_cuda or out.dim() != 2 or out.shape[0] != rows or out.stride(1) != 1
+                    or out.shape[1] < W * px):
+                raise ValueError(f"out: a uint8 CUDA tensor [{rows}, >= {W * px}] with contiguous rows")
+            base = result = out
+        pitch, ptr = base.stride(0), base.data_ptr()
+        dst = (C.c_void_p * count)(*[ptr + (i // cols) * th * pitch + (i % cols) * tw * px for i in range(count)])
+        uv = (C.c_void_p * count)(*[ptr + (H + (i // cols) * (th // 2)) * pitch + (i % cols) * tw for i in range(count)]) if nv12 else None
+        desc.pitch = pitch
+        sc = _export_scale(tile, None)
+        self._ordered(lambda a, d: self._L.glava_b200_export_scaled(self._h, s.ctypes.data, count, dst, uv, C.byref(desc),
+                                                                    C.byref(sc), a, d), None, None)
         return result
 
     @property
@@ -851,6 +930,27 @@ class ShardedRenderer(_StreamState, _StreamStyles, _FrameExport):
         a list of per-frame tensors).  Work queued on torch's current streams of those devices is waited for first; the
         frames are complete after sync()."""
         import torch
+        device_of = self._device_of()
+        s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, device_of)
+        for d in sorted({device_of(int(x)) for x in s}):
+            torch.cuda.current_stream(d).synchronize()
+        _check(self._L.glava_b200_sharded_export_frames(self._h, s.ctypes.data, s.shape[0], dst, C.byref(desc)))
+        return result
+
+    def export_scaled(self, streams, size, crop=None, fmt="rgba", over=False, background=(0, 0, 0), out=None):
+        """Renderer.export_scaled with global stream indices (glava_b200_sharded_export_scaled), destinations placed as
+        export_frames places them; the frames are complete after sync()."""
+        import torch
+        device_of = self._device_of()
+        s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, device_of, size)
+        sc = _export_scale(size, crop)
+        for d in sorted({device_of(int(x)) for x in s}):
+            torch.cuda.current_stream(d).synchronize()
+        _check(self._L.glava_b200_sharded_export_scaled(self._h, s.ctypes.data, s.shape[0], dst, None, C.byref(desc), C.byref(sc)))
+        return result
+
+    def _device_of(self):
+        """stream -> the CUDA device of the shard that owns it"""
         shards = self.shards
 
         def device_of(stream):
@@ -858,12 +958,7 @@ class ShardedRenderer(_StreamState, _StreamStyles, _FrameExport):
                 if first <= stream < first + cnt:
                     return d
             return shards[0][0]
-
-        s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, device_of)
-        for d in sorted({device_of(int(x)) for x in s}):
-            torch.cuda.current_stream(d).synchronize()
-        _check(self._L.glava_b200_sharded_export_frames(self._h, s.ctypes.data, s.shape[0], dst, C.byref(desc)))
-        return result
+        return device_of
 
     def close(self):
         if getattr(self, "_h", None):

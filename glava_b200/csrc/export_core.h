@@ -101,5 +101,91 @@ GLB_HD size_t export_mark_index(int slot, int w, int h, int rows, int y, int str
 }
 GLB_HD bool export_row_read(uint32_t mark, int y) { return y >= (int) (mark & 0xffffu) && y < (int) (mark >> 16); }
 
+// ---- scaled export (DESIGN 4.11): exact integer area average ------------------------------------------------------------
+// Along one axis `n` source pixels shrink to `m` outputs (1 <= m <= n <= 16384): output X covers [X n, (X + 1) n) and source
+// i covers [i m, (i + 1) m); the weight of i in X is the length of their overlap.  The span of X is [first, last]; interior
+// weights are all m, the two edge weights are given (first == last only when n == m, weight n).  Every product fits 32 bits.
+struct ExportSpan { int first, last; uint32_t w_first, w_last; };
+GLB_HD ExportSpan export_span(int X, int n, int m) {
+    const uint32_t a = (uint32_t) X * (uint32_t) n, b = a + (uint32_t) n;
+    ExportSpan s;
+    s.first = (int) (a / (uint32_t) m);
+    s.last = (int) ((b - 1u) / (uint32_t) m);
+    const uint32_t e = (uint32_t) (s.first + 1) * (uint32_t) m;
+    s.w_first = (e < b ? e : b) - a;
+    s.w_last = b - (uint32_t) s.last * (uint32_t) m;
+    return s;
+}
+// the weight of source index i (first <= i <= last) in the span
+GLB_HD uint32_t export_span_weight(const ExportSpan& s, int i, int m) {
+    return i == s.first ? s.w_first : i == s.last ? s.w_last : (uint32_t) m;
+}
+// Crop coordinates are top-down as the export writes them: crop row r is framebuffer row h - 1 - (src_y + r), and crop
+// column i is framebuffer column src_x + i, whose mark word is that of strip (src_x + i) >> 7 (export_mark_index).  A
+// footprint can straddle strips, so it is walked strip by strip.
+GLB_HD int export_fb_row(int h, int src_y, int r) { return h - 1 - src_y - r; }
+// The mark-aware walk of a footprint's framebuffer rows [y, y_end) in one strip goes band by band: the band that holds y
+// ends at the returned row, and of its rows only [*ra, *rb) may be non-zero (`mark`: the band's word; rows == 0, no marks:
+// one band, every row read).  A band the marks call empty costs one word, however many footprint rows it holds.
+GLB_HD int export_band_rows(int y, int y_end, int rows, uint32_t mark, int* ra, int* rb) {
+    if (!rows) { *ra = y; *rb = y_end; return y_end; }
+    const int band_end = y - y % rows + rows, end = band_end < y_end ? band_end : y_end;
+    const int lo = (int) (mark & 0xffffu), hi = (int) (mark >> 16);
+    *ra = lo > y ? lo : y;
+    *rb = hi < end ? hi : end;
+    return end;
+}
+
+// floor(x / d) for every x < 2^63 as umulhi(x, mul) >> shift, d >= 2: shift = floor(log2(d - 1)), mul = ceil(2^(64 + shift) / d)
+// (< 2^64 because d > 2^shift).  With e = mul d - 2^(64 + shift) in [0, d), x mul / 2^(64 + shift) = x / d + x e / (d 2^(64 +
+// shift)), and x e < 2^63 2^(shift + 1) = 2^(64 + shift), so the error stays under 1 / d and never crosses an integer.
+// d == 1: mul = 0, the quotient is x.
+struct ExportRecip { uint64_t mul; int shift; };
+inline ExportRecip export_recip(uint64_t d) {                 // host code
+    if (d < 2) return { 0, 0 };
+    int s = 63;
+    while (!((d - 1) >> s)) --s;
+    const unsigned __int128 k = (unsigned __int128) 1 << (64 + s);
+    return { (uint64_t) ((k + d - 1) / d), s };
+}
+GLB_HD uint64_t export_div(uint64_t x, const ExportRecip& r) {
+    if (!r.mul) return x;
+#ifdef __CUDA_ARCH__
+    return __umul64hi(x, r.mul) >> r.shift;
+#else
+    return (uint64_t) (((unsigned __int128) x * r.mul) >> 64) >> r.shift;
+#endif
+}
+
+// One output pixel's sums: per channel sum of w * (composited) pixel and the total weight w of the pixels summed.  Only
+// non-zero pixels are summed: a zero pixel, read or skipped by the marks, stands for `zc` = what a zero pixel becomes
+// (export_px of 0 before any R / B swap), and export_scaled_px adds those in with the weight the sums lack.
+// Per source row the sums are 32-bit (at most 255 * src_w); the fold over rows is 64-bit (at most 255 * d < 2^36).
+GLB_HD void export_acc(const ExportFmt& f, uint32_t px, uint32_t w, uint32_t acc[4], uint32_t* wsum) {
+    if (!px) return;
+    if (f.over) px = export_over(px, f.bg, f.native);
+#pragma unroll
+    for (int c = 0; c < 4; ++c) acc[c] += w * ((px >> (8 * c)) & 255u);
+    *wsum += w;
+}
+GLB_HD void export_fold(const uint32_t row[4], uint32_t row_w, uint32_t wy, uint64_t acc[4], uint64_t* wsum) {
+#pragma unroll
+    for (int c = 0; c < 4; ++c) acc[c] += (uint64_t) wy * row[c];
+    *wsum += (uint64_t) wy * row_w;
+}
+// The output pixel (before any R / B swap): per channel (sum + (d - wsum) zc + d / 2) / d, d = src_w * src_h, the sum of all
+// weights; composited, alpha is 255.  All sums zero: zc itself.
+GLB_HD uint32_t export_scaled_px(const ExportFmt& f, const uint64_t acc[4], uint64_t wsum, uint64_t d, const ExportRecip& r, uint32_t zc) {
+    if (!wsum) return zc;
+    uint32_t out = f.over ? 0xff000000u : 0u;
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+        if (c == 3 && f.over) break;
+        const uint64_t x = acc[c] + (d - wsum) * ((zc >> (8 * c)) & 255u) + (d >> 1);
+        out |= (uint32_t) export_div(x, r) << (8 * c);
+    }
+    return out;
+}
+
 }  // namespace glb
 #endif

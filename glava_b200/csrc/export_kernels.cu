@@ -7,6 +7,9 @@
 // streaming stores (RGBA / BGRA) or two 4-byte Y stores and one 4-byte CbCr store (NV12).  With dirty-row marks the warp
 // reads only the rows its strip's band words say may be non-zero (export_core.h); every other row is zero pixels that are
 // never loaded.  Widths that are not a multiple of 4 take a per-pixel tail.
+//
+// glava_b200_export_scaled (DESIGN 4.11) is export_scaled_kernel below: the same frames, cropped and shrunk by the exact
+// area average of export_core.h, in one launch with its own entry and argument structs.
 #include "internal.h"
 #include "export_core.h"
 
@@ -100,6 +103,109 @@ int launch_export(const ExportArgs& a, void* stream) {
     else export_kernel<uint64_t><<<grid, 256, 0, (cudaStream_t) stream>>>(a);
     const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(GLAVA_B200_ECUDA, "export kernel launch: %s", cudaGetErrorString(e));
+    return 0;
+}
+
+// ---- glava_b200_export_scaled (DESIGN 4.11) --------------------------------------------------------------------------------
+// The grid is flattened over (listed entry, output row — NV12: row pair —, run of 32 output columns) on grid.x, one warp per
+// item, lane = output column.  With marks a lane walks its footprint strip by strip and, within a strip, band by band of the dirty-row
+// marks (export_band_rows): one mark word per band says which of its rows may be non-zero, and only those rows are visited,
+// so the rows of a band the marks call empty cost one load together (visiting every footprint row and loading its word
+// made the headline thumbnails slower than the full-size export).  A visited row's span is summed from aligned quads
+// (16-byte loads when rows are 16-byte aligned; neighbouring lanes read neighbouring segments) in 32-bit per channel and
+// folded into 64-bit sums with the row's weight.  NV12 chroma takes the right neighbour's pixels of both rows by shuffle.
+
+// output pixel (X, Y) of the lane, before any R / B swap; active = false: a lane past out_w (the sums stay empty)
+__device__ __forceinline__ uint32_t scaled_px(const ScaledArgs& a, const ExportFmt& f, const uint32_t* frame, int slot, int Y,
+                                              bool active, const ExportSpan& sx, const ExportRecip& rcp, uint32_t zc) {
+    const ExportSpan sy = export_span(Y, a.src_h, a.out_h);
+    const int x0 = a.src_x + sx.first, x1 = a.src_x + sx.last;
+    // framebuffer rows [yb, ye) of the footprint; row y is crop row h - 1 - src_y - y
+    const int yb = export_fb_row(a.h, a.src_y, sy.last), ye = export_fb_row(a.h, a.src_y, sy.first) + 1;
+    const int rows = a.marks ? a.mark_rows : 0;
+    uint64_t acc[4] = { 0u, 0u, 0u, 0u }, wsum = 0u;
+    // without marks the whole span is one pass (strip by strip, a lane whose span straddles strips would hold its warp)
+    for (int strip = x0 >> 7, last = rows ? x1 >> 7 : strip; active && strip <= last; ++strip) {
+        const int qa = max(x0, strip << 7) & ~3, qb = rows ? min(x1, (strip << 7) + 127) : x1;
+        for (int y = yb; y < ye;) {
+            int ra, rb;
+            const uint32_t mark = rows ? __ldg(a.marks + export_mark_index(slot, a.w, a.h, rows, y, strip)) : 0u;
+            y = export_band_rows(y, ye, rows, mark, &ra, &rb);
+            for (int yy = ra; yy < rb; ++yy) {
+                const uint32_t* src = frame + (size_t) yy * a.w;
+                uint32_t row[4] = { 0u, 0u, 0u, 0u }, row_w = 0u;
+                for (int qx = qa; qx <= qb; qx += 4) {
+                    uint32_t px[4];
+                    if ((a.w & 3) == 0) {
+                        const uint4 v = __ldcs(reinterpret_cast<const uint4*>(src + qx));
+                        px[0] = v.x; px[1] = v.y; px[2] = v.z; px[3] = v.w;
+                    } else {
+#pragma unroll
+                        for (int k = 0; k < 4; ++k) px[k] = qx + k >= x0 && qx + k <= x1 ? __ldcs(src + qx + k) : 0u;
+                    }
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) {
+                        const int x = qx + k;
+                        if (x >= x0 && x <= x1) export_acc(f, px[k], export_span_weight(sx, x - a.src_x, a.out_w), row, &row_w);
+                    }
+                }
+                export_fold(row, row_w, export_span_weight(sy, a.h - 1 - a.src_y - yy, a.out_h), acc, &wsum);
+            }
+        }
+    }
+    return export_scaled_px(f, acc, wsum, (uint64_t) a.src_w * (uint64_t) a.src_h, rcp, zc);
+}
+
+template <typename Index>
+__global__ void __launch_bounds__(256) export_scaled_kernel(const __grid_constant__ ScaledArgs a) {
+    const ExportFmt f = { a.format, a.over, a.native, a.bg };
+    const ExportRecip rcp = { a.div_mul, a.div_shift };
+    const bool nv12 = a.format == GLAVA_B200_EXPORT_NV12;
+    const uint32_t zc = f.over ? export_over(0u, f.bg, f.native) : 0u;   // what a zero pixel becomes
+    const Index runs = (Index) ((a.out_w + 31) >> 5), per = runs * (Index) (nv12 ? a.out_h >> 1 : a.out_h);
+    const Index items = (Index) a.count * per;
+    const Index warps = (Index) (((size_t) gridDim.x * blockDim.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    for (Index it = (Index) (((size_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5); it < items; it += warps) {
+        const Index k = it / per, rem = it - k * per;
+        const int u = (int) (rem / runs), X = (int) (rem - (Index) u * runs) * 32 + lane;
+        const bool active = X < a.out_w;
+        const ScaledEntry* e = a.list + k;
+        const int slot = __ldg(&e->slot);
+        const uint32_t* frame = reinterpret_cast<const uint32_t*>(a.fb) + (size_t) slot * a.h * a.w;
+        const ExportSpan sx = export_span(active ? X : 0, a.src_w, a.out_w);
+        uint8_t* const dst = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst)));
+        if (nv12) {                                         // out_w even: the whole 2x2 block is in this warp
+            const uint32_t top = scaled_px(a, f, frame, slot, 2 * u, active, sx, rcp, zc);
+            const uint32_t bot = scaled_px(a, f, frame, slot, 2 * u + 1, active, sx, rcp, zc);
+            const uint32_t top1 = __shfl_down_sync(0xffffffffu, top, 1), bot1 = __shfl_down_sync(0xffffffffu, bot, 1);
+            if (!active) continue;
+            uint8_t* const r0 = dst + (size_t) (2 * u) * a.pitch + X;
+            __stcs(r0, (uint8_t) export_y(top));
+            __stcs(r0 + a.pitch, (uint8_t) export_y(bot));
+            if (!(lane & 1)) {
+                uint8_t* const uv = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst_uv)));
+                __stcs(reinterpret_cast<unsigned short*>(uv + (size_t) u * a.pitch + X),
+                       (unsigned short) export_cbcr(export_avg4(top, top1, bot, bot1)));
+            }
+        } else {
+            uint32_t px = scaled_px(a, f, frame, slot, u, active, sx, rcp, zc);
+            if (!active) continue;
+            if (a.format == GLAVA_B200_EXPORT_BGRA) px = export_swap_rb(px);
+            __stcs(reinterpret_cast<uint32_t*>(dst + (size_t) u * a.pitch) + X, px);
+        }
+    }
+}
+
+int launch_export_scaled(const ScaledArgs& a, void* stream) {
+    const uint64_t units = a.format == GLAVA_B200_EXPORT_NV12 ? (uint64_t) (a.out_h >> 1) : (uint64_t) a.out_h;
+    const uint64_t items = (uint64_t) a.count * (uint64_t) ((a.out_w + 31) >> 5) * units;
+    const uint64_t blocks = (items + 7) / 8;                // 8 warps per CTA
+    const unsigned grid = blocks < 132u * 16u ? (unsigned) (blocks ? blocks : 1) : 132u * 16u;
+    if (items + ((uint64_t) grid << 3) < (1ull << 32)) export_scaled_kernel<uint32_t><<<grid, 256, 0, (cudaStream_t) stream>>>(a);
+    else export_scaled_kernel<uint64_t><<<grid, 256, 0, (cudaStream_t) stream>>>(a);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(GLAVA_B200_ECUDA, "scaled export kernel launch: %s", cudaGetErrorString(e));
     return 0;
 }
 

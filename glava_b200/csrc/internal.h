@@ -207,6 +207,29 @@ struct ExportArgs {
     size_t pitch, uv_offset;
 };
 int launch_export(const ExportArgs& a, void* stream);
+// export_kernels.cu: glava_b200_export_scaled (DESIGN 4.11), one launch for the whole list, its own entry and argument
+// structs so that export_kernel keeps its machine code.  Crop and output size are common to the list; d = src_w * src_h is
+// divided by as export_core.h export_div with (div_mul, div_shift).
+struct alignas(8) ScaledEntry {
+    uint8_t* dst;               // output row 0 (RGBA / BGRA pixels, or NV12 Y bytes)
+    uint8_t* dst_uv;            // NV12: CbCr row 0 (unused otherwise)
+    int      slot;              // framebuffer slot of the listed stream
+    int      pad;
+};
+struct ScaledArgs {
+    const uint8_t*  fb;         // [slots][h][w] RGBA8
+    const uint32_t* marks;      // as ExportArgs
+    int             mark_rows;
+    const ScaledEntry* list;
+    int    count, w, h;
+    int    format, over, native;
+    uint32_t bg;
+    size_t pitch;
+    int    src_x, src_y, src_w, src_h, out_w, out_h;   // crop in top-down coordinates, output size
+    uint64_t div_mul;
+    int    div_shift;
+};
+int launch_export_scaled(const ScaledArgs& a, void* stream);
 // capi.cu, for export.cpp: what the frame export reads of a renderer, and the slot where it keeps its own per-renderer
 // state (*attach, released by *attach_free when the renderer is destroyed)
 struct RendererView {
@@ -221,6 +244,19 @@ RendererView renderer_view(glava_b200* r);
 // export.cpp, for sharded.cpp: every refusal of glava_b200_export_frames that does not depend on the other shards (nothing
 // is enqueued)
 int export_check(glava_b200* r, const int* streams, int count, void* const* dst, const glava_b200_export* desc, const char* who);
+// export.cpp, for export_scaled.cpp: the format and flag checks of a descriptor; its pitch and uv_offset against a w x h
+// output (`what` names it in the message: "frame" / "output"); a destination pointer (null, alignment, device memory, device)
+int export_desc_format(const glava_b200_export& d, const char* who);
+int export_desc_size(int w, int h, const glava_b200_export& d, const char* what, const char* who);
+int export_dst_check(const RendererView& v, const void* p, const char* name, int i, const char* who);
+// the list of one export: export_list_begin returns a pinned host buffer of at least `bytes` (not yet read by an earlier
+// copy); export_list_end makes the renderer's stream wait for `after_event` (or nothing), then copies `bytes` of it into the
+// device list it returns.  Four pinned buffers are used in turn, sized in bytes for either entry type.
+int export_list_begin(const RendererView& v, size_t bytes, void** host);
+int export_list_end(const RendererView& v, size_t bytes, void* after_event, const void** d_list);
+// export_scaled.cpp, for sharded.cpp: every refusal of glava_b200_export_scaled that does not depend on the other shards
+int export_scaled_check(glava_b200* r, const int* streams, int count, void* const* dst, void* const* dst_uv,
+                        const glava_b200_export* desc, const glava_b200_export_scale* scale, const char* who);
 // capi.cu, for sharded.cpp: the blob checks of glava_b200_load_streams (nothing is touched), and save / load with one
 // host pointer per listed stream (the blobs of one shard's streams are not contiguous in the caller's array)
 int state_check_blobs(const glava_b200* r, const void* const* blobs, int count, const char* who);

@@ -394,6 +394,40 @@ int glava_b200_export_bytes(const glava_b200* r, const glava_b200_export* desc, 
 int glava_b200_export_frames(glava_b200* r, const int* streams, int count, void* const* dst,
                              const glava_b200_export* desc, void* after_event, void* done_event);
 
+/* Scaled and cropped export (DESIGN.md §4.11), for thumbnails, encoder ladders and mosaics: glava_b200_export_frames of a
+ * source rectangle shrunk to out_w x out_h, in the same single launch, reading only the rows the marks let through.
+ *   glava_b200_export_scaled   the frames glava_b200_export_frames would export (same ordering, events and streams rules),
+ *                              each cut to the rectangle `scale` names and downscaled by the exact area average: output
+ *                              column X covers source columns [X src_w, (X + 1) src_w) / out_w, weighted by overlap, rows
+ *                              likewise, and every channel is (sum of w * c + D / 2) / D with D = src_w * src_h in 64-bit
+ *                              integers.  A constant image stays constant; the whole frame at its own size is exactly
+ *                              glava_b200_export_frames.  RGBA / BGRA without EXPORT_OVER average the stored channels
+ *                              (premultiplied under native opacity); with it, and for NV12, each source pixel is composited
+ *                              first and alpha is 255.  NV12 is the export's arithmetic on the scaled image (Y per pixel,
+ *                              chroma per 2x2 output block), so out_w and out_h are even.
+ *     dst[i]                   out_h rows of out_w * 4 bytes (RGBA / BGRA) or out_w bytes (Y), `pitch` bytes apart
+ *     dst_uv                   NV12: dst_uv[i] receives the out_h / 2 CbCr rows (a mosaic tile's chroma need not sit at one
+ *                              offset from its luma); NULL: dst[i] + (uv_offset ? uv_offset : pitch * out_h)
+ *   Nothing outside each out_w x out_h rectangle and its chroma rows is written: pitch padding and neighbouring tiles keep
+ *   their bytes.  dst[i], dst_uv[i], pitch and uv_offset are multiples of 16 (a mosaic tile starts at a multiple of 4 pixels
+ *   in RGBA, of 16 in NV12).  Besides every refusal of glava_b200_export_frames (pitch and uv_offset measured against the
+ *   output), a null `scale`, a rectangle that is empty or leaves the frame, upscaling, odd NV12 output dimensions, a
+ *   misaligned, null, host or other-device dst_uv[i], and dst_uv for RGBA / BGRA are GLAVA_B200_EINVAL with nothing enqueued.
+ *   glava_b200_export_scaled_bytes   the bytes one destination spans (pitch * out_h; NV12 with dst_uv NULL: uv_offset +
+ *                              pitch * out_h / 2), after the same descriptor and rectangle checks.
+ *   glava_b200_sharded_export_scaled  the same with global stream indices, dst[i] / dst_uv[i] on the device of the shard
+ *                              that owns streams[i]; every entry is checked before any shard starts. */
+typedef struct {
+    int src_x, src_y, src_w, src_h;   /* source rectangle, top-down (row 0 = framebuffer row h - 1); src_w == src_h == 0:
+                                         the whole frame */
+    int out_w, out_h;                 /* 1 <= out_w <= src_w, 1 <= out_h <= src_h: downscale only */
+} glava_b200_export_scale;
+int glava_b200_export_scaled_bytes(const glava_b200* r, const glava_b200_export* desc, const glava_b200_export_scale* scale,
+                                   size_t* bytes);
+int glava_b200_export_scaled(glava_b200* r, const int* streams, int count, void* const* dst, void* const* dst_uv,
+                             const glava_b200_export* desc, const glava_b200_export_scale* scale, void* after_event,
+                             void* done_event);
+
 /* ---- one handle for a batch spread over several GPUs of a node (csrc/sharded.cpp) -------------------------------------
  * The streams of a batch are independent (one GLava process each, in the reference), so the batch is cut into contiguous
  * blocks, one per device — glava_b200_shard_range: counts differ by at most one — and nothing crosses between devices (no
@@ -420,6 +454,9 @@ const void* glava_b200_sharded_frame_device(glava_b200_sharded* s, int stream, i
 int  glava_b200_sharded_textures(glava_b200_sharded* s, uint16_t* out_l, uint16_t* out_r);
 int  glava_b200_sharded_export_frames(glava_b200_sharded* s, const int* streams, int count, void* const* dst,
                                       const glava_b200_export* desc);   /* global indices; see glava_b200_export_frames */
+int  glava_b200_sharded_export_scaled(glava_b200_sharded* s, const int* streams, int count, void* const* dst,
+                                      void* const* dst_uv, const glava_b200_export* desc,
+                                      const glava_b200_export_scale* scale);   /* global indices; see glava_b200_export_scaled */
 
 /* ---- lifetime of individual streams: reset, save and load (DESIGN.md §4.8) -------------------------------------------
  * A stream's state is what its next update reads besides its new audio: gravity store and average ring, the latest

@@ -1,4 +1,4 @@
-"""Development aid: are the kernels of two builds the same machine code?  Compiles raster_kernels.cu / spectrum_kernels.cu of
+"""Development aid: are the kernels of two builds the same machine code?  Compiles the raster, spectrum, chain and export kernels of
 a base git revision and of the working tree for sm_90a and compares the SASS of every kernel instruction by instruction,
 ignoring constant-bank parameter offsets (they move when glava_b200_params grows at its end).  No GPU needed.
 
@@ -35,7 +35,7 @@ def main(base):
         wt = os.path.join(tmp, "base")
         subprocess.run(["git", "worktree", "add", "-q", wt, base], cwd=ROOT, check=True)
         try:
-            for src in ("raster_kernels.cu", "spectrum_kernels.cu", "chain_kernels.cu"):
+            for src in ("raster_kernels.cu", "spectrum_kernels.cu", "chain_kernels.cu", "export_kernels.cu"):
                 objs = []
                 for tree, tag in ((wt, "base"), (ROOT, "new")):
                     obj = os.path.join(tmp, tag + "_" + src + ".o")
