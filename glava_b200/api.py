@@ -254,6 +254,8 @@ def lib():
     L.glava_b200_export_scaled_bytes.argtypes = [vp, C.POINTER(Export), C.POINTER(ExportScale), C.POINTER(C.c_size_t)]
     L.glava_b200_export_scaled.argtypes = [vp, vp, i32, vp, vp, C.POINTER(Export), C.POINTER(ExportScale), vp, vp]
     L.glava_b200_sharded_export_scaled.argtypes = [vp, vp, i32, vp, vp, C.POINTER(Export), C.POINTER(ExportScale)]
+    L.glava_b200_overlay_frames.argtypes = [vp, vp, i32, vp, vp, C.POINTER(Export), vp, vp]
+    L.glava_b200_sharded_overlay_frames.argtypes = [vp, vp, i32, vp, vp, C.POINTER(Export)]
     _lib = L
     # errors surface as Python exceptions; keep stderr quiet
     _quiet = C.CFUNCTYPE(None, cp)(lambda msg: None)
@@ -464,6 +466,70 @@ class _FrameExport:
         desc.pitch = pitch
         desc.uv_offset = pitch * h if nv12 else 0
         return s, desc, (C.c_void_p * max(count, 1))(*dst), result
+
+    def _overlay_plan(self, streams, images, at, fmt):
+        """-> (stream list, Export, dst pointers, dst_uv pointers or None) of an overlay (DESIGN 4.12).  images: one uint8
+        CUDA tensor per entry (one may repeat) or one [count, ...] tensor, each [H, W, 4] (RGBA / BGRA) or [H * 3 / 2, W]
+        (NV12, CbCr rows from row H) with contiguous rows and one pitch for all; at: (x, y) of each frame's top-left
+        corner in its image (None: (0, 0)).  Raises ValueError for a rectangle that leaves its image or whose rows do
+        not start at multiples of 16 bytes (the device refuses the rest)."""
+        import torch
+        s = np.ascontiguousarray(np.asarray(streams, dtype=np.int64).reshape(-1), dtype=np.int32)
+        count = int(s.shape[0])
+        if fmt not in EXPORT_FORMATS:
+            raise ValueError(f"format {fmt!r}: one of {sorted(EXPORT_FORMATS)}")
+        nv12 = fmt == "nv12"
+
+        def describe(t, what):
+            """-> (H, W, pitch) of one image"""
+            if t.dtype != torch.uint8 or not t.is_cuda or t.dim() != (2 if nv12 else 3) or (not nv12 and t.shape[2] != 4):
+                raise ValueError(f"{what}: a uint8 CUDA tensor {'[H * 3 / 2, W]' if nv12 else '[H, W, 4]'} "
+                                 f"(got {t.dtype} {tuple(t.shape)})")
+            if (nv12 and t.stride(1) != 1) or (not nv12 and (t.stride(1), t.stride(2)) != (4, 1)):
+                raise ValueError(f"{what}: rows must be contiguous")
+            H, W = (t.shape[0] * 2 // 3, t.shape[1]) if nv12 else (t.shape[0], t.shape[1])
+            if nv12 and (t.shape[0] % 3 or H % 2):
+                raise ValueError(f"{what}: NV12 has H * 3 / 2 rows with H even (got {t.shape[0]})")
+            return H, W, t.stride(0)
+
+        # per entry: (base address, H, W, pitch), each image described once (1024 entries cost no 1024 tensor views)
+        if isinstance(images, (list, tuple)):
+            seen, ents = {}, []
+            for i, t in enumerate(images):
+                if id(t) not in seen:
+                    seen[id(t)] = (t.data_ptr(),) + describe(t, f"images[{i}]")
+                ents.append(seen[id(t)])
+        else:
+            if images.dim() < 1 or images.shape[0] != count:
+                raise ValueError(f"images: {count} images, got a tensor {tuple(images.shape)}")
+            one = describe(images[0], "images[0]") if count else None
+            ents = [(images.data_ptr() + i * images.stride(0),) + one for i in range(count)]
+        if len(ents) != count:
+            raise ValueError(f"images: {count} images, got {len(ents)}")
+        at = [(0, 0)] * count if at is None else [(int(x), int(y)) for x, y in at]
+        if len(at) != count:
+            raise ValueError(f"at: {count} positions, got {len(at)}")
+        w, h = self.params.w, self.params.h
+        px = 1 if nv12 else 4
+        dst, uv, pitch = [], [], None
+        for i, ((base, H, W, ip), (x, y)) in enumerate(zip(ents, at)):
+            if pitch is None:
+                pitch = ip
+            elif ip != pitch:
+                raise ValueError(f"images[{i}]: pitch {ip}, the others {pitch}: one pitch per call")
+            if x < 0 or y < 0 or x + w > W or y + h > H:
+                raise ValueError(f"images[{i}]: the {w}x{h} frame at ({x}, {y}) leaves the {W}x{H} image")
+            d = base + y * pitch + x * px
+            u = base + (H + y // 2) * pitch + x if nv12 else None
+            if d % 16 or (nv12 and (y % 2 or u % 16)):
+                raise ValueError(f"images[{i}]: the frame at ({x}, {y}) does not start at a multiple of 16 bytes"
+                                 + (" on an even row" if nv12 else ""))
+            dst.append(d)
+            uv.append(u)
+        desc = _export_desc(fmt, False, (0, 0, 0))
+        desc.pitch = pitch or 0
+        arr = (C.c_void_p * max(count, 1))(*dst)
+        return s, desc, arr, (C.c_void_p * max(count, 1))(*uv) if nv12 else None
 
 
 def _export_desc(fmt, over, background):
@@ -787,6 +853,16 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
                                                                     C.byref(sc), a, d), after, done)
         return result
 
+    def overlay_frames(self, streams, images, at=None, fmt="nv12", after=None, done=None):
+        """The current frames of `streams` composited in place onto the caller's images (glava_b200_overlay_frames): under
+        native opacity premultiplied "over" the image's pixels, blended in Y'CbCr for NV12; under any other opacity the
+        opaque bytes export_frames writes.  images and at: see _overlay_plan; rectangles of one call must not overlap.
+        after / done and the ordering against torch's current stream as export_frames.  Returns images."""
+        s, desc, dst, uv = self._overlay_plan(streams, images, at, fmt)
+        self._ordered(lambda a, d: self._L.glava_b200_overlay_frames(self._h, s.ctypes.data, s.shape[0], dst, uv, C.byref(desc),
+                                                                     a, d), after, done)
+        return images
+
     def export_mosaic(self, streams, cols, tile, fmt="nv12", background=(0, 0, 0), out=None):
         """The frames of `streams` shrunk to tile = (w, h) and laid out row-major, `cols` tiles per row, in one picture, by
         one export_scaled call with a destination (and for NV12 a chroma destination) per tile.  Returns [H * 3 / 2, W]
@@ -948,6 +1024,18 @@ class ShardedRenderer(_StreamState, _StreamStyles, _FrameExport):
             torch.cuda.current_stream(d).synchronize()
         _check(self._L.glava_b200_sharded_export_scaled(self._h, s.ctypes.data, s.shape[0], dst, None, C.byref(desc), C.byref(sc)))
         return result
+
+    def overlay_frames(self, streams, images, at=None, fmt="nv12"):
+        """Renderer.overlay_frames with global stream indices (glava_b200_sharded_overlay_frames), each image on the device
+        of the shard that owns its stream.  Work queued on torch's current streams of those devices is waited for first;
+        the images are complete after sync()."""
+        import torch
+        device_of = self._device_of()
+        s, desc, dst, uv = self._overlay_plan(streams, images, at, fmt)
+        for d in sorted({device_of(int(x)) for x in s if 0 <= int(x) < self.batch}):
+            torch.cuda.current_stream(d).synchronize()
+        _check(self._L.glava_b200_sharded_overlay_frames(self._h, s.ctypes.data, s.shape[0], dst, uv, C.byref(desc)))
+        return images
 
     def _device_of(self):
         """stream -> the CUDA device of the shard that owns it"""

@@ -187,5 +187,79 @@ GLB_HD uint32_t export_scaled_px(const ExportFmt& f, const uint64_t acc[4], uint
     return out;
 }
 
+// ---- overlay (DESIGN 4.12): the frame composited onto the caller's image ----------------------------------------------------
+// Native opacity only (any other opacity writes export_frames' opaque bytes).  The premultiplied "over" GLava's window
+// performs on the desktop, with the caller's pixel d as the desktop, in all four channels: C = min(255, c + mul_norm8(d_c,
+// 255 - a)), alpha likewise.  px and d in the same byte order (a BGRA destination takes export_swap_rb(px)).  A zero pixel
+// leaves d as it is: mul_norm8(d, 255) = d.
+GLB_HD uint32_t overlay_px(uint32_t px, uint32_t d) {
+    const uint32_t ia = 255u - (px >> 24);
+    uint32_t out = 0u;
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+        const uint32_t v = ((px >> (8 * c)) & 255u) + mul_norm8((d >> (8 * c)) & 255u, ia);
+        out |= (v > 255u ? 255u : v) << (8 * c);
+    }
+    return out;
+}
+// NV12 blends in Y'CbCr: the limited-range transform is affine, so the composite of premultiplied c (alpha a) over a pixel
+// whose code value is V_D is off a/255 + M c + (1 - a/255) V_D exactly.  In the 16-bit fixed point of export_y /
+// export_cbcr the first and last terms are one fraction T / 255, T = off a + (255 - a) V_D <= 255 * 255, rounded down in
+// 2^-16 units (T 2^16 + 127 < 2^32).  a = 255 gives export_y / export_cbcr; a = 0 with c = 0 gives V_D back.
+GLB_HD uint32_t overlay_frac(uint32_t off, uint32_t a, uint32_t vd) {
+    return (((off * a + (255u - a) * vd) << GLB_YUV_SHIFT) + 127u) / 255u;
+}
+GLB_HD uint32_t overlay_clamp(int v) { return v < 0 ? 0u : v > 255 ? 255u : (uint32_t) v; }
+// the Y byte of pixel px (stored, premultiplied) over a Y byte yd
+GLB_HD uint32_t overlay_y(uint32_t px, uint32_t yd) {
+    const int r = (int) (px & 255u), g = (int) ((px >> 8) & 255u), b = (int) ((px >> 16) & 255u);
+    const int t = (int) overlay_frac(16u, px >> 24, yd);
+    return overlay_clamp((GLB_Y_R * r + GLB_Y_G * g + GLB_Y_B * b + t + GLB_YUV_HALF) >> GLB_YUV_SHIFT);
+}
+// the (Cb, Cr) pair of a block average m (overlay_avg4: alpha included) over the pair uvd (Cb low byte, Cr high)
+GLB_HD uint32_t overlay_cbcr(uint32_t m, uint32_t uvd) {
+    const int r = (int) (m & 255u), g = (int) ((m >> 8) & 255u), b = (int) ((m >> 16) & 255u);
+    const uint32_t a = m >> 24;
+    const int tb = (int) overlay_frac(128u, a, uvd & 255u), tr = (int) overlay_frac(128u, a, (uvd >> 8) & 255u);
+    const int cb = (GLB_CB_R * r + GLB_CB_G * g + GLB_CB_B * b + tb + GLB_YUV_HALF) >> GLB_YUV_SHIFT;
+    const int cr = (GLB_CR_R * r + GLB_CR_G * g + GLB_CR_B * b + tr + GLB_YUV_HALF) >> GLB_YUV_SHIFT;
+    return overlay_clamp(cb) | (overlay_clamp(cr) << 8);
+}
+// export_avg4 in all four channels: the chroma block of the overlay averages the stored pixels, alpha included
+GLB_HD uint32_t overlay_avg4(uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+    uint32_t out = 0;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const uint32_t s = ((a >> (8 * k)) & 255u) + ((b >> (8 * k)) & 255u) + ((c >> (8 * k)) & 255u) + ((d >> (8 * k)) & 255u);
+        out |= ((s + 2u) >> 2) << (8 * k);
+    }
+    return out;
+}
+// NV12 of a quad (rows 2j and 2j + 1, four pixels each) over the destination's Y words yt / yb and CbCr word uv (two pairs):
+// updates them in place
+GLB_HD void overlay_nv12_quad(const uint32_t top[4], const uint32_t bot[4], uint32_t* yt, uint32_t* yb, uint32_t* uv) {
+    uint32_t t = 0u, b = 0u;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        t |= overlay_y(top[k], (*yt >> (8 * k)) & 255u) << (8 * k);
+        b |= overlay_y(bot[k], (*yb >> (8 * k)) & 255u) << (8 * k);
+    }
+    *yt = t; *yb = b;
+    *uv = overlay_cbcr(overlay_avg4(top[0], top[1], bot[0], bot[1]), *uv & 0xffffu) |
+          (overlay_cbcr(overlay_avg4(top[2], top[3], bot[2], bot[3]), *uv >> 16) << 16);
+}
+// NV12 under dirty-row marks, one warp per band [b0, b1) of a strip: the output row pairs it visits are [*ja, *jb) (pair j =
+// framebuffer rows h - 1 - 2j and h - 2 - 2j), those that hold a row of [lo, hi), the rows the band's word lets through
+// (lo < hi).  With odd band heights a pair can straddle a band edge; it belongs to the band of its upper framebuffer row if
+// that row is marked, else to the other band.  So the band drops its top pair when that pair's upper row is b1 (the first
+// row of the band above, overlay_top_straddles) and the band above marks it, and its bottom pair's lower row, below b0, is
+// read when the band below marks it.  Returns whether the bottom pair straddles (the band below's word is then needed).
+GLB_HD bool overlay_band_pairs(int h, int b0, int lo, int hi, int* ja, int* jb) {
+    *ja = (h - hi) >> 1;
+    *jb = ((h - 1 - lo) >> 1) + 1;
+    return h - 2 - 2 * (*jb - 1) < b0;
+}
+GLB_HD bool overlay_top_straddles(int h, int b1, int ja) { return h - 1 - 2 * ja >= b1; }
+
 }  // namespace glb
 #endif

@@ -9,7 +9,8 @@
 // never loaded.  Widths that are not a multiple of 4 take a per-pixel tail.
 //
 // glava_b200_export_scaled (DESIGN 4.11) is export_scaled_kernel below: the same frames, cropped and shrunk by the exact
-// area average of export_core.h, in one launch with its own entry and argument structs.
+// area average of export_core.h, in one launch with its own entry and argument structs.  glava_b200_overlay_frames (DESIGN
+// 4.12) is overlay_kernel: the same frames composited onto the caller's images in place, likewise with its own structs.
 #include "internal.h"
 #include "export_core.h"
 
@@ -206,6 +207,158 @@ int launch_export_scaled(const ScaledArgs& a, void* stream) {
     else export_scaled_kernel<uint64_t><<<grid, 256, 0, (cudaStream_t) stream>>>(a);
     const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(GLAVA_B200_ECUDA, "scaled export kernel launch: %s", cudaGetErrorString(e));
+    return 0;
+}
+
+// ---- glava_b200_overlay_frames (DESIGN 4.12) -------------------------------------------------------------------------------
+// Native opacity: a quad of four framebuffer pixels that is not all zero is loaded together with the destination bytes under
+// it, blended (export_core.h overlay_px / overlay_nv12_quad) and stored back; an all-zero quad touches nothing.  With marks
+// the items are bands (Band = true): one warp per (entry, band of mark_rows rows, strip); a band whose word is empty costs
+// that word, otherwise only its marked rows are visited (NV12: the row pairs overlay_band_pairs gives it).  Without marks,
+// and under any other opacity (the rectangle then gets export_kernel's opaque bytes, every row), one warp per (entry, output
+// row pair, strip) as export_kernel.  A lane owns a quad; widths that are not a multiple of 4 take a per-pixel tail.
+
+__device__ __forceinline__ void overlay_load(const uint32_t* frame, int w, int y, int x, uint32_t px[4]) {
+    const uint32_t* row = frame + (size_t) y * w;
+    if ((w & 3) == 0) {
+        const uint4 v = __ldcs(reinterpret_cast<const uint4*>(row + x));
+        px[0] = v.x; px[1] = v.y; px[2] = v.z; px[3] = v.w;
+    } else {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) px[k] = x + k < w ? __ldcs(row + x + k) : 0u;
+    }
+}
+
+// native RGBA / BGRA: the quad at x of one destination row
+__device__ __forceinline__ void overlay_rgba(uint8_t* row, int x, int w, bool bgra, const uint32_t in[4]) {
+    if ((in[0] | in[1] | in[2] | in[3]) == 0u) return;
+    uint32_t px[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) px[k] = bgra ? export_swap_rb(in[k]) : in[k];
+    uint32_t* out = reinterpret_cast<uint32_t*>(row) + x;
+    if (x + 4 <= w) {                                       // dst and pitch: multiples of 16
+        uint4 d = __ldcs(reinterpret_cast<const uint4*>(out));
+        d.x = overlay_px(px[0], d.x); d.y = overlay_px(px[1], d.y); d.z = overlay_px(px[2], d.z); d.w = overlay_px(px[3], d.w);
+        __stcs(reinterpret_cast<uint4*>(out), d);
+    } else {
+        for (int k = 0; k < 4 && x + k < w; ++k) __stcs(out + k, overlay_px(px[k], __ldcs(out + k)));
+    }
+}
+
+// NV12 of the quad at x of output rows 2j, 2j + 1 (r0: row 2j's Y bytes, uv: the pair's CbCr row); native: blended onto the
+// bytes there, skipped when all eight pixels are zero; otherwise export_kernel's bytes (f: composite, opacity not native)
+__device__ __forceinline__ void overlay_nv12(const ExportFmt& f, bool native, uint8_t* r0, uint8_t* uv, size_t pitch, int x, int w,
+                                             const uint32_t top[4], const uint32_t bot[4]) {
+    const bool full = x + 4 <= w;                           // else w even: the last two pixels of a row
+    uint32_t yt, yb, c;
+    if (native) {
+        if ((top[0] | top[1] | top[2] | top[3] | bot[0] | bot[1] | bot[2] | bot[3]) == 0u) return;
+        if (full) {
+            yt = __ldcs(reinterpret_cast<const uint32_t*>(r0 + x));
+            yb = __ldcs(reinterpret_cast<const uint32_t*>(r0 + pitch + x));
+            c = __ldcs(reinterpret_cast<const uint32_t*>(uv + x));
+        } else {
+            yt = __ldcs(reinterpret_cast<const unsigned short*>(r0 + x));
+            yb = __ldcs(reinterpret_cast<const unsigned short*>(r0 + pitch + x));
+            c = __ldcs(reinterpret_cast<const unsigned short*>(uv + x));
+        }
+        overlay_nv12_quad(top, bot, &yt, &yb, &c);
+    } else {
+        c = export_nv12_quad(f, top, bot, &yt, &yb);
+    }
+    if (full) {
+        __stcs(reinterpret_cast<uint32_t*>(r0 + x), yt);
+        __stcs(reinterpret_cast<uint32_t*>(r0 + pitch + x), yb);
+        __stcs(reinterpret_cast<uint32_t*>(uv + x), c);
+    } else {
+        __stcs(reinterpret_cast<unsigned short*>(r0 + x), (unsigned short) yt);
+        __stcs(reinterpret_cast<unsigned short*>(r0 + pitch + x), (unsigned short) yb);
+        __stcs(reinterpret_cast<unsigned short*>(uv + x), (unsigned short) c);
+    }
+}
+
+__device__ __forceinline__ uint32_t overlay_mark(const OverlayArgs& a, int slot, int y, int strip) {
+    return __ldg(a.marks + export_mark_index(slot, a.w, a.h, a.mark_rows, y, strip));
+}
+
+template <typename Index, bool Band>
+__global__ void __launch_bounds__(256) overlay_kernel(const __grid_constant__ OverlayArgs a) {
+    const ExportFmt f = { a.format, 1, 0, 0u };             // any other opacity: the stored colour, alpha 255
+    const bool nv12 = a.format == GLAVA_B200_EXPORT_NV12, bgra = a.format == GLAVA_B200_EXPORT_BGRA;
+    const int rows = Band ? a.mark_rows : 2;
+    const Index strips = (Index) ((a.w + 127) >> 7), per = strips * (Index) ((a.h + rows - 1) / rows);
+    const Index items = (Index) a.count * per;
+    const Index warps = (Index) (((size_t) gridDim.x * blockDim.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    for (Index it = (Index) (((size_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5); it < items; it += warps) {
+        const Index k = it / per, rem = it - k * per;
+        const int u = (int) (rem / strips), strip = (int) (rem - (Index) u * strips);
+        const int x = strip * 128 + lane * 4;
+        if (x >= a.w) continue;
+        const OverlayEntry* e = a.list + k;
+        const int slot = __ldg(&e->slot);
+        const uint32_t* frame = reinterpret_cast<const uint32_t*>(a.fb) + (size_t) slot * a.h * a.w;
+        uint8_t* const dst = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst)));
+        if (Band) {                                         // native, marks: band u
+            const int b0 = u * rows, b1 = min(b0 + rows, a.h);
+            const uint32_t mark = overlay_mark(a, slot, b0, strip);
+            const int lo = max((int) (mark & 0xffffu), b0), hi = min((int) (mark >> 16), b1);
+            if (lo >= hi) continue;
+            if (!nv12) {
+                for (int y = lo; y < hi; ++y) {
+                    uint32_t q[4];
+                    overlay_load(frame, a.w, y, x, q);
+                    overlay_rgba(dst + (size_t) (a.h - 1 - y) * a.pitch, x, a.w, bgra, q);
+                }
+                continue;
+            }
+            uint8_t* const dst_uv = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst_uv)));
+            int ja, jb;
+            const uint32_t below = overlay_band_pairs(a.h, b0, lo, hi, &ja, &jb) ? overlay_mark(a, slot, b0 - 1, strip) : 0u;
+            if (overlay_top_straddles(a.h, b1, ja) && export_row_read(overlay_mark(a, slot, b1, strip), b1)) ++ja;
+            for (int j = ja; j < jb; ++j) {
+                const int y0 = a.h - 1 - 2 * j, y1 = y0 - 1;
+                uint32_t top[4] = { 0u, 0u, 0u, 0u }, bot[4] = { 0u, 0u, 0u, 0u };
+                if (y0 >= lo && y0 < hi) overlay_load(frame, a.w, y0, x, top);
+                if (y1 >= b0 ? y1 >= lo && y1 < hi : export_row_read(below, y1)) overlay_load(frame, a.w, y1, x, bot);
+                overlay_nv12(f, true, dst + (size_t) (2 * j) * a.pitch, dst_uv + (size_t) j * a.pitch, a.pitch, x, a.w, top, bot);
+            }
+        } else {                                            // output rows 2u, 2u + 1: framebuffer rows y0, y0 - 1
+            const int y0 = a.h - 1 - 2 * u, y1 = y0 - 1;
+            uint32_t top[4] = { 0u, 0u, 0u, 0u }, bot[4] = { 0u, 0u, 0u, 0u };
+            if (!a.marks || export_row_read(overlay_mark(a, slot, y0, strip), y0)) overlay_load(frame, a.w, y0, x, top);
+            if (y1 >= 0 && (!a.marks || export_row_read(overlay_mark(a, slot, y1, strip), y1))) overlay_load(frame, a.w, y1, x, bot);
+            uint8_t* const r0 = dst + (size_t) (2 * u) * a.pitch;
+            if (nv12) {
+                uint8_t* const dst_uv = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst_uv)));
+                overlay_nv12(f, a.native, r0, dst_uv + (size_t) u * a.pitch, a.pitch, x, a.w, top, bot);
+            } else if (a.native) {
+                overlay_rgba(r0, x, a.w, bgra, top);
+                if (y1 >= 0) overlay_rgba(r0 + a.pitch, x, a.w, bgra, bot);
+            } else {
+                store_rgba(f, r0, x, a.w, top, export_px(f, 0u));
+                if (y1 >= 0) store_rgba(f, r0 + a.pitch, x, a.w, bot, export_px(f, 0u));
+            }
+        }
+    }
+}
+
+int launch_overlay(const OverlayArgs& a, void* stream) {
+    const int rows = a.band ? a.mark_rows : 2;
+    const uint64_t items = (uint64_t) a.count * (uint64_t) ((a.w + 127) >> 7) * (uint64_t) ((a.h + rows - 1) / rows);
+    const uint64_t blocks = (items + 7) / 8;                // 8 warps per CTA
+    const unsigned grid = blocks < 132u * 16u ? (unsigned) (blocks ? blocks : 1) : 132u * 16u;
+    cudaStream_t st = (cudaStream_t) stream;
+    const bool narrow = items + ((uint64_t) grid << 3) < (1ull << 32);
+    if (a.band) {
+        if (narrow) overlay_kernel<uint32_t, true><<<grid, 256, 0, st>>>(a);
+        else overlay_kernel<uint64_t, true><<<grid, 256, 0, st>>>(a);
+    } else {
+        if (narrow) overlay_kernel<uint32_t, false><<<grid, 256, 0, st>>>(a);
+        else overlay_kernel<uint64_t, false><<<grid, 256, 0, st>>>(a);
+    }
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(GLAVA_B200_ECUDA, "overlay kernel launch: %s", cudaGetErrorString(e));
     return 0;
 }
 

@@ -230,6 +230,25 @@ struct ScaledArgs {
     int    div_shift;
 };
 int launch_export_scaled(const ScaledArgs& a, void* stream);
+// export_kernels.cu: glava_b200_overlay_frames (DESIGN 4.12), one launch for the whole list, its own entry and argument
+// structs.  band = 1 (native opacity with marks): one warp per (entry, band of mark_rows rows, strip), else one per
+// (entry, output row pair, strip) as export_kernel.
+struct alignas(8) OverlayEntry {
+    uint8_t* dst;               // the rectangle's top-left pixel (RGBA / BGRA) or Y byte
+    uint8_t* dst_uv;            // NV12: its first CbCr byte (unused otherwise)
+    int      slot;              // framebuffer slot of the listed stream
+    int      pad;
+};
+struct OverlayArgs {
+    const uint8_t*  fb;         // [slots][h][w] RGBA8
+    const uint32_t* marks;      // as ExportArgs
+    int             mark_rows;
+    const OverlayEntry* list;
+    int    count, w, h;
+    int    format, native, band;
+    size_t pitch;
+};
+int launch_overlay(const OverlayArgs& a, void* stream);
 // capi.cu, for export.cpp: what the frame export reads of a renderer, and the slot where it keeps its own per-renderer
 // state (*attach, released by *attach_free when the renderer is destroyed)
 struct RendererView {
@@ -257,6 +276,14 @@ int export_list_end(const RendererView& v, size_t bytes, void* after_event, cons
 // export_scaled.cpp, for sharded.cpp: every refusal of glava_b200_export_scaled that does not depend on the other shards
 int export_scaled_check(glava_b200* r, const int* streams, int count, void* const* dst, void* const* dst_uv,
                         const glava_b200_export* desc, const glava_b200_export_scale* scale, const char* who);
+// overlay.cpp, for sharded.cpp: every refusal of glava_b200_overlay_frames that depends on one renderer alone (the
+// overlap and framebuffer tests are overlay_geometry_check's); nothing is enqueued
+int overlay_check(glava_b200* r, const int* streams, int count, void* const* dst, void* const* dst_uv,
+                  const glava_b200_export* desc, const char* who);
+// The rectangles of a list (w x h frames, `desc`'s format and pitch; dst_uv null: dst + uv_offset) must not overlap each
+// other nor any of the `nfb` byte ranges [fb[k], fb[k] + fb_bytes[k]) (framebuffer arrays)
+int overlay_geometry_check(int w, int h, int count, void* const* dst, void* const* dst_uv, const glava_b200_export& desc,
+                           const uint8_t* const* fb, const size_t* fb_bytes, int nfb, const char* who);
 // capi.cu, for sharded.cpp: the blob checks of glava_b200_load_streams (nothing is touched), and save / load with one
 // host pointer per listed stream (the blobs of one shard's streams are not contiguous in the caller's array)
 int state_check_blobs(const glava_b200* r, const void* const* blobs, int count, const char* who);

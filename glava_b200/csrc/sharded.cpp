@@ -372,6 +372,49 @@ int glava_b200_sharded_export_scaled(glava_b200_sharded* g, const int* streams, 
     });
 }
 
+// Overlay (DESIGN 4.12), as glava_b200_sharded_export_scaled; besides each shard's own checks, the rectangles of the whole
+// list must not overlap each other nor any shard's framebuffer (shards may share a device)
+int glava_b200_sharded_overlay_frames(glava_b200_sharded* g, const int* streams, int count, void* const* dst, void* const* dst_uv,
+                                      const glava_b200_export* desc) {
+    clear_error();
+    const char* who = "glava_b200_sharded_overlay_frames";
+    if (!g || !desc) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
+    if (count < 1) return fail(GLAVA_B200_EINVAL, "%s: count %d < 1", who, count);
+    if (!streams || !dst) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
+    std::vector<std::vector<int>> idx(g->shards.size());
+    std::vector<std::vector<void*>> ptr(g->shards.size()), uv(g->shards.size());
+    for (int i = 0; i < count; ++i) {
+        const int s = streams[i];
+        if (s < 0 || s >= g->batch) return fail(GLAVA_B200_EINVAL, "%s: stream %d out of range (batch %d)", who, s, g->batch);
+        for (size_t k = 0; k < g->shards.size(); ++k) {
+            const Shard* sh = g->shards[k];
+            if (s >= sh->first && s < sh->first + sh->count) {
+                idx[k].push_back(s - sh->first); ptr[k].push_back(dst[i]); uv[k].push_back(dst_uv ? dst_uv[i] : nullptr);
+                break;
+            }
+        }
+    }
+    std::vector<const uint8_t*> fb;
+    std::vector<size_t> fb_bytes;
+    for (size_t k = 0; k < g->shards.size(); ++k) {
+        const RendererView v = renderer_view(g->shards[k]->r);
+        fb.push_back(v.fb); fb_bytes.push_back((size_t) v.slots * (size_t) v.h * (size_t) v.w * 4);
+        if (idx[k].empty()) continue;
+        const int rc = overlay_check(g->shards[k]->r, idx[k].data(), (int) idx[k].size(), ptr[k].data(), dst_uv ? uv[k].data() : nullptr,
+                                     desc, who);
+        if (rc) return rc;
+    }
+    const RendererView v0 = renderer_view(g->shards[0]->r);
+    const int rc = overlay_geometry_check(v0.w, v0.h, count, dst, dst_uv, *desc, fb.data(), fb_bytes.data(), (int) fb.size(), who);
+    if (rc) return rc;
+    return broadcast(g, [&](Shard& s) {
+        const size_t k = (size_t) (std::find(g->shards.begin(), g->shards.end(), &s) - g->shards.begin());
+        if (idx[k].empty()) return 0;
+        return glava_b200_overlay_frames(s.r, idx[k].data(), (int) idx[k].size(), ptr[k].data(), dst_uv ? uv[k].data() : nullptr,
+                                         desc, nullptr, nullptr);
+    });
+}
+
 int glava_b200_sharded_textures(glava_b200_sharded* g, uint16_t* out_l, uint16_t* out_r) {
     clear_error();
     if (!g) return fail(GLAVA_B200_EINVAL, "null argument");

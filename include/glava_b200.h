@@ -428,6 +428,34 @@ int glava_b200_export_scaled(glava_b200* r, const int* streams, int count, void*
                              const glava_b200_export* desc, const glava_b200_export_scale* scale, void* after_event,
                              void* done_event);
 
+/* Overlay onto the caller's images (DESIGN.md §4.12), for audiograms, music channels and compositing over video: the frames
+ * drawn over a picture the caller holds in DEVICE memory, in place, in one launch that touches only what the frame covers.
+ *   glava_b200_overlay_frames  composites the current frame of streams[i] — what glava_b200_export_frames would export
+ *                              (same ordering, events and streams rules), top-down — onto the w x h rectangle at dst[i]:
+ *     dst[i]                   the rectangle's top-left pixel (RGBA / BGRA: 4-byte pixels) or Y byte (NV12), `pitch`
+ *                              bytes per row; the caller's image around it is never touched
+ *     dst_uv                   NV12: dst_uv[i] is the rectangle's first CbCr byte; NULL: dst[i] + (uv_offset ? uv_offset :
+ *                              pitch * h), as glava_b200_export_scaled
+ *     desc                     format and pitch (and uv_offset) as the export; flags must be 0, background is unused
+ *   Under setopacity "native" (premultiply_alpha) the stored premultiplied pixel goes "over" the caller's pixel D, as
+ *   GLava's window goes over the desktop: RGBA / BGRA C = min(255, c + mul_norm8(D, 255 - a)) in all four channels (D
+ *   opaque or premultiplied); NV12 blends in Y'CbCr without a trip through RGB, Y = clamp((Y_R r + Y_G g + Y_B b +
+ *   floor((T 2^16 + 127) / 255) + 2^15) >> 16), T = 16 a + (255 - a) Y_D, and Cb / Cr likewise with T = 128 a + (255 - a)
+ *   Cb_D (Cr_D) from the (s + 2) >> 2 average of the 2x2 block's stored pixels, alpha included (export_core.h).  A zero
+ *   pixel leaves D exactly as it was, and rows the dirty-row marks skip and all-zero quads are neither read nor written.
+ *   An opaque pixel gives exactly glava_b200_export_frames' bytes.  Under any other opacity GLava's window is opaque: the
+ *   rectangle gets exactly what glava_b200_export_frames writes (RGBA / BGRA with EXPORT_OVER, or NV12).
+ *   Besides the refusals of glava_b200_export_scaled that apply (format, pitch, uv_offset, alignment, null / host /
+ *   other-device dst or dst_uv, dst_uv for RGBA / BGRA, odd NV12 frames, stream range, count < 1, an unbuilt renderer),
+ *   any flag, a rectangle that meets the renderer's framebuffer array and two rectangles of one call that overlap (luma
+ *   and chroma planes included: each entry reads and writes its bytes; layers go in separate calls) are GLAVA_B200_EINVAL
+ *   with nothing enqueued.
+ *   glava_b200_sharded_overlay_frames  the same with global stream indices, dst[i] / dst_uv[i] on the device of the shard
+ *                              that owns streams[i]; every entry, the overlap of the whole list and every shard's
+ *                              framebuffer are checked before any shard starts. */
+int glava_b200_overlay_frames(glava_b200* r, const int* streams, int count, void* const* dst, void* const* dst_uv,
+                              const glava_b200_export* desc, void* after_event, void* done_event);
+
 /* ---- one handle for a batch spread over several GPUs of a node (csrc/sharded.cpp) -------------------------------------
  * The streams of a batch are independent (one GLava process each, in the reference), so the batch is cut into contiguous
  * blocks, one per device — glava_b200_shard_range: counts differ by at most one — and nothing crosses between devices (no
@@ -457,6 +485,8 @@ int  glava_b200_sharded_export_frames(glava_b200_sharded* s, const int* streams,
 int  glava_b200_sharded_export_scaled(glava_b200_sharded* s, const int* streams, int count, void* const* dst,
                                       void* const* dst_uv, const glava_b200_export* desc,
                                       const glava_b200_export_scale* scale);   /* global indices; see glava_b200_export_scaled */
+int  glava_b200_sharded_overlay_frames(glava_b200_sharded* s, const int* streams, int count, void* const* dst,
+                                       void* const* dst_uv, const glava_b200_export* desc);   /* see glava_b200_overlay_frames */
 
 /* ---- lifetime of individual streams: reset, save and load (DESIGN.md §4.8) -------------------------------------------
  * A stream's state is what its next update reads besides its new audio: gravity store and average ring, the latest
