@@ -1,13 +1,18 @@
-// export.cpp — the host half of frame export (DESIGN 4.10): glava_b200_export_bytes, glava_b200_export_frames and the
-// checks glava_b200_sharded_export_frames runs before any shard starts.  It reads the renderer through capi.cu's
-// renderer_view and keeps its list buffers in the renderer's attachment slot; the kernel is export_kernels.cu.  The
-// descriptor and destination checks and the list buffers also serve the scaled export (export_scaled.cpp).
+// export.cpp — the host half of the three caller-buffer exports (DESIGN 4.10–4.12): glava_b200_export_frames,
+// glava_b200_export_scaled and glava_b200_overlay_frames, their byte counts, and the checks the sharded forms run before any
+// shard starts.  The three calls share one check, one list fill and one enqueue; what differs by kind is the output size
+// (the frame, or the scale rectangle's), the flags allowed, and the kernel's own argument fields.  It reads the renderer
+// through capi.cu's renderer_view and keeps its list buffers in the renderer's attachment slot; the kernels are
+// export_kernels.cu.
 #include "internal.h"
 #include "cuda_owner.h"
+#include "export_core.h"
 
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstring>
+#include <vector>
 
 using namespace glb;
 
@@ -19,9 +24,11 @@ using namespace glb;
 
 namespace {
 
-// The entry list of one renderer: it goes up from four pinned buffers in turn into one device list (read by the export
-// kernel on the raster stream, behind the copy that fills it), allocated on first use and grown to the longest list, in
-// bytes so that either entry type (ExportEntry, ScaledEntry) fits; ev[i]: the copy out of h[i] is done
+const char* const kCallName[] = { "glava_b200_export_frames", "glava_b200_export_scaled", "glava_b200_overlay_frames" };
+
+// The entry list of one renderer: it goes up from four pinned buffers in turn into one device list (read by the kernel on
+// the raster stream, behind the copy that fills it), allocated on first use and grown to the longest list, in bytes so
+// that either entry type (ExportEntry, ExportEntryUV) fits; ev[i]: the copy out of h[i] is done
 struct ExportList {
     PinnedBuf<uint8_t> h[4]; DevBuf<uint8_t> d; Event ev[4]; int cur = 0; size_t cap = 0;
 };
@@ -49,17 +56,8 @@ int list_room(const RendererView& v, size_t bytes, ExportList** out) {
     return 0;
 }
 
-}  // namespace
-
-namespace glb {
-// The checks of a descriptor: format and flags, then pitch and uv_offset against a w x h output
-int export_desc_format(const glava_b200_export& d, const char* who) {
-    if (d.format != GLAVA_B200_EXPORT_RGBA && d.format != GLAVA_B200_EXPORT_BGRA && d.format != GLAVA_B200_EXPORT_NV12)
-        return fail(GLAVA_B200_EINVAL, "%s: unknown format %d", who, d.format);
-    if (d.flags & ~GLAVA_B200_EXPORT_OVER) return fail(GLAVA_B200_EINVAL, "%s: unknown flags 0x%x", who, d.flags);
-    return 0;
-}
-int export_desc_size(int w, int h, const glava_b200_export& d, const char* what, const char* who) {
+// pitch and uv_offset against a w x h output (`what` names it in the message: "frame" / "output")
+int desc_size(int w, int h, const glava_b200_export& d, const char* what, const char* who) {
     const bool nv12 = d.format == GLAVA_B200_EXPORT_NV12;
     if (nv12 && ((w | h) & 1)) return fail(GLAVA_B200_EINVAL, "%s: NV12 needs an even width and height, the %s is %dx%d", who, what, w, h);
     const size_t row = nv12 ? (size_t) w : (size_t) w * 4;
@@ -71,7 +69,32 @@ int export_desc_size(int w, int h, const glava_b200_export& d, const char* what,
     return 0;
 }
 
-int export_dst_check(const RendererView& v, const void* p, const char* name, int i, const char* who) {
+// The descriptor of a call of `kind` against a w x h frame: format and flags, the scale rectangle (the scaled export
+// only), then pitch and uv_offset against the output.  *q: the rectangle with the whole-frame default applied (the
+// whole frame at its own size for the other kinds), so q->out_w x q->out_h is the output size.
+int desc_check(ExportKind kind, int w, int h, const glava_b200_export& d, const glava_b200_export_scale* s,
+               glava_b200_export_scale* q, const char* who) {
+    if (d.format != GLAVA_B200_EXPORT_RGBA && d.format != GLAVA_B200_EXPORT_BGRA && d.format != GLAVA_B200_EXPORT_NV12)
+        return fail(GLAVA_B200_EINVAL, "%s: unknown format %d", who, d.format);
+    if (d.flags & ~GLAVA_B200_EXPORT_OVER) return fail(GLAVA_B200_EINVAL, "%s: unknown flags 0x%x", who, d.flags);
+    if (kind == ExportKind::overlay && d.flags) return fail(GLAVA_B200_EINVAL, "%s: flags 0x%x: the overlay takes none", who, d.flags);
+    *q = { 0, 0, w, h, w, h };
+    if (kind != ExportKind::scaled) return desc_size(w, h, d, "frame", who);
+    if (!s) return fail(GLAVA_B200_EINVAL, "%s: null scale", who);
+    *q = *s;
+    if (!q->src_x && !q->src_y && !q->src_w && !q->src_h) { q->src_w = w; q->src_h = h; }
+    if (q->src_x < 0 || q->src_y < 0 || q->src_w < 1 || q->src_h < 1 || (int64_t) q->src_x + q->src_w > w ||
+        (int64_t) q->src_y + q->src_h > h)
+        return fail(GLAVA_B200_EINVAL, "%s: source rectangle (%d, %d) %dx%d is empty or leaves the %dx%d frame", who, q->src_x,
+                    q->src_y, q->src_w, q->src_h, w, h);
+    if (q->out_w < 1 || q->out_h < 1 || q->out_w > q->src_w || q->out_h > q->src_h)
+        return fail(GLAVA_B200_EINVAL, "%s: output %dx%d must be at least 1x1 and at most the %dx%d source (no upscaling)", who,
+                    q->out_w, q->out_h, q->src_w, q->src_h);
+    return desc_size(q->out_w, q->out_h, d, "output", who);
+}
+
+// a destination pointer: null, alignment, device memory, device
+int dst_check(const RendererView& v, const void* p, const char* name, int i, const char* who) {
     if (!p || ((uintptr_t) p & 15))
         return fail(GLAVA_B200_EINVAL, "%s: %s[%d] = %p is null or not 16-byte aligned", who, name, i, p);
     cudaPointerAttributes at;
@@ -84,39 +107,171 @@ int export_dst_check(const RendererView& v, const void* p, const char* name, int
     return 0;
 }
 
-int export_list_begin(const RendererView& v, size_t bytes, void** host) {
-    ExportList* L = nullptr;
-    int rc;
-    if ((rc = list_room(v, bytes, &L)) != 0) return rc;
-    CU(cudaEventSynchronize(L->ev[L->cur]));                // the copy that last read h[cur] (four exports ago)
-    *host = L->h[L->cur];
+// the byte count of one destination of a call of `kind`
+int output_bytes(ExportKind kind, const glava_b200* r, const glava_b200_export* desc, const glava_b200_export_scale* scale,
+                 size_t* bytes, const char* who) {
+    clear_error();
+    glava_b200_params p;
+    if (!r || !desc || !bytes || glava_b200_get_params(r, &p) != 0) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
+    glava_b200_export_scale q;
+    const int rc = desc_check(kind, p.w, p.h, *desc, scale, &q, who);
+    if (rc) return rc;
+    const size_t h = (size_t) q.out_h;
+    if (desc->format != GLAVA_B200_EXPORT_NV12) *bytes = desc->pitch * h;
+    else *bytes = (desc->uv_offset ? desc->uv_offset : desc->pitch * h) + desc->pitch * (h / 2);
     return 0;
 }
 
-int export_list_end(const RendererView& v, size_t bytes, void* after_event, const void** d_list) {
-    ExportList* L = static_cast<ExportList*>(*v.attach);
+// The fields every kind's argument struct has (they share names and meaning)
+template <typename Args>
+void common_args(Args& a, const RendererView& v, const void* d_list, int count, const glava_b200_export& d) {
+    a.fb = v.fb;
+    // marks the last raster pass kept describe the framebuffer, whatever GLAVA_B200_FULL_STORE says (it only makes that pass
+    // store every zero row); mark_key 0: none, or a kernel that keeps none wrote the frame since
+    a.marks = v.mark_key ? v.marks : nullptr;
+    a.mark_rows = v.mark_key >> 2;
+    a.list = static_cast<decltype(a.list)>(d_list); a.count = count; a.w = v.w; a.h = v.h;
+    a.format = d.format;
+    a.native = v.native;
+    a.pitch = d.pitch;
+}
+
+uint32_t background(const glava_b200_export& d) {
+    return (uint32_t) d.background[0] | ((uint32_t) d.background[1] << 8) | ((uint32_t) d.background[2] << 16);
+}
+
+// One plane of one entry's rectangle: `rows` rows of the common row bytes, the common pitch apart, from byte address p
+struct Rect { uintptr_t p; size_t rows; int entry; bool uv; };
+
+// Two rectangles of one pitch P and row bytes B, a starting first (a.p <= b.p): with q, m = divmod(b.p - a.p, P), b's row 0
+// meets a's row q when m < B and a's row q + 1 when P - m < B, and b's later rows meet a's later rows only if row 0 does
+bool rects_meet(const Rect& a, const Rect& b, size_t P, size_t B) {
+    const uintptr_t d = b.p - a.p, q = d / P, m = d % P;
+    return (q < a.rows && m < B) || (q + 1 < a.rows && P - m < B);
+}
+
+// whether rows of r meet the byte range [f0, f1)
+bool rect_meets_range(const Rect& r, size_t P, size_t B, uintptr_t f0, uintptr_t f1) {
+    if (f1 <= r.p || f0 >= r.p + (r.rows - 1) * P + B) return false;
+    size_t k = f0 <= r.p ? 0 : (f0 - r.p) / P;              // the first row that ends past f0
+    if (r.p + k * P + B <= f0) ++k;
+    return k < r.rows && r.p + k * P < f1;
+}
+
+}  // namespace
+
+namespace glb {
+int overlay_geometry_check(int w, int h, int count, void* const* dst, void* const* dst_uv, const glava_b200_export& desc,
+                           const uint8_t* const* fb, const size_t* fb_bytes, int nfb, const char* who) {
+    const bool nv12 = desc.format == GLAVA_B200_EXPORT_NV12;
+    const size_t P = desc.pitch, B = nv12 ? (size_t) w : (size_t) w * 4;
+    const size_t uv_offset = desc.uv_offset ? desc.uv_offset : P * (size_t) h;
+    std::vector<Rect> rs;
+    rs.reserve((size_t) count * (nv12 ? 2 : 1));
+    for (int i = 0; i < count; ++i) {
+        rs.push_back({ (uintptr_t) dst[i], (size_t) h, i, false });
+        if (nv12) rs.push_back({ dst_uv ? (uintptr_t) dst_uv[i] : (uintptr_t) dst[i] + uv_offset, (size_t) h / 2, i, true });
+    }
+    for (const Rect& r : rs)
+        for (int k = 0; k < nfb; ++k)
+            if (rect_meets_range(r, P, B, (uintptr_t) fb[k], (uintptr_t) fb[k] + fb_bytes[k]))
+                return fail(GLAVA_B200_EINVAL, "%s: the %s rectangle of entry %d overlaps the renderer's framebuffer", who,
+                            r.uv ? "CbCr" : "destination", r.entry);
+    // by address: a rectangle can only meet those that start before its last row ends
+    std::sort(rs.begin(), rs.end(), [](const Rect& a, const Rect& b) { return a.p < b.p; });
+    for (size_t i = 0; i < rs.size(); ++i) {
+        const uintptr_t end = rs[i].p + (rs[i].rows - 1) * P + B;
+        for (size_t j = i + 1; j < rs.size() && rs[j].p < end; ++j)
+            if (rects_meet(rs[i], rs[j], P, B)) {
+                const Rect& a = rs[i].entry < rs[j].entry ? rs[i] : rs[j];
+                const Rect& b = rs[i].entry < rs[j].entry ? rs[j] : rs[i];
+                return fail(GLAVA_B200_EINVAL, "%s: the %s rectangle of entry %d overlaps the %s rectangle of entry %d (layers go in "
+                            "separate calls)", who, a.uv ? "CbCr" : "destination", a.entry, b.uv ? "CbCr" : "destination", b.entry);
+            }
+    }
+    return 0;
+}
+
+int export_check(ExportKind kind, glava_b200* r, const int* streams, int count, void* const* dst, void* const* dst_uv,
+                 const glava_b200_export* desc, const glava_b200_export_scale* scale, const char* who, glava_b200_export_scale* q) {
+    const RendererView v = renderer_view(r);
+    if (!v.built) return fail(GLAVA_B200_EINVAL, "%s: the renderer has no tables: a reconfigure or resize failed and must be repeated", who);
+    glava_b200_export_scale local;
+    int rc = desc_check(kind, v.w, v.h, *desc, scale, q ? q : &local, who);
+    if (rc) return rc;
+    if (dst_uv && desc->format != GLAVA_B200_EXPORT_NV12) return fail(GLAVA_B200_EINVAL, "%s: dst_uv is for NV12 only", who);
+    if (count < 1) return fail(GLAVA_B200_EINVAL, "%s: count %d < 1", who, count);
+    if (!streams || !dst) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
+    for (int i = 0; i < count; ++i) {
+        if (streams[i] < 0 || streams[i] >= v.batch)
+            return fail(GLAVA_B200_EINVAL, "%s: stream %d out of range (batch %d)", who, streams[i], v.batch);
+        if ((rc = dst_check(v, dst[i], "dst", i, who)) != 0) return rc;
+        if (dst_uv && (rc = dst_check(v, dst_uv[i], "dst_uv", i, who)) != 0) return rc;
+    }
+    return 0;
+}
+
+// On the handle's stream, where readback copies: after the latest raster pass, before the next one can overwrite a slot
+int export_run(ExportKind kind, glava_b200* r, const int* streams, int count, void* const* dst, void* const* dst_uv,
+               const glava_b200_export* desc, const glava_b200_export_scale* scale, void* after_event, void* done_event) {
+    clear_error();
+    const char* who = kCallName[(int) kind];
+    if (!r || !desc) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
+    glava_b200_export_scale q;
+    int rc = export_check(kind, r, streams, count, dst, dst_uv, desc, scale, who, &q);
+    if (rc) return rc;
+    const RendererView v = renderer_view(r);
+    if (kind == ExportKind::overlay) {
+        const size_t fb_bytes = (size_t) v.slots * (size_t) v.h * (size_t) v.w * 4;
+        if ((rc = overlay_geometry_check(v.w, v.h, count, dst, dst_uv, *desc, &v.fb, &fb_bytes, 1, who)) != 0) return rc;
+    }
+    const bool nv12 = desc->format == GLAVA_B200_EXPORT_NV12;
+    const size_t uv_offset = desc->uv_offset ? desc->uv_offset : desc->pitch * (size_t) q.out_h;
+    CU(cudaSetDevice(v.device));
+    // export_kernel's entries have no chroma pointer (its machine code stays as measured); the others carry one per entry
+    const size_t bytes = (size_t) count * (kind == ExportKind::frames ? sizeof(ExportEntry) : sizeof(ExportEntryUV));
+    ExportList* L = nullptr;
+    if ((rc = list_room(v, bytes, &L)) != 0) return rc;
+    CU(cudaEventSynchronize(L->ev[L->cur]));                // the copy that last read h[cur] (four calls ago)
+    uint8_t* const host = L->h[L->cur];
+    for (int i = 0; i < count; ++i) {
+        uint8_t* const d = (uint8_t*) dst[i];
+        const int slot = streams[i] % v.slots;
+        if (kind == ExportKind::frames) reinterpret_cast<ExportEntry*>(host)[i] = { d, slot, 0 };
+        else reinterpret_cast<ExportEntryUV*>(host)[i] = { d, !nv12 ? nullptr : dst_uv ? (uint8_t*) dst_uv[i] : d + uv_offset, slot, 0 };
+    }
     cudaStream_t st = (cudaStream_t) v.stream;
     const int k = L->cur;
     if (after_event) CU(cudaStreamWaitEvent(st, (cudaEvent_t) after_event, 0));
     CU(cudaMemcpyAsync(L->d, L->h[k], bytes, cudaMemcpyHostToDevice, st));
     CU(cudaEventRecord(L->ev[k], st));
     L->cur = (k + 1) & 3;
-    *d_list = L->d;
-    return 0;
-}
-
-int export_check(glava_b200* r, const int* streams, int count, void* const* dst, const glava_b200_export* desc, const char* who) {
-    const RendererView v = renderer_view(r);
-    if (!v.built) return fail(GLAVA_B200_EINVAL, "%s: the renderer has no tables: a reconfigure or resize failed and must be repeated", who);
-    int rc = export_desc_format(*desc, who);
-    if (rc || (rc = export_desc_size(v.w, v.h, *desc, "frame", who)) != 0) return rc;
-    if (count < 1) return fail(GLAVA_B200_EINVAL, "%s: count %d < 1", who, count);
-    if (!streams || !dst) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
-    for (int i = 0; i < count; ++i) {
-        if (streams[i] < 0 || streams[i] >= v.batch)
-            return fail(GLAVA_B200_EINVAL, "%s: stream %d out of range (batch %d)", who, streams[i], v.batch);
-        if ((rc = export_dst_check(v, dst[i], "dst", i, who)) != 0) return rc;
+    const void* d_list = L->d;
+    if (kind == ExportKind::frames) {
+        ExportArgs a = {};
+        common_args(a, v, d_list, count, *desc);
+        a.over = nv12 || (desc->flags & GLAVA_B200_EXPORT_OVER) ? 1 : 0;
+        a.bg = background(*desc);
+        a.uv_offset = uv_offset;
+        rc = launch_export(a, v.stream);
+    } else if (kind == ExportKind::scaled) {
+        ScaledArgs a = {};
+        common_args(a, v, d_list, count, *desc);
+        a.over = nv12 || (desc->flags & GLAVA_B200_EXPORT_OVER) ? 1 : 0;
+        a.bg = background(*desc);
+        a.src_x = q.src_x; a.src_y = q.src_y; a.src_w = q.src_w; a.src_h = q.src_h; a.out_w = q.out_w; a.out_h = q.out_h;
+        const ExportRecip rcp = export_recip((uint64_t) q.src_w * (uint64_t) q.src_h);
+        a.div_mul = rcp.mul; a.div_shift = rcp.shift;
+        rc = launch_export_scaled(a, v.stream);
+    } else {
+        OverlayArgs a = {};
+        common_args(a, v, d_list, count, *desc);
+        a.band = a.native && a.marks && a.mark_rows > 0 ? 1 : 0;   // band items wherever marks exist (DESIGN 4.12)
+        rc = launch_overlay(a, v.stream);
     }
+    if (rc) return rc;
+    ++*v.launches;
+    if (done_event) CU(cudaEventRecord((cudaEvent_t) done_event, st));
     return 0;
 }
 }  // namespace glb
@@ -124,54 +279,25 @@ int export_check(glava_b200* r, const int* streams, int count, void* const* dst,
 extern "C" {
 
 int glava_b200_export_bytes(const glava_b200* r, const glava_b200_export* desc, size_t* bytes) {
-    clear_error();
-    const char* who = "glava_b200_export_bytes";
-    glava_b200_params p;
-    if (!r || !desc || !bytes || glava_b200_get_params(r, &p) != 0) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
-    int rc = export_desc_format(*desc, who);
-    if (rc || (rc = export_desc_size(p.w, p.h, *desc, "frame", who)) != 0) return rc;
-    const size_t h = (size_t) p.h;
-    if (desc->format != GLAVA_B200_EXPORT_NV12) *bytes = desc->pitch * h;
-    else *bytes = (desc->uv_offset ? desc->uv_offset : desc->pitch * h) + desc->pitch * (h / 2);
-    return 0;
+    return output_bytes(ExportKind::frames, r, desc, nullptr, bytes, "glava_b200_export_bytes");
+}
+int glava_b200_export_scaled_bytes(const glava_b200* r, const glava_b200_export* desc, const glava_b200_export_scale* scale,
+                                   size_t* bytes) {
+    return output_bytes(ExportKind::scaled, r, desc, scale, bytes, "glava_b200_export_scaled_bytes");
 }
 
-// On the handle's stream, where readback copies: after the latest raster pass, before the next one can overwrite a slot
 int glava_b200_export_frames(glava_b200* r, const int* streams, int count, void* const* dst, const glava_b200_export* desc,
                              void* after_event, void* done_event) {
-    clear_error();
-    const char* who = "glava_b200_export_frames";
-    if (!r || !desc) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
-    int rc = export_check(r, streams, count, dst, desc, who);
-    if (rc) return rc;
-    const RendererView v = renderer_view(r);
-    cudaStream_t st = (cudaStream_t) v.stream;
-    CU(cudaSetDevice(v.device));
-    void* host = nullptr;
-    const void* d_list = nullptr;
-    if ((rc = export_list_begin(v, (size_t) count * sizeof(ExportEntry), &host)) != 0) return rc;
-    ExportEntry* list = static_cast<ExportEntry*>(host);
-    for (int i = 0; i < count; ++i) {
-        list[i].dst = (uint8_t*) dst[i]; list[i].slot = streams[i] % v.slots; list[i].pad = 0;
-    }
-    if ((rc = export_list_end(v, (size_t) count * sizeof(ExportEntry), after_event, &d_list)) != 0) return rc;
-    ExportArgs a = {};
-    a.fb = v.fb;
-    // marks the last raster pass kept describe the framebuffer, whatever GLAVA_B200_FULL_STORE says (it only makes that pass
-    // store every zero row); mark_key 0: none, or a kernel that keeps none wrote the frame since
-    a.marks = v.mark_key ? v.marks : nullptr;
-    a.mark_rows = v.mark_key >> 2;
-    a.list = static_cast<const ExportEntry*>(d_list); a.count = count; a.w = v.w; a.h = v.h;
-    a.format = desc->format;
-    a.over = desc->format == GLAVA_B200_EXPORT_NV12 || (desc->flags & GLAVA_B200_EXPORT_OVER) ? 1 : 0;
-    a.native = v.native;
-    a.bg = (uint32_t) desc->background[0] | ((uint32_t) desc->background[1] << 8) | ((uint32_t) desc->background[2] << 16);
-    a.pitch = desc->pitch;
-    a.uv_offset = desc->uv_offset ? desc->uv_offset : desc->pitch * (size_t) v.h;
-    if ((rc = launch_export(a, st)) != 0) return rc;
-    ++*v.launches;
-    if (done_event) CU(cudaEventRecord((cudaEvent_t) done_event, st));
-    return 0;
+    return export_run(ExportKind::frames, r, streams, count, dst, nullptr, desc, nullptr, after_event, done_event);
+}
+int glava_b200_export_scaled(glava_b200* r, const int* streams, int count, void* const* dst, void* const* dst_uv,
+                             const glava_b200_export* desc, const glava_b200_export_scale* scale, void* after_event,
+                             void* done_event) {
+    return export_run(ExportKind::scaled, r, streams, count, dst, dst_uv, desc, scale, after_event, done_event);
+}
+int glava_b200_overlay_frames(glava_b200* r, const int* streams, int count, void* const* dst, void* const* dst_uv,
+                              const glava_b200_export* desc, void* after_event, void* done_event) {
+    return export_run(ExportKind::overlay, r, streams, count, dst, dst_uv, desc, nullptr, after_event, done_event);
 }
 
 }  // extern "C"

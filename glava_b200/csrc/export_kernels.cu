@@ -1,4 +1,4 @@
-// export_kernels.cu — glava_b200_export_frames (capi.cu, DESIGN 4.10): the current frames of a list of streams, flipped
+// export_kernels.cu — glava_b200_export_frames (DESIGN 4.10): the current frames of a list of streams, flipped
 // top-down and written as RGBA / BGRA (optionally composited) or NV12 into the caller's device buffers.
 //
 // One launch per call.  The list (destination, framebuffer slot) reaches the device in one small copy; the grid is
@@ -9,8 +9,9 @@
 // never loaded.  Widths that are not a multiple of 4 take a per-pixel tail.
 //
 // glava_b200_export_scaled (DESIGN 4.11) is export_scaled_kernel below: the same frames, cropped and shrunk by the exact
-// area average of export_core.h, in one launch with its own entry and argument structs.  glava_b200_overlay_frames (DESIGN
-// 4.12) is overlay_kernel: the same frames composited onto the caller's images in place, likewise with its own structs.
+// area average of export_core.h, in one launch with its own argument struct.  glava_b200_overlay_frames (DESIGN 4.12) is
+// overlay_kernel: the same frames composited onto the caller's images in place, likewise with its own argument struct.
+// Both take entries with a chroma pointer (ExportEntryUV); export_kernel keeps ExportEntry.  The host half is export.cpp.
 #include "internal.h"
 #include "export_core.h"
 
@@ -24,16 +25,31 @@ __device__ __forceinline__ bool row_read(const ExportArgs& a, int slot, int y, i
     return export_row_read(__ldg(a.marks + export_mark_index(slot, a.w, a.h, a.mark_rows, y, strip)), y);
 }
 
-// the quad at x of framebuffer row y (pixels past the right edge read as 0)
-__device__ __forceinline__ void load_quad(const ExportArgs& a, const uint32_t* frame, int y, int x, uint32_t px[4]) {
-    const uint32_t* row = frame + (size_t) y * a.w;
-    if ((a.w & 3) == 0) {                                   // rows are 16-byte aligned
+// the quad at x of framebuffer row y of a w-pixel-wide frame (pixels past the right edge read as 0)
+__device__ __forceinline__ void load_quad(const uint32_t* frame, int w, int y, int x, uint32_t px[4]) {
+    const uint32_t* row = frame + (size_t) y * w;
+    if ((w & 3) == 0) {                                     // rows are 16-byte aligned
         const uint4 v = __ldcs(reinterpret_cast<const uint4*>(row + x));
         px[0] = v.x; px[1] = v.y; px[2] = v.z; px[3] = v.w;
     } else {
 #pragma unroll
-        for (int k = 0; k < 4; ++k) px[k] = x + k < a.w ? __ldcs(row + x + k) : 0u;
+        for (int k = 0; k < 4; ++k) px[k] = x + k < w ? __ldcs(row + x + k) : 0u;
     }
+}
+
+// The grid of one launch over `items` warp items, 8 per CTA: grid-stride beyond 16 CTAs per SM of an H100 SXM, with 32-bit
+// item arithmetic whenever the item count allows (every realistic list: 1024 1080p frames are 8.3 M row-pair items)
+struct ExportGrid { unsigned blocks; bool narrow; };
+static ExportGrid export_grid(uint64_t items) {
+    const uint64_t blocks = (items + 7) / 8;
+    const unsigned grid = blocks < 132u * 16u ? (unsigned) (blocks ? blocks : 1) : 132u * 16u;
+    return { grid, items + ((uint64_t) grid << 3) < (1ull << 32) };
+}
+
+static int launch_status(const char* what) {
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(GLAVA_B200_ECUDA, "%s kernel launch: %s", what, cudaGetErrorString(e));
+    return 0;
 }
 
 // zpx: what a zero pixel becomes (a quad of zero pixels skips the per-pixel arithmetic)
@@ -72,8 +88,8 @@ __global__ void __launch_bounds__(256) export_kernel(const __grid_constant__ Exp
         // output rows 2j and 2j + 1 are framebuffer rows h - 1 - 2j and h - 2 - 2j
         const int y0 = a.h - 1 - 2 * j, y1 = y0 - 1;
         uint32_t top[4] = { 0u, 0u, 0u, 0u }, bot[4] = { 0u, 0u, 0u, 0u };
-        if (row_read(a, slot, y0, strip)) load_quad(a, frame, y0, x, top);
-        if (y1 >= 0 && row_read(a, slot, y1, strip)) load_quad(a, frame, y1, x, bot);
+        if (row_read(a, slot, y0, strip)) load_quad(frame, a.w, y0, x, top);
+        if (y1 >= 0 && row_read(a, slot, y1, strip)) load_quad(frame, a.w, y1, x, bot);
         uint8_t* const r0 = dst + (size_t) (2 * j) * a.pitch;
         if (a.format == GLAVA_B200_EXPORT_NV12) {           // h even: both rows exist
             uint32_t yt = zy, yb = zy, uv = zuv;
@@ -96,15 +112,10 @@ __global__ void __launch_bounds__(256) export_kernel(const __grid_constant__ Exp
 }
 
 int launch_export(const ExportArgs& a, void* stream) {
-    const uint64_t items = (uint64_t) a.count * (uint64_t) ((a.w + 127) >> 7) * (uint64_t) ((a.h + 1) >> 1);
-    const uint64_t blocks = (items + 7) / 8;                // 8 warps per CTA
-    const unsigned grid = blocks < 132u * 16u ? (unsigned) (blocks ? blocks : 1) : 132u * 16u;   // grid-stride beyond 16 CTAs per SM of an H100 SXM
-    // 32-bit item arithmetic whenever the item count allows (every realistic list: 1024 1080p frames are 8.3 M items)
-    if (items + ((uint64_t) grid << 3) < (1ull << 32)) export_kernel<uint32_t><<<grid, 256, 0, (cudaStream_t) stream>>>(a);
-    else export_kernel<uint64_t><<<grid, 256, 0, (cudaStream_t) stream>>>(a);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail(GLAVA_B200_ECUDA, "export kernel launch: %s", cudaGetErrorString(e));
-    return 0;
+    const ExportGrid g = export_grid((uint64_t) a.count * (uint64_t) ((a.w + 127) >> 7) * (uint64_t) ((a.h + 1) >> 1));
+    if (g.narrow) export_kernel<uint32_t><<<g.blocks, 256, 0, (cudaStream_t) stream>>>(a);
+    else export_kernel<uint64_t><<<g.blocks, 256, 0, (cudaStream_t) stream>>>(a);
+    return launch_status("export");
 }
 
 // ---- glava_b200_export_scaled (DESIGN 4.11) --------------------------------------------------------------------------------
@@ -171,7 +182,7 @@ __global__ void __launch_bounds__(256) export_scaled_kernel(const __grid_constan
         const Index k = it / per, rem = it - k * per;
         const int u = (int) (rem / runs), X = (int) (rem - (Index) u * runs) * 32 + lane;
         const bool active = X < a.out_w;
-        const ScaledEntry* e = a.list + k;
+        const ExportEntryUV* e = a.list + k;
         const int slot = __ldg(&e->slot);
         const uint32_t* frame = reinterpret_cast<const uint32_t*>(a.fb) + (size_t) slot * a.h * a.w;
         const ExportSpan sx = export_span(active ? X : 0, a.src_w, a.out_w);
@@ -200,14 +211,10 @@ __global__ void __launch_bounds__(256) export_scaled_kernel(const __grid_constan
 
 int launch_export_scaled(const ScaledArgs& a, void* stream) {
     const uint64_t units = a.format == GLAVA_B200_EXPORT_NV12 ? (uint64_t) (a.out_h >> 1) : (uint64_t) a.out_h;
-    const uint64_t items = (uint64_t) a.count * (uint64_t) ((a.out_w + 31) >> 5) * units;
-    const uint64_t blocks = (items + 7) / 8;                // 8 warps per CTA
-    const unsigned grid = blocks < 132u * 16u ? (unsigned) (blocks ? blocks : 1) : 132u * 16u;
-    if (items + ((uint64_t) grid << 3) < (1ull << 32)) export_scaled_kernel<uint32_t><<<grid, 256, 0, (cudaStream_t) stream>>>(a);
-    else export_scaled_kernel<uint64_t><<<grid, 256, 0, (cudaStream_t) stream>>>(a);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail(GLAVA_B200_ECUDA, "scaled export kernel launch: %s", cudaGetErrorString(e));
-    return 0;
+    const ExportGrid g = export_grid((uint64_t) a.count * (uint64_t) ((a.out_w + 31) >> 5) * units);
+    if (g.narrow) export_scaled_kernel<uint32_t><<<g.blocks, 256, 0, (cudaStream_t) stream>>>(a);
+    else export_scaled_kernel<uint64_t><<<g.blocks, 256, 0, (cudaStream_t) stream>>>(a);
+    return launch_status("scaled export");
 }
 
 // ---- glava_b200_overlay_frames (DESIGN 4.12) -------------------------------------------------------------------------------
@@ -217,17 +224,6 @@ int launch_export_scaled(const ScaledArgs& a, void* stream) {
 // that word, otherwise only its marked rows are visited (NV12: the row pairs overlay_band_pairs gives it).  Without marks,
 // and under any other opacity (the rectangle then gets export_kernel's opaque bytes, every row), one warp per (entry, output
 // row pair, strip) as export_kernel.  A lane owns a quad; widths that are not a multiple of 4 take a per-pixel tail.
-
-__device__ __forceinline__ void overlay_load(const uint32_t* frame, int w, int y, int x, uint32_t px[4]) {
-    const uint32_t* row = frame + (size_t) y * w;
-    if ((w & 3) == 0) {
-        const uint4 v = __ldcs(reinterpret_cast<const uint4*>(row + x));
-        px[0] = v.x; px[1] = v.y; px[2] = v.z; px[3] = v.w;
-    } else {
-#pragma unroll
-        for (int k = 0; k < 4; ++k) px[k] = x + k < w ? __ldcs(row + x + k) : 0u;
-    }
-}
 
 // native RGBA / BGRA: the quad at x of one destination row
 __device__ __forceinline__ void overlay_rgba(uint8_t* row, int x, int w, bool bgra, const uint32_t in[4]) {
@@ -295,7 +291,7 @@ __global__ void __launch_bounds__(256) overlay_kernel(const __grid_constant__ Ov
         const int u = (int) (rem / strips), strip = (int) (rem - (Index) u * strips);
         const int x = strip * 128 + lane * 4;
         if (x >= a.w) continue;
-        const OverlayEntry* e = a.list + k;
+        const ExportEntryUV* e = a.list + k;
         const int slot = __ldg(&e->slot);
         const uint32_t* frame = reinterpret_cast<const uint32_t*>(a.fb) + (size_t) slot * a.h * a.w;
         uint8_t* const dst = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst)));
@@ -307,7 +303,7 @@ __global__ void __launch_bounds__(256) overlay_kernel(const __grid_constant__ Ov
             if (!nv12) {
                 for (int y = lo; y < hi; ++y) {
                     uint32_t q[4];
-                    overlay_load(frame, a.w, y, x, q);
+                    load_quad(frame, a.w, y, x, q);
                     overlay_rgba(dst + (size_t) (a.h - 1 - y) * a.pitch, x, a.w, bgra, q);
                 }
                 continue;
@@ -319,15 +315,15 @@ __global__ void __launch_bounds__(256) overlay_kernel(const __grid_constant__ Ov
             for (int j = ja; j < jb; ++j) {
                 const int y0 = a.h - 1 - 2 * j, y1 = y0 - 1;
                 uint32_t top[4] = { 0u, 0u, 0u, 0u }, bot[4] = { 0u, 0u, 0u, 0u };
-                if (y0 >= lo && y0 < hi) overlay_load(frame, a.w, y0, x, top);
-                if (y1 >= b0 ? y1 >= lo && y1 < hi : export_row_read(below, y1)) overlay_load(frame, a.w, y1, x, bot);
+                if (y0 >= lo && y0 < hi) load_quad(frame, a.w, y0, x, top);
+                if (y1 >= b0 ? y1 >= lo && y1 < hi : export_row_read(below, y1)) load_quad(frame, a.w, y1, x, bot);
                 overlay_nv12(f, true, dst + (size_t) (2 * j) * a.pitch, dst_uv + (size_t) j * a.pitch, a.pitch, x, a.w, top, bot);
             }
         } else {                                            // output rows 2u, 2u + 1: framebuffer rows y0, y0 - 1
             const int y0 = a.h - 1 - 2 * u, y1 = y0 - 1;
             uint32_t top[4] = { 0u, 0u, 0u, 0u }, bot[4] = { 0u, 0u, 0u, 0u };
-            if (!a.marks || export_row_read(overlay_mark(a, slot, y0, strip), y0)) overlay_load(frame, a.w, y0, x, top);
-            if (y1 >= 0 && (!a.marks || export_row_read(overlay_mark(a, slot, y1, strip), y1))) overlay_load(frame, a.w, y1, x, bot);
+            if (!a.marks || export_row_read(overlay_mark(a, slot, y0, strip), y0)) load_quad(frame, a.w, y0, x, top);
+            if (y1 >= 0 && (!a.marks || export_row_read(overlay_mark(a, slot, y1, strip), y1))) load_quad(frame, a.w, y1, x, bot);
             uint8_t* const r0 = dst + (size_t) (2 * u) * a.pitch;
             if (nv12) {
                 uint8_t* const dst_uv = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst_uv)));
@@ -345,21 +341,16 @@ __global__ void __launch_bounds__(256) overlay_kernel(const __grid_constant__ Ov
 
 int launch_overlay(const OverlayArgs& a, void* stream) {
     const int rows = a.band ? a.mark_rows : 2;
-    const uint64_t items = (uint64_t) a.count * (uint64_t) ((a.w + 127) >> 7) * (uint64_t) ((a.h + rows - 1) / rows);
-    const uint64_t blocks = (items + 7) / 8;                // 8 warps per CTA
-    const unsigned grid = blocks < 132u * 16u ? (unsigned) (blocks ? blocks : 1) : 132u * 16u;
+    const ExportGrid g = export_grid((uint64_t) a.count * (uint64_t) ((a.w + 127) >> 7) * (uint64_t) ((a.h + rows - 1) / rows));
     cudaStream_t st = (cudaStream_t) stream;
-    const bool narrow = items + ((uint64_t) grid << 3) < (1ull << 32);
     if (a.band) {
-        if (narrow) overlay_kernel<uint32_t, true><<<grid, 256, 0, st>>>(a);
-        else overlay_kernel<uint64_t, true><<<grid, 256, 0, st>>>(a);
+        if (g.narrow) overlay_kernel<uint32_t, true><<<g.blocks, 256, 0, st>>>(a);
+        else overlay_kernel<uint64_t, true><<<g.blocks, 256, 0, st>>>(a);
     } else {
-        if (narrow) overlay_kernel<uint32_t, false><<<grid, 256, 0, st>>>(a);
-        else overlay_kernel<uint64_t, false><<<grid, 256, 0, st>>>(a);
+        if (g.narrow) overlay_kernel<uint32_t, false><<<g.blocks, 256, 0, st>>>(a);
+        else overlay_kernel<uint64_t, false><<<g.blocks, 256, 0, st>>>(a);
     }
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail(GLAVA_B200_ECUDA, "overlay kernel launch: %s", cudaGetErrorString(e));
-    return 0;
+    return launch_status("overlay");
 }
 
 }  // namespace glb

@@ -207,20 +207,22 @@ struct ExportArgs {
     size_t pitch, uv_offset;
 };
 int launch_export(const ExportArgs& a, void* stream);
-// export_kernels.cu: glava_b200_export_scaled (DESIGN 4.11), one launch for the whole list, its own entry and argument
-// structs so that export_kernel keeps its machine code.  Crop and output size are common to the list; d = src_w * src_h is
-// divided by as export_core.h export_div with (div_mul, div_shift).
-struct alignas(8) ScaledEntry {
+// The entry of the scaled export and the overlay: ExportEntry with a chroma pointer, so that one call can fill an NV12
+// mosaic, where each tile's chroma sits at a different offset from its luma
+struct alignas(8) ExportEntryUV {
     uint8_t* dst;               // output row 0 (RGBA / BGRA pixels, or NV12 Y bytes)
     uint8_t* dst_uv;            // NV12: CbCr row 0 (unused otherwise)
     int      slot;              // framebuffer slot of the listed stream
     int      pad;
 };
+// export_kernels.cu: glava_b200_export_scaled (DESIGN 4.11), one launch for the whole list, its own argument struct and
+// ExportEntryUV entries so that export_kernel keeps its machine code.  Crop and output size are common to the list; d = src_w * src_h is
+// divided by as export_core.h export_div with (div_mul, div_shift).
 struct ScaledArgs {
     const uint8_t*  fb;         // [slots][h][w] RGBA8
     const uint32_t* marks;      // as ExportArgs
     int             mark_rows;
-    const ScaledEntry* list;
+    const ExportEntryUV* list;
     int    count, w, h;
     int    format, over, native;
     uint32_t bg;
@@ -230,20 +232,14 @@ struct ScaledArgs {
     int    div_shift;
 };
 int launch_export_scaled(const ScaledArgs& a, void* stream);
-// export_kernels.cu: glava_b200_overlay_frames (DESIGN 4.12), one launch for the whole list, its own entry and argument
-// structs.  band = 1 (native opacity with marks): one warp per (entry, band of mark_rows rows, strip), else one per
-// (entry, output row pair, strip) as export_kernel.
-struct alignas(8) OverlayEntry {
-    uint8_t* dst;               // the rectangle's top-left pixel (RGBA / BGRA) or Y byte
-    uint8_t* dst_uv;            // NV12: its first CbCr byte (unused otherwise)
-    int      slot;              // framebuffer slot of the listed stream
-    int      pad;
-};
+// export_kernels.cu: glava_b200_overlay_frames (DESIGN 4.12), one launch for the whole list, its own argument struct and
+// ExportEntryUV entries.  band = 1 (native opacity with marks): one warp per (entry, band of mark_rows rows, strip), else one per
+// (entry, output row pair, strip) as export_kernel.  An entry's dst is the rectangle's top-left pixel or Y byte.
 struct OverlayArgs {
     const uint8_t*  fb;         // [slots][h][w] RGBA8
     const uint32_t* marks;      // as ExportArgs
     int             mark_rows;
-    const OverlayEntry* list;
+    const ExportEntryUV* list;
     int    count, w, h;
     int    format, native, band;
     size_t pitch;
@@ -260,26 +256,19 @@ struct RendererView {
     void** attach; void (**attach_free)(void*);
 };
 RendererView renderer_view(glava_b200* r);
-// export.cpp, for sharded.cpp: every refusal of glava_b200_export_frames that does not depend on the other shards (nothing
-// is enqueued)
-int export_check(glava_b200* r, const int* streams, int count, void* const* dst, const glava_b200_export* desc, const char* who);
-// export.cpp, for export_scaled.cpp: the format and flag checks of a descriptor; its pitch and uv_offset against a w x h
-// output (`what` names it in the message: "frame" / "output"); a destination pointer (null, alignment, device memory, device)
-int export_desc_format(const glava_b200_export& d, const char* who);
-int export_desc_size(int w, int h, const glava_b200_export& d, const char* what, const char* who);
-int export_dst_check(const RendererView& v, const void* p, const char* name, int i, const char* who);
-// the list of one export: export_list_begin returns a pinned host buffer of at least `bytes` (not yet read by an earlier
-// copy); export_list_end makes the renderer's stream wait for `after_event` (or nothing), then copies `bytes` of it into the
-// device list it returns.  Four pinned buffers are used in turn, sized in bytes for either entry type.
-int export_list_begin(const RendererView& v, size_t bytes, void** host);
-int export_list_end(const RendererView& v, size_t bytes, void* after_event, const void** d_list);
-// export_scaled.cpp, for sharded.cpp: every refusal of glava_b200_export_scaled that does not depend on the other shards
-int export_scaled_check(glava_b200* r, const int* streams, int count, void* const* dst, void* const* dst_uv,
-                        const glava_b200_export* desc, const glava_b200_export_scale* scale, const char* who);
-// overlay.cpp, for sharded.cpp: every refusal of glava_b200_overlay_frames that depends on one renderer alone (the
-// overlap and framebuffer tests are overlay_geometry_check's); nothing is enqueued
-int overlay_check(glava_b200* r, const int* streams, int count, void* const* dst, void* const* dst_uv,
-                  const glava_b200_export* desc, const char* who);
+// export.cpp: the three caller-buffer exports, which differ in output size (the scaled export's is its rectangle's), the
+// flags they take and their kernel
+enum class ExportKind { frames, scaled, overlay };
+// Every refusal of a call of `kind` that depends on this renderer alone, in the call's order (the overlay's overlap and
+// framebuffer tests are overlay_geometry_check's); nothing is enqueued.  dst_uv and scale may be null; q (if non-null)
+// receives the scale rectangle with its defaults applied, the whole frame for the other kinds.
+int export_check(ExportKind kind, glava_b200* r, const int* streams, int count, void* const* dst, void* const* dst_uv,
+                 const glava_b200_export* desc, const glava_b200_export_scale* scale, const char* who,
+                 glava_b200_export_scale* q = nullptr);
+// The call of `kind` on one renderer (glava_b200_export_frames / _export_scaled / glava_b200_overlay_frames): every check,
+// then the list copy and the kernel on the raster stream behind `after_event` (or nothing), then `done_event` (or nothing)
+int export_run(ExportKind kind, glava_b200* r, const int* streams, int count, void* const* dst, void* const* dst_uv,
+               const glava_b200_export* desc, const glava_b200_export_scale* scale, void* after_event, void* done_event);
 // The rectangles of a list (w x h frames, `desc`'s format and pitch; dst_uv null: dst + uv_offset) must not overlap each
 // other nor any of the `nfb` byte ranges [fb[k], fb[k] + fb_bytes[k]) (framebuffer arrays)
 int overlay_geometry_check(int w, int h, int count, void* const* dst, void* const* dst_uv, const glava_b200_export& desc,

@@ -307,77 +307,13 @@ int glava_b200_sharded_get_stream_styles(const glava_b200_sharded* g, const int*
     return 0;
 }
 
-// Frame export (DESIGN 4.10), global stream indices (repeats allowed): every index, the descriptor and every destination
-// (on the device of the shard that owns its stream) are checked before any shard starts; the shards then issue at once.
-int glava_b200_sharded_export_frames(glava_b200_sharded* g, const int* streams, int count, void* const* dst, const glava_b200_export* desc) {
+// The caller-buffer exports (DESIGN 4.10–4.12), global stream indices (repeats allowed): the list is split by shard, dst[i]
+// and dst_uv[i] travelling with streams[i].  Every shard's part passes the single-renderer checks, and for an overlay the
+// whole list the overlap test against itself and every shard's framebuffer (shards may share a device), before any shard
+// starts; the shards then issue at once.
+static int sharded_export(glava_b200_sharded* g, ExportKind kind, const int* streams, int count, void* const* dst,
+                          void* const* dst_uv, const glava_b200_export* desc, const glava_b200_export_scale* scale, const char* who) {
     clear_error();
-    const char* who = "glava_b200_sharded_export_frames";
-    if (!g || !desc) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
-    if (count < 1) return fail(GLAVA_B200_EINVAL, "%s: count %d < 1", who, count);
-    if (!streams || !dst) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
-    std::vector<std::vector<int>> idx(g->shards.size());
-    std::vector<std::vector<void*>> ptr(g->shards.size());
-    for (int i = 0; i < count; ++i) {
-        const int s = streams[i];
-        if (s < 0 || s >= g->batch) return fail(GLAVA_B200_EINVAL, "%s: stream %d out of range (batch %d)", who, s, g->batch);
-        for (size_t k = 0; k < g->shards.size(); ++k) {
-            const Shard* sh = g->shards[k];
-            if (s >= sh->first && s < sh->first + sh->count) { idx[k].push_back(s - sh->first); ptr[k].push_back(dst[i]); break; }
-        }
-    }
-    for (size_t k = 0; k < g->shards.size(); ++k) {
-        if (idx[k].empty()) continue;
-        const int rc = export_check(g->shards[k]->r, idx[k].data(), (int) idx[k].size(), ptr[k].data(), desc, who);
-        if (rc) return rc;
-    }
-    return broadcast(g, [&](Shard& s) {
-        const size_t k = (size_t) (std::find(g->shards.begin(), g->shards.end(), &s) - g->shards.begin());
-        if (idx[k].empty()) return 0;
-        return glava_b200_export_frames(s.r, idx[k].data(), (int) idx[k].size(), ptr[k].data(), desc, nullptr, nullptr);
-    });
-}
-
-// Scaled export (DESIGN 4.11), as glava_b200_sharded_export_frames; dst_uv[i] travels with dst[i]
-int glava_b200_sharded_export_scaled(glava_b200_sharded* g, const int* streams, int count, void* const* dst, void* const* dst_uv,
-                                     const glava_b200_export* desc, const glava_b200_export_scale* scale) {
-    clear_error();
-    const char* who = "glava_b200_sharded_export_scaled";
-    if (!g || !desc) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
-    if (count < 1) return fail(GLAVA_B200_EINVAL, "%s: count %d < 1", who, count);
-    if (!streams || !dst) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
-    std::vector<std::vector<int>> idx(g->shards.size());
-    std::vector<std::vector<void*>> ptr(g->shards.size()), uv(g->shards.size());
-    for (int i = 0; i < count; ++i) {
-        const int s = streams[i];
-        if (s < 0 || s >= g->batch) return fail(GLAVA_B200_EINVAL, "%s: stream %d out of range (batch %d)", who, s, g->batch);
-        for (size_t k = 0; k < g->shards.size(); ++k) {
-            const Shard* sh = g->shards[k];
-            if (s >= sh->first && s < sh->first + sh->count) {
-                idx[k].push_back(s - sh->first); ptr[k].push_back(dst[i]); uv[k].push_back(dst_uv ? dst_uv[i] : nullptr);
-                break;
-            }
-        }
-    }
-    for (size_t k = 0; k < g->shards.size(); ++k) {
-        if (idx[k].empty()) continue;
-        const int rc = export_scaled_check(g->shards[k]->r, idx[k].data(), (int) idx[k].size(), ptr[k].data(),
-                                           dst_uv ? uv[k].data() : nullptr, desc, scale, who);
-        if (rc) return rc;
-    }
-    return broadcast(g, [&](Shard& s) {
-        const size_t k = (size_t) (std::find(g->shards.begin(), g->shards.end(), &s) - g->shards.begin());
-        if (idx[k].empty()) return 0;
-        return glava_b200_export_scaled(s.r, idx[k].data(), (int) idx[k].size(), ptr[k].data(), dst_uv ? uv[k].data() : nullptr,
-                                        desc, scale, nullptr, nullptr);
-    });
-}
-
-// Overlay (DESIGN 4.12), as glava_b200_sharded_export_scaled; besides each shard's own checks, the rectangles of the whole
-// list must not overlap each other nor any shard's framebuffer (shards may share a device)
-int glava_b200_sharded_overlay_frames(glava_b200_sharded* g, const int* streams, int count, void* const* dst, void* const* dst_uv,
-                                      const glava_b200_export* desc) {
-    clear_error();
-    const char* who = "glava_b200_sharded_overlay_frames";
     if (!g || !desc) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
     if (count < 1) return fail(GLAVA_B200_EINVAL, "%s: count %d < 1", who, count);
     if (!streams || !dst) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
@@ -400,19 +336,33 @@ int glava_b200_sharded_overlay_frames(glava_b200_sharded* g, const int* streams,
         const RendererView v = renderer_view(g->shards[k]->r);
         fb.push_back(v.fb); fb_bytes.push_back((size_t) v.slots * (size_t) v.h * (size_t) v.w * 4);
         if (idx[k].empty()) continue;
-        const int rc = overlay_check(g->shards[k]->r, idx[k].data(), (int) idx[k].size(), ptr[k].data(), dst_uv ? uv[k].data() : nullptr,
-                                     desc, who);
+        const int rc = export_check(kind, g->shards[k]->r, idx[k].data(), (int) idx[k].size(), ptr[k].data(),
+                                    dst_uv ? uv[k].data() : nullptr, desc, scale, who);
         if (rc) return rc;
     }
-    const RendererView v0 = renderer_view(g->shards[0]->r);
-    const int rc = overlay_geometry_check(v0.w, v0.h, count, dst, dst_uv, *desc, fb.data(), fb_bytes.data(), (int) fb.size(), who);
-    if (rc) return rc;
+    if (kind == ExportKind::overlay) {
+        const RendererView v0 = renderer_view(g->shards[0]->r);
+        const int rc = overlay_geometry_check(v0.w, v0.h, count, dst, dst_uv, *desc, fb.data(), fb_bytes.data(), (int) fb.size(), who);
+        if (rc) return rc;
+    }
     return broadcast(g, [&](Shard& s) {
         const size_t k = (size_t) (std::find(g->shards.begin(), g->shards.end(), &s) - g->shards.begin());
         if (idx[k].empty()) return 0;
-        return glava_b200_overlay_frames(s.r, idx[k].data(), (int) idx[k].size(), ptr[k].data(), dst_uv ? uv[k].data() : nullptr,
-                                         desc, nullptr, nullptr);
+        return export_run(kind, s.r, idx[k].data(), (int) idx[k].size(), ptr[k].data(), dst_uv ? uv[k].data() : nullptr, desc,
+                          scale, nullptr, nullptr);
     });
+}
+
+int glava_b200_sharded_export_frames(glava_b200_sharded* g, const int* streams, int count, void* const* dst, const glava_b200_export* desc) {
+    return sharded_export(g, ExportKind::frames, streams, count, dst, nullptr, desc, nullptr, "glava_b200_sharded_export_frames");
+}
+int glava_b200_sharded_export_scaled(glava_b200_sharded* g, const int* streams, int count, void* const* dst, void* const* dst_uv,
+                                     const glava_b200_export* desc, const glava_b200_export_scale* scale) {
+    return sharded_export(g, ExportKind::scaled, streams, count, dst, dst_uv, desc, scale, "glava_b200_sharded_export_scaled");
+}
+int glava_b200_sharded_overlay_frames(glava_b200_sharded* g, const int* streams, int count, void* const* dst, void* const* dst_uv,
+                                      const glava_b200_export* desc) {
+    return sharded_export(g, ExportKind::overlay, streams, count, dst, dst_uv, desc, nullptr, "glava_b200_sharded_overlay_frames");
 }
 
 int glava_b200_sharded_textures(glava_b200_sharded* g, uint16_t* out_l, uint16_t* out_r) {

@@ -1,6 +1,6 @@
 """Frame export (DESIGN 4.10) on the host: the pixel arithmetic of export_core.h through a g++ shim, and the refusals and
 enqueued work of glava_b200_export_frames / _export_bytes through capi.cu and export.cpp built against the fake runtime of
-tests/fakecuda.
+tests/fakecuda (tests/export_fake.py).
 
 The shim's t_export walks one framebuffer slot the way export_kernels.cu does (row pairs, 128-pixel strips, quads, the
 dirty-row marks deciding which rows are read) with the same core functions, so the layout and the mark logic are checked
@@ -12,7 +12,8 @@ import subprocess
 import numpy as np
 import pytest
 
-from tests import fakecuda
+from tests import export_fake
+from tests.export_fake import desc_of
 
 CSRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "glava_b200", "csrc")
 RGBA, BGRA, NV12, OVER = 0, 1, 2, 1
@@ -281,85 +282,13 @@ def test_mark_aware_walk_equals_a_full_read(shim, w, h, rows, fmt):
 
 
 # ---- refusals and enqueued work through the fake runtime -----------------------------------------------------------------
-# capi.cu, export.cpp and config.cpp built with g++ against tests/fakecuda's runtime and launchers, plus what the export adds:
-# cudaPointerGetAttributes (device memory = the pointers the test registers) and a launch_export that counts its calls
-FAKE_EXPORT = r"""
-#include "internal.h"
-#include <set>
-static std::set<const void*> g_dev;
-static long g_exports = 0;
-extern "C" void export_fake_device(const void* p) { g_dev.insert(p); }
-extern "C" long export_fake_launches(void) { return g_exports; }
-extern "C" cudaError_t cudaPointerGetAttributes(cudaPointerAttributes* a, const void* p) {
-    *a = cudaPointerAttributes();
-    a->type = g_dev.count(p) ? cudaMemoryTypeDevice : cudaMemoryTypeUnregistered;
-    a->device = 0;
-    return cudaSuccess;
-}
-namespace glb {
-int launch_export(const ExportArgs& a, void*) {
-    ++g_exports;
-    return a.fb && a.list && a.count > 0 && (!a.marks || a.mark_rows > 0) ? 0 : fail(GLAVA_B200_EINVAL, "export launch: missing buffers");
-}
-}
-"""
-
-
+# capi.cu, export.cpp and config.cpp built with g++ against tests/fakecuda's runtime (tests/export_fake.py)
 @pytest.fixture(scope="module")
-def fake(tmp_path_factory):
-    inc = fakecuda.cuda_include()
-    if inc is None:
+def fake():
+    L = export_fake.lib()
+    if L is None:
         pytest.skip("no CUDA toolkit headers")
-    from glava_b200.api import Export, Params
-    d = tmp_path_factory.mktemp("export_fake")
-    src, so = d / "export_fake.cpp", d / "libexport_fake.so"
-    src.write_text(FAKE_EXPORT)
-    subprocess.run(["g++", "-O1", "-std=c++17", "-fPIC", "-shared", "-ffp-contract=off", "-Wno-unknown-pragmas", "-I", inc,
-                    "-I", CSRC, "-x", "c++", "-include", "cuda_runtime.h", "-o", str(so),
-                    os.path.join(CSRC, "capi.cu"), os.path.join(CSRC, "export.cpp"), os.path.join(CSRC, "config.cpp"),
-                    os.path.join(fakecuda.HERE, "fakecuda.cpp"), str(src), "-lpthread", "-Wl,-Bsymbolic"], check=True)
-    L = C.CDLL(str(so))
-    vp, i32, P = C.c_void_p, C.c_int, C.POINTER(Params)
-    sig = {
-        "glava_b200_default_params": (i32, [P, C.c_char_p]), "glava_b200_new": (vp, [P, i32, i32]),
-        "glava_b200_destroy": (None, [vp]), "glava_b200_reconfigure": (i32, [vp, P]), "glava_b200_get_params": (i32, [vp, P]),
-        "glava_b200_update": (i32, [vp, vp, vp, C.c_size_t, i32]), "glava_b200_last_error": (C.c_char_p, []),
-        "glava_b200_set_abort_hook": (None, [vp]), "glava_b200_export_frames": (i32, [vp, vp, i32, vp, C.POINTER(Export), vp, vp]),
-        "glava_b200_export_bytes": (i32, [vp, C.POINTER(Export), C.POINTER(C.c_size_t)]),
-        "cudaMalloc": (i32, [C.POINTER(vp), C.c_size_t]), "cudaFree": (i32, [vp]), "cudaEventCreate": (i32, [C.POINTER(vp)]),
-        "cudaEventDestroy": (i32, [vp]), "fake_trace": (C.c_char_p, []), "fake_fail_at": (None, [C.c_long]),
-        "fake_live": (C.c_long, [i32]), "export_fake_device": (None, [vp]), "export_fake_launches": (C.c_long, []),
-    }
-    for name, (res, args) in sig.items():
-        fn = getattr(L, name)
-        fn.restype, fn.argtypes = res, args
-    L._quiet = C.CFUNCTYPE(None, C.c_char_p)(lambda msg: None)
-    L.glava_b200_set_abort_hook(C.cast(L._quiet, vp))
-
-    def renderer(module="bars", **kw):
-        p = Params()
-        assert L.glava_b200_default_params(C.byref(p), module.encode()) == 0
-        for k, v in kw.items():
-            setattr(p, k, v)
-        h = L.glava_b200_new(C.byref(p), 2, 0)
-        assert h, L.glava_b200_last_error()
-        return C.c_void_p(h), p
-
-    def device_buf(nbytes=1 << 16):
-        b = C.c_void_p()
-        assert L.cudaMalloc(C.byref(b), nbytes) == 0
-        L.export_fake_device(b)
-        return b
-
-    L.renderer, L.device_buf = renderer, device_buf
     return L
-
-
-def desc_of(fmt, pitch, flags=0, uv=0):
-    from glava_b200.api import Export
-    d = Export()
-    d.format, d.flags, d.pitch, d.uv_offset = fmt, flags, pitch, uv
-    return d
 
 
 def _export(L, h, streams, dsts, d, after=None, done=None):

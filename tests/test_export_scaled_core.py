@@ -1,16 +1,16 @@
 """Scaled and cropped export (DESIGN 4.11) on the host: the area average of export_core.h through a g++ shim that walks one
 framebuffer slot the way export_scaled_kernel does (runs of 32 output columns, strip by strip, band by band of the
 dirty-row marks, aligned quads), against an independent numpy restatement built from interval overlaps, bit for bit; the exactness of the
-reciprocal division over its whole range; and the refusals and enqueued work of glava_b200_export_scaled through capi.cu,
-export.cpp and export_scaled.cpp built against the fake runtime of tests/fakecuda."""
+reciprocal division over its whole range; and the refusals and enqueued work of glava_b200_export_scaled through capi.cu
+and export.cpp built against the fake runtime of tests/fakecuda (tests/export_fake.py)."""
 import ctypes as C
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
-from tests import fakecuda
+from tests import export_fake
+from tests.export_fake import desc_of
 from tests.test_export_core import SHIM as PLAIN_SHIM
 from tests.test_export_core import BGRA, CSRC, NV12, RGBA, export, marked_frame, nv12_np, over_np, pack, premultiplied
 
@@ -270,93 +270,12 @@ def test_marks_are_honoured_and_skipped_rows_never_read(shim, w, h, rows, crop, 
 
 
 # ---- refusals and enqueued work through the fake runtime -----------------------------------------------------------------
-FAKE_EXPORT = r"""
-#include "internal.h"
-#include <set>
-static std::set<const void*> g_dev;
-static long g_exports = 0;
-static glb::ScaledArgs g_last;
-extern "C" void export_fake_device(const void* p) { g_dev.insert(p); }
-extern "C" long export_fake_launches(void) { return g_exports; }
-extern "C" void export_fake_last(int* out) {
-    out[0] = g_last.src_x; out[1] = g_last.src_y; out[2] = g_last.src_w; out[3] = g_last.src_h; out[4] = g_last.out_w;
-    out[5] = g_last.out_h; out[6] = g_last.count; out[7] = g_last.over;
-}
-extern "C" cudaError_t cudaPointerGetAttributes(cudaPointerAttributes* a, const void* p) {
-    *a = cudaPointerAttributes();
-    a->type = g_dev.count(p) ? cudaMemoryTypeDevice : cudaMemoryTypeUnregistered;
-    a->device = 0;
-    return cudaSuccess;
-}
-namespace glb {
-int launch_export(const ExportArgs& a, void*) { ++g_exports; return a.fb && a.list ? 0 : fail(GLAVA_B200_EINVAL, "missing buffers"); }
-int launch_export_scaled(const ScaledArgs& a, void*) {
-    ++g_exports; g_last = a;
-    return a.fb && a.list && a.count > 0 && (!a.marks || a.mark_rows > 0) ? 0 : fail(GLAVA_B200_EINVAL, "scaled launch: missing buffers");
-}
-}
-"""
-
-
 @pytest.fixture(scope="module")
-def fake(tmp_path_factory):
-    inc = fakecuda.cuda_include()
-    if inc is None:
+def fake():
+    L = export_fake.lib()
+    if L is None:
         pytest.skip("no CUDA toolkit headers")
-    from glava_b200.api import Export, ExportScale, Params
-    d = tmp_path_factory.mktemp("export_scaled_fake")
-    src, so = d / "export_fake.cpp", d / "libexport_scaled_fake.so"
-    src.write_text(FAKE_EXPORT)
-    subprocess.run(["g++", "-O1", "-std=c++17", "-fPIC", "-shared", "-ffp-contract=off", "-Wno-unknown-pragmas", "-I", inc,
-                    "-I", CSRC, "-x", "c++", "-include", "cuda_runtime.h", "-o", str(so),
-                    os.path.join(CSRC, "capi.cu"), os.path.join(CSRC, "export.cpp"), os.path.join(CSRC, "export_scaled.cpp"),
-                    os.path.join(CSRC, "config.cpp"), os.path.join(fakecuda.HERE, "fakecuda.cpp"), str(src), "-lpthread",
-                    "-Wl,-Bsymbolic"], check=True)
-    L = C.CDLL(str(so))
-    vp, i32, P = C.c_void_p, C.c_int, C.POINTER(Params)
-    sig = {
-        "glava_b200_default_params": (i32, [P, C.c_char_p]), "glava_b200_new": (vp, [P, i32, i32]),
-        "glava_b200_destroy": (None, [vp]), "glava_b200_reconfigure": (i32, [vp, P]),
-        "glava_b200_update": (i32, [vp, vp, vp, C.c_size_t, i32]), "glava_b200_last_error": (C.c_char_p, []),
-        "glava_b200_set_abort_hook": (None, [vp]),
-        "glava_b200_export_scaled": (i32, [vp, vp, i32, vp, vp, C.POINTER(Export), C.POINTER(ExportScale), vp, vp]),
-        "glava_b200_export_scaled_bytes": (i32, [vp, C.POINTER(Export), C.POINTER(ExportScale), C.POINTER(C.c_size_t)]),
-        "glava_b200_export_frames": (i32, [vp, vp, i32, vp, C.POINTER(Export), vp, vp]),
-        "cudaMalloc": (i32, [C.POINTER(vp), C.c_size_t]), "cudaFree": (i32, [vp]), "cudaEventCreate": (i32, [C.POINTER(vp)]),
-        "cudaEventDestroy": (i32, [vp]), "fake_trace": (C.c_char_p, []), "fake_fail_at": (None, [C.c_long]),
-        "fake_live": (C.c_long, [i32]), "export_fake_device": (None, [vp]), "export_fake_launches": (C.c_long, []),
-        "export_fake_last": (None, [vp]),
-    }
-    for name, (res, args) in sig.items():
-        fn = getattr(L, name)
-        fn.restype, fn.argtypes = res, args
-    L._quiet = C.CFUNCTYPE(None, C.c_char_p)(lambda msg: None)
-    L.glava_b200_set_abort_hook(C.cast(L._quiet, vp))
-
-    def renderer(module="bars", **kw):
-        p = Params()
-        assert L.glava_b200_default_params(C.byref(p), module.encode()) == 0
-        for k, v in kw.items():
-            setattr(p, k, v)
-        h = L.glava_b200_new(C.byref(p), 2, 0)
-        assert h, L.glava_b200_last_error()
-        return C.c_void_p(h), p
-
-    def device_buf(nbytes=1 << 16):
-        b = C.c_void_p()
-        assert L.cudaMalloc(C.byref(b), nbytes) == 0
-        L.export_fake_device(b)
-        return b
-
-    L.renderer, L.device_buf = renderer, device_buf
     return L
-
-
-def desc_of(fmt, pitch, flags=0, uv=0):
-    from glava_b200.api import Export
-    d = Export()
-    d.format, d.flags, d.pitch, d.uv_offset = fmt, flags, pitch, uv
-    return d
 
 
 def scale_of(out, crop=(0, 0, 0, 0)):

@@ -116,10 +116,8 @@ def test_identities_with_export_frames(built, native):
             assert torch.equal(img, r.export_frames([1, 0], "nv12")), "nv12"
 
 
-@pytest.mark.parametrize("item", ["band", "pair"])
-def test_bars_1080p_with_live_stale_and_no_marks(built, item, monkeypatch):
-    if item == "pair":                                                 # row-pair items under marks as well
-        monkeypatch.setenv("GLAVA_B200_OVERLAY_ITEM", "pair")
+@pytest.mark.parametrize("item", ["band"])                            # the only item shape under native opacity with marks
+def test_bars_1080p_with_live_stale_and_no_marks(built, item):
     p = g.default_params("bars", n=4096, w=1920, h=1080)
     p.lazy_smooth = 1
     with g.Renderer(p, batch=3) as r:

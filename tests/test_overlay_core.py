@@ -2,16 +2,16 @@
 through a g++ shim against numpy restatements, exhaustively where the space allows, with the float64 bound of the Y'CbCr
 blend and the identities that tie the overlay to the export; a g++ walk of overlay_kernel's loops (band items under the
 dirty-row marks, row-pair items otherwise) bit for bit against the restatement over sentinel-filled images; the overlap
-test against brute force; and the refusals and enqueued work of glava_b200_overlay_frames through capi.cu, export.cpp and
-overlay.cpp built against the fake runtime of tests/fakecuda."""
+test against brute force; and the refusals and enqueued work of glava_b200_overlay_frames through capi.cu and export.cpp
+built against the fake runtime of tests/fakecuda (tests/export_fake.py)."""
 import ctypes as C
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
-from tests import fakecuda
+from tests import export_fake
+from tests.export_fake import desc_of
 from tests.test_export_core import SHIM as PLAIN_SHIM
 from tests.test_export_core import BGRA, CSRC, NV12, RGBA, bt709_fixed, export, marked_frame, nv12_np, over_np, pack, premultiplied
 
@@ -420,93 +420,11 @@ def brute_meets(rects, P, B, f0, f1):
     return any(p + k * P < f1 and p + k * P + B > f0 for p, n in rects for k in range(n))
 
 
-FAKE = r"""
-#include "internal.h"
-#include <map>
-static std::map<uintptr_t, size_t> g_dev;                 // device allocations: start -> bytes
-static long g_launches = 0;
-static glb::OverlayArgs g_last;
-extern "C" void export_fake_device(const void* p, size_t n) { g_dev[(uintptr_t) p] = n; }
-extern "C" long export_fake_launches(void) { return g_launches; }
-extern "C" void overlay_fake_last(int* out) { out[0] = g_last.count; out[1] = g_last.band; out[2] = g_last.native; out[3] = g_last.format; }
-extern "C" cudaError_t cudaPointerGetAttributes(cudaPointerAttributes* a, const void* p) {
-    *a = cudaPointerAttributes();
-    auto it = g_dev.upper_bound((uintptr_t) p);            // a pointer anywhere inside an allocation
-    const bool dev = it != g_dev.begin() && (uintptr_t) p < std::prev(it)->first + std::prev(it)->second;
-    a->type = dev ? cudaMemoryTypeDevice : cudaMemoryTypeUnregistered;
-    a->device = 0;
-    return cudaSuccess;
-}
-// overlay_geometry_check on plain addresses: NV12 (chroma rows at uv[i]) when uv is non-null
-extern "C" int t_geometry(int w, int h, int count, const uintptr_t* dst, const uintptr_t* uv, size_t pitch, uintptr_t fb, size_t fb_bytes) {
-    glava_b200_export d = {};
-    d.format = uv ? GLAVA_B200_EXPORT_NV12 : GLAVA_B200_EXPORT_RGBA;
-    d.pitch = pitch;
-    const uint8_t* f = (const uint8_t*) fb;
-    return glb::overlay_geometry_check(w, h, count, (void* const*) dst, (void* const*) uv, d, &f, &fb_bytes, 1, "t_geometry");
-}
-namespace glb {
-int launch_export(const ExportArgs& a, void*) { ++g_launches; return a.fb && a.list ? 0 : fail(GLAVA_B200_EINVAL, "missing buffers"); }
-int launch_overlay(const OverlayArgs& a, void*) {
-    ++g_launches; g_last = a;
-    return a.fb && a.list && a.count > 0 && (!a.band || (a.marks && a.mark_rows > 0 && a.native)) ? 0
-                                                                                                : fail(GLAVA_B200_EINVAL, "overlay launch: bad arguments");
-}
-}
-"""
-
-
 @pytest.fixture(scope="module")
-def fake(tmp_path_factory):
-    inc = fakecuda.cuda_include()
-    if inc is None:
+def fake():
+    L = export_fake.lib()
+    if L is None:
         pytest.skip("no CUDA toolkit headers")
-    from glava_b200.api import Export, Params
-    d = tmp_path_factory.mktemp("overlay_fake")
-    src, so = d / "overlay_fake.cpp", d / "liboverlay_fake.so"
-    src.write_text(FAKE)
-    subprocess.run(["g++", "-O1", "-std=c++17", "-fPIC", "-shared", "-ffp-contract=off", "-Wno-unknown-pragmas", "-I", inc,
-                    "-I", CSRC, "-x", "c++", "-include", "cuda_runtime.h", "-o", str(so),
-                    os.path.join(CSRC, "capi.cu"), os.path.join(CSRC, "export.cpp"), os.path.join(CSRC, "overlay.cpp"),
-                    os.path.join(CSRC, "config.cpp"), os.path.join(fakecuda.HERE, "fakecuda.cpp"), str(src), "-lpthread",
-                    "-Wl,-Bsymbolic"], check=True)
-    L = C.CDLL(str(so))
-    vp, i32, P = C.c_void_p, C.c_int, C.POINTER(Params)
-    sig = {
-        "glava_b200_default_params": (i32, [P, C.c_char_p]), "glava_b200_new": (vp, [P, i32, i32]),
-        "glava_b200_destroy": (None, [vp]), "glava_b200_reconfigure": (i32, [vp, P]),
-        "glava_b200_update": (i32, [vp, vp, vp, C.c_size_t, i32]), "glava_b200_last_error": (C.c_char_p, []),
-        "glava_b200_set_abort_hook": (None, [vp]), "glava_b200_framebuffer_device": (vp, [vp]),
-        "glava_b200_overlay_frames": (i32, [vp, vp, i32, vp, vp, C.POINTER(Export), vp, vp]),
-        "glava_b200_export_frames": (i32, [vp, vp, i32, vp, C.POINTER(Export), vp, vp]),
-        "cudaMalloc": (i32, [C.POINTER(vp), C.c_size_t]), "cudaFree": (i32, [vp]), "cudaEventCreate": (i32, [C.POINTER(vp)]),
-        "cudaEventDestroy": (i32, [vp]), "fake_trace": (C.c_char_p, []), "fake_fail_at": (None, [C.c_long]),
-        "fake_live": (C.c_long, [i32]), "export_fake_device": (None, [vp, C.c_size_t]), "export_fake_launches": (C.c_long, []),
-        "overlay_fake_last": (None, [vp]),
-        "t_geometry": (i32, [i32, i32, i32, vp, vp, C.c_size_t, C.c_size_t, C.c_size_t]),
-    }
-    for name, (res, args) in sig.items():
-        fn = getattr(L, name)
-        fn.restype, fn.argtypes = res, args
-    L._quiet = C.CFUNCTYPE(None, C.c_char_p)(lambda msg: None)
-    L.glava_b200_set_abort_hook(C.cast(L._quiet, vp))
-
-    def renderer(module="bars", batch=2, **kw):
-        p = Params()
-        assert L.glava_b200_default_params(C.byref(p), module.encode()) == 0
-        for k, v in kw.items():
-            setattr(p, k, v)
-        h = L.glava_b200_new(C.byref(p), batch, 0)
-        assert h, L.glava_b200_last_error()
-        return C.c_void_p(h), p
-
-    def device_buf(nbytes=1 << 16):
-        b = C.c_void_p()
-        assert L.cudaMalloc(C.byref(b), nbytes) == 0
-        L.export_fake_device(b, nbytes)
-        return b
-
-    L.renderer, L.device_buf = renderer, device_buf
     return L
 
 
@@ -553,13 +471,6 @@ def test_a_mosaic_of_1024_tiles_checks_fast(fake):
     dst[700] = dst[699] + 16                                         # one tile shifted onto its neighbour
     assert fake.t_geometry(tw, th, 1024, (C.c_size_t * 1024)(*dst), u, P, 1 << 20, 4096) != 0
     assert "entry 699" in fake.glava_b200_last_error().decode()
-
-
-def desc_of(fmt, pitch, flags=0, uv=0):
-    from glava_b200.api import Export
-    d = Export()
-    d.format, d.flags, d.pitch, d.uv_offset = fmt, flags, pitch, uv
-    return d
 
 
 def _overlay(L, h, streams, dsts, d, uvs=None, after=None, done=None):

@@ -1,9 +1,8 @@
 """Overlay rates (glava_b200_overlay_frames, DESIGN 4.12) on one GPU, with the card and its power limit read in the same run.
 Per workload (bench.py's inputs and warm-up), device time (torch.profiler: every kernel and copy a leg enqueues, per call;
 the CUDA-event wall time beside it) of 1024 streams composited onto same-size images, legs
-alternated over rounds: the overlay in NV12 and RGBA with band items (the default under marks) and with row-pair items
-(GLAVA_B200_OVERLAY_ITEM=pair), export_frames of the same streams in NV12 and RGBA, and the caller-side baseline: an RGBA
-export into scratch followed by a torch blend onto the images.  Bytes per call = the framebuffer rows the marks let through
+alternated over rounds: the overlay in NV12 and RGBA, export_frames of the same streams in NV12 and RGBA, and the
+caller-side baseline: an RGBA export into scratch followed by a torch blend onto the images.  Bytes per call = the framebuffer rows the marks let through
 (counted from read-back frames of a stream sample as tools/export_bench.py counts them; every row for modules without
 marks) plus the destination bytes read and written, over the median time, against the data sheet's 3.35 TB/s unless
 MEASURED_PEAKS.json gives a peak.  Overlay legs count the destination bytes under non-zero quads twice (read and written).
@@ -23,10 +22,9 @@ from bench import HOP, hbm_peak, workload      # noqa: E402  (stdlib only at imp
 from tools.export_bench import read_fraction   # noqa: E402
 from tools.style_bench import card             # noqa: E402
 
-# (name, kind, format): kind "overlay" (band items), "overlay_pair" (row-pair items), "export" (export_frames), "baseline"
-LEGS = (("overlay_nv12", "overlay", "nv12"), ("overlay_pair_nv12", "overlay_pair", "nv12"), ("export_nv12", "export", "nv12"),
-        ("overlay_rgba", "overlay", "rgba"), ("overlay_pair_rgba", "overlay_pair", "rgba"), ("export_rgba", "export", "rgba"),
-        ("baseline_rgba", "baseline", "rgba"))
+# (name, kind, format): kind "overlay", "export" (export_frames), "baseline"
+LEGS = (("overlay_nv12", "overlay", "nv12"), ("export_nv12", "export", "nv12"), ("overlay_rgba", "overlay", "rgba"),
+        ("export_rgba", "export", "rgba"), ("baseline_rgba", "baseline", "rgba"))
 COUNT = 1024
 
 
@@ -84,12 +82,10 @@ def main():
             def plan(leg):
                 """the leg as one call with everything Python decides computed once (host time then stays off the clock)"""
                 key, kind, fmt = leg
-                if kind in ("overlay", "overlay_pair"):
+                if kind == "overlay":
                     s, desc, dst, uv = r._overlay_plan(streams, imgs[fmt], None, fmt)
-                    item = "pair" if kind == "overlay_pair" else "band"
 
                     def call():
-                        os.environ["GLAVA_B200_OVERLAY_ITEM"] = item
                         g.api._check(r._L.glava_b200_overlay_frames(r._h, s.ctypes.data, COUNT, dst, uv, C.byref(desc), None, None))
                     return call
                 out = r.export_frames(streams, "rgba" if kind == "baseline" else fmt)
@@ -112,7 +108,6 @@ def main():
             for leg in LEGS:                                  # allocates, warms the list buffers and the kernels
                 calls[leg[0]] = plan(leg)
                 calls[leg[0]]()
-            os.environ.pop("GLAVA_B200_OVERLAY_ITEM", None)
             torch.cuda.synchronize()
             sample = np.linspace(0, batch - 1, 32).astype(int)
             frac = read_fraction(g, r, p, module, sample)
@@ -134,7 +129,6 @@ def main():
                                  for e in prof.key_averages())
                     times[leg[0]].append(dev_us / 1e3 / args.reps)
                     walls[leg[0]].append(a.elapsed_time(b) / args.reps)
-            os.environ.pop("GLAVA_B200_OVERLAY_ITEM", None)
             legs = {}
             for key, kind, fmt in LEGS:
                 ms = float(np.median(times[key]))
