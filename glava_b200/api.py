@@ -126,6 +126,12 @@ class ExportScale(C.Structure):
                 ("out_h", C.c_int)]
 
 
+class ExportRung(C.Structure):
+    """glava_b200_export_rung: one rung of an encoder ladder — its destinations' descriptor and its scale rectangle"""
+    _fields_ = [("desc", Export), ("scale", ExportScale)]
+
+
+LADDER_MAX = 8
 EXPORT_RGBA, EXPORT_BGRA, EXPORT_NV12 = 0, 1, 2
 EXPORT_OVER = 1
 EXPORT_FORMATS = {"rgba": EXPORT_RGBA, "bgra": EXPORT_BGRA, "nv12": EXPORT_NV12}
@@ -256,6 +262,8 @@ def lib():
     L.glava_b200_sharded_export_scaled.argtypes = [vp, vp, i32, vp, vp, C.POINTER(Export), C.POINTER(ExportScale)]
     L.glava_b200_overlay_frames.argtypes = [vp, vp, i32, vp, vp, C.POINTER(Export), vp, vp]
     L.glava_b200_sharded_overlay_frames.argtypes = [vp, vp, i32, vp, vp, C.POINTER(Export)]
+    L.glava_b200_export_ladder.argtypes = [vp, vp, i32, C.POINTER(ExportRung), i32, vp, vp, vp, vp]
+    L.glava_b200_sharded_export_ladder.argtypes = [vp, vp, i32, C.POINTER(ExportRung), i32, vp, vp]
     _lib = L
     # errors surface as Python exceptions; keep stderr quiet
     _quiet = C.CFUNCTYPE(None, cp)(lambda msg: None)
@@ -466,6 +474,33 @@ class _FrameExport:
         desc.pitch = pitch
         desc.uv_offset = pitch * h if nv12 else 0
         return s, desc, (C.c_void_p * max(count, 1))(*dst), result
+
+    def _ladder_plan(self, streams, rungs, out, device_of):
+        """-> (stream list, ExportRung array, nrungs, [count][nrungs] dst pointers, [one result per rung]) of an encoder
+        ladder (DESIGN 4.13): each rung planned by _export_plan as export_scaled plans it.  rungs: dicts with export_scaled's
+        keywords size (None: the frame's), crop, fmt (default "nv12"), over and background; out: None or one entry per
+        rung in any form export_scaled takes"""
+        rungs = list(rungs)
+        outs = [None] * len(rungs) if out is None else list(out)
+        if len(outs) != len(rungs):
+            raise ValueError(f"out: one entry per rung ({len(rungs)}), got {len(outs)}")
+        p = self.params
+        s = np.ascontiguousarray(np.asarray(list(streams), dtype=np.int64).reshape(-1), dtype=np.int32)
+        arr = (ExportRung * max(len(rungs), 1))()
+        ptrs, results = [], []
+        for j, (rung, o) in enumerate(zip(rungs, outs)):
+            unknown = set(rung) - {"size", "crop", "fmt", "over", "background"}
+            if unknown:
+                raise ValueError(f"rungs[{j}]: unknown keys {sorted(unknown)}")
+            size = rung.get("size") or (p.w, p.h)
+            _, desc, dst, result = self._export_plan(s, rung.get("fmt", "nv12"), rung.get("over", False),
+                                                     rung.get("background", (0, 0, 0)), o, device_of, size)
+            arr[j].desc, arr[j].scale = desc, _export_scale(size, rung.get("crop"))
+            ptrs.append(dst)
+            results.append(result)
+        count, n = int(s.shape[0]), len(rungs)
+        dst = (C.c_void_p * max(count * n, 1))(*[ptrs[j][i] for i in range(count) for j in range(n)])
+        return s, arr, n, dst, results
 
     def _overlay_plan(self, streams, images, at, fmt):
         """-> (stream list, Export, dst pointers, dst_uv pointers or None) of an overlay (DESIGN 4.12).  images: one uint8
@@ -853,6 +888,17 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
                                                                     C.byref(sc), a, d), after, done)
         return result
 
+    def export_ladder(self, streams, rungs, out=None, after=None, done=None):
+        """Several sizes of each frame in one launch that reads each source row about once (glava_b200_export_ladder), for
+        an encoder ladder: rungs = [dict(size=(w, h) or None for the frame's, crop=None, fmt="nv12", over=False,
+        background=(0, 0, 0)), ...], at most LADDER_MAX.  Rung j is exactly export_scaled(streams, **rungs[j]) at this
+        point in call order.  out: None or one entry per rung in any form export_scaled takes.  Returns one result per rung,
+        shaped as export_scaled returns it; after / done and the ordering against torch's current stream as export_frames."""
+        s, arr, n, dst, results = self._ladder_plan(streams, rungs, out, lambda stream: self.device)
+        self._ordered(lambda a, d: self._L.glava_b200_export_ladder(self._h, s.ctypes.data, s.shape[0], arr, n, dst, None, a, d),
+                      after, done)
+        return results
+
     def overlay_frames(self, streams, images, at=None, fmt="nv12", after=None, done=None):
         """The current frames of `streams` composited in place onto the caller's images (glava_b200_overlay_frames): under
         native opacity premultiplied "over" the image's pixels, blended in Y'CbCr for NV12; under any other opacity the
@@ -1024,6 +1070,17 @@ class ShardedRenderer(_StreamState, _StreamStyles, _FrameExport):
             torch.cuda.current_stream(d).synchronize()
         _check(self._L.glava_b200_sharded_export_scaled(self._h, s.ctypes.data, s.shape[0], dst, None, C.byref(desc), C.byref(sc)))
         return result
+
+    def export_ladder(self, streams, rungs, out=None):
+        """Renderer.export_ladder with global stream indices (glava_b200_sharded_export_ladder), destinations placed as
+        export_frames places them; the frames are complete after sync()."""
+        import torch
+        device_of = self._device_of()
+        s, arr, n, dst, results = self._ladder_plan(streams, rungs, out, device_of)
+        for d in sorted({device_of(int(x)) for x in s}):
+            torch.cuda.current_stream(d).synchronize()
+        _check(self._L.glava_b200_sharded_export_ladder(self._h, s.ctypes.data, s.shape[0], arr, n, dst, None))
+        return results
 
     def overlay_frames(self, streams, images, at=None, fmt="nv12"):
         """Renderer.overlay_frames with global stream indices (glava_b200_sharded_overlay_frames), each image on the device

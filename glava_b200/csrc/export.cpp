@@ -3,10 +3,10 @@
 // shard starts.  The three calls share one check, one list fill and one enqueue; what differs by kind is the output size
 // (the frame, or the scale rectangle's), the flags allowed, and the kernel's own argument fields.  It reads the renderer
 // through capi.cu's renderer_view and keeps its list buffers in the renderer's attachment slot; the kernels are
-// export_kernels.cu.
+// export_kernels.cu.  The list buffers and the enqueue are export_list.h's, shared with the ladder (export_ladder.cpp).
 #include "internal.h"
-#include "cuda_owner.h"
 #include "export_core.h"
+#include "export_list.h"
 
 #include <cuda_runtime.h>
 
@@ -16,45 +16,9 @@
 
 using namespace glb;
 
-#define CU(call)                                                                                      \
-    do {                                                                                              \
-        cudaError_t e_ = (call);                                                                      \
-        if (e_ != cudaSuccess) return fail(GLAVA_B200_ECUDA, "%s: %s", #call, cudaGetErrorString(e_)); \
-    } while (0)
-
 namespace {
 
 const char* const kCallName[] = { "glava_b200_export_frames", "glava_b200_export_scaled", "glava_b200_overlay_frames" };
-
-// The entry list of one renderer: it goes up from four pinned buffers in turn into one device list (read by the kernel on
-// the raster stream, behind the copy that fills it), allocated on first use and grown to the longest list, in bytes so
-// that either entry type (ExportEntry, ExportEntryUV) fits; ev[i]: the copy out of h[i] is done
-struct ExportList {
-    PinnedBuf<uint8_t> h[4]; DevBuf<uint8_t> d; Event ev[4]; int cur = 0; size_t cap = 0;
-};
-void release_list(void* p) { delete static_cast<ExportList*>(p); }
-
-// room for `bytes` of list (the buffers are replaced only once the raster stream has drained)
-int list_room(const RendererView& v, size_t bytes, ExportList** out) {
-    if (!*v.attach) {
-        *v.attach = new ExportList();
-        *v.attach_free = release_list;
-    }
-    ExportList* L = static_cast<ExportList*>(*v.attach);
-    *out = L;
-    int rc;
-    if (!L->ev[3].get())                                    // created last: the four events are complete
-        for (Event& e : L->ev) if ((rc = e.create()) != 0) return rc;
-    if (bytes <= L->cap) return 0;
-    CU(cudaStreamSynchronize((cudaStream_t) v.stream));
-    L->cap = 0;
-    size_t cap = 64 * sizeof(ExportEntry);
-    while (cap < bytes) cap *= 2;
-    if ((rc = L->d.alloc(cap)) != 0) return rc;
-    for (PinnedBuf<uint8_t>& h : L->h) if ((rc = h.alloc(cap)) != 0) return rc;
-    L->cap = cap;
-    return 0;
-}
 
 // pitch and uv_offset against a w x h output (`what` names it in the message: "frame" / "output")
 int desc_size(int w, int h, const glava_b200_export& d, const char* what, const char* who) {
@@ -136,10 +100,6 @@ void common_args(Args& a, const RendererView& v, const void* d_list, int count, 
     a.pitch = d.pitch;
 }
 
-uint32_t background(const glava_b200_export& d) {
-    return (uint32_t) d.background[0] | ((uint32_t) d.background[1] << 8) | ((uint32_t) d.background[2] << 16);
-}
-
 // One plane of one entry's rectangle: `rows` rows of the common row bytes, the common pitch apart, from byte address p
 struct Rect { uintptr_t p; size_t rows; int entry; bool uv; };
 
@@ -161,6 +121,33 @@ bool rect_meets_range(const Rect& r, size_t P, size_t B, uintptr_t f0, uintptr_t
 }  // namespace
 
 namespace glb {
+static void release_list(void* p) { delete static_cast<ExportList*>(p); }
+
+int list_room(const RendererView& v, size_t bytes, ExportList** out) {
+    if (!*v.attach) {
+        *v.attach = new ExportList();
+        *v.attach_free = release_list;
+    }
+    ExportList* L = static_cast<ExportList*>(*v.attach);
+    *out = L;
+    int rc;
+    if (!L->ev[3].get())                                    // created last: the four events are complete
+        for (Event& e : L->ev) if ((rc = e.create()) != 0) return rc;
+    if (bytes <= L->cap) return 0;
+    CU(cudaStreamSynchronize((cudaStream_t) v.stream));
+    L->cap = 0;
+    size_t cap = 64 * sizeof(ExportEntry);
+    while (cap < bytes) cap *= 2;
+    if ((rc = L->d.alloc(cap)) != 0) return rc;
+    for (PinnedBuf<uint8_t>& h : L->h) if ((rc = h.alloc(cap)) != 0) return rc;
+    L->cap = cap;
+    return 0;
+}
+
+uint32_t background(const glava_b200_export& d) {
+    return (uint32_t) d.background[0] | ((uint32_t) d.background[1] << 8) | ((uint32_t) d.background[2] << 16);
+}
+
 int overlay_geometry_check(int w, int h, int count, void* const* dst, void* const* dst_uv, const glava_b200_export& desc,
                            const uint8_t* const* fb, const size_t* fb_bytes, int nfb, const char* who) {
     const bool nv12 = desc.format == GLAVA_B200_EXPORT_NV12;
@@ -240,40 +227,32 @@ int export_run(ExportKind kind, glava_b200* r, const int* streams, int count, vo
         if (kind == ExportKind::frames) reinterpret_cast<ExportEntry*>(host)[i] = { d, slot, 0 };
         else reinterpret_cast<ExportEntryUV*>(host)[i] = { d, !nv12 ? nullptr : dst_uv ? (uint8_t*) dst_uv[i] : d + uv_offset, slot, 0 };
     }
-    cudaStream_t st = (cudaStream_t) v.stream;
-    const int k = L->cur;
-    if (after_event) CU(cudaStreamWaitEvent(st, (cudaEvent_t) after_event, 0));
-    CU(cudaMemcpyAsync(L->d, L->h[k], bytes, cudaMemcpyHostToDevice, st));
-    CU(cudaEventRecord(L->ev[k], st));
-    L->cur = (k + 1) & 3;
-    const void* d_list = L->d;
-    if (kind == ExportKind::frames) {
-        ExportArgs a = {};
-        common_args(a, v, d_list, count, *desc);
-        a.over = nv12 || (desc->flags & GLAVA_B200_EXPORT_OVER) ? 1 : 0;
-        a.bg = background(*desc);
-        a.uv_offset = uv_offset;
-        rc = launch_export(a, v.stream);
-    } else if (kind == ExportKind::scaled) {
-        ScaledArgs a = {};
-        common_args(a, v, d_list, count, *desc);
-        a.over = nv12 || (desc->flags & GLAVA_B200_EXPORT_OVER) ? 1 : 0;
-        a.bg = background(*desc);
-        a.src_x = q.src_x; a.src_y = q.src_y; a.src_w = q.src_w; a.src_h = q.src_h; a.out_w = q.out_w; a.out_h = q.out_h;
-        const ExportRecip rcp = export_recip((uint64_t) q.src_w * (uint64_t) q.src_h);
-        a.div_mul = rcp.mul; a.div_shift = rcp.shift;
-        rc = launch_export_scaled(a, v.stream);
-    } else {
+    return list_enqueue(v, L, bytes, after_event, done_event, [&](const void* d_list) {
+        if (kind == ExportKind::frames) {
+            ExportArgs a = {};
+            common_args(a, v, d_list, count, *desc);
+            a.over = nv12 || (desc->flags & GLAVA_B200_EXPORT_OVER) ? 1 : 0;
+            a.bg = background(*desc);
+            a.uv_offset = uv_offset;
+            return launch_export(a, v.stream);
+        }
+        if (kind == ExportKind::scaled) {
+            ScaledArgs a = {};
+            common_args(a, v, d_list, count, *desc);
+            a.over = nv12 || (desc->flags & GLAVA_B200_EXPORT_OVER) ? 1 : 0;
+            a.bg = background(*desc);
+            a.src_x = q.src_x; a.src_y = q.src_y; a.src_w = q.src_w; a.src_h = q.src_h; a.out_w = q.out_w; a.out_h = q.out_h;
+            const ExportRecip rcp = export_recip((uint64_t) q.src_w * (uint64_t) q.src_h);
+            a.div_mul = rcp.mul; a.div_shift = rcp.shift;
+            return launch_export_scaled(a, v.stream);
+        }
         OverlayArgs a = {};
         common_args(a, v, d_list, count, *desc);
         a.band = a.native && a.marks && a.mark_rows > 0 ? 1 : 0;   // band items wherever marks exist (DESIGN 4.12)
-        rc = launch_overlay(a, v.stream);
-    }
-    if (rc) return rc;
-    ++*v.launches;
-    if (done_event) CU(cudaEventRecord((cudaEvent_t) done_event, st));
-    return 0;
+        return launch_overlay(a, v.stream);
+    });
 }
+
 }  // namespace glb
 
 extern "C" {

@@ -187,6 +187,15 @@ GLB_HD uint32_t export_scaled_px(const ExportFmt& f, const uint64_t acc[4], uint
     return out;
 }
 
+// ---- encoder ladder (DESIGN 4.13): one unit of the schedule ------------------------------------------------------------
+// A unit is one item of a rung's standalone kernel: (rung, row, col) with row = output row pair and col = 128-pixel strip of
+// a whole-frame rung (export_kernel), row = output row (NV12: row pair) and col = run of 32 output columns otherwise
+// (export_scaled_kernel).  Packed as rung << 56 | row << 28 | col.
+GLB_HD uint64_t ladder_unit(int rung, int row, int col) { return ((uint64_t) rung << 56) | ((uint64_t) row << 28) | (uint64_t) col; }
+GLB_HD int ladder_unit_rung(uint64_t u) { return (int) (u >> 56); }
+GLB_HD int ladder_unit_row(uint64_t u) { return (int) ((u >> 28) & 0xfffffffu); }
+GLB_HD int ladder_unit_col(uint64_t u) { return (int) (u & 0xfffffffu); }
+
 // ---- overlay (DESIGN 4.12): the frame composited onto the caller's image ----------------------------------------------------
 // Native opacity only (any other opacity writes export_frames' opaque bytes).  The premultiplied "over" GLava's window
 // performs on the desktop, with the caller's pixel d as the desktop, in all four channels: C = min(255, c + mul_norm8(d_c,

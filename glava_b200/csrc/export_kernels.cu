@@ -11,7 +11,9 @@
 // glava_b200_export_scaled (DESIGN 4.11) is export_scaled_kernel below: the same frames, cropped and shrunk by the exact
 // area average of export_core.h, in one launch with its own argument struct.  glava_b200_overlay_frames (DESIGN 4.12) is
 // overlay_kernel: the same frames composited onto the caller's images in place, likewise with its own argument struct.
-// Both take entries with a chroma pointer (ExportEntryUV); export_kernel keeps ExportEntry.  The host half is export.cpp.
+// Both take entries with a chroma pointer (ExportEntryUV); export_kernel keeps ExportEntry.  glava_b200_export_ladder
+// (DESIGN 4.13) is export_ladder_kernel: every rung of every entry in one launch, each unit run by the per-item body of
+// the rung's standalone kernel.  The host half is export.cpp.
 #include "internal.h"
 #include "export_core.h"
 
@@ -20,20 +22,31 @@
 namespace glb {
 
 // whether row y of the strip must be read (false: it is all zero in memory)
-__device__ __forceinline__ bool row_read(const ExportArgs& a, int slot, int y, int strip) {
+template <typename A>
+__device__ __forceinline__ bool row_read(const A& a, int slot, int y, int strip) {
     if (!a.marks) return true;
     return export_row_read(__ldg(a.marks + export_mark_index(slot, a.w, a.h, a.mark_rows, y, strip)), y);
 }
 
+// Framebuffer loads.  A standalone export reads each line once, so it streams them (evict-first, ld.global.cs); the ladder
+// reads a line once per rung and wants the later rungs to find it in L2, so it loads at normal priority (Keep: ld.global.cg)
+template <bool Keep>
+__device__ __forceinline__ uint4 fb_load4(const uint32_t* p) {
+    return Keep ? __ldcg(reinterpret_cast<const uint4*>(p)) : __ldcs(reinterpret_cast<const uint4*>(p));
+}
+template <bool Keep>
+__device__ __forceinline__ uint32_t fb_load(const uint32_t* p) { return Keep ? __ldcg(p) : __ldcs(p); }
+
 // the quad at x of framebuffer row y of a w-pixel-wide frame (pixels past the right edge read as 0)
+template <bool Keep = false>
 __device__ __forceinline__ void load_quad(const uint32_t* frame, int w, int y, int x, uint32_t px[4]) {
     const uint32_t* row = frame + (size_t) y * w;
     if ((w & 3) == 0) {                                     // rows are 16-byte aligned
-        const uint4 v = __ldcs(reinterpret_cast<const uint4*>(row + x));
+        const uint4 v = fb_load4<Keep>(row + x);
         px[0] = v.x; px[1] = v.y; px[2] = v.z; px[3] = v.w;
     } else {
 #pragma unroll
-        for (int k = 0; k < 4; ++k) px[k] = x + k < w ? __ldcs(row + x + k) : 0u;
+        for (int k = 0; k < 4; ++k) px[k] = x + k < w ? fb_load<Keep>(row + x + k) : 0u;
     }
 }
 
@@ -65,6 +78,37 @@ __device__ __forceinline__ void store_rgba(const ExportFmt& f, uint8_t* row, int
         for (int k = 0; k < 4 && x + k < w; ++k) __stcs(out + k, px[k]);
 }
 
+// One item of export_kernel (and of a ladder's whole-frame rung): output rows 2j and 2j + 1 (framebuffer rows h - 1 - 2j and
+// h - 2 - 2j) of the quad at x of `strip`; the NV12 CbCr plane's row 0 is dst + uv_offset; zy / zuv / zpx: what zero pixels
+// become.
+// A reads w, h, marks, mark_rows, format and pitch.
+template <bool Keep, typename A>
+__device__ __forceinline__ void export_item(const A& a, const ExportFmt& f, const uint32_t* frame, int slot, uint8_t* dst,
+                                            size_t uv_offset, int j, int strip, int x, uint32_t zy, uint32_t zuv, uint32_t zpx) {
+    const int y0 = a.h - 1 - 2 * j, y1 = y0 - 1;
+    uint32_t top[4] = { 0u, 0u, 0u, 0u }, bot[4] = { 0u, 0u, 0u, 0u };
+    if (row_read(a, slot, y0, strip)) load_quad<Keep>(frame, a.w, y0, x, top);
+    if (y1 >= 0 && row_read(a, slot, y1, strip)) load_quad<Keep>(frame, a.w, y1, x, bot);
+    uint8_t* const r0 = dst + (size_t) (2 * j) * a.pitch;
+    if (a.format == GLAVA_B200_EXPORT_NV12) {               // h even: both rows exist
+        uint32_t yt = zy, yb = zy, c = zuv;
+        if ((top[0] | top[1] | top[2] | top[3] | bot[0] | bot[1] | bot[2] | bot[3]) != 0u) c = export_nv12_quad(f, top, bot, &yt, &yb);
+        uint8_t* const pu = dst + uv_offset + (size_t) j * a.pitch + x;
+        if (x + 4 <= a.w) {
+            __stcs(reinterpret_cast<uint32_t*>(r0 + x), yt);
+            __stcs(reinterpret_cast<uint32_t*>(r0 + a.pitch + x), yb);
+            __stcs(reinterpret_cast<uint32_t*>(pu), c);
+        } else {                                            // w even: the last two pixels of a row
+            __stcs(reinterpret_cast<unsigned short*>(r0 + x), (unsigned short) yt);
+            __stcs(reinterpret_cast<unsigned short*>(r0 + a.pitch + x), (unsigned short) yb);
+            __stcs(reinterpret_cast<unsigned short*>(pu), (unsigned short) c);
+        }
+    } else {
+        store_rgba(f, r0, x, a.w, top, zpx);
+        if (y1 >= 0) store_rgba(f, r0 + a.pitch, x, a.w, bot, zpx);
+    }
+}
+
 template <typename Index>
 __global__ void __launch_bounds__(256) export_kernel(const __grid_constant__ ExportArgs a) {
     const ExportFmt f = { a.format, a.over, a.native, a.bg };
@@ -85,7 +129,8 @@ __global__ void __launch_bounds__(256) export_kernel(const __grid_constant__ Exp
         uint8_t* const dst = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst)));
         const int slot = __ldg(&e->slot);
         const uint32_t* frame = reinterpret_cast<const uint32_t*>(a.fb) + (size_t) slot * a.h * a.w;
-        // output rows 2j and 2j + 1 are framebuffer rows h - 1 - 2j and h - 2 - 2j
+        // export_item<false>(a, ..., a.uv_offset, ...) written out: called, ptxas orders four register moves of zpx
+        // differently, and this kernel keeps the machine code it was measured with
         const int y0 = a.h - 1 - 2 * j, y1 = y0 - 1;
         uint32_t top[4] = { 0u, 0u, 0u, 0u }, bot[4] = { 0u, 0u, 0u, 0u };
         if (row_read(a, slot, y0, strip)) load_quad(frame, a.w, y0, x, top);
@@ -127,8 +172,10 @@ int launch_export(const ExportArgs& a, void* stream) {
 // (16-byte loads when rows are 16-byte aligned; neighbouring lanes read neighbouring segments) in 32-bit per channel and
 // folded into 64-bit sums with the row's weight.  NV12 chroma takes the right neighbour's pixels of both rows by shuffle.
 
-// output pixel (X, Y) of the lane, before any R / B swap; active = false: a lane past out_w (the sums stay empty)
-__device__ __forceinline__ uint32_t scaled_px(const ScaledArgs& a, const ExportFmt& f, const uint32_t* frame, int slot, int Y,
+// output pixel (X, Y) of the lane, before any R / B swap; active = false: a lane past out_w (the sums stay empty).  A reads
+// w, h, marks, mark_rows and the rectangle (src_*, out_*) as ScaledArgs names them.
+template <bool Keep, typename A>
+__device__ __forceinline__ uint32_t scaled_px(const A& a, const ExportFmt& f, const uint32_t* frame, int slot, int Y,
                                               bool active, const ExportSpan& sx, const ExportRecip& rcp, uint32_t zc) {
     const ExportSpan sy = export_span(Y, a.src_h, a.out_h);
     const int x0 = a.src_x + sx.first, x1 = a.src_x + sx.last;
@@ -149,11 +196,11 @@ __device__ __forceinline__ uint32_t scaled_px(const ScaledArgs& a, const ExportF
                 for (int qx = qa; qx <= qb; qx += 4) {
                     uint32_t px[4];
                     if ((a.w & 3) == 0) {
-                        const uint4 v = __ldcs(reinterpret_cast<const uint4*>(src + qx));
+                        const uint4 v = fb_load4<Keep>(src + qx);
                         px[0] = v.x; px[1] = v.y; px[2] = v.z; px[3] = v.w;
                     } else {
 #pragma unroll
-                        for (int k = 0; k < 4; ++k) px[k] = qx + k >= x0 && qx + k <= x1 ? __ldcs(src + qx + k) : 0u;
+                        for (int k = 0; k < 4; ++k) px[k] = qx + k >= x0 && qx + k <= x1 ? fb_load<Keep>(src + qx + k) : 0u;
                     }
 #pragma unroll
                     for (int k = 0; k < 4; ++k) {
@@ -166,6 +213,37 @@ __device__ __forceinline__ uint32_t scaled_px(const ScaledArgs& a, const ExportF
         }
     }
     return export_scaled_px(f, acc, wsum, (uint64_t) a.src_w * (uint64_t) a.src_h, rcp, zc);
+}
+
+// One item of export_scaled_kernel (and of a ladder's other rungs): output row u (NV12: rows 2u and 2u + 1) at column X of
+// the lane; zc: what a zero pixel becomes.  A as scaled_px, and fb, format and pitch.
+template <bool Keep, typename A>
+__device__ __forceinline__ void scaled_item(const A& a, const ExportFmt& f, const ExportRecip& rcp, uint32_t zc, bool nv12,
+                                            const ExportEntryUV* e, int u, int X, int lane) {
+    const bool active = X < a.out_w;
+    const int slot = __ldg(&e->slot);
+    const uint32_t* frame = reinterpret_cast<const uint32_t*>(a.fb) + (size_t) slot * a.h * a.w;
+    const ExportSpan sx = export_span(active ? X : 0, a.src_w, a.out_w);
+    uint8_t* const dst = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst)));
+    if (nv12) {                                             // out_w even: the whole 2x2 block is in this warp
+        const uint32_t top = scaled_px<Keep>(a, f, frame, slot, 2 * u, active, sx, rcp, zc);
+        const uint32_t bot = scaled_px<Keep>(a, f, frame, slot, 2 * u + 1, active, sx, rcp, zc);
+        const uint32_t top1 = __shfl_down_sync(0xffffffffu, top, 1), bot1 = __shfl_down_sync(0xffffffffu, bot, 1);
+        if (!active) return;
+        uint8_t* const r0 = dst + (size_t) (2 * u) * a.pitch + X;
+        __stcs(r0, (uint8_t) export_y(top));
+        __stcs(r0 + a.pitch, (uint8_t) export_y(bot));
+        if (!(lane & 1)) {
+            uint8_t* const uv = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst_uv)));
+            __stcs(reinterpret_cast<unsigned short*>(uv + (size_t) u * a.pitch + X),
+                   (unsigned short) export_cbcr(export_avg4(top, top1, bot, bot1)));
+        }
+    } else {
+        uint32_t px = scaled_px<Keep>(a, f, frame, slot, u, active, sx, rcp, zc);
+        if (!active) return;
+        if (a.format == GLAVA_B200_EXPORT_BGRA) px = export_swap_rb(px);
+        __stcs(reinterpret_cast<uint32_t*>(dst + (size_t) u * a.pitch) + X, px);
+    }
 }
 
 template <typename Index>
@@ -181,31 +259,7 @@ __global__ void __launch_bounds__(256) export_scaled_kernel(const __grid_constan
     for (Index it = (Index) (((size_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5); it < items; it += warps) {
         const Index k = it / per, rem = it - k * per;
         const int u = (int) (rem / runs), X = (int) (rem - (Index) u * runs) * 32 + lane;
-        const bool active = X < a.out_w;
-        const ExportEntryUV* e = a.list + k;
-        const int slot = __ldg(&e->slot);
-        const uint32_t* frame = reinterpret_cast<const uint32_t*>(a.fb) + (size_t) slot * a.h * a.w;
-        const ExportSpan sx = export_span(active ? X : 0, a.src_w, a.out_w);
-        uint8_t* const dst = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst)));
-        if (nv12) {                                         // out_w even: the whole 2x2 block is in this warp
-            const uint32_t top = scaled_px(a, f, frame, slot, 2 * u, active, sx, rcp, zc);
-            const uint32_t bot = scaled_px(a, f, frame, slot, 2 * u + 1, active, sx, rcp, zc);
-            const uint32_t top1 = __shfl_down_sync(0xffffffffu, top, 1), bot1 = __shfl_down_sync(0xffffffffu, bot, 1);
-            if (!active) continue;
-            uint8_t* const r0 = dst + (size_t) (2 * u) * a.pitch + X;
-            __stcs(r0, (uint8_t) export_y(top));
-            __stcs(r0 + a.pitch, (uint8_t) export_y(bot));
-            if (!(lane & 1)) {
-                uint8_t* const uv = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst_uv)));
-                __stcs(reinterpret_cast<unsigned short*>(uv + (size_t) u * a.pitch + X),
-                       (unsigned short) export_cbcr(export_avg4(top, top1, bot, bot1)));
-            }
-        } else {
-            uint32_t px = scaled_px(a, f, frame, slot, u, active, sx, rcp, zc);
-            if (!active) continue;
-            if (a.format == GLAVA_B200_EXPORT_BGRA) px = export_swap_rb(px);
-            __stcs(reinterpret_cast<uint32_t*>(dst + (size_t) u * a.pitch) + X, px);
-        }
+        scaled_item<false>(a, f, rcp, zc, nv12, a.list + k, u, X, lane);
     }
 }
 
@@ -215,6 +269,59 @@ int launch_export_scaled(const ScaledArgs& a, void* stream) {
     if (g.narrow) export_scaled_kernel<uint32_t><<<g.blocks, 256, 0, (cudaStream_t) stream>>>(a);
     else export_scaled_kernel<uint64_t><<<g.blocks, 256, 0, (cudaStream_t) stream>>>(a);
     return launch_status("scaled export");
+}
+
+// ---- glava_b200_export_ladder (DESIGN 4.13) --------------------------------------------------------------------------------
+// One warp per (entry, unit of the schedule), the unit fastest: a unit is one item of the rung's standalone kernel, run by
+// that kernel's own body (export_item / scaled_item) with the rung's fields, so every rung is bit for bit its standalone
+// call.  The schedule sorts one entry's units by the first source row they read, so the warps in flight cover a few source
+// rows of one frame across all rungs; framebuffer loads keep normal L2 priority (Keep) for the rungs that follow.
+
+// the fields export_item / scaled_item read, for one rung (named as ExportArgs / ScaledArgs name them)
+struct RungView {
+    const uint8_t*  fb;
+    const uint32_t* marks;
+    int mark_rows, w, h, format;
+    size_t pitch;
+    int src_x, src_y, src_w, src_h, out_w, out_h;
+};
+
+template <typename Index>
+__global__ void __launch_bounds__(256) export_ladder_kernel(const __grid_constant__ LadderArgs a) {
+    const Index units = (Index) a.units, items = (Index) a.count * units;
+    const Index warps = (Index) (((size_t) gridDim.x * blockDim.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    for (Index it = (Index) (((size_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5); it < items; it += warps) {
+        const Index k = it / units;
+        const uint64_t unit = __ldg(reinterpret_cast<const unsigned long long*>(a.sched) + (it - k * units));
+        const int rung = ladder_unit_rung(unit), row = ladder_unit_row(unit), col = ladder_unit_col(unit);
+        const LadderRung& g = a.rung[rung];
+        const RungView v = { a.fb, a.marks, a.mark_rows, a.w, a.h, g.format, g.pitch, g.src_x, g.src_y, g.src_w, g.src_h, g.out_w, g.out_h };
+        const ExportFmt f = { g.format, g.over, a.native, g.bg };
+        const ExportEntryUV* e = a.list + (size_t) k * a.nrungs + rung;
+        if (g.whole) {
+            const int x = col * 128 + lane * 4;
+            if (x >= a.w) continue;
+            uint8_t* const dst = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst)));
+            // the entry's CbCr pointer as an offset from its luma (unsigned: the chroma may lie before it)
+            const size_t uv_offset = g.format == GLAVA_B200_EXPORT_NV12
+                                         ? (size_t) (__ldg(reinterpret_cast<const unsigned long long*>(&e->dst_uv)) - (unsigned long long) dst)
+                                         : 0;
+            const int slot = __ldg(&e->slot);
+            const uint32_t* frame = reinterpret_cast<const uint32_t*>(a.fb) + (size_t) slot * a.h * a.w;
+            export_item<true>(v, f, frame, slot, dst, uv_offset, row, col, x, g.zy, g.zuv, g.zpx);
+        } else {
+            const ExportRecip rcp = { g.div_mul, g.div_shift };
+            scaled_item<true>(v, f, rcp, g.zc, g.format == GLAVA_B200_EXPORT_NV12, e, row, col * 32 + lane, lane);
+        }
+    }
+}
+
+int launch_export_ladder(const LadderArgs& a, void* stream) {
+    const ExportGrid g = export_grid((uint64_t) a.count * (uint64_t) a.units);
+    if (g.narrow) export_ladder_kernel<uint32_t><<<g.blocks, 256, 0, (cudaStream_t) stream>>>(a);
+    else export_ladder_kernel<uint64_t><<<g.blocks, 256, 0, (cudaStream_t) stream>>>(a);
+    return launch_status("ladder export");
 }
 
 // ---- glava_b200_overlay_frames (DESIGN 4.12) -------------------------------------------------------------------------------

@@ -1,0 +1,143 @@
+// export_ladder.cpp — the host half of glava_b200_export_ladder (DESIGN 4.13): every rung checked by export.cpp's
+// export_check as a scaled export that names the rung, the schedule of ladder_plan.h built once per geometry and kept on
+// the device, one [count][nrungs] list and one launch of export_ladder_kernel (export_kernels.cu) through export_list.h's
+// enqueue.  Kept apart from export.cpp so that the other exports build and link without the ladder's launcher.
+#include "internal.h"
+#include "export_core.h"
+#include "export_list.h"
+#include "ladder_plan.h"
+
+#include <cuda_runtime.h>
+
+#include <cstdio>
+#include <vector>
+
+namespace glb {
+
+int ladder_shape_check(const glava_b200_export_rung* rungs, int nrungs, const char* who) {
+    if (!rungs) return fail(GLAVA_B200_EINVAL, "%s: null rungs", who);
+    if (nrungs < 1 || nrungs > GLAVA_B200_LADDER_MAX)
+        return fail(GLAVA_B200_EINVAL, "%s: nrungs %d must be 1 to %d", who, nrungs, GLAVA_B200_LADDER_MAX);
+    return 0;
+}
+
+int ladder_check(glava_b200* r, const int* streams, int count, const glava_b200_export_rung* rungs, int nrungs, void* const* dst,
+                 void* const* dst_uv, const char* who, glava_b200_export_scale* q) {
+    int rc = ladder_shape_check(rungs, nrungs, who);
+    if (rc) return rc;
+    if (count < 1) return fail(GLAVA_B200_EINVAL, "%s: count %d < 1", who, count);
+    if (!streams || !dst) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
+    // rung j's destinations, as glava_b200_export_scaled would take them
+    std::vector<void*> d((size_t) count), uv((size_t) count);
+    for (int j = 0; j < nrungs; ++j) {
+        char name[96];
+        snprintf(name, sizeof(name), "%s: rung %d", who, j);
+        const bool nv12 = rungs[j].desc.format == GLAVA_B200_EXPORT_NV12;
+        for (int i = 0; i < count; ++i) {
+            d[i] = dst[(size_t) i * nrungs + j];
+            uv[i] = dst_uv ? dst_uv[(size_t) i * nrungs + j] : nullptr;
+            if (uv[i] && !nv12)
+                return fail(GLAVA_B200_EINVAL, "%s: dst_uv[%d] is for NV12 only (entry %d)", name, i * nrungs + j, i);
+        }
+        rc = export_check(ExportKind::scaled, r, streams, count, d.data(), dst_uv && nv12 ? uv.data() : nullptr, &rungs[j].desc,
+                          &rungs[j].scale, name, q ? q + j : nullptr);
+        if (rc) return rc;
+    }
+    return 0;
+}
+
+// the device schedule for `geom`, built and uploaded on the raster stream when the geometry differs from the last ladder's
+static int ladder_schedule_room(const RendererView& v, ExportList* L, const LadderGeom* geom, int nrungs, uint32_t* units) {
+    std::vector<int> key = { v.w, v.h, nrungs };
+    for (int j = 0; j < nrungs; ++j) {
+        const LadderGeom& g = geom[j];
+        key.insert(key.end(), { g.src_x, g.src_y, g.src_w, g.src_h, g.out_w, g.out_h, (int) g.whole, (int) g.nv12 });
+    }
+    if (key == L->sched_key && L->sched_cap) { *units = (uint32_t) L->sched_h.size(); return 0; }
+    L->sched_key.clear();
+    cudaStream_t st = (cudaStream_t) v.stream;
+    CU(cudaStreamSynchronize(st));                          // a ladder still running reads the old schedule and sched_h
+    L->sched_h = ladder_schedule(v.w, v.h, geom, nrungs);
+    const size_t bytes = L->sched_h.size() * sizeof(uint64_t);
+    if (bytes > L->sched_cap) {
+        L->sched_cap = 0;
+        int rc;
+        if ((rc = L->sched.alloc(bytes)) != 0) return rc;
+        L->sched_cap = bytes;
+    }
+    CU(cudaMemcpyAsync(L->sched, L->sched_h.data(), bytes, cudaMemcpyHostToDevice, st));
+    L->sched_key = key;
+    *units = (uint32_t) L->sched_h.size();
+    return 0;
+}
+
+int ladder_run(glava_b200* r, const int* streams, int count, const glava_b200_export_rung* rungs, int nrungs, void* const* dst,
+               void* const* dst_uv, void* after_event, void* done_event, const char* who) {
+    clear_error();
+    if (!r) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
+    glava_b200_export_scale q[GLAVA_B200_LADDER_MAX];
+    int rc = ladder_check(r, streams, count, rungs, nrungs, dst, dst_uv, who, q);
+    if (rc) return rc;
+    const RendererView v = renderer_view(r);
+    LadderGeom geom[GLAVA_B200_LADDER_MAX];
+    size_t uv_offset[GLAVA_B200_LADDER_MAX];
+    for (int j = 0; j < nrungs; ++j) {
+        geom[j] = { q[j].src_x, q[j].src_y, q[j].src_w, q[j].src_h, q[j].out_w, q[j].out_h, false,
+                    rungs[j].desc.format == GLAVA_B200_EXPORT_NV12 };
+        geom[j].whole = ladder_whole(v.w, v.h, geom[j]);
+        uv_offset[j] = rungs[j].desc.uv_offset ? rungs[j].desc.uv_offset : rungs[j].desc.pitch * (size_t) q[j].out_h;
+    }
+    CU(cudaSetDevice(v.device));
+    const size_t n = (size_t) count * (size_t) nrungs, bytes = n * sizeof(ExportEntryUV);
+    ExportList* L = nullptr;
+    if ((rc = list_room(v, bytes, &L)) != 0) return rc;
+    uint32_t units = 0;
+    if ((rc = ladder_schedule_room(v, L, geom, nrungs, &units)) != 0) return rc;
+    CU(cudaEventSynchronize(L->ev[L->cur]));                // the copy that last read h[cur] (four calls ago)
+    ExportEntryUV* const host = reinterpret_cast<ExportEntryUV*>((uint8_t*) L->h[L->cur]);
+    for (int i = 0; i < count; ++i) {
+        const int slot = streams[i] % v.slots;
+        for (int j = 0; j < nrungs; ++j) {
+            const size_t e = (size_t) i * nrungs + j;
+            uint8_t* const d = (uint8_t*) dst[e];
+            uint8_t* const uv = !geom[j].nv12 ? nullptr : dst_uv ? (uint8_t*) dst_uv[e] : d + uv_offset[j];
+            host[e] = { d, uv, slot, 0 };
+        }
+    }
+    return list_enqueue(v, L, bytes, after_event, done_event, [&](const void* d_list) {
+        LadderArgs a = {};
+        a.fb = v.fb;
+        a.marks = v.mark_key ? v.marks : nullptr;           // as common_args
+        a.mark_rows = v.mark_key >> 2;
+        a.list = static_cast<const ExportEntryUV*>(d_list); a.count = count; a.w = v.w; a.h = v.h;
+        a.native = v.native; a.nrungs = nrungs;
+        a.sched = L->sched; a.units = units;
+        for (int j = 0; j < nrungs; ++j) {
+            const glava_b200_export& d = rungs[j].desc;
+            LadderRung& g = a.rung[j];
+            g.format = d.format;
+            g.over = geom[j].nv12 || (d.flags & GLAVA_B200_EXPORT_OVER) ? 1 : 0;
+            g.whole = geom[j].whole ? 1 : 0;
+            g.bg = background(d);
+            g.pitch = d.pitch;
+            g.src_x = q[j].src_x; g.src_y = q[j].src_y; g.src_w = q[j].src_w; g.src_h = q[j].src_h;
+            g.out_w = q[j].out_w; g.out_h = q[j].out_h;
+            const ExportRecip rcp = export_recip((uint64_t) q[j].src_w * (uint64_t) q[j].src_h);
+            g.div_mul = rcp.mul; g.div_shift = rcp.shift;
+            // what a zero pixel becomes, as export_kernel and export_scaled_kernel compute it before their loops
+            const ExportFmt f = { g.format, g.over, v.native, g.bg };
+            const uint32_t zero4[4] = { 0u, 0u, 0u, 0u };
+            uint32_t zy1;
+            g.zuv = export_nv12_quad(f, zero4, zero4, &g.zy, &zy1);
+            g.zpx = export_px(f, 0u);
+            g.zc = f.over ? export_over(0u, f.bg, f.native) : 0u;
+        }
+        return launch_export_ladder(a, v.stream);
+    });
+}
+}  // namespace glb
+
+extern "C" int glava_b200_export_ladder(glava_b200* r, const int* streams, int count, const glava_b200_export_rung* rungs,
+                                        int nrungs, void* const* dst, void* const* dst_uv, void* after_event, void* done_event) {
+    return glb::ladder_run(r, streams, count, rungs, nrungs, dst, dst_uv, after_event, done_event, "glava_b200_export_ladder");
+}

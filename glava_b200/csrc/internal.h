@@ -245,6 +245,31 @@ struct OverlayArgs {
     size_t pitch;
 };
 int launch_overlay(const OverlayArgs& a, void* stream);
+// export_kernels.cu: glava_b200_export_ladder (DESIGN 4.13), one launch for every rung of every entry.  Per rung what a
+// standalone call would take: the whole frame at its own size (whole = 1) runs export_kernel's items, every other rung
+// export_scaled_kernel's; z*: what a zero pixel becomes under the rung's format (export_core.h, filled on the host).
+struct LadderRung {
+    int    format, over, whole;
+    uint32_t bg;
+    size_t pitch;
+    int    src_x, src_y, src_w, src_h, out_w, out_h;   // as ScaledArgs
+    uint64_t div_mul;
+    int    div_shift;
+    uint32_t zpx, zy, zuv, zc;  // export_kernel's zpx / zy / zuv, export_scaled_kernel's zc
+};
+// The grid is flattened over (entry, unit of `sched`), the unit fastest; list: [count][nrungs] entries
+struct LadderArgs {
+    const uint8_t*  fb;         // [slots][h][w] RGBA8
+    const uint32_t* marks;      // as ExportArgs
+    int             mark_rows;
+    const ExportEntryUV* list;
+    int    count, w, h;
+    int    native, nrungs;
+    const uint64_t* sched;      // ladder_plan.h units, sorted by the first framebuffer row they read
+    uint32_t units;
+    LadderRung rung[GLAVA_B200_LADDER_MAX];
+};
+int launch_export_ladder(const LadderArgs& a, void* stream);
 // capi.cu, for export.cpp: what the frame export reads of a renderer, and the slot where it keeps its own per-renderer
 // state (*attach, released by *attach_free when the renderer is destroyed)
 struct RendererView {
@@ -258,7 +283,7 @@ struct RendererView {
 RendererView renderer_view(glava_b200* r);
 // export.cpp: the three caller-buffer exports, which differ in output size (the scaled export's is its rectangle's), the
 // flags they take and their kernel
-enum class ExportKind { frames, scaled, overlay };
+enum class ExportKind { frames, scaled, overlay, ladder };
 // Every refusal of a call of `kind` that depends on this renderer alone, in the call's order (the overlay's overlap and
 // framebuffer tests are overlay_geometry_check's); nothing is enqueued.  dst_uv and scale may be null; q (if non-null)
 // receives the scale rectangle with its defaults applied, the whole frame for the other kinds.
@@ -269,6 +294,14 @@ int export_check(ExportKind kind, glava_b200* r, const int* streams, int count, 
 // then the list copy and the kernel on the raster stream behind `after_event` (or nothing), then `done_event` (or nothing)
 int export_run(ExportKind kind, glava_b200* r, const int* streams, int count, void* const* dst, void* const* dst_uv,
                const glava_b200_export* desc, const glava_b200_export_scale* scale, void* after_event, void* done_event);
+// export_ladder.cpp, glava_b200_export_ladder: `rungs` non-null and 1 <= nrungs <= GLAVA_B200_LADDER_MAX (checked first, also by the sharded form
+// before it splits the list); then export_check of the scaled kind once per rung, `who` extended by the rung's index; dst and
+// dst_uv are [count][nrungs].  q (if non-null): [nrungs] rectangles with their defaults applied.
+int ladder_shape_check(const glava_b200_export_rung* rungs, int nrungs, const char* who);
+int ladder_check(glava_b200* r, const int* streams, int count, const glava_b200_export_rung* rungs, int nrungs, void* const* dst,
+                 void* const* dst_uv, const char* who, glava_b200_export_scale* q = nullptr);
+int ladder_run(glava_b200* r, const int* streams, int count, const glava_b200_export_rung* rungs, int nrungs, void* const* dst,
+               void* const* dst_uv, void* after_event, void* done_event, const char* who);
 // The rectangles of a list (w x h frames, `desc`'s format and pitch; dst_uv null: dst + uv_offset) must not overlap each
 // other nor any of the `nfb` byte ranges [fb[k], fb[k] + fb_bytes[k]) (framebuffer arrays)
 int overlay_geometry_check(int w, int h, int count, void* const* dst, void* const* dst_uv, const glava_b200_export& desc,

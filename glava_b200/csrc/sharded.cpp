@@ -310,13 +310,17 @@ int glava_b200_sharded_get_stream_styles(const glava_b200_sharded* g, const int*
 // The caller-buffer exports (DESIGN 4.10–4.12), global stream indices (repeats allowed): the list is split by shard, dst[i]
 // and dst_uv[i] travelling with streams[i].  Every shard's part passes the single-renderer checks, and for an overlay the
 // whole list the overlap test against itself and every shard's framebuffer (shards may share a device), before any shard
-// starts; the shards then issue at once.
+// starts; the shards then issue at once.  A ladder (rungs non-null) carries nrungs destinations per entry.
 static int sharded_export(glava_b200_sharded* g, ExportKind kind, const int* streams, int count, void* const* dst,
-                          void* const* dst_uv, const glava_b200_export* desc, const glava_b200_export_scale* scale, const char* who) {
+                          void* const* dst_uv, const glava_b200_export* desc, const glava_b200_export_scale* scale, const char* who,
+                          const glava_b200_export_rung* rungs = nullptr, int nrungs = 1) {
     clear_error();
-    if (!g || !desc) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
+    const bool ladder = kind == ExportKind::ladder;
+    if (!g || (!ladder && !desc)) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
+    if (ladder) { const int rc = ladder_shape_check(rungs, nrungs, who); if (rc) return rc; }
     if (count < 1) return fail(GLAVA_B200_EINVAL, "%s: count %d < 1", who, count);
     if (!streams || !dst) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
+    const size_t per = ladder ? (size_t) nrungs : 1;
     std::vector<std::vector<int>> idx(g->shards.size());
     std::vector<std::vector<void*>> ptr(g->shards.size()), uv(g->shards.size());
     for (int i = 0; i < count; ++i) {
@@ -325,7 +329,10 @@ static int sharded_export(glava_b200_sharded* g, ExportKind kind, const int* str
         for (size_t k = 0; k < g->shards.size(); ++k) {
             const Shard* sh = g->shards[k];
             if (s >= sh->first && s < sh->first + sh->count) {
-                idx[k].push_back(s - sh->first); ptr[k].push_back(dst[i]); uv[k].push_back(dst_uv ? dst_uv[i] : nullptr);
+                idx[k].push_back(s - sh->first);
+                for (size_t j = 0; j < per; ++j) {
+                    ptr[k].push_back(dst[i * per + j]); uv[k].push_back(dst_uv ? dst_uv[i * per + j] : nullptr);
+                }
                 break;
             }
         }
@@ -336,8 +343,10 @@ static int sharded_export(glava_b200_sharded* g, ExportKind kind, const int* str
         const RendererView v = renderer_view(g->shards[k]->r);
         fb.push_back(v.fb); fb_bytes.push_back((size_t) v.slots * (size_t) v.h * (size_t) v.w * 4);
         if (idx[k].empty()) continue;
-        const int rc = export_check(kind, g->shards[k]->r, idx[k].data(), (int) idx[k].size(), ptr[k].data(),
-                                    dst_uv ? uv[k].data() : nullptr, desc, scale, who);
+        const int rc = ladder ? ladder_check(g->shards[k]->r, idx[k].data(), (int) idx[k].size(), rungs, nrungs, ptr[k].data(),
+                                             dst_uv ? uv[k].data() : nullptr, who)
+                              : export_check(kind, g->shards[k]->r, idx[k].data(), (int) idx[k].size(), ptr[k].data(),
+                                             dst_uv ? uv[k].data() : nullptr, desc, scale, who);
         if (rc) return rc;
     }
     if (kind == ExportKind::overlay) {
@@ -348,6 +357,9 @@ static int sharded_export(glava_b200_sharded* g, ExportKind kind, const int* str
     return broadcast(g, [&](Shard& s) {
         const size_t k = (size_t) (std::find(g->shards.begin(), g->shards.end(), &s) - g->shards.begin());
         if (idx[k].empty()) return 0;
+        if (ladder)
+            return ladder_run(s.r, idx[k].data(), (int) idx[k].size(), rungs, nrungs, ptr[k].data(), dst_uv ? uv[k].data() : nullptr,
+                              nullptr, nullptr, who);
         return export_run(kind, s.r, idx[k].data(), (int) idx[k].size(), ptr[k].data(), dst_uv ? uv[k].data() : nullptr, desc,
                           scale, nullptr, nullptr);
     });
@@ -363,6 +375,11 @@ int glava_b200_sharded_export_scaled(glava_b200_sharded* g, const int* streams, 
 int glava_b200_sharded_overlay_frames(glava_b200_sharded* g, const int* streams, int count, void* const* dst, void* const* dst_uv,
                                       const glava_b200_export* desc) {
     return sharded_export(g, ExportKind::overlay, streams, count, dst, dst_uv, desc, nullptr, "glava_b200_sharded_overlay_frames");
+}
+int glava_b200_sharded_export_ladder(glava_b200_sharded* g, const int* streams, int count, const glava_b200_export_rung* rungs,
+                                     int nrungs, void* const* dst, void* const* dst_uv) {
+    return sharded_export(g, ExportKind::ladder, streams, count, dst, dst_uv, nullptr, nullptr, "glava_b200_sharded_export_ladder",
+                          rungs, nrungs);
 }
 
 int glava_b200_sharded_textures(glava_b200_sharded* g, uint16_t* out_l, uint16_t* out_r) {

@@ -428,6 +428,33 @@ int glava_b200_export_scaled(glava_b200* r, const int* streams, int count, void*
                              const glava_b200_export* desc, const glava_b200_export_scale* scale, void* after_event,
                              void* done_event);
 
+/* Encoder ladder (DESIGN.md §4.13): several sizes of each frame in one launch that reads each source row about once, for an
+ * ABR ladder whose rungs NVENC cannot scale itself (say 1080p, 720p and 360p NV12 beside an RGBA thumbnail).
+ *   glava_b200_export_ladder   rung j of entry i gets exactly the bytes glava_b200_export_scaled(r, &streams[i], 1,
+ *                              &dst[i * nrungs + j], dst_uv ? &dst_uv[i * nrungs + j] : NULL, &rungs[j].desc,
+ *                              &rungs[j].scale, ...) would write at this point in call order (framebuffer ring, styles and
+ *                              repeated streams included); a rung that is the whole frame at its own size is therefore
+ *                              glava_b200_export_frames, bit for bit.  Formats and flags may differ between rungs.  Ordering
+ *                              and events as glava_b200_export_frames: waits for `after_event` on the device, runs on the
+ *                              handle's stream behind the latest pass, records `done_event`, returns without a host wait.
+ *     dst                      [count][nrungs] destinations; each rung's size is glava_b200_export_scaled_bytes(r,
+ *                              &rungs[j].desc, &rungs[j].scale, &n) (there is no separate byte-count call)
+ *     dst_uv                   NULL, or [count][nrungs] CbCr destinations as glava_b200_export_scaled's, NULL entries for
+ *                              RGBA / BGRA rungs
+ *   Nothing outside a rung's rectangle and its chroma rows is written; like glava_b200_export_scaled the call does not check
+ *   whether destinations overlap.  Every refusal of glava_b200_export_scaled, checked per rung (the message names the rung),
+ *   nrungs < 1 or > GLAVA_B200_LADDER_MAX, null `rungs` and a non-null dst_uv entry for an RGBA / BGRA rung are
+ *   GLAVA_B200_EINVAL with nothing enqueued.
+ *   glava_b200_sharded_export_ladder  the same with global stream indices, each entry's destinations on the device of the
+ *                              shard that owns streams[i]; every entry of every rung is checked before any shard starts. */
+typedef struct {
+    glava_b200_export       desc;     /* format, flags, background, pitch, uv_offset of this rung's destinations */
+    glava_b200_export_scale scale;    /* source rectangle and output size, as glava_b200_export_scaled */
+} glava_b200_export_rung;
+#define GLAVA_B200_LADDER_MAX 8
+int glava_b200_export_ladder(glava_b200* r, const int* streams, int count, const glava_b200_export_rung* rungs, int nrungs,
+                             void* const* dst, void* const* dst_uv, void* after_event, void* done_event);
+
 /* Overlay onto the caller's images (DESIGN.md §4.12), for audiograms, music channels and compositing over video: the frames
  * drawn over a picture the caller holds in DEVICE memory, in place, in one launch that touches only what the frame covers.
  *   glava_b200_overlay_frames  composites the current frame of streams[i] — what glava_b200_export_frames would export
@@ -487,6 +514,9 @@ int  glava_b200_sharded_export_scaled(glava_b200_sharded* s, const int* streams,
                                       const glava_b200_export_scale* scale);   /* global indices; see glava_b200_export_scaled */
 int  glava_b200_sharded_overlay_frames(glava_b200_sharded* s, const int* streams, int count, void* const* dst,
                                        void* const* dst_uv, const glava_b200_export* desc);   /* see glava_b200_overlay_frames */
+int  glava_b200_sharded_export_ladder(glava_b200_sharded* s, const int* streams, int count,
+                                      const glava_b200_export_rung* rungs, int nrungs, void* const* dst,
+                                      void* const* dst_uv);   /* global indices; see glava_b200_export_ladder */
 
 /* ---- lifetime of individual streams: reset, save and load (DESIGN.md §4.8) -------------------------------------------
  * A stream's state is what its next update reads besides its new audio: gravity store and average ring, the latest
