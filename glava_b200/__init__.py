@@ -15,11 +15,13 @@ raises.
 from .api import (Params, Color, Renderer, GlavaError, default_params, load_config, lib, lib_path,
                   MODULES, pinned_empty, Pipe, ShardedRenderer, stream_state_bytes, STATE_HEADER_BYTES,
                   StreamStyle, stream_style, style_params, STYLE_AMPLIFY, STYLE_FG, STYLE_BG,
-                  Export, ExportScale, ExportRung, LADDER_MAX, EXPORT_RGBA, EXPORT_BGRA, EXPORT_NV12, EXPORT_OVER)
+                  Export, ExportScale, ExportRung, LADDER_MAX, EXPORT_RGBA, EXPORT_BGRA, EXPORT_NV12, EXPORT_I420,
+                  EXPORT_YUV444, EXPORT_P010, EXPORT_OVER)
 from . import audio
 from .synth import synth_pcm_int16, fifo_to_float, StreamRings
 
 __all__ = ["audio", "Params", "Color", "Renderer", "GlavaError", "default_params", "load_config", "lib",
            "lib_path", "MODULES", "pinned_empty", "Pipe", "ShardedRenderer", "stream_state_bytes", "STATE_HEADER_BYTES",
            "StreamStyle", "stream_style", "style_params", "STYLE_AMPLIFY", "STYLE_FG", "STYLE_BG",
-           "Export", "ExportScale", "ExportRung", "LADDER_MAX", "EXPORT_RGBA", "EXPORT_BGRA", "EXPORT_NV12", "EXPORT_OVER", "synth_pcm_int16", "fifo_to_float", "StreamRings"]
+           "Export", "ExportScale", "ExportRung", "LADDER_MAX", "EXPORT_RGBA", "EXPORT_BGRA", "EXPORT_NV12", "EXPORT_I420",
+           "EXPORT_YUV444", "EXPORT_P010", "EXPORT_OVER", "synth_pcm_int16", "fifo_to_float", "StreamRings"]

@@ -133,8 +133,43 @@ class ExportRung(C.Structure):
 
 LADDER_MAX = 8
 EXPORT_RGBA, EXPORT_BGRA, EXPORT_NV12 = 0, 1, 2
+EXPORT_I420, EXPORT_YUV444, EXPORT_P010 = 4, 5, 6
 EXPORT_OVER = 1
-EXPORT_FORMATS = {"rgba": EXPORT_RGBA, "bgra": EXPORT_BGRA, "nv12": EXPORT_NV12}
+EXPORT_FORMATS = {"rgba": EXPORT_RGBA, "bgra": EXPORT_BGRA, "nv12": EXPORT_NV12, "i420": EXPORT_I420,
+                  "yuv444": EXPORT_YUV444, "p010": EXPORT_P010}
+OVERLAY_FORMATS = ("rgba", "bgra", "nv12")
+
+
+def _export_layout(fmt, w, h):
+    """(rows, row bytes, pitch multiple) of one w x h output of `fmt` held as rows of one pitch: RGBA / BGRA h rows of w * 4
+    bytes; NV12 / P010 h * 3 / 2 rows of w (P010: w uint16) samples, Y then CbCr; I420 h * 3 / 2 rows, the Y plane then the
+    Cb and Cr planes back to back at pitch / 2 (pitch a multiple of 32); YUV444 3 h rows, the Y, Cb and Cr planes"""
+    if fmt in ("rgba", "bgra"):
+        return h, w * 4, 16
+    if fmt == "yuv444":
+        return 3 * h, w, 16
+    return h * 3 // 2, w * 2 if fmt == "p010" else w, 32 if fmt == "i420" else 16
+
+
+def _export_views(fmt, t, w, h):
+    """what an export into t returns: t is uint8 [..., rows, pitch] with contiguous rows as _export_layout describes.  RGBA /
+    BGRA [..., h, w, 4], NV12 [..., h * 3 / 2, w] uint8, P010 [..., h * 3 / 2, w] uint16, I420 / YUV444 the plane views
+    (Y, Cb, Cr), each [..., rows, cols]"""
+    import torch
+    P = t.shape[-1]
+    if fmt in ("rgba", "bgra"):
+        return t[..., :w * 4].unflatten(-1, (w, 4))
+    if fmt == "nv12":
+        return t[..., :w]
+    if fmt == "p010":
+        return t.view(torch.uint16)[..., :w]
+    flat = t.flatten(-2)
+    cw, ch, cp = (w // 2, h // 2, P // 2) if fmt == "i420" else (w, h, P)
+    n = ch * cp
+    y = flat[..., :P * h].unflatten(-1, (h, P))[..., :w]
+    cb = flat[..., P * h:P * h + n].unflatten(-1, (ch, cp))[..., :cw]
+    cr = flat[..., P * h + n:P * h + 2 * n].unflatten(-1, (ch, cp))[..., :cw]
+    return y, cb, cr
 
 
 _lib = None
@@ -426,53 +461,52 @@ class _FrameExport:
     def _export_plan(self, streams, fmt, over, background, out, device_of, size=None):
         """-> (stream list, Export, [dst pointers], what to return).  device_of(stream): the CUDA device of a stream's
         frame.  size: (w, h) of each output, None: the frame's.  out: None (allocate), one uint8 tensor [count, rows, ...]
-        whose dim 1 steps by the pitch, or a list of count tensors [rows, ...] with one common pitch; rows = h (RGBA / BGRA)
-        or h * 3 / 2 (NV12)"""
+        whose dim 1 steps by the pitch, or a list of count tensors [rows, ...] with one common pitch; rows as
+        _export_layout gives them (h for RGBA / BGRA, h * 3 / 2 for NV12, I420 and P010, 3 h for YUV444; I420 and YUV444
+        keep their planes back to back from row h); P010 also takes uint16 tensors"""
         import torch
         s = np.ascontiguousarray(np.asarray(streams, dtype=np.int64).reshape(-1), dtype=np.int32)
         count = int(s.shape[0])
         devices = [device_of(int(x)) for x in s]
         p = self.params
         w, h = (p.w, p.h) if size is None else (int(size[0]), int(size[1]))
-        nv12 = fmt == "nv12"
-        rows, row_bytes = (h * 3 // 2, w) if nv12 else (h, w * 4)
         desc = _export_desc(fmt, over, background)
-
-        def frame_view(t):
-            return t[:, :row_bytes] if nv12 else t[:, :row_bytes].unflatten(1, (w, 4))
+        rows, row_bytes, align = _export_layout(fmt, w, h)
+        dtypes = (torch.uint8, torch.uint16) if fmt == "p010" else (torch.uint8,)
 
         if out is None:
-            pitch = (row_bytes + 15) // 16 * 16
+            pitch = (row_bytes + align - 1) // align * align
             if len(set(devices)) <= 1:
                 base = torch.empty((count, rows, pitch), dtype=torch.uint8, device=f"cuda:{devices[0] if devices else 0}")
                 dst = [base.data_ptr() + i * rows * pitch for i in range(count)]
-                result = base[:, :, :row_bytes] if nv12 else base[:, :, :row_bytes].unflatten(2, (w, 4))
+                result = _export_views(fmt, base, w, h)
             else:
                 bufs = [torch.empty((rows, pitch), dtype=torch.uint8, device=f"cuda:{d}") for d in devices]
                 dst = [b.data_ptr() for b in bufs]
-                result = [frame_view(b) for b in bufs]
+                result = [_export_views(fmt, b, w, h) for b in bufs]
         else:
             tensors = list(out) if isinstance(out, (list, tuple)) else None
             if tensors is None:
-                if out.dtype != torch.uint8 or not out.is_cuda or out.dim() < 3 or out.shape[0] != count or out.shape[1] != rows:
+                if out.dtype not in dtypes or not out.is_cuda or out.dim() < 3 or out.shape[0] != count or out.shape[1] != rows:
                     raise ValueError(f"out: a uint8 CUDA tensor [{count}, {rows}, ...] (got {out.dtype} {tuple(out.shape)})")
-                pitch = out.stride(1)
-                dst = [out.data_ptr() + i * out.stride(0) for i in range(count)]
+                pitch = out.stride(1) * out.element_size()
+                dst = [out.data_ptr() + i * out.stride(0) * out.element_size() for i in range(count)]
                 row = out[0, 0]
             else:
                 if len(tensors) != count:
                     raise ValueError(f"out: {count} tensors, got {len(tensors)}")
                 for t in tensors:
-                    if t.dtype != torch.uint8 or not t.is_cuda or t.dim() < 2 or t.shape[0] != rows or t.stride(0) != tensors[0].stride(0):
+                    if (t.dtype != tensors[0].dtype or t.dtype not in dtypes or not t.is_cuda or t.dim() < 2 or t.shape[0] != rows
+                            or t.stride(0) != tensors[0].stride(0)):
                         raise ValueError(f"out: uint8 CUDA tensors [{rows}, ...] with one pitch (got {t.dtype} {tuple(t.shape)})")
-                pitch = tensors[0].stride(0)
+                pitch = tensors[0].stride(0) * tensors[0].element_size()
                 dst = [t.data_ptr() for t in tensors]
                 row = tensors[0][0]
-            if not row.is_contiguous() or row.numel() < row_bytes:
+            if not row.is_contiguous() or row.numel() * row.element_size() < row_bytes:
                 raise ValueError(f"out: every row must hold {row_bytes} contiguous bytes")
             result = out
         desc.pitch = pitch
-        desc.uv_offset = pitch * h if nv12 else 0
+        desc.uv_offset = pitch * h if fmt in ("nv12", "p010") else 0
         return s, desc, (C.c_void_p * max(count, 1))(*dst), result
 
     def _ladder_plan(self, streams, rungs, out, device_of):
@@ -511,8 +545,8 @@ class _FrameExport:
         import torch
         s = np.ascontiguousarray(np.asarray(streams, dtype=np.int64).reshape(-1), dtype=np.int32)
         count = int(s.shape[0])
-        if fmt not in EXPORT_FORMATS:
-            raise ValueError(f"format {fmt!r}: one of {sorted(EXPORT_FORMATS)}")
+        if fmt not in OVERLAY_FORMATS:
+            raise ValueError(f"format {fmt!r}: the overlay takes one of {list(OVERLAY_FORMATS)}")
         nv12 = fmt == "nv12"
 
         def describe(t, what):
@@ -854,8 +888,10 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
     def export_frames(self, streams, fmt="rgba", over=False, background=(0, 0, 0), out=None, after=None, done=None):
         """The current frames of `streams` (repeats allowed) top-down in the caller's device memory (glava_b200_export_frames):
         fmt "rgba" / "bgra" ([h, w, 4] per frame; over=True composites over `background` as GLava's window shows it) or
-        "nv12" ([h * 3 / 2, w]: Y rows, then interleaved CbCr rows; always composited).  out: see _export_plan; None
-        allocates [count, h, w, 4] / [count, h * 3 / 2, w] (rows padded to a multiple of 16 bytes).  Returns out.
+        "nv12" ([h * 3 / 2, w]: Y rows, then interleaved CbCr rows), "p010" (the same as uint16 samples, 10-bit code << 6),
+        "i420" / "yuv444" (a tuple of plane views Y [h, w], Cb and Cr [h / 2, w / 2] or [h, w] of one back-to-back
+        allocation); the YUV formats are always composited.  out: see _export_plan; None allocates [count, ...] of those
+        shapes (rows padded to a multiple of 16 bytes, 32 for I420).  Returns out.
         after / done: torch.cuda.Event or cudaEvent_t handles — the export waits for `after` on the device and records
         `done` behind itself.  Left None, the export is ordered after the work already queued on torch's current stream,
         and that stream waits for the export (the tensors can be used right away)."""
@@ -880,8 +916,8 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
     def export_scaled(self, streams, size, crop=None, fmt="rgba", over=False, background=(0, 0, 0), out=None, after=None,
                       done=None):
         """export_frames of a source rectangle shrunk to size = (w, h) by the exact area average (glava_b200_export_scaled):
-        crop = (x, y, w, h) in top-down coordinates (y = 0 is the top row), None: the whole frame.  Downscale only; NV12
-        needs an even w and h.  Shapes, out, after and done as export_frames, with the output size in place of the frame's."""
+        crop = (x, y, w, h) in top-down coordinates (y = 0 is the top row), None: the whole frame.  Downscale only; NV12,
+        I420 and P010 need an even w and h.  Shapes, out, after and done as export_frames, with the output size in place of the frame's."""
         s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, lambda stream: self.device, size)
         sc = _export_scale(size, crop)
         self._ordered(lambda a, d: self._L.glava_b200_export_scaled(self._h, s.ctypes.data, s.shape[0], dst, None, C.byref(desc),
@@ -911,11 +947,13 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
 
     def export_mosaic(self, streams, cols, tile, fmt="nv12", background=(0, 0, 0), out=None):
         """The frames of `streams` shrunk to tile = (w, h) and laid out row-major, `cols` tiles per row, in one picture, by
-        one export_scaled call with a destination (and for NV12 a chroma destination) per tile.  Returns [H * 3 / 2, W]
-        for NV12 (Y rows, then CbCr rows) or [H, W, 4], W = cols * w, H = rows * h: one surface to hand to an encoder.
-        Tiles start at multiples of 16 bytes, so w is a multiple of 16 (NV12) or 4 (RGBA / BGRA).  out: a uint8 CUDA
-        tensor [H * 3 / 2 or H, pitch] whose rows hold W (NV12) or W * 4 contiguous bytes; tiles past the last stream keep
-        its bytes (out None: black).  Ordered against torch's current stream as export_frames without events."""
+        one export_scaled call with a destination and a chroma destination per tile.  W = cols * w, H = rows * h; returns
+        [H * 3 / 2, W] for NV12 (uint8) and P010 (uint16), Y rows then CbCr rows, the plane views (Y, Cb, Cr) for I420 and
+        YUV444, or [H, W, 4]: one surface to hand to an encoder.  Tiles start at multiples of 16 bytes in every plane, so w
+        is a multiple of 16 (NV12, YUV444), 32 (I420), 8 (P010) or 4 (RGBA / BGRA).  out: a CUDA tensor [rows, pitch] whose
+        rows hold the picture's row bytes, rows as _export_layout gives them for W x H (I420 / YUV444: the chroma planes
+        back to back from row H); tiles past the last stream keep its bytes (out None: black).  Ordered against torch's
+        current stream as export_frames without events."""
         import torch
         s = np.ascontiguousarray(np.asarray(streams, dtype=np.int64).reshape(-1), dtype=np.int32)
         count, cols = int(s.shape[0]), int(cols)
@@ -923,23 +961,40 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
         if count < 1 or cols < 1:
             raise ValueError("export_mosaic: at least one stream and one column")
         desc = _export_desc(fmt, False, background)
-        nv12, px = fmt == "nv12", 1 if fmt == "nv12" else 4
         W, H = cols * tw, (count + cols - 1) // cols * th
-        rows = H * 3 // 2 if nv12 else H
+        rows, row_bytes, align = _export_layout(fmt, W, H)
+        px = {"rgba": 4, "bgra": 4, "p010": 2}.get(fmt, 1)
         if out is None:
-            base = torch.empty((rows, (W * px + 15) // 16 * 16), dtype=torch.uint8, device=f"cuda:{self.device}")
+            base = torch.empty((rows, (row_bytes + align - 1) // align * align), dtype=torch.uint8, device=f"cuda:{self.device}")
             if count % cols:                                  # black where no stream lands
-                base[:H].fill_(16 if nv12 else 0)
-                base[H:].fill_(128)
-            result = base[:, :W] if nv12 else base[:, :W * 4].unflatten(1, (W, 4))
+                if fmt == "p010":
+                    base.view(torch.uint16)[:H].fill_(64 << 6)
+                    base.view(torch.uint16)[H:].fill_(512 << 6)
+                elif fmt in ("rgba", "bgra"):
+                    base.fill_(0)
+                else:
+                    base[:H].fill_(16)
+                    base[H:].fill_(128)
+            result = _export_views(fmt, base, W, H)
         else:
-            if (out.dtype != torch.uint8 or not out.is_cuda or out.dim() != 2 or out.shape[0] != rows or out.stride(1) != 1
-                    or out.shape[1] < W * px):
-                raise ValueError(f"out: a uint8 CUDA tensor [{rows}, >= {W * px}] with contiguous rows")
+            dtypes = (torch.uint8, torch.uint16) if fmt == "p010" else (torch.uint8,)
+            if (out.dtype not in dtypes or not out.is_cuda or out.dim() != 2 or out.shape[0] != rows or out.stride(1) != 1
+                    or out.shape[1] * out.element_size() < row_bytes):
+                raise ValueError(f"out: a uint8 CUDA tensor [{rows}, >= {row_bytes}] with contiguous rows")
             base = result = out
-        pitch, ptr = base.stride(0), base.data_ptr()
+        pitch, ptr = base.stride(0) * base.element_size(), base.data_ptr()
         dst = (C.c_void_p * count)(*[ptr + (i // cols) * th * pitch + (i % cols) * tw * px for i in range(count)])
-        uv = (C.c_void_p * count)(*[ptr + (H + (i // cols) * (th // 2)) * pitch + (i % cols) * tw for i in range(count)]) if nv12 else None
+        if fmt in ("nv12", "p010"):
+            uv = [ptr + (H + (i // cols) * (th // 2)) * pitch + (i % cols) * tw * px for i in range(count)]
+        elif fmt == "i420":                                   # Cr one whole chroma plane past Cb
+            uv = [ptr + H * pitch + (i // cols) * (th // 2) * (pitch // 2) + (i % cols) * (tw // 2) for i in range(count)]
+            desc.uv_offset = (pitch // 2) * (H // 2)
+        elif fmt == "yuv444":
+            uv = [ptr + (H + (i // cols) * th) * pitch + (i % cols) * tw for i in range(count)]
+            desc.uv_offset = pitch * H
+        else:
+            uv = None
+        uv = (C.c_void_p * count)(*uv) if uv else None
         desc.pitch = pitch
         sc = _export_scale(tile, None)
         self._ordered(lambda a, d: self._L.glava_b200_export_scaled(self._h, s.ctypes.data, count, dst, uv, C.byref(desc),

@@ -20,16 +20,38 @@ namespace {
 
 const char* const kCallName[] = { "glava_b200_export_frames", "glava_b200_export_scaled", "glava_b200_overlay_frames" };
 
+const char* format_name(int format) {
+    switch (format) {
+    case GLAVA_B200_EXPORT_RGBA: return "RGBA";
+    case GLAVA_B200_EXPORT_BGRA: return "BGRA";
+    case GLAVA_B200_EXPORT_NV12: return "NV12";
+    case GLAVA_B200_EXPORT_I420: return "I420";
+    case GLAVA_B200_EXPORT_YUV444: return "YUV444";
+    case GLAVA_B200_EXPORT_P010: return "P010";
+    default: return nullptr;
+    }
+}
+
 // pitch and uv_offset against a w x h output (`what` names it in the message: "frame" / "output")
 int desc_size(int w, int h, const glava_b200_export& d, const char* what, const char* who) {
-    const bool nv12 = d.format == GLAVA_B200_EXPORT_NV12;
-    if (nv12 && ((w | h) & 1)) return fail(GLAVA_B200_EINVAL, "%s: NV12 needs an even width and height, the %s is %dx%d", who, what, w, h);
-    const size_t row = nv12 ? (size_t) w : (size_t) w * 4;
+    const int fmt = d.format;
+    const char* name = format_name(fmt);
+    if (export_420(fmt) && ((w | h) & 1))
+        return fail(GLAVA_B200_EINVAL, "%s: %s needs an even width and height, the %s is %dx%d", who, name, what, w, h);
+    const size_t row = !export_yuv(fmt) ? (size_t) w * 4 : fmt == GLAVA_B200_EXPORT_P010 ? (size_t) w * 2 : (size_t) w;
     if (d.pitch % 16 || d.pitch < row)
         return fail(GLAVA_B200_EINVAL, "%s: pitch %zu must be a multiple of 16 and at least %zu", who, d.pitch, row);
-    if (nv12 && (d.uv_offset % 16 || (d.uv_offset && d.uv_offset < d.pitch * (size_t) h)))
+    if (fmt == GLAVA_B200_EXPORT_I420 && d.pitch % 32)
+        return fail(GLAVA_B200_EINVAL, "%s: I420 pitch %zu must be a multiple of 32, so that chroma rows (pitch / 2) stay 16-byte "
+                    "aligned", who, d.pitch);
+    if ((fmt == GLAVA_B200_EXPORT_NV12 || fmt == GLAVA_B200_EXPORT_P010) &&
+        (d.uv_offset % 16 || (d.uv_offset && d.uv_offset < d.pitch * (size_t) h)))
         return fail(GLAVA_B200_EINVAL, "%s: uv_offset %zu must be a multiple of 16 and at least pitch * h = %zu (or 0)", who,
                     d.uv_offset, d.pitch * (size_t) h);
+    const size_t plane = export_planes(fmt, d.pitch, 0, h).plane;
+    if (export_planar(fmt) && (d.uv_offset % 16 || (d.uv_offset && d.uv_offset < plane)))
+        return fail(GLAVA_B200_EINVAL, "%s: %s uv_offset %zu (Cb plane to Cr plane) must be a multiple of 16 and at least one "
+                    "chroma plane, %zu bytes (or 0)", who, name, d.uv_offset, plane);
     return 0;
 }
 
@@ -38,8 +60,9 @@ int desc_size(int w, int h, const glava_b200_export& d, const char* what, const 
 // whole frame at its own size for the other kinds), so q->out_w x q->out_h is the output size.
 int desc_check(ExportKind kind, int w, int h, const glava_b200_export& d, const glava_b200_export_scale* s,
                glava_b200_export_scale* q, const char* who) {
-    if (d.format != GLAVA_B200_EXPORT_RGBA && d.format != GLAVA_B200_EXPORT_BGRA && d.format != GLAVA_B200_EXPORT_NV12)
-        return fail(GLAVA_B200_EINVAL, "%s: unknown format %d", who, d.format);
+    if (!format_name(d.format)) return fail(GLAVA_B200_EINVAL, "%s: unknown format %d", who, d.format);
+    if (kind == ExportKind::overlay && d.format != GLAVA_B200_EXPORT_NV12 && export_yuv(d.format))
+        return fail(GLAVA_B200_EINVAL, "%s: format %s: the overlay takes RGBA, BGRA or NV12", who, format_name(d.format));
     if (d.flags & ~GLAVA_B200_EXPORT_OVER) return fail(GLAVA_B200_EINVAL, "%s: unknown flags 0x%x", who, d.flags);
     if (kind == ExportKind::overlay && d.flags) return fail(GLAVA_B200_EINVAL, "%s: flags 0x%x: the overlay takes none", who, d.flags);
     *q = { 0, 0, w, h, w, h };
@@ -81,8 +104,10 @@ int output_bytes(ExportKind kind, const glava_b200* r, const glava_b200_export* 
     const int rc = desc_check(kind, p.w, p.h, *desc, scale, &q, who);
     if (rc) return rc;
     const size_t h = (size_t) q.out_h;
-    if (desc->format != GLAVA_B200_EXPORT_NV12) *bytes = desc->pitch * h;
-    else *bytes = (desc->uv_offset ? desc->uv_offset : desc->pitch * h) + desc->pitch * (h / 2);
+    const ExportPlanes pl = export_planes(desc->format, desc->pitch, desc->uv_offset, q.out_h);
+    if (!export_yuv(desc->format)) *bytes = desc->pitch * h;
+    else if (export_planar(desc->format)) *bytes = pl.cb + pl.cr + pl.plane;
+    else *bytes = pl.cb + desc->pitch * (h / 2);
     return 0;
 }
 
@@ -186,7 +211,9 @@ int export_check(ExportKind kind, glava_b200* r, const int* streams, int count, 
     glava_b200_export_scale local;
     int rc = desc_check(kind, v.w, v.h, *desc, scale, q ? q : &local, who);
     if (rc) return rc;
-    if (dst_uv && desc->format != GLAVA_B200_EXPORT_NV12) return fail(GLAVA_B200_EINVAL, "%s: dst_uv is for NV12 only", who);
+    if (dst_uv && !export_yuv(desc->format))
+        return fail(GLAVA_B200_EINVAL, "%s: dst_uv is for NV12 only, or I420, YUV444 and P010: %s has no chroma plane", who,
+                    format_name(desc->format));
     if (count < 1) return fail(GLAVA_B200_EINVAL, "%s: count %d < 1", who, count);
     if (!streams || !dst) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
     for (int i = 0; i < count; ++i) {
@@ -212,8 +239,8 @@ int export_run(ExportKind kind, glava_b200* r, const int* streams, int count, vo
         const size_t fb_bytes = (size_t) v.slots * (size_t) v.h * (size_t) v.w * 4;
         if ((rc = overlay_geometry_check(v.w, v.h, count, dst, dst_uv, *desc, &v.fb, &fb_bytes, 1, who)) != 0) return rc;
     }
-    const bool nv12 = desc->format == GLAVA_B200_EXPORT_NV12;
-    const size_t uv_offset = desc->uv_offset ? desc->uv_offset : desc->pitch * (size_t) q.out_h;
+    const bool yuv = export_yuv(desc->format);
+    const ExportPlanes pl = export_planes(desc->format, desc->pitch, desc->uv_offset, q.out_h);
     CU(cudaSetDevice(v.device));
     // export_kernel's entries have no chroma pointer (its machine code stays as measured); the others carry one per entry
     const size_t bytes = (size_t) count * (kind == ExportKind::frames ? sizeof(ExportEntry) : sizeof(ExportEntryUV));
@@ -225,25 +252,27 @@ int export_run(ExportKind kind, glava_b200* r, const int* streams, int count, vo
         uint8_t* const d = (uint8_t*) dst[i];
         const int slot = streams[i] % v.slots;
         if (kind == ExportKind::frames) reinterpret_cast<ExportEntry*>(host)[i] = { d, slot, 0 };
-        else reinterpret_cast<ExportEntryUV*>(host)[i] = { d, !nv12 ? nullptr : dst_uv ? (uint8_t*) dst_uv[i] : d + uv_offset, slot, 0 };
+        else reinterpret_cast<ExportEntryUV*>(host)[i] = { d, !yuv ? nullptr : dst_uv ? (uint8_t*) dst_uv[i] : d + pl.cb, slot, 0 };
     }
     return list_enqueue(v, L, bytes, after_event, done_event, [&](const void* d_list) {
         if (kind == ExportKind::frames) {
             ExportArgs a = {};
             common_args(a, v, d_list, count, *desc);
-            a.over = nv12 || (desc->flags & GLAVA_B200_EXPORT_OVER) ? 1 : 0;
+            a.over = yuv || (desc->flags & GLAVA_B200_EXPORT_OVER) ? 1 : 0;
             a.bg = background(*desc);
-            a.uv_offset = uv_offset;
+            a.uv_offset = pl.cb;
+            a.cr_offset = pl.cr;
             return launch_export(a, v.stream);
         }
         if (kind == ExportKind::scaled) {
             ScaledArgs a = {};
             common_args(a, v, d_list, count, *desc);
-            a.over = nv12 || (desc->flags & GLAVA_B200_EXPORT_OVER) ? 1 : 0;
+            a.over = yuv || (desc->flags & GLAVA_B200_EXPORT_OVER) ? 1 : 0;
             a.bg = background(*desc);
             a.src_x = q.src_x; a.src_y = q.src_y; a.src_w = q.src_w; a.src_h = q.src_h; a.out_w = q.out_w; a.out_h = q.out_h;
             const ExportRecip rcp = export_recip((uint64_t) q.src_w * (uint64_t) q.src_h);
             a.div_mul = rcp.mul; a.div_shift = rcp.shift;
+            a.cr_offset = pl.cr;
             return launch_export_scaled(a, v.stream);
         }
         OverlayArgs a = {};

@@ -12,8 +12,8 @@ namespace glb {
 // What one export call does to every pixel: the public format, whether it composites, the renderer's opacity
 // (premultiply_alpha != 0: native, the frame is premultiplied over a transparent target) and the background 0x00BBGGRR
 struct ExportFmt {
-    int      format;            // GLAVA_B200_EXPORT_RGBA / _BGRA / _NV12
-    int      over;              // composite (always for NV12)
+    int      format;            // GLAVA_B200_EXPORT_*
+    int      over;              // composite (always for the YUV formats)
     int      native;
     uint32_t bg;
 };
@@ -90,6 +90,120 @@ GLB_HD uint32_t export_nv12_quad(const ExportFmt& f, const uint32_t top[4], cons
         *y_bot |= export_y(b[k]) << (8 * k);
     }
     return export_cbcr(export_avg4(t[0], t[1], b[0], b[1])) | (export_cbcr(export_avg4(t[2], t[3], b[2], b[3])) << 16);
+}
+
+// ---- I420, YUV 4:4:4 and P010 (DESIGN 4.14) ------------------------------------------------------------------------------
+GLB_HD bool export_yuv(int format) {                   // a format with chroma planes
+    return format == GLAVA_B200_EXPORT_NV12 || format == GLAVA_B200_EXPORT_I420 || format == GLAVA_B200_EXPORT_YUV444 ||
+           format == GLAVA_B200_EXPORT_P010;
+}
+GLB_HD bool export_420(int format) {                   // chroma per 2x2 block: w and h even, items are row pairs
+    return format == GLAVA_B200_EXPORT_NV12 || format == GLAVA_B200_EXPORT_I420 || format == GLAVA_B200_EXPORT_P010;
+}
+GLB_HD bool export_planar(int format) { return format == GLAVA_B200_EXPORT_I420 || format == GLAVA_B200_EXPORT_YUV444; }
+
+// Where the chroma of a destination lies, from the descriptor and the output height: `cb`, the bytes from the luma to the
+// chroma plane (NV12 / P010: the CbCr plane, uv_offset or pitch * h; I420 / YUV444: the Cb plane, right after the luma);
+// `cr`, the bytes from Cb to Cr (planar only: uv_offset, or 0 for one chroma plane, back to back); `plane`, the bytes of
+// one planar chroma plane (I420: h / 2 rows of pitch / 2)
+struct ExportPlanes { size_t cb, cr, plane; };
+GLB_HD ExportPlanes export_planes(int format, size_t pitch, size_t uv_offset, int h) {
+    ExportPlanes p = { uv_offset ? uv_offset : pitch * (size_t) h, 0, 0 };
+    if (export_planar(format)) {
+        p.plane = format == GLAVA_B200_EXPORT_I420 ? (pitch / 2) * (size_t) (h / 2) : pitch * (size_t) h;
+        p.cb = pitch * (size_t) h;
+        p.cr = uv_offset ? uv_offset : p.plane;
+    }
+    return p;
+}
+
+// I420: NV12's CbCr word (Cb0, Cr0, Cb1, Cr1) as the two Cb bytes and the two Cr bytes
+GLB_HD uint32_t export_cb_pair(uint32_t uv) { return (uv & 0xffu) | ((uv >> 8) & 0xff00u); }
+GLB_HD uint32_t export_cr_pair(uint32_t uv) { return ((uv >> 8) & 0xffu) | ((uv >> 16) & 0xff00u); }
+
+// YUV 4:4:4 of one row's quad: Y, Cb and Cr of each composited pixel, four bytes each
+GLB_HD void export_444_quad(const ExportFmt& f, const uint32_t in[4], uint32_t* y, uint32_t* cb, uint32_t* cr) {
+    *y = 0u; *cb = 0u; *cr = 0u;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const uint32_t c = export_over(in[k], f.bg, f.native), uv = export_cbcr(c);
+        *y |= export_y(c) << (8 * k);
+        *cb |= (uv & 255u) << (8 * k);
+        *cr |= (uv >> 8) << (8 * k);
+    }
+}
+
+// P010: BT.709 limited range at 10 bits, Y = 64 + 876/255 Y', C = 512 + 896/255 (...), built as the 8-bit coefficients are
+// (scaled by 2^16 and rounded; the blue coefficient of Cb and the red one of Cr minus the sum of the other two, so every grey
+// has Cb = Cr = 512).  Black gives (64, 512, 512), white (940, 512, 512); over all 2^24 colours each code is within 0.503 code
+// values of float64 (tests/test_export_formats_core.py).
+#define GLB_Y10_R 47864
+#define GLB_Y10_G 161017
+#define GLB_Y10_B 16255
+#define GLB_CB10_R (-26383)
+#define GLB_CB10_G (-88755)
+#define GLB_CB10_B (-(GLB_CB10_R + GLB_CB10_G))
+#define GLB_CR10_G (-104580)
+#define GLB_CR10_B (-10557)
+#define GLB_CR10_R (-(GLB_CR10_G + GLB_CR10_B))
+// the 10-bit Y code of a composited pixel
+GLB_HD uint32_t export_y10(uint32_t c) {
+    const int r = (int) (c & 255u), g = (int) ((c >> 8) & 255u), b = (int) ((c >> 16) & 255u);
+    return (uint32_t) ((GLB_Y10_R * r + GLB_Y10_G * g + GLB_Y10_B * b + (64 << GLB_YUV_SHIFT) + GLB_YUV_HALF) >> GLB_YUV_SHIFT);
+}
+// The per-channel sums (0..1020) of a 2x2 block's four composited pixels, 10 bits each (R low).  P010 chroma takes these
+// exact sums, not NV12's (s + 2) >> 2 byte: the two bits that average rounds away are what 10 bits carry.
+GLB_HD uint32_t export_sum4(uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+    uint32_t out = 0;
+#pragma unroll
+    for (int k = 0; k < 3; ++k)
+        out |= (((a >> (8 * k)) & 255u) + ((b >> (8 * k)) & 255u) + ((c >> (8 * k)) & 255u) + ((d >> (8 * k)) & 255u)) << (10 * k);
+    return out;
+}
+// the 10-bit (Cb, Cr) codes of block sums s (export_sum4), Cb in the low 16 bits: the 16-bit coefficients over sums four
+// times the average, so shift 18; every accumulator stays in [0, 2^31)
+GLB_HD uint32_t export_cbcr10(uint32_t s) {
+    const int r = (int) (s & 1023u), g = (int) ((s >> 10) & 1023u), b = (int) (s >> 20);
+    const int cb = (GLB_CB10_R * r + GLB_CB10_G * g + GLB_CB10_B * b + (512 << 18) + (1 << 17)) >> 18;
+    const int cr = (GLB_CR10_R * r + GLB_CR10_G * g + GLB_CR10_B * b + (512 << 18) + (1 << 17)) >> 18;
+    return (uint32_t) cb | ((uint32_t) cr << 16);
+}
+// P010 of a quad of output rows 2j (top) and 2j + 1 (bot): per row its four Y samples as two words (little-endian uint16,
+// code << 6), and the (Cb, Cr) sample pairs of the quad's two 2x2 blocks, one word each
+GLB_HD void export_p010_quad(const ExportFmt& f, const uint32_t top[4], const uint32_t bot[4], uint32_t yt[2], uint32_t yb[2],
+                             uint32_t uv[2]) {
+    uint32_t t[4], b[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        t[k] = export_over(top[k], f.bg, f.native);
+        b[k] = export_over(bot[k], f.bg, f.native);
+    }
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+        yt[k] = (export_y10(t[2 * k]) << 6) | (export_y10(t[2 * k + 1]) << 22);
+        yb[k] = (export_y10(b[2 * k]) << 6) | (export_y10(b[2 * k + 1]) << 22);
+        uv[k] = export_cbcr10(export_sum4(t[2 * k], t[2 * k + 1], b[2 * k], b[2 * k + 1])) << 6;
+    }
+}
+
+// What zero pixels become in a new format's quad, for the kernels' all-zero shortcut: y, the luma word of a row (P010: one
+// of its two equal words); u and v, I420's Cb and Cr pairs, YUV 4:4:4's Cb and Cr words, P010's CbCr word (v unused)
+struct ExportZero { uint32_t y, u, v; };
+GLB_HD ExportZero export_zero(const ExportFmt& f) {
+    const uint32_t z[4] = { 0u, 0u, 0u, 0u };
+    ExportZero o = { 0u, 0u, 0u };
+    if (f.format == GLAVA_B200_EXPORT_YUV444) {
+        export_444_quad(f, z, &o.y, &o.u, &o.v);
+    } else if (f.format == GLAVA_B200_EXPORT_P010) {
+        uint32_t yt[2], yb[2], uv[2];
+        export_p010_quad(f, z, z, yt, yb, uv);
+        o.y = yt[0]; o.u = uv[0];
+    } else {
+        uint32_t yb;
+        const uint32_t uv = export_nv12_quad(f, z, z, &o.y, &yb);
+        o.u = export_cb_pair(uv); o.v = export_cr_pair(uv);
+    }
+    return o;
 }
 
 // ---- mark-aware reads ----------------------------------------------------------------------------------------------------

@@ -13,7 +13,8 @@
 // overlay_kernel: the same frames composited onto the caller's images in place, likewise with its own argument struct.
 // Both take entries with a chroma pointer (ExportEntryUV); export_kernel keeps ExportEntry.  glava_b200_export_ladder
 // (DESIGN 4.13) is export_ladder_kernel: every rung of every entry in one launch, each unit run by the per-item body of
-// the rung's standalone kernel.  The host half is export.cpp.
+// the rung's standalone kernel.  I420, YUV 4:4:4 and P010 (DESIGN 4.14) run kernels of their own with the same items
+// (export_yuv_kernel, export_scaled_yuv_kernel, export_ladder_yuv_kernel).  The host half is export.cpp.
 #include "internal.h"
 #include "export_core.h"
 
@@ -156,9 +157,118 @@ __global__ void __launch_bounds__(256) export_kernel(const __grid_constant__ Exp
     }
 }
 
+// ---- I420, YUV 4:4:4 and P010 (DESIGN 4.14) --------------------------------------------------------------------------------
+// export_kernel's items (output row pair x 128-pixel strip, a quad per lane) with the new formats' stores, in kernels of their
+// own so that export_kernel keeps its machine code.  I420: two 4-byte Y stores and a 2-byte Cb and a 2-byte Cr store
+// (chroma rows pitch / 2 apart); YUV 4:4:4: a 4-byte Y, Cb and Cr store per row; P010: an 8-byte Y store per row and an
+// 8-byte CbCr store.  Past the last full quad: I420 and P010 have an even width (the last two pixels of a row), YUV 4:4:4
+// stores byte by byte.
+
+// the first n (1..4) bytes of v at p (n == 4: p is 4-byte aligned)
+__device__ __forceinline__ void store_bytes(uint8_t* p, uint32_t v, int n) {
+    if (n >= 4) __stcs(reinterpret_cast<uint32_t*>(p), v);
+    else
+        for (int k = 0; k < n; ++k) __stcs(p + k, (uint8_t) (v >> (8 * k)));
+}
+
+// YUV 4:4:4 of one row's quad: n pixels of Y at py, Cb at pu and Cr cr bytes past it
+__device__ __forceinline__ void store_444(const ExportFmt& f, const uint32_t q[4], uint8_t* py, uint8_t* pu, size_t cr, int n,
+                                          const ExportZero& z) {
+    uint32_t y = z.y, u = z.u, v = z.v;
+    if ((q[0] | q[1] | q[2] | q[3]) != 0u) export_444_quad(f, q, &y, &u, &v);
+    store_bytes(py, y, n);
+    store_bytes(pu, u, n);
+    store_bytes(pu + cr, v, n);
+}
+
+// One item of export_yuv_kernel (and of a ladder's whole-frame I420 / YUV444 / P010 rung): as export_item, with the chroma
+// plane at `cb` (I420 / YUV444: Cb, Cr `cr` bytes further; P010: CbCr) and z what zero pixels become.  fmt: a constant in
+// the standalone kernels, the rung's format in the ladder.  A reads w, h, marks, mark_rows and pitch.
+template <bool Keep, typename A>
+__device__ __forceinline__ void yuv_item(const A& a, const ExportFmt& f, int fmt, const uint32_t* frame, int slot, uint8_t* dst,
+                                         uint8_t* cb, size_t cr, int j, int strip, int x, const ExportZero& z) {
+    const int y0 = a.h - 1 - 2 * j, y1 = y0 - 1;
+    uint32_t top[4] = { 0u, 0u, 0u, 0u }, bot[4] = { 0u, 0u, 0u, 0u };
+    if (row_read(a, slot, y0, strip)) load_quad<Keep>(frame, a.w, y0, x, top);
+    if (y1 >= 0 && row_read(a, slot, y1, strip)) load_quad<Keep>(frame, a.w, y1, x, bot);
+    uint8_t* const r0 = dst + (size_t) (2 * j) * a.pitch;
+    const bool full = x + 4 <= a.w;
+    if (fmt == GLAVA_B200_EXPORT_YUV444) {                  // any w and h
+        const int n = full ? 4 : a.w - x;
+        const size_t o = (size_t) (2 * j) * a.pitch + x;
+        store_444(f, top, dst + o, cb + o, cr, n, z);
+        if (y1 >= 0) store_444(f, bot, dst + o + a.pitch, cb + o + a.pitch, cr, n, z);
+        return;
+    }
+    const bool any = (top[0] | top[1] | top[2] | top[3] | bot[0] | bot[1] | bot[2] | bot[3]) != 0u;
+    if (fmt == GLAVA_B200_EXPORT_I420) {                    // w and h even
+        uint32_t yt = z.y, yb = z.y, u = z.u, v = z.v;
+        if (any) {
+            const uint32_t uv = export_nv12_quad(f, top, bot, &yt, &yb);
+            u = export_cb_pair(uv); v = export_cr_pair(uv);
+        }
+        uint8_t* const pu = cb + (size_t) j * (a.pitch >> 1) + (x >> 1);
+        if (full) {
+            __stcs(reinterpret_cast<uint32_t*>(r0 + x), yt);
+            __stcs(reinterpret_cast<uint32_t*>(r0 + a.pitch + x), yb);
+            __stcs(reinterpret_cast<unsigned short*>(pu), (unsigned short) u);
+            __stcs(reinterpret_cast<unsigned short*>(pu + cr), (unsigned short) v);
+        } else {                                            // the last two pixels of a row
+            __stcs(reinterpret_cast<unsigned short*>(r0 + x), (unsigned short) yt);
+            __stcs(reinterpret_cast<unsigned short*>(r0 + a.pitch + x), (unsigned short) yb);
+            __stcs(pu, (uint8_t) u);
+            __stcs(pu + cr, (uint8_t) v);
+        }
+        return;
+    }
+    uint32_t yt[2] = { z.y, z.y }, yb[2] = { z.y, z.y }, uv[2] = { z.u, z.u };   // P010, w and h even
+    if (any) export_p010_quad(f, top, bot, yt, yb, uv);
+    uint8_t* const pu = cb + (size_t) j * a.pitch + 2 * x;
+    if (full) {
+        __stcs(reinterpret_cast<uint2*>(r0 + 2 * x), make_uint2(yt[0], yt[1]));
+        __stcs(reinterpret_cast<uint2*>(r0 + a.pitch + 2 * x), make_uint2(yb[0], yb[1]));
+        __stcs(reinterpret_cast<uint2*>(pu), make_uint2(uv[0], uv[1]));
+    } else {
+        __stcs(reinterpret_cast<uint32_t*>(r0 + 2 * x), yt[0]);
+        __stcs(reinterpret_cast<uint32_t*>(r0 + a.pitch + 2 * x), yb[0]);
+        __stcs(reinterpret_cast<uint32_t*>(pu), uv[0]);
+    }
+}
+
+template <typename Index, int Fmt>
+__global__ void __launch_bounds__(256) export_yuv_kernel(const __grid_constant__ ExportArgs a) {
+    const ExportFmt f = { Fmt, 1, a.native, a.bg };
+    const Index strips = (Index) ((a.w + 127) >> 7), per = strips * (Index) ((a.h + 1) >> 1);
+    const Index items = (Index) a.count * per;
+    const Index warps = (Index) (((size_t) gridDim.x * blockDim.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    const ExportZero z = export_zero(f);                    // once per thread, as export_kernel's constants
+    for (Index it = (Index) (((size_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5); it < items; it += warps) {
+        const Index k = it / per, rem = it - k * per;
+        const int j = (int) (rem / strips), strip = (int) (rem - (Index) j * strips);
+        const int x = strip * 128 + lane * 4;
+        if (x >= a.w) continue;
+        const ExportEntry* e = a.list + k;
+        uint8_t* const dst = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst)));
+        const int slot = __ldg(&e->slot);
+        const uint32_t* frame = reinterpret_cast<const uint32_t*>(a.fb) + (size_t) slot * a.h * a.w;
+        yuv_item<false>(a, f, Fmt, frame, slot, dst, dst + a.uv_offset, a.cr_offset, j, strip, x, z);
+    }
+}
+
+template <typename Index>
+static void launch_yuv(const ExportArgs& a, unsigned blocks, cudaStream_t st) {
+    if (a.format == GLAVA_B200_EXPORT_I420) export_yuv_kernel<Index, GLAVA_B200_EXPORT_I420><<<blocks, 256, 0, st>>>(a);
+    else if (a.format == GLAVA_B200_EXPORT_YUV444) export_yuv_kernel<Index, GLAVA_B200_EXPORT_YUV444><<<blocks, 256, 0, st>>>(a);
+    else export_yuv_kernel<Index, GLAVA_B200_EXPORT_P010><<<blocks, 256, 0, st>>>(a);
+}
+
 int launch_export(const ExportArgs& a, void* stream) {
     const ExportGrid g = export_grid((uint64_t) a.count * (uint64_t) ((a.w + 127) >> 7) * (uint64_t) ((a.h + 1) >> 1));
-    if (g.narrow) export_kernel<uint32_t><<<g.blocks, 256, 0, (cudaStream_t) stream>>>(a);
+    if (a.format != GLAVA_B200_EXPORT_NV12 && export_yuv(a.format)) {
+        if (g.narrow) launch_yuv<uint32_t>(a, g.blocks, (cudaStream_t) stream);
+        else launch_yuv<uint64_t>(a, g.blocks, (cudaStream_t) stream);
+    } else if (g.narrow) export_kernel<uint32_t><<<g.blocks, 256, 0, (cudaStream_t) stream>>>(a);
     else export_kernel<uint64_t><<<g.blocks, 256, 0, (cudaStream_t) stream>>>(a);
     return launch_status("export");
 }
@@ -263,10 +373,82 @@ __global__ void __launch_bounds__(256) export_scaled_kernel(const __grid_constan
     }
 }
 
+// One item of export_scaled_yuv_kernel (and of a ladder's other I420 / YUV444 / P010 rungs), as scaled_item: output row u
+// (I420 / P010: rows 2u and 2u + 1, the chroma of each 2x2 block from the right neighbour by shuffle) at column X of the
+// lane.  The chroma plane is the entry's dst_uv (I420 / YUV444: Cb, Cr `cr` bytes further; P010: CbCr).
+template <bool Keep, typename A>
+__device__ __forceinline__ void scaled_yuv_item(const A& a, const ExportFmt& f, int fmt, const ExportRecip& rcp, uint32_t zc,
+                                                size_t cr, const ExportEntryUV* e, int u, int X, int lane) {
+    const bool active = X < a.out_w;
+    const int slot = __ldg(&e->slot);
+    const uint32_t* frame = reinterpret_cast<const uint32_t*>(a.fb) + (size_t) slot * a.h * a.w;
+    const ExportSpan sx = export_span(active ? X : 0, a.src_w, a.out_w);
+    uint8_t* const dst = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst)));
+    uint8_t* const cb = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst_uv)));
+    if (fmt == GLAVA_B200_EXPORT_YUV444) {
+        const uint32_t px = scaled_px<Keep>(a, f, frame, slot, u, active, sx, rcp, zc);
+        if (!active) return;
+        const size_t o = (size_t) u * a.pitch + X;
+        const uint32_t uv = export_cbcr(px);
+        __stcs(dst + o, (uint8_t) export_y(px));
+        __stcs(cb + o, (uint8_t) uv);
+        __stcs(cb + cr + o, (uint8_t) (uv >> 8));
+        return;
+    }
+    // out_w even: the whole 2x2 block is in this warp
+    const uint32_t top = scaled_px<Keep>(a, f, frame, slot, 2 * u, active, sx, rcp, zc);
+    const uint32_t bot = scaled_px<Keep>(a, f, frame, slot, 2 * u + 1, active, sx, rcp, zc);
+    const uint32_t top1 = __shfl_down_sync(0xffffffffu, top, 1), bot1 = __shfl_down_sync(0xffffffffu, bot, 1);
+    if (!active) return;
+    if (fmt == GLAVA_B200_EXPORT_I420) {
+        uint8_t* const r0 = dst + (size_t) (2 * u) * a.pitch + X;
+        __stcs(r0, (uint8_t) export_y(top));
+        __stcs(r0 + a.pitch, (uint8_t) export_y(bot));
+        if (!(lane & 1)) {
+            const uint32_t uv = export_cbcr(export_avg4(top, top1, bot, bot1));
+            uint8_t* const pu = cb + (size_t) u * (a.pitch >> 1) + (X >> 1);
+            __stcs(pu, (uint8_t) uv);
+            __stcs(pu + cr, (uint8_t) (uv >> 8));
+        }
+    } else {                                                // P010
+        uint8_t* const r0 = dst + (size_t) (2 * u) * a.pitch + 2 * X;
+        __stcs(reinterpret_cast<unsigned short*>(r0), (unsigned short) (export_y10(top) << 6));
+        __stcs(reinterpret_cast<unsigned short*>(r0 + a.pitch), (unsigned short) (export_y10(bot) << 6));
+        if (!(lane & 1))
+            __stcs(reinterpret_cast<uint32_t*>(cb + (size_t) u * a.pitch + 2 * X), export_cbcr10(export_sum4(top, top1, bot, bot1)) << 6);
+    }
+}
+
+template <typename Index, int Fmt>
+__global__ void __launch_bounds__(256) export_scaled_yuv_kernel(const __grid_constant__ ScaledArgs a) {
+    const ExportFmt f = { Fmt, 1, a.native, a.bg };
+    const ExportRecip rcp = { a.div_mul, a.div_shift };
+    const uint32_t zc = export_over(0u, f.bg, f.native);    // what a zero pixel becomes
+    const Index runs = (Index) ((a.out_w + 31) >> 5), per = runs * (Index) (Fmt == GLAVA_B200_EXPORT_YUV444 ? a.out_h : a.out_h >> 1);
+    const Index items = (Index) a.count * per;
+    const Index warps = (Index) (((size_t) gridDim.x * blockDim.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    for (Index it = (Index) (((size_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5); it < items; it += warps) {
+        const Index k = it / per, rem = it - k * per;
+        const int u = (int) (rem / runs), X = (int) (rem - (Index) u * runs) * 32 + lane;
+        scaled_yuv_item<false>(a, f, Fmt, rcp, zc, a.cr_offset, a.list + k, u, X, lane);
+    }
+}
+
+template <typename Index>
+static void launch_scaled_yuv(const ScaledArgs& a, unsigned blocks, cudaStream_t st) {
+    if (a.format == GLAVA_B200_EXPORT_I420) export_scaled_yuv_kernel<Index, GLAVA_B200_EXPORT_I420><<<blocks, 256, 0, st>>>(a);
+    else if (a.format == GLAVA_B200_EXPORT_YUV444) export_scaled_yuv_kernel<Index, GLAVA_B200_EXPORT_YUV444><<<blocks, 256, 0, st>>>(a);
+    else export_scaled_yuv_kernel<Index, GLAVA_B200_EXPORT_P010><<<blocks, 256, 0, st>>>(a);
+}
+
 int launch_export_scaled(const ScaledArgs& a, void* stream) {
-    const uint64_t units = a.format == GLAVA_B200_EXPORT_NV12 ? (uint64_t) (a.out_h >> 1) : (uint64_t) a.out_h;
+    const uint64_t units = export_420(a.format) ? (uint64_t) (a.out_h >> 1) : (uint64_t) a.out_h;
     const ExportGrid g = export_grid((uint64_t) a.count * (uint64_t) ((a.out_w + 31) >> 5) * units);
-    if (g.narrow) export_scaled_kernel<uint32_t><<<g.blocks, 256, 0, (cudaStream_t) stream>>>(a);
+    if (a.format != GLAVA_B200_EXPORT_NV12 && export_yuv(a.format)) {
+        if (g.narrow) launch_scaled_yuv<uint32_t>(a, g.blocks, (cudaStream_t) stream);
+        else launch_scaled_yuv<uint64_t>(a, g.blocks, (cudaStream_t) stream);
+    } else if (g.narrow) export_scaled_kernel<uint32_t><<<g.blocks, 256, 0, (cudaStream_t) stream>>>(a);
     else export_scaled_kernel<uint64_t><<<g.blocks, 256, 0, (cudaStream_t) stream>>>(a);
     return launch_status("scaled export");
 }
@@ -286,8 +468,10 @@ struct RungView {
     int src_x, src_y, src_w, src_h, out_w, out_h;
 };
 
-template <typename Index>
-__global__ void __launch_bounds__(256) export_ladder_kernel(const __grid_constant__ LadderArgs a) {
+// The ladder's loop; Yuv: the rungs may be I420, YUV444 or P010 (export_ladder_yuv_kernel), else they are NV12, RGBA or
+// BGRA (export_ladder_kernel, whose code does not see the new formats)
+template <typename Index, bool Yuv>
+__device__ __forceinline__ void ladder_loop(const LadderArgs& a) {
     const Index units = (Index) a.units, items = (Index) a.count * units;
     const Index warps = (Index) (((size_t) gridDim.x * blockDim.x) >> 5);
     const int lane = threadIdx.x & 31;
@@ -299,7 +483,22 @@ __global__ void __launch_bounds__(256) export_ladder_kernel(const __grid_constan
         const RungView v = { a.fb, a.marks, a.mark_rows, a.w, a.h, g.format, g.pitch, g.src_x, g.src_y, g.src_w, g.src_h, g.out_w, g.out_h };
         const ExportFmt f = { g.format, g.over, a.native, g.bg };
         const ExportEntryUV* e = a.list + (size_t) k * a.nrungs + rung;
-        if (g.whole) {
+        if (Yuv && g.format != GLAVA_B200_EXPORT_NV12 && export_yuv(g.format)) {
+            const size_t cr = a.yuv[rung].cr_offset;
+            if (g.whole) {
+                const int x = col * 128 + lane * 4;
+                if (x >= a.w) continue;
+                uint8_t* const dst = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst)));
+                uint8_t* const cb = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst_uv)));
+                const int slot = __ldg(&e->slot);
+                const uint32_t* frame = reinterpret_cast<const uint32_t*>(a.fb) + (size_t) slot * a.h * a.w;
+                const ExportZero z = { a.yuv[rung].zy, a.yuv[rung].zu, a.yuv[rung].zv };
+                yuv_item<true>(v, f, g.format, frame, slot, dst, cb, cr, row, col, x, z);
+            } else {
+                const ExportRecip rcp = { g.div_mul, g.div_shift };
+                scaled_yuv_item<true>(v, f, g.format, rcp, g.zc, cr, e, row, col * 32 + lane, lane);
+            }
+        } else if (g.whole) {
             const int x = col * 128 + lane * 4;
             if (x >= a.w) continue;
             uint8_t* const dst = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst)));
@@ -317,10 +516,21 @@ __global__ void __launch_bounds__(256) export_ladder_kernel(const __grid_constan
     }
 }
 
+template <typename Index>
+__global__ void __launch_bounds__(256) export_ladder_kernel(const __grid_constant__ LadderArgs a) { ladder_loop<Index, false>(a); }
+template <typename Index>
+__global__ void __launch_bounds__(256) export_ladder_yuv_kernel(const __grid_constant__ LadderArgs a) { ladder_loop<Index, true>(a); }
+
 int launch_export_ladder(const LadderArgs& a, void* stream) {
     const ExportGrid g = export_grid((uint64_t) a.count * (uint64_t) a.units);
-    if (g.narrow) export_ladder_kernel<uint32_t><<<g.blocks, 256, 0, (cudaStream_t) stream>>>(a);
-    else export_ladder_kernel<uint64_t><<<g.blocks, 256, 0, (cudaStream_t) stream>>>(a);
+    bool yuv = false;
+    for (int j = 0; j < a.nrungs; ++j) yuv |= a.rung[j].format != GLAVA_B200_EXPORT_NV12 && export_yuv(a.rung[j].format);
+    cudaStream_t st = (cudaStream_t) stream;
+    if (yuv) {
+        if (g.narrow) export_ladder_yuv_kernel<uint32_t><<<g.blocks, 256, 0, st>>>(a);
+        else export_ladder_yuv_kernel<uint64_t><<<g.blocks, 256, 0, st>>>(a);
+    } else if (g.narrow) export_ladder_kernel<uint32_t><<<g.blocks, 256, 0, st>>>(a);
+    else export_ladder_kernel<uint64_t><<<g.blocks, 256, 0, st>>>(a);
     return launch_status("ladder export");
 }
 

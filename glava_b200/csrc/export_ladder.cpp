@@ -32,14 +32,15 @@ int ladder_check(glava_b200* r, const int* streams, int count, const glava_b200_
     for (int j = 0; j < nrungs; ++j) {
         char name[96];
         snprintf(name, sizeof(name), "%s: rung %d", who, j);
-        const bool nv12 = rungs[j].desc.format == GLAVA_B200_EXPORT_NV12;
+        const bool yuv = export_yuv(rungs[j].desc.format);
         for (int i = 0; i < count; ++i) {
             d[i] = dst[(size_t) i * nrungs + j];
             uv[i] = dst_uv ? dst_uv[(size_t) i * nrungs + j] : nullptr;
-            if (uv[i] && !nv12)
-                return fail(GLAVA_B200_EINVAL, "%s: dst_uv[%d] is for NV12 only (entry %d)", name, i * nrungs + j, i);
+            if (uv[i] && !yuv)
+                return fail(GLAVA_B200_EINVAL, "%s: dst_uv[%d] is for NV12 only, or I420, YUV444 and P010 (entry %d)", name,
+                            i * nrungs + j, i);
         }
-        rc = export_check(ExportKind::scaled, r, streams, count, d.data(), dst_uv && nv12 ? uv.data() : nullptr, &rungs[j].desc,
+        rc = export_check(ExportKind::scaled, r, streams, count, d.data(), dst_uv && yuv ? uv.data() : nullptr, &rungs[j].desc,
                           &rungs[j].scale, name, q ? q + j : nullptr);
         if (rc) return rc;
     }
@@ -51,7 +52,7 @@ static int ladder_schedule_room(const RendererView& v, ExportList* L, const Ladd
     std::vector<int> key = { v.w, v.h, nrungs };
     for (int j = 0; j < nrungs; ++j) {
         const LadderGeom& g = geom[j];
-        key.insert(key.end(), { g.src_x, g.src_y, g.src_w, g.src_h, g.out_w, g.out_h, (int) g.whole, (int) g.nv12 });
+        key.insert(key.end(), { g.src_x, g.src_y, g.src_w, g.src_h, g.out_w, g.out_h, (int) g.whole, (int) g.pairs });
     }
     if (key == L->sched_key && L->sched_cap) { *units = (uint32_t) L->sched_h.size(); return 0; }
     L->sched_key.clear();
@@ -80,12 +81,12 @@ int ladder_run(glava_b200* r, const int* streams, int count, const glava_b200_ex
     if (rc) return rc;
     const RendererView v = renderer_view(r);
     LadderGeom geom[GLAVA_B200_LADDER_MAX];
-    size_t uv_offset[GLAVA_B200_LADDER_MAX];
+    ExportPlanes planes[GLAVA_B200_LADDER_MAX];
     for (int j = 0; j < nrungs; ++j) {
-        geom[j] = { q[j].src_x, q[j].src_y, q[j].src_w, q[j].src_h, q[j].out_w, q[j].out_h, false,
-                    rungs[j].desc.format == GLAVA_B200_EXPORT_NV12 };
+        const glava_b200_export& d = rungs[j].desc;
+        geom[j] = { q[j].src_x, q[j].src_y, q[j].src_w, q[j].src_h, q[j].out_w, q[j].out_h, false, export_420(d.format) };
         geom[j].whole = ladder_whole(v.w, v.h, geom[j]);
-        uv_offset[j] = rungs[j].desc.uv_offset ? rungs[j].desc.uv_offset : rungs[j].desc.pitch * (size_t) q[j].out_h;
+        planes[j] = export_planes(d.format, d.pitch, d.uv_offset, q[j].out_h);
     }
     CU(cudaSetDevice(v.device));
     const size_t n = (size_t) count * (size_t) nrungs, bytes = n * sizeof(ExportEntryUV);
@@ -100,7 +101,7 @@ int ladder_run(glava_b200* r, const int* streams, int count, const glava_b200_ex
         for (int j = 0; j < nrungs; ++j) {
             const size_t e = (size_t) i * nrungs + j;
             uint8_t* const d = (uint8_t*) dst[e];
-            uint8_t* const uv = !geom[j].nv12 ? nullptr : dst_uv ? (uint8_t*) dst_uv[e] : d + uv_offset[j];
+            uint8_t* const uv = !export_yuv(rungs[j].desc.format) ? nullptr : dst_uv ? (uint8_t*) dst_uv[e] : d + planes[j].cb;
             host[e] = { d, uv, slot, 0 };
         }
     }
@@ -116,7 +117,7 @@ int ladder_run(glava_b200* r, const int* streams, int count, const glava_b200_ex
             const glava_b200_export& d = rungs[j].desc;
             LadderRung& g = a.rung[j];
             g.format = d.format;
-            g.over = geom[j].nv12 || (d.flags & GLAVA_B200_EXPORT_OVER) ? 1 : 0;
+            g.over = export_yuv(d.format) || (d.flags & GLAVA_B200_EXPORT_OVER) ? 1 : 0;
             g.whole = geom[j].whole ? 1 : 0;
             g.bg = background(d);
             g.pitch = d.pitch;
@@ -131,6 +132,9 @@ int ladder_run(glava_b200* r, const int* streams, int count, const glava_b200_ex
             g.zuv = export_nv12_quad(f, zero4, zero4, &g.zy, &zy1);
             g.zpx = export_px(f, 0u);
             g.zc = f.over ? export_over(0u, f.bg, f.native) : 0u;
+            // and as export_yuv_kernel computes them for I420, YUV444 and P010
+            const ExportZero z = export_zero(f);
+            a.yuv[j] = { planes[j].cr, z.y, z.u, z.v };
         }
         return launch_export_ladder(a, v.stream);
     });

@@ -13,8 +13,9 @@
 
 namespace glb {
 
-// One rung as the schedule sees it: its rectangle (defaults applied), whether it is the whole frame at its own size, NV12
-struct LadderGeom { int src_x, src_y, src_w, src_h, out_w, out_h; bool whole, nv12; };
+// One rung as the schedule sees it: its rectangle (defaults applied), whether it is the whole frame at its own size, and
+// whether its scaled items are 4:2:0 row pairs (NV12, I420, P010)
+struct LadderGeom { int src_x, src_y, src_w, src_h, out_w, out_h; bool whole, pairs; };
 
 // the whole frame of a w x h renderer at its own size: export_kernel's items
 inline bool ladder_whole(int w, int h, const LadderGeom& g) {
@@ -24,7 +25,7 @@ inline bool ladder_whole(int w, int h, const LadderGeom& g) {
 // the top-down index of the first source row unit `row` of rung g reads
 inline int ladder_first_row(const LadderGeom& g, int row) {
     if (g.whole) return 2 * row;
-    return g.src_y + export_span(g.nv12 ? 2 * row : row, g.src_h, g.out_h).first;
+    return g.src_y + export_span(g.pairs ? 2 * row : row, g.src_h, g.out_h).first;
 }
 
 // the units of every rung of a w x h frame, in schedule order
@@ -33,7 +34,7 @@ inline std::vector<uint64_t> ladder_schedule(int w, int h, const LadderGeom* run
     std::vector<Keyed> all;
     for (int r = 0; r < nrungs; ++r) {
         const LadderGeom& g = rungs[r];
-        const int rows = g.whole ? (h + 1) >> 1 : g.nv12 ? g.out_h >> 1 : g.out_h;
+        const int rows = g.whole ? (h + 1) >> 1 : g.pairs ? g.out_h >> 1 : g.out_h;
         const int cols = g.whole ? (w + 127) >> 7 : (g.out_w + 31) >> 5;
         for (int row = 0; row < rows; ++row) {
             const int first = ladder_first_row(g, row);

@@ -361,34 +361,53 @@ int   glava_b200_framebuffer_ipc(glava_b200* r, void* handle, size_t handle_byte
  *     GLAVA_B200_EXPORT_NV12   Y plane of h rows x w bytes, then the interleaved CbCr plane of h / 2 rows x w bytes at
  *                              `uv_offset` (0: pitch * h); BT.709 limited range in 16-bit fixed point (export_core.h),
  *                              chroma from the per-channel average (s + 2) >> 2 of each composited 2x2 block; w and h even
- *   GLAVA_B200_EXPORT_OVER     (implied for NV12) the opaque colour GLava's window shows over `background` (RGB8,
+ *     GLAVA_B200_EXPORT_I420   planar 4:2:0 (yuv420p): Y plane of h rows x w bytes at `pitch`, then the Cb and Cr planes of
+ *                              h / 2 rows x w / 2 bytes at `pitch / 2`; NV12's arithmetic, so Y equals NV12's Y and Cb / Cr
+ *                              the deinterleaved NV12 CbCr plane, bit for bit; w and h even, pitch a multiple of 32
+ *     GLAVA_B200_EXPORT_YUV444 planar 4:4:4: Y, Cb and Cr planes of h rows x w bytes at `pitch`; Y as NV12's, Cb / Cr per
+ *                              composited pixel with no averaging
+ *     GLAVA_B200_EXPORT_P010   10-bit 4:2:0: Y plane of h rows x w little-endian uint16, then the interleaved CbCr plane of
+ *                              h / 2 rows x w / 2 (Cb, Cr) uint16 pairs, both at `pitch` (>= 2 w); each sample is the 10-bit
+ *                              BT.709 limited-range code << 6; chroma from the exact per-channel sums of each composited
+ *                              2x2 block (export_core.h); w and h even
+ *   Where the chroma planes go: NV12 and P010 put the CbCr plane at `uv_offset` from dst[i] (0: pitch * h).  I420 and
+ *   YUV444 put the Cb plane right after the luma, at dst[i] + pitch * h, and `uv_offset` is the distance from Cb to Cr (0: the
+ *   Cb plane's own size, so the planes sit back to back as a yuv420p / yuv444p buffer does); when set it is at least one
+ *   chroma plane.  All YUV formats are composited (EXPORT_OVER implied).
+ *   GLAVA_B200_EXPORT_OVER     (implied for the YUV formats) the opaque colour GLava's window shows over `background` (RGB8,
  *                              byte 3 unused): under setopacity "native" (premultiply_alpha) C = min(255, c +
  *                              mul_norm8(bg, 255 - a)) per channel; under any other opacity the stored colour (the window
  *                              ignores alpha and the clear colour already stands in for the desktop).  Alpha becomes 255.
  *                              Without it RGBA / BGRA carry the stored pixels, alpha included.
- *   dst[i], pitch and uv_offset are multiples of 16, pitch >= the row bytes, uv_offset (when set) >= pitch * h.  An unknown
- *   format or flag, odd NV12 dimensions, a misaligned or short pitch, a null, host or other-device dst, a stream out of
- *   range, count < 1 and a renderer a failed rebuild left unbuilt are GLAVA_B200_EINVAL with nothing enqueued.
+ *   dst[i], pitch and uv_offset are multiples of 16, pitch >= the row bytes, uv_offset (when set) >= pitch * h (I420 /
+ *   YUV444: >= one chroma plane).  An unknown format or flag, odd NV12 / I420 / P010 dimensions, a misaligned or short pitch
+ *   (I420: not a multiple of 32), a null, host or other-device dst, a stream out of range, count < 1 and a renderer a failed
+ *   rebuild left unbuilt are GLAVA_B200_EINVAL with nothing enqueued.  Format 3 is unassigned.
  *   The work runs on the handle's stream (glava_b200_cuda_stream) after the latest raster pass and before the next one can
  *   overwrite a slot, so an update issued right after this call cannot change what it exports.  `after_event` (a
  *   cudaEvent_t, or NULL): the export waits for it on the device before writing the destinations — it holds back the
  *   handle's stream, and so the next raster pass, until then.  `done_event` (or NULL) is recorded after the export.
  *   Returns once the work is enqueued, without a host wait.
- *   glava_b200_export_bytes    the bytes one destination spans for `desc` on this renderer (pitch * h; NV12: uv_offset +
- *                              pitch * h / 2), after the same descriptor checks.
+ *   glava_b200_export_bytes    the bytes one destination spans for `desc` on this renderer (pitch * h; NV12 / P010:
+ *                              uv_offset + pitch * h / 2; I420 / YUV444: pitch * h + the Cb to Cr distance + one chroma
+ *                              plane), after the same descriptor checks.
  *   glava_b200_sharded_export_frames  the same with global stream indices, dst[i] on the device of the shard that owns
  *                              streams[i]; every index and pointer is checked before any shard starts, the shards issue
  *                              concurrently, and glava_b200_sharded_sync completes the work. */
 #define GLAVA_B200_EXPORT_RGBA 0
 #define GLAVA_B200_EXPORT_BGRA 1
 #define GLAVA_B200_EXPORT_NV12 2
+#define GLAVA_B200_EXPORT_I420 4
+#define GLAVA_B200_EXPORT_YUV444 5
+#define GLAVA_B200_EXPORT_P010 6
 #define GLAVA_B200_EXPORT_OVER 1u
 typedef struct {
-    int      format;            /* GLAVA_B200_EXPORT_RGBA / _BGRA / _NV12 */
+    int      format;            /* GLAVA_B200_EXPORT_RGBA / _BGRA / _NV12 / _I420 / _YUV444 / _P010 */
     uint32_t flags;             /* GLAVA_B200_EXPORT_OVER */
     uint8_t  background[4];     /* R, G, B of the opaque background the composite uses; byte 3 unused */
-    size_t   pitch;             /* bytes from one output row to the next (both NV12 planes) */
-    size_t   uv_offset;         /* NV12: bytes from dst[i] to the CbCr plane, 0 = pitch * h */
+    size_t   pitch;             /* bytes from one output row to the next (every plane; I420 chroma rows: pitch / 2) */
+    size_t   uv_offset;         /* NV12 / P010: bytes from dst[i] to the CbCr plane, 0 = pitch * h; I420 / YUV444: bytes
+                                   from the Cb plane to the Cr plane, 0 = one chroma plane */
 } glava_b200_export;
 int glava_b200_export_bytes(const glava_b200* r, const glava_b200_export* desc, size_t* bytes);
 int glava_b200_export_frames(glava_b200* r, const int* streams, int count, void* const* dst,
@@ -404,17 +423,21 @@ int glava_b200_export_frames(glava_b200* r, const int* streams, int count, void*
  *                              glava_b200_export_frames.  RGBA / BGRA without EXPORT_OVER average the stored channels
  *                              (premultiplied under native opacity); with it, and for NV12, each source pixel is composited
  *                              first and alpha is 255.  NV12 is the export's arithmetic on the scaled image (Y per pixel,
- *                              chroma per 2x2 output block), so out_w and out_h are even.
- *     dst[i]                   out_h rows of out_w * 4 bytes (RGBA / BGRA) or out_w bytes (Y), `pitch` bytes apart
- *     dst_uv                   NV12: dst_uv[i] receives the out_h / 2 CbCr rows (a mosaic tile's chroma need not sit at one
- *                              offset from its luma); NULL: dst[i] + (uv_offset ? uv_offset : pitch * out_h)
+ *                              chroma per 2x2 output block), so out_w and out_h are even; I420, YUV444 and P010 likewise
+ *                              apply their own arithmetic to the scaled image (out_w and out_h even for I420 and P010).
+ *     dst[i]                   out_h rows of out_w * 4 bytes (RGBA / BGRA), out_w bytes (Y) or out_w uint16 (P010 Y),
+ *                              `pitch` bytes apart
+ *     dst_uv                   NV12 / P010: dst_uv[i] receives the out_h / 2 CbCr rows (a mosaic tile's chroma need not sit
+ *                              at one offset from its luma); NULL: dst[i] + (uv_offset ? uv_offset : pitch * out_h).
+ *                              I420 / YUV444: dst_uv[i] is the Cb plane, NULL: dst[i] + pitch * out_h; the Cr plane is
+ *                              uv_offset past it (0: the Cb plane's size), which lets a planar mosaic tile find its Cr rows
  *   Nothing outside each out_w x out_h rectangle and its chroma rows is written: pitch padding and neighbouring tiles keep
  *   their bytes.  dst[i], dst_uv[i], pitch and uv_offset are multiples of 16 (a mosaic tile starts at a multiple of 4 pixels
  *   in RGBA, of 16 in NV12).  Besides every refusal of glava_b200_export_frames (pitch and uv_offset measured against the
  *   output), a null `scale`, a rectangle that is empty or leaves the frame, upscaling, odd NV12 output dimensions, a
  *   misaligned, null, host or other-device dst_uv[i], and dst_uv for RGBA / BGRA are GLAVA_B200_EINVAL with nothing enqueued.
- *   glava_b200_export_scaled_bytes   the bytes one destination spans (pitch * out_h; NV12 with dst_uv NULL: uv_offset +
- *                              pitch * out_h / 2), after the same descriptor and rectangle checks.
+ *   glava_b200_export_scaled_bytes   the bytes one destination spans (as glava_b200_export_bytes with out_h for h, dst_uv
+ *                              NULL), after the same descriptor and rectangle checks.
  *   glava_b200_sharded_export_scaled  the same with global stream indices, dst[i] / dst_uv[i] on the device of the shard
  *                              that owns streams[i]; every entry is checked before any shard starts. */
 typedef struct {
@@ -472,6 +495,7 @@ int glava_b200_export_ladder(glava_b200* r, const int* streams, int count, const
  *   pixel leaves D exactly as it was, and rows the dirty-row marks skip and all-zero quads are neither read nor written.
  *   An opaque pixel gives exactly glava_b200_export_frames' bytes.  Under any other opacity GLava's window is opaque: the
  *   rectangle gets exactly what glava_b200_export_frames writes (RGBA / BGRA with EXPORT_OVER, or NV12).
+ *   The overlay takes RGBA, BGRA and NV12; I420, YUV444 and P010 are refused by name.
  *   Besides the refusals of glava_b200_export_scaled that apply (format, pitch, uv_offset, alignment, null / host /
  *   other-device dst or dst_uv, dst_uv for RGBA / BGRA, odd NV12 frames, stream range, count < 1, an unbuilt renderer),
  *   any flag, a rectangle that meets the renderer's framebuffer array and two rectangles of one call that overlap (luma
