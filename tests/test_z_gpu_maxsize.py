@@ -1,5 +1,5 @@
-"""-m gpu: the largest shapes of BASELINE.json — 7680x4320 frames, setbufsize 16384 — checked against the oracle on row
-bands (the oracle renders only the requested rows, so 33 M-pixel frames stay cheap): bottom rows, the rows around the
+"""-m gpu: the largest shapes of BASELINE.json — 7680x4320 frames, setbufsize 16384 — and the largest sides the renderer
+takes (16384 x 256, 256 x 16384), checked against the oracle on row bands (the oracle renders only the requested rows, so 33 M-pixel frames stay cheap): bottom rows, the rows around the
 tallest bars, the vertical centre and the top rows, bit-exact."""
 import numpy as np
 import pytest
@@ -18,7 +18,10 @@ def _tex(orc, op, n, seed):
 
 
 @pytest.mark.parametrize("module,n,w,h", [("bars", 16384, 7680, 4320), ("radial", 8192, 3840, 2160), ("graph", 16384, 7680, 4320),
-                                          ("wave", 4096, 7680, 4320), ("circle", 4096, 3840, 2160)])
+                                          ("wave", 4096, 7680, 4320), ("circle", 4096, 3840, 2160),
+                                          # the largest sides the renderer takes: 128 strips of 128 pixels, 16384 rows
+                                          ("bars", 4096, 16384, 256), ("graph", 4096, 16384, 256), ("wave", 4096, 16384, 256),
+                                          ("bars", 4096, 256, 16384), ("graph", 4096, 256, 16384), ("wave", 4096, 256, 16384)])
 def test_largest_frames_row_bands_bit_exact(orc_pm, module, n, w, h, built):
     p = g.default_params(module, n=n, w=w, h=h)
     op = params_from(p)
