@@ -92,7 +92,10 @@ inline RasterTables raster_tables(const glava_b200_params& p, const RasterKnobs&
     t.geo_caches = p.module == GLAVA_B200_MOD_RADIAL ? geo_caches : 1;
     // circle: only when the module samples a pre-smoothed texture, i.e. smooth_audio() is a single texelFetch
     if (p.module == GLAVA_B200_MOD_RADIAL || (p.module == GLAVA_B200_MOD_CIRCLE && p.smooth_pass)) {
-        const size_t bytes = polar_geo_box(p, t.box);
+        // radial caches lie back to back, `geo_bytes` apart: a box of w x h pixels takes 25 B per pixel, so the stride is
+        // rounded up to 256 B, else cache 1 of a box whose w * h is not a multiple of 16 starts off the 16-byte alignment
+        // of its int4 entries
+        const size_t bytes = (polar_geo_box(p, t.box) + 255) & ~(size_t) 255;
         t.geo = bytes > 0 && bytes * (size_t) t.geo_caches <= ((size_t) 512 << 20) && !k.no_geo;
         t.geo_bytes = t.geo ? bytes : 0;
         // per-tile annulus from bucketed texture min / max (DESIGN 4.2): off by default, GLAVA_B200_CTILE=1 enables it (the

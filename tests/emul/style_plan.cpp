@@ -25,4 +25,10 @@ void emul_styled_raster_plan(const glava_b200_params* sp, int slots, int geo_cac
     for (size_t i = 0; i < sizeof(v) / sizeof(v[0]); ++i) out[i] = v[i];
 }
 
+// box[4] = { x0, y0, w, h }: the polar geometry box of a renderer whose style slots have the parameters sp[0 .. slots)
+// (polar_geo_box of style_reach_params, as raster_tables builds it); all 0 for the other modules
+void emul_styled_geo_box(const glava_b200_params* sp, int slots, int* box) {
+    polar_geo_box(style_reach_params(sp[0], sp, slots), box);
+}
+
 }  // extern "C"

@@ -7,7 +7,8 @@
 // exists, and reports a pending runtime error as its launch failure, as the real launchers' post-launch check does.
 // Between fake_trace_begin and fake_trace_end both halves write a trace of the calls that enqueue work or wait for it
 // (launches, copies, fills, event records and waits, synchronisations), one line each, with streams and events numbered
-// in the order they were created since fake_trace_begin (s0: the legacy default stream).
+// in the order they were created since fake_trace_begin (s0: the legacy default stream).  launch_polar_geo records the
+// parameters and the box of every call, so that a test can check which geometry caches the rebuild path asks for.
 #include <cuda_runtime.h>
 
 #include "../../glava_b200/csrc/internal.h"
@@ -20,6 +21,7 @@
 #include <map>
 #include <set>
 #include <string>
+#include <vector>
 
 namespace {
 enum Kind { BUF, PINNED, EVENT, STREAM, KINDS };
@@ -32,6 +34,8 @@ bool g_tracing = false;
 std::string g_trace;
 std::map<const void*, int> g_ids[KINDS];
 int g_next_id[KINDS];
+struct GeoCall { glava_b200_params p; int box[4]; int misalign; };
+std::vector<GeoCall> g_geo;
 
 void trace(const char* fmt, ...) {
     if (!g_tracing) return;
@@ -171,7 +175,17 @@ long fake_violations(void) { return g_violations; }
 const char* fake_first_violation(void) { return g_violation.c_str(); }
 long fake_stale(void) { return g_stale; }
 long fake_reached(void) { return g_reached; }
-void fake_clear(void) { g_launches = g_violations = g_stale = g_reached = 0; g_violation.clear(); g_last = cudaSuccess; }
+void fake_clear(void) { g_launches = g_violations = g_stale = g_reached = 0; g_violation.clear(); g_last = cudaSuccess; g_geo.clear(); }
+// the launch_polar_geo calls since fake_clear: their count, and call i's parameters and box; returns the cache address
+// modulo 16, which must be 0 for its int4 entries (the fake's buffers are 16-byte aligned, as cudaMalloc's are), or -1: no
+// such call
+long fake_geo_calls(void) { return (long) g_geo.size(); }
+int fake_geo_call(long i, glava_b200_params* p, int* box) {
+    if (i < 0 || i >= (long) g_geo.size()) return -1;
+    *p = g_geo[(size_t) i].p;
+    for (int k = 0; k < 4; ++k) box[k] = g_geo[(size_t) i].box[k];
+    return g_geo[(size_t) i].misalign;
+}
 // start a trace: streams and events are numbered from 1 in the order they are created from now on
 void fake_trace_begin(void) {
     g_trace.clear();
@@ -203,7 +217,14 @@ int launch_raster(const glava_b200_params&, const RasterPlan& pl, const RasterAr
 }
 int launch_bars_rowtab(const glava_b200_params&, void* d_rowtab, void* st) { return launched("row table", st, d_rowtab != nullptr); }
 int launch_texmm(const glava_b200_params&, const uint16_t* tex, uint32_t* out, int, void* st) { return launched("texmm", st, tex && out); }
-int launch_polar_geo(const glava_b200_params&, void* d_geo, const int*, void* st) { return launched("polar geometry", st, d_geo != nullptr); }
+int launch_polar_geo(const glava_b200_params& p, void* d_geo, const int* box, void* st) {
+    GeoCall c;
+    c.p = p;
+    for (int k = 0; k < 4; ++k) c.box[k] = box[k];
+    c.misalign = (int) ((uintptr_t) d_geo % 16);
+    g_geo.push_back(c);
+    return launched("polar geometry", st, d_geo != nullptr);
+}
 size_t circle_tile_bytes(const glava_b200_params& p, int* ntx, int* nty) {
     *ntx = (p.w + 127) / 128; *nty = (p.h + 7) / 8;
     return (size_t) *ntx * *nty * (sizeof(int4) + sizeof(int));

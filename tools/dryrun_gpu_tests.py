@@ -2,7 +2,8 @@
 to validate the test scripts themselves (golden keys, expectations, parameter plumbing) when no GPU is at hand.  The device
 plumbing stays untested, of course.
 
-    python tools/dryrun_gpu_tests.py
+    python tools/dryrun_gpu_tests.py                  # the scripts of SCRIPTS
+    python tools/dryrun_gpu_tests.py tests/x.py ...    # these scripts instead (paths relative to the repository root)
 """
 import sys, ctypes as C
 import os
@@ -20,12 +21,26 @@ class Fake:
         rc = g.lib().glava_b200_load_config  # noqa
         self.params = params.copy(); self.batch = batch; self.nsz = params.n; self._launch = 0; self._h = 1
         self.frames = [None] * batch
+        self.styles = [g.StreamStyle() for _ in range(batch)]
+    # stream styles: stream s renders what a renderer of style_params(params, style_s) renders
+    def set_stream_styles(self, streams, styles):
+        streams, styles = list(streams), list(styles)
+        assert len(streams) == len(styles) and len(set(streams)) == len(streams)
+        for s, st in zip(streams, styles):
+            assert 0 <= s < self.batch
+            g.style_params(self.params, st)                       # refused styles raise, as the library's call does
+            self.styles[s] = g.stream_style(st)
+    def get_stream_styles(self, streams):
+        return [self.styles[s] for s in streams]
+    def _stream_params(self, s):
+        return g.style_params(self.params, self.styles[s]) if self.styles[s].set else self.params
     def raster_textures(self, tl, tr=None):
         tl = np.asarray(tl); tr = tl if tr is None else np.asarray(tr)
         for s in range(self.batch):
-            key = (bytes(self.params), tl[s].tobytes(), tr[s].tobytes())
+            q = self._stream_params(s)
+            key = (bytes(q), tl[s].tobytes(), tr[s].tobytes())
             if key not in _frames:
-                _frames[key] = emul.raster(self.params, tl[s], tr[s])
+                _frames[key] = emul.raster(q, tl[s], tr[s])
             self.frames[s] = _frames[key].copy()
         self._launch += self._raster_launches()
     def _raster_launches(self):
@@ -46,7 +61,7 @@ class Fake:
         rb = lb if rb is None else rb
         self._tex = [st.update(lb[s], rb[s], modified)[2:] for s, st in enumerate(self._streams)]
         self.nsz = self._streams[0].n
-        self.frames = [emul.raster(self.params, t[0], t[1]) for t in self._tex]
+        self.frames = [emul.raster(self._stream_params(s), t[0], t[1]) for s, t in enumerate(self._tex)]
     def textures(self):
         return np.stack([t[0] for t in self._tex]), np.stack([t[1] for t in self._tex])
     def reconfigure(self, p): self.params = p.copy(); self._launch += 1
@@ -65,7 +80,7 @@ def fake_apply(self, renderer):
         return
     self._last = self.binds(); renderer.reconfigure(self.params())
 api.Pipe.apply = fake_apply
-sys.exit(pytest.main(["-x", "-q", "-m", "gpu", "-p", "no:cacheprovider",
-                      ROOT + "/tests/test_zz_gpu_blend.py", ROOT + "/tests/test_zz_gpu_color_expr.py", ROOT + "/tests/test_zz_gpu_pipe.py", ROOT + "/tests/test_glsl_golden.py", ROOT + "/tests/test_zz_rd_golden.py", ROOT + "/tests/test_llvmpipe_golden.py",
-                      ROOT + "/tests/test_gpu_raster_variants.py",
-                      ]))
+SCRIPTS = ["tests/test_zz_gpu_blend.py", "tests/test_zz_gpu_color_expr.py", "tests/test_zz_gpu_pipe.py", "tests/test_glsl_golden.py",
+           "tests/test_zz_rd_golden.py", "tests/test_llvmpipe_golden.py", "tests/test_gpu_raster_variants.py"]
+sys.exit(pytest.main(["-x", "-q", "-m", "gpu", "-p", "no:cacheprovider"] +
+                     [os.path.join(ROOT, f) for f in (sys.argv[1:] or SCRIPTS)]))
