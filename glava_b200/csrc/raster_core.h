@@ -40,6 +40,92 @@ GLB_HD float cop_smoothstep(float e0, float e1, float x) {
     return (t * t) * (3.0f - (2.0f * t));
 }
 GLB_HD float& cop_lane(f4& r, int k) { return k == 0 ? r.r : (k == 1 ? r.g : (k == 2 ? r.b : r.a)); }
+// ---- the colour VM's transcendentals over the whole float range (DESIGN §4.5) ----
+// The module kernels call gl_math.h with bounded, positive arguments; a user's expression can pass any float.  These
+// wrappers give gl_math.h's results where its reductions hold, and IEEE's answers beyond: sin / cos / tan of any finite x
+// lie in [-1, 1] (Payne-Hanek past |x| = 8192), log is -inf at +-0, NaN below 0 and at NaN, +inf at +inf and finite on
+// subnormals, atan(+-inf, +-inf) is +-pi/4 or +-3pi/4.  Integer and correctly rounded float operations only, so the
+// device and the host build agree bit for bit.
+GLB_HD float cvm_inf() { return glm_u2f(0x7f800000u); }
+GLB_HD float cvm_nan() { return glm_u2f(0x7fffffffu); }
+// bits 32 (j - 1) + 1 .. 32 j after the binary point of 2/pi; word 0 stands for 32 zero bits before it
+GLB_HD uint32_t cvm_2opi_word(int j) {
+    switch (j) {
+        case 1: return 0xa2f9836eu; case 2: return 0x4e441529u; case 3: return 0xfc2757d1u; case 4: return 0xf534ddc0u;
+        case 5: return 0xdb629599u; case 6: return 0x3c439041u; case 7: return 0xfe5163abu; default: return 0u;
+    }
+}
+GLB_HD uint32_t cvm_funnel(uint32_t hi, uint32_t lo, int s) { return s ? (hi << s) | (lo >> (32 - s)) : hi; }
+// x = r + q pi/2 (mod 2 pi), |r| <= pi/4, for finite |x| > 8192.  |x| = m 2^e with m < 2^24, so x 2/pi = m sum_k t_k 2^(e - k)
+// over the bits t_k of 2/pi; the terms k <= e - 2 are multiples of 4.  The 96 bits from k = e - 1 on form W, and
+// x 2/pi = m W 2^-94 (mod 4) up to less than 2^-71 from the bits past W.
+GLB_HD float cvm_reduce_large(float x, int* q) {
+    const uint32_t u = glm_f2u(x);
+    const uint64_t m = (u & 0x007fffffu) | 0x00800000u;
+    const int k0 = (int) ((u >> 23) & 0xffu) - 120, i = k0 >> 5, s = k0 & 31;   // k0 = (e - 1) + 31: bit offset in the words
+    const uint32_t t0 = cvm_2opi_word(i), t1 = cvm_2opi_word(i + 1), t2 = cvm_2opi_word(i + 2), t3 = cvm_2opi_word(i + 3);
+    const uint64_t p2 = m * cvm_funnel(t2, t3, s);
+    const uint64_t p1 = m * cvm_funnel(t1, t2, s) + (p2 >> 32);
+    const uint64_t p0 = m * cvm_funnel(t0, t1, s) + (p1 >> 32);
+    int k = (int) ((p0 >> 30) & 3u);
+    int64_t f = (int64_t) (((p0 & 0x3fffffffu) << 32) | (p1 & 0xffffffffu));  // the fraction in units of 2^-62
+    if (f >= ((int64_t) 1 << 61)) { f -= (int64_t) 1 << 62; k += 1; }        // to the nearest quadrant
+    // r = f 2^-62 pi/2, with f split into two floats and pi/2 into PIO2_HI + PIO2_LO (as glm_sin)
+    const float fh = (float) f, fl = (float) (f - (int64_t) fh);
+    float r = glm_fma(fh, 1.57079637050628662109375f, glm_fma(fh, -4.37113900018624283e-08f, glm_mul(fl, 1.57079637050628662109375f)));
+    r = glm_mul(r, 0x1p-62f);
+    if (u >> 31) { r = -r; k = -k; }
+    *q = k & 3;
+    return r;
+}
+// any x: glm_sin's own reduction up to |x| = 8192, Payne-Hanek beyond, NaN for inf and NaN
+GLB_HD float cvm_reduce(float x, int* q) {
+    const float ax = glm_abs(x);
+    if (ax <= 8192.0f) {
+        const float kf = glm_rint(glm_mul(x, 0.6366197466850281f));
+        float r = glm_fma(-kf, 1.57079637050628662109375f, x);
+        r = glm_fma(-kf, -4.37113900018624283e-08f, r);
+        *q = (int) kf & 3;
+        return r;
+    }
+    if (!(ax < cvm_inf())) { *q = 0; return cvm_nan(); }
+    return cvm_reduce_large(x, q);
+}
+// sin(r + q pi/2), |r| <= pi/4: glm_sin's polynomials
+GLB_HD float cvm_sin_q(float r, int q) {
+    const float z = glm_mul(r, r);
+    float s = glm_fma(z, -1.9515295891e-4f, 8.3321608736e-3f);
+    s = glm_fma(z, s, -1.6666654611e-1f);
+    s = glm_fma(glm_mul(s, z), r, r);
+    float c = glm_fma(z, 2.443315711809948e-5f, -1.388731625493765e-3f);
+    c = glm_fma(z, c, 4.166664568298827e-2f);
+    c = glm_fma(glm_mul(c, z), z, glm_fma(-0.5f, z, 1.0f));
+    const float res = (q & 1) ? c : s;
+    return (q & 2) ? -res : res;
+}
+GLB_HD float cvm_sin(float x) {
+    if (glm_abs(x) <= 8192.0f) return glm_sin(x);
+    int q; const float r = cvm_reduce(x, &q);
+    return cvm_sin_q(r, q);
+}
+GLB_HD float cvm_cos(float x) { int q; const float r = cvm_reduce(x, &q); return cvm_sin_q(r, q + 1); }
+GLB_HD float cvm_tan(float x) { int q; const float r = cvm_reduce(x, &q); return glm_div(cvm_sin_q(r, q), cvm_sin_q(r, q + 1)); }
+GLB_HD float cvm_log(float x) {
+    if (!(x > 0.0f)) return x == 0.0f ? -cvm_inf() : cvm_nan();
+    if (x == cvm_inf()) return x;
+    if (x < 1.17549435e-38f) return glm_add(glm_log(glm_mul(x, 16777216.0f)), -16.63553233343868742f);   // subnormal: log(x 2^24) - 24 ln 2
+    return glm_log(x);
+}
+// glm_exp returns 0 below ln 2^-149; e^x rounds to 2^-149 down to ln 2^-150
+GLB_HD float cvm_exp(float x) { return (x < -103.278929f && x > -103.972077f) ? glm_u2f(1u) : glm_exp(x); }
+GLB_HD float cvm_pow(float x, float y) { return x == 0.0f ? glm_pow(x, y) : cvm_exp(glm_mul(y, cvm_log(x))); }
+GLB_HD float cvm_atan2(float y, float x) {
+    if (glm_abs(x) == cvm_inf() && glm_abs(y) == cvm_inf()) {
+        const float r = x > 0.0f ? 0.785398185253143310546875f : 2.35619449615478515625f;   // float(pi/4), float(3 pi/4)
+        return (glm_f2u(y) & 0x80000000u) ? -r : r;
+    }
+    return glm_atan2(y, x);
+}
 GLB_HD_NOINLINE f4 eval_color_prog(const glava_b200_color_prog& c, float x) {
     f4 reg[GLAVA_B200_COLOR_REGS];
     for (int i = 0; i < GLAVA_B200_COLOR_REGS; ++i) reg[i] = mk4(0.0f, 0.0f, 0.0f, 0.0f);
@@ -74,9 +160,9 @@ GLB_HD_NOINLINE f4 eval_color_prog(const glava_b200_color_prog& c, float x) {
             case GLAVA_B200_COP_CEIL:  GLB_COP1(ceilf(v));
             case GLAVA_B200_COP_FRACT: GLB_COP1(v - floorf(v));
             case GLAVA_B200_COP_SQRT:  GLB_COP1(sqrtf(v));
-            case GLAVA_B200_COP_SIN:   GLB_COP1(glm_sin(v));
-            case GLAVA_B200_COP_COS:   GLB_COP1(glm_sin(v + (GLB_PI / 2.0f)));
-            case GLAVA_B200_COP_LOG:   GLB_COP1(glm_log(v));
+            case GLAVA_B200_COP_SIN:   GLB_COP1(cvm_sin(v));
+            case GLAVA_B200_COP_COS:   GLB_COP1(cvm_cos(v));
+            case GLAVA_B200_COP_LOG:   GLB_COP1(cvm_log(v));
             case GLAVA_B200_COP_SIGN:  GLB_COP1(g_sign(v));
             case GLAVA_B200_COP_TRUNC: GLB_COP1(truncf(v));
             case GLAVA_B200_COP_MIX:   GLB_COP3((v * (1.0f - u)) + (w * u));
@@ -90,12 +176,12 @@ GLB_HD_NOINLINE f4 eval_color_prog(const glava_b200_color_prog& c, float x) {
             case GLAVA_B200_COP_OR:    GLB_COP2((v != 0.0f || w != 0.0f) ? 1.0f : 0.0f);
             case GLAVA_B200_COP_NOT:   GLB_COP1(v != 0.0f ? 0.0f : 1.0f);
             case GLAVA_B200_COP_SELECT: GLB_COP3(u != 0.0f ? v : w);
-            case GLAVA_B200_COP_EXP:   GLB_COP1(glm_exp(v));
+            case GLAVA_B200_COP_EXP:   GLB_COP1(cvm_exp(v));
             case GLAVA_B200_COP_EXP2:  GLB_COP1(glm_exp2(v));
-            case GLAVA_B200_COP_LOG2:  GLB_COP1(glm_log(v) * 1.44269504088896341f);
-            case GLAVA_B200_COP_POW:   GLB_COP2(glm_pow(v, w));
-            case GLAVA_B200_COP_ATAN2: GLB_COP2(glm_atan2(v, w));
-            case GLAVA_B200_COP_TAN:   GLB_COP1(glm_sin(v) / glm_sin(v + (GLB_PI / 2.0f)));
+            case GLAVA_B200_COP_LOG2:  GLB_COP1(cvm_log(v) * 1.44269504088896341f);
+            case GLAVA_B200_COP_POW:   GLB_COP2(cvm_pow(v, w));
+            case GLAVA_B200_COP_ATAN2: GLB_COP2(cvm_atan2(v, w));
+            case GLAVA_B200_COP_TAN:   GLB_COP1(cvm_tan(v));
             default: break;
         }
     }

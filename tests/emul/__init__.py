@@ -31,6 +31,8 @@ def lib():
         L.emul_raster.argtypes = [vp, vp, vp, vp, i32, i32]
         L.emul_raster_fast.argtypes = [vp, vp, vp, vp]
         L.emul_eval_color.argtypes = [vp, C.c_float, vp]
+        L.emul_radial_geo.argtypes = [vp, vp]
+        L.emul_radial_from_geo.argtypes = [vp, vp, vp, vp, vp]
         L.emul_lazy_k5.argtypes = [vp, i32, i32, vp, vp, vp]
         L.emul_lazy_epi_n.argtypes = [vp]
         L.emul_k5_table.argtypes = [vp, vp, vp]
@@ -93,6 +95,23 @@ def raster(params, tex_l, tex_r, fast=False):
     else:
         lib().emul_raster(C.addressof(params), tl.ctypes.data, tr.ctypes.data, out.ctypes.data, 0, params.h)
     return out
+
+
+class RadialGeo:
+    """raster(params, tl, tr) for radial, with the audio-independent half of every pixel (the colour program included)
+    computed once: frames(tl, tr) is then cheap for each further texture pair"""
+
+    def __init__(self, params):
+        self.p = params
+        self.geo = np.empty(params.w * params.h * lib().emul_radial_geo_bytes(), np.uint8)
+        lib().emul_radial_geo(C.addressof(params), self.geo.ctypes.data)
+
+    def frame(self, tex_l, tex_r):
+        tl = np.ascontiguousarray(tex_l, dtype=np.uint16)
+        tr = np.ascontiguousarray(tex_r, dtype=np.uint16)
+        out = np.zeros((self.p.h, self.p.w, 4), dtype=np.uint8)
+        lib().emul_radial_from_geo(C.addressof(self.p), self.geo.ctypes.data, tl.ctypes.data, tr.ctypes.data, out.ctypes.data)
+        return out
 
 
 def bufscale(pcm, k):

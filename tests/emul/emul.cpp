@@ -191,26 +191,31 @@ int emul_raster_fast(const glava_b200_params* pp, const uint16_t* tl, const uint
     if (p.module == GLAVA_B200_MOD_BARS && !p.bars_mirror_yx) {
         std::vector<BarsCol> col(p.w);
         for (int x = 0; x < p.w; ++x) col[x] = bars_column(p, t, (float) x + 0.5f, p.w);
-        const bool has_outline = p.bars_outline_width > 0.0f;
+        const bool has_outline = p.bars_outline_width > 0.0f, native = p.premultiply_alpha != 0;
+        const uint32_t bg = native ? 0u : stage_bg<false>(p);
         for (int y = 0; y < p.h; ++y) {
             float fy = (float) y + 0.5f, d = p.bars_flip ? (float) p.h - fy : fy;
-            BarsRow rc = bars_row(p, d);
+            BarsRow rc = native ? bars_row(p, d) : bars_row_t<false>(p, d);
             for (int x = 0; x < p.w; ++x) {
                 uint32_t below = (col[x].cls == 1) ? rc.fill : rc.outl;
-                uint32_t v = (d < col[x].vm) ? below : ((has_outline && d <= col[x].v) ? rc.outl : 0u);
-                dst[(size_t) y * p.w + x] = col[x].cls ? v : 0u;
+                uint32_t v = (d < col[x].vm) ? below : ((has_outline && d <= col[x].v) ? rc.outl : bg);
+                dst[(size_t) y * p.w + x] = col[x].cls ? v : bg;
             }
         }
         return 0;
     }
     if (p.module == GLAVA_B200_MOD_GRAPH) {
+        // row colours once per row, as the row table; non-native opacity blends them (graph_row_t<false>)
+        const bool native = p.premultiply_alpha != 0;
         std::vector<float> s(p.w + 2, 0.0f);
         for (int x = 0; x < p.w; ++x) s[x + 1] = graph_height(p, t, x);
+        std::vector<uint32_t> row(p.h);
+        for (int y = 0; y < p.h; ++y) row[y] = native ? graph_row(p, y) : graph_row_t<false>(p, y);
         for (int y = 0; y < p.h; ++y) {
-            uint32_t row3[3] = { y > 0 ? graph_row(p, y - 1) : 0u, graph_row(p, y), y + 1 < p.h ? graph_row(p, y + 1) : 0u };
+            uint32_t row3[3] = { y > 0 ? row[y - 1] : 0u, row[y], y + 1 < p.h ? row[y + 1] : 0u };
             for (int x = 0; x < p.w; ++x) {
                 const float s3[3] = { s[x], s[x + 1], s[x + 2] };
-                dst[(size_t) y * p.w + x] = graph_px_cols(p, s3, row3, x, y);
+                dst[(size_t) y * p.w + x] = native ? graph_px_cols(p, s3, row3, x, y) : graph_px_cols_t<false>(p, s3, row3, x, y);
             }
         }
         return 0;
@@ -237,6 +242,32 @@ int emul_raster_fast(const glava_b200_params* pp, const uint16_t* tl, const uint
         return 0;
     }
     return -1;
+}
+
+// radial_px in its two halves: the audio-independent geometry of every pixel (which evaluates the colour program) once,
+// then any number of textures against it.  Equal to emul_raster for radial by construction (radial_px is the same code).
+int emul_radial_geo_bytes(void) { return (int) sizeof(RadialGeo); }
+void emul_radial_geo(const glava_b200_params* pp, void* geo) {
+    const glava_b200_params p = raster_view(*pp);
+    RadialGeo* g = static_cast<RadialGeo*>(geo);
+    for (int y = 0; y < p.h; ++y) for (int x = 0; x < p.w; ++x) g[(size_t) y * p.w + x] = radial_geometry(p, x, y);
+}
+void emul_radial_from_geo(const glava_b200_params* pp, const void* geo, const uint16_t* tl, const uint16_t* tr, uint8_t* out) {
+    const glava_b200_params p = raster_view(*pp);
+    AudioTex t; t.l = tl; t.r = tr; t.n = p.n; t.pre_smoothed = p.smooth_pass; t.sp = smooth_params(p);
+    const RadialGeo* gs = static_cast<const RadialGeo*>(geo);
+    uint32_t* dst = reinterpret_cast<uint32_t*>(out);
+    for (size_t i = 0; i < (size_t) p.w * p.h; ++i) {
+        const RadialGeo& g = gs[i];
+        uint32_t px = g.unlit;
+        if (g.bar >= 0) {
+            const float v = radial_bar_value(p, t, g.bar);
+            if (!(p.radial_bar_outline_width > 0.0f)) px = (g.dR <= v) ? g.lit : g.unlit;
+            else if (g.dR <= v - p.radial_bar_outline_width) px = g.lit;
+            else px = (g.dR <= v) ? g.band : g.unlit;
+        }
+        dst[i] = px;
+    }
 }
 
 // ---- optional rd_update stages (chain_core.h): the kernels' per-element functions driven the way the kernels do ----
