@@ -135,6 +135,8 @@ LADDER_MAX = 8
 EXPORT_RGBA, EXPORT_BGRA, EXPORT_NV12 = 0, 1, 2
 EXPORT_I420, EXPORT_YUV444, EXPORT_P010 = 4, 5, 6
 EXPORT_OVER = 1
+EXPORT_FULL_RANGE, EXPORT_BT601 = 0x100, 0x200          # the Y'CbCr encoding (DESIGN 4.15); neither: BT.709 limited range
+EXPORT_MATRICES = {"bt709": 0, "bt601": EXPORT_BT601}
 EXPORT_FORMATS = {"rgba": EXPORT_RGBA, "bgra": EXPORT_BGRA, "nv12": EXPORT_NV12, "i420": EXPORT_I420,
                   "yuv444": EXPORT_YUV444, "p010": EXPORT_P010}
 OVERLAY_FORMATS = ("rgba", "bgra", "nv12")
@@ -458,19 +460,20 @@ class _StreamStyles:
 class _FrameExport:
     """export_frames over the handle's C entry point: destinations as torch tensors (DESIGN 4.10)"""
 
-    def _export_plan(self, streams, fmt, over, background, out, device_of, size=None):
+    def _export_plan(self, streams, fmt, over, background, out, device_of, size=None, matrix="bt709", full_range=False):
         """-> (stream list, Export, [dst pointers], what to return).  device_of(stream): the CUDA device of a stream's
         frame.  size: (w, h) of each output, None: the frame's.  out: None (allocate), one uint8 tensor [count, rows, ...]
         whose dim 1 steps by the pitch, or a list of count tensors [rows, ...] with one common pitch; rows as
         _export_layout gives them (h for RGBA / BGRA, h * 3 / 2 for NV12, I420 and P010, 3 h for YUV444; I420 and YUV444
-        keep their planes back to back from row h); P010 also takes uint16 tensors"""
+        keep their planes back to back from row h); P010 also takes uint16 tensors.  matrix / full_range: the Y'CbCr
+        encoding (_export_desc)"""
         import torch
         s = np.ascontiguousarray(np.asarray(streams, dtype=np.int64).reshape(-1), dtype=np.int32)
         count = int(s.shape[0])
         devices = [device_of(int(x)) for x in s]
         p = self.params
         w, h = (p.w, p.h) if size is None else (int(size[0]), int(size[1]))
-        desc = _export_desc(fmt, over, background)
+        desc = _export_desc(fmt, over, background, matrix, full_range)
         rows, row_bytes, align = _export_layout(fmt, w, h)
         dtypes = (torch.uint8, torch.uint16) if fmt == "p010" else (torch.uint8,)
 
@@ -512,8 +515,8 @@ class _FrameExport:
     def _ladder_plan(self, streams, rungs, out, device_of):
         """-> (stream list, ExportRung array, nrungs, [count][nrungs] dst pointers, [one result per rung]) of an encoder
         ladder (DESIGN 4.13): each rung planned by _export_plan as export_scaled plans it.  rungs: dicts with export_scaled's
-        keywords size (None: the frame's), crop, fmt (default "nv12"), over and background; out: None or one entry per
-        rung in any form export_scaled takes"""
+        keywords size (None: the frame's), crop, fmt (default "nv12"), over, background, matrix and full_range; out: None
+        or one entry per rung in any form export_scaled takes"""
         rungs = list(rungs)
         outs = [None] * len(rungs) if out is None else list(out)
         if len(outs) != len(rungs):
@@ -523,12 +526,13 @@ class _FrameExport:
         arr = (ExportRung * max(len(rungs), 1))()
         ptrs, results = [], []
         for j, (rung, o) in enumerate(zip(rungs, outs)):
-            unknown = set(rung) - {"size", "crop", "fmt", "over", "background"}
+            unknown = set(rung) - {"size", "crop", "fmt", "over", "background", "matrix", "full_range"}
             if unknown:
                 raise ValueError(f"rungs[{j}]: unknown keys {sorted(unknown)}")
             size = rung.get("size") or (p.w, p.h)
             _, desc, dst, result = self._export_plan(s, rung.get("fmt", "nv12"), rung.get("over", False),
-                                                     rung.get("background", (0, 0, 0)), o, device_of, size)
+                                                     rung.get("background", (0, 0, 0)), o, device_of, size,
+                                                     rung.get("matrix", "bt709"), rung.get("full_range", False))
             arr[j].desc, arr[j].scale = desc, _export_scale(size, rung.get("crop"))
             ptrs.append(dst)
             results.append(result)
@@ -536,12 +540,13 @@ class _FrameExport:
         dst = (C.c_void_p * max(count * n, 1))(*[ptrs[j][i] for i in range(count) for j in range(n)])
         return s, arr, n, dst, results
 
-    def _overlay_plan(self, streams, images, at, fmt):
+    def _overlay_plan(self, streams, images, at, fmt, matrix="bt709", full_range=False):
         """-> (stream list, Export, dst pointers, dst_uv pointers or None) of an overlay (DESIGN 4.12).  images: one uint8
         CUDA tensor per entry (one may repeat) or one [count, ...] tensor, each [H, W, 4] (RGBA / BGRA) or [H * 3 / 2, W]
         (NV12, CbCr rows from row H) with contiguous rows and one pitch for all; at: (x, y) of each frame's top-left
         corner in its image (None: (0, 0)).  Raises ValueError for a rectangle that leaves its image or whose rows do
-        not start at multiples of 16 bytes (the device refuses the rest)."""
+        not start at multiples of 16 bytes (the device refuses the rest).  matrix / full_range: the encoding of an NV12
+        picture (_export_desc)."""
         import torch
         s = np.ascontiguousarray(np.asarray(streams, dtype=np.int64).reshape(-1), dtype=np.int32)
         count = int(s.shape[0])
@@ -595,19 +600,23 @@ class _FrameExport:
                                  + (" on an even row" if nv12 else ""))
             dst.append(d)
             uv.append(u)
-        desc = _export_desc(fmt, False, (0, 0, 0))
+        desc = _export_desc(fmt, False, (0, 0, 0), matrix, full_range)
         desc.pitch = pitch or 0
         arr = (C.c_void_p * max(count, 1))(*dst)
         return s, desc, arr, (C.c_void_p * max(count, 1))(*uv) if nv12 else None
 
 
-def _export_desc(fmt, over, background):
-    """the Export descriptor of a format name, the composite flag and an RGB(A) background (pitch and uv_offset 0)"""
+def _export_desc(fmt, over, background, matrix="bt709", full_range=False):
+    """the Export descriptor of a format name, the composite flag, an RGB(A) background (pitch and uv_offset 0) and the
+    Y'CbCr encoding: matrix "bt709" or "bt601", full_range (DESIGN 4.15; the defaults set no flag, and a matrix or range
+    on RGBA / BGRA reaches the library's refusal)"""
     if fmt not in EXPORT_FORMATS:
         raise ValueError(f"format {fmt!r}: one of {sorted(EXPORT_FORMATS)}")
+    if matrix not in EXPORT_MATRICES:
+        raise ValueError(f"matrix {matrix!r}: one of {sorted(EXPORT_MATRICES)}")
     desc = Export()
     desc.format = EXPORT_FORMATS[fmt]
-    desc.flags = EXPORT_OVER if over else 0
+    desc.flags = (EXPORT_OVER if over else 0) | EXPORT_MATRICES[matrix] | (EXPORT_FULL_RANGE if full_range else 0)
     bg = [int(v) for v in background]
     assert len(bg) in (3, 4), background
     desc.background = (C.c_uint8 * 4)(*bg[:3], 0)
@@ -885,7 +894,8 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
     def framebuffer_device(self):
         return self._L.glava_b200_framebuffer_device(self._h)
 
-    def export_frames(self, streams, fmt="rgba", over=False, background=(0, 0, 0), out=None, after=None, done=None):
+    def export_frames(self, streams, fmt="rgba", over=False, background=(0, 0, 0), out=None, after=None, done=None,
+                      matrix="bt709", full_range=False):
         """The current frames of `streams` (repeats allowed) top-down in the caller's device memory (glava_b200_export_frames):
         fmt "rgba" / "bgra" ([h, w, 4] per frame; over=True composites over `background` as GLava's window shows it) or
         "nv12" ([h * 3 / 2, w]: Y rows, then interleaved CbCr rows), "p010" (the same as uint16 samples, 10-bit code << 6),
@@ -894,8 +904,11 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
         shapes (rows padded to a multiple of 16 bytes, 32 for I420).  Returns out.
         after / done: torch.cuda.Event or cudaEvent_t handles — the export waits for `after` on the device and records
         `done` behind itself.  Left None, the export is ordered after the work already queued on torch's current stream,
-        and that stream waits for the export (the tensors can be used right away)."""
-        s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, lambda stream: self.device)
+        and that stream waits for the export (the tensors can be used right away).
+        matrix ("bt709" / "bt601") and full_range: the Y'CbCr encoding of NV12, I420, YUV444 and P010 (DESIGN 4.15; the
+        default is BT.709 limited range; matrix="bt601", full_range=True is JPEG's)."""
+        s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, lambda stream: self.device, None, matrix,
+                                                 full_range)
         self._ordered(lambda a, d: self._L.glava_b200_export_frames(self._h, s.ctypes.data, s.shape[0], dst, C.byref(desc), a, d),
                       after, done)
         return result
@@ -914,11 +927,13 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
             cur.wait_stream(own)
 
     def export_scaled(self, streams, size, crop=None, fmt="rgba", over=False, background=(0, 0, 0), out=None, after=None,
-                      done=None):
+                      done=None, matrix="bt709", full_range=False):
         """export_frames of a source rectangle shrunk to size = (w, h) by the exact area average (glava_b200_export_scaled):
         crop = (x, y, w, h) in top-down coordinates (y = 0 is the top row), None: the whole frame.  Downscale only; NV12,
-        I420 and P010 need an even w and h.  Shapes, out, after and done as export_frames, with the output size in place of the frame's."""
-        s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, lambda stream: self.device, size)
+        I420 and P010 need an even w and h.  Shapes, out, after, done, matrix and full_range as export_frames, with the output
+        size in place of the frame's."""
+        s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, lambda stream: self.device, size, matrix,
+                                                 full_range)
         sc = _export_scale(size, crop)
         self._ordered(lambda a, d: self._L.glava_b200_export_scaled(self._h, s.ctypes.data, s.shape[0], dst, None, C.byref(desc),
                                                                     C.byref(sc), a, d), after, done)
@@ -927,7 +942,7 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
     def export_ladder(self, streams, rungs, out=None, after=None, done=None):
         """Several sizes of each frame in one launch that reads each source row about once (glava_b200_export_ladder), for
         an encoder ladder: rungs = [dict(size=(w, h) or None for the frame's, crop=None, fmt="nv12", over=False,
-        background=(0, 0, 0)), ...], at most LADDER_MAX.  Rung j is exactly export_scaled(streams, **rungs[j]) at this
+        background=(0, 0, 0), matrix="bt709", full_range=False), ...], at most LADDER_MAX; rungs may mix encodings.  Rung j is exactly export_scaled(streams, **rungs[j]) at this
         point in call order.  out: None or one entry per rung in any form export_scaled takes.  Returns one result per rung,
         shaped as export_scaled returns it; after / done and the ordering against torch's current stream as export_frames."""
         s, arr, n, dst, results = self._ladder_plan(streams, rungs, out, lambda stream: self.device)
@@ -935,17 +950,18 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
                       after, done)
         return results
 
-    def overlay_frames(self, streams, images, at=None, fmt="nv12", after=None, done=None):
+    def overlay_frames(self, streams, images, at=None, fmt="nv12", after=None, done=None, matrix="bt709", full_range=False):
         """The current frames of `streams` composited in place onto the caller's images (glava_b200_overlay_frames): under
         native opacity premultiplied "over" the image's pixels, blended in Y'CbCr for NV12; under any other opacity the
         opaque bytes export_frames writes.  images and at: see _overlay_plan; rectangles of one call must not overlap.
-        after / done and the ordering against torch's current stream as export_frames.  Returns images."""
-        s, desc, dst, uv = self._overlay_plan(streams, images, at, fmt)
+        after / done and the ordering against torch's current stream as export_frames.  matrix / full_range: the encoding
+        of NV12 pictures, which the blend works in (DESIGN 4.15).  Returns images."""
+        s, desc, dst, uv = self._overlay_plan(streams, images, at, fmt, matrix, full_range)
         self._ordered(lambda a, d: self._L.glava_b200_overlay_frames(self._h, s.ctypes.data, s.shape[0], dst, uv, C.byref(desc),
                                                                      a, d), after, done)
         return images
 
-    def export_mosaic(self, streams, cols, tile, fmt="nv12", background=(0, 0, 0), out=None):
+    def export_mosaic(self, streams, cols, tile, fmt="nv12", background=(0, 0, 0), out=None, matrix="bt709", full_range=False):
         """The frames of `streams` shrunk to tile = (w, h) and laid out row-major, `cols` tiles per row, in one picture, by
         one export_scaled call with a destination and a chroma destination per tile.  W = cols * w, H = rows * h; returns
         [H * 3 / 2, W] for NV12 (uint8) and P010 (uint16), Y rows then CbCr rows, the plane views (Y, Cb, Cr) for I420 and
@@ -953,14 +969,14 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
         is a multiple of 16 (NV12, YUV444), 32 (I420), 8 (P010) or 4 (RGBA / BGRA).  out: a CUDA tensor [rows, pitch] whose
         rows hold the picture's row bytes, rows as _export_layout gives them for W x H (I420 / YUV444: the chroma planes
         back to back from row H); tiles past the last stream keep its bytes (out None: black).  Ordered against torch's
-        current stream as export_frames without events."""
+        current stream as export_frames without events.  matrix / full_range as export_frames (black: Y 0 in full range)."""
         import torch
         s = np.ascontiguousarray(np.asarray(streams, dtype=np.int64).reshape(-1), dtype=np.int32)
         count, cols = int(s.shape[0]), int(cols)
         tw, th = (int(v) for v in tile)
         if count < 1 or cols < 1:
             raise ValueError("export_mosaic: at least one stream and one column")
-        desc = _export_desc(fmt, False, background)
+        desc = _export_desc(fmt, False, background, matrix, full_range)
         W, H = cols * tw, (count + cols - 1) // cols * th
         rows, row_bytes, align = _export_layout(fmt, W, H)
         px = {"rgba": 4, "bgra": 4, "p010": 2}.get(fmt, 1)
@@ -968,12 +984,12 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
             base = torch.empty((rows, (row_bytes + align - 1) // align * align), dtype=torch.uint8, device=f"cuda:{self.device}")
             if count % cols:                                  # black where no stream lands
                 if fmt == "p010":
-                    base.view(torch.uint16)[:H].fill_(64 << 6)
+                    base.view(torch.uint16)[:H].fill_(0 if full_range else 64 << 6)
                     base.view(torch.uint16)[H:].fill_(512 << 6)
                 elif fmt in ("rgba", "bgra"):
                     base.fill_(0)
                 else:
-                    base[:H].fill_(16)
+                    base[:H].fill_(0 if full_range else 16)
                     base[H:].fill_(128)
             result = _export_views(fmt, base, W, H)
         else:
@@ -1101,25 +1117,26 @@ class ShardedRenderer(_StreamState, _StreamStyles, _FrameExport):
         _check(self._L.glava_b200_sharded_textures(self._h, l.ctypes.data, r.ctypes.data))
         return l, r
 
-    def export_frames(self, streams, fmt="rgba", over=False, background=(0, 0, 0), out=None):
+    def export_frames(self, streams, fmt="rgba", over=False, background=(0, 0, 0), out=None, matrix="bt709", full_range=False):
         """Renderer.export_frames with global stream indices (glava_b200_sharded_export_frames): each destination on the
         device of the shard that owns its stream (out None: one tensor when every listed stream lives on one device, else
         a list of per-frame tensors).  Work queued on torch's current streams of those devices is waited for first; the
-        frames are complete after sync()."""
+        frames are complete after sync().  matrix / full_range as Renderer.export_frames."""
         import torch
         device_of = self._device_of()
-        s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, device_of)
+        s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, device_of, None, matrix, full_range)
         for d in sorted({device_of(int(x)) for x in s}):
             torch.cuda.current_stream(d).synchronize()
         _check(self._L.glava_b200_sharded_export_frames(self._h, s.ctypes.data, s.shape[0], dst, C.byref(desc)))
         return result
 
-    def export_scaled(self, streams, size, crop=None, fmt="rgba", over=False, background=(0, 0, 0), out=None):
+    def export_scaled(self, streams, size, crop=None, fmt="rgba", over=False, background=(0, 0, 0), out=None, matrix="bt709",
+                      full_range=False):
         """Renderer.export_scaled with global stream indices (glava_b200_sharded_export_scaled), destinations placed as
-        export_frames places them; the frames are complete after sync()."""
+        export_frames places them; the frames are complete after sync().  matrix / full_range as Renderer.export_frames."""
         import torch
         device_of = self._device_of()
-        s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, device_of, size)
+        s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, device_of, size, matrix, full_range)
         sc = _export_scale(size, crop)
         for d in sorted({device_of(int(x)) for x in s}):
             torch.cuda.current_stream(d).synchronize()
@@ -1137,13 +1154,13 @@ class ShardedRenderer(_StreamState, _StreamStyles, _FrameExport):
         _check(self._L.glava_b200_sharded_export_ladder(self._h, s.ctypes.data, s.shape[0], arr, n, dst, None))
         return results
 
-    def overlay_frames(self, streams, images, at=None, fmt="nv12"):
+    def overlay_frames(self, streams, images, at=None, fmt="nv12", matrix="bt709", full_range=False):
         """Renderer.overlay_frames with global stream indices (glava_b200_sharded_overlay_frames), each image on the device
         of the shard that owns its stream.  Work queued on torch's current streams of those devices is waited for first;
-        the images are complete after sync()."""
+        the images are complete after sync().  matrix / full_range as Renderer.overlay_frames."""
         import torch
         device_of = self._device_of()
-        s, desc, dst, uv = self._overlay_plan(streams, images, at, fmt)
+        s, desc, dst, uv = self._overlay_plan(streams, images, at, fmt, matrix, full_range)
         for d in sorted({device_of(int(x)) for x in s if 0 <= int(x) < self.batch}):
             torch.cuda.current_stream(d).synchronize()
         _check(self._L.glava_b200_sharded_overlay_frames(self._h, s.ctypes.data, s.shape[0], dst, uv, C.byref(desc)))

@@ -63,8 +63,15 @@ int desc_check(ExportKind kind, int w, int h, const glava_b200_export& d, const 
     if (!format_name(d.format)) return fail(GLAVA_B200_EINVAL, "%s: unknown format %d", who, d.format);
     if (kind == ExportKind::overlay && d.format != GLAVA_B200_EXPORT_NV12 && export_yuv(d.format))
         return fail(GLAVA_B200_EINVAL, "%s: format %s: the overlay takes RGBA, BGRA or NV12", who, format_name(d.format));
-    if (d.flags & ~GLAVA_B200_EXPORT_OVER) return fail(GLAVA_B200_EINVAL, "%s: unknown flags 0x%x", who, d.flags);
-    if (kind == ExportKind::overlay && d.flags) return fail(GLAVA_B200_EINVAL, "%s: flags 0x%x: the overlay takes none", who, d.flags);
+    // the colour bits (DESIGN 4.15) are flags of the Y'CbCr formats only
+    const uint32_t colour = GLAVA_B200_EXPORT_FULL_RANGE | GLAVA_B200_EXPORT_BT601;
+    if (d.flags & ~(GLAVA_B200_EXPORT_OVER | colour)) return fail(GLAVA_B200_EINVAL, "%s: unknown flags 0x%x", who, d.flags);
+    if ((d.flags & colour) && !export_yuv(d.format))
+        return fail(GLAVA_B200_EINVAL, "%s: flags 0x%x: %s has no matrix or range (EXPORT_FULL_RANGE and EXPORT_BT601 are for the "
+                    "Y'CbCr formats)", who, d.flags, format_name(d.format));
+    if (kind == ExportKind::overlay && (d.flags & ~colour))
+        return fail(GLAVA_B200_EINVAL, "%s: flags 0x%x: the overlay takes none%s", who, d.flags,
+                    export_yuv(d.format) ? " but EXPORT_FULL_RANGE and EXPORT_BT601" : "");
     *q = { 0, 0, w, h, w, h };
     if (kind != ExportKind::scaled) return desc_size(w, h, d, "frame", who);
     if (!s) return fail(GLAVA_B200_EINVAL, "%s: null scale", who);
@@ -262,6 +269,7 @@ int export_run(ExportKind kind, glava_b200* r, const int* streams, int count, vo
             a.bg = background(*desc);
             a.uv_offset = pl.cb;
             a.cr_offset = pl.cr;
+            a.enc = export_enc(desc->flags);
             return launch_export(a, v.stream);
         }
         if (kind == ExportKind::scaled) {
@@ -273,11 +281,13 @@ int export_run(ExportKind kind, glava_b200* r, const int* streams, int count, vo
             const ExportRecip rcp = export_recip((uint64_t) q.src_w * (uint64_t) q.src_h);
             a.div_mul = rcp.mul; a.div_shift = rcp.shift;
             a.cr_offset = pl.cr;
+            a.enc = export_enc(desc->flags);
             return launch_export_scaled(a, v.stream);
         }
         OverlayArgs a = {};
         common_args(a, v, d_list, count, *desc);
         a.band = a.native && a.marks && a.mark_rows > 0 ? 1 : 0;   // band items wherever marks exist (DESIGN 4.12)
+        a.enc = export_enc(desc->flags);
         return launch_overlay(a, v.stream);
     });
 }

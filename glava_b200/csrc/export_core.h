@@ -1,5 +1,5 @@
 // export_core.h — the pixel arithmetic of glava_b200_export_frames (DESIGN 4.10) as __host__ __device__ functions: the
-// composite over an opaque background, RGB -> BT.709 limited-range Y / Cb / Cr in integer fixed point, the 2x2 chroma
+// composite over an opaque background, RGB -> Y / Cb / Cr in integer fixed point (BT.709 or BT.601, limited or full range), the 2x2 chroma
 // average, and which framebuffer rows the dirty-row marks say must be read.  export_kernels.cu and the host test tier
 // (tests/test_export_core.py) compile this same code.
 #ifndef GLAVA_B200_EXPORT_CORE_H
@@ -56,16 +56,64 @@ GLB_HD uint32_t export_px(const ExportFmt& f, uint32_t px) {
 #define GLB_CR_G (-26145)
 #define GLB_CR_B (-2639)
 #define GLB_CR_R (-(GLB_CR_G + GLB_CR_B))
+
+// ---- colour encodings (DESIGN 4.15) --------------------------------------------------------------------------------------
+// The Y'CbCr formats write one of four encodings, chosen by the descriptor's GLAVA_B200_EXPORT_FULL_RANGE (0x100) and
+// GLAVA_B200_EXPORT_BT601 (0x200) bits: E = flags >> 8 & 3, 0 BT.709 limited range (flags 0, the literals above and
+// below), 1 BT.709 full range, 2 BT.601 limited, 3 BT.601 full.  Every set is built by yuv_coef from (Kr, Kb, range, bits):
+// limited range Y = 16 + 219/255 Y', C = 128 + 224/255 P (10 bits: 64 + 876/255 Y', 512 + 896/255 P); full range (H.273,
+// JFIF) Y = Y', C = 128 + P (10 bits: 1023/255 Y', 512 + 1023/255 P), P = (B - Y') / (2 (1 - Kb)) for Cb, (R - Y') /
+// (2 (1 - Kr)) for Cr.  Coefficients scaled by 2^16 and rounded half away from zero; the blue coefficient of Cb and the red
+// one of Cr are minus the sum of the other two, so every grey has Cb = Cr = 128 (512) exactly.  Full range reaches 255.5
+// (1023.5) before rounding in blue's Cb and red's Cr, so its codes are clamped to 255 (1023); limited range never leaves
+// [16, 240] ([64, 960]) and is not.  Accumulators, 8 bits: |coefficient sums| <= 2^16 (full), so a code's sum is within
+// 255 * 2^16 + (128 << 16) + 2^15 < 2^25; 10 bits, per pixel <= 262915 * 255 + (512 << 16) + 2^15 < 2^27, P010 chroma over
+// block sums (<= 1020, shift 18) <= 131458 * 1020 + (512 << 18) + 2^17 < 2^29; every minimum is >= 0 (DESIGN 4.15).
+struct YuvCoef { int yr, yg, yb, cbr, cbg, cbb, crr, crg, crb, yoff, coff, top; bool full; };
+constexpr int yuv_round(double x) { return x < 0 ? -(int) (-x + 0.5) : (int) (x + 0.5); }
+constexpr YuvCoef yuv_coef(double kr, double kb, bool full, int bits) {
+    const double kg = 1 - kr - kb, s = 1 << GLB_YUV_SHIFT;
+    const double top = bits == 10 ? 1023 : 255;
+    const double ys = full ? top / 255 : (bits == 10 ? 876.0 : 219.0) / 255;
+    const double cs = full ? top / 255 : (bits == 10 ? 896.0 : 224.0) / 255;
+    const int cbr = yuv_round(-kr / (2 * (1 - kb)) * cs * s), cbg = yuv_round(-kg / (2 * (1 - kb)) * cs * s);
+    const int crg = yuv_round(-kg / (2 * (1 - kr)) * cs * s), crb = yuv_round(-kb / (2 * (1 - kr)) * cs * s);
+    return { yuv_round(kr * ys * s), yuv_round(kg * ys * s), yuv_round(kb * ys * s), cbr, cbg, -(cbr + cbg), -(crg + crb), crg,
+             crb, full ? 0 : bits == 10 ? 64 : 16, bits == 10 ? 512 : 128, (int) top, full };
+}
+// the set of encoding E (0..3) at 8 or 10 bits: BT.709 Kr, Kb = 0.2126, 0.0722; BT.601 0.299, 0.114
+constexpr YuvCoef yuv_enc(int E, int bits) { return yuv_coef(E & 2 ? 0.299 : 0.2126, E & 2 ? 0.114 : 0.0722, (E & 1) != 0, bits); }
+constexpr bool yuv_same(const YuvCoef& a, int yr, int yg, int yb, int cbr, int cbg, int crg, int crb) {
+    return a.yr == yr && a.yg == yg && a.yb == yb && a.cbr == cbr && a.cbg == cbg && a.cbb == -(cbr + cbg) && a.crg == crg &&
+           a.crb == crb && a.crr == -(crg + crb);
+}
+static_assert(yuv_same(yuv_enc(0, 8), GLB_Y_R, GLB_Y_G, GLB_Y_B, GLB_CB_R, GLB_CB_G, GLB_CR_G, GLB_CR_B), "BT.709 limited 8-bit");
+// the encoding index of a descriptor's flags
+GLB_HD int export_enc(uint32_t flags) { return (int) ((flags >> 8) & 3u); }
+// a code of set S from its accumulator (scaled by 2^shift, rounding included): full range clamps to the top code
+template <int E, int Bits>
+GLB_HD uint32_t yuv_code(int acc, int shift) {
+    constexpr YuvCoef S = yuv_enc(E, Bits);
+    const int v = acc >> shift;
+    if constexpr (S.full) return (uint32_t) (v > S.top ? S.top : v);
+    return (uint32_t) v;
+}
+
+// the Y code of a composited pixel under encoding E (E = 0: the BT.709 limited byte above)
+template <int E = 0>
 GLB_HD uint32_t export_y(uint32_t c) {
+    constexpr YuvCoef S = yuv_enc(E, 8);
     const int r = (int) (c & 255u), g = (int) ((c >> 8) & 255u), b = (int) ((c >> 16) & 255u);
-    return (uint32_t) ((GLB_Y_R * r + GLB_Y_G * g + GLB_Y_B * b + (16 << GLB_YUV_SHIFT) + GLB_YUV_HALF) >> GLB_YUV_SHIFT);
+    return yuv_code<E, 8>(S.yr * r + S.yg * g + S.yb * b + (S.yoff << GLB_YUV_SHIFT) + GLB_YUV_HALF, GLB_YUV_SHIFT);
 }
 // (Cb, Cr) as the two bytes of NV12's interleaved plane: Cb low, Cr high
+template <int E = 0>
 GLB_HD uint32_t export_cbcr(uint32_t c) {
+    constexpr YuvCoef S = yuv_enc(E, 8);
     const int r = (int) (c & 255u), g = (int) ((c >> 8) & 255u), b = (int) ((c >> 16) & 255u);
-    const int cb = (GLB_CB_R * r + GLB_CB_G * g + GLB_CB_B * b + (128 << GLB_YUV_SHIFT) + GLB_YUV_HALF) >> GLB_YUV_SHIFT;
-    const int cr = (GLB_CR_R * r + GLB_CR_G * g + GLB_CR_B * b + (128 << GLB_YUV_SHIFT) + GLB_YUV_HALF) >> GLB_YUV_SHIFT;
-    return (uint32_t) cb | ((uint32_t) cr << 8);
+    const uint32_t cb = yuv_code<E, 8>(S.cbr * r + S.cbg * g + S.cbb * b + (S.coff << GLB_YUV_SHIFT) + GLB_YUV_HALF, GLB_YUV_SHIFT);
+    const uint32_t cr = yuv_code<E, 8>(S.crr * r + S.crg * g + S.crb * b + (S.coff << GLB_YUV_SHIFT) + GLB_YUV_HALF, GLB_YUV_SHIFT);
+    return cb | (cr << 8);
 }
 // The chroma sample of a 2x2 block: the per-channel average (s + 2) >> 2 of its four composited pixels
 GLB_HD uint32_t export_avg4(uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
@@ -79,6 +127,7 @@ GLB_HD uint32_t export_avg4(uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
 }
 // NV12 of a quad of output rows 2j (top) and 2j + 1 (bot): four Y bytes per row, and the (Cb, Cr) pairs of the quad's two
 // 2x2 blocks as one little-endian word (Cb0, Cr0, Cb1, Cr1)
+template <int E = 0>
 GLB_HD uint32_t export_nv12_quad(const ExportFmt& f, const uint32_t top[4], const uint32_t bot[4], uint32_t* y_top, uint32_t* y_bot) {
     uint32_t t[4], b[4];
     *y_top = 0u; *y_bot = 0u;
@@ -86,10 +135,10 @@ GLB_HD uint32_t export_nv12_quad(const ExportFmt& f, const uint32_t top[4], cons
     for (int k = 0; k < 4; ++k) {
         t[k] = export_over(top[k], f.bg, f.native);
         b[k] = export_over(bot[k], f.bg, f.native);
-        *y_top |= export_y(t[k]) << (8 * k);
-        *y_bot |= export_y(b[k]) << (8 * k);
+        *y_top |= export_y<E>(t[k]) << (8 * k);
+        *y_bot |= export_y<E>(b[k]) << (8 * k);
     }
-    return export_cbcr(export_avg4(t[0], t[1], b[0], b[1])) | (export_cbcr(export_avg4(t[2], t[3], b[2], b[3])) << 16);
+    return export_cbcr<E>(export_avg4(t[0], t[1], b[0], b[1])) | (export_cbcr<E>(export_avg4(t[2], t[3], b[2], b[3])) << 16);
 }
 
 // ---- I420, YUV 4:4:4 and P010 (DESIGN 4.14) ------------------------------------------------------------------------------
@@ -122,12 +171,13 @@ GLB_HD uint32_t export_cb_pair(uint32_t uv) { return (uv & 0xffu) | ((uv >> 8) &
 GLB_HD uint32_t export_cr_pair(uint32_t uv) { return ((uv >> 8) & 0xffu) | ((uv >> 16) & 0xff00u); }
 
 // YUV 4:4:4 of one row's quad: Y, Cb and Cr of each composited pixel, four bytes each
+template <int E = 0>
 GLB_HD void export_444_quad(const ExportFmt& f, const uint32_t in[4], uint32_t* y, uint32_t* cb, uint32_t* cr) {
     *y = 0u; *cb = 0u; *cr = 0u;
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-        const uint32_t c = export_over(in[k], f.bg, f.native), uv = export_cbcr(c);
-        *y |= export_y(c) << (8 * k);
+        const uint32_t c = export_over(in[k], f.bg, f.native), uv = export_cbcr<E>(c);
+        *y |= export_y<E>(c) << (8 * k);
         *cb |= (uv & 255u) << (8 * k);
         *cr |= (uv >> 8) << (8 * k);
     }
@@ -146,10 +196,14 @@ GLB_HD void export_444_quad(const ExportFmt& f, const uint32_t in[4], uint32_t* 
 #define GLB_CR10_G (-104580)
 #define GLB_CR10_B (-10557)
 #define GLB_CR10_R (-(GLB_CR10_G + GLB_CR10_B))
+static_assert(yuv_same(yuv_enc(0, 10), GLB_Y10_R, GLB_Y10_G, GLB_Y10_B, GLB_CB10_R, GLB_CB10_G, GLB_CR10_G, GLB_CR10_B),
+              "BT.709 limited 10-bit");
 // the 10-bit Y code of a composited pixel
+template <int E = 0>
 GLB_HD uint32_t export_y10(uint32_t c) {
+    constexpr YuvCoef S = yuv_enc(E, 10);
     const int r = (int) (c & 255u), g = (int) ((c >> 8) & 255u), b = (int) ((c >> 16) & 255u);
-    return (uint32_t) ((GLB_Y10_R * r + GLB_Y10_G * g + GLB_Y10_B * b + (64 << GLB_YUV_SHIFT) + GLB_YUV_HALF) >> GLB_YUV_SHIFT);
+    return yuv_code<E, 10>(S.yr * r + S.yg * g + S.yb * b + (S.yoff << GLB_YUV_SHIFT) + GLB_YUV_HALF, GLB_YUV_SHIFT);
 }
 // The per-channel sums (0..1020) of a 2x2 block's four composited pixels, 10 bits each (R low).  P010 chroma takes these
 // exact sums, not NV12's (s + 2) >> 2 byte: the two bits that average rounds away are what 10 bits carry.
@@ -162,14 +216,17 @@ GLB_HD uint32_t export_sum4(uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
 }
 // the 10-bit (Cb, Cr) codes of block sums s (export_sum4), Cb in the low 16 bits: the 16-bit coefficients over sums four
 // times the average, so shift 18; every accumulator stays in [0, 2^31)
+template <int E = 0>
 GLB_HD uint32_t export_cbcr10(uint32_t s) {
+    constexpr YuvCoef S = yuv_enc(E, 10);
     const int r = (int) (s & 1023u), g = (int) ((s >> 10) & 1023u), b = (int) (s >> 20);
-    const int cb = (GLB_CB10_R * r + GLB_CB10_G * g + GLB_CB10_B * b + (512 << 18) + (1 << 17)) >> 18;
-    const int cr = (GLB_CR10_R * r + GLB_CR10_G * g + GLB_CR10_B * b + (512 << 18) + (1 << 17)) >> 18;
-    return (uint32_t) cb | ((uint32_t) cr << 16);
+    const uint32_t cb = yuv_code<E, 10>(S.cbr * r + S.cbg * g + S.cbb * b + (S.coff << 18) + (1 << 17), 18);
+    const uint32_t cr = yuv_code<E, 10>(S.crr * r + S.crg * g + S.crb * b + (S.coff << 18) + (1 << 17), 18);
+    return cb | (cr << 16);
 }
 // P010 of a quad of output rows 2j (top) and 2j + 1 (bot): per row its four Y samples as two words (little-endian uint16,
 // code << 6), and the (Cb, Cr) sample pairs of the quad's two 2x2 blocks, one word each
+template <int E = 0>
 GLB_HD void export_p010_quad(const ExportFmt& f, const uint32_t top[4], const uint32_t bot[4], uint32_t yt[2], uint32_t yb[2],
                              uint32_t uv[2]) {
     uint32_t t[4], b[4];
@@ -180,27 +237,28 @@ GLB_HD void export_p010_quad(const ExportFmt& f, const uint32_t top[4], const ui
     }
 #pragma unroll
     for (int k = 0; k < 2; ++k) {
-        yt[k] = (export_y10(t[2 * k]) << 6) | (export_y10(t[2 * k + 1]) << 22);
-        yb[k] = (export_y10(b[2 * k]) << 6) | (export_y10(b[2 * k + 1]) << 22);
-        uv[k] = export_cbcr10(export_sum4(t[2 * k], t[2 * k + 1], b[2 * k], b[2 * k + 1])) << 6;
+        yt[k] = (export_y10<E>(t[2 * k]) << 6) | (export_y10<E>(t[2 * k + 1]) << 22);
+        yb[k] = (export_y10<E>(b[2 * k]) << 6) | (export_y10<E>(b[2 * k + 1]) << 22);
+        uv[k] = export_cbcr10<E>(export_sum4(t[2 * k], t[2 * k + 1], b[2 * k], b[2 * k + 1])) << 6;
     }
 }
 
 // What zero pixels become in a new format's quad, for the kernels' all-zero shortcut: y, the luma word of a row (P010: one
 // of its two equal words); u and v, I420's Cb and Cr pairs, YUV 4:4:4's Cb and Cr words, P010's CbCr word (v unused)
 struct ExportZero { uint32_t y, u, v; };
+template <int E = 0>
 GLB_HD ExportZero export_zero(const ExportFmt& f) {
     const uint32_t z[4] = { 0u, 0u, 0u, 0u };
     ExportZero o = { 0u, 0u, 0u };
     if (f.format == GLAVA_B200_EXPORT_YUV444) {
-        export_444_quad(f, z, &o.y, &o.u, &o.v);
+        export_444_quad<E>(f, z, &o.y, &o.u, &o.v);
     } else if (f.format == GLAVA_B200_EXPORT_P010) {
         uint32_t yt[2], yb[2], uv[2];
-        export_p010_quad(f, z, z, yt, yb, uv);
+        export_p010_quad<E>(f, z, z, yt, yb, uv);
         o.y = yt[0]; o.u = uv[0];
     } else {
         uint32_t yb;
-        const uint32_t uv = export_nv12_quad(f, z, z, &o.y, &yb);
+        const uint32_t uv = export_nv12_quad<E>(f, z, z, &o.y, &yb);
         o.u = export_cb_pair(uv); o.v = export_cr_pair(uv);
     }
     return o;
@@ -333,19 +391,24 @@ GLB_HD uint32_t overlay_frac(uint32_t off, uint32_t a, uint32_t vd) {
     return (((off * a + (255u - a) * vd) << GLB_YUV_SHIFT) + 127u) / 255u;
 }
 GLB_HD uint32_t overlay_clamp(int v) { return v < 0 ? 0u : v > 255 ? 255u : (uint32_t) v; }
-// the Y byte of pixel px (stored, premultiplied) over a Y byte yd
+// the Y byte of pixel px (stored, premultiplied) over a Y byte yd, the destination in encoding E (DESIGN 4.15: the offset
+// is 16 in limited range, 0 in full range; every set keeps "a zero pixel leaves yd" and "an opaque pixel gives export_y")
+template <int E = 0>
 GLB_HD uint32_t overlay_y(uint32_t px, uint32_t yd) {
+    constexpr YuvCoef S = yuv_enc(E, 8);
     const int r = (int) (px & 255u), g = (int) ((px >> 8) & 255u), b = (int) ((px >> 16) & 255u);
-    const int t = (int) overlay_frac(16u, px >> 24, yd);
-    return overlay_clamp((GLB_Y_R * r + GLB_Y_G * g + GLB_Y_B * b + t + GLB_YUV_HALF) >> GLB_YUV_SHIFT);
+    const int t = (int) overlay_frac((uint32_t) S.yoff, px >> 24, yd);
+    return overlay_clamp((S.yr * r + S.yg * g + S.yb * b + t + GLB_YUV_HALF) >> GLB_YUV_SHIFT);
 }
 // the (Cb, Cr) pair of a block average m (overlay_avg4: alpha included) over the pair uvd (Cb low byte, Cr high)
+template <int E = 0>
 GLB_HD uint32_t overlay_cbcr(uint32_t m, uint32_t uvd) {
+    constexpr YuvCoef S = yuv_enc(E, 8);
     const int r = (int) (m & 255u), g = (int) ((m >> 8) & 255u), b = (int) ((m >> 16) & 255u);
     const uint32_t a = m >> 24;
-    const int tb = (int) overlay_frac(128u, a, uvd & 255u), tr = (int) overlay_frac(128u, a, (uvd >> 8) & 255u);
-    const int cb = (GLB_CB_R * r + GLB_CB_G * g + GLB_CB_B * b + tb + GLB_YUV_HALF) >> GLB_YUV_SHIFT;
-    const int cr = (GLB_CR_R * r + GLB_CR_G * g + GLB_CR_B * b + tr + GLB_YUV_HALF) >> GLB_YUV_SHIFT;
+    const int tb = (int) overlay_frac((uint32_t) S.coff, a, uvd & 255u), tr = (int) overlay_frac((uint32_t) S.coff, a, (uvd >> 8) & 255u);
+    const int cb = (S.cbr * r + S.cbg * g + S.cbb * b + tb + GLB_YUV_HALF) >> GLB_YUV_SHIFT;
+    const int cr = (S.crr * r + S.crg * g + S.crb * b + tr + GLB_YUV_HALF) >> GLB_YUV_SHIFT;
     return overlay_clamp(cb) | (overlay_clamp(cr) << 8);
 }
 // export_avg4 in all four channels: the chroma block of the overlay averages the stored pixels, alpha included
@@ -360,16 +423,17 @@ GLB_HD uint32_t overlay_avg4(uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
 }
 // NV12 of a quad (rows 2j and 2j + 1, four pixels each) over the destination's Y words yt / yb and CbCr word uv (two pairs):
 // updates them in place
+template <int E = 0>
 GLB_HD void overlay_nv12_quad(const uint32_t top[4], const uint32_t bot[4], uint32_t* yt, uint32_t* yb, uint32_t* uv) {
     uint32_t t = 0u, b = 0u;
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-        t |= overlay_y(top[k], (*yt >> (8 * k)) & 255u) << (8 * k);
-        b |= overlay_y(bot[k], (*yb >> (8 * k)) & 255u) << (8 * k);
+        t |= overlay_y<E>(top[k], (*yt >> (8 * k)) & 255u) << (8 * k);
+        b |= overlay_y<E>(bot[k], (*yb >> (8 * k)) & 255u) << (8 * k);
     }
     *yt = t; *yb = b;
-    *uv = overlay_cbcr(overlay_avg4(top[0], top[1], bot[0], bot[1]), *uv & 0xffffu) |
-          (overlay_cbcr(overlay_avg4(top[2], top[3], bot[2], bot[3]), *uv >> 16) << 16);
+    *uv = overlay_cbcr<E>(overlay_avg4(top[0], top[1], bot[0], bot[1]), *uv & 0xffffu) |
+          (overlay_cbcr<E>(overlay_avg4(top[2], top[3], bot[2], bot[3]), *uv >> 16) << 16);
 }
 // NV12 under dirty-row marks, one warp per band [b0, b1) of a strip: the output row pairs it visits are [*ja, *jb) (pair j =
 // framebuffer rows h - 1 - 2j and h - 2 - 2j), those that hold a row of [lo, hi), the rows the band's word lets through

@@ -20,7 +20,20 @@
 
 #include <cuda_runtime.h>
 
+#include <type_traits>
+
 namespace glb {
+
+static_assert(sizeof(LadderRung) == 80, "LadderRung keeps its size: enc sits in what was padding");
+
+// f(std::integral_constant<int, E>()) for the encoding E = enc, 1..3 (DESIGN 4.15): the launchers run these instantiations
+// for any encoding but 0, whose kernels are the ones every call without a colour bit ran before there were encodings
+template <typename F>
+static void for_enc(int enc, F&& f) {
+    if (enc == 1) f(std::integral_constant<int, 1>());
+    else if (enc == 2) f(std::integral_constant<int, 2>());
+    else f(std::integral_constant<int, 3>());
+}
 
 // whether row y of the strip must be read (false: it is all zero in memory)
 template <typename A>
@@ -81,9 +94,9 @@ __device__ __forceinline__ void store_rgba(const ExportFmt& f, uint8_t* row, int
 
 // One item of export_kernel (and of a ladder's whole-frame rung): output rows 2j and 2j + 1 (framebuffer rows h - 1 - 2j and
 // h - 2 - 2j) of the quad at x of `strip`; the NV12 CbCr plane's row 0 is dst + uv_offset; zy / zuv / zpx: what zero pixels
-// become.
+// become.  E: the encoding of NV12 (DESIGN 4.15).
 // A reads w, h, marks, mark_rows, format and pitch.
-template <bool Keep, typename A>
+template <bool Keep, int E = 0, typename A>
 __device__ __forceinline__ void export_item(const A& a, const ExportFmt& f, const uint32_t* frame, int slot, uint8_t* dst,
                                             size_t uv_offset, int j, int strip, int x, uint32_t zy, uint32_t zuv, uint32_t zpx) {
     const int y0 = a.h - 1 - 2 * j, y1 = y0 - 1;
@@ -93,7 +106,7 @@ __device__ __forceinline__ void export_item(const A& a, const ExportFmt& f, cons
     uint8_t* const r0 = dst + (size_t) (2 * j) * a.pitch;
     if (a.format == GLAVA_B200_EXPORT_NV12) {               // h even: both rows exist
         uint32_t yt = zy, yb = zy, c = zuv;
-        if ((top[0] | top[1] | top[2] | top[3] | bot[0] | bot[1] | bot[2] | bot[3]) != 0u) c = export_nv12_quad(f, top, bot, &yt, &yb);
+        if ((top[0] | top[1] | top[2] | top[3] | bot[0] | bot[1] | bot[2] | bot[3]) != 0u) c = export_nv12_quad<E>(f, top, bot, &yt, &yb);
         uint8_t* const pu = dst + uv_offset + (size_t) j * a.pitch + x;
         if (x + 4 <= a.w) {
             __stcs(reinterpret_cast<uint32_t*>(r0 + x), yt);
@@ -157,6 +170,30 @@ __global__ void __launch_bounds__(256) export_kernel(const __grid_constant__ Exp
     }
 }
 
+// export_kernel's NV12 under encoding E = 1..3 (DESIGN 4.15): the same items, run by export_item
+template <typename Index, int E>
+__global__ void __launch_bounds__(256) export_nv12_enc_kernel(const __grid_constant__ ExportArgs a) {
+    const ExportFmt f = { GLAVA_B200_EXPORT_NV12, 1, a.native, a.bg };
+    const Index strips = (Index) ((a.w + 127) >> 7), per = strips * (Index) ((a.h + 1) >> 1);
+    const Index items = (Index) a.count * per;
+    const Index warps = (Index) (((size_t) gridDim.x * blockDim.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    const uint32_t zero4[4] = { 0u, 0u, 0u, 0u };
+    uint32_t zy, zy1;
+    const uint32_t zuv = export_nv12_quad<E>(f, zero4, zero4, &zy, &zy1);
+    for (Index it = (Index) (((size_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5); it < items; it += warps) {
+        const Index k = it / per, rem = it - k * per;
+        const int j = (int) (rem / strips), strip = (int) (rem - (Index) j * strips);
+        const int x = strip * 128 + lane * 4;
+        if (x >= a.w) continue;
+        const ExportEntry* e = a.list + k;
+        uint8_t* const dst = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst)));
+        const int slot = __ldg(&e->slot);
+        const uint32_t* frame = reinterpret_cast<const uint32_t*>(a.fb) + (size_t) slot * a.h * a.w;
+        export_item<false, E>(a, f, frame, slot, dst, a.uv_offset, j, strip, x, zy, zuv, 0u);
+    }
+}
+
 // ---- I420, YUV 4:4:4 and P010 (DESIGN 4.14) --------------------------------------------------------------------------------
 // export_kernel's items (output row pair x 128-pixel strip, a quad per lane) with the new formats' stores, in kernels of their
 // own so that export_kernel keeps its machine code.  I420: two 4-byte Y stores and a 2-byte Cb and a 2-byte Cr store
@@ -172,10 +209,11 @@ __device__ __forceinline__ void store_bytes(uint8_t* p, uint32_t v, int n) {
 }
 
 // YUV 4:4:4 of one row's quad: n pixels of Y at py, Cb at pu and Cr cr bytes past it
+template <int E>
 __device__ __forceinline__ void store_444(const ExportFmt& f, const uint32_t q[4], uint8_t* py, uint8_t* pu, size_t cr, int n,
                                           const ExportZero& z) {
     uint32_t y = z.y, u = z.u, v = z.v;
-    if ((q[0] | q[1] | q[2] | q[3]) != 0u) export_444_quad(f, q, &y, &u, &v);
+    if ((q[0] | q[1] | q[2] | q[3]) != 0u) export_444_quad<E>(f, q, &y, &u, &v);
     store_bytes(py, y, n);
     store_bytes(pu, u, n);
     store_bytes(pu + cr, v, n);
@@ -183,8 +221,8 @@ __device__ __forceinline__ void store_444(const ExportFmt& f, const uint32_t q[4
 
 // One item of export_yuv_kernel (and of a ladder's whole-frame I420 / YUV444 / P010 rung): as export_item, with the chroma
 // plane at `cb` (I420 / YUV444: Cb, Cr `cr` bytes further; P010: CbCr) and z what zero pixels become.  fmt: a constant in
-// the standalone kernels, the rung's format in the ladder.  A reads w, h, marks, mark_rows and pitch.
-template <bool Keep, typename A>
+// the standalone kernels, the rung's format in the ladder; E the encoding.  A reads w, h, marks, mark_rows and pitch.
+template <bool Keep, int E = 0, typename A>
 __device__ __forceinline__ void yuv_item(const A& a, const ExportFmt& f, int fmt, const uint32_t* frame, int slot, uint8_t* dst,
                                          uint8_t* cb, size_t cr, int j, int strip, int x, const ExportZero& z) {
     const int y0 = a.h - 1 - 2 * j, y1 = y0 - 1;
@@ -196,15 +234,15 @@ __device__ __forceinline__ void yuv_item(const A& a, const ExportFmt& f, int fmt
     if (fmt == GLAVA_B200_EXPORT_YUV444) {                  // any w and h
         const int n = full ? 4 : a.w - x;
         const size_t o = (size_t) (2 * j) * a.pitch + x;
-        store_444(f, top, dst + o, cb + o, cr, n, z);
-        if (y1 >= 0) store_444(f, bot, dst + o + a.pitch, cb + o + a.pitch, cr, n, z);
+        store_444<E>(f, top, dst + o, cb + o, cr, n, z);
+        if (y1 >= 0) store_444<E>(f, bot, dst + o + a.pitch, cb + o + a.pitch, cr, n, z);
         return;
     }
     const bool any = (top[0] | top[1] | top[2] | top[3] | bot[0] | bot[1] | bot[2] | bot[3]) != 0u;
     if (fmt == GLAVA_B200_EXPORT_I420) {                    // w and h even
         uint32_t yt = z.y, yb = z.y, u = z.u, v = z.v;
         if (any) {
-            const uint32_t uv = export_nv12_quad(f, top, bot, &yt, &yb);
+            const uint32_t uv = export_nv12_quad<E>(f, top, bot, &yt, &yb);
             u = export_cb_pair(uv); v = export_cr_pair(uv);
         }
         uint8_t* const pu = cb + (size_t) j * (a.pitch >> 1) + (x >> 1);
@@ -222,7 +260,7 @@ __device__ __forceinline__ void yuv_item(const A& a, const ExportFmt& f, int fmt
         return;
     }
     uint32_t yt[2] = { z.y, z.y }, yb[2] = { z.y, z.y }, uv[2] = { z.u, z.u };   // P010, w and h even
-    if (any) export_p010_quad(f, top, bot, yt, yb, uv);
+    if (any) export_p010_quad<E>(f, top, bot, yt, yb, uv);
     uint8_t* const pu = cb + (size_t) j * a.pitch + 2 * x;
     if (full) {
         __stcs(reinterpret_cast<uint2*>(r0 + 2 * x), make_uint2(yt[0], yt[1]));
@@ -235,14 +273,14 @@ __device__ __forceinline__ void yuv_item(const A& a, const ExportFmt& f, int fmt
     }
 }
 
-template <typename Index, int Fmt>
-__global__ void __launch_bounds__(256) export_yuv_kernel(const __grid_constant__ ExportArgs a) {
+template <typename Index, int Fmt, int E>
+__device__ __forceinline__ void yuv_loop(const ExportArgs& a) {
     const ExportFmt f = { Fmt, 1, a.native, a.bg };
     const Index strips = (Index) ((a.w + 127) >> 7), per = strips * (Index) ((a.h + 1) >> 1);
     const Index items = (Index) a.count * per;
     const Index warps = (Index) (((size_t) gridDim.x * blockDim.x) >> 5);
     const int lane = threadIdx.x & 31;
-    const ExportZero z = export_zero(f);                    // once per thread, as export_kernel's constants
+    const ExportZero z = export_zero<E>(f);                 // once per thread, as export_kernel's constants
     for (Index it = (Index) (((size_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5); it < items; it += warps) {
         const Index k = it / per, rem = it - k * per;
         const int j = (int) (rem / strips), strip = (int) (rem - (Index) j * strips);
@@ -252,20 +290,40 @@ __global__ void __launch_bounds__(256) export_yuv_kernel(const __grid_constant__
         uint8_t* const dst = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst)));
         const int slot = __ldg(&e->slot);
         const uint32_t* frame = reinterpret_cast<const uint32_t*>(a.fb) + (size_t) slot * a.h * a.w;
-        yuv_item<false>(a, f, Fmt, frame, slot, dst, dst + a.uv_offset, a.cr_offset, j, strip, x, z);
+        yuv_item<false, E>(a, f, Fmt, frame, slot, dst, dst + a.uv_offset, a.cr_offset, j, strip, x, z);
     }
 }
 
+template <typename Index, int Fmt>
+__global__ void __launch_bounds__(256) export_yuv_kernel(const __grid_constant__ ExportArgs a) { yuv_loop<Index, Fmt, 0>(a); }
+// under encoding E = 1..3
+template <typename Index, int Fmt, int E>
+__global__ void __launch_bounds__(256) export_yuv_enc_kernel(const __grid_constant__ ExportArgs a) { yuv_loop<Index, Fmt, E>(a); }
+
 template <typename Index>
 static void launch_yuv(const ExportArgs& a, unsigned blocks, cudaStream_t st) {
-    if (a.format == GLAVA_B200_EXPORT_I420) export_yuv_kernel<Index, GLAVA_B200_EXPORT_I420><<<blocks, 256, 0, st>>>(a);
+    if (a.enc) {
+        for_enc(a.enc, [&](auto e) {
+            constexpr int E = decltype(e)::value;
+            if (a.format == GLAVA_B200_EXPORT_I420) export_yuv_enc_kernel<Index, GLAVA_B200_EXPORT_I420, E><<<blocks, 256, 0, st>>>(a);
+            else if (a.format == GLAVA_B200_EXPORT_YUV444) export_yuv_enc_kernel<Index, GLAVA_B200_EXPORT_YUV444, E><<<blocks, 256, 0, st>>>(a);
+            else export_yuv_enc_kernel<Index, GLAVA_B200_EXPORT_P010, E><<<blocks, 256, 0, st>>>(a);
+        });
+    } else if (a.format == GLAVA_B200_EXPORT_I420) export_yuv_kernel<Index, GLAVA_B200_EXPORT_I420><<<blocks, 256, 0, st>>>(a);
     else if (a.format == GLAVA_B200_EXPORT_YUV444) export_yuv_kernel<Index, GLAVA_B200_EXPORT_YUV444><<<blocks, 256, 0, st>>>(a);
     else export_yuv_kernel<Index, GLAVA_B200_EXPORT_P010><<<blocks, 256, 0, st>>>(a);
 }
 
 int launch_export(const ExportArgs& a, void* stream) {
     const ExportGrid g = export_grid((uint64_t) a.count * (uint64_t) ((a.w + 127) >> 7) * (uint64_t) ((a.h + 1) >> 1));
-    if (a.format != GLAVA_B200_EXPORT_NV12 && export_yuv(a.format)) {
+    cudaStream_t st = (cudaStream_t) stream;
+    if (a.enc && a.format == GLAVA_B200_EXPORT_NV12) {
+        for_enc(a.enc, [&](auto e) {
+            constexpr int E = decltype(e)::value;
+            if (g.narrow) export_nv12_enc_kernel<uint32_t, E><<<g.blocks, 256, 0, st>>>(a);
+            else export_nv12_enc_kernel<uint64_t, E><<<g.blocks, 256, 0, st>>>(a);
+        });
+    } else if (a.format != GLAVA_B200_EXPORT_NV12 && export_yuv(a.format)) {
         if (g.narrow) launch_yuv<uint32_t>(a, g.blocks, (cudaStream_t) stream);
         else launch_yuv<uint64_t>(a, g.blocks, (cudaStream_t) stream);
     } else if (g.narrow) export_kernel<uint32_t><<<g.blocks, 256, 0, (cudaStream_t) stream>>>(a);
@@ -326,8 +384,8 @@ __device__ __forceinline__ uint32_t scaled_px(const A& a, const ExportFmt& f, co
 }
 
 // One item of export_scaled_kernel (and of a ladder's other rungs): output row u (NV12: rows 2u and 2u + 1) at column X of
-// the lane; zc: what a zero pixel becomes.  A as scaled_px, and fb, format and pitch.
-template <bool Keep, typename A>
+// the lane; zc: what a zero pixel becomes; E the encoding of NV12.  A as scaled_px, and fb, format and pitch.
+template <bool Keep, int E = 0, typename A>
 __device__ __forceinline__ void scaled_item(const A& a, const ExportFmt& f, const ExportRecip& rcp, uint32_t zc, bool nv12,
                                             const ExportEntryUV* e, int u, int X, int lane) {
     const bool active = X < a.out_w;
@@ -341,12 +399,12 @@ __device__ __forceinline__ void scaled_item(const A& a, const ExportFmt& f, cons
         const uint32_t top1 = __shfl_down_sync(0xffffffffu, top, 1), bot1 = __shfl_down_sync(0xffffffffu, bot, 1);
         if (!active) return;
         uint8_t* const r0 = dst + (size_t) (2 * u) * a.pitch + X;
-        __stcs(r0, (uint8_t) export_y(top));
-        __stcs(r0 + a.pitch, (uint8_t) export_y(bot));
+        __stcs(r0, (uint8_t) export_y<E>(top));
+        __stcs(r0 + a.pitch, (uint8_t) export_y<E>(bot));
         if (!(lane & 1)) {
             uint8_t* const uv = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst_uv)));
             __stcs(reinterpret_cast<unsigned short*>(uv + (size_t) u * a.pitch + X),
-                   (unsigned short) export_cbcr(export_avg4(top, top1, bot, bot1)));
+                   (unsigned short) export_cbcr<E>(export_avg4(top, top1, bot, bot1)));
         }
     } else {
         uint32_t px = scaled_px<Keep>(a, f, frame, slot, u, active, sx, rcp, zc);
@@ -356,8 +414,8 @@ __device__ __forceinline__ void scaled_item(const A& a, const ExportFmt& f, cons
     }
 }
 
-template <typename Index>
-__global__ void __launch_bounds__(256) export_scaled_kernel(const __grid_constant__ ScaledArgs a) {
+template <typename Index, int E>
+__device__ __forceinline__ void scaled_loop(const ScaledArgs& a) {
     const ExportFmt f = { a.format, a.over, a.native, a.bg };
     const ExportRecip rcp = { a.div_mul, a.div_shift };
     const bool nv12 = a.format == GLAVA_B200_EXPORT_NV12;
@@ -369,14 +427,20 @@ __global__ void __launch_bounds__(256) export_scaled_kernel(const __grid_constan
     for (Index it = (Index) (((size_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5); it < items; it += warps) {
         const Index k = it / per, rem = it - k * per;
         const int u = (int) (rem / runs), X = (int) (rem - (Index) u * runs) * 32 + lane;
-        scaled_item<false>(a, f, rcp, zc, nv12, a.list + k, u, X, lane);
+        scaled_item<false, E>(a, f, rcp, zc, nv12, a.list + k, u, X, lane);
     }
 }
 
+template <typename Index>
+__global__ void __launch_bounds__(256) export_scaled_kernel(const __grid_constant__ ScaledArgs a) { scaled_loop<Index, 0>(a); }
+// NV12 under encoding E = 1..3
+template <typename Index, int E>
+__global__ void __launch_bounds__(256) export_scaled_enc_kernel(const __grid_constant__ ScaledArgs a) { scaled_loop<Index, E>(a); }
+
 // One item of export_scaled_yuv_kernel (and of a ladder's other I420 / YUV444 / P010 rungs), as scaled_item: output row u
 // (I420 / P010: rows 2u and 2u + 1, the chroma of each 2x2 block from the right neighbour by shuffle) at column X of the
-// lane.  The chroma plane is the entry's dst_uv (I420 / YUV444: Cb, Cr `cr` bytes further; P010: CbCr).
-template <bool Keep, typename A>
+// lane.  The chroma plane is the entry's dst_uv (I420 / YUV444: Cb, Cr `cr` bytes further; P010: CbCr); E the encoding.
+template <bool Keep, int E = 0, typename A>
 __device__ __forceinline__ void scaled_yuv_item(const A& a, const ExportFmt& f, int fmt, const ExportRecip& rcp, uint32_t zc,
                                                 size_t cr, const ExportEntryUV* e, int u, int X, int lane) {
     const bool active = X < a.out_w;
@@ -389,8 +453,8 @@ __device__ __forceinline__ void scaled_yuv_item(const A& a, const ExportFmt& f, 
         const uint32_t px = scaled_px<Keep>(a, f, frame, slot, u, active, sx, rcp, zc);
         if (!active) return;
         const size_t o = (size_t) u * a.pitch + X;
-        const uint32_t uv = export_cbcr(px);
-        __stcs(dst + o, (uint8_t) export_y(px));
+        const uint32_t uv = export_cbcr<E>(px);
+        __stcs(dst + o, (uint8_t) export_y<E>(px));
         __stcs(cb + o, (uint8_t) uv);
         __stcs(cb + cr + o, (uint8_t) (uv >> 8));
         return;
@@ -402,25 +466,25 @@ __device__ __forceinline__ void scaled_yuv_item(const A& a, const ExportFmt& f, 
     if (!active) return;
     if (fmt == GLAVA_B200_EXPORT_I420) {
         uint8_t* const r0 = dst + (size_t) (2 * u) * a.pitch + X;
-        __stcs(r0, (uint8_t) export_y(top));
-        __stcs(r0 + a.pitch, (uint8_t) export_y(bot));
+        __stcs(r0, (uint8_t) export_y<E>(top));
+        __stcs(r0 + a.pitch, (uint8_t) export_y<E>(bot));
         if (!(lane & 1)) {
-            const uint32_t uv = export_cbcr(export_avg4(top, top1, bot, bot1));
+            const uint32_t uv = export_cbcr<E>(export_avg4(top, top1, bot, bot1));
             uint8_t* const pu = cb + (size_t) u * (a.pitch >> 1) + (X >> 1);
             __stcs(pu, (uint8_t) uv);
             __stcs(pu + cr, (uint8_t) (uv >> 8));
         }
     } else {                                                // P010
         uint8_t* const r0 = dst + (size_t) (2 * u) * a.pitch + 2 * X;
-        __stcs(reinterpret_cast<unsigned short*>(r0), (unsigned short) (export_y10(top) << 6));
-        __stcs(reinterpret_cast<unsigned short*>(r0 + a.pitch), (unsigned short) (export_y10(bot) << 6));
+        __stcs(reinterpret_cast<unsigned short*>(r0), (unsigned short) (export_y10<E>(top) << 6));
+        __stcs(reinterpret_cast<unsigned short*>(r0 + a.pitch), (unsigned short) (export_y10<E>(bot) << 6));
         if (!(lane & 1))
-            __stcs(reinterpret_cast<uint32_t*>(cb + (size_t) u * a.pitch + 2 * X), export_cbcr10(export_sum4(top, top1, bot, bot1)) << 6);
+            __stcs(reinterpret_cast<uint32_t*>(cb + (size_t) u * a.pitch + 2 * X), export_cbcr10<E>(export_sum4(top, top1, bot, bot1)) << 6);
     }
 }
 
-template <typename Index, int Fmt>
-__global__ void __launch_bounds__(256) export_scaled_yuv_kernel(const __grid_constant__ ScaledArgs a) {
+template <typename Index, int Fmt, int E>
+__device__ __forceinline__ void scaled_yuv_loop(const ScaledArgs& a) {
     const ExportFmt f = { Fmt, 1, a.native, a.bg };
     const ExportRecip rcp = { a.div_mul, a.div_shift };
     const uint32_t zc = export_over(0u, f.bg, f.native);    // what a zero pixel becomes
@@ -431,13 +495,28 @@ __global__ void __launch_bounds__(256) export_scaled_yuv_kernel(const __grid_con
     for (Index it = (Index) (((size_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5); it < items; it += warps) {
         const Index k = it / per, rem = it - k * per;
         const int u = (int) (rem / runs), X = (int) (rem - (Index) u * runs) * 32 + lane;
-        scaled_yuv_item<false>(a, f, Fmt, rcp, zc, a.cr_offset, a.list + k, u, X, lane);
+        scaled_yuv_item<false, E>(a, f, Fmt, rcp, zc, a.cr_offset, a.list + k, u, X, lane);
     }
+}
+
+template <typename Index, int Fmt>
+__global__ void __launch_bounds__(256) export_scaled_yuv_kernel(const __grid_constant__ ScaledArgs a) { scaled_yuv_loop<Index, Fmt, 0>(a); }
+// under encoding E = 1..3
+template <typename Index, int Fmt, int E>
+__global__ void __launch_bounds__(256) export_scaled_yuv_enc_kernel(const __grid_constant__ ScaledArgs a) {
+    scaled_yuv_loop<Index, Fmt, E>(a);
 }
 
 template <typename Index>
 static void launch_scaled_yuv(const ScaledArgs& a, unsigned blocks, cudaStream_t st) {
-    if (a.format == GLAVA_B200_EXPORT_I420) export_scaled_yuv_kernel<Index, GLAVA_B200_EXPORT_I420><<<blocks, 256, 0, st>>>(a);
+    if (a.enc) {
+        for_enc(a.enc, [&](auto e) {
+            constexpr int E = decltype(e)::value;
+            if (a.format == GLAVA_B200_EXPORT_I420) export_scaled_yuv_enc_kernel<Index, GLAVA_B200_EXPORT_I420, E><<<blocks, 256, 0, st>>>(a);
+            else if (a.format == GLAVA_B200_EXPORT_YUV444) export_scaled_yuv_enc_kernel<Index, GLAVA_B200_EXPORT_YUV444, E><<<blocks, 256, 0, st>>>(a);
+            else export_scaled_yuv_enc_kernel<Index, GLAVA_B200_EXPORT_P010, E><<<blocks, 256, 0, st>>>(a);
+        });
+    } else if (a.format == GLAVA_B200_EXPORT_I420) export_scaled_yuv_kernel<Index, GLAVA_B200_EXPORT_I420><<<blocks, 256, 0, st>>>(a);
     else if (a.format == GLAVA_B200_EXPORT_YUV444) export_scaled_yuv_kernel<Index, GLAVA_B200_EXPORT_YUV444><<<blocks, 256, 0, st>>>(a);
     else export_scaled_yuv_kernel<Index, GLAVA_B200_EXPORT_P010><<<blocks, 256, 0, st>>>(a);
 }
@@ -445,7 +524,14 @@ static void launch_scaled_yuv(const ScaledArgs& a, unsigned blocks, cudaStream_t
 int launch_export_scaled(const ScaledArgs& a, void* stream) {
     const uint64_t units = export_420(a.format) ? (uint64_t) (a.out_h >> 1) : (uint64_t) a.out_h;
     const ExportGrid g = export_grid((uint64_t) a.count * (uint64_t) ((a.out_w + 31) >> 5) * units);
-    if (a.format != GLAVA_B200_EXPORT_NV12 && export_yuv(a.format)) {
+    cudaStream_t st = (cudaStream_t) stream;
+    if (a.enc && a.format == GLAVA_B200_EXPORT_NV12) {
+        for_enc(a.enc, [&](auto e) {
+            constexpr int E = decltype(e)::value;
+            if (g.narrow) export_scaled_enc_kernel<uint32_t, E><<<g.blocks, 256, 0, st>>>(a);
+            else export_scaled_enc_kernel<uint64_t, E><<<g.blocks, 256, 0, st>>>(a);
+        });
+    } else if (a.format != GLAVA_B200_EXPORT_NV12 && export_yuv(a.format)) {
         if (g.narrow) launch_scaled_yuv<uint32_t>(a, g.blocks, (cudaStream_t) stream);
         else launch_scaled_yuv<uint64_t>(a, g.blocks, (cudaStream_t) stream);
     } else if (g.narrow) export_scaled_kernel<uint32_t><<<g.blocks, 256, 0, (cudaStream_t) stream>>>(a);
@@ -468,8 +554,47 @@ struct RungView {
     int src_x, src_y, src_w, src_h, out_w, out_h;
 };
 
+// One unit of export_ladder_enc_kernel: the item of rung g's standalone kernel under encoding E; Yuv as ladder_loop
+template <bool Yuv, int E>
+__device__ __forceinline__ void ladder_item(const LadderArgs& a, const LadderRung& g, const ExportEntryUV* e, int rung, int row,
+                                            int col, int lane) {
+    const RungView v = { a.fb, a.marks, a.mark_rows, a.w, a.h, g.format, g.pitch, g.src_x, g.src_y, g.src_w, g.src_h, g.out_w, g.out_h };
+    const ExportFmt f = { g.format, g.over, a.native, g.bg };
+    if (Yuv && g.format != GLAVA_B200_EXPORT_NV12 && export_yuv(g.format)) {
+        const size_t cr = a.yuv[rung].cr_offset;
+        if (g.whole) {
+            const int x = col * 128 + lane * 4;
+            if (x >= a.w) return;
+            uint8_t* const dst = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst)));
+            uint8_t* const cb = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst_uv)));
+            const int slot = __ldg(&e->slot);
+            const uint32_t* frame = reinterpret_cast<const uint32_t*>(a.fb) + (size_t) slot * a.h * a.w;
+            const ExportZero z = { a.yuv[rung].zy, a.yuv[rung].zu, a.yuv[rung].zv };
+            yuv_item<true, E>(v, f, g.format, frame, slot, dst, cb, cr, row, col, x, z);
+        } else {
+            const ExportRecip rcp = { g.div_mul, g.div_shift };
+            scaled_yuv_item<true, E>(v, f, g.format, rcp, g.zc, cr, e, row, col * 32 + lane, lane);
+        }
+    } else if (g.whole) {
+        const int x = col * 128 + lane * 4;
+        if (x >= a.w) return;
+        uint8_t* const dst = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst)));
+        // the entry's CbCr pointer as an offset from its luma (unsigned: the chroma may lie before it)
+        const size_t uv_offset = g.format == GLAVA_B200_EXPORT_NV12
+                                     ? (size_t) (__ldg(reinterpret_cast<const unsigned long long*>(&e->dst_uv)) - (unsigned long long) dst)
+                                     : 0;
+        const int slot = __ldg(&e->slot);
+        const uint32_t* frame = reinterpret_cast<const uint32_t*>(a.fb) + (size_t) slot * a.h * a.w;
+        export_item<true, E>(v, f, frame, slot, dst, uv_offset, row, col, x, g.zy, g.zuv, g.zpx);
+    } else {
+        const ExportRecip rcp = { g.div_mul, g.div_shift };
+        scaled_item<true, E>(v, f, rcp, g.zc, g.format == GLAVA_B200_EXPORT_NV12, e, row, col * 32 + lane, lane);
+    }
+}
+
 // The ladder's loop; Yuv: the rungs may be I420, YUV444 or P010 (export_ladder_yuv_kernel), else they are NV12, RGBA or
-// BGRA (export_ladder_kernel, whose code does not see the new formats)
+// BGRA (export_ladder_kernel, whose code does not see the new formats).  Every rung is encoding 0.  ladder_item<Yuv, 0>
+// written out: called, ptxas schedules the 64-bit index kernel differently, and these kernels keep their machine code.
 template <typename Index, bool Yuv>
 __device__ __forceinline__ void ladder_loop(const LadderArgs& a) {
     const Index units = (Index) a.units, items = (Index) a.count * units;
@@ -516,17 +641,45 @@ __device__ __forceinline__ void ladder_loop(const LadderArgs& a) {
     }
 }
 
+// The loop of export_ladder_enc_kernel: any format and encoding per rung, each unit run by the instantiation of its rung's
+template <typename Index>
+__device__ __forceinline__ void ladder_enc_loop(const LadderArgs& a) {
+    const Index units = (Index) a.units, items = (Index) a.count * units;
+    const Index warps = (Index) (((size_t) gridDim.x * blockDim.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    for (Index it = (Index) (((size_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5); it < items; it += warps) {
+        const Index k = it / units;
+        const uint64_t unit = __ldg(reinterpret_cast<const unsigned long long*>(a.sched) + (it - k * units));
+        const int rung = ladder_unit_rung(unit), row = ladder_unit_row(unit), col = ladder_unit_col(unit);
+        const LadderRung& g = a.rung[rung];
+        const ExportEntryUV* e = a.list + (size_t) k * a.nrungs + rung;
+        if (g.enc == 1) ladder_item<true, 1>(a, g, e, rung, row, col, lane);
+        else if (g.enc == 2) ladder_item<true, 2>(a, g, e, rung, row, col, lane);
+        else if (g.enc == 3) ladder_item<true, 3>(a, g, e, rung, row, col, lane);
+        else ladder_item<true, 0>(a, g, e, rung, row, col, lane);
+    }
+}
+
 template <typename Index>
 __global__ void __launch_bounds__(256) export_ladder_kernel(const __grid_constant__ LadderArgs a) { ladder_loop<Index, false>(a); }
 template <typename Index>
 __global__ void __launch_bounds__(256) export_ladder_yuv_kernel(const __grid_constant__ LadderArgs a) { ladder_loop<Index, true>(a); }
+// any format and encoding per rung (DESIGN 4.15)
+template <typename Index>
+__global__ void __launch_bounds__(256) export_ladder_enc_kernel(const __grid_constant__ LadderArgs a) { ladder_enc_loop<Index>(a); }
 
 int launch_export_ladder(const LadderArgs& a, void* stream) {
     const ExportGrid g = export_grid((uint64_t) a.count * (uint64_t) a.units);
-    bool yuv = false;
-    for (int j = 0; j < a.nrungs; ++j) yuv |= a.rung[j].format != GLAVA_B200_EXPORT_NV12 && export_yuv(a.rung[j].format);
+    bool yuv = false, enc = false;
+    for (int j = 0; j < a.nrungs; ++j) {
+        yuv |= a.rung[j].format != GLAVA_B200_EXPORT_NV12 && export_yuv(a.rung[j].format);
+        enc |= a.rung[j].enc != 0;
+    }
     cudaStream_t st = (cudaStream_t) stream;
-    if (yuv) {
+    if (enc) {
+        if (g.narrow) export_ladder_enc_kernel<uint32_t><<<g.blocks, 256, 0, st>>>(a);
+        else export_ladder_enc_kernel<uint64_t><<<g.blocks, 256, 0, st>>>(a);
+    } else if (yuv) {
         if (g.narrow) export_ladder_yuv_kernel<uint32_t><<<g.blocks, 256, 0, st>>>(a);
         else export_ladder_yuv_kernel<uint64_t><<<g.blocks, 256, 0, st>>>(a);
     } else if (g.narrow) export_ladder_kernel<uint32_t><<<g.blocks, 256, 0, st>>>(a);
@@ -559,7 +712,9 @@ __device__ __forceinline__ void overlay_rgba(uint8_t* row, int x, int w, bool bg
 }
 
 // NV12 of the quad at x of output rows 2j, 2j + 1 (r0: row 2j's Y bytes, uv: the pair's CbCr row); native: blended onto the
-// bytes there, skipped when all eight pixels are zero; otherwise export_kernel's bytes (f: composite, opacity not native)
+// bytes there, skipped when all eight pixels are zero; otherwise export_kernel's bytes (f: composite, opacity not native).
+// E: the destination's encoding.
+template <int E>
 __device__ __forceinline__ void overlay_nv12(const ExportFmt& f, bool native, uint8_t* r0, uint8_t* uv, size_t pitch, int x, int w,
                                              const uint32_t top[4], const uint32_t bot[4]) {
     const bool full = x + 4 <= w;                           // else w even: the last two pixels of a row
@@ -575,9 +730,9 @@ __device__ __forceinline__ void overlay_nv12(const ExportFmt& f, bool native, ui
             yb = __ldcs(reinterpret_cast<const unsigned short*>(r0 + pitch + x));
             c = __ldcs(reinterpret_cast<const unsigned short*>(uv + x));
         }
-        overlay_nv12_quad(top, bot, &yt, &yb, &c);
+        overlay_nv12_quad<E>(top, bot, &yt, &yb, &c);
     } else {
-        c = export_nv12_quad(f, top, bot, &yt, &yb);
+        c = export_nv12_quad<E>(f, top, bot, &yt, &yb);
     }
     if (full) {
         __stcs(reinterpret_cast<uint32_t*>(r0 + x), yt);
@@ -594,8 +749,8 @@ __device__ __forceinline__ uint32_t overlay_mark(const OverlayArgs& a, int slot,
     return __ldg(a.marks + export_mark_index(slot, a.w, a.h, a.mark_rows, y, strip));
 }
 
-template <typename Index, bool Band>
-__global__ void __launch_bounds__(256) overlay_kernel(const __grid_constant__ OverlayArgs a) {
+template <typename Index, bool Band, int E>
+__device__ __forceinline__ void overlay_loop(const OverlayArgs& a) {
     const ExportFmt f = { a.format, 1, 0, 0u };             // any other opacity: the stored colour, alpha 255
     const bool nv12 = a.format == GLAVA_B200_EXPORT_NV12, bgra = a.format == GLAVA_B200_EXPORT_BGRA;
     const int rows = Band ? a.mark_rows : 2;
@@ -634,7 +789,7 @@ __global__ void __launch_bounds__(256) overlay_kernel(const __grid_constant__ Ov
                 uint32_t top[4] = { 0u, 0u, 0u, 0u }, bot[4] = { 0u, 0u, 0u, 0u };
                 if (y0 >= lo && y0 < hi) load_quad(frame, a.w, y0, x, top);
                 if (y1 >= b0 ? y1 >= lo && y1 < hi : export_row_read(below, y1)) load_quad(frame, a.w, y1, x, bot);
-                overlay_nv12(f, true, dst + (size_t) (2 * j) * a.pitch, dst_uv + (size_t) j * a.pitch, a.pitch, x, a.w, top, bot);
+                overlay_nv12<E>(f, true, dst + (size_t) (2 * j) * a.pitch, dst_uv + (size_t) j * a.pitch, a.pitch, x, a.w, top, bot);
             }
         } else {                                            // output rows 2u, 2u + 1: framebuffer rows y0, y0 - 1
             const int y0 = a.h - 1 - 2 * u, y1 = y0 - 1;
@@ -644,7 +799,7 @@ __global__ void __launch_bounds__(256) overlay_kernel(const __grid_constant__ Ov
             uint8_t* const r0 = dst + (size_t) (2 * u) * a.pitch;
             if (nv12) {
                 uint8_t* const dst_uv = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst_uv)));
-                overlay_nv12(f, a.native, r0, dst_uv + (size_t) u * a.pitch, a.pitch, x, a.w, top, bot);
+                overlay_nv12<E>(f, a.native, r0, dst_uv + (size_t) u * a.pitch, a.pitch, x, a.w, top, bot);
             } else if (a.native) {
                 overlay_rgba(r0, x, a.w, bgra, top);
                 if (y1 >= 0) overlay_rgba(r0 + a.pitch, x, a.w, bgra, bot);
@@ -656,11 +811,28 @@ __global__ void __launch_bounds__(256) overlay_kernel(const __grid_constant__ Ov
     }
 }
 
+template <typename Index, bool Band>
+__global__ void __launch_bounds__(256) overlay_kernel(const __grid_constant__ OverlayArgs a) { overlay_loop<Index, Band, 0>(a); }
+// NV12 destinations in encoding E = 1..3
+template <typename Index, bool Band, int E>
+__global__ void __launch_bounds__(256) overlay_enc_kernel(const __grid_constant__ OverlayArgs a) { overlay_loop<Index, Band, E>(a); }
+
 int launch_overlay(const OverlayArgs& a, void* stream) {
     const int rows = a.band ? a.mark_rows : 2;
     const ExportGrid g = export_grid((uint64_t) a.count * (uint64_t) ((a.w + 127) >> 7) * (uint64_t) ((a.h + rows - 1) / rows));
     cudaStream_t st = (cudaStream_t) stream;
-    if (a.band) {
+    if (a.enc) {
+        for_enc(a.enc, [&](auto e) {
+            constexpr int E = decltype(e)::value;
+            if (a.band) {
+                if (g.narrow) overlay_enc_kernel<uint32_t, true, E><<<g.blocks, 256, 0, st>>>(a);
+                else overlay_enc_kernel<uint64_t, true, E><<<g.blocks, 256, 0, st>>>(a);
+            } else {
+                if (g.narrow) overlay_enc_kernel<uint32_t, false, E><<<g.blocks, 256, 0, st>>>(a);
+                else overlay_enc_kernel<uint64_t, false, E><<<g.blocks, 256, 0, st>>>(a);
+            }
+        });
+    } else if (a.band) {
         if (g.narrow) overlay_kernel<uint32_t, true><<<g.blocks, 256, 0, st>>>(a);
         else overlay_kernel<uint64_t, true><<<g.blocks, 256, 0, st>>>(a);
     } else {

@@ -47,6 +47,15 @@ int ladder_check(glava_b200* r, const int* streams, int count, const glava_b200_
     return 0;
 }
 
+// What zero pixels become in a rung under encoding E: NV12's zy / zuv into g, and export_zero for the other Y'CbCr formats
+template <int E>
+static ExportZero rung_zero(const ExportFmt& f, LadderRung* g) {
+    const uint32_t zero4[4] = { 0u, 0u, 0u, 0u };
+    uint32_t zy1;
+    g->zuv = export_nv12_quad<E>(f, zero4, zero4, &g->zy, &zy1);
+    return export_zero<E>(f);
+}
+
 // the device schedule for `geom`, built and uploaded on the raster stream when the geometry differs from the last ladder's
 static int ladder_schedule_room(const RendererView& v, ExportList* L, const LadderGeom* geom, int nrungs, uint32_t* units) {
     std::vector<int> key = { v.w, v.h, nrungs };
@@ -125,15 +134,19 @@ int ladder_run(glava_b200* r, const int* streams, int count, const glava_b200_ex
             g.out_w = q[j].out_w; g.out_h = q[j].out_h;
             const ExportRecip rcp = export_recip((uint64_t) q[j].src_w * (uint64_t) q[j].src_h);
             g.div_mul = rcp.mul; g.div_shift = rcp.shift;
+            g.enc = export_enc(d.flags);
             // what a zero pixel becomes, as export_kernel and export_scaled_kernel compute it before their loops
             const ExportFmt f = { g.format, g.over, v.native, g.bg };
-            const uint32_t zero4[4] = { 0u, 0u, 0u, 0u };
-            uint32_t zy1;
-            g.zuv = export_nv12_quad(f, zero4, zero4, &g.zy, &zy1);
             g.zpx = export_px(f, 0u);
             g.zc = f.over ? export_over(0u, f.bg, f.native) : 0u;
-            // and as export_yuv_kernel computes them for I420, YUV444 and P010
-            const ExportZero z = export_zero(f);
+            // NV12's words, and I420's, YUV444's and P010's as export_yuv_kernel computes them, in the rung's encoding
+            ExportZero z;
+            switch (g.enc) {
+            case 1: z = rung_zero<1>(f, &g); break;
+            case 2: z = rung_zero<2>(f, &g); break;
+            case 3: z = rung_zero<3>(f, &g); break;
+            default: z = rung_zero<0>(f, &g); break;
+            }
             a.yuv[j] = { planes[j].cr, z.y, z.u, z.v };
         }
         return launch_export_ladder(a, v.stream);

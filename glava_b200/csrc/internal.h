@@ -206,8 +206,10 @@ struct ExportArgs {
     uint32_t bg;
     size_t pitch, uv_offset;    // uv_offset: luma to chroma plane (export_core.h ExportPlanes cb)
     size_t cr_offset;           // I420 / YUV444: Cb to Cr plane (ExportPlanes cr)
+    int    enc;                 // Y'CbCr encoding, export_core.h export_enc of the flags (0: BT.709 limited range)
 };
-// NV12, RGBA and BGRA run export_kernel; I420, YUV444 and P010 export_yuv_kernel
+// NV12, RGBA and BGRA run export_kernel; I420, YUV444 and P010 export_yuv_kernel; any other encoding than 0 the kernels'
+// instantiations for it (export_nv12_enc_kernel, export_yuv_enc_kernel)
 int launch_export(const ExportArgs& a, void* stream);
 // The entry of the scaled export and the overlay: ExportEntry with a chroma pointer, so that one call can fill an NV12
 // mosaic, where each tile's chroma sits at a different offset from its luma
@@ -233,8 +235,10 @@ struct ScaledArgs {
     uint64_t div_mul;
     int    div_shift;
     size_t cr_offset;           // as ExportArgs
+    int    enc;                 // as ExportArgs
 };
-// NV12, RGBA and BGRA run export_scaled_kernel; I420, YUV444 and P010 export_scaled_yuv_kernel
+// NV12, RGBA and BGRA run export_scaled_kernel; I420, YUV444 and P010 export_scaled_yuv_kernel; enc != 0 their
+// instantiations for it (export_scaled_enc_kernel, export_scaled_yuv_enc_kernel)
 int launch_export_scaled(const ScaledArgs& a, void* stream);
 // export_kernels.cu: glava_b200_overlay_frames (DESIGN 4.12), one launch for the whole list, its own argument struct and
 // ExportEntryUV entries.  band = 1 (native opacity with marks): one warp per (entry, band of mark_rows rows, strip), else one per
@@ -247,6 +251,7 @@ struct OverlayArgs {
     int    count, w, h;
     int    format, native, band;
     size_t pitch;
+    int    enc;                 // NV12: the destination's encoding, as ExportArgs (enc != 0 runs overlay_enc_kernel)
 };
 int launch_overlay(const OverlayArgs& a, void* stream);
 // export_kernels.cu: glava_b200_export_ladder (DESIGN 4.13), one launch for every rung of every entry.  Per rung what a
@@ -260,6 +265,7 @@ struct LadderRung {
     uint64_t div_mul;
     int    div_shift;
     uint32_t zpx, zy, zuv, zc;  // export_kernel's zpx / zy / zuv, export_scaled_kernel's zc
+    int    enc;                 // as ExportArgs (in what was padding: the struct keeps its 80 bytes)
 };
 // The grid is flattened over (entry, unit of `sched`), the unit fastest; list: [count][nrungs] entries
 struct LadderArgs {
@@ -275,7 +281,8 @@ struct LadderArgs {
     // I420 / YUV444 / P010 rungs: the Cb to Cr distance (ExportArgs cr_offset) and export_core.h export_zero of the rung
     struct { size_t cr_offset; uint32_t zy, zu, zv; } yuv[GLAVA_B200_LADDER_MAX];
 };
-// export_ladder_kernel, or export_ladder_yuv_kernel when a rung is I420, YUV444 or P010
+// export_ladder_kernel, or export_ladder_yuv_kernel when a rung is I420, YUV444 or P010, or export_ladder_enc_kernel when a
+// rung has an encoding other than 0
 int launch_export_ladder(const LadderArgs& a, void* stream);
 // capi.cu, for export.cpp: what the frame export reads of a renderer, and the slot where it keeps its own per-renderer
 // state (*attach, released by *attach_free when the renderer is destroyed)

@@ -359,7 +359,8 @@ int   glava_b200_framebuffer_ipc(glava_b200* r, void* handle, size_t handle_byte
  *     GLAVA_B200_EXPORT_RGBA   h rows of w * 4 bytes R,G,B,A, `pitch` bytes apart
  *     GLAVA_B200_EXPORT_BGRA   the same as B,G,R,A (what compositors and NVENC's ARGB input take)
  *     GLAVA_B200_EXPORT_NV12   Y plane of h rows x w bytes, then the interleaved CbCr plane of h / 2 rows x w bytes at
- *                              `uv_offset` (0: pitch * h); BT.709 limited range in 16-bit fixed point (export_core.h),
+ *                              `uv_offset` (0: pitch * h); BT.709 limited range (or as the colour flags below say) in
+ *                              16-bit fixed point (export_core.h),
  *                              chroma from the per-channel average (s + 2) >> 2 of each composited 2x2 block; w and h even
  *     GLAVA_B200_EXPORT_I420   planar 4:2:0 (yuv420p): Y plane of h rows x w bytes at `pitch`, then the Cb and Cr planes of
  *                              h / 2 rows x w / 2 bytes at `pitch / 2`; NV12's arithmetic, so Y equals NV12's Y and Cb / Cr
@@ -368,7 +369,7 @@ int   glava_b200_framebuffer_ipc(glava_b200* r, void* handle, size_t handle_byte
  *                              composited pixel with no averaging
  *     GLAVA_B200_EXPORT_P010   10-bit 4:2:0: Y plane of h rows x w little-endian uint16, then the interleaved CbCr plane of
  *                              h / 2 rows x w / 2 (Cb, Cr) uint16 pairs, both at `pitch` (>= 2 w); each sample is the 10-bit
- *                              BT.709 limited-range code << 6; chroma from the exact per-channel sums of each composited
+ *                              BT.709 limited-range code (or as the colour flags say) << 6; chroma from the exact per-channel sums of each composited
  *                              2x2 block (export_core.h); w and h even
  *   Where the chroma planes go: NV12 and P010 put the CbCr plane at `uv_offset` from dst[i] (0: pitch * h).  I420 and
  *   YUV444 put the Cb plane right after the luma, at dst[i] + pitch * h, and `uv_offset` is the distance from Cb to Cr (0: the
@@ -379,6 +380,13 @@ int   glava_b200_framebuffer_ipc(glava_b200* r, void* handle, size_t handle_byte
  *                              mul_norm8(bg, 255 - a)) per channel; under any other opacity the stored colour (the window
  *                              ignores alpha and the clear colour already stands in for the desktop).  Alpha becomes 255.
  *                              Without it RGBA / BGRA carry the stored pixels, alpha included.
+ *   GLAVA_B200_EXPORT_FULL_RANGE, GLAVA_B200_EXPORT_BT601   the Y'CbCr encoding of NV12, I420, YUV444 and P010 (DESIGN.md
+ *                              §4.15).  Neither: BT.709 limited range.  BT601 takes Kr, Kb = 0.299, 0.114 for BT.709's
+ *                              0.2126, 0.0722; FULL_RANGE writes Y = Y', C = 128 + P over 0..255 (10 bits: 1023/255 Y',
+ *                              512 + 1023/255 P, clamped to 1023) for limited range's 16 + 219/255 Y', 128 + 224/255 P
+ *                              (64 + 876/255 Y', 512 + 896/255 P).  Both: the JFIF encoding JPEG encoders take (nvJPEG's
+ *                              YUV input, libjpeg-turbo's raw data, ffmpeg's yuvj420p).  Every grey has Cb = Cr = 128
+ *                              (512).  RGBA / BGRA with either bit are GLAVA_B200_EINVAL (no matrix or range).
  *   dst[i], pitch and uv_offset are multiples of 16, pitch >= the row bytes, uv_offset (when set) >= pitch * h (I420 /
  *   YUV444: >= one chroma plane).  An unknown format or flag, odd NV12 / I420 / P010 dimensions, a misaligned or short pitch
  *   (I420: not a multiple of 32), a null, host or other-device dst, a stream out of range, count < 1 and a renderer a failed
@@ -401,9 +409,11 @@ int   glava_b200_framebuffer_ipc(glava_b200* r, void* handle, size_t handle_byte
 #define GLAVA_B200_EXPORT_YUV444 5
 #define GLAVA_B200_EXPORT_P010 6
 #define GLAVA_B200_EXPORT_OVER 1u
+#define GLAVA_B200_EXPORT_FULL_RANGE 0x100u
+#define GLAVA_B200_EXPORT_BT601 0x200u
 typedef struct {
     int      format;            /* GLAVA_B200_EXPORT_RGBA / _BGRA / _NV12 / _I420 / _YUV444 / _P010 */
-    uint32_t flags;             /* GLAVA_B200_EXPORT_OVER */
+    uint32_t flags;             /* GLAVA_B200_EXPORT_OVER, and for the Y'CbCr formats _FULL_RANGE / _BT601 */
     uint8_t  background[4];     /* R, G, B of the opaque background the composite uses; byte 3 unused */
     size_t   pitch;             /* bytes from one output row to the next (every plane; I420 chroma rows: pitch / 2) */
     size_t   uv_offset;         /* NV12 / P010: bytes from dst[i] to the CbCr plane, 0 = pitch * h; I420 / YUV444: bytes
@@ -457,7 +467,8 @@ int glava_b200_export_scaled(glava_b200* r, const int* streams, int count, void*
  *                              &dst[i * nrungs + j], dst_uv ? &dst_uv[i * nrungs + j] : NULL, &rungs[j].desc,
  *                              &rungs[j].scale, ...) would write at this point in call order (framebuffer ring, styles and
  *                              repeated streams included); a rung that is the whole frame at its own size is therefore
- *                              glava_b200_export_frames, bit for bit.  Formats and flags may differ between rungs.  Ordering
+ *                              glava_b200_export_frames, bit for bit.  Formats and flags, colour flags included, may differ
+ *                              between rungs, so one ladder can mix encodings.  Ordering
  *                              and events as glava_b200_export_frames: waits for `after_event` on the device, runs on the
  *                              handle's stream behind the latest pass, records `done_event`, returns without a host wait.
  *     dst                      [count][nrungs] destinations; each rung's size is glava_b200_export_scaled_bytes(r,
@@ -486,7 +497,9 @@ int glava_b200_export_ladder(glava_b200* r, const int* streams, int count, const
  *                              bytes per row; the caller's image around it is never touched
  *     dst_uv                   NV12: dst_uv[i] is the rectangle's first CbCr byte; NULL: dst[i] + (uv_offset ? uv_offset :
  *                              pitch * h), as glava_b200_export_scaled
- *     desc                     format and pitch (and uv_offset) as the export; flags must be 0, background is unused
+ *     desc                     format and pitch (and uv_offset) as the export; background is unused; flags 0, or for
+ *                              NV12 the colour flags EXPORT_FULL_RANGE / EXPORT_BT601, the picture's encoding: the blend
+ *                              takes that set's coefficients and offsets (full range: T = 0 a + (255 - a) Y_D for Y)
  *   Under setopacity "native" (premultiply_alpha) the stored premultiplied pixel goes "over" the caller's pixel D, as
  *   GLava's window goes over the desktop: RGBA / BGRA C = min(255, c + mul_norm8(D, 255 - a)) in all four channels (D
  *   opaque or premultiplied); NV12 blends in Y'CbCr without a trip through RGB, Y = clamp((Y_R r + Y_G g + Y_B b +
@@ -498,7 +511,7 @@ int glava_b200_export_ladder(glava_b200* r, const int* streams, int count, const
  *   The overlay takes RGBA, BGRA and NV12; I420, YUV444 and P010 are refused by name.
  *   Besides the refusals of glava_b200_export_scaled that apply (format, pitch, uv_offset, alignment, null / host /
  *   other-device dst or dst_uv, dst_uv for RGBA / BGRA, odd NV12 frames, stream range, count < 1, an unbuilt renderer),
- *   any flag, a rectangle that meets the renderer's framebuffer array and two rectangles of one call that overlap (luma
+ *   any other flag, a rectangle that meets the renderer's framebuffer array and two rectangles of one call that overlap (luma
  *   and chroma planes included: each entry reads and writes its bytes; layers go in separate calls) are GLAVA_B200_EINVAL
  *   with nothing enqueued.
  *   glava_b200_sharded_overlay_frames  the same with global stream indices, dst[i] / dst_uv[i] on the device of the shard
