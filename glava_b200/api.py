@@ -134,39 +134,47 @@ class ExportRung(C.Structure):
 LADDER_MAX = 8
 EXPORT_RGBA, EXPORT_BGRA, EXPORT_NV12 = 0, 1, 2
 EXPORT_I420, EXPORT_YUV444, EXPORT_P010 = 4, 5, 6
+EXPORT_YUV420P10, EXPORT_YUV444P10 = 7, 8                # planar 10-bit, LSB-aligned (yuv420p10le / yuv444p10le, DESIGN 4.16)
 EXPORT_OVER = 1
 EXPORT_FULL_RANGE, EXPORT_BT601 = 0x100, 0x200          # the Y'CbCr encoding (DESIGN 4.15); neither: BT.709 limited range
 EXPORT_MATRICES = {"bt709": 0, "bt601": EXPORT_BT601}
 EXPORT_FORMATS = {"rgba": EXPORT_RGBA, "bgra": EXPORT_BGRA, "nv12": EXPORT_NV12, "i420": EXPORT_I420,
-                  "yuv444": EXPORT_YUV444, "p010": EXPORT_P010}
+                  "yuv444": EXPORT_YUV444, "p010": EXPORT_P010, "yuv420p10": EXPORT_YUV420P10,
+                  "yuv444p10": EXPORT_YUV444P10}
 OVERLAY_FORMATS = ("rgba", "bgra", "nv12")
+# the formats whose samples are uint16, which also take uint16 `out` tensors
+WIDE_FORMATS = ("p010", "yuv420p10", "yuv444p10")
 
 
 def _export_layout(fmt, w, h):
     """(rows, row bytes, pitch multiple) of one w x h output of `fmt` held as rows of one pitch: RGBA / BGRA h rows of w * 4
-    bytes; NV12 / P010 h * 3 / 2 rows of w (P010: w uint16) samples, Y then CbCr; I420 h * 3 / 2 rows, the Y plane then the
-    Cb and Cr planes back to back at pitch / 2 (pitch a multiple of 32); YUV444 3 h rows, the Y, Cb and Cr planes"""
+    bytes; NV12 / P010 h * 3 / 2 rows of w (P010: w uint16) samples, Y then CbCr; I420 / YUV420P10 h * 3 / 2 rows, the Y
+    plane then the Cb and Cr planes back to back at pitch / 2 (pitch a multiple of 32); YUV444 / YUV444P10 3 h rows, the Y,
+    Cb and Cr planes; the 10-bit formats hold w uint16 per row"""
     if fmt in ("rgba", "bgra"):
         return h, w * 4, 16
-    if fmt == "yuv444":
-        return 3 * h, w, 16
-    return h * 3 // 2, w * 2 if fmt == "p010" else w, 32 if fmt == "i420" else 16
+    row = w * 2 if fmt in WIDE_FORMATS else w
+    if fmt in ("yuv444", "yuv444p10"):
+        return 3 * h, row, 16
+    return h * 3 // 2, row, 32 if fmt in ("i420", "yuv420p10") else 16
 
 
 def _export_views(fmt, t, w, h):
     """what an export into t returns: t is uint8 [..., rows, pitch] with contiguous rows as _export_layout describes.  RGBA /
     BGRA [..., h, w, 4], NV12 [..., h * 3 / 2, w] uint8, P010 [..., h * 3 / 2, w] uint16, I420 / YUV444 the plane views
-    (Y, Cb, Cr), each [..., rows, cols]"""
+    (Y, Cb, Cr), each [..., rows, cols], YUV420P10 / YUV444P10 the same as uint16"""
     import torch
-    P = t.shape[-1]
     if fmt in ("rgba", "bgra"):
         return t[..., :w * 4].unflatten(-1, (w, 4))
     if fmt == "nv12":
         return t[..., :w]
+    if fmt in WIDE_FORMATS:
+        t = t.view(torch.uint16)
     if fmt == "p010":
-        return t.view(torch.uint16)[..., :w]
+        return t[..., :w]
+    P = t.shape[-1]                                           # the pitch in samples
     flat = t.flatten(-2)
-    cw, ch, cp = (w // 2, h // 2, P // 2) if fmt == "i420" else (w, h, P)
+    cw, ch, cp = (w // 2, h // 2, P // 2) if fmt in ("i420", "yuv420p10") else (w, h, P)
     n = ch * cp
     y = flat[..., :P * h].unflatten(-1, (h, P))[..., :w]
     cb = flat[..., P * h:P * h + n].unflatten(-1, (ch, cp))[..., :cw]
@@ -464,9 +472,9 @@ class _FrameExport:
         """-> (stream list, Export, [dst pointers], what to return).  device_of(stream): the CUDA device of a stream's
         frame.  size: (w, h) of each output, None: the frame's.  out: None (allocate), one uint8 tensor [count, rows, ...]
         whose dim 1 steps by the pitch, or a list of count tensors [rows, ...] with one common pitch; rows as
-        _export_layout gives them (h for RGBA / BGRA, h * 3 / 2 for NV12, I420 and P010, 3 h for YUV444; I420 and YUV444
-        keep their planes back to back from row h); P010 also takes uint16 tensors.  matrix / full_range: the Y'CbCr
-        encoding (_export_desc)"""
+        _export_layout gives them (h for RGBA / BGRA, h * 3 / 2 for NV12, I420, P010 and YUV420P10, 3 h for YUV444 and
+        YUV444P10; the planar formats keep their planes back to back from row h); P010, YUV420P10 and YUV444P10 also take
+        uint16 tensors.  matrix / full_range: the Y'CbCr encoding (_export_desc)"""
         import torch
         s = np.ascontiguousarray(np.asarray(streams, dtype=np.int64).reshape(-1), dtype=np.int32)
         count = int(s.shape[0])
@@ -475,7 +483,7 @@ class _FrameExport:
         w, h = (p.w, p.h) if size is None else (int(size[0]), int(size[1]))
         desc = _export_desc(fmt, over, background, matrix, full_range)
         rows, row_bytes, align = _export_layout(fmt, w, h)
-        dtypes = (torch.uint8, torch.uint16) if fmt == "p010" else (torch.uint8,)
+        dtypes = (torch.uint8, torch.uint16) if fmt in WIDE_FORMATS else (torch.uint8,)
 
         if out is None:
             pitch = (row_bytes + align - 1) // align * align
@@ -900,12 +908,13 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
         fmt "rgba" / "bgra" ([h, w, 4] per frame; over=True composites over `background` as GLava's window shows it) or
         "nv12" ([h * 3 / 2, w]: Y rows, then interleaved CbCr rows), "p010" (the same as uint16 samples, 10-bit code << 6),
         "i420" / "yuv444" (a tuple of plane views Y [h, w], Cb and Cr [h / 2, w / 2] or [h, w] of one back-to-back
-        allocation); the YUV formats are always composited.  out: see _export_plan; None allocates [count, ...] of those
-        shapes (rows padded to a multiple of 16 bytes, 32 for I420).  Returns out.
+        allocation), "yuv420p10" / "yuv444p10" (the same planes as uint16 samples holding the 10-bit code in their low bits:
+        ffmpeg's yuv420p10le / yuv444p10le); the YUV formats are always composited.  out: see _export_plan; None allocates
+        [count, ...] of those shapes (rows padded to a multiple of 16 bytes, 32 for I420 and YUV420P10).  Returns out.
         after / done: torch.cuda.Event or cudaEvent_t handles — the export waits for `after` on the device and records
         `done` behind itself.  Left None, the export is ordered after the work already queued on torch's current stream,
         and that stream waits for the export (the tensors can be used right away).
-        matrix ("bt709" / "bt601") and full_range: the Y'CbCr encoding of NV12, I420, YUV444 and P010 (DESIGN 4.15; the
+        matrix ("bt709" / "bt601") and full_range: the Y'CbCr encoding of every YUV format (DESIGN 4.15; the
         default is BT.709 limited range; matrix="bt601", full_range=True is JPEG's)."""
         s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, lambda stream: self.device, None, matrix,
                                                  full_range)
@@ -930,7 +939,7 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
                       done=None, matrix="bt709", full_range=False):
         """export_frames of a source rectangle shrunk to size = (w, h) by the exact area average (glava_b200_export_scaled):
         crop = (x, y, w, h) in top-down coordinates (y = 0 is the top row), None: the whole frame.  Downscale only; NV12,
-        I420 and P010 need an even w and h.  Shapes, out, after, done, matrix and full_range as export_frames, with the output
+        I420, P010 and YUV420P10 need an even w and h.  Shapes, out, after, done, matrix and full_range as export_frames, with the output
         size in place of the frame's."""
         s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, lambda stream: self.device, size, matrix,
                                                  full_range)
@@ -965,11 +974,12 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
         """The frames of `streams` shrunk to tile = (w, h) and laid out row-major, `cols` tiles per row, in one picture, by
         one export_scaled call with a destination and a chroma destination per tile.  W = cols * w, H = rows * h; returns
         [H * 3 / 2, W] for NV12 (uint8) and P010 (uint16), Y rows then CbCr rows, the plane views (Y, Cb, Cr) for I420 and
-        YUV444, or [H, W, 4]: one surface to hand to an encoder.  Tiles start at multiples of 16 bytes in every plane, so w
-        is a multiple of 16 (NV12, YUV444), 32 (I420), 8 (P010) or 4 (RGBA / BGRA).  out: a CUDA tensor [rows, pitch] whose
-        rows hold the picture's row bytes, rows as _export_layout gives them for W x H (I420 / YUV444: the chroma planes
-        back to back from row H); tiles past the last stream keep its bytes (out None: black).  Ordered against torch's
-        current stream as export_frames without events.  matrix / full_range as export_frames (black: Y 0 in full range)."""
+        YUV444 (uint8) and YUV420P10 and YUV444P10 (uint16), or [H, W, 4]: one surface to hand to an encoder.  Tiles start
+        at multiples of 16 bytes in every plane, so w is a multiple of 16 (NV12, YUV444, YUV420P10), 32 (I420), 8 (P010,
+        YUV444P10) or 4 (RGBA / BGRA).  out: a CUDA tensor [rows, pitch] whose rows hold the picture's row bytes, rows as
+        _export_layout gives them for W x H (planar formats: the chroma planes back to back from row H); tiles past the last
+        stream keep its bytes (out None: black).  Ordered against torch's current stream as export_frames without events.
+        matrix / full_range as export_frames (black: Y 0 in full range)."""
         import torch
         s = np.ascontiguousarray(np.asarray(streams, dtype=np.int64).reshape(-1), dtype=np.int32)
         count, cols = int(s.shape[0]), int(cols)
@@ -979,13 +989,16 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
         desc = _export_desc(fmt, False, background, matrix, full_range)
         W, H = cols * tw, (count + cols - 1) // cols * th
         rows, row_bytes, align = _export_layout(fmt, W, H)
-        px = {"rgba": 4, "bgra": 4, "p010": 2}.get(fmt, 1)
+        px = {"rgba": 4, "bgra": 4}.get(fmt, 2 if fmt in WIDE_FORMATS else 1)
         if out is None:
             base = torch.empty((rows, (row_bytes + align - 1) // align * align), dtype=torch.uint8, device=f"cuda:{self.device}")
             if count % cols:                                  # black where no stream lands
                 if fmt == "p010":
                     base.view(torch.uint16)[:H].fill_(0 if full_range else 64 << 6)
                     base.view(torch.uint16)[H:].fill_(512 << 6)
+                elif fmt in ("yuv420p10", "yuv444p10"):
+                    base.view(torch.uint16)[:H].fill_(0 if full_range else 64)
+                    base.view(torch.uint16)[H:].fill_(512)
                 elif fmt in ("rgba", "bgra"):
                     base.fill_(0)
                 else:
@@ -993,7 +1006,7 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
                     base[H:].fill_(128)
             result = _export_views(fmt, base, W, H)
         else:
-            dtypes = (torch.uint8, torch.uint16) if fmt == "p010" else (torch.uint8,)
+            dtypes = (torch.uint8, torch.uint16) if fmt in WIDE_FORMATS else (torch.uint8,)
             if (out.dtype not in dtypes or not out.is_cuda or out.dim() != 2 or out.shape[0] != rows or out.stride(1) != 1
                     or out.shape[1] * out.element_size() < row_bytes):
                 raise ValueError(f"out: a uint8 CUDA tensor [{rows}, >= {row_bytes}] with contiguous rows")
@@ -1002,11 +1015,11 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
         dst = (C.c_void_p * count)(*[ptr + (i // cols) * th * pitch + (i % cols) * tw * px for i in range(count)])
         if fmt in ("nv12", "p010"):
             uv = [ptr + (H + (i // cols) * (th // 2)) * pitch + (i % cols) * tw * px for i in range(count)]
-        elif fmt == "i420":                                   # Cr one whole chroma plane past Cb
-            uv = [ptr + H * pitch + (i // cols) * (th // 2) * (pitch // 2) + (i % cols) * (tw // 2) for i in range(count)]
+        elif fmt in ("i420", "yuv420p10"):                    # Cr one whole chroma plane past Cb
+            uv = [ptr + H * pitch + (i // cols) * (th // 2) * (pitch // 2) + (i % cols) * (tw // 2) * px for i in range(count)]
             desc.uv_offset = (pitch // 2) * (H // 2)
-        elif fmt == "yuv444":
-            uv = [ptr + (H + (i // cols) * th) * pitch + (i % cols) * tw for i in range(count)]
+        elif fmt in ("yuv444", "yuv444p10"):
+            uv = [ptr + (H + (i // cols) * th) * pitch + (i % cols) * tw * px for i in range(count)]
             desc.uv_offset = pitch * H
         else:
             uv = None

@@ -28,6 +28,8 @@ const char* format_name(int format) {
     case GLAVA_B200_EXPORT_I420: return "I420";
     case GLAVA_B200_EXPORT_YUV444: return "YUV444";
     case GLAVA_B200_EXPORT_P010: return "P010";
+    case GLAVA_B200_EXPORT_YUV420P10: return "YUV420P10";
+    case GLAVA_B200_EXPORT_YUV444P10: return "YUV444P10";
     default: return nullptr;
     }
 }
@@ -38,12 +40,13 @@ int desc_size(int w, int h, const glava_b200_export& d, const char* what, const 
     const char* name = format_name(fmt);
     if (export_420(fmt) && ((w | h) & 1))
         return fail(GLAVA_B200_EINVAL, "%s: %s needs an even width and height, the %s is %dx%d", who, name, what, w, h);
-    const size_t row = !export_yuv(fmt) ? (size_t) w * 4 : fmt == GLAVA_B200_EXPORT_P010 ? (size_t) w * 2 : (size_t) w;
+    const size_t row = !export_ycbcr(fmt) ? (size_t) w * 4
+                       : fmt == GLAVA_B200_EXPORT_P010 || export_p10(fmt) ? (size_t) w * 2 : (size_t) w;
     if (d.pitch % 16 || d.pitch < row)
         return fail(GLAVA_B200_EINVAL, "%s: pitch %zu must be a multiple of 16 and at least %zu", who, d.pitch, row);
-    if (fmt == GLAVA_B200_EXPORT_I420 && d.pitch % 32)
-        return fail(GLAVA_B200_EINVAL, "%s: I420 pitch %zu must be a multiple of 32, so that chroma rows (pitch / 2) stay 16-byte "
-                    "aligned", who, d.pitch);
+    if ((fmt == GLAVA_B200_EXPORT_I420 || fmt == GLAVA_B200_EXPORT_YUV420P10) && d.pitch % 32)
+        return fail(GLAVA_B200_EINVAL, "%s: %s pitch %zu must be a multiple of 32, so that chroma rows (pitch / 2) stay 16-byte "
+                    "aligned", who, name, d.pitch);
     if ((fmt == GLAVA_B200_EXPORT_NV12 || fmt == GLAVA_B200_EXPORT_P010) &&
         (d.uv_offset % 16 || (d.uv_offset && d.uv_offset < d.pitch * (size_t) h)))
         return fail(GLAVA_B200_EINVAL, "%s: uv_offset %zu must be a multiple of 16 and at least pitch * h = %zu (or 0)", who,
@@ -61,17 +64,17 @@ int desc_size(int w, int h, const glava_b200_export& d, const char* what, const 
 int desc_check(ExportKind kind, int w, int h, const glava_b200_export& d, const glava_b200_export_scale* s,
                glava_b200_export_scale* q, const char* who) {
     if (!format_name(d.format)) return fail(GLAVA_B200_EINVAL, "%s: unknown format %d", who, d.format);
-    if (kind == ExportKind::overlay && d.format != GLAVA_B200_EXPORT_NV12 && export_yuv(d.format))
+    if (kind == ExportKind::overlay && d.format != GLAVA_B200_EXPORT_NV12 && export_ycbcr(d.format))
         return fail(GLAVA_B200_EINVAL, "%s: format %s: the overlay takes RGBA, BGRA or NV12", who, format_name(d.format));
     // the colour bits (DESIGN 4.15) are flags of the Y'CbCr formats only
     const uint32_t colour = GLAVA_B200_EXPORT_FULL_RANGE | GLAVA_B200_EXPORT_BT601;
     if (d.flags & ~(GLAVA_B200_EXPORT_OVER | colour)) return fail(GLAVA_B200_EINVAL, "%s: unknown flags 0x%x", who, d.flags);
-    if ((d.flags & colour) && !export_yuv(d.format))
+    if ((d.flags & colour) && !export_ycbcr(d.format))
         return fail(GLAVA_B200_EINVAL, "%s: flags 0x%x: %s has no matrix or range (EXPORT_FULL_RANGE and EXPORT_BT601 are for the "
                     "Y'CbCr formats)", who, d.flags, format_name(d.format));
     if (kind == ExportKind::overlay && (d.flags & ~colour))
         return fail(GLAVA_B200_EINVAL, "%s: flags 0x%x: the overlay takes none%s", who, d.flags,
-                    export_yuv(d.format) ? " but EXPORT_FULL_RANGE and EXPORT_BT601" : "");
+                    export_ycbcr(d.format) ? " but EXPORT_FULL_RANGE and EXPORT_BT601" : "");
     *q = { 0, 0, w, h, w, h };
     if (kind != ExportKind::scaled) return desc_size(w, h, d, "frame", who);
     if (!s) return fail(GLAVA_B200_EINVAL, "%s: null scale", who);
@@ -112,7 +115,7 @@ int output_bytes(ExportKind kind, const glava_b200* r, const glava_b200_export* 
     if (rc) return rc;
     const size_t h = (size_t) q.out_h;
     const ExportPlanes pl = export_planes(desc->format, desc->pitch, desc->uv_offset, q.out_h);
-    if (!export_yuv(desc->format)) *bytes = desc->pitch * h;
+    if (!export_ycbcr(desc->format)) *bytes = desc->pitch * h;
     else if (export_planar(desc->format)) *bytes = pl.cb + pl.cr + pl.plane;
     else *bytes = pl.cb + desc->pitch * (h / 2);
     return 0;
@@ -218,8 +221,9 @@ int export_check(ExportKind kind, glava_b200* r, const int* streams, int count, 
     glava_b200_export_scale local;
     int rc = desc_check(kind, v.w, v.h, *desc, scale, q ? q : &local, who);
     if (rc) return rc;
-    if (dst_uv && !export_yuv(desc->format))
-        return fail(GLAVA_B200_EINVAL, "%s: dst_uv is for NV12 only, or I420, YUV444 and P010: %s has no chroma plane", who,
+    if (dst_uv && !export_ycbcr(desc->format))
+        return fail(GLAVA_B200_EINVAL, "%s: dst_uv is for NV12 only, or I420, YUV444, P010, YUV420P10 and YUV444P10: %s has no "
+                    "chroma plane", who,
                     format_name(desc->format));
     if (count < 1) return fail(GLAVA_B200_EINVAL, "%s: count %d < 1", who, count);
     if (!streams || !dst) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
@@ -246,7 +250,7 @@ int export_run(ExportKind kind, glava_b200* r, const int* streams, int count, vo
         const size_t fb_bytes = (size_t) v.slots * (size_t) v.h * (size_t) v.w * 4;
         if ((rc = overlay_geometry_check(v.w, v.h, count, dst, dst_uv, *desc, &v.fb, &fb_bytes, 1, who)) != 0) return rc;
     }
-    const bool yuv = export_yuv(desc->format);
+    const bool yuv = export_ycbcr(desc->format);
     const ExportPlanes pl = export_planes(desc->format, desc->pitch, desc->uv_offset, q.out_h);
     CU(cudaSetDevice(v.device));
     // export_kernel's entries have no chroma pointer (its machine code stays as measured); the others carry one per entry

@@ -146,20 +146,28 @@ GLB_HD bool export_yuv(int format) {                   // a format with chroma p
     return format == GLAVA_B200_EXPORT_NV12 || format == GLAVA_B200_EXPORT_I420 || format == GLAVA_B200_EXPORT_YUV444 ||
            format == GLAVA_B200_EXPORT_P010;
 }
+// The planar 10-bit formats (DESIGN 4.16) run kernels of their own, so export_yuv, which the existing ladder kernels evaluate
+// at run time, does not name them; the host checks take export_ycbcr, every format with chroma planes
+GLB_HD bool export_p10(int format) { return format == GLAVA_B200_EXPORT_YUV420P10 || format == GLAVA_B200_EXPORT_YUV444P10; }
+GLB_HD bool export_ycbcr(int format) { return export_yuv(format) || export_p10(format); }
 GLB_HD bool export_420(int format) {                   // chroma per 2x2 block: w and h even, items are row pairs
-    return format == GLAVA_B200_EXPORT_NV12 || format == GLAVA_B200_EXPORT_I420 || format == GLAVA_B200_EXPORT_P010;
+    return format == GLAVA_B200_EXPORT_NV12 || format == GLAVA_B200_EXPORT_I420 || format == GLAVA_B200_EXPORT_P010 ||
+           format == GLAVA_B200_EXPORT_YUV420P10;
 }
-GLB_HD bool export_planar(int format) { return format == GLAVA_B200_EXPORT_I420 || format == GLAVA_B200_EXPORT_YUV444; }
+GLB_HD bool export_planar(int format) {
+    return format == GLAVA_B200_EXPORT_I420 || format == GLAVA_B200_EXPORT_YUV444 || export_p10(format);
+}
 
 // Where the chroma of a destination lies, from the descriptor and the output height: `cb`, the bytes from the luma to the
-// chroma plane (NV12 / P010: the CbCr plane, uv_offset or pitch * h; I420 / YUV444: the Cb plane, right after the luma);
-// `cr`, the bytes from Cb to Cr (planar only: uv_offset, or 0 for one chroma plane, back to back); `plane`, the bytes of
-// one planar chroma plane (I420: h / 2 rows of pitch / 2)
+// chroma plane (NV12 / P010: the CbCr plane, uv_offset or pitch * h; the planar formats: the Cb plane, right after the
+// luma); `cr`, the bytes from Cb to Cr (planar only: uv_offset, or 0 for one chroma plane, back to back); `plane`, the bytes
+// of one planar chroma plane (I420 / YUV420P10: h / 2 rows of pitch / 2)
 struct ExportPlanes { size_t cb, cr, plane; };
 GLB_HD ExportPlanes export_planes(int format, size_t pitch, size_t uv_offset, int h) {
     ExportPlanes p = { uv_offset ? uv_offset : pitch * (size_t) h, 0, 0 };
     if (export_planar(format)) {
-        p.plane = format == GLAVA_B200_EXPORT_I420 ? (pitch / 2) * (size_t) (h / 2) : pitch * (size_t) h;
+        p.plane = format == GLAVA_B200_EXPORT_I420 || format == GLAVA_B200_EXPORT_YUV420P10 ? (pitch / 2) * (size_t) (h / 2)
+                                                                                             : pitch * (size_t) h;
         p.cb = pitch * (size_t) h;
         p.cr = uv_offset ? uv_offset : p.plane;
     }
@@ -262,6 +270,63 @@ GLB_HD ExportZero export_zero(const ExportFmt& f) {
         o.u = export_cb_pair(uv); o.v = export_cr_pair(uv);
     }
     return o;
+}
+
+// ---- planar 10-bit: yuv420p10le and yuv444p10le (DESIGN 4.16) -------------------------------------------------------------
+// Little-endian uint16 samples holding the 10-bit code in their low bits.  Y is export_y10 (P010's code without the << 6).
+// 4:2:0 chroma is P010's, export_cbcr10 of the exact block sums.  4:4:4 chroma is export_cbcr10 of the pixel's channels
+// times 4, the sums of a 2x2 block of that pixel: with X = coef c + (off << 16), (4 X + 2^17) >> 18 = (X + 2^15) >> 16, the
+// per-pixel 10-bit code, so no new rounding enters.
+template <int E = 0>
+GLB_HD uint32_t export_cbcr10_px(uint32_t c) {
+    const uint32_t s = (c & 255u) | (((c >> 8) & 255u) << 10) | (((c >> 16) & 255u) << 20);
+    return export_cbcr10<E>(s << 2);
+}
+// yuv420p10le of a quad of output rows 2j (top) and 2j + 1 (bot): per row its four Y samples as two words (two uint16
+// each), and the Cb samples and the Cr samples of the quad's two 2x2 blocks, one word each
+template <int E = 0>
+GLB_HD void export_i010_quad(const ExportFmt& f, const uint32_t top[4], const uint32_t bot[4], uint32_t yt[2], uint32_t yb[2],
+                             uint32_t* cb, uint32_t* cr) {
+    uint32_t t[4], b[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        t[k] = export_over(top[k], f.bg, f.native);
+        b[k] = export_over(bot[k], f.bg, f.native);
+    }
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+        yt[k] = export_y10<E>(t[2 * k]) | (export_y10<E>(t[2 * k + 1]) << 16);
+        yb[k] = export_y10<E>(b[2 * k]) | (export_y10<E>(b[2 * k + 1]) << 16);
+    }
+    const uint32_t c0 = export_cbcr10<E>(export_sum4(t[0], t[1], b[0], b[1]));
+    const uint32_t c1 = export_cbcr10<E>(export_sum4(t[2], t[3], b[2], b[3]));
+    *cb = (c0 & 0xffffu) | (c1 << 16);
+    *cr = (c0 >> 16) | (c1 & 0xffff0000u);
+}
+// yuv444p10le of one row's quad: the Y, Cb and Cr samples of each composited pixel, two words each
+template <int E = 0>
+GLB_HD void export_444p10_quad(const ExportFmt& f, const uint32_t in[4], uint32_t y[2], uint32_t cb[2], uint32_t cr[2]) {
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+        const uint32_t c0 = export_over(in[2 * k], f.bg, f.native), c1 = export_over(in[2 * k + 1], f.bg, f.native);
+        const uint32_t uv0 = export_cbcr10_px<E>(c0), uv1 = export_cbcr10_px<E>(c1);
+        y[k] = export_y10<E>(c0) | (export_y10<E>(c1) << 16);
+        cb[k] = (uv0 & 0xffffu) | (uv1 << 16);
+        cr[k] = (uv0 >> 16) | (uv1 & 0xffff0000u);
+    }
+}
+// export_zero of the planar 10-bit formats: y, one of a row's two equal luma words; u and v, the Cb and Cr words (YUV420P10:
+// the quad's two blocks; YUV444P10: one of a row's two equal words)
+template <int E = 0>
+GLB_HD ExportZero export_zero10(const ExportFmt& f) {
+    const uint32_t z[4] = { 0u, 0u, 0u, 0u };
+    uint32_t y[2], yb[2], u[2], v[2];
+    if (f.format == GLAVA_B200_EXPORT_YUV444P10) {
+        export_444p10_quad<E>(f, z, y, u, v);
+    } else {
+        export_i010_quad<E>(f, z, z, y, yb, &u[0], &v[0]);
+    }
+    return { y[0], u[0], v[0] };
 }
 
 // ---- mark-aware reads ----------------------------------------------------------------------------------------------------

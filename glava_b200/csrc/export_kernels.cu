@@ -14,7 +14,8 @@
 // Both take entries with a chroma pointer (ExportEntryUV); export_kernel keeps ExportEntry.  glava_b200_export_ladder
 // (DESIGN 4.13) is export_ladder_kernel: every rung of every entry in one launch, each unit run by the per-item body of
 // the rung's standalone kernel.  I420, YUV 4:4:4 and P010 (DESIGN 4.14) run kernels of their own with the same items
-// (export_yuv_kernel, export_scaled_yuv_kernel, export_ladder_yuv_kernel).  The host half is export.cpp.
+// (export_yuv_kernel, export_scaled_yuv_kernel, export_ladder_yuv_kernel), as do the planar 10-bit formats (DESIGN 4.16:
+// export_p10_kernel, export_scaled_p10_kernel, export_ladder_p10_kernel).  The host half is export.cpp.
 #include "internal.h"
 #include "export_core.h"
 
@@ -314,10 +315,114 @@ static void launch_yuv(const ExportArgs& a, unsigned blocks, cudaStream_t st) {
     else export_yuv_kernel<Index, GLAVA_B200_EXPORT_P010><<<blocks, 256, 0, st>>>(a);
 }
 
+// ---- planar 10-bit: YUV420P10 and YUV444P10 (DESIGN 4.16) -----------------------------------------------------------------
+// export_kernel's items again, with little-endian uint16 samples holding the 10-bit code in their low bits: YUV420P10 an
+// 8-byte Y store per row and a 4-byte Cb and a 4-byte Cr store (chroma rows pitch / 2 apart), YUV444P10 an 8-byte Y, Cb and
+// Cr store per row.  Past the last full quad YUV420P10 has an even width (the last two pixels of a row) and YUV444P10
+// stores sample by sample.  These kernels have no earlier form to keep, so all four encodings are instantiations of one
+// template.
+
+// f(std::integral_constant<int, E>()) for the encoding E = enc, 0..3
+template <typename F>
+static void for_any_enc(int enc, F&& f) {
+    if (enc == 0) f(std::integral_constant<int, 0>());
+    else for_enc(enc, f);
+}
+
+// the first n (1..4) uint16 samples of the words v[0], v[1] at p (n == 4: p is 8-byte aligned); the tail is written out,
+// since indexing v by a run-time sample number puts the words on the stack
+__device__ __forceinline__ void store_u16(uint8_t* p, const uint32_t v[2], int n) {
+    unsigned short* const q = reinterpret_cast<unsigned short*>(p);
+    if (n >= 4) {
+        __stcs(reinterpret_cast<uint2*>(p), make_uint2(v[0], v[1]));
+        return;
+    }
+    __stcs(q, (unsigned short) v[0]);
+    if (n > 1) __stcs(q + 1, (unsigned short) (v[0] >> 16));
+    if (n > 2) __stcs(q + 2, (unsigned short) v[1]);
+}
+
+// YUV444P10 of one row's quad: n samples of Y at py, Cb at pu and Cr cr bytes past it
+template <int E>
+__device__ __forceinline__ void store_444p10(const ExportFmt& f, const uint32_t q[4], uint8_t* py, uint8_t* pu, size_t cr, int n,
+                                             const ExportZero& z) {
+    uint32_t y[2] = { z.y, z.y }, u[2] = { z.u, z.u }, v[2] = { z.v, z.v };
+    if ((q[0] | q[1] | q[2] | q[3]) != 0u) export_444p10_quad<E>(f, q, y, u, v);
+    store_u16(py, y, n);
+    store_u16(pu, u, n);
+    store_u16(pu + cr, v, n);
+}
+
+// One item of export_p10_kernel (and of a ladder's whole-frame planar 10-bit rung), as yuv_item: the Cb plane at `cb`, Cr
+// `cr` bytes further; z what zero pixels become (export_zero10).  A reads w, h, marks, mark_rows and pitch.
+template <bool Keep, int E, typename A>
+__device__ __forceinline__ void p10_item(const A& a, const ExportFmt& f, int fmt, const uint32_t* frame, int slot, uint8_t* dst,
+                                         uint8_t* cb, size_t cr, int j, int strip, int x, const ExportZero& z) {
+    const int y0 = a.h - 1 - 2 * j, y1 = y0 - 1;
+    uint32_t top[4] = { 0u, 0u, 0u, 0u }, bot[4] = { 0u, 0u, 0u, 0u };
+    if (row_read(a, slot, y0, strip)) load_quad<Keep>(frame, a.w, y0, x, top);
+    if (y1 >= 0 && row_read(a, slot, y1, strip)) load_quad<Keep>(frame, a.w, y1, x, bot);
+    const size_t o = (size_t) (2 * j) * a.pitch + 2 * (size_t) x;
+    const bool full = x + 4 <= a.w;
+    if (fmt == GLAVA_B200_EXPORT_YUV444P10) {               // any w and h
+        const int n = full ? 4 : a.w - x;
+        store_444p10<E>(f, top, dst + o, cb + o, cr, n, z);
+        if (y1 >= 0) store_444p10<E>(f, bot, dst + o + a.pitch, cb + o + a.pitch, cr, n, z);
+        return;
+    }
+    uint32_t yt[2] = { z.y, z.y }, yb[2] = { z.y, z.y }, u = z.u, v = z.v;   // YUV420P10, w and h even
+    if ((top[0] | top[1] | top[2] | top[3] | bot[0] | bot[1] | bot[2] | bot[3]) != 0u) export_i010_quad<E>(f, top, bot, yt, yb, &u, &v);
+    uint8_t* const pu = cb + (size_t) j * (a.pitch >> 1) + x;   // x / 2 samples of 2 bytes
+    if (full) {
+        __stcs(reinterpret_cast<uint2*>(dst + o), make_uint2(yt[0], yt[1]));
+        __stcs(reinterpret_cast<uint2*>(dst + o + a.pitch), make_uint2(yb[0], yb[1]));
+        __stcs(reinterpret_cast<uint32_t*>(pu), u);
+        __stcs(reinterpret_cast<uint32_t*>(pu + cr), v);
+    } else {                                                // the last two pixels of a row
+        __stcs(reinterpret_cast<uint32_t*>(dst + o), yt[0]);
+        __stcs(reinterpret_cast<uint32_t*>(dst + o + a.pitch), yb[0]);
+        __stcs(reinterpret_cast<unsigned short*>(pu), (unsigned short) u);
+        __stcs(reinterpret_cast<unsigned short*>(pu + cr), (unsigned short) v);
+    }
+}
+
+template <typename Index, int Fmt, int E>
+__global__ void __launch_bounds__(256) export_p10_kernel(const __grid_constant__ ExportArgs a) {
+    const ExportFmt f = { Fmt, 1, a.native, a.bg };
+    const Index strips = (Index) ((a.w + 127) >> 7), per = strips * (Index) ((a.h + 1) >> 1);
+    const Index items = (Index) a.count * per;
+    const Index warps = (Index) (((size_t) gridDim.x * blockDim.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    const ExportZero z = export_zero10<E>(f);               // once per thread, as export_kernel's constants
+    for (Index it = (Index) (((size_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5); it < items; it += warps) {
+        const Index k = it / per, rem = it - k * per;
+        const int j = (int) (rem / strips), strip = (int) (rem - (Index) j * strips);
+        const int x = strip * 128 + lane * 4;
+        if (x >= a.w) continue;
+        const ExportEntry* e = a.list + k;
+        uint8_t* const dst = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst)));
+        const int slot = __ldg(&e->slot);
+        const uint32_t* frame = reinterpret_cast<const uint32_t*>(a.fb) + (size_t) slot * a.h * a.w;
+        p10_item<false, E>(a, f, Fmt, frame, slot, dst, dst + a.uv_offset, a.cr_offset, j, strip, x, z);
+    }
+}
+
+template <typename Index>
+static void launch_p10(const ExportArgs& a, unsigned blocks, cudaStream_t st) {
+    for_any_enc(a.enc, [&](auto e) {
+        constexpr int E = decltype(e)::value;
+        if (a.format == GLAVA_B200_EXPORT_YUV420P10) export_p10_kernel<Index, GLAVA_B200_EXPORT_YUV420P10, E><<<blocks, 256, 0, st>>>(a);
+        else export_p10_kernel<Index, GLAVA_B200_EXPORT_YUV444P10, E><<<blocks, 256, 0, st>>>(a);
+    });
+}
+
 int launch_export(const ExportArgs& a, void* stream) {
     const ExportGrid g = export_grid((uint64_t) a.count * (uint64_t) ((a.w + 127) >> 7) * (uint64_t) ((a.h + 1) >> 1));
     cudaStream_t st = (cudaStream_t) stream;
-    if (a.enc && a.format == GLAVA_B200_EXPORT_NV12) {
+    if (export_p10(a.format)) {
+        if (g.narrow) launch_p10<uint32_t>(a, g.blocks, st);
+        else launch_p10<uint64_t>(a, g.blocks, st);
+    } else if (a.enc && a.format == GLAVA_B200_EXPORT_NV12) {
         for_enc(a.enc, [&](auto e) {
             constexpr int E = decltype(e)::value;
             if (g.narrow) export_nv12_enc_kernel<uint32_t, E><<<g.blocks, 256, 0, st>>>(a);
@@ -521,11 +626,77 @@ static void launch_scaled_yuv(const ScaledArgs& a, unsigned blocks, cudaStream_t
     else export_scaled_yuv_kernel<Index, GLAVA_B200_EXPORT_P010><<<blocks, 256, 0, st>>>(a);
 }
 
+// One item of export_scaled_p10_kernel (and of a ladder's other planar 10-bit rungs), as scaled_yuv_item: output row u
+// (YUV420P10: rows 2u and 2u + 1, the chroma of each 2x2 block from the right neighbour by shuffle) at column X of the lane,
+// one uint16 sample per store.  The Cb plane is the entry's dst_uv, Cr `cr` bytes further; E the encoding.
+template <bool Keep, int E, typename A>
+__device__ __forceinline__ void scaled_p10_item(const A& a, const ExportFmt& f, int fmt, const ExportRecip& rcp, uint32_t zc,
+                                                size_t cr, const ExportEntryUV* e, int u, int X, int lane) {
+    const bool active = X < a.out_w;
+    const int slot = __ldg(&e->slot);
+    const uint32_t* frame = reinterpret_cast<const uint32_t*>(a.fb) + (size_t) slot * a.h * a.w;
+    const ExportSpan sx = export_span(active ? X : 0, a.src_w, a.out_w);
+    uint8_t* const dst = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst)));
+    uint8_t* const cb = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst_uv)));
+    if (fmt == GLAVA_B200_EXPORT_YUV444P10) {
+        const uint32_t px = scaled_px<Keep>(a, f, frame, slot, u, active, sx, rcp, zc);
+        if (!active) return;
+        const size_t o = (size_t) u * a.pitch + 2 * (size_t) X;
+        const uint32_t uv = export_cbcr10_px<E>(px);
+        __stcs(reinterpret_cast<unsigned short*>(dst + o), (unsigned short) export_y10<E>(px));
+        __stcs(reinterpret_cast<unsigned short*>(cb + o), (unsigned short) uv);
+        __stcs(reinterpret_cast<unsigned short*>(cb + cr + o), (unsigned short) (uv >> 16));
+        return;
+    }
+    // YUV420P10, out_w even: the whole 2x2 block is in this warp
+    const uint32_t top = scaled_px<Keep>(a, f, frame, slot, 2 * u, active, sx, rcp, zc);
+    const uint32_t bot = scaled_px<Keep>(a, f, frame, slot, 2 * u + 1, active, sx, rcp, zc);
+    const uint32_t top1 = __shfl_down_sync(0xffffffffu, top, 1), bot1 = __shfl_down_sync(0xffffffffu, bot, 1);
+    if (!active) return;
+    uint8_t* const r0 = dst + (size_t) (2 * u) * a.pitch + 2 * (size_t) X;
+    __stcs(reinterpret_cast<unsigned short*>(r0), (unsigned short) export_y10<E>(top));
+    __stcs(reinterpret_cast<unsigned short*>(r0 + a.pitch), (unsigned short) export_y10<E>(bot));
+    if (!(lane & 1)) {
+        const uint32_t uv = export_cbcr10<E>(export_sum4(top, top1, bot, bot1));
+        uint8_t* const pu = cb + (size_t) u * (a.pitch >> 1) + X;   // X / 2 samples of 2 bytes
+        __stcs(reinterpret_cast<unsigned short*>(pu), (unsigned short) uv);
+        __stcs(reinterpret_cast<unsigned short*>(pu + cr), (unsigned short) (uv >> 16));
+    }
+}
+
+template <typename Index, int Fmt, int E>
+__global__ void __launch_bounds__(256) export_scaled_p10_kernel(const __grid_constant__ ScaledArgs a) {
+    const ExportFmt f = { Fmt, 1, a.native, a.bg };
+    const ExportRecip rcp = { a.div_mul, a.div_shift };
+    const uint32_t zc = export_over(0u, f.bg, f.native);    // what a zero pixel becomes
+    const Index runs = (Index) ((a.out_w + 31) >> 5), per = runs * (Index) (Fmt == GLAVA_B200_EXPORT_YUV444P10 ? a.out_h : a.out_h >> 1);
+    const Index items = (Index) a.count * per;
+    const Index warps = (Index) (((size_t) gridDim.x * blockDim.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    for (Index it = (Index) (((size_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5); it < items; it += warps) {
+        const Index k = it / per, rem = it - k * per;
+        const int u = (int) (rem / runs), X = (int) (rem - (Index) u * runs) * 32 + lane;
+        scaled_p10_item<false, E>(a, f, Fmt, rcp, zc, a.cr_offset, a.list + k, u, X, lane);
+    }
+}
+
+template <typename Index>
+static void launch_scaled_p10(const ScaledArgs& a, unsigned blocks, cudaStream_t st) {
+    for_any_enc(a.enc, [&](auto e) {
+        constexpr int E = decltype(e)::value;
+        if (a.format == GLAVA_B200_EXPORT_YUV420P10) export_scaled_p10_kernel<Index, GLAVA_B200_EXPORT_YUV420P10, E><<<blocks, 256, 0, st>>>(a);
+        else export_scaled_p10_kernel<Index, GLAVA_B200_EXPORT_YUV444P10, E><<<blocks, 256, 0, st>>>(a);
+    });
+}
+
 int launch_export_scaled(const ScaledArgs& a, void* stream) {
     const uint64_t units = export_420(a.format) ? (uint64_t) (a.out_h >> 1) : (uint64_t) a.out_h;
     const ExportGrid g = export_grid((uint64_t) a.count * (uint64_t) ((a.out_w + 31) >> 5) * units);
     cudaStream_t st = (cudaStream_t) stream;
-    if (a.enc && a.format == GLAVA_B200_EXPORT_NV12) {
+    if (export_p10(a.format)) {
+        if (g.narrow) launch_scaled_p10<uint32_t>(a, g.blocks, st);
+        else launch_scaled_p10<uint64_t>(a, g.blocks, st);
+    } else if (a.enc && a.format == GLAVA_B200_EXPORT_NV12) {
         for_enc(a.enc, [&](auto e) {
             constexpr int E = decltype(e)::value;
             if (g.narrow) export_scaled_enc_kernel<uint32_t, E><<<g.blocks, 256, 0, st>>>(a);
@@ -668,15 +839,67 @@ __global__ void __launch_bounds__(256) export_ladder_yuv_kernel(const __grid_con
 template <typename Index>
 __global__ void __launch_bounds__(256) export_ladder_enc_kernel(const __grid_constant__ LadderArgs a) { ladder_enc_loop<Index>(a); }
 
+// One unit of a planar 10-bit rung of export_ladder_p10_kernel under encoding E: the item of its standalone kernel
+// (export_p10_kernel / export_scaled_p10_kernel), as ladder_item runs the other Y'CbCr rungs
+template <int E>
+__device__ __forceinline__ void ladder_p10_item(const LadderArgs& a, const LadderRung& g, const ExportEntryUV* e, int rung, int row,
+                                                int col, int lane) {
+    const RungView v = { a.fb, a.marks, a.mark_rows, a.w, a.h, g.format, g.pitch, g.src_x, g.src_y, g.src_w, g.src_h, g.out_w, g.out_h };
+    const ExportFmt f = { g.format, g.over, a.native, g.bg };
+    const size_t cr = a.yuv[rung].cr_offset;
+    if (g.whole) {
+        const int x = col * 128 + lane * 4;
+        if (x >= a.w) return;
+        uint8_t* const dst = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst)));
+        uint8_t* const cb = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst_uv)));
+        const int slot = __ldg(&e->slot);
+        const uint32_t* frame = reinterpret_cast<const uint32_t*>(a.fb) + (size_t) slot * a.h * a.w;
+        const ExportZero z = { a.yuv[rung].zy, a.yuv[rung].zu, a.yuv[rung].zv };
+        p10_item<true, E>(v, f, g.format, frame, slot, dst, cb, cr, row, col, x, z);
+    } else {
+        const ExportRecip rcp = { g.div_mul, g.div_shift };
+        scaled_p10_item<true, E>(v, f, g.format, rcp, g.zc, cr, e, row, col * 32 + lane, lane);
+    }
+}
+
+// Any format and encoding per rung, launched only when a rung is YUV420P10 or YUV444P10 (DESIGN 4.16): planar 10-bit
+// units run ladder_p10_item, the others ladder_item, each in its rung's encoding
+template <typename Index>
+__global__ void __launch_bounds__(256) export_ladder_p10_kernel(const __grid_constant__ LadderArgs a) {
+    const Index units = (Index) a.units, items = (Index) a.count * units;
+    const Index warps = (Index) (((size_t) gridDim.x * blockDim.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    for (Index it = (Index) (((size_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5); it < items; it += warps) {
+        const Index k = it / units;
+        const uint64_t unit = __ldg(reinterpret_cast<const unsigned long long*>(a.sched) + (it - k * units));
+        const int rung = ladder_unit_rung(unit), row = ladder_unit_row(unit), col = ladder_unit_col(unit);
+        const LadderRung& g = a.rung[rung];
+        const ExportEntryUV* e = a.list + (size_t) k * a.nrungs + rung;
+        if (export_p10(g.format)) {
+            if (g.enc == 1) ladder_p10_item<1>(a, g, e, rung, row, col, lane);
+            else if (g.enc == 2) ladder_p10_item<2>(a, g, e, rung, row, col, lane);
+            else if (g.enc == 3) ladder_p10_item<3>(a, g, e, rung, row, col, lane);
+            else ladder_p10_item<0>(a, g, e, rung, row, col, lane);
+        } else if (g.enc == 1) ladder_item<true, 1>(a, g, e, rung, row, col, lane);
+        else if (g.enc == 2) ladder_item<true, 2>(a, g, e, rung, row, col, lane);
+        else if (g.enc == 3) ladder_item<true, 3>(a, g, e, rung, row, col, lane);
+        else ladder_item<true, 0>(a, g, e, rung, row, col, lane);
+    }
+}
+
 int launch_export_ladder(const LadderArgs& a, void* stream) {
     const ExportGrid g = export_grid((uint64_t) a.count * (uint64_t) a.units);
-    bool yuv = false, enc = false;
+    bool yuv = false, enc = false, p10 = false;
     for (int j = 0; j < a.nrungs; ++j) {
         yuv |= a.rung[j].format != GLAVA_B200_EXPORT_NV12 && export_yuv(a.rung[j].format);
         enc |= a.rung[j].enc != 0;
+        p10 |= export_p10(a.rung[j].format);
     }
     cudaStream_t st = (cudaStream_t) stream;
-    if (enc) {
+    if (p10) {
+        if (g.narrow) export_ladder_p10_kernel<uint32_t><<<g.blocks, 256, 0, st>>>(a);
+        else export_ladder_p10_kernel<uint64_t><<<g.blocks, 256, 0, st>>>(a);
+    } else if (enc) {
         if (g.narrow) export_ladder_enc_kernel<uint32_t><<<g.blocks, 256, 0, st>>>(a);
         else export_ladder_enc_kernel<uint64_t><<<g.blocks, 256, 0, st>>>(a);
     } else if (yuv) {

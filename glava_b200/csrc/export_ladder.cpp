@@ -32,12 +32,13 @@ int ladder_check(glava_b200* r, const int* streams, int count, const glava_b200_
     for (int j = 0; j < nrungs; ++j) {
         char name[96];
         snprintf(name, sizeof(name), "%s: rung %d", who, j);
-        const bool yuv = export_yuv(rungs[j].desc.format);
+        const bool yuv = export_ycbcr(rungs[j].desc.format);
         for (int i = 0; i < count; ++i) {
             d[i] = dst[(size_t) i * nrungs + j];
             uv[i] = dst_uv ? dst_uv[(size_t) i * nrungs + j] : nullptr;
             if (uv[i] && !yuv)
-                return fail(GLAVA_B200_EINVAL, "%s: dst_uv[%d] is for NV12 only, or I420, YUV444 and P010 (entry %d)", name,
+                return fail(GLAVA_B200_EINVAL, "%s: dst_uv[%d] is for NV12 only, or I420, YUV444, P010, YUV420P10 and YUV444P10 "
+                            "(entry %d)", name,
                             i * nrungs + j, i);
         }
         rc = export_check(ExportKind::scaled, r, streams, count, d.data(), dst_uv && yuv ? uv.data() : nullptr, &rungs[j].desc,
@@ -47,13 +48,14 @@ int ladder_check(glava_b200* r, const int* streams, int count, const glava_b200_
     return 0;
 }
 
-// What zero pixels become in a rung under encoding E: NV12's zy / zuv into g, and export_zero for the other Y'CbCr formats
+// What zero pixels become in a rung under encoding E: NV12's zy / zuv into g, and export_zero (planar 10-bit: export_zero10)
+// for the other Y'CbCr formats
 template <int E>
 static ExportZero rung_zero(const ExportFmt& f, LadderRung* g) {
     const uint32_t zero4[4] = { 0u, 0u, 0u, 0u };
     uint32_t zy1;
     g->zuv = export_nv12_quad<E>(f, zero4, zero4, &g->zy, &zy1);
-    return export_zero<E>(f);
+    return export_p10(f.format) ? export_zero10<E>(f) : export_zero<E>(f);
 }
 
 // the device schedule for `geom`, built and uploaded on the raster stream when the geometry differs from the last ladder's
@@ -110,7 +112,7 @@ int ladder_run(glava_b200* r, const int* streams, int count, const glava_b200_ex
         for (int j = 0; j < nrungs; ++j) {
             const size_t e = (size_t) i * nrungs + j;
             uint8_t* const d = (uint8_t*) dst[e];
-            uint8_t* const uv = !export_yuv(rungs[j].desc.format) ? nullptr : dst_uv ? (uint8_t*) dst_uv[e] : d + planes[j].cb;
+            uint8_t* const uv = !export_ycbcr(rungs[j].desc.format) ? nullptr : dst_uv ? (uint8_t*) dst_uv[e] : d + planes[j].cb;
             host[e] = { d, uv, slot, 0 };
         }
     }
@@ -126,7 +128,7 @@ int ladder_run(glava_b200* r, const int* streams, int count, const glava_b200_ex
             const glava_b200_export& d = rungs[j].desc;
             LadderRung& g = a.rung[j];
             g.format = d.format;
-            g.over = export_yuv(d.format) || (d.flags & GLAVA_B200_EXPORT_OVER) ? 1 : 0;
+            g.over = export_ycbcr(d.format) || (d.flags & GLAVA_B200_EXPORT_OVER) ? 1 : 0;
             g.whole = geom[j].whole ? 1 : 0;
             g.bg = background(d);
             g.pitch = d.pitch;
@@ -139,7 +141,8 @@ int ladder_run(glava_b200* r, const int* streams, int count, const glava_b200_ex
             const ExportFmt f = { g.format, g.over, v.native, g.bg };
             g.zpx = export_px(f, 0u);
             g.zc = f.over ? export_over(0u, f.bg, f.native) : 0u;
-            // NV12's words, and I420's, YUV444's and P010's as export_yuv_kernel computes them, in the rung's encoding
+            // NV12's words, and the other Y'CbCr formats' as export_yuv_kernel / export_p10_kernel compute them, in the
+            // rung's encoding
             ExportZero z;
             switch (g.enc) {
             case 1: z = rung_zero<1>(f, &g); break;

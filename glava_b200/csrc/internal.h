@@ -205,17 +205,17 @@ struct ExportArgs {
     int    format, over, native;  // export_core.h ExportFmt
     uint32_t bg;
     size_t pitch, uv_offset;    // uv_offset: luma to chroma plane (export_core.h ExportPlanes cb)
-    size_t cr_offset;           // I420 / YUV444: Cb to Cr plane (ExportPlanes cr)
+    size_t cr_offset;           // planar formats: Cb to Cr plane (ExportPlanes cr)
     int    enc;                 // Y'CbCr encoding, export_core.h export_enc of the flags (0: BT.709 limited range)
 };
 // NV12, RGBA and BGRA run export_kernel; I420, YUV444 and P010 export_yuv_kernel; any other encoding than 0 the kernels'
-// instantiations for it (export_nv12_enc_kernel, export_yuv_enc_kernel)
+// instantiations for it (export_nv12_enc_kernel, export_yuv_enc_kernel); YUV420P10 and YUV444P10 export_p10_kernel
 int launch_export(const ExportArgs& a, void* stream);
 // The entry of the scaled export and the overlay: ExportEntry with a chroma pointer, so that one call can fill an NV12
 // mosaic, where each tile's chroma sits at a different offset from its luma
 struct alignas(8) ExportEntryUV {
     uint8_t* dst;               // output row 0 (RGBA / BGRA pixels, or Y samples)
-    uint8_t* dst_uv;            // NV12 / P010: CbCr row 0; I420 / YUV444: Cb row 0 (unused for RGBA / BGRA)
+    uint8_t* dst_uv;            // NV12 / P010: CbCr row 0; planar formats: Cb row 0 (unused for RGBA / BGRA)
     int      slot;              // framebuffer slot of the listed stream
     int      pad;
 };
@@ -238,7 +238,8 @@ struct ScaledArgs {
     int    enc;                 // as ExportArgs
 };
 // NV12, RGBA and BGRA run export_scaled_kernel; I420, YUV444 and P010 export_scaled_yuv_kernel; enc != 0 their
-// instantiations for it (export_scaled_enc_kernel, export_scaled_yuv_enc_kernel)
+// instantiations for it (export_scaled_enc_kernel, export_scaled_yuv_enc_kernel); YUV420P10 and YUV444P10
+// export_scaled_p10_kernel
 int launch_export_scaled(const ScaledArgs& a, void* stream);
 // export_kernels.cu: glava_b200_overlay_frames (DESIGN 4.12), one launch for the whole list, its own argument struct and
 // ExportEntryUV entries.  band = 1 (native opacity with marks): one warp per (entry, band of mark_rows rows, strip), else one per
@@ -278,11 +279,12 @@ struct LadderArgs {
     const uint64_t* sched;      // ladder_plan.h units, sorted by the first framebuffer row they read
     uint32_t units;
     LadderRung rung[GLAVA_B200_LADDER_MAX];
-    // I420 / YUV444 / P010 rungs: the Cb to Cr distance (ExportArgs cr_offset) and export_core.h export_zero of the rung
+    // Y'CbCr rungs but NV12: the Cb to Cr distance (ExportArgs cr_offset) and export_core.h export_zero (planar 10-bit:
+    // export_zero10) of the rung
     struct { size_t cr_offset; uint32_t zy, zu, zv; } yuv[GLAVA_B200_LADDER_MAX];
 };
 // export_ladder_kernel, or export_ladder_yuv_kernel when a rung is I420, YUV444 or P010, or export_ladder_enc_kernel when a
-// rung has an encoding other than 0
+// rung has an encoding other than 0, or export_ladder_p10_kernel when a rung is YUV420P10 or YUV444P10
 int launch_export_ladder(const LadderArgs& a, void* stream);
 // capi.cu, for export.cpp: what the frame export reads of a renderer, and the slot where it keeps its own per-renderer
 // state (*attach, released by *attach_free when the renderer is destroyed)

@@ -371,34 +371,41 @@ int   glava_b200_framebuffer_ipc(glava_b200* r, void* handle, size_t handle_byte
  *                              h / 2 rows x w / 2 (Cb, Cr) uint16 pairs, both at `pitch` (>= 2 w); each sample is the 10-bit
  *                              BT.709 limited-range code (or as the colour flags say) << 6; chroma from the exact per-channel sums of each composited
  *                              2x2 block (export_core.h); w and h even
- *   Where the chroma planes go: NV12 and P010 put the CbCr plane at `uv_offset` from dst[i] (0: pitch * h).  I420 and
- *   YUV444 put the Cb plane right after the luma, at dst[i] + pitch * h, and `uv_offset` is the distance from Cb to Cr (0: the
- *   Cb plane's own size, so the planes sit back to back as a yuv420p / yuv444p buffer does); when set it is at least one
- *   chroma plane.  All YUV formats are composited (EXPORT_OVER implied).
+ *     GLAVA_B200_EXPORT_YUV420P10  planar 10-bit 4:2:0 (ffmpeg's yuv420p10le): Y plane of h rows x w little-endian uint16 at
+ *                              `pitch` (>= 2 w), then the Cb and Cr planes of h / 2 rows x w / 2 uint16 at `pitch / 2`;
+ *                              each sample is the 10-bit code in its low bits (0..1023): P010's Y and chroma >> 6, bit for
+ *                              bit (DESIGN.md §4.16); w and h even, pitch a multiple of 32
+ *     GLAVA_B200_EXPORT_YUV444P10  planar 10-bit 4:4:4 (yuv444p10le): Y, Cb and Cr planes of h rows x w uint16 at `pitch`
+ *                              (>= 2 w), LSB-aligned; Y as YUV420P10's, Cb / Cr per composited pixel with no averaging
+ *   Where the chroma planes go: NV12 and P010 put the CbCr plane at `uv_offset` from dst[i] (0: pitch * h).  The planar
+ *   formats (I420, YUV444, YUV420P10, YUV444P10) put the Cb plane right after the luma, at dst[i] + pitch * h, and
+ *   `uv_offset` is the distance from Cb to Cr (0: the Cb plane's own size, so the planes sit back to back as a yuv420p /
+ *   yuv444p buffer does); when set it is at least one chroma plane.  All YUV formats are composited (EXPORT_OVER implied).
  *   GLAVA_B200_EXPORT_OVER     (implied for the YUV formats) the opaque colour GLava's window shows over `background` (RGB8,
  *                              byte 3 unused): under setopacity "native" (premultiply_alpha) C = min(255, c +
  *                              mul_norm8(bg, 255 - a)) per channel; under any other opacity the stored colour (the window
  *                              ignores alpha and the clear colour already stands in for the desktop).  Alpha becomes 255.
  *                              Without it RGBA / BGRA carry the stored pixels, alpha included.
- *   GLAVA_B200_EXPORT_FULL_RANGE, GLAVA_B200_EXPORT_BT601   the Y'CbCr encoding of NV12, I420, YUV444 and P010 (DESIGN.md
+ *   GLAVA_B200_EXPORT_FULL_RANGE, GLAVA_B200_EXPORT_BT601   the Y'CbCr encoding of every YUV format (DESIGN.md
  *                              §4.15).  Neither: BT.709 limited range.  BT601 takes Kr, Kb = 0.299, 0.114 for BT.709's
  *                              0.2126, 0.0722; FULL_RANGE writes Y = Y', C = 128 + P over 0..255 (10 bits: 1023/255 Y',
  *                              512 + 1023/255 P, clamped to 1023) for limited range's 16 + 219/255 Y', 128 + 224/255 P
  *                              (64 + 876/255 Y', 512 + 896/255 P).  Both: the JFIF encoding JPEG encoders take (nvJPEG's
  *                              YUV input, libjpeg-turbo's raw data, ffmpeg's yuvj420p).  Every grey has Cb = Cr = 128
  *                              (512).  RGBA / BGRA with either bit are GLAVA_B200_EINVAL (no matrix or range).
- *   dst[i], pitch and uv_offset are multiples of 16, pitch >= the row bytes, uv_offset (when set) >= pitch * h (I420 /
- *   YUV444: >= one chroma plane).  An unknown format or flag, odd NV12 / I420 / P010 dimensions, a misaligned or short pitch
- *   (I420: not a multiple of 32), a null, host or other-device dst, a stream out of range, count < 1 and a renderer a failed
- *   rebuild left unbuilt are GLAVA_B200_EINVAL with nothing enqueued.  Format 3 is unassigned.
+ *   dst[i], pitch and uv_offset are multiples of 16, pitch >= the row bytes, uv_offset (when set) >= pitch * h (planar
+ *   formats: >= one chroma plane).  An unknown format or flag, odd NV12 / I420 / P010 / YUV420P10 dimensions, a misaligned
+ *   or short pitch (I420, YUV420P10: not a multiple of 32), a null, host or other-device dst, a stream out of range, count
+ *   < 1 and a renderer a failed rebuild left unbuilt are GLAVA_B200_EINVAL with nothing enqueued.  Formats 3 and 9 and
+ *   above are unassigned.
  *   The work runs on the handle's stream (glava_b200_cuda_stream) after the latest raster pass and before the next one can
  *   overwrite a slot, so an update issued right after this call cannot change what it exports.  `after_event` (a
  *   cudaEvent_t, or NULL): the export waits for it on the device before writing the destinations — it holds back the
  *   handle's stream, and so the next raster pass, until then.  `done_event` (or NULL) is recorded after the export.
  *   Returns once the work is enqueued, without a host wait.
  *   glava_b200_export_bytes    the bytes one destination spans for `desc` on this renderer (pitch * h; NV12 / P010:
- *                              uv_offset + pitch * h / 2; I420 / YUV444: pitch * h + the Cb to Cr distance + one chroma
- *                              plane), after the same descriptor checks.
+ *                              uv_offset + pitch * h / 2; the planar formats: pitch * h + the Cb to Cr distance + one
+ *                              chroma plane), after the same descriptor checks.
  *   glava_b200_sharded_export_frames  the same with global stream indices, dst[i] on the device of the shard that owns
  *                              streams[i]; every index and pointer is checked before any shard starts, the shards issue
  *                              concurrently, and glava_b200_sharded_sync completes the work. */
@@ -408,16 +415,20 @@ int   glava_b200_framebuffer_ipc(glava_b200* r, void* handle, size_t handle_byte
 #define GLAVA_B200_EXPORT_I420 4
 #define GLAVA_B200_EXPORT_YUV444 5
 #define GLAVA_B200_EXPORT_P010 6
+#define GLAVA_B200_EXPORT_YUV420P10 7
+#define GLAVA_B200_EXPORT_YUV444P10 8
 #define GLAVA_B200_EXPORT_OVER 1u
 #define GLAVA_B200_EXPORT_FULL_RANGE 0x100u
 #define GLAVA_B200_EXPORT_BT601 0x200u
 typedef struct {
-    int      format;            /* GLAVA_B200_EXPORT_RGBA / _BGRA / _NV12 / _I420 / _YUV444 / _P010 */
+    int      format;            /* GLAVA_B200_EXPORT_RGBA / _BGRA / _NV12 / _I420 / _YUV444 / _P010 / _YUV420P10 /
+                                   _YUV444P10 */
     uint32_t flags;             /* GLAVA_B200_EXPORT_OVER, and for the Y'CbCr formats _FULL_RANGE / _BT601 */
     uint8_t  background[4];     /* R, G, B of the opaque background the composite uses; byte 3 unused */
-    size_t   pitch;             /* bytes from one output row to the next (every plane; I420 chroma rows: pitch / 2) */
-    size_t   uv_offset;         /* NV12 / P010: bytes from dst[i] to the CbCr plane, 0 = pitch * h; I420 / YUV444: bytes
-                                   from the Cb plane to the Cr plane, 0 = one chroma plane */
+    size_t   pitch;             /* bytes from one output row to the next (every plane; I420 / YUV420P10 chroma rows:
+                                   pitch / 2) */
+    size_t   uv_offset;         /* NV12 / P010: bytes from dst[i] to the CbCr plane, 0 = pitch * h; the planar formats:
+                                   bytes from the Cb plane to the Cr plane, 0 = one chroma plane */
 } glava_b200_export;
 int glava_b200_export_bytes(const glava_b200* r, const glava_b200_export* desc, size_t* bytes);
 int glava_b200_export_frames(glava_b200* r, const int* streams, int count, void* const* dst,
@@ -433,17 +444,18 @@ int glava_b200_export_frames(glava_b200* r, const int* streams, int count, void*
  *                              glava_b200_export_frames.  RGBA / BGRA without EXPORT_OVER average the stored channels
  *                              (premultiplied under native opacity); with it, and for NV12, each source pixel is composited
  *                              first and alpha is 255.  NV12 is the export's arithmetic on the scaled image (Y per pixel,
- *                              chroma per 2x2 output block), so out_w and out_h are even; I420, YUV444 and P010 likewise
- *                              apply their own arithmetic to the scaled image (out_w and out_h even for I420 and P010).
- *     dst[i]                   out_h rows of out_w * 4 bytes (RGBA / BGRA), out_w bytes (Y) or out_w uint16 (P010 Y),
- *                              `pitch` bytes apart
+ *                              chroma per 2x2 output block), so out_w and out_h are even; the other YUV formats likewise
+ *                              apply their own arithmetic to the scaled image (out_w and out_h even for I420, P010 and
+ *                              YUV420P10).
+ *     dst[i]                   out_h rows of out_w * 4 bytes (RGBA / BGRA), out_w bytes (Y) or out_w uint16 (P010 and
+ *                              the planar 10-bit formats' Y), `pitch` bytes apart
  *     dst_uv                   NV12 / P010: dst_uv[i] receives the out_h / 2 CbCr rows (a mosaic tile's chroma need not sit
  *                              at one offset from its luma); NULL: dst[i] + (uv_offset ? uv_offset : pitch * out_h).
- *                              I420 / YUV444: dst_uv[i] is the Cb plane, NULL: dst[i] + pitch * out_h; the Cr plane is
+ *                              Planar formats: dst_uv[i] is the Cb plane, NULL: dst[i] + pitch * out_h; the Cr plane is
  *                              uv_offset past it (0: the Cb plane's size), which lets a planar mosaic tile find its Cr rows
  *   Nothing outside each out_w x out_h rectangle and its chroma rows is written: pitch padding and neighbouring tiles keep
  *   their bytes.  dst[i], dst_uv[i], pitch and uv_offset are multiples of 16 (a mosaic tile starts at a multiple of 4 pixels
- *   in RGBA, of 16 in NV12).  Besides every refusal of glava_b200_export_frames (pitch and uv_offset measured against the
+ *   in RGBA, of 16 in NV12 and YUV420P10, of 8 in YUV444P10).  Besides every refusal of glava_b200_export_frames (pitch and uv_offset measured against the
  *   output), a null `scale`, a rectangle that is empty or leaves the frame, upscaling, odd NV12 output dimensions, a
  *   misaligned, null, host or other-device dst_uv[i], and dst_uv for RGBA / BGRA are GLAVA_B200_EINVAL with nothing enqueued.
  *   glava_b200_export_scaled_bytes   the bytes one destination spans (as glava_b200_export_bytes with out_h for h, dst_uv
@@ -508,7 +520,7 @@ int glava_b200_export_ladder(glava_b200* r, const int* streams, int count, const
  *   pixel leaves D exactly as it was, and rows the dirty-row marks skip and all-zero quads are neither read nor written.
  *   An opaque pixel gives exactly glava_b200_export_frames' bytes.  Under any other opacity GLava's window is opaque: the
  *   rectangle gets exactly what glava_b200_export_frames writes (RGBA / BGRA with EXPORT_OVER, or NV12).
- *   The overlay takes RGBA, BGRA and NV12; I420, YUV444 and P010 are refused by name.
+ *   The overlay takes RGBA, BGRA and NV12; I420, YUV444, P010, YUV420P10 and YUV444P10 are refused by name.
  *   Besides the refusals of glava_b200_export_scaled that apply (format, pitch, uv_offset, alignment, null / host /
  *   other-device dst or dst_uv, dst_uv for RGBA / BGRA, odd NV12 frames, stream range, count < 1, an unbuilt renderer),
  *   any other flag, a rectangle that meets the renderer's framebuffer array and two rectangles of one call that overlap (luma
