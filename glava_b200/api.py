@@ -131,6 +131,18 @@ class ExportRung(C.Structure):
     _fields_ = [("desc", Export), ("scale", ExportScale)]
 
 
+class Picture(C.Structure):
+    """glava_b200_picture: one entry's plane pointers, each at the frame rectangle's first sample: Y; CbCr (NV12, P010) or
+    Cb; Cr (the planar formats, else NULL)"""
+    _fields_ = [("plane", C.c_void_p * 3)]
+
+
+class OverlayPlanesDesc(C.Structure):
+    """glava_b200_overlay_planes_desc: the picture format (EXPORT_NV12, _I420, _YUV444, _P010, _YUV420P10, _YUV444P10), the
+    colour flags (EXPORT_FULL_RANGE / EXPORT_BT601), the luma pitch and the pitch of every chroma plane, in bytes"""
+    _fields_ = [("format", C.c_int), ("flags", C.c_uint32), ("pitch", C.c_size_t), ("chroma_pitch", C.c_size_t)]
+
+
 LADDER_MAX = 8
 EXPORT_RGBA, EXPORT_BGRA, EXPORT_NV12 = 0, 1, 2
 EXPORT_I420, EXPORT_YUV444, EXPORT_P010 = 4, 5, 6
@@ -142,6 +154,8 @@ EXPORT_FORMATS = {"rgba": EXPORT_RGBA, "bgra": EXPORT_BGRA, "nv12": EXPORT_NV12,
                   "yuv444": EXPORT_YUV444, "p010": EXPORT_P010, "yuv420p10": EXPORT_YUV420P10,
                   "yuv444p10": EXPORT_YUV444P10}
 OVERLAY_FORMATS = ("rgba", "bgra", "nv12")
+# the formats overlay_planes takes: decoded pictures, one tensor per plane (DESIGN 4.17)
+PLANES_FORMATS = ("nv12", "i420", "yuv444", "p010", "yuv420p10", "yuv444p10")
 # the formats whose samples are uint16, which also take uint16 `out` tensors
 WIDE_FORMATS = ("p010", "yuv420p10", "yuv444p10")
 
@@ -309,6 +323,8 @@ def lib():
     L.glava_b200_sharded_overlay_frames.argtypes = [vp, vp, i32, vp, vp, C.POINTER(Export)]
     L.glava_b200_export_ladder.argtypes = [vp, vp, i32, C.POINTER(ExportRung), i32, vp, vp, vp, vp]
     L.glava_b200_sharded_export_ladder.argtypes = [vp, vp, i32, C.POINTER(ExportRung), i32, vp, vp]
+    L.glava_b200_overlay_planes.argtypes = [vp, vp, i32, C.POINTER(Picture), C.POINTER(OverlayPlanesDesc), vp, vp]
+    L.glava_b200_sharded_overlay_planes.argtypes = [vp, vp, i32, C.POINTER(Picture), C.POINTER(OverlayPlanesDesc)]
     _lib = L
     # errors surface as Python exceptions; keep stderr quiet
     _quiet = C.CFUNCTYPE(None, cp)(lambda msg: None)
@@ -612,6 +628,99 @@ class _FrameExport:
         desc.pitch = pitch or 0
         arr = (C.c_void_p * max(count, 1))(*dst)
         return s, desc, arr, (C.c_void_p * max(count, 1))(*uv) if nv12 else None
+
+    def _planes_plan(self, streams, pictures, at, fmt, matrix="bt709", full_range=False):
+        """-> (stream list, OverlayPlanesDesc, Picture array) of an overlay onto decoded pictures (DESIGN 4.17).  pictures:
+        one tuple of plane tensors per entry (a tuple may repeat), or one tuple of batched [count, rows, cols] plane tensors;
+        a tuple is (Y, CbCr) for NV12 and P010, (Y, Cb, Cr) otherwise, each CUDA, uint8 (the 8-bit formats) or uint16 or
+        uint8 with doubled width (the 10-bit formats), with contiguous rows: Y [H, W], NV12 CbCr [H / 2, W] bytes, P010 CbCr
+        [H / 2, W] samples, I420 / YUV420P10 Cb and Cr [H / 2, W / 2], YUV444 / YUV444P10 Cb and Cr [H, W] (export_frames'
+        plane views).  Every luma plane has one pitch and every chroma plane one pitch.  at: (x, y) of each frame's top-left
+        in luma samples (None: (0, 0)).  Raises ValueError for a rectangle that leaves its picture, mixed pitches within a
+        plane kind, or a plane start that is not 16-byte aligned (the library refuses the rest)."""
+        import torch
+        if fmt not in PLANES_FORMATS:
+            raise ValueError(f"format {fmt!r}: overlay_planes takes one of {list(PLANES_FORMATS)} "
+                             "(RGBA and BGRA images go to overlay_frames)")
+        s = np.ascontiguousarray(np.asarray(streams, dtype=np.int64).reshape(-1), dtype=np.int32)
+        count = int(s.shape[0])
+        nplanes = 2 if fmt in ("nv12", "p010") else 3
+        sb = 2 if fmt in WIDE_FORMATS else 1                  # bytes per sample
+        c420 = fmt in ("nv12", "i420", "p010", "yuv420p10")
+
+        def describe(planes, what, batched):
+            """-> ([base address per plane], H, W, pitch, chroma pitch) of one picture (batched: of entry 0)"""
+            planes = tuple(planes)
+            if len(planes) != nplanes:
+                raise ValueError(f"{what}: {fmt} has {nplanes} planes, got {len(planes)}")
+            dims = 3 if batched else 2
+            bases, shapes, pitches = [], [], []
+            for p, t in enumerate(planes):
+                ok = t.dtype in ((torch.uint8, torch.uint16) if sb == 2 else (torch.uint8,))
+                if not ok or not t.is_cuda or t.dim() != dims:
+                    raise ValueError(f"{what}[{p}]: a {'uint16 or uint8' if sb == 2 else 'uint8'} CUDA tensor of {dims} "
+                                     f"dimensions (got {t.dtype} {tuple(t.shape)})")
+                if t.stride(-1) != 1:
+                    raise ValueError(f"{what}[{p}]: rows must be contiguous")
+                if batched and t.shape[0] != count:
+                    raise ValueError(f"{what}[{p}]: {count} pictures, got {t.shape[0]}")
+                bases.append(t.data_ptr())
+                shapes.append((t.shape[-2], t.shape[-1] * t.element_size()))   # rows, row bytes
+                pitches.append(t.stride(-2) * t.element_size())
+            H, W = shapes[0][0], shapes[0][1] // sb
+            crows = H // 2 if c420 else H
+            cbytes = {"nv12": W, "p010": 2 * W, "i420": W // 2, "yuv420p10": W, "yuv444": W, "yuv444p10": 2 * W}[fmt]
+            for p in range(1, nplanes):
+                if shapes[p][0] != crows or shapes[p][1] < cbytes:
+                    raise ValueError(f"{what}[{p}]: a {W}x{H} {fmt} picture has chroma planes of {crows} rows of {cbytes} "
+                                     f"bytes (got {shapes[p][0]} rows of {shapes[p][1]})")
+            if nplanes == 3 and pitches[1] != pitches[2]:
+                raise ValueError(f"{what}: Cb pitch {pitches[1]}, Cr pitch {pitches[2]}: one chroma pitch per call")
+            steps = [t.stride(0) * t.element_size() for t in planes] if batched else None
+            return bases, H, W, pitches[0], pitches[1], steps
+
+        if isinstance(pictures, (list, tuple)) and len(pictures) and isinstance(pictures[0], torch.Tensor):
+            bases, H, W, P, CP, steps = describe(pictures, "pictures", True)
+            ents = [([b + i * st for b, st in zip(bases, steps)], H, W, P, CP) for i in range(count)]
+        else:
+            seen, ents = {}, []
+            for i, pic in enumerate(pictures):
+                if id(pic) not in seen:
+                    seen[id(pic)] = describe(pic, f"pictures[{i}]", False)[:5]
+                ents.append(seen[id(pic)])
+        if len(ents) != count:
+            raise ValueError(f"pictures: {count} pictures, got {len(ents)}")
+        at = [(0, 0)] * count if at is None else [(int(x), int(y)) for x, y in at]
+        if len(at) != count:
+            raise ValueError(f"at: {count} positions, got {len(at)}")
+        w, h = self.params.w, self.params.h
+        arr = (Picture * max(count, 1))()
+        pitch = cpitch = None
+        for i, ((bases, H, W, P, CP), (x, y)) in enumerate(zip(ents, at)):
+            if pitch is None:
+                pitch, cpitch = P, CP
+            elif (P, CP) != (pitch, cpitch):
+                raise ValueError(f"pictures[{i}]: pitches {P} / {CP}, the others {pitch} / {cpitch}: one luma and one chroma "
+                                 "pitch per call")
+            if x < 0 or y < 0 or x + w > W or y + h > H:
+                raise ValueError(f"pictures[{i}]: the {w}x{h} frame at ({x}, {y}) leaves the {W}x{H} picture")
+            if c420 and (x % 2 or y % 2):
+                raise ValueError(f"pictures[{i}]: a {fmt} frame starts at an even (x, y), got ({x}, {y})")
+            cx, cy = (x // 2, y // 2) if c420 else (x, y)
+            cs = {"nv12": 2, "p010": 4, "i420": 1, "yuv420p10": 2}.get(fmt, sb)   # chroma bytes per chroma position
+            ptrs = [bases[0] + y * P + x * sb] + [bases[p] + cy * CP + cx * cs for p in range(1, nplanes)]
+            for p, a in enumerate(ptrs):
+                if a % 16:
+                    raise ValueError(f"pictures[{i}]: the frame at ({x}, {y}) starts plane {p} at an address that is not a "
+                                     "multiple of 16 bytes")
+            arr[i].plane = (C.c_void_p * 3)(*(ptrs + [None] * (3 - nplanes)))
+        desc = OverlayPlanesDesc()
+        desc.format = EXPORT_FORMATS[fmt]
+        if matrix not in EXPORT_MATRICES:
+            raise ValueError(f"matrix {matrix!r}: one of {sorted(EXPORT_MATRICES)}")
+        desc.flags = EXPORT_MATRICES[matrix] | (EXPORT_FULL_RANGE if full_range else 0)
+        desc.pitch, desc.chroma_pitch = pitch or 0, cpitch or 0
+        return s, desc, arr
 
 
 def _export_desc(fmt, over, background, matrix="bt709", full_range=False):
@@ -970,6 +1079,19 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
                                                                      a, d), after, done)
         return images
 
+    def overlay_planes(self, streams, pictures, at=None, fmt="i420", matrix="bt709", full_range=False, after=None, done=None):
+        """The current frames of `streams` composited in place onto decoded pictures, one tensor per plane
+        (glava_b200_overlay_planes): NV12, I420, YUV444, P010, YUV420P10 or YUV444P10, the planes of each picture at their
+        own addresses with one luma and one chroma pitch per call — ffmpeg's AVFrame planes, NVDEC surfaces, or what
+        export_frames returns.  Native opacity blends in Y'CbCr in the picture's encoding (matrix / full_range) as
+        overlay_frames blends NV12; any other opacity writes export_frames' bytes.  pictures and at: see _planes_plan;
+        rectangles of one call must not overlap in any plane.  after / done and the ordering against torch's current
+        stream as export_frames.  Returns pictures."""
+        s, desc, arr = self._planes_plan(streams, pictures, at, fmt, matrix, full_range)
+        self._ordered(lambda a, d: self._L.glava_b200_overlay_planes(self._h, s.ctypes.data, s.shape[0], arr, C.byref(desc), a, d),
+                      after, done)
+        return pictures
+
     def export_mosaic(self, streams, cols, tile, fmt="nv12", background=(0, 0, 0), out=None, matrix="bt709", full_range=False):
         """The frames of `streams` shrunk to tile = (w, h) and laid out row-major, `cols` tiles per row, in one picture, by
         one export_scaled call with a destination and a chroma destination per tile.  W = cols * w, H = rows * h; returns
@@ -1178,6 +1300,18 @@ class ShardedRenderer(_StreamState, _StreamStyles, _FrameExport):
             torch.cuda.current_stream(d).synchronize()
         _check(self._L.glava_b200_sharded_overlay_frames(self._h, s.ctypes.data, s.shape[0], dst, uv, C.byref(desc)))
         return images
+
+    def overlay_planes(self, streams, pictures, at=None, fmt="i420", matrix="bt709", full_range=False):
+        """Renderer.overlay_planes with global stream indices (glava_b200_sharded_overlay_planes), each picture on the device
+        of the shard that owns its stream.  Work queued on torch's current streams of those devices is waited for first;
+        the pictures are complete after sync()."""
+        import torch
+        device_of = self._device_of()
+        s, desc, arr = self._planes_plan(streams, pictures, at, fmt, matrix, full_range)
+        for d in sorted({device_of(int(x)) for x in s if 0 <= int(x) < self.batch}):
+            torch.cuda.current_stream(d).synchronize()
+        _check(self._L.glava_b200_sharded_overlay_planes(self._h, s.ctypes.data, s.shape[0], arr, C.byref(desc)))
+        return pictures
 
     def _device_of(self):
         """stream -> the CUDA device of the shard that owns it"""

@@ -90,20 +90,6 @@ int desc_check(ExportKind kind, int w, int h, const glava_b200_export& d, const 
     return desc_size(q->out_w, q->out_h, d, "output", who);
 }
 
-// a destination pointer: null, alignment, device memory, device
-int dst_check(const RendererView& v, const void* p, const char* name, int i, const char* who) {
-    if (!p || ((uintptr_t) p & 15))
-        return fail(GLAVA_B200_EINVAL, "%s: %s[%d] = %p is null or not 16-byte aligned", who, name, i, p);
-    cudaPointerAttributes at;
-    memset(&at, 0, sizeof(at));
-    if (cudaPointerGetAttributes(&at, p) != cudaSuccess) { cudaGetLastError(); at.type = cudaMemoryTypeUnregistered; }
-    if (at.type != cudaMemoryTypeDevice && at.type != cudaMemoryTypeManaged)
-        return fail(GLAVA_B200_EINVAL, "%s: %s[%d] = %p is not device memory", who, name, i, p);
-    if (at.device != v.device)
-        return fail(GLAVA_B200_EINVAL, "%s: %s[%d] is on device %d, the renderer on device %d", who, name, i, at.device, v.device);
-    return 0;
-}
-
 // the byte count of one destination of a call of `kind`
 int output_bytes(ExportKind kind, const glava_b200* r, const glava_b200_export* desc, const glava_b200_export_scale* scale,
                  size_t* bytes, const char* who) {
@@ -135,8 +121,22 @@ void common_args(Args& a, const RendererView& v, const void* d_list, int count, 
     a.pitch = d.pitch;
 }
 
-// One plane of one entry's rectangle: `rows` rows of the common row bytes, the common pitch apart, from byte address p
-struct Rect { uintptr_t p; size_t rows; int entry; bool uv; };
+}  // namespace
+
+namespace glb {
+// a destination pointer: null, alignment, device memory, device (export_list.h)
+int dst_check(const RendererView& v, const void* p, const char* name, int i, const char* who) {
+    if (!p || ((uintptr_t) p & 15))
+        return fail(GLAVA_B200_EINVAL, "%s: %s[%d] = %p is null or not 16-byte aligned", who, name, i, p);
+    cudaPointerAttributes at;
+    memset(&at, 0, sizeof(at));
+    if (cudaPointerGetAttributes(&at, p) != cudaSuccess) { cudaGetLastError(); at.type = cudaMemoryTypeUnregistered; }
+    if (at.type != cudaMemoryTypeDevice && at.type != cudaMemoryTypeManaged)
+        return fail(GLAVA_B200_EINVAL, "%s: %s[%d] = %p is not device memory", who, name, i, p);
+    if (at.device != v.device)
+        return fail(GLAVA_B200_EINVAL, "%s: %s[%d] is on device %d, the renderer on device %d", who, name, i, at.device, v.device);
+    return 0;
+}
 
 // Two rectangles of one pitch P and row bytes B, a starting first (a.p <= b.p): with q, m = divmod(b.p - a.p, P), b's row 0
 // meets a's row q when m < B and a's row q + 1 when P - m < B, and b's later rows meet a's later rows only if row 0 does
@@ -153,9 +153,6 @@ bool rect_meets_range(const Rect& r, size_t P, size_t B, uintptr_t f0, uintptr_t
     return k < r.rows && r.p + k * P < f1;
 }
 
-}  // namespace
-
-namespace glb {
 static void release_list(void* p) { delete static_cast<ExportList*>(p); }
 
 int list_room(const RendererView& v, size_t bytes, ExportList** out) {

@@ -513,5 +513,146 @@ GLB_HD bool overlay_band_pairs(int h, int b0, int lo, int hi, int* ja, int* jb) 
 }
 GLB_HD bool overlay_top_straddles(int h, int b1, int ja) { return h - 1 - 2 * ja >= b1; }
 
+// ---- overlay onto decoded pictures (DESIGN 4.17): I420, YUV 4:4:4 and the 10-bit formats ------------------------------------
+// 8-bit I420 is NV12's arithmetic (overlay_y, overlay_cbcr of the block's overlay_avg4); YUV 4:4:4 takes overlay_cbcr of
+// each pixel (the average of a 2x2 block of one pixel is that pixel).  10 bits build the same fraction at 10 bits:
+//   Y   = clamp((coef c + F + 2^15) >> 16),      F = floor((T 2^16 + 127) / 255),   T = off a + (255 - a) V_D <= 1023 * 255
+//   4:2:0 chroma from the block's exact sums S (export_sum4) and alpha sum S_a (0..1020), as P010's export chroma:
+//   C   = clamp((coef S + 4 G + 2^17) >> 18),    G = floor((T' 2^16 + 509) / 1020), T' = off S_a + (1020 - S_a) V_D
+//   4:4:4 chroma: the same of the pixel's channels and alpha times 4 (as export_cbcr10_px).
+// T 2^16 passes 2^32, so F and G are taken exactly in 32 bits from T = 255 q + r (T' = 1020 q + r): F = q 2^16 + floor((r
+// 2^16 + 127) / 255).  A zero pixel (block) gives V_D back, an opaque one (a = 255, S_a = 1020) export_y10 / export_cbcr10.
+// Accumulators are signed: |coef c| <= 262915 * 255 and F <= 1023 * 2^16 keep Y's under 2^28; |coef S| <= 131458 * 1020
+// and 4 G <= 1023 * 2^18 keep chroma's under 2^29.  Codes clamp to [0, 1023]: stored colours above their alpha (not
+// premultiplied) can leave the range, as they can at 8 bits (overlay_clamp).
+GLB_HD uint32_t overlay_frac10(uint32_t off, uint32_t a, uint32_t vd) {
+    const uint32_t t = off * a + (255u - a) * vd, q = t / 255u;
+    return (q << GLB_YUV_SHIFT) + (((t - 255u * q) << GLB_YUV_SHIFT) + 127u) / 255u;
+}
+GLB_HD uint32_t overlay_frac10_4(uint32_t off, uint32_t sa, uint32_t vd) {
+    const uint32_t t = off * sa + (1020u - sa) * vd, q = t / 1020u;
+    return (q << GLB_YUV_SHIFT) + (((t - 1020u * q) << GLB_YUV_SHIFT) + 509u) / 1020u;
+}
+GLB_HD uint32_t overlay_clamp10(int v) { return v < 0 ? 0u : v > 1023 ? 1023u : (uint32_t) v; }
+// the 10-bit Y code of pixel px (stored, premultiplied) over the code yd, in encoding E
+template <int E = 0>
+GLB_HD uint32_t overlay_y10(uint32_t px, uint32_t yd) {
+    constexpr YuvCoef S = yuv_enc(E, 10);
+    const int r = (int) (px & 255u), g = (int) ((px >> 8) & 255u), b = (int) ((px >> 16) & 255u);
+    const int t = (int) overlay_frac10((uint32_t) S.yoff, px >> 24, yd);
+    return overlay_clamp10((S.yr * r + S.yg * g + S.yb * b + t + GLB_YUV_HALF) >> GLB_YUV_SHIFT);
+}
+// the 10-bit (Cb, Cr) codes, Cb in the low 16 bits, of block sums s (export_sum4) with alpha sum sa over the codes cbd, crd
+template <int E = 0>
+GLB_HD uint32_t overlay_cbcr10(uint32_t s, uint32_t sa, uint32_t cbd, uint32_t crd) {
+    constexpr YuvCoef S = yuv_enc(E, 10);
+    const int r = (int) (s & 1023u), g = (int) ((s >> 10) & 1023u), b = (int) (s >> 20);
+    const int gb = (int) overlay_frac10_4((uint32_t) S.coff, sa, cbd), gr = (int) overlay_frac10_4((uint32_t) S.coff, sa, crd);
+    const int cb = (S.cbr * r + S.cbg * g + S.cbb * b + 4 * gb + (1 << 17)) >> 18;
+    const int cr = (S.crr * r + S.crg * g + S.crb * b + 4 * gr + (1 << 17)) >> 18;
+    return overlay_clamp10(cb) | (overlay_clamp10(cr) << 16);
+}
+GLB_HD uint32_t overlay_asum4(uint32_t a, uint32_t b, uint32_t c, uint32_t d) { return (a >> 24) + (b >> 24) + (c >> 24) + (d >> 24); }
+
+// A 10-bit sample of the caller's picture holds its code as v >> 6 (P010: Msb) or v & 1023 (planar); a blended sample is
+// written with the other bits zero, and a sample no non-zero pixel covers keeps all 16 bits.
+template <bool Msb> GLB_HD uint32_t overlay_code10(uint32_t v) { return Msb ? (v & 0xffffu) >> 6 : v & 1023u; }
+template <bool Msb> GLB_HD uint32_t overlay_sample10(uint32_t code) { return Msb ? code << 6 : code; }
+// Y of pixel px over sample v
+template <int E, bool Msb>
+GLB_HD uint32_t overlay_y10_sample(uint32_t px, uint32_t v) {
+    return px ? overlay_sample10<Msb>(overlay_y10<E>(px, overlay_code10<Msb>(v))) : v & 0xffffu;
+}
+// Y of pixels p0, p1 over a word of two samples (p0's low)
+template <int E, bool Msb>
+GLB_HD uint32_t overlay_y10_word(uint32_t p0, uint32_t p1, uint32_t v) {
+    return overlay_y10_sample<E, Msb>(p0, v) | (overlay_y10_sample<E, Msb>(p1, v >> 16) << 16);
+}
+// the (Cb, Cr) samples of a 2x2 block over the samples cb, cr: Cb low, Cr high
+template <int E, bool Msb>
+GLB_HD uint32_t overlay_block10(uint32_t p0, uint32_t p1, uint32_t p2, uint32_t p3, uint32_t cb, uint32_t cr) {
+    if ((p0 | p1 | p2 | p3) == 0u) return (cb & 0xffffu) | (cr << 16);
+    const uint32_t c = overlay_cbcr10<E>(export_sum4(p0, p1, p2, p3), overlay_asum4(p0, p1, p2, p3), overlay_code10<Msb>(cb),
+                                         overlay_code10<Msb>(cr));
+    return overlay_sample10<Msb>(c & 0xffffu) | (overlay_sample10<Msb>(c >> 16) << 16);
+}
+// the (Cb, Cr) samples of one pixel (4:4:4) over the samples cb, cr: a 2x2 block of that pixel
+template <int E, bool Msb>
+GLB_HD uint32_t overlay_px10(uint32_t px, uint32_t cb, uint32_t cr) { return overlay_block10<E, Msb>(px, px, px, px, cb, cr); }
+
+// I420 of a quad (rows 2j and 2j + 1) over the Y words yt / yb and the Cb and Cr pairs cb / cr (two bytes each): NV12's
+// overlay_nv12_quad on the interleaved pairs, so I420 is NV12 deinterleaved bit for bit
+template <int E = 0>
+GLB_HD void overlay_i420_quad(const uint32_t top[4], const uint32_t bot[4], uint32_t* yt, uint32_t* yb, uint32_t* cb, uint32_t* cr) {
+    uint32_t uv = (*cb & 0xffu) | ((*cr & 0xffu) << 8) | ((*cb & 0xff00u) << 8) | ((*cr & 0xff00u) << 16);
+    overlay_nv12_quad<E>(top, bot, yt, yb, &uv);
+    *cb = export_cb_pair(uv); *cr = export_cr_pair(uv);
+}
+// YUV 4:4:4 of one row's quad over the Y, Cb and Cr words (four bytes each)
+template <int E = 0>
+GLB_HD void overlay_444_quad(const uint32_t in[4], uint32_t* y, uint32_t* cb, uint32_t* cr) {
+    uint32_t oy = 0u, ou = 0u, ov = 0u;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        oy |= overlay_y<E>(in[k], (*y >> (8 * k)) & 255u) << (8 * k);
+        const uint32_t uv = overlay_cbcr<E>(in[k], ((*cb >> (8 * k)) & 255u) | (((*cr >> (8 * k)) & 255u) << 8));
+        ou |= (uv & 255u) << (8 * k);
+        ov |= (uv >> 8) << (8 * k);
+    }
+    *y = oy; *cb = ou; *cr = ov;
+}
+// P010 (Msb) or YUV420P10 of a quad over the Y words yt[2] / yb[2] (two samples each) and the chroma of its two blocks:
+// P010 uv[2], one (Cb, Cr) word per block; YUV420P10 uv[0] the two Cb samples, uv[1] the two Cr samples
+template <int E, bool Msb>
+GLB_HD void overlay_p10_quad(const uint32_t top[4], const uint32_t bot[4], uint32_t yt[2], uint32_t yb[2], uint32_t uv[2]) {
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+        yt[k] = overlay_y10_word<E, Msb>(top[2 * k], top[2 * k + 1], yt[k]);
+        yb[k] = overlay_y10_word<E, Msb>(bot[2 * k], bot[2 * k + 1], yb[k]);
+    }
+    if (Msb) {
+#pragma unroll
+        for (int k = 0; k < 2; ++k) uv[k] = overlay_block10<E, true>(top[2 * k], top[2 * k + 1], bot[2 * k], bot[2 * k + 1], uv[k], uv[k] >> 16);
+    } else {
+        // sample by sample: packing both blocks' results through overlay_block10's words let nvcc 12.9 (sm_90a) merge a
+        // kept Cr sample's bits into the blended one; tests/test_gpu_overlay_planes.py pins the result on the device
+        uint32_t cb[2], cr[2];
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+            cb[k] = (uv[0] >> (16 * k)) & 0xffffu;
+            cr[k] = (uv[1] >> (16 * k)) & 0xffffu;
+            if ((top[2 * k] | top[2 * k + 1] | bot[2 * k] | bot[2 * k + 1]) != 0u) {
+                const uint32_t c = overlay_cbcr10<E>(export_sum4(top[2 * k], top[2 * k + 1], bot[2 * k], bot[2 * k + 1]),
+                                                     overlay_asum4(top[2 * k], top[2 * k + 1], bot[2 * k], bot[2 * k + 1]),
+                                                     cb[k] & 1023u, cr[k] & 1023u);
+                cb[k] = c & 0xffffu;
+                cr[k] = c >> 16;
+            }
+        }
+        uv[0] = cb[0] | (cb[1] << 16);
+        uv[1] = cr[0] | (cr[1] << 16);
+    }
+}
+// YUV444P10 of one row's quad over the Y, Cb and Cr words y[2], cb[2], cr[2] (two samples each)
+template <int E = 0>
+GLB_HD void overlay_444p10_quad(const uint32_t in[4], uint32_t y[2], uint32_t cb[2], uint32_t cr[2]) {
+#pragma unroll
+    for (int k = 0; k < 2; ++k) y[k] = overlay_y10_word<E, false>(in[2 * k], in[2 * k + 1], y[k]);
+    // sample by sample, as overlay_p10_quad's planar chroma
+    uint32_t u[4], v[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        u[k] = (cb[k >> 1] >> (16 * (k & 1))) & 0xffffu;
+        v[k] = (cr[k >> 1] >> (16 * (k & 1))) & 0xffffu;
+        if (in[k]) {
+            const uint32_t c = overlay_cbcr10<E>(export_sum4(in[k], in[k], in[k], in[k]), 4u * (in[k] >> 24), u[k] & 1023u, v[k] & 1023u);
+            u[k] = c & 0xffffu;
+            v[k] = c >> 16;
+        }
+    }
+    cb[0] = u[0] | (u[1] << 16); cb[1] = u[2] | (u[3] << 16);
+    cr[0] = v[0] | (v[1] << 16); cr[1] = v[2] | (v[3] << 16);
+}
+
 }  // namespace glb
 #endif

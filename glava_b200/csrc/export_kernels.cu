@@ -968,8 +968,71 @@ __device__ __forceinline__ void overlay_nv12(const ExportFmt& f, bool native, ui
     }
 }
 
-__device__ __forceinline__ uint32_t overlay_mark(const OverlayArgs& a, int slot, int y, int strip) {
+template <typename A>
+__device__ __forceinline__ uint32_t overlay_mark(const A& a, int slot, int y, int strip) {
     return __ldg(a.marks + export_mark_index(slot, a.w, a.h, a.mark_rows, y, strip));
+}
+
+// The walk of overlay_loop below (its items and mark-aware reads) with what a format does to the destination left to Body,
+// for glava_b200_overlay_planes (DESIGN 4.17).  overlay_loop keeps its own written-out copy: run through this template,
+// ptxas orders the row-pair item's blocks differently, and overlay_kernel / overlay_enc_kernel keep their machine code.
+// Body (the destination of one entry):
+//   b.a                       the argument struct (fb, marks, mark_rows, list, count, w, h)
+//   Body::dst(e)              the entry's first plane
+//   b.pairs()                 band items walk output row pairs (4:2:0), else output rows
+//   b.row(e, dst, r, x, q)    native: the quad q at x onto output row r
+//   b.chroma(e)               the entry's chroma, loaded once per band item that walks pairs
+//   b.pair(dst, c, j, x, t, b)  native: the quads of output rows 2j and 2j + 1
+//   b.item(e, dst, u, x, t, b, y1)   a row-pair item: output rows 2u and 2u + 1 (framebuffer row y1 >= 0), any opacity
+template <typename Index, bool Band, typename Body>
+__device__ __forceinline__ void overlay_walk(const Body& b) {
+    const auto& a = b.a;
+    const int rows = Band ? a.mark_rows : 2;
+    const Index strips = (Index) ((a.w + 127) >> 7), per = strips * (Index) ((a.h + rows - 1) / rows);
+    const Index items = (Index) a.count * per;
+    const Index warps = (Index) (((size_t) gridDim.x * blockDim.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    for (Index it = (Index) (((size_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5); it < items; it += warps) {
+        const Index k = it / per, rem = it - k * per;
+        const int u = (int) (rem / strips), strip = (int) (rem - (Index) u * strips);
+        const int x = strip * 128 + lane * 4;
+        if (x >= a.w) continue;
+        const auto* e = a.list + k;
+        const int slot = __ldg(&e->slot);
+        const uint32_t* frame = reinterpret_cast<const uint32_t*>(a.fb) + (size_t) slot * a.h * a.w;
+        uint8_t* const dst = Body::dst(e);
+        if (Band) {                                         // native, marks: band u
+            const int b0 = u * rows, b1 = min(b0 + rows, a.h);
+            const uint32_t mark = overlay_mark(a, slot, b0, strip);
+            const int lo = max((int) (mark & 0xffffu), b0), hi = min((int) (mark >> 16), b1);
+            if (lo >= hi) continue;
+            if (!b.pairs()) {
+                for (int y = lo; y < hi; ++y) {
+                    uint32_t q[4];
+                    load_quad(frame, a.w, y, x, q);
+                    b.row(e, dst, a.h - 1 - y, x, q);
+                }
+                continue;
+            }
+            const auto c = b.chroma(e);
+            int ja, jb;
+            const uint32_t below = overlay_band_pairs(a.h, b0, lo, hi, &ja, &jb) ? overlay_mark(a, slot, b0 - 1, strip) : 0u;
+            if (overlay_top_straddles(a.h, b1, ja) && export_row_read(overlay_mark(a, slot, b1, strip), b1)) ++ja;
+            for (int j = ja; j < jb; ++j) {
+                const int y0 = a.h - 1 - 2 * j, y1 = y0 - 1;
+                uint32_t top[4] = { 0u, 0u, 0u, 0u }, bot[4] = { 0u, 0u, 0u, 0u };
+                if (y0 >= lo && y0 < hi) load_quad(frame, a.w, y0, x, top);
+                if (y1 >= b0 ? y1 >= lo && y1 < hi : export_row_read(below, y1)) load_quad(frame, a.w, y1, x, bot);
+                b.pair(dst, c, j, x, top, bot);
+            }
+        } else {                                            // output rows 2u, 2u + 1: framebuffer rows y0, y0 - 1
+            const int y0 = a.h - 1 - 2 * u, y1 = y0 - 1;
+            uint32_t top[4] = { 0u, 0u, 0u, 0u }, bot[4] = { 0u, 0u, 0u, 0u };
+            if (!a.marks || export_row_read(overlay_mark(a, slot, y0, strip), y0)) load_quad(frame, a.w, y0, x, top);
+            if (y1 >= 0 && (!a.marks || export_row_read(overlay_mark(a, slot, y1, strip), y1))) load_quad(frame, a.w, y1, x, bot);
+            b.item(e, dst, u, x, top, bot, y1);
+        }
+    }
 }
 
 template <typename Index, bool Band, int E>
@@ -1063,6 +1126,209 @@ int launch_overlay(const OverlayArgs& a, void* stream) {
         else overlay_kernel<uint64_t, false><<<g.blocks, 256, 0, st>>>(a);
     }
     return launch_status("overlay");
+}
+
+// ---- glava_b200_overlay_planes (DESIGN 4.17) -------------------------------------------------------------------------------
+// overlay_walk onto decoded pictures: per entry three plane pointers (OverlayPlanesEntry), one luma pitch and one
+// chroma pitch per call.  NV12 runs overlay_frames' own item body (overlay_nv12); I420, P010 and YUV420P10 walk row pairs as
+// NV12 does; YUV444 and YUV444P10 walk rows as RGBA does.  Native opacity blends (export_core.h overlay_*_quad) and leaves
+// all-zero quads alone; any other opacity writes export_frames' bytes of the format.  Tails: the last two pixels of a row
+// for the 4:2:0 formats (w even), sample by sample for the 4:4:4 ones.  One kernel per format and encoding.
+
+// the first n (1..4) bytes at p as a word (n == 4: p is 4-byte aligned)
+__device__ __forceinline__ uint32_t load_bytes(const uint8_t* p, int n) {
+    if (n >= 4) return __ldcs(reinterpret_cast<const uint32_t*>(p));
+    uint32_t v = 0u;
+    for (int k = 0; k < n; ++k) v |= (uint32_t) __ldcs(p + k) << (8 * k);
+    return v;
+}
+// the first n (1..4) uint16 samples at p as two words (n == 4: p is 8-byte aligned); as store_u16, written out
+__device__ __forceinline__ void load_u16(const uint8_t* p, uint32_t v[2], int n) {
+    if (n >= 4) {
+        const uint2 d = __ldcs(reinterpret_cast<const uint2*>(p));
+        v[0] = d.x; v[1] = d.y;
+        return;
+    }
+    const unsigned short* const q = reinterpret_cast<const unsigned short*>(p);
+    v[0] = __ldcs(q); v[1] = 0u;
+    if (n > 1) v[0] |= (uint32_t) __ldcs(q + 1) << 16;
+    if (n > 2) v[1] = __ldcs(q + 2);
+}
+
+template <int Fmt, int E>
+struct OverlayPlanesBody {
+    static constexpr bool k420 = Fmt == GLAVA_B200_EXPORT_NV12 || Fmt == GLAVA_B200_EXPORT_I420 || Fmt == GLAVA_B200_EXPORT_P010 ||
+                                 Fmt == GLAVA_B200_EXPORT_YUV420P10;
+    static constexpr bool kPlanar = Fmt == GLAVA_B200_EXPORT_I420 || Fmt == GLAVA_B200_EXPORT_YUV444 || Fmt == GLAVA_B200_EXPORT_YUV420P10 ||
+                                    Fmt == GLAVA_B200_EXPORT_YUV444P10;
+    struct Chroma { uint8_t* cb; uint8_t* cr; };
+    const OverlayPlanesArgs& a;
+    ExportFmt f;                                            // any other opacity: the stored colour, alpha 255
+    __device__ __forceinline__ explicit OverlayPlanesBody(const OverlayPlanesArgs& a_) : a(a_), f{ Fmt, 1, 0, 0u } {}
+    static __device__ __forceinline__ uint8_t* plane(const OverlayPlanesEntry* e, int p) {
+        return reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->plane[p])));
+    }
+    static __device__ __forceinline__ uint8_t* dst(const OverlayPlanesEntry* e) { return plane(e, 0); }
+    __device__ __forceinline__ bool pairs() const { return k420; }
+    __device__ __forceinline__ Chroma chroma(const OverlayPlanesEntry* e) const { return { plane(e, 1), kPlanar ? plane(e, 2) : nullptr }; }
+
+    // 4:4:4: the quad at x of output row r (native: blended, all zero: untouched)
+    __device__ __forceinline__ void row444(bool native, uint8_t* dst, Chroma c, int r, int x, const uint32_t q[4]) const {
+        if (native && (q[0] | q[1] | q[2] | q[3]) == 0u) return;
+        const int n = x + 4 <= a.w ? 4 : a.w - x;
+        if (Fmt == GLAVA_B200_EXPORT_YUV444) {
+            uint8_t* const py = dst + (size_t) r * a.pitch + x;
+            uint8_t* const pu = c.cb + (size_t) r * a.chroma_pitch + x;
+            uint8_t* const pv = c.cr + (size_t) r * a.chroma_pitch + x;
+            uint32_t y, u, v;
+            if (native) {
+                y = load_bytes(py, n); u = load_bytes(pu, n); v = load_bytes(pv, n);
+                overlay_444_quad<E>(q, &y, &u, &v);
+            } else {
+                export_444_quad<E>(f, q, &y, &u, &v);
+            }
+            store_bytes(py, y, n); store_bytes(pu, u, n); store_bytes(pv, v, n);
+        } else {                                            // YUV444P10
+            uint8_t* const py = dst + (size_t) r * a.pitch + 2 * (size_t) x;
+            uint8_t* const pu = c.cb + (size_t) r * a.chroma_pitch + 2 * (size_t) x;
+            uint8_t* const pv = c.cr + (size_t) r * a.chroma_pitch + 2 * (size_t) x;
+            uint32_t y[2], u[2], v[2];
+            if (native) {
+                load_u16(py, y, n); load_u16(pu, u, n); load_u16(pv, v, n);
+                overlay_444p10_quad<E>(q, y, u, v);
+            } else {
+                export_444p10_quad<E>(f, q, y, u, v);
+            }
+            store_u16(py, y, n); store_u16(pu, u, n); store_u16(pv, v, n);
+        }
+    }
+    // 4:2:0: the quads at x of output rows 2j and 2j + 1 (native: blended, all eight pixels zero: untouched)
+    __device__ __forceinline__ void pair420(bool native, uint8_t* dst, Chroma c, int j, int x, const uint32_t top[4],
+                                            const uint32_t bot[4]) const {
+        uint8_t* const r0 = dst + (size_t) (2 * j) * a.pitch;
+        uint8_t* const cj = c.cb + (size_t) j * a.chroma_pitch;
+        if (Fmt == GLAVA_B200_EXPORT_NV12) {
+            overlay_nv12<E>(f, native, r0, cj, a.pitch, x, a.w, top, bot);
+            return;
+        }
+        if (native && (top[0] | top[1] | top[2] | top[3] | bot[0] | bot[1] | bot[2] | bot[3]) == 0u) return;
+        const bool full = x + 4 <= a.w;                     // else w even: the last two pixels of a row
+        if (Fmt == GLAVA_B200_EXPORT_I420) {
+            uint8_t* const pu = cj + (x >> 1);
+            uint8_t* const pv = c.cr + (size_t) j * a.chroma_pitch + (x >> 1);
+            uint32_t yt, yb, u, v;
+            if (native) {
+                yt = load_bytes(r0 + x, full ? 4 : 2); yb = load_bytes(r0 + a.pitch + x, full ? 4 : 2);
+                u = load_bytes(pu, full ? 2 : 1); v = load_bytes(pv, full ? 2 : 1);
+                overlay_i420_quad<E>(top, bot, &yt, &yb, &u, &v);
+            } else {
+                const uint32_t uv = export_nv12_quad<E>(f, top, bot, &yt, &yb);
+                u = export_cb_pair(uv); v = export_cr_pair(uv);
+            }
+            if (full) {
+                __stcs(reinterpret_cast<uint32_t*>(r0 + x), yt);
+                __stcs(reinterpret_cast<uint32_t*>(r0 + a.pitch + x), yb);
+                __stcs(reinterpret_cast<unsigned short*>(pu), (unsigned short) u);
+                __stcs(reinterpret_cast<unsigned short*>(pv), (unsigned short) v);
+            } else {
+                __stcs(reinterpret_cast<unsigned short*>(r0 + x), (unsigned short) yt);
+                __stcs(reinterpret_cast<unsigned short*>(r0 + a.pitch + x), (unsigned short) yb);
+                __stcs(pu, (uint8_t) u);
+                __stcs(pv, (uint8_t) v);
+            }
+            return;
+        }
+        // P010: chroma words (Cb, Cr) per block at cj + 2x; YUV420P10: two Cb samples at cj + x, two Cr samples in the Cr plane
+        constexpr bool msb = Fmt == GLAVA_B200_EXPORT_P010;
+        uint8_t* const py = r0 + 2 * (size_t) x;
+        uint8_t* const pu = msb ? cj + 2 * (size_t) x : cj + x;
+        uint8_t* const pv = msb ? nullptr : c.cr + (size_t) j * a.chroma_pitch + x;
+        uint32_t yt[2] = { 0u, 0u }, yb[2] = { 0u, 0u }, uv[2] = { 0u, 0u };
+        if (native) {
+            if (full) {
+                const uint2 t = __ldcs(reinterpret_cast<const uint2*>(py)), b = __ldcs(reinterpret_cast<const uint2*>(py + a.pitch));
+                yt[0] = t.x; yt[1] = t.y; yb[0] = b.x; yb[1] = b.y;
+                if (msb) {
+                    const uint2 d = __ldcs(reinterpret_cast<const uint2*>(pu));
+                    uv[0] = d.x; uv[1] = d.y;
+                } else {
+                    uv[0] = __ldcs(reinterpret_cast<const uint32_t*>(pu)); uv[1] = __ldcs(reinterpret_cast<const uint32_t*>(pv));
+                }
+            } else {
+                yt[0] = __ldcs(reinterpret_cast<const uint32_t*>(py)); yb[0] = __ldcs(reinterpret_cast<const uint32_t*>(py + a.pitch));
+                if (msb) uv[0] = __ldcs(reinterpret_cast<const uint32_t*>(pu));
+                else { uv[0] = __ldcs(reinterpret_cast<const unsigned short*>(pu)); uv[1] = __ldcs(reinterpret_cast<const unsigned short*>(pv)); }
+            }
+            overlay_p10_quad<E, msb>(top, bot, yt, yb, uv);
+        } else if (msb) {
+            export_p010_quad<E>(f, top, bot, yt, yb, uv);
+        } else {
+            export_i010_quad<E>(f, top, bot, yt, yb, &uv[0], &uv[1]);
+        }
+        if (full) {
+            __stcs(reinterpret_cast<uint2*>(py), make_uint2(yt[0], yt[1]));
+            __stcs(reinterpret_cast<uint2*>(py + a.pitch), make_uint2(yb[0], yb[1]));
+            if (msb) __stcs(reinterpret_cast<uint2*>(pu), make_uint2(uv[0], uv[1]));
+            else { __stcs(reinterpret_cast<uint32_t*>(pu), uv[0]); __stcs(reinterpret_cast<uint32_t*>(pv), uv[1]); }
+        } else {
+            __stcs(reinterpret_cast<uint32_t*>(py), yt[0]);
+            __stcs(reinterpret_cast<uint32_t*>(py + a.pitch), yb[0]);
+            if (msb) __stcs(reinterpret_cast<uint32_t*>(pu), uv[0]);
+            else { __stcs(reinterpret_cast<unsigned short*>(pu), (unsigned short) uv[0]); __stcs(reinterpret_cast<unsigned short*>(pv), (unsigned short) uv[1]); }
+        }
+    }
+
+    __device__ __forceinline__ void row(const OverlayPlanesEntry* e, uint8_t* dst, int r, int x, const uint32_t q[4]) const {
+        row444(true, dst, chroma(e), r, x, q);
+    }
+    __device__ __forceinline__ void pair(uint8_t* dst, Chroma c, int j, int x, const uint32_t top[4], const uint32_t bot[4]) const {
+        pair420(true, dst, c, j, x, top, bot);
+    }
+    __device__ __forceinline__ void item(const OverlayPlanesEntry* e, uint8_t* dst, int u, int x, const uint32_t top[4],
+                                         const uint32_t bot[4], int y1) const {
+        const Chroma c = chroma(e);
+        if (k420) {
+            pair420(a.native, dst, c, u, x, top, bot);
+        } else {
+            row444(a.native, dst, c, 2 * u, x, top);
+            if (y1 >= 0) row444(a.native, dst, c, 2 * u + 1, x, bot);
+        }
+    }
+};
+
+template <typename Index, bool Band, int Fmt, int E>
+__global__ void __launch_bounds__(256) overlay_planes_kernel(const __grid_constant__ OverlayPlanesArgs a) {
+    overlay_walk<Index, Band>(OverlayPlanesBody<Fmt, E>(a));
+}
+
+template <int Fmt>
+static void launch_planes(const OverlayPlanesArgs& a, const ExportGrid& g, cudaStream_t st) {
+    for_any_enc(a.enc, [&](auto e) {
+        constexpr int E = decltype(e)::value;
+        if (a.band) {
+            if (g.narrow) overlay_planes_kernel<uint32_t, true, Fmt, E><<<g.blocks, 256, 0, st>>>(a);
+            else overlay_planes_kernel<uint64_t, true, Fmt, E><<<g.blocks, 256, 0, st>>>(a);
+        } else {
+            if (g.narrow) overlay_planes_kernel<uint32_t, false, Fmt, E><<<g.blocks, 256, 0, st>>>(a);
+            else overlay_planes_kernel<uint64_t, false, Fmt, E><<<g.blocks, 256, 0, st>>>(a);
+        }
+    });
+}
+
+int launch_overlay_planes(const OverlayPlanesArgs& a, void* stream) {
+    const int rows = a.band ? a.mark_rows : 2;
+    const ExportGrid g = export_grid((uint64_t) a.count * (uint64_t) ((a.w + 127) >> 7) * (uint64_t) ((a.h + rows - 1) / rows));
+    cudaStream_t st = (cudaStream_t) stream;
+    switch (a.format) {
+    case GLAVA_B200_EXPORT_NV12: launch_planes<GLAVA_B200_EXPORT_NV12>(a, g, st); break;
+    case GLAVA_B200_EXPORT_I420: launch_planes<GLAVA_B200_EXPORT_I420>(a, g, st); break;
+    case GLAVA_B200_EXPORT_YUV444: launch_planes<GLAVA_B200_EXPORT_YUV444>(a, g, st); break;
+    case GLAVA_B200_EXPORT_P010: launch_planes<GLAVA_B200_EXPORT_P010>(a, g, st); break;
+    case GLAVA_B200_EXPORT_YUV420P10: launch_planes<GLAVA_B200_EXPORT_YUV420P10>(a, g, st); break;
+    case GLAVA_B200_EXPORT_YUV444P10: launch_planes<GLAVA_B200_EXPORT_YUV444P10>(a, g, st); break;
+    default: return fail(GLAVA_B200_EINVAL, "planes overlay launch: format %d", a.format);
+    }
+    return launch_status("planes overlay");
 }
 
 }  // namespace glb

@@ -35,6 +35,16 @@ int list_room(const RendererView& v, size_t bytes, ExportList** out);
 // the background of a descriptor as 0x00BBGGRR
 uint32_t background(const glava_b200_export& d);
 
+// (export.cpp, shared with overlay_planes.cpp) a destination pointer: null, 16-byte alignment, device memory, the
+// renderer's device; `name`[i] names it in the message
+int dst_check(const RendererView& v, const void* p, const char* name, int i, const char* who);
+// One plane of one entry's rectangle: `rows` rows of the common row bytes, the common pitch apart, from byte address p
+struct Rect { uintptr_t p; size_t rows; int entry; bool uv; };
+// Two rectangles of one pitch P and row bytes B, a starting first (a.p <= b.p): whether any rows meet
+bool rects_meet(const Rect& a, const Rect& b, size_t P, size_t B);
+// whether rows of r meet the byte range [f0, f1)
+bool rect_meets_range(const Rect& r, size_t P, size_t B, uintptr_t f0, uintptr_t f1);
+
 // The enqueue every call shares, on the raster stream: wait for after_event, copy the list out of the pinned buffer the
 // caller filled (h[cur]) and record its event, launch(device list), then done_event
 template <typename Launch>

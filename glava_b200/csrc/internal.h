@@ -255,6 +255,25 @@ struct OverlayArgs {
     int    enc;                 // NV12: the destination's encoding, as ExportArgs (enc != 0 runs overlay_enc_kernel)
 };
 int launch_overlay(const OverlayArgs& a, void* stream);
+// export_kernels.cu: glava_b200_overlay_planes (DESIGN 4.17), one launch for the whole list.  Items as OverlayArgs'; an
+// entry holds the rectangle's first sample in each plane (Y; CbCr for NV12 / P010, else Cb; Cr for the planar formats)
+struct alignas(16) OverlayPlanesEntry {
+    uint8_t* plane[3];
+    int      slot;              // framebuffer slot of the listed stream
+    int      pad;
+};
+struct OverlayPlanesArgs {
+    const uint8_t*  fb;         // [slots][h][w] RGBA8
+    const uint32_t* marks;      // as ExportArgs
+    int             mark_rows;
+    const OverlayPlanesEntry* list;
+    int    count, w, h;
+    int    format, native, band;   // format: NV12, I420, YUV444, P010, YUV420P10 or YUV444P10
+    size_t pitch, chroma_pitch;    // bytes between luma rows, between rows of every chroma plane
+    int    enc;                 // the picture's encoding, as ExportArgs
+};
+// overlay_planes_kernel, instantiated per format, encoding, item kind and index width
+int launch_overlay_planes(const OverlayPlanesArgs& a, void* stream);
 // export_kernels.cu: glava_b200_export_ladder (DESIGN 4.13), one launch for every rung of every entry.  Per rung what a
 // standalone call would take: the whole frame at its own size (whole = 1) runs export_kernel's items, every other rung
 // export_scaled_kernel's; z*: what a zero pixel becomes under the rung's format (export_core.h, filled on the host).
@@ -322,6 +341,20 @@ int ladder_run(glava_b200* r, const int* streams, int count, const glava_b200_ex
 // other nor any of the `nfb` byte ranges [fb[k], fb[k] + fb_bytes[k]) (framebuffer arrays)
 int overlay_geometry_check(int w, int h, int count, void* const* dst, void* const* dst_uv, const glava_b200_export& desc,
                            const uint8_t* const* fb, const size_t* fb_bytes, int nfb, const char* who);
+// overlay_planes.cpp, glava_b200_overlay_planes (DESIGN 4.17).  planes_geometry: the descriptor against a w x h frame (format,
+// flags, even 4:2:0 sizes, both pitches) and the planes' shapes; planes_check: every refusal that depends on this renderer
+// alone (the overlap and framebuffer tests are planes_geometry_check's, over rectangles each with its own pitch P and row
+// bytes B); planes_run: the call on one renderer.
+struct PlanesGeom { int planes; size_t luma_row, chroma_row; int chroma_rows; };
+struct PlaneRect { uintptr_t p; size_t rows, P, B; int entry, plane; };
+int planes_geometry(int w, int h, const glava_b200_overlay_planes_desc& d, PlanesGeom* g, const char* who);
+int planes_check(glava_b200* r, const int* streams, int count, const glava_b200_picture* pics,
+                 const glava_b200_overlay_planes_desc* desc, const char* who);
+bool plane_rects_meet(const PlaneRect& a, const PlaneRect& b);
+int planes_geometry_check(int w, int h, int count, const glava_b200_picture* pics, const glava_b200_overlay_planes_desc& desc,
+                          const uint8_t* const* fb, const size_t* fb_bytes, int nfb, const char* who);
+int planes_run(glava_b200* r, const int* streams, int count, const glava_b200_picture* pics, const glava_b200_overlay_planes_desc* desc,
+               void* after_event, void* done_event, const char* who);
 // capi.cu, for sharded.cpp: the blob checks of glava_b200_load_streams (nothing is touched), and save / load with one
 // host pointer per listed stream (the blobs of one shard's streams are not contiguous in the caller's array)
 int state_check_blobs(const glava_b200* r, const void* const* blobs, int count, const char* who);

@@ -382,6 +382,48 @@ int glava_b200_sharded_export_ladder(glava_b200_sharded* g, const int* streams, 
                           rungs, nrungs);
 }
 
+// glava_b200_overlay_planes with global stream indices: the list split by shard (pics[i] travelling with streams[i]), every
+// shard's part checked as one renderer, then the whole list's overlap and every shard's framebuffer, before any shard starts
+int glava_b200_sharded_overlay_planes(glava_b200_sharded* g, const int* streams, int count, const glava_b200_picture* pics,
+                                      const glava_b200_overlay_planes_desc* desc) {
+    clear_error();
+    const char* who = "glava_b200_sharded_overlay_planes";
+    if (!g || !desc) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
+    if (count < 1) return fail(GLAVA_B200_EINVAL, "%s: count %d < 1", who, count);
+    if (!streams || !pics) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
+    std::vector<std::vector<int>> idx(g->shards.size());
+    std::vector<std::vector<glava_b200_picture>> part(g->shards.size());
+    for (int i = 0; i < count; ++i) {
+        const int s = streams[i];
+        if (s < 0 || s >= g->batch) return fail(GLAVA_B200_EINVAL, "%s: stream %d out of range (batch %d)", who, s, g->batch);
+        for (size_t k = 0; k < g->shards.size(); ++k) {
+            const Shard* sh = g->shards[k];
+            if (s >= sh->first && s < sh->first + sh->count) {
+                idx[k].push_back(s - sh->first);
+                part[k].push_back(pics[i]);
+                break;
+            }
+        }
+    }
+    std::vector<const uint8_t*> fb;
+    std::vector<size_t> fb_bytes;
+    for (size_t k = 0; k < g->shards.size(); ++k) {
+        const RendererView v = renderer_view(g->shards[k]->r);
+        fb.push_back(v.fb); fb_bytes.push_back((size_t) v.slots * (size_t) v.h * (size_t) v.w * 4);
+        if (idx[k].empty()) continue;
+        const int rc = planes_check(g->shards[k]->r, idx[k].data(), (int) idx[k].size(), part[k].data(), desc, who);
+        if (rc) return rc;
+    }
+    const RendererView v0 = renderer_view(g->shards[0]->r);
+    const int rc = planes_geometry_check(v0.w, v0.h, count, pics, *desc, fb.data(), fb_bytes.data(), (int) fb.size(), who);
+    if (rc) return rc;
+    return broadcast(g, [&](Shard& s) {
+        const size_t k = (size_t) (std::find(g->shards.begin(), g->shards.end(), &s) - g->shards.begin());
+        if (idx[k].empty()) return 0;
+        return planes_run(s.r, idx[k].data(), (int) idx[k].size(), part[k].data(), desc, nullptr, nullptr, who);
+    });
+}
+
 int glava_b200_sharded_textures(glava_b200_sharded* g, uint16_t* out_l, uint16_t* out_r) {
     clear_error();
     if (!g) return fail(GLAVA_B200_EINVAL, "null argument");

@@ -520,7 +520,8 @@ int glava_b200_export_ladder(glava_b200* r, const int* streams, int count, const
  *   pixel leaves D exactly as it was, and rows the dirty-row marks skip and all-zero quads are neither read nor written.
  *   An opaque pixel gives exactly glava_b200_export_frames' bytes.  Under any other opacity GLava's window is opaque: the
  *   rectangle gets exactly what glava_b200_export_frames writes (RGBA / BGRA with EXPORT_OVER, or NV12).
- *   The overlay takes RGBA, BGRA and NV12; I420, YUV444, P010, YUV420P10 and YUV444P10 are refused by name.
+ *   The overlay takes RGBA, BGRA and NV12; I420, YUV444, P010, YUV420P10 and YUV444P10 are refused by name (decoded
+ *   pictures in those formats, with per-plane pointers and pitches, go to glava_b200_overlay_planes below).
  *   Besides the refusals of glava_b200_export_scaled that apply (format, pitch, uv_offset, alignment, null / host /
  *   other-device dst or dst_uv, dst_uv for RGBA / BGRA, odd NV12 frames, stream range, count < 1, an unbuilt renderer),
  *   any other flag, a rectangle that meets the renderer's framebuffer array and two rectangles of one call that overlap (luma
@@ -531,6 +532,42 @@ int glava_b200_export_ladder(glava_b200* r, const int* streams, int count, const
  *                              framebuffer are checked before any shard starts. */
 int glava_b200_overlay_frames(glava_b200* r, const int* streams, int count, void* const* dst, void* const* dst_uv,
                               const glava_b200_export* desc, void* after_event, void* done_event);
+
+/* Overlay onto decoded pictures (DESIGN.md §4.17): what a decoder or ffmpeg hands over — NV12, I420, YUV444, P010,
+ * YUV420P10 or YUV444P10, each plane at its own pointer, luma and chroma rows at their own pitches.
+ *   glava_b200_overlay_planes  composites the current frame of streams[i] onto the w x h rectangle of pics[i], exactly as
+ *                              glava_b200_overlay_frames does onto NV12 (same ordering, events, streams and opacity rules;
+ *                              NV12 runs its item body), top-down at the rectangle's origin:
+ *     pics[i].plane[0]         the rectangle's first Y sample, `pitch` bytes per row
+ *     pics[i].plane[1]         NV12 / P010: its first CbCr pair; the planar formats: its first Cb sample
+ *     pics[i].plane[2]         the planar formats: its first Cr sample; NULL for NV12 and P010
+ *     desc                     format, flags (0, or EXPORT_FULL_RANGE / EXPORT_BT601: the picture's encoding), the luma
+ *                              pitch and one chroma pitch for every chroma plane; 4:2:0 chroma is w/2 x h/2
+ *   10-bit samples hold their code as v >> 6 (P010) or v & 1023 (YUV420P10, YUV444P10).  Under native opacity the blend is
+ *   overlay_frames' NV12 blend (I420: bit for bit NV12 deinterleaved; YUV444: chroma per pixel), and at 10 bits the same
+ *   fraction at 10 bits with 4:2:0 chroma from the block's exact sums, as P010's export (export_core.h).  A blended 10-bit
+ *   sample is written with its other bits zero; a sample no non-zero pixel covers (a luma sample under a zero pixel, a chroma
+ *   sample whose pixel or 2x2 block is all zero) keeps all 16 bits, and rows the marks skip and all-zero quads are neither
+ *   read nor written.  Under any other opacity every sample of the rectangle gets glava_b200_export_frames' bytes.
+ *   GLAVA_B200_EINVAL, with nothing enqueued, for: a null argument, count < 1, an unbuilt renderer; RGBA, BGRA (those go to
+ *   glava_b200_overlay_frames) or an unknown format; any other flag; odd w or h for the 4:2:0 formats; a pitch or
+ *   chroma_pitch that is not a multiple of 16 or below the plane's row bytes (luma w, 2w at 10 bits; chroma w for NV12,
+ *   YUV444 and YUV420P10, w/2 for I420, 2w for P010 and YUV444P10); a plane pointer that is null, not 16-byte aligned, not
+ *   device memory or on another device; a non-null plane[2] for NV12 or P010; a stream out of range; a plane rectangle
+ *   that meets the renderer's framebuffer array; two plane rectangles of the call that overlap (every pair: across
+ *   entries, luma against chroma, Cb against Cr).
+ *   glava_b200_sharded_overlay_planes  the same with global stream indices, each picture on the device of the shard that
+ *                              owns streams[i]; every entry, the overlap of the whole list and every shard's framebuffer are
+ *                              checked before any shard starts. */
+typedef struct { void* plane[3]; } glava_b200_picture;
+typedef struct {
+    int      format;        /* GLAVA_B200_EXPORT_NV12, _I420, _YUV444, _P010, _YUV420P10, _YUV444P10 */
+    uint32_t flags;         /* 0, or GLAVA_B200_EXPORT_FULL_RANGE / GLAVA_B200_EXPORT_BT601 */
+    size_t   pitch;         /* bytes between luma rows */
+    size_t   chroma_pitch;  /* bytes between rows of every chroma plane */
+} glava_b200_overlay_planes_desc;
+int glava_b200_overlay_planes(glava_b200* r, const int* streams, int count, const glava_b200_picture* pics,
+                              const glava_b200_overlay_planes_desc* desc, void* after_event, void* done_event);
 
 /* ---- one handle for a batch spread over several GPUs of a node (csrc/sharded.cpp) -------------------------------------
  * The streams of a batch are independent (one GLava process each, in the reference), so the batch is cut into contiguous
@@ -563,6 +600,8 @@ int  glava_b200_sharded_export_scaled(glava_b200_sharded* s, const int* streams,
                                       const glava_b200_export_scale* scale);   /* global indices; see glava_b200_export_scaled */
 int  glava_b200_sharded_overlay_frames(glava_b200_sharded* s, const int* streams, int count, void* const* dst,
                                        void* const* dst_uv, const glava_b200_export* desc);   /* see glava_b200_overlay_frames */
+int  glava_b200_sharded_overlay_planes(glava_b200_sharded* s, const int* streams, int count, const glava_b200_picture* pics,
+                                       const glava_b200_overlay_planes_desc* desc);   /* see glava_b200_overlay_planes */
 int  glava_b200_sharded_export_ladder(glava_b200_sharded* s, const int* streams, int count,
                                       const glava_b200_export_rung* rungs, int nrungs, void* const* dst,
                                       void* const* dst_uv);   /* global indices; see glava_b200_export_ladder */
