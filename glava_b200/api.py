@@ -147,39 +147,49 @@ LADDER_MAX = 8
 EXPORT_RGBA, EXPORT_BGRA, EXPORT_NV12 = 0, 1, 2
 EXPORT_I420, EXPORT_YUV444, EXPORT_P010 = 4, 5, 6
 EXPORT_YUV420P10, EXPORT_YUV444P10 = 7, 8                # planar 10-bit, LSB-aligned (yuv420p10le / yuv444p10le, DESIGN 4.16)
+EXPORT_YUV422P, EXPORT_YUV422P10, EXPORT_UYVY = 10, 11, 12   # 4:2:2 (yuv422p / yuv422p10le / uyvy422, DESIGN 4.18)
 EXPORT_OVER = 1
 EXPORT_FULL_RANGE, EXPORT_BT601 = 0x100, 0x200          # the Y'CbCr encoding (DESIGN 4.15); neither: BT.709 limited range
 EXPORT_MATRICES = {"bt709": 0, "bt601": EXPORT_BT601}
 EXPORT_FORMATS = {"rgba": EXPORT_RGBA, "bgra": EXPORT_BGRA, "nv12": EXPORT_NV12, "i420": EXPORT_I420,
                   "yuv444": EXPORT_YUV444, "p010": EXPORT_P010, "yuv420p10": EXPORT_YUV420P10,
-                  "yuv444p10": EXPORT_YUV444P10}
+                  "yuv444p10": EXPORT_YUV444P10, "yuv422p": EXPORT_YUV422P, "yuv422p10": EXPORT_YUV422P10,
+                  "uyvy": EXPORT_UYVY}
 OVERLAY_FORMATS = ("rgba", "bgra", "nv12")
 # the formats overlay_planes takes: decoded pictures, one tensor per plane (DESIGN 4.17)
-PLANES_FORMATS = ("nv12", "i420", "yuv444", "p010", "yuv420p10", "yuv444p10")
+PLANES_FORMATS = ("nv12", "i420", "yuv444", "p010", "yuv420p10", "yuv444p10", "yuv422p", "yuv422p10", "uyvy")
 # the formats whose samples are uint16, which also take uint16 `out` tensors
-WIDE_FORMATS = ("p010", "yuv420p10", "yuv444p10")
+WIDE_FORMATS = ("p010", "yuv420p10", "yuv444p10", "yuv422p10")
 
 
 def _export_layout(fmt, w, h):
     """(rows, row bytes, pitch multiple) of one w x h output of `fmt` held as rows of one pitch: RGBA / BGRA h rows of w * 4
     bytes; NV12 / P010 h * 3 / 2 rows of w (P010: w uint16) samples, Y then CbCr; I420 / YUV420P10 h * 3 / 2 rows, the Y
     plane then the Cb and Cr planes back to back at pitch / 2 (pitch a multiple of 32); YUV444 / YUV444P10 3 h rows, the Y,
-    Cb and Cr planes; the 10-bit formats hold w uint16 per row"""
+    Cb and Cr planes; YUV422P / YUV422P10 2 h rows, the Y plane then the Cb and Cr planes of h rows at pitch / 2 (pitch a
+    multiple of 32); UYVY h rows of 2 w bytes; the 10-bit formats hold w uint16 per row"""
     if fmt in ("rgba", "bgra"):
         return h, w * 4, 16
+    if fmt == "uyvy":
+        return h, w * 2, 16
     row = w * 2 if fmt in WIDE_FORMATS else w
     if fmt in ("yuv444", "yuv444p10"):
         return 3 * h, row, 16
+    if fmt in ("yuv422p", "yuv422p10"):
+        return 2 * h, row, 32
     return h * 3 // 2, row, 32 if fmt in ("i420", "yuv420p10") else 16
 
 
 def _export_views(fmt, t, w, h):
     """what an export into t returns: t is uint8 [..., rows, pitch] with contiguous rows as _export_layout describes.  RGBA /
     BGRA [..., h, w, 4], NV12 [..., h * 3 / 2, w] uint8, P010 [..., h * 3 / 2, w] uint16, I420 / YUV444 the plane views
-    (Y, Cb, Cr), each [..., rows, cols], YUV420P10 / YUV444P10 the same as uint16"""
+    (Y, Cb, Cr), each [..., rows, cols], YUV420P10 / YUV444P10 the same as uint16; YUV422P / YUV422P10 (Y, Cb, Cr) with
+    Cb and Cr [..., h, w / 2]; UYVY [..., h, 2 w] uint8 (Cb, Y0, Cr, Y1 per pixel pair)"""
     import torch
     if fmt in ("rgba", "bgra"):
         return t[..., :w * 4].unflatten(-1, (w, 4))
+    if fmt == "uyvy":
+        return t[..., :w * 2]
     if fmt == "nv12":
         return t[..., :w]
     if fmt in WIDE_FORMATS:
@@ -188,7 +198,8 @@ def _export_views(fmt, t, w, h):
         return t[..., :w]
     P = t.shape[-1]                                           # the pitch in samples
     flat = t.flatten(-2)
-    cw, ch, cp = (w // 2, h // 2, P // 2) if fmt in ("i420", "yuv420p10") else (w, h, P)
+    cw, ch, cp = ((w // 2, h // 2, P // 2) if fmt in ("i420", "yuv420p10") else (w // 2, h, P // 2)
+                  if fmt in ("yuv422p", "yuv422p10") else (w, h, P))
     n = ch * cp
     y = flat[..., :P * h].unflatten(-1, (h, P))[..., :w]
     cb = flat[..., P * h:P * h + n].unflatten(-1, (ch, cp))[..., :cw]
@@ -488,9 +499,9 @@ class _FrameExport:
         """-> (stream list, Export, [dst pointers], what to return).  device_of(stream): the CUDA device of a stream's
         frame.  size: (w, h) of each output, None: the frame's.  out: None (allocate), one uint8 tensor [count, rows, ...]
         whose dim 1 steps by the pitch, or a list of count tensors [rows, ...] with one common pitch; rows as
-        _export_layout gives them (h for RGBA / BGRA, h * 3 / 2 for NV12, I420, P010 and YUV420P10, 3 h for YUV444 and
-        YUV444P10; the planar formats keep their planes back to back from row h); P010, YUV420P10 and YUV444P10 also take
-        uint16 tensors.  matrix / full_range: the Y'CbCr encoding (_export_desc)"""
+        _export_layout gives them (h for RGBA / BGRA and UYVY, h * 3 / 2 for NV12, I420, P010 and YUV420P10, 2 h for YUV422P
+        and YUV422P10, 3 h for YUV444 and YUV444P10; the planar formats keep their planes back to back from row h); P010,
+        YUV420P10, YUV444P10 and YUV422P10 also take uint16 tensors.  matrix / full_range: the Y'CbCr encoding (_export_desc)"""
         import torch
         s = np.ascontiguousarray(np.asarray(streams, dtype=np.int64).reshape(-1), dtype=np.int32)
         count = int(s.shape[0])
@@ -634,8 +645,9 @@ class _FrameExport:
         one tuple of plane tensors per entry (a tuple may repeat), or one tuple of batched [count, rows, cols] plane tensors;
         a tuple is (Y, CbCr) for NV12 and P010, (Y, Cb, Cr) otherwise, each CUDA, uint8 (the 8-bit formats) or uint16 or
         uint8 with doubled width (the 10-bit formats), with contiguous rows: Y [H, W], NV12 CbCr [H / 2, W] bytes, P010 CbCr
-        [H / 2, W] samples, I420 / YUV420P10 Cb and Cr [H / 2, W / 2], YUV444 / YUV444P10 Cb and Cr [H, W] (export_frames'
-        plane views).  Every luma plane has one pitch and every chroma plane one pitch.  at: (x, y) of each frame's top-left
+        [H / 2, W] samples, I420 / YUV420P10 Cb and Cr [H / 2, W / 2], YUV444 / YUV444P10 Cb and Cr [H, W], YUV422P /
+        YUV422P10 Cb and Cr [H, W / 2] (export_frames' plane views); UYVY is one plane [H, 2 W] of bytes, given as a tensor
+        or a 1-tuple (one [count, H, 2 W] tensor for a batch), and a 4:2:2 frame starts at an even x.  Every luma plane has one pitch and every chroma plane one pitch.  at: (x, y) of each frame's top-left
         in luma samples (None: (0, 0)).  Raises ValueError for a rectangle that leaves its picture, mixed pitches within a
         plane kind, or a plane start that is not 16-byte aligned (the library refuses the rest)."""
         import torch
@@ -644,13 +656,15 @@ class _FrameExport:
                              "(RGBA and BGRA images go to overlay_frames)")
         s = np.ascontiguousarray(np.asarray(streams, dtype=np.int64).reshape(-1), dtype=np.int32)
         count = int(s.shape[0])
-        nplanes = 2 if fmt in ("nv12", "p010") else 3
+        nplanes = 2 if fmt in ("nv12", "p010") else 1 if fmt == "uyvy" else 3
         sb = 2 if fmt in WIDE_FORMATS else 1                  # bytes per sample
+        px = 2 if fmt == "uyvy" else sb                       # luma-plane bytes per pixel (UYVY: its one packed plane)
         c420 = fmt in ("nv12", "i420", "p010", "yuv420p10")
+        c422 = fmt in ("yuv422p", "yuv422p10", "uyvy")
 
         def describe(planes, what, batched):
             """-> ([base address per plane], H, W, pitch, chroma pitch) of one picture (batched: of entry 0)"""
-            planes = tuple(planes)
+            planes = (planes,) if isinstance(planes, torch.Tensor) else tuple(planes)
             if len(planes) != nplanes:
                 raise ValueError(f"{what}: {fmt} has {nplanes} planes, got {len(planes)}")
             dims = 3 if batched else 2
@@ -667,9 +681,10 @@ class _FrameExport:
                 bases.append(t.data_ptr())
                 shapes.append((t.shape[-2], t.shape[-1] * t.element_size()))   # rows, row bytes
                 pitches.append(t.stride(-2) * t.element_size())
-            H, W = shapes[0][0], shapes[0][1] // sb
+            H, W = shapes[0][0], shapes[0][1] // px
             crows = H // 2 if c420 else H
-            cbytes = {"nv12": W, "p010": 2 * W, "i420": W // 2, "yuv420p10": W, "yuv444": W, "yuv444p10": 2 * W}[fmt]
+            cbytes = {"nv12": W, "p010": 2 * W, "i420": W // 2, "yuv420p10": W, "yuv444": W, "yuv444p10": 2 * W,
+                      "yuv422p": W // 2, "yuv422p10": W, "uyvy": 0}[fmt]
             for p in range(1, nplanes):
                 if shapes[p][0] != crows or shapes[p][1] < cbytes:
                     raise ValueError(f"{what}[{p}]: a {W}x{H} {fmt} picture has chroma planes of {crows} rows of {cbytes} "
@@ -677,8 +692,13 @@ class _FrameExport:
             if nplanes == 3 and pitches[1] != pitches[2]:
                 raise ValueError(f"{what}: Cb pitch {pitches[1]}, Cr pitch {pitches[2]}: one chroma pitch per call")
             steps = [t.stride(0) * t.element_size() for t in planes] if batched else None
-            return bases, H, W, pitches[0], pitches[1], steps
+            return bases, H, W, pitches[0], pitches[1] if nplanes > 1 else 0, steps
 
+        if fmt == "uyvy" and isinstance(pictures, torch.Tensor):  # UYVY: one batched tensor
+            pictures = (pictures,)
+        if fmt == "uyvy" and isinstance(pictures, (list, tuple)) and len(pictures) and isinstance(pictures[0], torch.Tensor) \
+                and pictures[0].dim() == 2:                   # one [H, 2W] tensor per picture
+            pictures = [(t,) for t in pictures]
         if isinstance(pictures, (list, tuple)) and len(pictures) and isinstance(pictures[0], torch.Tensor):
             bases, H, W, P, CP, steps = describe(pictures, "pictures", True)
             ents = [([b + i * st for b, st in zip(bases, steps)], H, W, P, CP) for i in range(count)]
@@ -706,9 +726,11 @@ class _FrameExport:
                 raise ValueError(f"pictures[{i}]: the {w}x{h} frame at ({x}, {y}) leaves the {W}x{H} picture")
             if c420 and (x % 2 or y % 2):
                 raise ValueError(f"pictures[{i}]: a {fmt} frame starts at an even (x, y), got ({x}, {y})")
-            cx, cy = (x // 2, y // 2) if c420 else (x, y)
+            if c422 and x % 2:
+                raise ValueError(f"pictures[{i}]: a {fmt} frame starts at an even x, got ({x}, {y})")
+            cx, cy = (x // 2, y // 2) if c420 else (x // 2, y) if c422 else (x, y)
             cs = {"nv12": 2, "p010": 4, "i420": 1, "yuv420p10": 2}.get(fmt, sb)   # chroma bytes per chroma position
-            ptrs = [bases[0] + y * P + x * sb] + [bases[p] + cy * CP + cx * cs for p in range(1, nplanes)]
+            ptrs = [bases[0] + y * P + x * px] + [bases[p] + cy * CP + cx * cs for p in range(1, nplanes)]
             for p, a in enumerate(ptrs):
                 if a % 16:
                     raise ValueError(f"pictures[{i}]: the frame at ({x}, {y}) starts plane {p} at an address that is not a "
@@ -1018,8 +1040,9 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
         "nv12" ([h * 3 / 2, w]: Y rows, then interleaved CbCr rows), "p010" (the same as uint16 samples, 10-bit code << 6),
         "i420" / "yuv444" (a tuple of plane views Y [h, w], Cb and Cr [h / 2, w / 2] or [h, w] of one back-to-back
         allocation), "yuv420p10" / "yuv444p10" (the same planes as uint16 samples holding the 10-bit code in their low bits:
-        ffmpeg's yuv420p10le / yuv444p10le); the YUV formats are always composited.  out: see _export_plan; None allocates
-        [count, ...] of those shapes (rows padded to a multiple of 16 bytes, 32 for I420 and YUV420P10).  Returns out.
+        ffmpeg's yuv420p10le / yuv444p10le), "yuv422p" / "yuv422p10" (Y [h, w], Cb and Cr [h, w / 2], uint8 / uint16) or
+        "uyvy" ([h, 2 w] uint8, Cb Y0 Cr Y1 per pixel pair); the YUV formats are always composited.  out: see _export_plan; None allocates
+        [count, ...] of those shapes (rows padded to a multiple of 16 bytes, 32 for I420, YUV420P10, YUV422P and YUV422P10).  Returns out.
         after / done: torch.cuda.Event or cudaEvent_t handles — the export waits for `after` on the device and records
         `done` behind itself.  Left None, the export is ordered after the work already queued on torch's current stream,
         and that stream waits for the export (the tensors can be used right away).
@@ -1048,7 +1071,7 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
                       done=None, matrix="bt709", full_range=False):
         """export_frames of a source rectangle shrunk to size = (w, h) by the exact area average (glava_b200_export_scaled):
         crop = (x, y, w, h) in top-down coordinates (y = 0 is the top row), None: the whole frame.  Downscale only; NV12,
-        I420, P010 and YUV420P10 need an even w and h.  Shapes, out, after, done, matrix and full_range as export_frames, with the output
+        I420, P010 and YUV420P10 need an even w and h, YUV422P, YUV422P10 and UYVY an even w.  Shapes, out, after, done, matrix and full_range as export_frames, with the output
         size in place of the frame's."""
         s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, lambda stream: self.device, size, matrix,
                                                  full_range)
@@ -1081,7 +1104,7 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
 
     def overlay_planes(self, streams, pictures, at=None, fmt="i420", matrix="bt709", full_range=False, after=None, done=None):
         """The current frames of `streams` composited in place onto decoded pictures, one tensor per plane
-        (glava_b200_overlay_planes): NV12, I420, YUV444, P010, YUV420P10 or YUV444P10, the planes of each picture at their
+        (glava_b200_overlay_planes): NV12, I420, YUV444, P010, YUV420P10, YUV444P10, YUV422P, YUV422P10 or UYVY, the planes of each picture at their
         own addresses with one luma and one chroma pitch per call — ffmpeg's AVFrame planes, NVDEC surfaces, or what
         export_frames returns.  Native opacity blends in Y'CbCr in the picture's encoding (matrix / full_range) as
         overlay_frames blends NV12; any other opacity writes export_frames' bytes.  pictures and at: see _planes_plan;
@@ -1096,9 +1119,10 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
         """The frames of `streams` shrunk to tile = (w, h) and laid out row-major, `cols` tiles per row, in one picture, by
         one export_scaled call with a destination and a chroma destination per tile.  W = cols * w, H = rows * h; returns
         [H * 3 / 2, W] for NV12 (uint8) and P010 (uint16), Y rows then CbCr rows, the plane views (Y, Cb, Cr) for I420 and
-        YUV444 (uint8) and YUV420P10 and YUV444P10 (uint16), or [H, W, 4]: one surface to hand to an encoder.  Tiles start
-        at multiples of 16 bytes in every plane, so w is a multiple of 16 (NV12, YUV444, YUV420P10), 32 (I420), 8 (P010,
-        YUV444P10) or 4 (RGBA / BGRA).  out: a CUDA tensor [rows, pitch] whose rows hold the picture's row bytes, rows as
+        YUV444 (uint8) and YUV420P10 and YUV444P10 (uint16), the same for YUV422P (uint8) and YUV422P10 (uint16), [H, 2 W]
+        for UYVY, or [H, W, 4]: one surface to hand to an encoder.  Tiles start at multiples of 16 bytes in every plane, so w
+        is a multiple of 16 (NV12, YUV444, YUV420P10, YUV422P10), 32 (I420, YUV422P), 8 (P010, YUV444P10, UYVY) or 4 (RGBA /
+        BGRA).  out: a CUDA tensor [rows, pitch] whose rows hold the picture's row bytes, rows as
         _export_layout gives them for W x H (planar formats: the chroma planes back to back from row H); tiles past the last
         stream keep its bytes (out None: black).  Ordered against torch's current stream as export_frames without events.
         matrix / full_range as export_frames (black: Y 0 in full range)."""
@@ -1111,16 +1135,18 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
         desc = _export_desc(fmt, False, background, matrix, full_range)
         W, H = cols * tw, (count + cols - 1) // cols * th
         rows, row_bytes, align = _export_layout(fmt, W, H)
-        px = {"rgba": 4, "bgra": 4}.get(fmt, 2 if fmt in WIDE_FORMATS else 1)
+        px = {"rgba": 4, "bgra": 4, "uyvy": 2}.get(fmt, 2 if fmt in WIDE_FORMATS else 1)
         if out is None:
             base = torch.empty((rows, (row_bytes + align - 1) // align * align), dtype=torch.uint8, device=f"cuda:{self.device}")
             if count % cols:                                  # black where no stream lands
                 if fmt == "p010":
                     base.view(torch.uint16)[:H].fill_(0 if full_range else 64 << 6)
                     base.view(torch.uint16)[H:].fill_(512 << 6)
-                elif fmt in ("yuv420p10", "yuv444p10"):
+                elif fmt in ("yuv420p10", "yuv444p10", "yuv422p10"):
                     base.view(torch.uint16)[:H].fill_(0 if full_range else 64)
                     base.view(torch.uint16)[H:].fill_(512)
+                elif fmt == "uyvy":                           # Cb, Y, Cr, Y: 128, 16 (full range 128, 0) per pixel
+                    base.view(torch.uint16).fill_(128 | (0 if full_range else 16) << 8)
                 elif fmt in ("rgba", "bgra"):
                     base.fill_(0)
                 else:
@@ -1140,6 +1166,9 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
         elif fmt in ("i420", "yuv420p10"):                    # Cr one whole chroma plane past Cb
             uv = [ptr + H * pitch + (i // cols) * (th // 2) * (pitch // 2) + (i % cols) * (tw // 2) * px for i in range(count)]
             desc.uv_offset = (pitch // 2) * (H // 2)
+        elif fmt in ("yuv422p", "yuv422p10"):                 # chroma rows pitch / 2 apart, Cr one plane past Cb
+            uv = [ptr + H * pitch + (i // cols) * th * (pitch // 2) + (i % cols) * (tw // 2) * px for i in range(count)]
+            desc.uv_offset = (pitch // 2) * H
         elif fmt in ("yuv444", "yuv444p10"):
             uv = [ptr + (H + (i // cols) * th) * pitch + (i % cols) * tw * px for i in range(count)]
             desc.uv_offset = pitch * H

@@ -30,6 +30,9 @@ const char* format_name(int format) {
     case GLAVA_B200_EXPORT_P010: return "P010";
     case GLAVA_B200_EXPORT_YUV420P10: return "YUV420P10";
     case GLAVA_B200_EXPORT_YUV444P10: return "YUV444P10";
+    case GLAVA_B200_EXPORT_YUV422P: return "YUV422P";
+    case GLAVA_B200_EXPORT_YUV422P10: return "YUV422P10";
+    case GLAVA_B200_EXPORT_UYVY: return "UYVY";
     default: return nullptr;
     }
 }
@@ -40,17 +43,25 @@ int desc_size(int w, int h, const glava_b200_export& d, const char* what, const 
     const char* name = format_name(fmt);
     if (export_420(fmt) && ((w | h) & 1))
         return fail(GLAVA_B200_EINVAL, "%s: %s needs an even width and height, the %s is %dx%d", who, name, what, w, h);
+    if (export_422(fmt) && (w & 1))                         // chroma per pixel pair; 4:2:2 rows are independent, any h
+        return fail(GLAVA_B200_EINVAL, "%s: %s needs an even width, the %s is %dx%d", who, name, what, w, h);
     const size_t row = !export_ycbcr(fmt) ? (size_t) w * 4
-                       : fmt == GLAVA_B200_EXPORT_P010 || export_p10(fmt) ? (size_t) w * 2 : (size_t) w;
+                       : fmt == GLAVA_B200_EXPORT_P010 || export_p10(fmt) || fmt == GLAVA_B200_EXPORT_YUV422P10 ||
+                                 fmt == GLAVA_B200_EXPORT_UYVY
+                           ? (size_t) w * 2
+                           : (size_t) w;
     if (d.pitch % 16 || d.pitch < row)
         return fail(GLAVA_B200_EINVAL, "%s: pitch %zu must be a multiple of 16 and at least %zu", who, d.pitch, row);
-    if ((fmt == GLAVA_B200_EXPORT_I420 || fmt == GLAVA_B200_EXPORT_YUV420P10) && d.pitch % 32)
+    if ((fmt == GLAVA_B200_EXPORT_I420 || fmt == GLAVA_B200_EXPORT_YUV420P10 || fmt == GLAVA_B200_EXPORT_YUV422P ||
+         fmt == GLAVA_B200_EXPORT_YUV422P10) && d.pitch % 32)
         return fail(GLAVA_B200_EINVAL, "%s: %s pitch %zu must be a multiple of 32, so that chroma rows (pitch / 2) stay 16-byte "
                     "aligned", who, name, d.pitch);
     if ((fmt == GLAVA_B200_EXPORT_NV12 || fmt == GLAVA_B200_EXPORT_P010) &&
         (d.uv_offset % 16 || (d.uv_offset && d.uv_offset < d.pitch * (size_t) h)))
         return fail(GLAVA_B200_EINVAL, "%s: uv_offset %zu must be a multiple of 16 and at least pitch * h = %zu (or 0)", who,
                     d.uv_offset, d.pitch * (size_t) h);
+    if (fmt == GLAVA_B200_EXPORT_UYVY && d.uv_offset)
+        return fail(GLAVA_B200_EINVAL, "%s: UYVY uv_offset %zu must be 0: UYVY has no chroma plane", who, d.uv_offset);
     const size_t plane = export_planes(fmt, d.pitch, 0, h).plane;
     if (export_planar(fmt) && (d.uv_offset % 16 || (d.uv_offset && d.uv_offset < plane)))
         return fail(GLAVA_B200_EINVAL, "%s: %s uv_offset %zu (Cb plane to Cr plane) must be a multiple of 16 and at least one "
@@ -101,7 +112,7 @@ int output_bytes(ExportKind kind, const glava_b200* r, const glava_b200_export* 
     if (rc) return rc;
     const size_t h = (size_t) q.out_h;
     const ExportPlanes pl = export_planes(desc->format, desc->pitch, desc->uv_offset, q.out_h);
-    if (!export_ycbcr(desc->format)) *bytes = desc->pitch * h;
+    if (!export_chroma_planes(desc->format)) *bytes = desc->pitch * h;   // RGBA, BGRA, UYVY: one plane
     else if (export_planar(desc->format)) *bytes = pl.cb + pl.cr + pl.plane;
     else *bytes = pl.cb + desc->pitch * (h / 2);
     return 0;
@@ -218,9 +229,9 @@ int export_check(ExportKind kind, glava_b200* r, const int* streams, int count, 
     glava_b200_export_scale local;
     int rc = desc_check(kind, v.w, v.h, *desc, scale, q ? q : &local, who);
     if (rc) return rc;
-    if (dst_uv && !export_ycbcr(desc->format))
-        return fail(GLAVA_B200_EINVAL, "%s: dst_uv is for NV12 only, or I420, YUV444, P010, YUV420P10 and YUV444P10: %s has no "
-                    "chroma plane", who,
+    if (dst_uv && !export_chroma_planes(desc->format))
+        return fail(GLAVA_B200_EINVAL, "%s: dst_uv is for NV12 only, or I420, YUV444, P010, YUV420P10, YUV444P10, YUV422P and "
+                    "YUV422P10: %s has no chroma plane", who,
                     format_name(desc->format));
     if (count < 1) return fail(GLAVA_B200_EINVAL, "%s: count %d < 1", who, count);
     if (!streams || !dst) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
@@ -247,7 +258,7 @@ int export_run(ExportKind kind, glava_b200* r, const int* streams, int count, vo
         const size_t fb_bytes = (size_t) v.slots * (size_t) v.h * (size_t) v.w * 4;
         if ((rc = overlay_geometry_check(v.w, v.h, count, dst, dst_uv, *desc, &v.fb, &fb_bytes, 1, who)) != 0) return rc;
     }
-    const bool yuv = export_ycbcr(desc->format);
+    const bool yuv = export_ycbcr(desc->format), planes = export_chroma_planes(desc->format);
     const ExportPlanes pl = export_planes(desc->format, desc->pitch, desc->uv_offset, q.out_h);
     CU(cudaSetDevice(v.device));
     // export_kernel's entries have no chroma pointer (its machine code stays as measured); the others carry one per entry
@@ -260,7 +271,7 @@ int export_run(ExportKind kind, glava_b200* r, const int* streams, int count, vo
         uint8_t* const d = (uint8_t*) dst[i];
         const int slot = streams[i] % v.slots;
         if (kind == ExportKind::frames) reinterpret_cast<ExportEntry*>(host)[i] = { d, slot, 0 };
-        else reinterpret_cast<ExportEntryUV*>(host)[i] = { d, !yuv ? nullptr : dst_uv ? (uint8_t*) dst_uv[i] : d + pl.cb, slot, 0 };
+        else reinterpret_cast<ExportEntryUV*>(host)[i] = { d, !planes ? nullptr : dst_uv ? (uint8_t*) dst_uv[i] : d + pl.cb, slot, 0 };
     }
     return list_enqueue(v, L, bytes, after_event, done_event, [&](const void* d_list) {
         if (kind == ExportKind::frames) {

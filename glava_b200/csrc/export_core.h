@@ -149,25 +149,34 @@ GLB_HD bool export_yuv(int format) {                   // a format with chroma p
 // The planar 10-bit formats (DESIGN 4.16) run kernels of their own, so export_yuv, which the existing ladder kernels evaluate
 // at run time, does not name them; the host checks take export_ycbcr, every format with chroma planes
 GLB_HD bool export_p10(int format) { return format == GLAVA_B200_EXPORT_YUV420P10 || format == GLAVA_B200_EXPORT_YUV444P10; }
-GLB_HD bool export_ycbcr(int format) { return export_yuv(format) || export_p10(format); }
+// The 4:2:2 formats (DESIGN 4.18), likewise kernels of their own: chroma per horizontal pixel pair, w even, any h
+GLB_HD bool export_422(int format) {
+    return format == GLAVA_B200_EXPORT_YUV422P || format == GLAVA_B200_EXPORT_YUV422P10 || format == GLAVA_B200_EXPORT_UYVY;
+}
+// every Y'CbCr format, the ones the colour flags apply to; export_chroma_planes: those with chroma planes (UYVY packs its
+// chroma into its one plane)
+GLB_HD bool export_ycbcr(int format) { return export_yuv(format) || export_p10(format) || export_422(format); }
+GLB_HD bool export_chroma_planes(int format) { return export_ycbcr(format) && format != GLAVA_B200_EXPORT_UYVY; }
 GLB_HD bool export_420(int format) {                   // chroma per 2x2 block: w and h even, items are row pairs
     return format == GLAVA_B200_EXPORT_NV12 || format == GLAVA_B200_EXPORT_I420 || format == GLAVA_B200_EXPORT_P010 ||
            format == GLAVA_B200_EXPORT_YUV420P10;
 }
 GLB_HD bool export_planar(int format) {
-    return format == GLAVA_B200_EXPORT_I420 || format == GLAVA_B200_EXPORT_YUV444 || export_p10(format);
+    return format == GLAVA_B200_EXPORT_I420 || format == GLAVA_B200_EXPORT_YUV444 || export_p10(format) ||
+           format == GLAVA_B200_EXPORT_YUV422P || format == GLAVA_B200_EXPORT_YUV422P10;
 }
 
 // Where the chroma of a destination lies, from the descriptor and the output height: `cb`, the bytes from the luma to the
 // chroma plane (NV12 / P010: the CbCr plane, uv_offset or pitch * h; the planar formats: the Cb plane, right after the
 // luma); `cr`, the bytes from Cb to Cr (planar only: uv_offset, or 0 for one chroma plane, back to back); `plane`, the bytes
-// of one planar chroma plane (I420 / YUV420P10: h / 2 rows of pitch / 2)
+// of one planar chroma plane (I420 / YUV420P10: h / 2 rows of pitch / 2; YUV422P / YUV422P10: h rows of pitch / 2)
 struct ExportPlanes { size_t cb, cr, plane; };
 GLB_HD ExportPlanes export_planes(int format, size_t pitch, size_t uv_offset, int h) {
     ExportPlanes p = { uv_offset ? uv_offset : pitch * (size_t) h, 0, 0 };
     if (export_planar(format)) {
         p.plane = format == GLAVA_B200_EXPORT_I420 || format == GLAVA_B200_EXPORT_YUV420P10 ? (pitch / 2) * (size_t) (h / 2)
-                                                                                             : pitch * (size_t) h;
+                  : format == GLAVA_B200_EXPORT_YUV422P || format == GLAVA_B200_EXPORT_YUV422P10 ? (pitch / 2) * (size_t) h
+                                                                                                 : pitch * (size_t) h;
         p.cb = pitch * (size_t) h;
         p.cr = uv_offset ? uv_offset : p.plane;
     }
@@ -329,6 +338,68 @@ GLB_HD ExportZero export_zero10(const ExportFmt& f) {
     return { y[0], u[0], v[0] };
 }
 
+// ---- 4:2:2: yuv422p, yuv422p10le and UYVY (DESIGN 4.18) -------------------------------------------------------------------
+// The chroma of a horizontal pixel pair (c0, c1) is the 4:2:0 chroma of the 2x2 block whose two rows are that pair, so no
+// new rounding enters: 8 bits export_cbcr of export_avg4(c0, c1, c0, c1) (per channel (2a + 2b + 2) >> 2 = (a + b + 1) >> 1,
+// NV12's chroma), 10 bits export_cbcr10 of export_sum4(c0, c1, c0, c1) (P010's exact-sum chroma, sums <= 1020).  Y is
+// export_y / export_y10 per pixel.
+// YUV422P of one row's quad: its four Y bytes, and the (Cb, Cr) pairs of its two pixel pairs as NV12's word (Cb0, Cr0, Cb1,
+// Cr1; export_cb_pair / export_cr_pair split it into the planes' bytes)
+template <int E = 0>
+GLB_HD uint32_t export_422_quad(const ExportFmt& f, const uint32_t in[4], uint32_t* y) {
+    uint32_t c[4];
+    *y = 0u;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        c[k] = export_over(in[k], f.bg, f.native);
+        *y |= export_y<E>(c[k]) << (8 * k);
+    }
+    return export_cbcr<E>(export_avg4(c[0], c[1], c[0], c[1])) | (export_cbcr<E>(export_avg4(c[2], c[3], c[2], c[3])) << 16);
+}
+// UYVY of the same: the Y word and the CbCr word interleaved as Cb, Y0, Cr, Y1 per pixel pair, one word per pair
+GLB_HD void export_uyvy_words(uint32_t y, uint32_t uv, uint32_t w[2]) {
+    w[0] = (uv & 0xffu) | ((y & 0xffu) << 8) | ((uv & 0xff00u) << 8) | ((y & 0xff00u) << 16);
+    w[1] = ((uv >> 16) & 0xffu) | (((y >> 16) & 0xffu) << 8) | (((uv >> 24) & 0xffu) << 16) | (y & 0xff000000u);
+}
+// and back: the Y word and the CbCr word of two UYVY words
+GLB_HD void export_uyvy_split(const uint32_t w[2], uint32_t* y, uint32_t* uv) {
+    *y = ((w[0] >> 8) & 0xffu) | ((w[0] >> 16) & 0xff00u) | ((w[1] << 8) & 0xff0000u) | (w[1] & 0xff000000u);
+    *uv = (w[0] & 0xffu) | ((w[0] >> 8) & 0xff00u) | ((w[1] & 0xffu) << 16) | ((w[1] << 8) & 0xff000000u);
+}
+// yuv422p10le of one row's quad: its four Y samples as two words, and the Cb samples and the Cr samples of its two pixel
+// pairs, one word each
+template <int E = 0>
+GLB_HD void export_422p10_quad(const ExportFmt& f, const uint32_t in[4], uint32_t y[2], uint32_t* cb, uint32_t* cr) {
+    uint32_t c[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) c[k] = export_over(in[k], f.bg, f.native);
+#pragma unroll
+    for (int k = 0; k < 2; ++k) y[k] = export_y10<E>(c[2 * k]) | (export_y10<E>(c[2 * k + 1]) << 16);
+    const uint32_t c0 = export_cbcr10<E>(export_sum4(c[0], c[1], c[0], c[1]));
+    const uint32_t c1 = export_cbcr10<E>(export_sum4(c[2], c[3], c[2], c[3]));
+    *cb = (c0 & 0xffffu) | (c1 << 16);
+    *cr = (c0 >> 16) | (c1 & 0xffff0000u);
+}
+// export_zero of the 4:2:2 formats: YUV422P y the Y word, u and v the Cb and Cr pairs; YUV422P10 y one of the two equal Y
+// words, u and v the Cb and Cr words; UYVY y the word of a pixel pair (u, v unused)
+template <int E = 0>
+GLB_HD ExportZero export_zero422(const ExportFmt& f) {
+    const uint32_t z[4] = { 0u, 0u, 0u, 0u };
+    ExportZero o = { 0u, 0u, 0u };
+    if (f.format == GLAVA_B200_EXPORT_YUV422P10) {
+        uint32_t y[2];
+        export_422p10_quad<E>(f, z, y, &o.u, &o.v);
+        o.y = y[0];
+    } else {
+        uint32_t y, w[2];
+        const uint32_t uv = export_422_quad<E>(f, z, &y);
+        export_uyvy_words(y, uv, w);
+        if (f.format == GLAVA_B200_EXPORT_UYVY) o.y = w[0];
+        else { o.y = y; o.u = export_cb_pair(uv); o.v = export_cr_pair(uv); }
+    }
+    return o;
+}
+
 // ---- mark-aware reads ----------------------------------------------------------------------------------------------------
 // When the last raster pass kept dirty-row marks (capi.cu mark_key != 0), slot s of the framebuffer has one word per (band of
 // `rows` rows, 128-pixel strip) at the band's first row (raster_core.h dirty_pack): rows [lo, hi) of the band may be non-zero,
@@ -432,6 +503,20 @@ GLB_HD uint64_t ladder_unit(int rung, int row, int col) { return ((uint64_t) run
 GLB_HD int ladder_unit_rung(uint64_t u) { return (int) (u >> 56); }
 GLB_HD int ladder_unit_row(uint64_t u) { return (int) ((u >> 28) & 0xfffffffu); }
 GLB_HD int ladder_unit_col(uint64_t u) { return (int) (u & 0xfffffffu); }
+// The kernel a ladder launches, from its rungs' formats and encodings (host code): export_ladder_422_kernel when a rung is
+// 4:2:2, else export_ladder_p10_kernel when one is planar 10-bit, else export_ladder_enc_kernel when one has an encoding
+// other than 0, else export_ladder_yuv_kernel when one is I420, YUV444 or P010, else export_ladder_kernel
+enum LadderKernel { ladder_plain = 0, ladder_yuv = 1, ladder_enc = 2, ladder_p10 = 3, ladder_422 = 4 };
+inline int ladder_kernel(const int* format, const int* enc, int n) {
+    bool yuv = false, e = false, p10 = false, k422 = false;
+    for (int j = 0; j < n; ++j) {
+        yuv |= format[j] != GLAVA_B200_EXPORT_NV12 && export_yuv(format[j]);
+        e |= enc[j] != 0;
+        p10 |= export_p10(format[j]);
+        k422 |= export_422(format[j]);
+    }
+    return k422 ? ladder_422 : p10 ? ladder_p10 : e ? ladder_enc : yuv ? ladder_yuv : ladder_plain;
+}
 
 // ---- overlay (DESIGN 4.12): the frame composited onto the caller's image ----------------------------------------------------
 // Native opacity only (any other opacity writes export_frames' opaque bytes).  The premultiplied "over" GLava's window
@@ -652,6 +737,42 @@ GLB_HD void overlay_444p10_quad(const uint32_t in[4], uint32_t y[2], uint32_t cb
     }
     cb[0] = u[0] | (u[1] << 16); cb[1] = u[2] | (u[3] << 16);
     cr[0] = v[0] | (v[1] << 16); cr[1] = v[2] | (v[3] << 16);
+}
+
+// ---- overlay onto 4:2:2 pictures (DESIGN 4.18) ----------------------------------------------------------------------------
+// The chroma of a pixel pair (p0, p1) is the 4:2:0 blend of the block whose two rows are that pair: 8 bits overlay_cbcr of
+// overlay_avg4(p0, p1, p0, p1), 10 bits overlay_cbcr10 of its sums.  A zero pair leaves its chroma (8 bits: overlay_cbcr of
+// 0 is uvd exactly), an opaque pair gives export_422_quad's / export_422p10_quad's chroma.
+// YUV422P (and UYVY, through export_uyvy_split) of one row's quad over the Y word y and the CbCr word uv (NV12's layout)
+template <int E = 0>
+GLB_HD void overlay_422_quad(const uint32_t in[4], uint32_t* y, uint32_t* uv) {
+    uint32_t oy = 0u;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) oy |= overlay_y<E>(in[k], (*y >> (8 * k)) & 255u) << (8 * k);
+    *y = oy;
+    *uv = overlay_cbcr<E>(overlay_avg4(in[0], in[1], in[0], in[1]), *uv & 0xffffu) |
+          (overlay_cbcr<E>(overlay_avg4(in[2], in[3], in[2], in[3]), *uv >> 16) << 16);
+}
+// YUV422P10 of one row's quad over the Y words y[2] and the Cb and Cr words cb, cr (two samples each); the chroma sample by
+// sample, as overlay_p10_quad's planar chroma
+template <int E = 0>
+GLB_HD void overlay_422p10_quad(const uint32_t in[4], uint32_t y[2], uint32_t* cb, uint32_t* cr) {
+#pragma unroll
+    for (int k = 0; k < 2; ++k) y[k] = overlay_y10_word<E, false>(in[2 * k], in[2 * k + 1], y[k]);
+    uint32_t u[2], v[2];
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+        const uint32_t p0 = in[2 * k], p1 = in[2 * k + 1];
+        u[k] = (*cb >> (16 * k)) & 0xffffu;
+        v[k] = (*cr >> (16 * k)) & 0xffffu;
+        if ((p0 | p1) != 0u) {
+            const uint32_t c = overlay_cbcr10<E>(export_sum4(p0, p1, p0, p1), overlay_asum4(p0, p1, p0, p1), u[k] & 1023u, v[k] & 1023u);
+            u[k] = c & 0xffffu;
+            v[k] = c >> 16;
+        }
+    }
+    *cb = u[0] | (u[1] << 16);
+    *cr = v[0] | (v[1] << 16);
 }
 
 }  // namespace glb

@@ -15,7 +15,8 @@
 // (DESIGN 4.13) is export_ladder_kernel: every rung of every entry in one launch, each unit run by the per-item body of
 // the rung's standalone kernel.  I420, YUV 4:4:4 and P010 (DESIGN 4.14) run kernels of their own with the same items
 // (export_yuv_kernel, export_scaled_yuv_kernel, export_ladder_yuv_kernel), as do the planar 10-bit formats (DESIGN 4.16:
-// export_p10_kernel, export_scaled_p10_kernel, export_ladder_p10_kernel).  The host half is export.cpp.
+// export_p10_kernel, export_scaled_p10_kernel, export_ladder_p10_kernel) and the 4:2:2 formats (DESIGN 4.18:
+// export_422_kernel, export_scaled_422_kernel, export_ladder_422_kernel).  The host half is export.cpp.
 #include "internal.h"
 #include "export_core.h"
 
@@ -416,10 +417,115 @@ static void launch_p10(const ExportArgs& a, unsigned blocks, cudaStream_t st) {
     });
 }
 
+// ---- 4:2:2: YUV422P, YUV422P10 and UYVY (DESIGN 4.18) ----------------------------------------------------------------------
+// export_kernel's items once more (output row pair x 128-pixel strip, a quad per lane), each row converted on its own, so an
+// odd h leaves the last pair one row.  Per lane per row: YUV422P a 4-byte Y store and a 2-byte Cb and a 2-byte Cr store
+// (chroma rows pitch / 2 apart), YUV422P10 an 8-byte Y store and a 4-byte Cb and a 4-byte Cr store, UYVY one 8-byte store.
+// Past the last full quad the width is 4k + 2: the last pixel pair of a row.  All four encodings are instantiations of one
+// template, as the planar 10-bit kernels are.
+
+// One row of a 4:2:2 item: the quad q at x of output row r (dst: row 0's luma or UYVY bytes, cb: row 0's Cb, Cr `cr` bytes
+// further); full: a whole quad, else the last pixel pair; z what zero pixels become (export_zero422)
+template <int E>
+__device__ __forceinline__ void row_422(const ExportFmt& f, int fmt, const uint32_t q[4], uint8_t* dst, uint8_t* cb, size_t cr,
+                                        size_t pitch, int r, int x, bool full, const ExportZero& z) {
+    const bool any = (q[0] | q[1] | q[2] | q[3]) != 0u;
+    if (fmt == GLAVA_B200_EXPORT_UYVY) {
+        uint32_t w[2] = { z.y, z.y };
+        if (any) {
+            uint32_t y;
+            const uint32_t uv = export_422_quad<E>(f, q, &y);
+            export_uyvy_words(y, uv, w);
+        }
+        uint8_t* const p = dst + (size_t) r * pitch + 2 * (size_t) x;
+        if (full) __stcs(reinterpret_cast<uint2*>(p), make_uint2(w[0], w[1]));
+        else __stcs(reinterpret_cast<uint32_t*>(p), w[0]);
+    } else if (fmt == GLAVA_B200_EXPORT_YUV422P) {
+        uint32_t y = z.y, u = z.u, v = z.v;
+        if (any) {
+            const uint32_t uv = export_422_quad<E>(f, q, &y);
+            u = export_cb_pair(uv); v = export_cr_pair(uv);
+        }
+        uint8_t* const py = dst + (size_t) r * pitch + x;
+        uint8_t* const pu = cb + (size_t) r * (pitch >> 1) + (x >> 1);
+        if (full) {
+            __stcs(reinterpret_cast<uint32_t*>(py), y);
+            __stcs(reinterpret_cast<unsigned short*>(pu), (unsigned short) u);
+            __stcs(reinterpret_cast<unsigned short*>(pu + cr), (unsigned short) v);
+        } else {
+            __stcs(reinterpret_cast<unsigned short*>(py), (unsigned short) y);
+            __stcs(pu, (uint8_t) u);
+            __stcs(pu + cr, (uint8_t) v);
+        }
+    } else {                                                // YUV422P10
+        uint32_t y[2] = { z.y, z.y }, u = z.u, v = z.v;
+        if (any) export_422p10_quad<E>(f, q, y, &u, &v);
+        uint8_t* const py = dst + (size_t) r * pitch + 2 * (size_t) x;
+        uint8_t* const pu = cb + (size_t) r * (pitch >> 1) + x;   // x / 2 samples of 2 bytes
+        if (full) {
+            __stcs(reinterpret_cast<uint2*>(py), make_uint2(y[0], y[1]));
+            __stcs(reinterpret_cast<uint32_t*>(pu), u);
+            __stcs(reinterpret_cast<uint32_t*>(pu + cr), v);
+        } else {
+            __stcs(reinterpret_cast<uint32_t*>(py), y[0]);
+            __stcs(reinterpret_cast<unsigned short*>(pu), (unsigned short) u);
+            __stcs(reinterpret_cast<unsigned short*>(pu + cr), (unsigned short) v);
+        }
+    }
+}
+
+// One item of export_422_kernel (and of a ladder's whole-frame 4:2:2 rung), as p10_item.  A reads w, h, marks, mark_rows
+// and pitch.
+template <bool Keep, int E, typename A>
+__device__ __forceinline__ void item_422(const A& a, const ExportFmt& f, int fmt, const uint32_t* frame, int slot, uint8_t* dst,
+                                         uint8_t* cb, size_t cr, int j, int strip, int x, const ExportZero& z) {
+    const int y0 = a.h - 1 - 2 * j, y1 = y0 - 1;
+    uint32_t top[4] = { 0u, 0u, 0u, 0u }, bot[4] = { 0u, 0u, 0u, 0u };
+    if (row_read(a, slot, y0, strip)) load_quad<Keep>(frame, a.w, y0, x, top);
+    if (y1 >= 0 && row_read(a, slot, y1, strip)) load_quad<Keep>(frame, a.w, y1, x, bot);
+    const bool full = x + 4 <= a.w;
+    row_422<E>(f, fmt, top, dst, cb, cr, a.pitch, 2 * j, x, full, z);
+    if (y1 >= 0) row_422<E>(f, fmt, bot, dst, cb, cr, a.pitch, 2 * j + 1, x, full, z);
+}
+
+template <typename Index, int Fmt, int E>
+__global__ void __launch_bounds__(256) export_422_kernel(const __grid_constant__ ExportArgs a) {
+    const ExportFmt f = { Fmt, 1, a.native, a.bg };
+    const Index strips = (Index) ((a.w + 127) >> 7), per = strips * (Index) ((a.h + 1) >> 1);
+    const Index items = (Index) a.count * per;
+    const Index warps = (Index) (((size_t) gridDim.x * blockDim.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    const ExportZero z = export_zero422<E>(f);              // once per thread, as export_kernel's constants
+    for (Index it = (Index) (((size_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5); it < items; it += warps) {
+        const Index k = it / per, rem = it - k * per;
+        const int j = (int) (rem / strips), strip = (int) (rem - (Index) j * strips);
+        const int x = strip * 128 + lane * 4;
+        if (x >= a.w) continue;
+        const ExportEntry* e = a.list + k;
+        uint8_t* const dst = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst)));
+        const int slot = __ldg(&e->slot);
+        const uint32_t* frame = reinterpret_cast<const uint32_t*>(a.fb) + (size_t) slot * a.h * a.w;
+        item_422<false, E>(a, f, Fmt, frame, slot, dst, dst + a.uv_offset, a.cr_offset, j, strip, x, z);
+    }
+}
+
+template <typename Index>
+static void launch_422(const ExportArgs& a, unsigned blocks, cudaStream_t st) {
+    for_any_enc(a.enc, [&](auto e) {
+        constexpr int E = decltype(e)::value;
+        if (a.format == GLAVA_B200_EXPORT_YUV422P) export_422_kernel<Index, GLAVA_B200_EXPORT_YUV422P, E><<<blocks, 256, 0, st>>>(a);
+        else if (a.format == GLAVA_B200_EXPORT_YUV422P10) export_422_kernel<Index, GLAVA_B200_EXPORT_YUV422P10, E><<<blocks, 256, 0, st>>>(a);
+        else export_422_kernel<Index, GLAVA_B200_EXPORT_UYVY, E><<<blocks, 256, 0, st>>>(a);
+    });
+}
+
 int launch_export(const ExportArgs& a, void* stream) {
     const ExportGrid g = export_grid((uint64_t) a.count * (uint64_t) ((a.w + 127) >> 7) * (uint64_t) ((a.h + 1) >> 1));
     cudaStream_t st = (cudaStream_t) stream;
-    if (export_p10(a.format)) {
+    if (export_422(a.format)) {
+        if (g.narrow) launch_422<uint32_t>(a, g.blocks, st);
+        else launch_422<uint64_t>(a, g.blocks, st);
+    } else if (export_p10(a.format)) {
         if (g.narrow) launch_p10<uint32_t>(a, g.blocks, st);
         else launch_p10<uint64_t>(a, g.blocks, st);
     } else if (a.enc && a.format == GLAVA_B200_EXPORT_NV12) {
@@ -689,11 +795,83 @@ static void launch_scaled_p10(const ScaledArgs& a, unsigned blocks, cudaStream_t
     });
 }
 
+// One item of export_scaled_422_kernel (and of a ladder's other 4:2:2 rungs), as scaled_p10_item: output row u at column X
+// of the lane (out_w even: a pixel pair is an even lane and its right neighbour, whose pixel comes by shuffle).  The even
+// lane of a pair stores its chroma (UYVY: the pair's whole word).  The Cb plane is the entry's dst_uv, Cr `cr` bytes
+// further; E the encoding.
+template <bool Keep, int E, typename A>
+__device__ __forceinline__ void scaled_422_item(const A& a, const ExportFmt& f, int fmt, const ExportRecip& rcp, uint32_t zc,
+                                                size_t cr, const ExportEntryUV* e, int u, int X, int lane) {
+    const bool active = X < a.out_w;
+    const int slot = __ldg(&e->slot);
+    const uint32_t* frame = reinterpret_cast<const uint32_t*>(a.fb) + (size_t) slot * a.h * a.w;
+    const ExportSpan sx = export_span(active ? X : 0, a.src_w, a.out_w);
+    uint8_t* const dst = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst)));
+    const uint32_t px = scaled_px<Keep>(a, f, frame, slot, u, active, sx, rcp, zc);
+    const uint32_t px1 = __shfl_down_sync(0xffffffffu, px, 1);
+    if (!active) return;
+    if (fmt == GLAVA_B200_EXPORT_UYVY) {
+        if (!(lane & 1)) {
+            const uint32_t uv = export_cbcr<E>(export_avg4(px, px1, px, px1));
+            __stcs(reinterpret_cast<uint32_t*>(dst + (size_t) u * a.pitch + 2 * (size_t) X),
+                   (uv & 0xffu) | (export_y<E>(px) << 8) | ((uv & 0xff00u) << 8) | (export_y<E>(px1) << 24));
+        }
+        return;
+    }
+    uint8_t* const cb = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst_uv)));
+    if (fmt == GLAVA_B200_EXPORT_YUV422P) {
+        __stcs(dst + (size_t) u * a.pitch + X, (uint8_t) export_y<E>(px));
+        if (!(lane & 1)) {
+            const uint32_t uv = export_cbcr<E>(export_avg4(px, px1, px, px1));
+            uint8_t* const pu = cb + (size_t) u * (a.pitch >> 1) + (X >> 1);
+            __stcs(pu, (uint8_t) uv);
+            __stcs(pu + cr, (uint8_t) (uv >> 8));
+        }
+    } else {                                                // YUV422P10
+        __stcs(reinterpret_cast<unsigned short*>(dst + (size_t) u * a.pitch + 2 * (size_t) X), (unsigned short) export_y10<E>(px));
+        if (!(lane & 1)) {
+            const uint32_t uv = export_cbcr10<E>(export_sum4(px, px1, px, px1));
+            uint8_t* const pu = cb + (size_t) u * (a.pitch >> 1) + X;   // X / 2 samples of 2 bytes
+            __stcs(reinterpret_cast<unsigned short*>(pu), (unsigned short) uv);
+            __stcs(reinterpret_cast<unsigned short*>(pu + cr), (unsigned short) (uv >> 16));
+        }
+    }
+}
+
+template <typename Index, int Fmt, int E>
+__global__ void __launch_bounds__(256) export_scaled_422_kernel(const __grid_constant__ ScaledArgs a) {
+    const ExportFmt f = { Fmt, 1, a.native, a.bg };
+    const ExportRecip rcp = { a.div_mul, a.div_shift };
+    const uint32_t zc = export_over(0u, f.bg, f.native);    // what a zero pixel becomes
+    const Index runs = (Index) ((a.out_w + 31) >> 5), per = runs * (Index) a.out_h;
+    const Index items = (Index) a.count * per;
+    const Index warps = (Index) (((size_t) gridDim.x * blockDim.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    for (Index it = (Index) (((size_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5); it < items; it += warps) {
+        const Index k = it / per, rem = it - k * per;
+        const int u = (int) (rem / runs), X = (int) (rem - (Index) u * runs) * 32 + lane;
+        scaled_422_item<false, E>(a, f, Fmt, rcp, zc, a.cr_offset, a.list + k, u, X, lane);
+    }
+}
+
+template <typename Index>
+static void launch_scaled_422(const ScaledArgs& a, unsigned blocks, cudaStream_t st) {
+    for_any_enc(a.enc, [&](auto e) {
+        constexpr int E = decltype(e)::value;
+        if (a.format == GLAVA_B200_EXPORT_YUV422P) export_scaled_422_kernel<Index, GLAVA_B200_EXPORT_YUV422P, E><<<blocks, 256, 0, st>>>(a);
+        else if (a.format == GLAVA_B200_EXPORT_YUV422P10) export_scaled_422_kernel<Index, GLAVA_B200_EXPORT_YUV422P10, E><<<blocks, 256, 0, st>>>(a);
+        else export_scaled_422_kernel<Index, GLAVA_B200_EXPORT_UYVY, E><<<blocks, 256, 0, st>>>(a);
+    });
+}
+
 int launch_export_scaled(const ScaledArgs& a, void* stream) {
     const uint64_t units = export_420(a.format) ? (uint64_t) (a.out_h >> 1) : (uint64_t) a.out_h;
     const ExportGrid g = export_grid((uint64_t) a.count * (uint64_t) ((a.out_w + 31) >> 5) * units);
     cudaStream_t st = (cudaStream_t) stream;
-    if (export_p10(a.format)) {
+    if (export_422(a.format)) {
+        if (g.narrow) launch_scaled_422<uint32_t>(a, g.blocks, st);
+        else launch_scaled_422<uint64_t>(a, g.blocks, st);
+    } else if (export_p10(a.format)) {
         if (g.narrow) launch_scaled_p10<uint32_t>(a, g.blocks, st);
         else launch_scaled_p10<uint64_t>(a, g.blocks, st);
     } else if (a.enc && a.format == GLAVA_B200_EXPORT_NV12) {
@@ -887,22 +1065,76 @@ __global__ void __launch_bounds__(256) export_ladder_p10_kernel(const __grid_con
     }
 }
 
+// One unit of a 4:2:2 rung of export_ladder_422_kernel under encoding E: the item of its standalone kernel
+// (export_422_kernel / export_scaled_422_kernel), as ladder_p10_item
+template <int E>
+__device__ __forceinline__ void ladder_422_item(const LadderArgs& a, const LadderRung& g, const ExportEntryUV* e, int rung, int row,
+                                                int col, int lane) {
+    const RungView v = { a.fb, a.marks, a.mark_rows, a.w, a.h, g.format, g.pitch, g.src_x, g.src_y, g.src_w, g.src_h, g.out_w, g.out_h };
+    const ExportFmt f = { g.format, g.over, a.native, g.bg };
+    const size_t cr = a.yuv[rung].cr_offset;
+    if (g.whole) {
+        const int x = col * 128 + lane * 4;
+        if (x >= a.w) return;
+        uint8_t* const dst = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst)));
+        uint8_t* const cb = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst_uv)));
+        const int slot = __ldg(&e->slot);
+        const uint32_t* frame = reinterpret_cast<const uint32_t*>(a.fb) + (size_t) slot * a.h * a.w;
+        const ExportZero z = { a.yuv[rung].zy, a.yuv[rung].zu, a.yuv[rung].zv };
+        item_422<true, E>(v, f, g.format, frame, slot, dst, cb, cr, row, col, x, z);
+    } else {
+        const ExportRecip rcp = { g.div_mul, g.div_shift };
+        scaled_422_item<true, E>(v, f, g.format, rcp, g.zc, cr, e, row, col * 32 + lane, lane);
+    }
+}
+
+// Any format and encoding per rung, launched only when a rung is YUV422P, YUV422P10 or UYVY (DESIGN 4.18): 4:2:2 units run
+// ladder_422_item, planar 10-bit units ladder_p10_item, the others ladder_item, each in its rung's encoding, so that
+// export_ladder_p10_kernel and the older ladder kernels keep their machine code
+template <typename Index>
+__global__ void __launch_bounds__(256) export_ladder_422_kernel(const __grid_constant__ LadderArgs a) {
+    const Index units = (Index) a.units, items = (Index) a.count * units;
+    const Index warps = (Index) (((size_t) gridDim.x * blockDim.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    for (Index it = (Index) (((size_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5); it < items; it += warps) {
+        const Index k = it / units;
+        const uint64_t unit = __ldg(reinterpret_cast<const unsigned long long*>(a.sched) + (it - k * units));
+        const int rung = ladder_unit_rung(unit), row = ladder_unit_row(unit), col = ladder_unit_col(unit);
+        const LadderRung& g = a.rung[rung];
+        const ExportEntryUV* e = a.list + (size_t) k * a.nrungs + rung;
+        if (export_422(g.format)) {
+            if (g.enc == 1) ladder_422_item<1>(a, g, e, rung, row, col, lane);
+            else if (g.enc == 2) ladder_422_item<2>(a, g, e, rung, row, col, lane);
+            else if (g.enc == 3) ladder_422_item<3>(a, g, e, rung, row, col, lane);
+            else ladder_422_item<0>(a, g, e, rung, row, col, lane);
+        } else if (export_p10(g.format)) {
+            if (g.enc == 1) ladder_p10_item<1>(a, g, e, rung, row, col, lane);
+            else if (g.enc == 2) ladder_p10_item<2>(a, g, e, rung, row, col, lane);
+            else if (g.enc == 3) ladder_p10_item<3>(a, g, e, rung, row, col, lane);
+            else ladder_p10_item<0>(a, g, e, rung, row, col, lane);
+        } else if (g.enc == 1) ladder_item<true, 1>(a, g, e, rung, row, col, lane);
+        else if (g.enc == 2) ladder_item<true, 2>(a, g, e, rung, row, col, lane);
+        else if (g.enc == 3) ladder_item<true, 3>(a, g, e, rung, row, col, lane);
+        else ladder_item<true, 0>(a, g, e, rung, row, col, lane);
+    }
+}
+
 int launch_export_ladder(const LadderArgs& a, void* stream) {
     const ExportGrid g = export_grid((uint64_t) a.count * (uint64_t) a.units);
-    bool yuv = false, enc = false, p10 = false;
-    for (int j = 0; j < a.nrungs; ++j) {
-        yuv |= a.rung[j].format != GLAVA_B200_EXPORT_NV12 && export_yuv(a.rung[j].format);
-        enc |= a.rung[j].enc != 0;
-        p10 |= export_p10(a.rung[j].format);
-    }
+    int format[GLAVA_B200_LADDER_MAX], enc[GLAVA_B200_LADDER_MAX];
+    for (int j = 0; j < a.nrungs; ++j) { format[j] = a.rung[j].format; enc[j] = a.rung[j].enc; }
+    const int kind = ladder_kernel(format, enc, a.nrungs);
     cudaStream_t st = (cudaStream_t) stream;
-    if (p10) {
+    if (kind == ladder_422) {
+        if (g.narrow) export_ladder_422_kernel<uint32_t><<<g.blocks, 256, 0, st>>>(a);
+        else export_ladder_422_kernel<uint64_t><<<g.blocks, 256, 0, st>>>(a);
+    } else if (kind == ladder_p10) {
         if (g.narrow) export_ladder_p10_kernel<uint32_t><<<g.blocks, 256, 0, st>>>(a);
         else export_ladder_p10_kernel<uint64_t><<<g.blocks, 256, 0, st>>>(a);
-    } else if (enc) {
+    } else if (kind == ladder_enc) {
         if (g.narrow) export_ladder_enc_kernel<uint32_t><<<g.blocks, 256, 0, st>>>(a);
         else export_ladder_enc_kernel<uint64_t><<<g.blocks, 256, 0, st>>>(a);
-    } else if (yuv) {
+    } else if (kind == ladder_yuv) {
         if (g.narrow) export_ladder_yuv_kernel<uint32_t><<<g.blocks, 256, 0, st>>>(a);
         else export_ladder_yuv_kernel<uint64_t><<<g.blocks, 256, 0, st>>>(a);
     } else if (g.narrow) export_ladder_kernel<uint32_t><<<g.blocks, 256, 0, st>>>(a);
@@ -1133,7 +1365,8 @@ int launch_overlay(const OverlayArgs& a, void* stream) {
 // chroma pitch per call.  NV12 runs overlay_frames' own item body (overlay_nv12); I420, P010 and YUV420P10 walk row pairs as
 // NV12 does; YUV444 and YUV444P10 walk rows as RGBA does.  Native opacity blends (export_core.h overlay_*_quad) and leaves
 // all-zero quads alone; any other opacity writes export_frames' bytes of the format.  Tails: the last two pixels of a row
-// for the 4:2:0 formats (w even), sample by sample for the 4:4:4 ones.  One kernel per format and encoding.
+// for the 4:2:0 formats (w even), sample by sample for the 4:4:4 ones.  One kernel per format and encoding.  The 4:2:2
+// formats (DESIGN 4.18) walk rows through row422, each row's pixel pairs blended as 4:2:0 blocks of that pair, w even.
 
 // the first n (1..4) bytes at p as a word (n == 4: p is 4-byte aligned)
 __device__ __forceinline__ uint32_t load_bytes(const uint8_t* p, int n) {
@@ -1160,7 +1393,10 @@ struct OverlayPlanesBody {
     static constexpr bool k420 = Fmt == GLAVA_B200_EXPORT_NV12 || Fmt == GLAVA_B200_EXPORT_I420 || Fmt == GLAVA_B200_EXPORT_P010 ||
                                  Fmt == GLAVA_B200_EXPORT_YUV420P10;
     static constexpr bool kPlanar = Fmt == GLAVA_B200_EXPORT_I420 || Fmt == GLAVA_B200_EXPORT_YUV444 || Fmt == GLAVA_B200_EXPORT_YUV420P10 ||
-                                    Fmt == GLAVA_B200_EXPORT_YUV444P10;
+                                    Fmt == GLAVA_B200_EXPORT_YUV444P10 || Fmt == GLAVA_B200_EXPORT_YUV422P ||
+                                    Fmt == GLAVA_B200_EXPORT_YUV422P10;
+    // 4:2:2 (DESIGN 4.18) walks rows as 4:4:4 does, through row422; UYVY has no chroma plane
+    static constexpr bool k422 = Fmt == GLAVA_B200_EXPORT_YUV422P || Fmt == GLAVA_B200_EXPORT_YUV422P10 || Fmt == GLAVA_B200_EXPORT_UYVY;
     struct Chroma { uint8_t* cb; uint8_t* cr; };
     const OverlayPlanesArgs& a;
     ExportFmt f;                                            // any other opacity: the stored colour, alpha 255
@@ -1170,7 +1406,10 @@ struct OverlayPlanesBody {
     }
     static __device__ __forceinline__ uint8_t* dst(const OverlayPlanesEntry* e) { return plane(e, 0); }
     __device__ __forceinline__ bool pairs() const { return k420; }
-    __device__ __forceinline__ Chroma chroma(const OverlayPlanesEntry* e) const { return { plane(e, 1), kPlanar ? plane(e, 2) : nullptr }; }
+    __device__ __forceinline__ Chroma chroma(const OverlayPlanesEntry* e) const {
+        if constexpr (Fmt == GLAVA_B200_EXPORT_UYVY) return { nullptr, nullptr };
+        else return { plane(e, 1), kPlanar ? plane(e, 2) : nullptr };
+    }
 
     // 4:4:4: the quad at x of output row r (native: blended, all zero: untouched)
     __device__ __forceinline__ void row444(bool native, uint8_t* dst, Chroma c, int r, int x, const uint32_t q[4]) const {
@@ -1278,8 +1517,75 @@ struct OverlayPlanesBody {
         }
     }
 
+    // 4:2:2: the quad at x of output row r (native: blended, all zero: untouched); w even, so past the last full quad the
+    // last pixel pair of a row
+    __device__ __forceinline__ void row422(bool native, uint8_t* dst, Chroma c, int r, int x, const uint32_t q[4]) const {
+        if (native && (q[0] | q[1] | q[2] | q[3]) == 0u) return;
+        const bool full = x + 4 <= a.w;
+        if (Fmt == GLAVA_B200_EXPORT_UYVY) {
+            uint8_t* const p = dst + (size_t) r * a.pitch + 2 * (size_t) x;
+            uint32_t w[2] = { 0u, 0u }, y, uv;
+            if (native) {
+                if (full) {
+                    const uint2 d = __ldcs(reinterpret_cast<const uint2*>(p));
+                    w[0] = d.x; w[1] = d.y;
+                } else {
+                    w[0] = __ldcs(reinterpret_cast<const uint32_t*>(p));
+                }
+                export_uyvy_split(w, &y, &uv);
+                overlay_422_quad<E>(q, &y, &uv);
+            } else {
+                uv = export_422_quad<E>(f, q, &y);
+            }
+            export_uyvy_words(y, uv, w);
+            if (full) __stcs(reinterpret_cast<uint2*>(p), make_uint2(w[0], w[1]));
+            else __stcs(reinterpret_cast<uint32_t*>(p), w[0]);
+        } else if (Fmt == GLAVA_B200_EXPORT_YUV422P) {
+            uint8_t* const py = dst + (size_t) r * a.pitch + x;
+            uint8_t* const pu = c.cb + (size_t) r * a.chroma_pitch + (x >> 1);
+            uint8_t* const pv = c.cr + (size_t) r * a.chroma_pitch + (x >> 1);
+            uint32_t y, u, v;
+            if (native) {
+                y = load_bytes(py, full ? 4 : 2); u = load_bytes(pu, full ? 2 : 1); v = load_bytes(pv, full ? 2 : 1);
+                uint32_t uv = (u & 0xffu) | ((v & 0xffu) << 8) | ((u & 0xff00u) << 8) | ((v & 0xff00u) << 16);
+                overlay_422_quad<E>(q, &y, &uv);
+                u = export_cb_pair(uv); v = export_cr_pair(uv);
+            } else {
+                const uint32_t uv = export_422_quad<E>(f, q, &y);
+                u = export_cb_pair(uv); v = export_cr_pair(uv);
+            }
+            store_bytes(py, y, full ? 4 : 2); store_bytes(pu, u, full ? 2 : 1); store_bytes(pv, v, full ? 2 : 1);
+        } else {                                            // YUV422P10
+            uint8_t* const py = dst + (size_t) r * a.pitch + 2 * (size_t) x;
+            uint8_t* const pu = c.cb + (size_t) r * a.chroma_pitch + x;   // x / 2 samples of 2 bytes
+            uint8_t* const pv = c.cr + (size_t) r * a.chroma_pitch + x;
+            uint32_t y[2] = { 0u, 0u }, u, v;
+            if (native) {
+                if (full) {
+                    const uint2 d = __ldcs(reinterpret_cast<const uint2*>(py));
+                    y[0] = d.x; y[1] = d.y;
+                    u = __ldcs(reinterpret_cast<const uint32_t*>(pu)); v = __ldcs(reinterpret_cast<const uint32_t*>(pv));
+                } else {
+                    y[0] = __ldcs(reinterpret_cast<const uint32_t*>(py));
+                    u = __ldcs(reinterpret_cast<const unsigned short*>(pu)); v = __ldcs(reinterpret_cast<const unsigned short*>(pv));
+                }
+                overlay_422p10_quad<E>(q, y, &u, &v);
+            } else {
+                export_422p10_quad<E>(f, q, y, &u, &v);
+            }
+            if (full) {
+                __stcs(reinterpret_cast<uint2*>(py), make_uint2(y[0], y[1]));
+                __stcs(reinterpret_cast<uint32_t*>(pu), u); __stcs(reinterpret_cast<uint32_t*>(pv), v);
+            } else {
+                __stcs(reinterpret_cast<uint32_t*>(py), y[0]);
+                __stcs(reinterpret_cast<unsigned short*>(pu), (unsigned short) u); __stcs(reinterpret_cast<unsigned short*>(pv), (unsigned short) v);
+            }
+        }
+    }
+
     __device__ __forceinline__ void row(const OverlayPlanesEntry* e, uint8_t* dst, int r, int x, const uint32_t q[4]) const {
-        row444(true, dst, chroma(e), r, x, q);
+        if constexpr (k422) row422(true, dst, chroma(e), r, x, q);
+        else row444(true, dst, chroma(e), r, x, q);
     }
     __device__ __forceinline__ void pair(uint8_t* dst, Chroma c, int j, int x, const uint32_t top[4], const uint32_t bot[4]) const {
         pair420(true, dst, c, j, x, top, bot);
@@ -1289,6 +1595,9 @@ struct OverlayPlanesBody {
         const Chroma c = chroma(e);
         if (k420) {
             pair420(a.native, dst, c, u, x, top, bot);
+        } else if constexpr (k422) {
+            row422(a.native, dst, c, 2 * u, x, top);
+            if (y1 >= 0) row422(a.native, dst, c, 2 * u + 1, x, bot);
         } else {
             row444(a.native, dst, c, 2 * u, x, top);
             if (y1 >= 0) row444(a.native, dst, c, 2 * u + 1, x, bot);
@@ -1326,6 +1635,9 @@ int launch_overlay_planes(const OverlayPlanesArgs& a, void* stream) {
     case GLAVA_B200_EXPORT_P010: launch_planes<GLAVA_B200_EXPORT_P010>(a, g, st); break;
     case GLAVA_B200_EXPORT_YUV420P10: launch_planes<GLAVA_B200_EXPORT_YUV420P10>(a, g, st); break;
     case GLAVA_B200_EXPORT_YUV444P10: launch_planes<GLAVA_B200_EXPORT_YUV444P10>(a, g, st); break;
+    case GLAVA_B200_EXPORT_YUV422P: launch_planes<GLAVA_B200_EXPORT_YUV422P>(a, g, st); break;
+    case GLAVA_B200_EXPORT_YUV422P10: launch_planes<GLAVA_B200_EXPORT_YUV422P10>(a, g, st); break;
+    case GLAVA_B200_EXPORT_UYVY: launch_planes<GLAVA_B200_EXPORT_UYVY>(a, g, st); break;
     default: return fail(GLAVA_B200_EINVAL, "planes overlay launch: format %d", a.format);
     }
     return launch_status("planes overlay");

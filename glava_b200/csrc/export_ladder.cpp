@@ -32,13 +32,13 @@ int ladder_check(glava_b200* r, const int* streams, int count, const glava_b200_
     for (int j = 0; j < nrungs; ++j) {
         char name[96];
         snprintf(name, sizeof(name), "%s: rung %d", who, j);
-        const bool yuv = export_ycbcr(rungs[j].desc.format);
+        const bool yuv = export_chroma_planes(rungs[j].desc.format);
         for (int i = 0; i < count; ++i) {
             d[i] = dst[(size_t) i * nrungs + j];
             uv[i] = dst_uv ? dst_uv[(size_t) i * nrungs + j] : nullptr;
             if (uv[i] && !yuv)
-                return fail(GLAVA_B200_EINVAL, "%s: dst_uv[%d] is for NV12 only, or I420, YUV444, P010, YUV420P10 and YUV444P10 "
-                            "(entry %d)", name,
+                return fail(GLAVA_B200_EINVAL, "%s: dst_uv[%d] is for NV12 only, or I420, YUV444, P010, YUV420P10, YUV444P10, "
+                            "YUV422P and YUV422P10 (entry %d)", name,
                             i * nrungs + j, i);
         }
         rc = export_check(ExportKind::scaled, r, streams, count, d.data(), dst_uv && yuv ? uv.data() : nullptr, &rungs[j].desc,
@@ -48,14 +48,14 @@ int ladder_check(glava_b200* r, const int* streams, int count, const glava_b200_
     return 0;
 }
 
-// What zero pixels become in a rung under encoding E: NV12's zy / zuv into g, and export_zero (planar 10-bit: export_zero10)
-// for the other Y'CbCr formats
+// What zero pixels become in a rung under encoding E: NV12's zy / zuv into g, and export_zero (planar 10-bit: export_zero10;
+// 4:2:2: export_zero422) for the other Y'CbCr formats
 template <int E>
 static ExportZero rung_zero(const ExportFmt& f, LadderRung* g) {
     const uint32_t zero4[4] = { 0u, 0u, 0u, 0u };
     uint32_t zy1;
     g->zuv = export_nv12_quad<E>(f, zero4, zero4, &g->zy, &zy1);
-    return export_p10(f.format) ? export_zero10<E>(f) : export_zero<E>(f);
+    return export_422(f.format) ? export_zero422<E>(f) : export_p10(f.format) ? export_zero10<E>(f) : export_zero<E>(f);
 }
 
 // the device schedule for `geom`, built and uploaded on the raster stream when the geometry differs from the last ladder's
@@ -112,7 +112,7 @@ int ladder_run(glava_b200* r, const int* streams, int count, const glava_b200_ex
         for (int j = 0; j < nrungs; ++j) {
             const size_t e = (size_t) i * nrungs + j;
             uint8_t* const d = (uint8_t*) dst[e];
-            uint8_t* const uv = !export_ycbcr(rungs[j].desc.format) ? nullptr : dst_uv ? (uint8_t*) dst_uv[e] : d + planes[j].cb;
+            uint8_t* const uv = !export_chroma_planes(rungs[j].desc.format) ? nullptr : dst_uv ? (uint8_t*) dst_uv[e] : d + planes[j].cb;
             host[e] = { d, uv, slot, 0 };
         }
     }

@@ -1,4 +1,4 @@
-// overlay_planes.cpp — the host half of glava_b200_overlay_planes (DESIGN 4.17): the overlay onto decoded pictures, whose
+// overlay_planes.cpp — the host half of glava_b200_overlay_planes (DESIGN 4.17, 4.18): the overlay onto decoded pictures, whose
 // planes each have their own pointer and whose luma and chroma rows have their own pitches.  Its checks, the overlap test
 // of rectangles with two pitches, the list fill and one launch of overlay_planes_kernel (export_kernels.cu) through
 // export_list.h's enqueue.  Kept apart from export.cpp so that the other exports build and link without this launcher.
@@ -24,6 +24,9 @@ const char* planes_format_name(int format) {
     case GLAVA_B200_EXPORT_P010: return "P010";
     case GLAVA_B200_EXPORT_YUV420P10: return "YUV420P10";
     case GLAVA_B200_EXPORT_YUV444P10: return "YUV444P10";
+    case GLAVA_B200_EXPORT_YUV422P: return "YUV422P";
+    case GLAVA_B200_EXPORT_YUV422P10: return "YUV422P10";
+    case GLAVA_B200_EXPORT_UYVY: return "UYVY";
     default: return nullptr;
     }
 }
@@ -43,16 +46,25 @@ int planes_geometry(int w, int h, const glava_b200_overlay_planes_desc& d, Plane
     const uint32_t colour = GLAVA_B200_EXPORT_FULL_RANGE | GLAVA_B200_EXPORT_BT601;
     if (d.flags & ~colour)
         return fail(GLAVA_B200_EINVAL, "%s: flags 0x%x: the overlay takes none but EXPORT_FULL_RANGE and EXPORT_BT601", who, d.flags);
-    const bool c420 = export_420(fmt), wide = fmt == GLAVA_B200_EXPORT_P010 || export_p10(fmt);
+    const bool c420 = export_420(fmt), uyvy = fmt == GLAVA_B200_EXPORT_UYVY;
+    const bool wide = fmt == GLAVA_B200_EXPORT_P010 || export_p10(fmt) || fmt == GLAVA_B200_EXPORT_YUV422P10 || uyvy;
     if (c420 && ((w | h) & 1))
         return fail(GLAVA_B200_EINVAL, "%s: %s needs an even width and height, the frame is %dx%d", who, name, w, h);
-    g->planes = export_planar(fmt) ? 3 : 2;
-    g->luma_row = (size_t) w * (wide ? 2 : 1);
-    g->chroma_row = fmt == GLAVA_B200_EXPORT_I420 ? (size_t) w / 2
-                    : fmt == GLAVA_B200_EXPORT_P010 || fmt == GLAVA_B200_EXPORT_YUV444P10 ? (size_t) w * 2 : (size_t) w;
+    if (export_422(fmt) && (w & 1))
+        return fail(GLAVA_B200_EINVAL, "%s: %s needs an even width, the frame is %dx%d", who, name, w, h);
+    g->planes = uyvy ? 1 : export_planar(fmt) ? 3 : 2;
+    g->luma_row = (size_t) w * (wide ? 2 : 1);                // UYVY: its one plane, 2 bytes per pixel
+    g->chroma_row = fmt == GLAVA_B200_EXPORT_I420 || fmt == GLAVA_B200_EXPORT_YUV422P ? (size_t) w / 2
+                    : fmt == GLAVA_B200_EXPORT_P010 || fmt == GLAVA_B200_EXPORT_YUV444P10 ? (size_t) w * 2
+                    : uyvy ? 0 : (size_t) w;
     g->chroma_rows = c420 ? h / 2 : h;
     if (d.pitch % 16 || d.pitch < g->luma_row)
         return fail(GLAVA_B200_EINVAL, "%s: pitch %zu must be a multiple of 16 and at least %zu", who, d.pitch, g->luma_row);
+    if (uyvy) {
+        if (d.chroma_pitch)
+            return fail(GLAVA_B200_EINVAL, "%s: UYVY chroma_pitch %zu must be 0: UYVY has no chroma plane", who, d.chroma_pitch);
+        return 0;
+    }
     if (d.chroma_pitch % 16 || d.chroma_pitch < g->chroma_row)
         return fail(GLAVA_B200_EINVAL, "%s: %s chroma_pitch %zu must be a multiple of 16 and at least %zu", who, name, d.chroma_pitch,
                     g->chroma_row);
@@ -79,6 +91,9 @@ int planes_check(glava_b200* r, const int* streams, int count, const glava_b200_
         if (g.planes == 2 && pics[i].plane[2])
             return fail(GLAVA_B200_EINVAL, "%s: pics[%d].plane[2] must be NULL: %s has one interleaved chroma plane", who, i,
                         planes_format_name(desc->format));
+        if (g.planes == 1 && (pics[i].plane[1] || pics[i].plane[2]))
+            return fail(GLAVA_B200_EINVAL, "%s: pics[%d].plane[%d] must be NULL: UYVY has one packed plane", who, i,
+                        pics[i].plane[1] ? 1 : 2);
     }
     return 0;
 }

@@ -377,10 +377,20 @@ int   glava_b200_framebuffer_ipc(glava_b200* r, void* handle, size_t handle_byte
  *                              bit (DESIGN.md §4.16); w and h even, pitch a multiple of 32
  *     GLAVA_B200_EXPORT_YUV444P10  planar 10-bit 4:4:4 (yuv444p10le): Y, Cb and Cr planes of h rows x w uint16 at `pitch`
  *                              (>= 2 w), LSB-aligned; Y as YUV420P10's, Cb / Cr per composited pixel with no averaging
+ *     GLAVA_B200_EXPORT_YUV422P    planar 4:2:2 (yuv422p): Y plane of h rows x w bytes at `pitch`, then the Cb and Cr planes
+ *                              of h rows x w / 2 bytes at `pitch / 2`; Y as I420's, Cb / Cr of each horizontal pixel pair
+ *                              are I420's of the 2x2 block whose two rows are that pair (DESIGN.md §4.18); w even (any h),
+ *                              pitch a multiple of 32
+ *     GLAVA_B200_EXPORT_YUV422P10  planar 10-bit 4:2:2 (yuv422p10le, what ProRes 422 and DNxHR HQX encoders take): as
+ *                              YUV422P with LSB-aligned uint16 samples, Y rows of 2 w bytes and chroma rows of w bytes at
+ *                              `pitch / 2`; YUV420P10's arithmetic on the pair, as YUV422P's on I420's
+ *     GLAVA_B200_EXPORT_UYVY   packed 4:2:2 (ffmpeg's uyvy422, NDI's UYVY, DeckLink's 2vuy): one plane of h rows x 2 w
+ *                              bytes at `pitch`, each pixel pair the bytes Cb, Y0, Cr, Y1 of YUV422P; w even (any h)
  *   Where the chroma planes go: NV12 and P010 put the CbCr plane at `uv_offset` from dst[i] (0: pitch * h).  The planar
  *   formats (I420, YUV444, YUV420P10, YUV444P10) put the Cb plane right after the luma, at dst[i] + pitch * h, and
  *   `uv_offset` is the distance from Cb to Cr (0: the Cb plane's own size, so the planes sit back to back as a yuv420p /
- *   yuv444p buffer does); when set it is at least one chroma plane.  All YUV formats are composited (EXPORT_OVER implied).
+ *   yuv444p buffer does); when set it is at least one chroma plane.  YUV422P and YUV422P10 place their planes so too; UYVY
+ *   has no chroma plane, and its uv_offset is 0.  All YUV formats are composited (EXPORT_OVER implied).
  *   GLAVA_B200_EXPORT_OVER     (implied for the YUV formats) the opaque colour GLava's window shows over `background` (RGB8,
  *                              byte 3 unused): under setopacity "native" (premultiply_alpha) C = min(255, c +
  *                              mul_norm8(bg, 255 - a)) per channel; under any other opacity the stored colour (the window
@@ -394,16 +404,17 @@ int   glava_b200_framebuffer_ipc(glava_b200* r, void* handle, size_t handle_byte
  *                              YUV input, libjpeg-turbo's raw data, ffmpeg's yuvj420p).  Every grey has Cb = Cr = 128
  *                              (512).  RGBA / BGRA with either bit are GLAVA_B200_EINVAL (no matrix or range).
  *   dst[i], pitch and uv_offset are multiples of 16, pitch >= the row bytes, uv_offset (when set) >= pitch * h (planar
- *   formats: >= one chroma plane).  An unknown format or flag, odd NV12 / I420 / P010 / YUV420P10 dimensions, a misaligned
- *   or short pitch (I420, YUV420P10: not a multiple of 32), a null, host or other-device dst, a stream out of range, count
- *   < 1 and a renderer a failed rebuild left unbuilt are GLAVA_B200_EINVAL with nothing enqueued.  Formats 3 and 9 and
- *   above are unassigned.
+ *   formats: >= one chroma plane).  An unknown format or flag, odd NV12 / I420 / P010 / YUV420P10 dimensions, an odd
+ *   YUV422P / YUV422P10 / UYVY width, a misaligned or short pitch (I420, YUV420P10, YUV422P, YUV422P10: not a multiple of
+ *   32), a UYVY uv_offset other than 0, a null, host or other-device dst, a stream out of range, count < 1 and a renderer a
+ *   failed rebuild left unbuilt are GLAVA_B200_EINVAL with nothing enqueued.  Formats 3, 9 and 13 and above are
+ *   unassigned.
  *   The work runs on the handle's stream (glava_b200_cuda_stream) after the latest raster pass and before the next one can
  *   overwrite a slot, so an update issued right after this call cannot change what it exports.  `after_event` (a
  *   cudaEvent_t, or NULL): the export waits for it on the device before writing the destinations — it holds back the
  *   handle's stream, and so the next raster pass, until then.  `done_event` (or NULL) is recorded after the export.
  *   Returns once the work is enqueued, without a host wait.
- *   glava_b200_export_bytes    the bytes one destination spans for `desc` on this renderer (pitch * h; NV12 / P010:
+ *   glava_b200_export_bytes    the bytes one destination spans for `desc` on this renderer (pitch * h, UYVY included; NV12 / P010:
  *                              uv_offset + pitch * h / 2; the planar formats: pitch * h + the Cb to Cr distance + one
  *                              chroma plane), after the same descriptor checks.
  *   glava_b200_sharded_export_frames  the same with global stream indices, dst[i] on the device of the shard that owns
@@ -417,16 +428,19 @@ int   glava_b200_framebuffer_ipc(glava_b200* r, void* handle, size_t handle_byte
 #define GLAVA_B200_EXPORT_P010 6
 #define GLAVA_B200_EXPORT_YUV420P10 7
 #define GLAVA_B200_EXPORT_YUV444P10 8
+#define GLAVA_B200_EXPORT_YUV422P 10
+#define GLAVA_B200_EXPORT_YUV422P10 11
+#define GLAVA_B200_EXPORT_UYVY 12
 #define GLAVA_B200_EXPORT_OVER 1u
 #define GLAVA_B200_EXPORT_FULL_RANGE 0x100u
 #define GLAVA_B200_EXPORT_BT601 0x200u
 typedef struct {
     int      format;            /* GLAVA_B200_EXPORT_RGBA / _BGRA / _NV12 / _I420 / _YUV444 / _P010 / _YUV420P10 /
-                                   _YUV444P10 */
+                                   _YUV444P10 / _YUV422P / _YUV422P10 / _UYVY */
     uint32_t flags;             /* GLAVA_B200_EXPORT_OVER, and for the Y'CbCr formats _FULL_RANGE / _BT601 */
     uint8_t  background[4];     /* R, G, B of the opaque background the composite uses; byte 3 unused */
-    size_t   pitch;             /* bytes from one output row to the next (every plane; I420 / YUV420P10 chroma rows:
-                                   pitch / 2) */
+    size_t   pitch;             /* bytes from one output row to the next (every plane; I420 / YUV420P10 / YUV422P /
+                                   YUV422P10 chroma rows: pitch / 2) */
     size_t   uv_offset;         /* NV12 / P010: bytes from dst[i] to the CbCr plane, 0 = pitch * h; the planar formats:
                                    bytes from the Cb plane to the Cr plane, 0 = one chroma plane */
 } glava_b200_export;
@@ -446,7 +460,7 @@ int glava_b200_export_frames(glava_b200* r, const int* streams, int count, void*
  *                              first and alpha is 255.  NV12 is the export's arithmetic on the scaled image (Y per pixel,
  *                              chroma per 2x2 output block), so out_w and out_h are even; the other YUV formats likewise
  *                              apply their own arithmetic to the scaled image (out_w and out_h even for I420, P010 and
- *                              YUV420P10).
+ *                              YUV420P10; out_w even for YUV422P, YUV422P10 and UYVY).
  *     dst[i]                   out_h rows of out_w * 4 bytes (RGBA / BGRA), out_w bytes (Y) or out_w uint16 (P010 and
  *                              the planar 10-bit formats' Y), `pitch` bytes apart
  *     dst_uv                   NV12 / P010: dst_uv[i] receives the out_h / 2 CbCr rows (a mosaic tile's chroma need not sit
@@ -457,7 +471,8 @@ int glava_b200_export_frames(glava_b200* r, const int* streams, int count, void*
  *   their bytes.  dst[i], dst_uv[i], pitch and uv_offset are multiples of 16 (a mosaic tile starts at a multiple of 4 pixels
  *   in RGBA, of 16 in NV12 and YUV420P10, of 8 in YUV444P10).  Besides every refusal of glava_b200_export_frames (pitch and uv_offset measured against the
  *   output), a null `scale`, a rectangle that is empty or leaves the frame, upscaling, odd NV12 output dimensions, a
- *   misaligned, null, host or other-device dst_uv[i], and dst_uv for RGBA / BGRA are GLAVA_B200_EINVAL with nothing enqueued.
+ *   misaligned, null, host or other-device dst_uv[i], and dst_uv for RGBA / BGRA / UYVY are GLAVA_B200_EINVAL with nothing
+ *   enqueued.
  *   glava_b200_export_scaled_bytes   the bytes one destination spans (as glava_b200_export_bytes with out_h for h, dst_uv
  *                              NULL), after the same descriptor and rectangle checks.
  *   glava_b200_sharded_export_scaled  the same with global stream indices, dst[i] / dst_uv[i] on the device of the shard
@@ -486,10 +501,10 @@ int glava_b200_export_scaled(glava_b200* r, const int* streams, int count, void*
  *     dst                      [count][nrungs] destinations; each rung's size is glava_b200_export_scaled_bytes(r,
  *                              &rungs[j].desc, &rungs[j].scale, &n) (there is no separate byte-count call)
  *     dst_uv                   NULL, or [count][nrungs] CbCr destinations as glava_b200_export_scaled's, NULL entries for
- *                              RGBA / BGRA rungs
+ *                              RGBA / BGRA / UYVY rungs
  *   Nothing outside a rung's rectangle and its chroma rows is written; like glava_b200_export_scaled the call does not check
  *   whether destinations overlap.  Every refusal of glava_b200_export_scaled, checked per rung (the message names the rung),
- *   nrungs < 1 or > GLAVA_B200_LADDER_MAX, null `rungs` and a non-null dst_uv entry for an RGBA / BGRA rung are
+ *   nrungs < 1 or > GLAVA_B200_LADDER_MAX, null `rungs` and a non-null dst_uv entry for an RGBA / BGRA / UYVY rung are
  *   GLAVA_B200_EINVAL with nothing enqueued.
  *   glava_b200_sharded_export_ladder  the same with global stream indices, each entry's destinations on the device of the
  *                              shard that owns streams[i]; every entry of every rung is checked before any shard starts. */
@@ -520,7 +535,8 @@ int glava_b200_export_ladder(glava_b200* r, const int* streams, int count, const
  *   pixel leaves D exactly as it was, and rows the dirty-row marks skip and all-zero quads are neither read nor written.
  *   An opaque pixel gives exactly glava_b200_export_frames' bytes.  Under any other opacity GLava's window is opaque: the
  *   rectangle gets exactly what glava_b200_export_frames writes (RGBA / BGRA with EXPORT_OVER, or NV12).
- *   The overlay takes RGBA, BGRA and NV12; I420, YUV444, P010, YUV420P10 and YUV444P10 are refused by name (decoded
+ *   The overlay takes RGBA, BGRA and NV12; I420, YUV444, P010, YUV420P10, YUV444P10, YUV422P, YUV422P10 and UYVY are
+ *   refused by name (decoded
  *   pictures in those formats, with per-plane pointers and pitches, go to glava_b200_overlay_planes below).
  *   Besides the refusals of glava_b200_export_scaled that apply (format, pitch, uv_offset, alignment, null / host /
  *   other-device dst or dst_uv, dst_uv for RGBA / BGRA, odd NV12 frames, stream range, count < 1, an unbuilt renderer),
@@ -533,27 +549,31 @@ int glava_b200_export_ladder(glava_b200* r, const int* streams, int count, const
 int glava_b200_overlay_frames(glava_b200* r, const int* streams, int count, void* const* dst, void* const* dst_uv,
                               const glava_b200_export* desc, void* after_event, void* done_event);
 
-/* Overlay onto decoded pictures (DESIGN.md §4.17): what a decoder or ffmpeg hands over — NV12, I420, YUV444, P010,
- * YUV420P10 or YUV444P10, each plane at its own pointer, luma and chroma rows at their own pitches.
+/* Overlay onto decoded pictures (DESIGN.md §4.17, §4.18): what a decoder or ffmpeg hands over — NV12, I420, YUV444, P010,
+ * YUV420P10, YUV444P10, YUV422P, YUV422P10 or UYVY, each plane at its own pointer, luma and chroma rows at their own
+ * pitches.
  *   glava_b200_overlay_planes  composites the current frame of streams[i] onto the w x h rectangle of pics[i], exactly as
  *                              glava_b200_overlay_frames does onto NV12 (same ordering, events, streams and opacity rules;
  *                              NV12 runs its item body), top-down at the rectangle's origin:
- *     pics[i].plane[0]         the rectangle's first Y sample, `pitch` bytes per row
- *     pics[i].plane[1]         NV12 / P010: its first CbCr pair; the planar formats: its first Cb sample
- *     pics[i].plane[2]         the planar formats: its first Cr sample; NULL for NV12 and P010
+ *     pics[i].plane[0]         the rectangle's first Y sample (UYVY: its first Cb byte), `pitch` bytes per row
+ *     pics[i].plane[1]         NV12 / P010: its first CbCr pair; the planar formats: its first Cb sample; NULL for UYVY
+ *     pics[i].plane[2]         the planar formats: its first Cr sample; NULL for NV12, P010 and UYVY
  *     desc                     format, flags (0, or EXPORT_FULL_RANGE / EXPORT_BT601: the picture's encoding), the luma
- *                              pitch and one chroma pitch for every chroma plane; 4:2:0 chroma is w/2 x h/2
+ *                              pitch and one chroma pitch for every chroma plane (UYVY: 0); 4:2:0 chroma is w/2 x h/2,
+ *                              4:2:2 chroma w/2 x h
  *   10-bit samples hold their code as v >> 6 (P010) or v & 1023 (YUV420P10, YUV444P10).  Under native opacity the blend is
  *   overlay_frames' NV12 blend (I420: bit for bit NV12 deinterleaved; YUV444: chroma per pixel), and at 10 bits the same
- *   fraction at 10 bits with 4:2:0 chroma from the block's exact sums, as P010's export (export_core.h).  A blended 10-bit
+ *   fraction at 10 bits with 4:2:0 chroma from the block's exact sums, as P010's export (export_core.h); 4:2:2 chroma is
+ *   the 4:2:0 blend of the block whose two rows are the pixel pair.  A blended 10-bit
  *   sample is written with its other bits zero; a sample no non-zero pixel covers (a luma sample under a zero pixel, a chroma
  *   sample whose pixel or 2x2 block is all zero) keeps all 16 bits, and rows the marks skip and all-zero quads are neither
  *   read nor written.  Under any other opacity every sample of the rectangle gets glava_b200_export_frames' bytes.
  *   GLAVA_B200_EINVAL, with nothing enqueued, for: a null argument, count < 1, an unbuilt renderer; RGBA, BGRA (those go to
- *   glava_b200_overlay_frames) or an unknown format; any other flag; odd w or h for the 4:2:0 formats; a pitch or
- *   chroma_pitch that is not a multiple of 16 or below the plane's row bytes (luma w, 2w at 10 bits; chroma w for NV12,
- *   YUV444 and YUV420P10, w/2 for I420, 2w for P010 and YUV444P10); a plane pointer that is null, not 16-byte aligned, not
- *   device memory or on another device; a non-null plane[2] for NV12 or P010; a stream out of range; a plane rectangle
+ *   glava_b200_overlay_frames) or an unknown format; any other flag; odd w or h for the 4:2:0 formats, odd w for the 4:2:2
+ *   ones; a pitch or chroma_pitch that is not a multiple of 16 or below the plane's row bytes (luma w, 2w at 10 bits and
+ *   for UYVY; chroma w for NV12, YUV444, YUV420P10 and YUV422P10, w/2 for I420 and YUV422P, 2w for P010 and YUV444P10); a
+ *   UYVY chroma_pitch other than 0; a plane pointer that is null, not 16-byte aligned, not device memory or on another
+ *   device; a non-null plane[2] for NV12 or P010, a non-null plane[1] or plane[2] for UYVY; a stream out of range; a plane rectangle
  *   that meets the renderer's framebuffer array; two plane rectangles of the call that overlap (every pair: across
  *   entries, luma against chroma, Cb against Cr).
  *   glava_b200_sharded_overlay_planes  the same with global stream indices, each picture on the device of the shard that
@@ -561,7 +581,8 @@ int glava_b200_overlay_frames(glava_b200* r, const int* streams, int count, void
  *                              checked before any shard starts. */
 typedef struct { void* plane[3]; } glava_b200_picture;
 typedef struct {
-    int      format;        /* GLAVA_B200_EXPORT_NV12, _I420, _YUV444, _P010, _YUV420P10, _YUV444P10 */
+    int      format;        /* GLAVA_B200_EXPORT_NV12, _I420, _YUV444, _P010, _YUV420P10, _YUV444P10, _YUV422P,
+                               _YUV422P10, _UYVY */
     uint32_t flags;         /* 0, or GLAVA_B200_EXPORT_FULL_RANGE / GLAVA_B200_EXPORT_BT601 */
     size_t   pitch;         /* bytes between luma rows */
     size_t   chroma_pitch;  /* bytes between rows of every chroma plane */
