@@ -148,18 +148,22 @@ EXPORT_RGBA, EXPORT_BGRA, EXPORT_NV12 = 0, 1, 2
 EXPORT_I420, EXPORT_YUV444, EXPORT_P010 = 4, 5, 6
 EXPORT_YUV420P10, EXPORT_YUV444P10 = 7, 8                # planar 10-bit, LSB-aligned (yuv420p10le / yuv444p10le, DESIGN 4.16)
 EXPORT_YUV422P, EXPORT_YUV422P10, EXPORT_UYVY = 10, 11, 12   # 4:2:2 (yuv422p / yuv422p10le / uyvy422, DESIGN 4.18)
+EXPORT_YUVA420P, EXPORT_YUVA444P10 = 14, 15             # with an alpha plane (yuva420p / yuva444p10le, DESIGN 4.19)
 EXPORT_OVER = 1
+EXPORT_STRAIGHT = 4                                     # RGBA / BGRA with straight (unassociated) alpha (DESIGN 4.19)
 EXPORT_FULL_RANGE, EXPORT_BT601 = 0x100, 0x200          # the Y'CbCr encoding (DESIGN 4.15); neither: BT.709 limited range
 EXPORT_MATRICES = {"bt709": 0, "bt601": EXPORT_BT601}
 EXPORT_FORMATS = {"rgba": EXPORT_RGBA, "bgra": EXPORT_BGRA, "nv12": EXPORT_NV12, "i420": EXPORT_I420,
                   "yuv444": EXPORT_YUV444, "p010": EXPORT_P010, "yuv420p10": EXPORT_YUV420P10,
                   "yuv444p10": EXPORT_YUV444P10, "yuv422p": EXPORT_YUV422P, "yuv422p10": EXPORT_YUV422P10,
-                  "uyvy": EXPORT_UYVY}
+                  "uyvy": EXPORT_UYVY, "yuva420p": EXPORT_YUVA420P, "yuva444p10": EXPORT_YUVA444P10}
 OVERLAY_FORMATS = ("rgba", "bgra", "nv12")
 # the formats overlay_planes takes: decoded pictures, one tensor per plane (DESIGN 4.17)
 PLANES_FORMATS = ("nv12", "i420", "yuv444", "p010", "yuv420p10", "yuv444p10", "yuv422p", "yuv422p10", "uyvy")
 # the formats whose samples are uint16, which also take uint16 `out` tensors
-WIDE_FORMATS = ("p010", "yuv420p10", "yuv444p10", "yuv422p10")
+WIDE_FORMATS = ("p010", "yuv420p10", "yuv444p10", "yuv422p10", "yuva444p10")
+# the formats with an alpha plane, returned as (Y, Cb, Cr, A)
+ALPHA_FORMATS = ("yuva420p", "yuva444p10")
 
 
 def _export_layout(fmt, w, h):
@@ -167,12 +171,17 @@ def _export_layout(fmt, w, h):
     bytes; NV12 / P010 h * 3 / 2 rows of w (P010: w uint16) samples, Y then CbCr; I420 / YUV420P10 h * 3 / 2 rows, the Y
     plane then the Cb and Cr planes back to back at pitch / 2 (pitch a multiple of 32); YUV444 / YUV444P10 3 h rows, the Y,
     Cb and Cr planes; YUV422P / YUV422P10 2 h rows, the Y plane then the Cb and Cr planes of h rows at pitch / 2 (pitch a
-    multiple of 32); UYVY h rows of 2 w bytes; the 10-bit formats hold w uint16 per row"""
+    multiple of 32); UYVY h rows of 2 w bytes; YUVA420P 5 h / 2 rows, I420's planes then the A plane of h rows at pitch
+    (pitch a multiple of 32); YUVA444P10 4 h rows, the Y, Cb, Cr and A planes; the 10-bit formats hold w uint16 per row"""
     if fmt in ("rgba", "bgra"):
         return h, w * 4, 16
     if fmt == "uyvy":
         return h, w * 2, 16
     row = w * 2 if fmt in WIDE_FORMATS else w
+    if fmt == "yuva420p":
+        return h * 5 // 2, row, 32
+    if fmt == "yuva444p10":
+        return 4 * h, row, 16
     if fmt in ("yuv444", "yuv444p10"):
         return 3 * h, row, 16
     if fmt in ("yuv422p", "yuv422p10"):
@@ -184,7 +193,8 @@ def _export_views(fmt, t, w, h):
     """what an export into t returns: t is uint8 [..., rows, pitch] with contiguous rows as _export_layout describes.  RGBA /
     BGRA [..., h, w, 4], NV12 [..., h * 3 / 2, w] uint8, P010 [..., h * 3 / 2, w] uint16, I420 / YUV444 the plane views
     (Y, Cb, Cr), each [..., rows, cols], YUV420P10 / YUV444P10 the same as uint16; YUV422P / YUV422P10 (Y, Cb, Cr) with
-    Cb and Cr [..., h, w / 2]; UYVY [..., h, 2 w] uint8 (Cb, Y0, Cr, Y1 per pixel pair)"""
+    Cb and Cr [..., h, w / 2]; UYVY [..., h, 2 w] uint8 (Cb, Y0, Cr, Y1 per pixel pair); YUVA420P / YUVA444P10 (Y, Cb, Cr,
+    A) as I420 / YUV444P10 with A [..., h, w] (uint8 / uint16) after Cr"""
     import torch
     if fmt in ("rgba", "bgra"):
         return t[..., :w * 4].unflatten(-1, (w, 4))
@@ -198,12 +208,14 @@ def _export_views(fmt, t, w, h):
         return t[..., :w]
     P = t.shape[-1]                                           # the pitch in samples
     flat = t.flatten(-2)
-    cw, ch, cp = ((w // 2, h // 2, P // 2) if fmt in ("i420", "yuv420p10") else (w // 2, h, P // 2)
+    cw, ch, cp = ((w // 2, h // 2, P // 2) if fmt in ("i420", "yuv420p10", "yuva420p") else (w // 2, h, P // 2)
                   if fmt in ("yuv422p", "yuv422p10") else (w, h, P))
     n = ch * cp
     y = flat[..., :P * h].unflatten(-1, (h, P))[..., :w]
     cb = flat[..., P * h:P * h + n].unflatten(-1, (ch, cp))[..., :cw]
     cr = flat[..., P * h + n:P * h + 2 * n].unflatten(-1, (ch, cp))[..., :cw]
+    if fmt in ALPHA_FORMATS:
+        return y, cb, cr, flat[..., P * h + 2 * n:2 * P * h + 2 * n].unflatten(-1, (h, P))[..., :w]
     return y, cb, cr
 
 
@@ -495,20 +507,22 @@ class _StreamStyles:
 class _FrameExport:
     """export_frames over the handle's C entry point: destinations as torch tensors (DESIGN 4.10)"""
 
-    def _export_plan(self, streams, fmt, over, background, out, device_of, size=None, matrix="bt709", full_range=False):
+    def _export_plan(self, streams, fmt, over, background, out, device_of, size=None, matrix="bt709", full_range=False,
+                     straight=False):
         """-> (stream list, Export, [dst pointers], what to return).  device_of(stream): the CUDA device of a stream's
         frame.  size: (w, h) of each output, None: the frame's.  out: None (allocate), one uint8 tensor [count, rows, ...]
         whose dim 1 steps by the pitch, or a list of count tensors [rows, ...] with one common pitch; rows as
         _export_layout gives them (h for RGBA / BGRA and UYVY, h * 3 / 2 for NV12, I420, P010 and YUV420P10, 2 h for YUV422P
         and YUV422P10, 3 h for YUV444 and YUV444P10; the planar formats keep their planes back to back from row h); P010,
-        YUV420P10, YUV444P10 and YUV422P10 also take uint16 tensors.  matrix / full_range: the Y'CbCr encoding (_export_desc)"""
+        YUV420P10, YUV444P10 and YUV422P10 also take uint16 tensors.  matrix / full_range: the Y'CbCr encoding, straight:
+        straight alpha (_export_desc)"""
         import torch
         s = np.ascontiguousarray(np.asarray(streams, dtype=np.int64).reshape(-1), dtype=np.int32)
         count = int(s.shape[0])
         devices = [device_of(int(x)) for x in s]
         p = self.params
         w, h = (p.w, p.h) if size is None else (int(size[0]), int(size[1]))
-        desc = _export_desc(fmt, over, background, matrix, full_range)
+        desc = _export_desc(fmt, over, background, matrix, full_range, straight)
         rows, row_bytes, align = _export_layout(fmt, w, h)
         dtypes = (torch.uint8, torch.uint16) if fmt in WIDE_FORMATS else (torch.uint8,)
 
@@ -561,13 +575,14 @@ class _FrameExport:
         arr = (ExportRung * max(len(rungs), 1))()
         ptrs, results = [], []
         for j, (rung, o) in enumerate(zip(rungs, outs)):
-            unknown = set(rung) - {"size", "crop", "fmt", "over", "background", "matrix", "full_range"}
+            unknown = set(rung) - {"size", "crop", "fmt", "over", "background", "matrix", "full_range", "straight"}
             if unknown:
                 raise ValueError(f"rungs[{j}]: unknown keys {sorted(unknown)}")
             size = rung.get("size") or (p.w, p.h)
             _, desc, dst, result = self._export_plan(s, rung.get("fmt", "nv12"), rung.get("over", False),
                                                      rung.get("background", (0, 0, 0)), o, device_of, size,
-                                                     rung.get("matrix", "bt709"), rung.get("full_range", False))
+                                                     rung.get("matrix", "bt709"), rung.get("full_range", False),
+                                                     rung.get("straight", False))
             arr[j].desc, arr[j].scale = desc, _export_scale(size, rung.get("crop"))
             ptrs.append(dst)
             results.append(result)
@@ -745,17 +760,21 @@ class _FrameExport:
         return s, desc, arr
 
 
-def _export_desc(fmt, over, background, matrix="bt709", full_range=False):
-    """the Export descriptor of a format name, the composite flag, an RGB(A) background (pitch and uv_offset 0) and the
+def _export_desc(fmt, over, background, matrix="bt709", full_range=False, straight=False):
+    """the Export descriptor of a format name, the composite flag, an RGB(A) background (pitch and uv_offset 0), the
     Y'CbCr encoding: matrix "bt709" or "bt601", full_range (DESIGN 4.15; the defaults set no flag, and a matrix or range
-    on RGBA / BGRA reaches the library's refusal)"""
+    on RGBA / BGRA reaches the library's refusal) and straight alpha (DESIGN 4.19; on a Y'CbCr format it reaches the
+    library's refusal)"""
     if fmt not in EXPORT_FORMATS:
         raise ValueError(f"format {fmt!r}: one of {sorted(EXPORT_FORMATS)}")
     if matrix not in EXPORT_MATRICES:
         raise ValueError(f"matrix {matrix!r}: one of {sorted(EXPORT_MATRICES)}")
+    if straight and over:
+        raise ValueError("straight and over exclude each other: a composite is opaque")
     desc = Export()
     desc.format = EXPORT_FORMATS[fmt]
-    desc.flags = (EXPORT_OVER if over else 0) | EXPORT_MATRICES[matrix] | (EXPORT_FULL_RANGE if full_range else 0)
+    desc.flags = ((EXPORT_OVER if over else 0) | (EXPORT_STRAIGHT if straight else 0) | EXPORT_MATRICES[matrix]
+                  | (EXPORT_FULL_RANGE if full_range else 0))
     bg = [int(v) for v in background]
     assert len(bg) in (3, 4), background
     desc.background = (C.c_uint8 * 4)(*bg[:3], 0)
@@ -1034,14 +1053,17 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
         return self._L.glava_b200_framebuffer_device(self._h)
 
     def export_frames(self, streams, fmt="rgba", over=False, background=(0, 0, 0), out=None, after=None, done=None,
-                      matrix="bt709", full_range=False):
+                      matrix="bt709", full_range=False, straight=False):
         """The current frames of `streams` (repeats allowed) top-down in the caller's device memory (glava_b200_export_frames):
         fmt "rgba" / "bgra" ([h, w, 4] per frame; over=True composites over `background` as GLava's window shows it) or
         "nv12" ([h * 3 / 2, w]: Y rows, then interleaved CbCr rows), "p010" (the same as uint16 samples, 10-bit code << 6),
         "i420" / "yuv444" (a tuple of plane views Y [h, w], Cb and Cr [h / 2, w / 2] or [h, w] of one back-to-back
         allocation), "yuv420p10" / "yuv444p10" (the same planes as uint16 samples holding the 10-bit code in their low bits:
         ffmpeg's yuv420p10le / yuv444p10le), "yuv422p" / "yuv422p10" (Y [h, w], Cb and Cr [h, w / 2], uint8 / uint16) or
-        "uyvy" ([h, 2 w] uint8, Cb Y0 Cr Y1 per pixel pair); the YUV formats are always composited.  out: see _export_plan; None allocates
+        "uyvy" ([h, 2 w] uint8, Cb Y0 Cr Y1 per pixel pair), or "yuva420p" / "yuva444p10" (I420's / YUV444P10's planes and an A
+        plane [h, w]: (Y, Cb, Cr, A), ffmpeg's yuva420p / yuva444p10le, never composited: the straight colour and the frame's
+        alpha, DESIGN 4.19); the other YUV formats are always composited.  straight=True (RGBA / BGRA, not with over): the
+        colour un-premultiplied, as PNG and ffmpeg's rgba take it.  out: see _export_plan; None allocates
         [count, ...] of those shapes (rows padded to a multiple of 16 bytes, 32 for I420, YUV420P10, YUV422P and YUV422P10).  Returns out.
         after / done: torch.cuda.Event or cudaEvent_t handles — the export waits for `after` on the device and records
         `done` behind itself.  Left None, the export is ordered after the work already queued on torch's current stream,
@@ -1049,7 +1071,7 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
         matrix ("bt709" / "bt601") and full_range: the Y'CbCr encoding of every YUV format (DESIGN 4.15; the
         default is BT.709 limited range; matrix="bt601", full_range=True is JPEG's)."""
         s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, lambda stream: self.device, None, matrix,
-                                                 full_range)
+                                                 full_range, straight)
         self._ordered(lambda a, d: self._L.glava_b200_export_frames(self._h, s.ctypes.data, s.shape[0], dst, C.byref(desc), a, d),
                       after, done)
         return result
@@ -1068,13 +1090,13 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
             cur.wait_stream(own)
 
     def export_scaled(self, streams, size, crop=None, fmt="rgba", over=False, background=(0, 0, 0), out=None, after=None,
-                      done=None, matrix="bt709", full_range=False):
+                      done=None, matrix="bt709", full_range=False, straight=False):
         """export_frames of a source rectangle shrunk to size = (w, h) by the exact area average (glava_b200_export_scaled):
         crop = (x, y, w, h) in top-down coordinates (y = 0 is the top row), None: the whole frame.  Downscale only; NV12,
         I420, P010 and YUV420P10 need an even w and h, YUV422P, YUV422P10 and UYVY an even w.  Shapes, out, after, done, matrix and full_range as export_frames, with the output
-        size in place of the frame's."""
+        size in place of the frame's; straight as export_frames (the stored channels averaged, then un-premultiplied)."""
         s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, lambda stream: self.device, size, matrix,
-                                                 full_range)
+                                                 full_range, straight)
         sc = _export_scale(size, crop)
         self._ordered(lambda a, d: self._L.glava_b200_export_scaled(self._h, s.ctypes.data, s.shape[0], dst, None, C.byref(desc),
                                                                     C.byref(sc), a, d), after, done)
@@ -1083,7 +1105,7 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
     def export_ladder(self, streams, rungs, out=None, after=None, done=None):
         """Several sizes of each frame in one launch that reads each source row about once (glava_b200_export_ladder), for
         an encoder ladder: rungs = [dict(size=(w, h) or None for the frame's, crop=None, fmt="nv12", over=False,
-        background=(0, 0, 0), matrix="bt709", full_range=False), ...], at most LADDER_MAX; rungs may mix encodings.  Rung j is exactly export_scaled(streams, **rungs[j]) at this
+        background=(0, 0, 0), matrix="bt709", full_range=False, straight=False), ...], at most LADDER_MAX; rungs may mix encodings.  Rung j is exactly export_scaled(streams, **rungs[j]) at this
         point in call order.  out: None or one entry per rung in any form export_scaled takes.  Returns one result per rung,
         shaped as export_scaled returns it; after / done and the ordering against torch's current stream as export_frames."""
         s, arr, n, dst, results = self._ladder_plan(streams, rungs, out, lambda stream: self.device)
@@ -1132,6 +1154,8 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
         tw, th = (int(v) for v in tile)
         if count < 1 or cols < 1:
             raise ValueError("export_mosaic: at least one stream and one column")
+        if fmt in ALPHA_FORMATS:
+            raise ValueError(f"export_mosaic: format {fmt!r}: a mosaic is one opaque picture, it takes no alpha format")
         desc = _export_desc(fmt, False, background, matrix, full_range)
         W, H = cols * tw, (count + cols - 1) // cols * th
         rows, row_bytes, align = _export_layout(fmt, W, H)
@@ -1281,26 +1305,28 @@ class ShardedRenderer(_StreamState, _StreamStyles, _FrameExport):
         _check(self._L.glava_b200_sharded_textures(self._h, l.ctypes.data, r.ctypes.data))
         return l, r
 
-    def export_frames(self, streams, fmt="rgba", over=False, background=(0, 0, 0), out=None, matrix="bt709", full_range=False):
+    def export_frames(self, streams, fmt="rgba", over=False, background=(0, 0, 0), out=None, matrix="bt709", full_range=False,
+                      straight=False):
         """Renderer.export_frames with global stream indices (glava_b200_sharded_export_frames): each destination on the
         device of the shard that owns its stream (out None: one tensor when every listed stream lives on one device, else
         a list of per-frame tensors).  Work queued on torch's current streams of those devices is waited for first; the
-        frames are complete after sync().  matrix / full_range as Renderer.export_frames."""
+        frames are complete after sync().  matrix / full_range / straight as Renderer.export_frames."""
         import torch
         device_of = self._device_of()
-        s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, device_of, None, matrix, full_range)
+        s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, device_of, None, matrix, full_range, straight)
         for d in sorted({device_of(int(x)) for x in s}):
             torch.cuda.current_stream(d).synchronize()
         _check(self._L.glava_b200_sharded_export_frames(self._h, s.ctypes.data, s.shape[0], dst, C.byref(desc)))
         return result
 
     def export_scaled(self, streams, size, crop=None, fmt="rgba", over=False, background=(0, 0, 0), out=None, matrix="bt709",
-                      full_range=False):
+                      full_range=False, straight=False):
         """Renderer.export_scaled with global stream indices (glava_b200_sharded_export_scaled), destinations placed as
-        export_frames places them; the frames are complete after sync().  matrix / full_range as Renderer.export_frames."""
+        export_frames places them; the frames are complete after sync().  matrix / full_range / straight as
+        Renderer.export_frames."""
         import torch
         device_of = self._device_of()
-        s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, device_of, size, matrix, full_range)
+        s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, device_of, size, matrix, full_range, straight)
         sc = _export_scale(size, crop)
         for d in sorted({device_of(int(x)) for x in s}):
             torch.cuda.current_stream(d).synchronize()

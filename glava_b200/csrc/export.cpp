@@ -33,6 +33,8 @@ const char* format_name(int format) {
     case GLAVA_B200_EXPORT_YUV422P: return "YUV422P";
     case GLAVA_B200_EXPORT_YUV422P10: return "YUV422P10";
     case GLAVA_B200_EXPORT_UYVY: return "UYVY";
+    case GLAVA_B200_EXPORT_YUVA420P: return "YUVA420P";
+    case GLAVA_B200_EXPORT_YUVA444P10: return "YUVA444P10";
     default: return nullptr;
     }
 }
@@ -47,13 +49,13 @@ int desc_size(int w, int h, const glava_b200_export& d, const char* what, const 
         return fail(GLAVA_B200_EINVAL, "%s: %s needs an even width, the %s is %dx%d", who, name, what, w, h);
     const size_t row = !export_ycbcr(fmt) ? (size_t) w * 4
                        : fmt == GLAVA_B200_EXPORT_P010 || export_p10(fmt) || fmt == GLAVA_B200_EXPORT_YUV422P10 ||
-                                 fmt == GLAVA_B200_EXPORT_UYVY
+                                 fmt == GLAVA_B200_EXPORT_UYVY || fmt == GLAVA_B200_EXPORT_YUVA444P10
                            ? (size_t) w * 2
                            : (size_t) w;
     if (d.pitch % 16 || d.pitch < row)
         return fail(GLAVA_B200_EINVAL, "%s: pitch %zu must be a multiple of 16 and at least %zu", who, d.pitch, row);
     if ((fmt == GLAVA_B200_EXPORT_I420 || fmt == GLAVA_B200_EXPORT_YUV420P10 || fmt == GLAVA_B200_EXPORT_YUV422P ||
-         fmt == GLAVA_B200_EXPORT_YUV422P10) && d.pitch % 32)
+         fmt == GLAVA_B200_EXPORT_YUV422P10 || fmt == GLAVA_B200_EXPORT_YUVA420P) && d.pitch % 32)
         return fail(GLAVA_B200_EINVAL, "%s: %s pitch %zu must be a multiple of 32, so that chroma rows (pitch / 2) stay 16-byte "
                     "aligned", who, name, d.pitch);
     if ((fmt == GLAVA_B200_EXPORT_NV12 || fmt == GLAVA_B200_EXPORT_P010) &&
@@ -79,7 +81,20 @@ int desc_check(ExportKind kind, int w, int h, const glava_b200_export& d, const 
         return fail(GLAVA_B200_EINVAL, "%s: format %s: the overlay takes RGBA, BGRA or NV12", who, format_name(d.format));
     // the colour bits (DESIGN 4.15) are flags of the Y'CbCr formats only
     const uint32_t colour = GLAVA_B200_EXPORT_FULL_RANGE | GLAVA_B200_EXPORT_BT601;
-    if (d.flags & ~(GLAVA_B200_EXPORT_OVER | colour)) return fail(GLAVA_B200_EINVAL, "%s: unknown flags 0x%x", who, d.flags);
+    if (d.flags & ~(GLAVA_B200_EXPORT_OVER | GLAVA_B200_EXPORT_STRAIGHT | colour))
+        return fail(GLAVA_B200_EINVAL, "%s: unknown flags 0x%x", who, d.flags);
+    // transparency (DESIGN 4.19): straight alpha is RGBA / BGRA's alone, and never composited; the YUVA formats never are
+    if (kind == ExportKind::overlay && (d.flags & GLAVA_B200_EXPORT_STRAIGHT))
+        return fail(GLAVA_B200_EINVAL, "%s: flags 0x%x: EXPORT_STRAIGHT is for the exports; the overlay composites", who, d.flags);
+    if ((d.flags & GLAVA_B200_EXPORT_STRAIGHT) && (d.flags & GLAVA_B200_EXPORT_OVER))
+        return fail(GLAVA_B200_EINVAL, "%s: flags 0x%x: EXPORT_STRAIGHT and EXPORT_OVER exclude each other (a composite is "
+                    "opaque)", who, d.flags);
+    if ((d.flags & GLAVA_B200_EXPORT_STRAIGHT) && export_ycbcr(d.format))
+        return fail(GLAVA_B200_EINVAL, "%s: flags 0x%x: EXPORT_STRAIGHT is for RGBA and BGRA, not %s (YUVA420P and YUVA444P10 carry "
+                    "straight alpha)", who, d.flags, format_name(d.format));
+    if ((d.flags & GLAVA_B200_EXPORT_OVER) && export_yuva(d.format))
+        return fail(GLAVA_B200_EINVAL, "%s: flags 0x%x: %s is never composited (EXPORT_OVER), its A plane holds the frame's "
+                    "alpha", who, d.flags, format_name(d.format));
     if ((d.flags & colour) && !export_ycbcr(d.format))
         return fail(GLAVA_B200_EINVAL, "%s: flags 0x%x: %s has no matrix or range (EXPORT_FULL_RANGE and EXPORT_BT601 are for the "
                     "Y'CbCr formats)", who, d.flags, format_name(d.format));
@@ -113,6 +128,7 @@ int output_bytes(ExportKind kind, const glava_b200* r, const glava_b200_export* 
     const size_t h = (size_t) q.out_h;
     const ExportPlanes pl = export_planes(desc->format, desc->pitch, desc->uv_offset, q.out_h);
     if (!export_chroma_planes(desc->format)) *bytes = desc->pitch * h;   // RGBA, BGRA, UYVY: one plane
+    else if (export_yuva(desc->format)) *bytes = pl.cb + 2 * pl.cr + desc->pitch * h;   // A: pitch * h, past Cr
     else if (export_planar(desc->format)) *bytes = pl.cb + pl.cr + pl.plane;
     else *bytes = pl.cb + desc->pitch * (h / 2);
     return 0;
@@ -127,7 +143,7 @@ void common_args(Args& a, const RendererView& v, const void* d_list, int count, 
     a.marks = v.mark_key ? v.marks : nullptr;
     a.mark_rows = v.mark_key >> 2;
     a.list = static_cast<decltype(a.list)>(d_list); a.count = count; a.w = v.w; a.h = v.h;
-    a.format = d.format;
+    a.format = export_kernel_format(d.format, d.flags);
     a.native = v.native;
     a.pitch = d.pitch;
 }
@@ -230,8 +246,8 @@ int export_check(ExportKind kind, glava_b200* r, const int* streams, int count, 
     int rc = desc_check(kind, v.w, v.h, *desc, scale, q ? q : &local, who);
     if (rc) return rc;
     if (dst_uv && !export_chroma_planes(desc->format))
-        return fail(GLAVA_B200_EINVAL, "%s: dst_uv is for NV12 only, or I420, YUV444, P010, YUV420P10, YUV444P10, YUV422P and "
-                    "YUV422P10: %s has no chroma plane", who,
+        return fail(GLAVA_B200_EINVAL, "%s: dst_uv is for NV12 only, or I420, YUV444, P010, YUV420P10, YUV444P10, YUV422P, "
+                    "YUV422P10, YUVA420P and YUVA444P10: %s has no chroma plane", who,
                     format_name(desc->format));
     if (count < 1) return fail(GLAVA_B200_EINVAL, "%s: count %d < 1", who, count);
     if (!streams || !dst) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
@@ -259,6 +275,9 @@ int export_run(ExportKind kind, glava_b200* r, const int* streams, int count, vo
         if ((rc = overlay_geometry_check(v.w, v.h, count, dst, dst_uv, *desc, &v.fb, &fb_bytes, 1, who)) != 0) return rc;
     }
     const bool yuv = export_ycbcr(desc->format), planes = export_chroma_planes(desc->format);
+    // the alpha formats run under their kernel format code, composited only under any other opacity than native
+    const bool alpha = export_yuva(desc->format) || (desc->flags & GLAVA_B200_EXPORT_STRAIGHT);
+    const int over = alpha ? !v.native : yuv || (desc->flags & GLAVA_B200_EXPORT_OVER) ? 1 : 0;
     const ExportPlanes pl = export_planes(desc->format, desc->pitch, desc->uv_offset, q.out_h);
     CU(cudaSetDevice(v.device));
     // export_kernel's entries have no chroma pointer (its machine code stays as measured); the others carry one per entry
@@ -277,7 +296,7 @@ int export_run(ExportKind kind, glava_b200* r, const int* streams, int count, vo
         if (kind == ExportKind::frames) {
             ExportArgs a = {};
             common_args(a, v, d_list, count, *desc);
-            a.over = yuv || (desc->flags & GLAVA_B200_EXPORT_OVER) ? 1 : 0;
+            a.over = over;
             a.bg = background(*desc);
             a.uv_offset = pl.cb;
             a.cr_offset = pl.cr;
@@ -287,7 +306,7 @@ int export_run(ExportKind kind, glava_b200* r, const int* streams, int count, vo
         if (kind == ExportKind::scaled) {
             ScaledArgs a = {};
             common_args(a, v, d_list, count, *desc);
-            a.over = yuv || (desc->flags & GLAVA_B200_EXPORT_OVER) ? 1 : 0;
+            a.over = over;
             a.bg = background(*desc);
             a.src_x = q.src_x; a.src_y = q.src_y; a.src_w = q.src_w; a.src_h = q.src_h; a.out_w = q.out_w; a.out_h = q.out_h;
             const ExportRecip rcp = export_recip((uint64_t) q.src_w * (uint64_t) q.src_h);

@@ -153,28 +153,32 @@ GLB_HD bool export_p10(int format) { return format == GLAVA_B200_EXPORT_YUV420P1
 GLB_HD bool export_422(int format) {
     return format == GLAVA_B200_EXPORT_YUV422P || format == GLAVA_B200_EXPORT_YUV422P10 || format == GLAVA_B200_EXPORT_UYVY;
 }
+// The formats with an alpha plane (DESIGN 4.19), kernels of their own again: never composited, planar, A after Cr
+GLB_HD bool export_yuva(int format) { return format == GLAVA_B200_EXPORT_YUVA420P || format == GLAVA_B200_EXPORT_YUVA444P10; }
 // every Y'CbCr format, the ones the colour flags apply to; export_chroma_planes: those with chroma planes (UYVY packs its
 // chroma into its one plane)
-GLB_HD bool export_ycbcr(int format) { return export_yuv(format) || export_p10(format) || export_422(format); }
+GLB_HD bool export_ycbcr(int format) { return export_yuv(format) || export_p10(format) || export_422(format) || export_yuva(format); }
 GLB_HD bool export_chroma_planes(int format) { return export_ycbcr(format) && format != GLAVA_B200_EXPORT_UYVY; }
 GLB_HD bool export_420(int format) {                   // chroma per 2x2 block: w and h even, items are row pairs
     return format == GLAVA_B200_EXPORT_NV12 || format == GLAVA_B200_EXPORT_I420 || format == GLAVA_B200_EXPORT_P010 ||
-           format == GLAVA_B200_EXPORT_YUV420P10;
+           format == GLAVA_B200_EXPORT_YUV420P10 || format == GLAVA_B200_EXPORT_YUVA420P;
 }
 GLB_HD bool export_planar(int format) {
     return format == GLAVA_B200_EXPORT_I420 || format == GLAVA_B200_EXPORT_YUV444 || export_p10(format) ||
-           format == GLAVA_B200_EXPORT_YUV422P || format == GLAVA_B200_EXPORT_YUV422P10;
+           format == GLAVA_B200_EXPORT_YUV422P || format == GLAVA_B200_EXPORT_YUV422P10 || export_yuva(format);
 }
 
 // Where the chroma of a destination lies, from the descriptor and the output height: `cb`, the bytes from the luma to the
 // chroma plane (NV12 / P010: the CbCr plane, uv_offset or pitch * h; the planar formats: the Cb plane, right after the
-// luma); `cr`, the bytes from Cb to Cr (planar only: uv_offset, or 0 for one chroma plane, back to back); `plane`, the bytes
-// of one planar chroma plane (I420 / YUV420P10: h / 2 rows of pitch / 2; YUV422P / YUV422P10: h rows of pitch / 2)
+// luma); `cr`, the bytes from Cb to Cr (planar only: uv_offset, or 0 for one chroma plane, back to back; a YUVA format's
+// A plane lies as far again past Cr); `plane`, the bytes of one planar chroma plane (I420 / YUV420P10 / YUVA420P: h / 2
+// rows of pitch / 2; YUV422P / YUV422P10: h rows of pitch / 2)
 struct ExportPlanes { size_t cb, cr, plane; };
 GLB_HD ExportPlanes export_planes(int format, size_t pitch, size_t uv_offset, int h) {
     ExportPlanes p = { uv_offset ? uv_offset : pitch * (size_t) h, 0, 0 };
     if (export_planar(format)) {
-        p.plane = format == GLAVA_B200_EXPORT_I420 || format == GLAVA_B200_EXPORT_YUV420P10 ? (pitch / 2) * (size_t) (h / 2)
+        p.plane = format == GLAVA_B200_EXPORT_I420 || format == GLAVA_B200_EXPORT_YUV420P10 || format == GLAVA_B200_EXPORT_YUVA420P
+                      ? (pitch / 2) * (size_t) (h / 2)
                   : format == GLAVA_B200_EXPORT_YUV422P || format == GLAVA_B200_EXPORT_YUV422P10 ? (pitch / 2) * (size_t) h
                                                                                                  : pitch * (size_t) h;
         p.cb = pitch * (size_t) h;
@@ -400,6 +404,119 @@ GLB_HD ExportZero export_zero422(const ExportFmt& f) {
     return o;
 }
 
+// ---- transparency: straight RGBA / BGRA, yuva420p and yuva444p10le (DESIGN 4.19) --------------------------------------------
+// Under native opacity a stored pixel (c, a) is premultiplied over a transparent target.  Its straight (unassociated)
+// colour, per channel, is S = a == 0 ? 0 : min(255, (c 255 + a / 2) / a): the integer quotient rounded half up, exact on
+// host and device (plain unsigned division).  Wherever c <= a, mul_norm8(S, a) == c, so premultiplying S with the blend
+// path's own product gives the stored pixel back (tests/test_export_alpha_core.py, all 65536 pairs).  The min and the
+// a == 0 case only act where c > a: Graph runs no premultiply stage, so a translucent graph colour can store more
+// colour than alpha, an additive part straight alpha cannot hold; it is clamped.
+// The alpha formats are never composited: ExportFmt.over is set for them only under any other opacity than native, where
+// the frame is opaque and export_over makes every pixel (c, 255), whose straight colour is c.  So STRAIGHT is then
+// EXPORT_OVER's bytes, and the YUVA formats I420's / YUV444P10's Y, Cb and Cr with A = 255 (1023).
+// Straight RGBA / BGRA run these kernels under a format code of their own, the public format with GLB_EXPORT_STRAIGHT set
+// (public formats stay below it), chosen on the host by export_kernel_format.
+#define GLB_EXPORT_STRAIGHT 0x100
+GLB_HD bool export_straight(int format) { return (format & GLB_EXPORT_STRAIGHT) != 0; }
+GLB_HD bool export_alpha(int format) { return export_yuva(format) || export_straight(format); }   // the alpha kernels' formats
+inline int export_kernel_format(int format, uint32_t flags) {   // host code
+    return flags & GLAVA_B200_EXPORT_STRAIGHT ? format | GLB_EXPORT_STRAIGHT : format;
+}
+// one straight channel of stored colour c and alpha a
+GLB_HD uint32_t export_unpremul(uint32_t c, uint32_t a) {
+    if (!a) return 0u;
+    const uint32_t s = (c * 255u + (a >> 1)) / a;
+    return s > 255u ? 255u : s;
+}
+// the straight pixel (S_r, S_g, S_b, a) of a stored one; opaque and zero pixels need no division
+GLB_HD uint32_t export_straight_px(uint32_t px) {
+    const uint32_t a = px >> 24;
+    if (a == 255u || !px) return px;
+    uint32_t out = px & 0xff000000u;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) out |= export_unpremul((px >> (8 * c)) & 255u, a) << (8 * c);
+    return out;
+}
+// the pixel the alpha arithmetic starts from: stored, or composited (any other opacity than native: (c, 255))
+GLB_HD uint32_t export_alpha_in(const ExportFmt& f, uint32_t px) { return f.over ? export_over(px, f.bg, f.native) : px; }
+// the 10-bit alpha code: (a 1023 + 127) / 255, no ties, 0 -> 0, 255 -> 1023, within 0.495 of a 1023 / 255
+GLB_HD uint32_t export_a10(uint32_t a) { return (a * 1023u + 127u) / 255u; }
+// The straight colour of a 2x2 block for its 4:2:0 chroma, weighted by alpha: per channel min(255, (sum c 255 + sum a / 2)
+// / sum a), 0 when sum a = 0, i.e. the un-premultiplied block average.  Four opaque pixels give export_avg4 exactly:
+// (s 255 + 510) / 1020 = (s + 2) >> 2.  Zero-alpha pixels hold black and so weigh nothing, which keeps bar edges free of
+// dark fringes.
+GLB_HD uint32_t export_block_straight(uint32_t p0, uint32_t p1, uint32_t p2, uint32_t p3) {
+    const uint32_t sa = (p0 >> 24) + (p1 >> 24) + (p2 >> 24) + (p3 >> 24);
+    if (!sa) return 0u;
+    uint32_t out = 0u;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        const uint32_t s = ((p0 >> (8 * k)) & 255u) + ((p1 >> (8 * k)) & 255u) + ((p2 >> (8 * k)) & 255u) + ((p3 >> (8 * k)) & 255u);
+        const uint32_t v = (s * 255u + (sa >> 1)) / sa;
+        out |= (v > 255u ? 255u : v) << (8 * k);
+    }
+    return out;
+}
+// straight RGBA / BGRA of one stored pixel (fmt: the kernel format code)
+GLB_HD uint32_t export_straight_out(const ExportFmt& f, int fmt, uint32_t px) {
+    const uint32_t s = export_straight_px(export_alpha_in(f, px));
+    return (fmt & ~GLB_EXPORT_STRAIGHT) == GLAVA_B200_EXPORT_BGRA ? export_swap_rb(s) : s;
+}
+// yuva420p of a quad of output rows 2j (top) and 2j + 1 (bot): per row four Y bytes and four A bytes, and the Cb and Cr
+// bytes of the quad's two 2x2 blocks (I420's pairs)
+template <int E = 0>
+GLB_HD void export_yuva420_quad(const ExportFmt& f, const uint32_t top[4], const uint32_t bot[4], uint32_t* yt, uint32_t* yb,
+                                uint32_t* cb, uint32_t* cr, uint32_t* at, uint32_t* ab) {
+    uint32_t t[4], b[4];
+    *yt = 0u; *yb = 0u; *at = 0u; *ab = 0u;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        t[k] = export_alpha_in(f, top[k]);
+        b[k] = export_alpha_in(f, bot[k]);
+        *yt |= export_y<E>(export_straight_px(t[k])) << (8 * k);
+        *yb |= export_y<E>(export_straight_px(b[k])) << (8 * k);
+        *at |= (t[k] >> 24) << (8 * k);
+        *ab |= (b[k] >> 24) << (8 * k);
+    }
+    const uint32_t uv = export_cbcr<E>(export_block_straight(t[0], t[1], b[0], b[1])) |
+                        (export_cbcr<E>(export_block_straight(t[2], t[3], b[2], b[3])) << 16);
+    *cb = export_cb_pair(uv); *cr = export_cr_pair(uv);
+}
+// yuva444p10le of one row's quad: the Y, Cb, Cr and A samples of each pixel, two words each
+template <int E = 0>
+GLB_HD void export_yuva444p10_quad(const ExportFmt& f, const uint32_t in[4], uint32_t y[2], uint32_t cb[2], uint32_t cr[2],
+                                   uint32_t a[2]) {
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+        const uint32_t p0 = export_alpha_in(f, in[2 * k]), p1 = export_alpha_in(f, in[2 * k + 1]);
+        const uint32_t s0 = export_straight_px(p0), s1 = export_straight_px(p1);
+        const uint32_t uv0 = export_cbcr10_px<E>(s0), uv1 = export_cbcr10_px<E>(s1);
+        y[k] = export_y10<E>(s0) | (export_y10<E>(s1) << 16);
+        cb[k] = (uv0 & 0xffffu) | (uv1 << 16);
+        cr[k] = (uv0 >> 16) | (uv1 & 0xffff0000u);
+        a[k] = export_a10(p0 >> 24) | (export_a10(p1 >> 24) << 16);
+    }
+}
+// What zero pixels become in an alpha format, for the kernels' all-zero shortcut: YUVA420P y / a the Y / A word of a row,
+// u / v the Cb / Cr pairs; YUVA444P10 y, u, v, a one of a row's two equal words per plane; straight RGBA / BGRA y the pixel
+struct ExportZeroA { uint32_t y, u, v, a; };
+template <int E = 0>
+GLB_HD ExportZeroA export_zero_alpha(const ExportFmt& f) {
+    const uint32_t z[4] = { 0u, 0u, 0u, 0u };
+    ExportZeroA o = { 0u, 0u, 0u, 0u };
+    if (f.format == GLAVA_B200_EXPORT_YUVA420P) {
+        uint32_t yb, ab;
+        export_yuva420_quad<E>(f, z, z, &o.y, &yb, &o.u, &o.v, &o.a, &ab);
+    } else if (f.format == GLAVA_B200_EXPORT_YUVA444P10) {
+        uint32_t y[2], u[2], v[2], a[2];
+        export_yuva444p10_quad<E>(f, z, y, u, v, a);
+        o = { y[0], u[0], v[0], a[0] };
+    } else {
+        o.y = export_straight_out(f, f.format, 0u);
+    }
+    return o;
+}
+
 // ---- mark-aware reads ----------------------------------------------------------------------------------------------------
 // When the last raster pass kept dirty-row marks (capi.cu mark_key != 0), slot s of the framebuffer has one word per (band of
 // `rows` rows, 128-pixel strip) at the band's first row (raster_core.h dirty_pack): rows [lo, hi) of the band may be non-zero,
@@ -503,19 +620,21 @@ GLB_HD uint64_t ladder_unit(int rung, int row, int col) { return ((uint64_t) run
 GLB_HD int ladder_unit_rung(uint64_t u) { return (int) (u >> 56); }
 GLB_HD int ladder_unit_row(uint64_t u) { return (int) ((u >> 28) & 0xfffffffu); }
 GLB_HD int ladder_unit_col(uint64_t u) { return (int) (u & 0xfffffffu); }
-// The kernel a ladder launches, from its rungs' formats and encodings (host code): export_ladder_422_kernel when a rung is
-// 4:2:2, else export_ladder_p10_kernel when one is planar 10-bit, else export_ladder_enc_kernel when one has an encoding
-// other than 0, else export_ladder_yuv_kernel when one is I420, YUV444 or P010, else export_ladder_kernel
-enum LadderKernel { ladder_plain = 0, ladder_yuv = 1, ladder_enc = 2, ladder_p10 = 3, ladder_422 = 4 };
+// The kernel a ladder launches, from its rungs' formats (kernel format codes) and encodings (host code):
+// export_ladder_yuva_kernel when a rung is YUVA or straight RGBA / BGRA, else export_ladder_422_kernel when one is 4:2:2,
+// else export_ladder_p10_kernel when one is planar 10-bit, else export_ladder_enc_kernel when one has an encoding other
+// than 0, else export_ladder_yuv_kernel when one is I420, YUV444 or P010, else export_ladder_kernel
+enum LadderKernel { ladder_plain = 0, ladder_yuv = 1, ladder_enc = 2, ladder_p10 = 3, ladder_422 = 4, ladder_yuva = 5 };
 inline int ladder_kernel(const int* format, const int* enc, int n) {
-    bool yuv = false, e = false, p10 = false, k422 = false;
+    bool yuv = false, e = false, p10 = false, k422 = false, alpha = false;
     for (int j = 0; j < n; ++j) {
         yuv |= format[j] != GLAVA_B200_EXPORT_NV12 && export_yuv(format[j]);
         e |= enc[j] != 0;
         p10 |= export_p10(format[j]);
         k422 |= export_422(format[j]);
+        alpha |= export_alpha(format[j]);
     }
-    return k422 ? ladder_422 : p10 ? ladder_p10 : e ? ladder_enc : yuv ? ladder_yuv : ladder_plain;
+    return alpha ? ladder_yuva : k422 ? ladder_422 : p10 ? ladder_p10 : e ? ladder_enc : yuv ? ladder_yuv : ladder_plain;
 }
 
 // ---- overlay (DESIGN 4.12): the frame composited onto the caller's image ----------------------------------------------------

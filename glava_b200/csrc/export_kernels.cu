@@ -27,6 +27,7 @@
 namespace glb {
 
 static_assert(sizeof(LadderRung) == 80, "LadderRung keeps its size: enc sits in what was padding");
+static_assert(sizeof(LadderArgs{}.yuv[0]) == 24, "LadderArgs keeps its size: za sits in what was padding");
 
 // f(std::integral_constant<int, E>()) for the encoding E = enc, 1..3 (DESIGN 4.15): the launchers run these instantiations
 // for any encoding but 0, whose kernels are the ones every call without a colour bit ran before there were encodings
@@ -519,10 +520,127 @@ static void launch_422(const ExportArgs& a, unsigned blocks, cudaStream_t st) {
     });
 }
 
+// ---- transparency: YUVA420P, YUVA444P10 and straight RGBA / BGRA (DESIGN 4.19) ---------------------------------------------
+// export_kernel's items once more (output row pair x 128-pixel strip, a quad per lane).  Per lane: YUVA420P two 4-byte Y
+// stores, a 2-byte Cb and a 2-byte Cr store and two 4-byte A stores (A rows pitch apart, one Cb to Cr distance past Cr);
+// YUVA444P10 an 8-byte Y, Cb, Cr and A store per row; straight RGBA / BGRA a 16-byte store per row.  Past the last full quad
+// YUVA420P has an even width (the last two pixels of a row), the others store pixel by pixel.  Straight RGBA / BGRA run
+// under their kernel format code (export_core.h GLB_EXPORT_STRAIGHT) and encoding 0 only.
+
+// YUVA444P10 of one row's quad: n samples of Y at py, Cb at pu, Cr cr and A 2 cr bytes past it
+template <int E>
+__device__ __forceinline__ void store_yuva444p10(const ExportFmt& f, const uint32_t q[4], uint8_t* py, uint8_t* pu, size_t cr, int n,
+                                                 const ExportZeroA& z) {
+    uint32_t y[2] = { z.y, z.y }, u[2] = { z.u, z.u }, v[2] = { z.v, z.v }, al[2] = { z.a, z.a };
+    if ((q[0] | q[1] | q[2] | q[3]) != 0u) export_yuva444p10_quad<E>(f, q, y, u, v, al);
+    store_u16(py, y, n);
+    store_u16(pu, u, n);
+    store_u16(pu + cr, v, n);
+    store_u16(pu + 2 * cr, al, n);
+}
+
+// straight RGBA / BGRA of one row's quad at x (fmt: the kernel format code; zpx what a zero pixel becomes)
+__device__ __forceinline__ void store_straight(const ExportFmt& f, int fmt, uint8_t* row, int x, int w, const uint32_t in[4],
+                                               uint32_t zpx) {
+    uint32_t px[4] = { zpx, zpx, zpx, zpx };
+    if ((in[0] | in[1] | in[2] | in[3]) != 0u) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) px[k] = export_straight_out(f, fmt, in[k]);
+    }
+    uint32_t* out = reinterpret_cast<uint32_t*>(row) + x;
+    if (x + 4 <= w) __stcs(reinterpret_cast<uint4*>(out), make_uint4(px[0], px[1], px[2], px[3]));
+    else
+        for (int k = 0; k < 4 && x + k < w; ++k) __stcs(out + k, px[k]);
+}
+
+// One item of export_yuva_kernel (and of a ladder's whole-frame alpha rung), as p10_item: the Cb plane at `cb`, Cr `cr`
+// bytes further, A `cr` bytes past Cr; z what zero pixels become (export_zero_alpha).  A reads w, h, marks, mark_rows and
+// pitch.
+template <bool Keep, int E, typename A>
+__device__ __forceinline__ void yuva_item(const A& a, const ExportFmt& f, int fmt, const uint32_t* frame, int slot, uint8_t* dst,
+                                          uint8_t* cb, size_t cr, int j, int strip, int x, const ExportZeroA& z) {
+    const int y0 = a.h - 1 - 2 * j, y1 = y0 - 1;
+    uint32_t top[4] = { 0u, 0u, 0u, 0u }, bot[4] = { 0u, 0u, 0u, 0u };
+    if (row_read(a, slot, y0, strip)) load_quad<Keep>(frame, a.w, y0, x, top);
+    if (y1 >= 0 && row_read(a, slot, y1, strip)) load_quad<Keep>(frame, a.w, y1, x, bot);
+    const bool full = x + 4 <= a.w;
+    if (export_straight(fmt)) {                             // any w and h
+        uint8_t* const r0 = dst + (size_t) (2 * j) * a.pitch;
+        store_straight(f, fmt, r0, x, a.w, top, z.y);
+        if (y1 >= 0) store_straight(f, fmt, r0 + a.pitch, x, a.w, bot, z.y);
+        return;
+    }
+    if (fmt == GLAVA_B200_EXPORT_YUVA444P10) {              // any w and h
+        const int n = full ? 4 : a.w - x;
+        const size_t o = (size_t) (2 * j) * a.pitch + 2 * (size_t) x;
+        store_yuva444p10<E>(f, top, dst + o, cb + o, cr, n, z);
+        if (y1 >= 0) store_yuva444p10<E>(f, bot, dst + o + a.pitch, cb + o + a.pitch, cr, n, z);
+        return;
+    }
+    uint32_t yt = z.y, yb = z.y, u = z.u, v = z.v, at = z.a, ab = z.a;   // YUVA420P, w and h even
+    if ((top[0] | top[1] | top[2] | top[3] | bot[0] | bot[1] | bot[2] | bot[3]) != 0u)
+        export_yuva420_quad<E>(f, top, bot, &yt, &yb, &u, &v, &at, &ab);
+    const size_t o = (size_t) (2 * j) * a.pitch + x;
+    uint8_t* const pu = cb + (size_t) j * (a.pitch >> 1) + (x >> 1);
+    uint8_t* const pa = cb + 2 * cr + o;
+    if (full) {
+        __stcs(reinterpret_cast<uint32_t*>(dst + o), yt);
+        __stcs(reinterpret_cast<uint32_t*>(dst + o + a.pitch), yb);
+        __stcs(reinterpret_cast<unsigned short*>(pu), (unsigned short) u);
+        __stcs(reinterpret_cast<unsigned short*>(pu + cr), (unsigned short) v);
+        __stcs(reinterpret_cast<uint32_t*>(pa), at);
+        __stcs(reinterpret_cast<uint32_t*>(pa + a.pitch), ab);
+    } else {                                                // the last two pixels of a row
+        __stcs(reinterpret_cast<unsigned short*>(dst + o), (unsigned short) yt);
+        __stcs(reinterpret_cast<unsigned short*>(dst + o + a.pitch), (unsigned short) yb);
+        __stcs(pu, (uint8_t) u);
+        __stcs(pu + cr, (uint8_t) v);
+        __stcs(reinterpret_cast<unsigned short*>(pa), (unsigned short) at);
+        __stcs(reinterpret_cast<unsigned short*>(pa + a.pitch), (unsigned short) ab);
+    }
+}
+
+template <typename Index, int Fmt, int E>
+__global__ void __launch_bounds__(256) export_yuva_kernel(const __grid_constant__ ExportArgs a) {
+    const ExportFmt f = { Fmt, a.over, a.native, a.bg };
+    const Index strips = (Index) ((a.w + 127) >> 7), per = strips * (Index) ((a.h + 1) >> 1);
+    const Index items = (Index) a.count * per;
+    const Index warps = (Index) (((size_t) gridDim.x * blockDim.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    const ExportZeroA z = export_zero_alpha<E>(f);          // once per thread, as export_kernel's constants
+    for (Index it = (Index) (((size_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5); it < items; it += warps) {
+        const Index k = it / per, rem = it - k * per;
+        const int j = (int) (rem / strips), strip = (int) (rem - (Index) j * strips);
+        const int x = strip * 128 + lane * 4;
+        if (x >= a.w) continue;
+        const ExportEntry* e = a.list + k;
+        uint8_t* const dst = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst)));
+        const int slot = __ldg(&e->slot);
+        const uint32_t* frame = reinterpret_cast<const uint32_t*>(a.fb) + (size_t) slot * a.h * a.w;
+        yuva_item<false, E>(a, f, Fmt, frame, slot, dst, dst + a.uv_offset, a.cr_offset, j, strip, x, z);
+    }
+}
+
+template <typename Index>
+static void launch_yuva(const ExportArgs& a, unsigned blocks, cudaStream_t st) {
+    if (a.format == (GLAVA_B200_EXPORT_RGBA | GLB_EXPORT_STRAIGHT))
+        export_yuva_kernel<Index, GLAVA_B200_EXPORT_RGBA | GLB_EXPORT_STRAIGHT, 0><<<blocks, 256, 0, st>>>(a);
+    else if (a.format == (GLAVA_B200_EXPORT_BGRA | GLB_EXPORT_STRAIGHT))
+        export_yuva_kernel<Index, GLAVA_B200_EXPORT_BGRA | GLB_EXPORT_STRAIGHT, 0><<<blocks, 256, 0, st>>>(a);
+    else for_any_enc(a.enc, [&](auto e) {
+        constexpr int E = decltype(e)::value;
+        if (a.format == GLAVA_B200_EXPORT_YUVA420P) export_yuva_kernel<Index, GLAVA_B200_EXPORT_YUVA420P, E><<<blocks, 256, 0, st>>>(a);
+        else export_yuva_kernel<Index, GLAVA_B200_EXPORT_YUVA444P10, E><<<blocks, 256, 0, st>>>(a);
+    });
+}
+
 int launch_export(const ExportArgs& a, void* stream) {
     const ExportGrid g = export_grid((uint64_t) a.count * (uint64_t) ((a.w + 127) >> 7) * (uint64_t) ((a.h + 1) >> 1));
     cudaStream_t st = (cudaStream_t) stream;
-    if (export_422(a.format)) {
+    if (export_alpha(a.format)) {
+        if (g.narrow) launch_yuva<uint32_t>(a, g.blocks, st);
+        else launch_yuva<uint64_t>(a, g.blocks, st);
+    } else if (export_422(a.format)) {
         if (g.narrow) launch_422<uint32_t>(a, g.blocks, st);
         else launch_422<uint64_t>(a, g.blocks, st);
     } else if (export_p10(a.format)) {
@@ -864,11 +982,94 @@ static void launch_scaled_422(const ScaledArgs& a, unsigned blocks, cudaStream_t
     });
 }
 
+// One item of export_scaled_yuva_kernel (and of a ladder's other alpha rungs), as scaled_p10_item: output row u (YUVA420P:
+// rows 2u and 2u + 1, the chroma of each 2x2 block from the right neighbour by shuffle) at column X of the lane.  scaled_px
+// with f.over unset averages the stored channels, alpha included (export_scaled RGBA without EXPORT_OVER); the alpha
+// arithmetic then runs on that premultiplied image.  The Cb plane is the entry's dst_uv, Cr `cr` bytes further, A `cr`
+// bytes past Cr; fmt the kernel format code, E the encoding.
+template <bool Keep, int E, typename A>
+__device__ __forceinline__ void scaled_yuva_item(const A& a, const ExportFmt& f, int fmt, const ExportRecip& rcp, uint32_t zc,
+                                                 size_t cr, const ExportEntryUV* e, int u, int X, int lane) {
+    const bool active = X < a.out_w;
+    const int slot = __ldg(&e->slot);
+    const uint32_t* frame = reinterpret_cast<const uint32_t*>(a.fb) + (size_t) slot * a.h * a.w;
+    const ExportSpan sx = export_span(active ? X : 0, a.src_w, a.out_w);
+    uint8_t* const dst = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst)));
+    if (export_straight(fmt)) {
+        const uint32_t px = scaled_px<Keep>(a, f, frame, slot, u, active, sx, rcp, zc);
+        if (!active) return;
+        const uint32_t s = export_straight_px(px);
+        __stcs(reinterpret_cast<uint32_t*>(dst + (size_t) u * a.pitch) + X,
+               (fmt & ~GLB_EXPORT_STRAIGHT) == GLAVA_B200_EXPORT_BGRA ? export_swap_rb(s) : s);
+        return;
+    }
+    uint8_t* const cb = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst_uv)));
+    if (fmt == GLAVA_B200_EXPORT_YUVA444P10) {
+        const uint32_t px = scaled_px<Keep>(a, f, frame, slot, u, active, sx, rcp, zc);
+        if (!active) return;
+        const uint32_t s = export_straight_px(px), uv = export_cbcr10_px<E>(s);
+        const size_t o = (size_t) u * a.pitch + 2 * (size_t) X;
+        __stcs(reinterpret_cast<unsigned short*>(dst + o), (unsigned short) export_y10<E>(s));
+        __stcs(reinterpret_cast<unsigned short*>(cb + o), (unsigned short) uv);
+        __stcs(reinterpret_cast<unsigned short*>(cb + cr + o), (unsigned short) (uv >> 16));
+        __stcs(reinterpret_cast<unsigned short*>(cb + 2 * cr + o), (unsigned short) export_a10(px >> 24));
+        return;
+    }
+    // YUVA420P, out_w even: the whole 2x2 block is in this warp
+    const uint32_t top = scaled_px<Keep>(a, f, frame, slot, 2 * u, active, sx, rcp, zc);
+    const uint32_t bot = scaled_px<Keep>(a, f, frame, slot, 2 * u + 1, active, sx, rcp, zc);
+    const uint32_t top1 = __shfl_down_sync(0xffffffffu, top, 1), bot1 = __shfl_down_sync(0xffffffffu, bot, 1);
+    if (!active) return;
+    const size_t o = (size_t) (2 * u) * a.pitch + X;
+    __stcs(dst + o, (uint8_t) export_y<E>(export_straight_px(top)));
+    __stcs(dst + o + a.pitch, (uint8_t) export_y<E>(export_straight_px(bot)));
+    __stcs(cb + 2 * cr + o, (uint8_t) (top >> 24));
+    __stcs(cb + 2 * cr + o + a.pitch, (uint8_t) (bot >> 24));
+    if (!(lane & 1)) {
+        const uint32_t uv = export_cbcr<E>(export_block_straight(top, top1, bot, bot1));
+        uint8_t* const pu = cb + (size_t) u * (a.pitch >> 1) + (X >> 1);
+        __stcs(pu, (uint8_t) uv);
+        __stcs(pu + cr, (uint8_t) (uv >> 8));
+    }
+}
+
+template <typename Index, int Fmt, int E>
+__global__ void __launch_bounds__(256) export_scaled_yuva_kernel(const __grid_constant__ ScaledArgs a) {
+    const ExportFmt f = { Fmt, a.over, a.native, a.bg };
+    const ExportRecip rcp = { a.div_mul, a.div_shift };
+    const uint32_t zc = f.over ? export_over(0u, f.bg, f.native) : 0u;   // what a zero pixel becomes
+    const Index runs = (Index) ((a.out_w + 31) >> 5), per = runs * (Index) (Fmt == GLAVA_B200_EXPORT_YUVA420P ? a.out_h >> 1 : a.out_h);
+    const Index items = (Index) a.count * per;
+    const Index warps = (Index) (((size_t) gridDim.x * blockDim.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    for (Index it = (Index) (((size_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5); it < items; it += warps) {
+        const Index k = it / per, rem = it - k * per;
+        const int u = (int) (rem / runs), X = (int) (rem - (Index) u * runs) * 32 + lane;
+        scaled_yuva_item<false, E>(a, f, Fmt, rcp, zc, a.cr_offset, a.list + k, u, X, lane);
+    }
+}
+
+template <typename Index>
+static void launch_scaled_yuva(const ScaledArgs& a, unsigned blocks, cudaStream_t st) {
+    if (a.format == (GLAVA_B200_EXPORT_RGBA | GLB_EXPORT_STRAIGHT))
+        export_scaled_yuva_kernel<Index, GLAVA_B200_EXPORT_RGBA | GLB_EXPORT_STRAIGHT, 0><<<blocks, 256, 0, st>>>(a);
+    else if (a.format == (GLAVA_B200_EXPORT_BGRA | GLB_EXPORT_STRAIGHT))
+        export_scaled_yuva_kernel<Index, GLAVA_B200_EXPORT_BGRA | GLB_EXPORT_STRAIGHT, 0><<<blocks, 256, 0, st>>>(a);
+    else for_any_enc(a.enc, [&](auto e) {
+        constexpr int E = decltype(e)::value;
+        if (a.format == GLAVA_B200_EXPORT_YUVA420P) export_scaled_yuva_kernel<Index, GLAVA_B200_EXPORT_YUVA420P, E><<<blocks, 256, 0, st>>>(a);
+        else export_scaled_yuva_kernel<Index, GLAVA_B200_EXPORT_YUVA444P10, E><<<blocks, 256, 0, st>>>(a);
+    });
+}
+
 int launch_export_scaled(const ScaledArgs& a, void* stream) {
     const uint64_t units = export_420(a.format) ? (uint64_t) (a.out_h >> 1) : (uint64_t) a.out_h;
     const ExportGrid g = export_grid((uint64_t) a.count * (uint64_t) ((a.out_w + 31) >> 5) * units);
     cudaStream_t st = (cudaStream_t) stream;
-    if (export_422(a.format)) {
+    if (export_alpha(a.format)) {
+        if (g.narrow) launch_scaled_yuva<uint32_t>(a, g.blocks, st);
+        else launch_scaled_yuva<uint64_t>(a, g.blocks, st);
+    } else if (export_422(a.format)) {
         if (g.narrow) launch_scaled_422<uint32_t>(a, g.blocks, st);
         else launch_scaled_422<uint64_t>(a, g.blocks, st);
     } else if (export_p10(a.format)) {
@@ -1119,13 +1320,75 @@ __global__ void __launch_bounds__(256) export_ladder_422_kernel(const __grid_con
     }
 }
 
+// One unit of an alpha rung of export_ladder_yuva_kernel under encoding E: the item of its standalone kernel
+// (export_yuva_kernel / export_scaled_yuva_kernel), as ladder_p10_item; yuv[rung].za is what a zero pixel's A becomes
+template <int E>
+__device__ __forceinline__ void ladder_yuva_item(const LadderArgs& a, const LadderRung& g, const ExportEntryUV* e, int rung, int row,
+                                                 int col, int lane) {
+    const RungView v = { a.fb, a.marks, a.mark_rows, a.w, a.h, g.format, g.pitch, g.src_x, g.src_y, g.src_w, g.src_h, g.out_w, g.out_h };
+    const ExportFmt f = { g.format, g.over, a.native, g.bg };
+    const size_t cr = a.yuv[rung].cr_offset;
+    if (g.whole) {
+        const int x = col * 128 + lane * 4;
+        if (x >= a.w) return;
+        uint8_t* const dst = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst)));
+        uint8_t* const cb = reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst_uv)));
+        const int slot = __ldg(&e->slot);
+        const uint32_t* frame = reinterpret_cast<const uint32_t*>(a.fb) + (size_t) slot * a.h * a.w;
+        const ExportZeroA z = { a.yuv[rung].zy, a.yuv[rung].zu, a.yuv[rung].zv, a.yuv[rung].za };
+        yuva_item<true, E>(v, f, g.format, frame, slot, dst, cb, cr, row, col, x, z);
+    } else {
+        const ExportRecip rcp = { g.div_mul, g.div_shift };
+        scaled_yuva_item<true, E>(v, f, g.format, rcp, g.zc, cr, e, row, col * 32 + lane, lane);
+    }
+}
+
+// Any format and encoding per rung, launched only when a rung is YUVA420P, YUVA444P10 or straight RGBA / BGRA (DESIGN
+// 4.19): alpha units run ladder_yuva_item, 4:2:2 units ladder_422_item, planar 10-bit units ladder_p10_item, the others
+// ladder_item, each in its rung's encoding, so that the older ladder kernels keep their machine code
+template <typename Index>
+__global__ void __launch_bounds__(256) export_ladder_yuva_kernel(const __grid_constant__ LadderArgs a) {
+    const Index units = (Index) a.units, items = (Index) a.count * units;
+    const Index warps = (Index) (((size_t) gridDim.x * blockDim.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    for (Index it = (Index) (((size_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5); it < items; it += warps) {
+        const Index k = it / units;
+        const uint64_t unit = __ldg(reinterpret_cast<const unsigned long long*>(a.sched) + (it - k * units));
+        const int rung = ladder_unit_rung(unit), row = ladder_unit_row(unit), col = ladder_unit_col(unit);
+        const LadderRung& g = a.rung[rung];
+        const ExportEntryUV* e = a.list + (size_t) k * a.nrungs + rung;
+        if (export_alpha(g.format)) {
+            if (g.enc == 1) ladder_yuva_item<1>(a, g, e, rung, row, col, lane);
+            else if (g.enc == 2) ladder_yuva_item<2>(a, g, e, rung, row, col, lane);
+            else if (g.enc == 3) ladder_yuva_item<3>(a, g, e, rung, row, col, lane);
+            else ladder_yuva_item<0>(a, g, e, rung, row, col, lane);
+        } else if (export_422(g.format)) {
+            if (g.enc == 1) ladder_422_item<1>(a, g, e, rung, row, col, lane);
+            else if (g.enc == 2) ladder_422_item<2>(a, g, e, rung, row, col, lane);
+            else if (g.enc == 3) ladder_422_item<3>(a, g, e, rung, row, col, lane);
+            else ladder_422_item<0>(a, g, e, rung, row, col, lane);
+        } else if (export_p10(g.format)) {
+            if (g.enc == 1) ladder_p10_item<1>(a, g, e, rung, row, col, lane);
+            else if (g.enc == 2) ladder_p10_item<2>(a, g, e, rung, row, col, lane);
+            else if (g.enc == 3) ladder_p10_item<3>(a, g, e, rung, row, col, lane);
+            else ladder_p10_item<0>(a, g, e, rung, row, col, lane);
+        } else if (g.enc == 1) ladder_item<true, 1>(a, g, e, rung, row, col, lane);
+        else if (g.enc == 2) ladder_item<true, 2>(a, g, e, rung, row, col, lane);
+        else if (g.enc == 3) ladder_item<true, 3>(a, g, e, rung, row, col, lane);
+        else ladder_item<true, 0>(a, g, e, rung, row, col, lane);
+    }
+}
+
 int launch_export_ladder(const LadderArgs& a, void* stream) {
     const ExportGrid g = export_grid((uint64_t) a.count * (uint64_t) a.units);
     int format[GLAVA_B200_LADDER_MAX], enc[GLAVA_B200_LADDER_MAX];
     for (int j = 0; j < a.nrungs; ++j) { format[j] = a.rung[j].format; enc[j] = a.rung[j].enc; }
     const int kind = ladder_kernel(format, enc, a.nrungs);
     cudaStream_t st = (cudaStream_t) stream;
-    if (kind == ladder_422) {
+    if (kind == ladder_yuva) {
+        if (g.narrow) export_ladder_yuva_kernel<uint32_t><<<g.blocks, 256, 0, st>>>(a);
+        else export_ladder_yuva_kernel<uint64_t><<<g.blocks, 256, 0, st>>>(a);
+    } else if (kind == ladder_422) {
         if (g.narrow) export_ladder_422_kernel<uint32_t><<<g.blocks, 256, 0, st>>>(a);
         else export_ladder_422_kernel<uint64_t><<<g.blocks, 256, 0, st>>>(a);
     } else if (kind == ladder_p10) {

@@ -38,7 +38,7 @@ int ladder_check(glava_b200* r, const int* streams, int count, const glava_b200_
             uv[i] = dst_uv ? dst_uv[(size_t) i * nrungs + j] : nullptr;
             if (uv[i] && !yuv)
                 return fail(GLAVA_B200_EINVAL, "%s: dst_uv[%d] is for NV12 only, or I420, YUV444, P010, YUV420P10, YUV444P10, "
-                            "YUV422P and YUV422P10 (entry %d)", name,
+                            "YUV422P, YUV422P10, YUVA420P and YUVA444P10 (entry %d)", name,
                             i * nrungs + j, i);
         }
         rc = export_check(ExportKind::scaled, r, streams, count, d.data(), dst_uv && yuv ? uv.data() : nullptr, &rungs[j].desc,
@@ -49,13 +49,15 @@ int ladder_check(glava_b200* r, const int* streams, int count, const glava_b200_
 }
 
 // What zero pixels become in a rung under encoding E: NV12's zy / zuv into g, and export_zero (planar 10-bit: export_zero10;
-// 4:2:2: export_zero422) for the other Y'CbCr formats
+// 4:2:2: export_zero422; the alpha formats: export_zero_alpha) for the other formats
 template <int E>
-static ExportZero rung_zero(const ExportFmt& f, LadderRung* g) {
+static ExportZeroA rung_zero(const ExportFmt& f, LadderRung* g) {
     const uint32_t zero4[4] = { 0u, 0u, 0u, 0u };
     uint32_t zy1;
     g->zuv = export_nv12_quad<E>(f, zero4, zero4, &g->zy, &zy1);
-    return export_422(f.format) ? export_zero422<E>(f) : export_p10(f.format) ? export_zero10<E>(f) : export_zero<E>(f);
+    if (export_alpha(f.format)) return export_zero_alpha<E>(f);
+    const ExportZero z = export_422(f.format) ? export_zero422<E>(f) : export_p10(f.format) ? export_zero10<E>(f) : export_zero<E>(f);
+    return { z.y, z.u, z.v, 0u };
 }
 
 // the device schedule for `geom`, built and uploaded on the raster stream when the geometry differs from the last ladder's
@@ -127,8 +129,9 @@ int ladder_run(glava_b200* r, const int* streams, int count, const glava_b200_ex
         for (int j = 0; j < nrungs; ++j) {
             const glava_b200_export& d = rungs[j].desc;
             LadderRung& g = a.rung[j];
-            g.format = d.format;
-            g.over = export_ycbcr(d.format) || (d.flags & GLAVA_B200_EXPORT_OVER) ? 1 : 0;
+            g.format = export_kernel_format(d.format, d.flags);
+            // the alpha formats are composited only under any other opacity than native (export.cpp export_run)
+            g.over = export_alpha(g.format) ? !v.native : export_ycbcr(d.format) || (d.flags & GLAVA_B200_EXPORT_OVER) ? 1 : 0;
             g.whole = geom[j].whole ? 1 : 0;
             g.bg = background(d);
             g.pitch = d.pitch;
@@ -143,14 +146,14 @@ int ladder_run(glava_b200* r, const int* streams, int count, const glava_b200_ex
             g.zc = f.over ? export_over(0u, f.bg, f.native) : 0u;
             // NV12's words, and the other Y'CbCr formats' as export_yuv_kernel / export_p10_kernel compute them, in the
             // rung's encoding
-            ExportZero z;
+            ExportZeroA z;
             switch (g.enc) {
             case 1: z = rung_zero<1>(f, &g); break;
             case 2: z = rung_zero<2>(f, &g); break;
             case 3: z = rung_zero<3>(f, &g); break;
             default: z = rung_zero<0>(f, &g); break;
             }
-            a.yuv[j] = { planes[j].cr, z.y, z.u, z.v };
+            a.yuv[j] = { planes[j].cr, z.y, z.u, z.v, z.a };
         }
         return launch_export_ladder(a, v.stream);
     });

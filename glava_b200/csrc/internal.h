@@ -209,7 +209,8 @@ struct ExportArgs {
     int    enc;                 // Y'CbCr encoding, export_core.h export_enc of the flags (0: BT.709 limited range)
 };
 // NV12, RGBA and BGRA run export_kernel; I420, YUV444 and P010 export_yuv_kernel; any other encoding than 0 the kernels'
-// instantiations for it (export_nv12_enc_kernel, export_yuv_enc_kernel); YUV420P10 and YUV444P10 export_p10_kernel
+// instantiations for it (export_nv12_enc_kernel, export_yuv_enc_kernel); YUV420P10 and YUV444P10 export_p10_kernel;
+// YUVA420P, YUVA444P10 and straight RGBA / BGRA (format: export_core.h export_kernel_format) export_yuva_kernel
 int launch_export(const ExportArgs& a, void* stream);
 // The entry of the scaled export and the overlay: ExportEntry with a chroma pointer, so that one call can fill an NV12
 // mosaic, where each tile's chroma sits at a different offset from its luma
@@ -299,8 +300,8 @@ struct LadderArgs {
     uint32_t units;
     LadderRung rung[GLAVA_B200_LADDER_MAX];
     // Y'CbCr rungs but NV12: the Cb to Cr distance (ExportArgs cr_offset) and export_core.h export_zero (planar 10-bit:
-    // export_zero10) of the rung
-    struct { size_t cr_offset; uint32_t zy, zu, zv; } yuv[GLAVA_B200_LADDER_MAX];
+    // export_zero10) of the rung; alpha rungs export_zero_alpha, whose A word za sits in what was padding
+    struct { size_t cr_offset; uint32_t zy, zu, zv, za; } yuv[GLAVA_B200_LADDER_MAX];
 };
 // export_ladder_kernel, or export_ladder_yuv_kernel when a rung is I420, YUV444 or P010, or export_ladder_enc_kernel when a
 // rung has an encoding other than 0, or export_ladder_p10_kernel when a rung is YUV420P10 or YUV444P10

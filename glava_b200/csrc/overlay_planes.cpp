@@ -41,9 +41,14 @@ int planes_geometry(int w, int h, const glava_b200_overlay_planes_desc& d, Plane
     if (fmt == GLAVA_B200_EXPORT_RGBA || fmt == GLAVA_B200_EXPORT_BGRA)
         return fail(GLAVA_B200_EINVAL, "%s: format %s: RGBA and BGRA images go to glava_b200_overlay_frames", who,
                     fmt == GLAVA_B200_EXPORT_RGBA ? "RGBA" : "BGRA");
+    if (export_yuva(fmt))                                   // DESIGN 4.19: a transparent layer is exported, not blended onto
+        return fail(GLAVA_B200_EINVAL, "%s: format %s: the overlay writes no alpha plane", who,
+                    fmt == GLAVA_B200_EXPORT_YUVA420P ? "YUVA420P" : "YUVA444P10");
     const char* name = planes_format_name(fmt);
     if (!name) return fail(GLAVA_B200_EINVAL, "%s: unknown format %d", who, fmt);
     const uint32_t colour = GLAVA_B200_EXPORT_FULL_RANGE | GLAVA_B200_EXPORT_BT601;
+    if (d.flags & GLAVA_B200_EXPORT_STRAIGHT)
+        return fail(GLAVA_B200_EINVAL, "%s: flags 0x%x: EXPORT_STRAIGHT is for the exports; the overlay composites", who, d.flags);
     if (d.flags & ~colour)
         return fail(GLAVA_B200_EINVAL, "%s: flags 0x%x: the overlay takes none but EXPORT_FULL_RANGE and EXPORT_BT601", who, d.flags);
     const bool c420 = export_420(fmt), uyvy = fmt == GLAVA_B200_EXPORT_UYVY;

@@ -386,16 +386,34 @@ int   glava_b200_framebuffer_ipc(glava_b200* r, void* handle, size_t handle_byte
  *                              `pitch / 2`; YUV420P10's arithmetic on the pair, as YUV422P's on I420's
  *     GLAVA_B200_EXPORT_UYVY   packed 4:2:2 (ffmpeg's uyvy422, NDI's UYVY, DeckLink's 2vuy): one plane of h rows x 2 w
  *                              bytes at `pitch`, each pixel pair the bytes Cb, Y0, Cr, Y1 of YUV422P; w even (any h)
+ *     GLAVA_B200_EXPORT_YUVA420P   I420 with an alpha plane (ffmpeg's yuva420p, what libvpx-vp9 encodes as WebM with
+ *                              transparency): Y, Cb and Cr as I420 places them, then the A plane of h rows x w bytes at
+ *                              `pitch`, one Cb to Cr distance past Cr.  Never composited: Y per pixel and the chroma of each
+ *                              2x2 block are of the straight (unassociated) colour, the block's colour weighted by alpha,
+ *                              and A is the stored alpha (DESIGN.md §4.19); w and h even, pitch a multiple of 32
+ *     GLAVA_B200_EXPORT_YUVA444P10 YUV444P10 with an alpha plane (yuva444p10le, what ProRes 4444 encoders take): four
+ *                              planes of h rows x w LSB-aligned uint16 at `pitch`, Y, Cb, Cr and A, placed as YUVA420P's;
+ *                              YUV444P10's arithmetic on the straight colour, A = (a 1023 + 127) / 255
+ *   Under any opacity but native the frame is opaque: the YUVA formats write I420's / YUV444P10's Y, Cb and Cr bytes with
+ *   A = 255 (1023).  Zero pixels are transparent black under native opacity.
  *   Where the chroma planes go: NV12 and P010 put the CbCr plane at `uv_offset` from dst[i] (0: pitch * h).  The planar
  *   formats (I420, YUV444, YUV420P10, YUV444P10) put the Cb plane right after the luma, at dst[i] + pitch * h, and
  *   `uv_offset` is the distance from Cb to Cr (0: the Cb plane's own size, so the planes sit back to back as a yuv420p /
  *   yuv444p buffer does); when set it is at least one chroma plane.  YUV422P and YUV422P10 place their planes so too; UYVY
- *   has no chroma plane, and its uv_offset is 0.  All YUV formats are composited (EXPORT_OVER implied).
+ *   has no chroma plane, and its uv_offset is 0.  The YUVA formats put A one Cb to Cr distance past Cr, so with uv_offset
+ *   0 the four planes sit back to back as ffmpeg's yuva420p / yuva444p10le buffers do.  All YUV formats but YUVA420P and
+ *   YUVA444P10 are composited (EXPORT_OVER implied); EXPORT_OVER on a YUVA format is GLAVA_B200_EINVAL.
  *   GLAVA_B200_EXPORT_OVER     (implied for the YUV formats) the opaque colour GLava's window shows over `background` (RGB8,
  *                              byte 3 unused): under setopacity "native" (premultiply_alpha) C = min(255, c +
  *                              mul_norm8(bg, 255 - a)) per channel; under any other opacity the stored colour (the window
  *                              ignores alpha and the clear colour already stands in for the desktop).  Alpha becomes 255.
- *                              Without it RGBA / BGRA carry the stored pixels, alpha included.
+ *                              Without it RGBA / BGRA carry the stored pixels, alpha included (premultiplied under
+ *                              native opacity).
+ *   GLAVA_B200_EXPORT_STRAIGHT (RGBA / BGRA only, not with EXPORT_OVER) the stored pixel with its colour un-premultiplied,
+ *                              what PNG and ffmpeg's rgba / bgra mean: S = a == 0 ? 0 : min(255, (c 255 + a / 2) / a) per
+ *                              channel, alpha as stored; re-premultiplying S with the blend path's unorm8 product gives c
+ *                              back wherever c <= a (DESIGN.md §4.19).  Under any other opacity than native, EXPORT_OVER's
+ *                              bytes.
  *   GLAVA_B200_EXPORT_FULL_RANGE, GLAVA_B200_EXPORT_BT601   the Y'CbCr encoding of every YUV format (DESIGN.md
  *                              §4.15).  Neither: BT.709 limited range.  BT601 takes Kr, Kb = 0.299, 0.114 for BT.709's
  *                              0.2126, 0.0722; FULL_RANGE writes Y = Y', C = 128 + P over 0..255 (10 bits: 1023/255 Y',
@@ -406,9 +424,9 @@ int   glava_b200_framebuffer_ipc(glava_b200* r, void* handle, size_t handle_byte
  *   dst[i], pitch and uv_offset are multiples of 16, pitch >= the row bytes, uv_offset (when set) >= pitch * h (planar
  *   formats: >= one chroma plane).  An unknown format or flag, odd NV12 / I420 / P010 / YUV420P10 dimensions, an odd
  *   YUV422P / YUV422P10 / UYVY width, a misaligned or short pitch (I420, YUV420P10, YUV422P, YUV422P10: not a multiple of
- *   32), a UYVY uv_offset other than 0, a null, host or other-device dst, a stream out of range, count < 1 and a renderer a
- *   failed rebuild left unbuilt are GLAVA_B200_EINVAL with nothing enqueued.  Formats 3, 9 and 13 and above are
- *   unassigned.
+ *   32), a UYVY uv_offset other than 0, EXPORT_STRAIGHT with EXPORT_OVER or on a Y'CbCr format, EXPORT_OVER on a YUVA
+ *   format, a null, host or other-device dst, a stream out of range, count < 1 and a renderer a failed rebuild left unbuilt
+ *   are GLAVA_B200_EINVAL with nothing enqueued.  Formats 3, 9, 13 and 16 and above are unassigned.
  *   The work runs on the handle's stream (glava_b200_cuda_stream) after the latest raster pass and before the next one can
  *   overwrite a slot, so an update issued right after this call cannot change what it exports.  `after_event` (a
  *   cudaEvent_t, or NULL): the export waits for it on the device before writing the destinations — it holds back the
@@ -416,7 +434,8 @@ int   glava_b200_framebuffer_ipc(glava_b200* r, void* handle, size_t handle_byte
  *   Returns once the work is enqueued, without a host wait.
  *   glava_b200_export_bytes    the bytes one destination spans for `desc` on this renderer (pitch * h, UYVY included; NV12 / P010:
  *                              uv_offset + pitch * h / 2; the planar formats: pitch * h + the Cb to Cr distance + one
- *                              chroma plane), after the same descriptor checks.
+ *                              chroma plane; YUVA420P / YUVA444P10: pitch * h + twice the Cb to Cr distance + pitch * h),
+ *                              after the same descriptor checks.
  *   glava_b200_sharded_export_frames  the same with global stream indices, dst[i] on the device of the shard that owns
  *                              streams[i]; every index and pointer is checked before any shard starts, the shards issue
  *                              concurrently, and glava_b200_sharded_sync completes the work. */
@@ -431,18 +450,23 @@ int   glava_b200_framebuffer_ipc(glava_b200* r, void* handle, size_t handle_byte
 #define GLAVA_B200_EXPORT_YUV422P 10
 #define GLAVA_B200_EXPORT_YUV422P10 11
 #define GLAVA_B200_EXPORT_UYVY 12
+#define GLAVA_B200_EXPORT_YUVA420P 14
+#define GLAVA_B200_EXPORT_YUVA444P10 15
 #define GLAVA_B200_EXPORT_OVER 1u
+#define GLAVA_B200_EXPORT_STRAIGHT 0x4u
 #define GLAVA_B200_EXPORT_FULL_RANGE 0x100u
 #define GLAVA_B200_EXPORT_BT601 0x200u
 typedef struct {
     int      format;            /* GLAVA_B200_EXPORT_RGBA / _BGRA / _NV12 / _I420 / _YUV444 / _P010 / _YUV420P10 /
-                                   _YUV444P10 / _YUV422P / _YUV422P10 / _UYVY */
-    uint32_t flags;             /* GLAVA_B200_EXPORT_OVER, and for the Y'CbCr formats _FULL_RANGE / _BT601 */
+                                   _YUV444P10 / _YUV422P / _YUV422P10 / _UYVY / _YUVA420P / _YUVA444P10 */
+    uint32_t flags;             /* GLAVA_B200_EXPORT_OVER or (RGBA / BGRA) _STRAIGHT, and for the Y'CbCr formats
+                                   _FULL_RANGE / _BT601 */
     uint8_t  background[4];     /* R, G, B of the opaque background the composite uses; byte 3 unused */
     size_t   pitch;             /* bytes from one output row to the next (every plane; I420 / YUV420P10 / YUV422P /
                                    YUV422P10 chroma rows: pitch / 2) */
     size_t   uv_offset;         /* NV12 / P010: bytes from dst[i] to the CbCr plane, 0 = pitch * h; the planar formats:
-                                   bytes from the Cb plane to the Cr plane, 0 = one chroma plane */
+                                   bytes from the Cb plane to the Cr plane (YUVA: and from Cr to A), 0 = one chroma
+                                   plane */
 } glava_b200_export;
 int glava_b200_export_bytes(const glava_b200* r, const glava_b200_export* desc, size_t* bytes);
 int glava_b200_export_frames(glava_b200* r, const int* streams, int count, void* const* dst,
