@@ -348,6 +348,10 @@ def lib():
     L.glava_b200_sharded_export_ladder.argtypes = [vp, vp, i32, C.POINTER(ExportRung), i32, vp, vp]
     L.glava_b200_overlay_planes.argtypes = [vp, vp, i32, C.POINTER(Picture), C.POINTER(OverlayPlanesDesc), vp, vp]
     L.glava_b200_sharded_overlay_planes.argtypes = [vp, vp, i32, C.POINTER(Picture), C.POINTER(OverlayPlanesDesc)]
+    L.glava_b200_overlay_frames_opacity.argtypes = [vp, vp, i32, vp, vp, C.POINTER(Export), vp, vp, vp]
+    L.glava_b200_sharded_overlay_frames_opacity.argtypes = [vp, vp, i32, vp, vp, C.POINTER(Export), vp]
+    L.glava_b200_overlay_planes_opacity.argtypes = [vp, vp, i32, C.POINTER(Picture), C.POINTER(OverlayPlanesDesc), vp, vp, vp]
+    L.glava_b200_sharded_overlay_planes_opacity.argtypes = [vp, vp, i32, C.POINTER(Picture), C.POINTER(OverlayPlanesDesc), vp]
     _lib = L
     # errors surface as Python exceptions; keep stderr quiet
     _quiet = C.CFUNCTYPE(None, cp)(lambda msg: None)
@@ -589,6 +593,26 @@ class _FrameExport:
         count, n = int(s.shape[0]), len(rungs)
         dst = (C.c_void_p * max(count * n, 1))(*[ptrs[j][i] for i in range(count) for j in range(n)])
         return s, arr, n, dst, results
+
+    @staticmethod
+    def _opacity(opacity, count):
+        """-> None (opacity None) or the uint8 [count] opacities K = floor(255 o + 0.5) of an overlay (DESIGN 4.20).  opacity:
+        one float for every entry, or a sequence / 1-D array of `count` floats, each in [0, 1].  Raises ValueError for NaN,
+        a value outside [0, 1] or a wrong length."""
+        if opacity is None:
+            return None
+        if hasattr(opacity, "detach"):                        # a torch tensor, possibly on the device
+            opacity = opacity.detach().cpu().numpy()
+        o = np.asarray(opacity, dtype=np.float64)
+        if o.ndim == 0:
+            o = np.full(count, float(o))
+        elif o.ndim != 1 or o.shape[0] != count:
+            raise ValueError(f"opacity: one float or {count} of them, got shape {o.shape}")
+        if np.isnan(o).any():
+            raise ValueError("opacity: NaN")
+        if (o < 0).any() or (o > 1).any():
+            raise ValueError(f"opacity: values must lie in [0, 1] (got {o.min()} .. {o.max()})")
+        return np.ascontiguousarray(np.floor(255.0 * o + 0.5), dtype=np.uint8)
 
     def _overlay_plan(self, streams, images, at, fmt, matrix="bt709", full_range=False):
         """-> (stream list, Export, dst pointers, dst_uv pointers or None) of an overlay (DESIGN 4.12).  images: one uint8
@@ -1113,28 +1137,42 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
                       after, done)
         return results
 
-    def overlay_frames(self, streams, images, at=None, fmt="nv12", after=None, done=None, matrix="bt709", full_range=False):
+    def overlay_frames(self, streams, images, at=None, fmt="nv12", after=None, done=None, matrix="bt709", full_range=False,
+                       opacity=None):
         """The current frames of `streams` composited in place onto the caller's images (glava_b200_overlay_frames): under
         native opacity premultiplied "over" the image's pixels, blended in Y'CbCr for NV12; under any other opacity the
         opaque bytes export_frames writes.  images and at: see _overlay_plan; rectangles of one call must not overlap.
         after / done and the ordering against torch's current stream as export_frames.  matrix / full_range: the encoding
-        of NV12 pictures, which the blend works in (DESIGN 4.15).  Returns images."""
+        of NV12 pictures, which the blend works in (DESIGN 4.15).  opacity: None, or one float in [0, 1] for every entry or
+        one per entry, each frame composited at that strength (glava_b200_overlay_frames_opacity, DESIGN 4.20; under
+        any other opacity than native the opaque frame is faded over the image).  Returns images."""
         s, desc, dst, uv = self._overlay_plan(streams, images, at, fmt, matrix, full_range)
-        self._ordered(lambda a, d: self._L.glava_b200_overlay_frames(self._h, s.ctypes.data, s.shape[0], dst, uv, C.byref(desc),
-                                                                     a, d), after, done)
+        k = self._opacity(opacity, s.shape[0])
+        if k is None:
+            self._ordered(lambda a, d: self._L.glava_b200_overlay_frames(self._h, s.ctypes.data, s.shape[0], dst, uv, C.byref(desc),
+                                                                         a, d), after, done)
+        else:
+            self._ordered(lambda a, d: self._L.glava_b200_overlay_frames_opacity(self._h, s.ctypes.data, s.shape[0], dst, uv,
+                                                                                 C.byref(desc), k.ctypes.data, a, d), after, done)
         return images
 
-    def overlay_planes(self, streams, pictures, at=None, fmt="i420", matrix="bt709", full_range=False, after=None, done=None):
+    def overlay_planes(self, streams, pictures, at=None, fmt="i420", matrix="bt709", full_range=False, after=None, done=None,
+                       opacity=None):
         """The current frames of `streams` composited in place onto decoded pictures, one tensor per plane
         (glava_b200_overlay_planes): NV12, I420, YUV444, P010, YUV420P10, YUV444P10, YUV422P, YUV422P10 or UYVY, the planes of each picture at their
         own addresses with one luma and one chroma pitch per call — ffmpeg's AVFrame planes, NVDEC surfaces, or what
         export_frames returns.  Native opacity blends in Y'CbCr in the picture's encoding (matrix / full_range) as
         overlay_frames blends NV12; any other opacity writes export_frames' bytes.  pictures and at: see _planes_plan;
         rectangles of one call must not overlap in any plane.  after / done and the ordering against torch's current
-        stream as export_frames.  Returns pictures."""
+        stream as export_frames.  opacity: as overlay_frames (glava_b200_overlay_planes_opacity).  Returns pictures."""
         s, desc, arr = self._planes_plan(streams, pictures, at, fmt, matrix, full_range)
-        self._ordered(lambda a, d: self._L.glava_b200_overlay_planes(self._h, s.ctypes.data, s.shape[0], arr, C.byref(desc), a, d),
-                      after, done)
+        k = self._opacity(opacity, s.shape[0])
+        if k is None:
+            self._ordered(lambda a, d: self._L.glava_b200_overlay_planes(self._h, s.ctypes.data, s.shape[0], arr, C.byref(desc), a, d),
+                          after, done)
+        else:
+            self._ordered(lambda a, d: self._L.glava_b200_overlay_planes_opacity(self._h, s.ctypes.data, s.shape[0], arr,
+                                                                                 C.byref(desc), k.ctypes.data, a, d), after, done)
         return pictures
 
     def export_mosaic(self, streams, cols, tile, fmt="nv12", background=(0, 0, 0), out=None, matrix="bt709", full_range=False):
@@ -1344,28 +1382,38 @@ class ShardedRenderer(_StreamState, _StreamStyles, _FrameExport):
         _check(self._L.glava_b200_sharded_export_ladder(self._h, s.ctypes.data, s.shape[0], arr, n, dst, None))
         return results
 
-    def overlay_frames(self, streams, images, at=None, fmt="nv12", matrix="bt709", full_range=False):
+    def overlay_frames(self, streams, images, at=None, fmt="nv12", matrix="bt709", full_range=False, opacity=None):
         """Renderer.overlay_frames with global stream indices (glava_b200_sharded_overlay_frames), each image on the device
         of the shard that owns its stream.  Work queued on torch's current streams of those devices is waited for first;
-        the images are complete after sync().  matrix / full_range as Renderer.overlay_frames."""
+        the images are complete after sync().  matrix / full_range / opacity as Renderer.overlay_frames."""
         import torch
         device_of = self._device_of()
         s, desc, dst, uv = self._overlay_plan(streams, images, at, fmt, matrix, full_range)
+        k = self._opacity(opacity, s.shape[0])
         for d in sorted({device_of(int(x)) for x in s if 0 <= int(x) < self.batch}):
             torch.cuda.current_stream(d).synchronize()
-        _check(self._L.glava_b200_sharded_overlay_frames(self._h, s.ctypes.data, s.shape[0], dst, uv, C.byref(desc)))
+        if k is None:
+            _check(self._L.glava_b200_sharded_overlay_frames(self._h, s.ctypes.data, s.shape[0], dst, uv, C.byref(desc)))
+        else:
+            _check(self._L.glava_b200_sharded_overlay_frames_opacity(self._h, s.ctypes.data, s.shape[0], dst, uv, C.byref(desc),
+                                                                     k.ctypes.data))
         return images
 
-    def overlay_planes(self, streams, pictures, at=None, fmt="i420", matrix="bt709", full_range=False):
+    def overlay_planes(self, streams, pictures, at=None, fmt="i420", matrix="bt709", full_range=False, opacity=None):
         """Renderer.overlay_planes with global stream indices (glava_b200_sharded_overlay_planes), each picture on the device
         of the shard that owns its stream.  Work queued on torch's current streams of those devices is waited for first;
-        the pictures are complete after sync()."""
+        the pictures are complete after sync().  opacity as Renderer.overlay_frames."""
         import torch
         device_of = self._device_of()
         s, desc, arr = self._planes_plan(streams, pictures, at, fmt, matrix, full_range)
+        k = self._opacity(opacity, s.shape[0])
         for d in sorted({device_of(int(x)) for x in s if 0 <= int(x) < self.batch}):
             torch.cuda.current_stream(d).synchronize()
-        _check(self._L.glava_b200_sharded_overlay_planes(self._h, s.ctypes.data, s.shape[0], arr, C.byref(desc)))
+        if k is None:
+            _check(self._L.glava_b200_sharded_overlay_planes(self._h, s.ctypes.data, s.shape[0], arr, C.byref(desc)))
+        else:
+            _check(self._L.glava_b200_sharded_overlay_planes_opacity(self._h, s.ctypes.data, s.shape[0], arr, C.byref(desc),
+                                                                     k.ctypes.data))
         return pictures
 
     def _device_of(self):

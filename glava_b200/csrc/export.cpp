@@ -262,9 +262,10 @@ int export_check(ExportKind kind, glava_b200* r, const int* streams, int count, 
 
 // On the handle's stream, where readback copies: after the latest raster pass, before the next one can overwrite a slot
 int export_run(ExportKind kind, glava_b200* r, const int* streams, int count, void* const* dst, void* const* dst_uv,
-               const glava_b200_export* desc, const glava_b200_export_scale* scale, void* after_event, void* done_event) {
+               const glava_b200_export* desc, const glava_b200_export_scale* scale, void* after_event, void* done_event,
+               const uint8_t* opacity, const char* who) {
     clear_error();
-    const char* who = kCallName[(int) kind];
+    if (!who) who = kCallName[(int) kind];
     if (!r || !desc) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
     glava_b200_export_scale q;
     int rc = export_check(kind, r, streams, count, dst, dst_uv, desc, scale, who, &q);
@@ -280,18 +281,25 @@ int export_run(ExportKind kind, glava_b200* r, const int* streams, int count, vo
     const int over = alpha ? !v.native : yuv || (desc->flags & GLAVA_B200_EXPORT_OVER) ? 1 : 0;
     const ExportPlanes pl = export_planes(desc->format, desc->pitch, desc->uv_offset, q.out_h);
     CU(cudaSetDevice(v.device));
+    // the overlay's opacity (DESIGN 4.20): the fade kernel unless every K is 255, K = 0 entries left out of the list
+    const bool fade = opacity_fades(opacity, count);
+    int n = 0;
+    for (int i = 0; i < count; ++i) n += !fade || opacity[i] ? 1 : 0;
     // export_kernel's entries have no chroma pointer (its machine code stays as measured); the others carry one per entry
-    const size_t bytes = (size_t) count * (kind == ExportKind::frames ? sizeof(ExportEntry) : sizeof(ExportEntryUV));
+    const size_t bytes = (size_t) n * (kind == ExportKind::frames ? sizeof(ExportEntry) : sizeof(ExportEntryUV));
     ExportList* L = nullptr;
     if ((rc = list_room(v, bytes, &L)) != 0) return rc;
     CU(cudaEventSynchronize(L->ev[L->cur]));                // the copy that last read h[cur] (four calls ago)
     uint8_t* const host = L->h[L->cur];
-    for (int i = 0; i < count; ++i) {
+    for (int i = 0, k = 0; i < count; ++i) {
+        if (fade && !opacity[i]) continue;
         uint8_t* const d = (uint8_t*) dst[i];
         const int slot = streams[i] % v.slots;
-        if (kind == ExportKind::frames) reinterpret_cast<ExportEntry*>(host)[i] = { d, slot, 0 };
-        else reinterpret_cast<ExportEntryUV*>(host)[i] = { d, !planes ? nullptr : dst_uv ? (uint8_t*) dst_uv[i] : d + pl.cb, slot, 0 };
+        const int pad = fade ? opacity[i] : 0;
+        if (kind == ExportKind::frames) reinterpret_cast<ExportEntry*>(host)[k++] = { d, slot, 0 };
+        else reinterpret_cast<ExportEntryUV*>(host)[k++] = { d, !planes ? nullptr : dst_uv ? (uint8_t*) dst_uv[i] : d + pl.cb, slot, pad };
     }
+    count = n;
     return list_enqueue(v, L, bytes, after_event, done_event, [&](const void* d_list) {
         if (kind == ExportKind::frames) {
             ExportArgs a = {};
@@ -319,6 +327,7 @@ int export_run(ExportKind kind, glava_b200* r, const int* streams, int count, vo
         common_args(a, v, d_list, count, *desc);
         a.band = a.native && a.marks && a.mark_rows > 0 ? 1 : 0;   // band items wherever marks exist (DESIGN 4.12)
         a.enc = export_enc(desc->flags);
+        a.fade = fade ? 1 : 0;
         return launch_overlay(a, v.stream);
     });
 }
@@ -347,6 +356,11 @@ int glava_b200_export_scaled(glava_b200* r, const int* streams, int count, void*
 int glava_b200_overlay_frames(glava_b200* r, const int* streams, int count, void* const* dst, void* const* dst_uv,
                               const glava_b200_export* desc, void* after_event, void* done_event) {
     return export_run(ExportKind::overlay, r, streams, count, dst, dst_uv, desc, nullptr, after_event, done_event);
+}
+int glava_b200_overlay_frames_opacity(glava_b200* r, const int* streams, int count, void* const* dst, void* const* dst_uv,
+                                      const glava_b200_export* desc, const uint8_t* opacity, void* after_event, void* done_event) {
+    return export_run(ExportKind::overlay, r, streams, count, dst, dst_uv, desc, nullptr, after_event, done_event, opacity,
+                      "glava_b200_overlay_frames_opacity");
 }
 
 }  // extern "C"

@@ -717,6 +717,19 @@ GLB_HD bool overlay_band_pairs(int h, int b0, int lo, int hi, int* ja, int* jb) 
 }
 GLB_HD bool overlay_top_straddles(int h, int b1, int ja) { return h - 1 - 2 * ja >= b1; }
 
+// ---- overlay opacity (DESIGN 4.20) ------------------------------------------------------------------------------------------
+// The pixel an overlay at opacity K (0..255) composites: all four channels of the premultiplied pixel scaled by K / 255 in
+// the blend path's unorm8 product, then blended by the format's own native blend.  mul_norm8(x, 255) = x and mul_norm8(x,
+// 0) = 0, so K = 255 is the plain overlay and K = 0 a zero pixel; the product is monotonic, so c <= a stays c' <= a'.
+GLB_HD uint32_t fade_px(uint32_t px, uint32_t k) {
+    uint32_t out = 0u;
+#pragma unroll
+    for (int c = 0; c < 4; ++c) out |= mul_norm8((px >> (8 * c)) & 255u, k) << (8 * c);
+    return out;
+}
+// Any other opacity than native: GLava's window is opaque, the pixel is the stored colour with alpha 255 (export_over), faded
+GLB_HD uint32_t fade_opaque(uint32_t px, uint32_t k) { return fade_px(px | 0xff000000u, k); }
+
 // ---- overlay onto decoded pictures (DESIGN 4.17): I420, YUV 4:4:4 and the 10-bit formats ------------------------------------
 // 8-bit I420 is NV12's arithmetic (overlay_y, overlay_cbcr of the block's overlay_avg4); YUV 4:4:4 takes overlay_cbcr of
 // each pixel (the average of a 2x2 block of one pixel is that pixel).  10 bits build the same fraction at 10 bits:

@@ -28,6 +28,8 @@ namespace glb {
 
 static_assert(sizeof(LadderRung) == 80, "LadderRung keeps its size: enc sits in what was padding");
 static_assert(sizeof(LadderArgs{}.yuv[0]) == 24, "LadderArgs keeps its size: za sits in what was padding");
+static_assert(sizeof(OverlayArgs) == 72 && sizeof(OverlayPlanesArgs) == 80, "the overlay arguments keep their size: fade sits in "
+              "what was padding");
 
 // f(std::integral_constant<int, E>()) for the encoding E = enc, 1..3 (DESIGN 4.15): the launchers run these instantiations
 // for any encoding but 0, whose kernels are the ones every call without a colour bit ran before there were encodings
@@ -1598,11 +1600,15 @@ __global__ void __launch_bounds__(256) overlay_kernel(const __grid_constant__ Ov
 template <typename Index, bool Band, int E>
 __global__ void __launch_bounds__(256) overlay_enc_kernel(const __grid_constant__ OverlayArgs a) { overlay_loop<Index, Band, E>(a); }
 
+static void launch_overlay_fade(const OverlayArgs& a, const ExportGrid& g, cudaStream_t st);   // DESIGN 4.20, below
+
 int launch_overlay(const OverlayArgs& a, void* stream) {
     const int rows = a.band ? a.mark_rows : 2;
     const ExportGrid g = export_grid((uint64_t) a.count * (uint64_t) ((a.w + 127) >> 7) * (uint64_t) ((a.h + rows - 1) / rows));
     cudaStream_t st = (cudaStream_t) stream;
-    if (a.enc) {
+    if (a.fade) {
+        launch_overlay_fade(a, g, st);
+    } else if (a.enc) {
         for_enc(a.enc, [&](auto e) {
             constexpr int E = decltype(e)::value;
             if (a.band) {
@@ -1874,7 +1880,14 @@ __global__ void __launch_bounds__(256) overlay_planes_kernel(const __grid_consta
 }
 
 template <int Fmt>
+static void launch_planes_fade(const OverlayPlanesArgs& a, const ExportGrid& g, cudaStream_t st);   // DESIGN 4.20, below
+
+template <int Fmt>
 static void launch_planes(const OverlayPlanesArgs& a, const ExportGrid& g, cudaStream_t st) {
+    if (a.fade) {
+        launch_planes_fade<Fmt>(a, g, st);
+        return;
+    }
     for_any_enc(a.enc, [&](auto e) {
         constexpr int E = decltype(e)::value;
         if (a.band) {
@@ -1904,6 +1917,118 @@ int launch_overlay_planes(const OverlayPlanesArgs& a, void* stream) {
     default: return fail(GLAVA_B200_EINVAL, "planes overlay launch: format %d", a.format);
     }
     return launch_status("planes overlay");
+}
+
+// ---- overlay opacity (DESIGN 4.20) ----------------------------------------------------------------------------------------
+// overlay_frames and overlay_planes at a per-entry opacity K (1..254 somewhere in the list; the host drops K = 0 entries and
+// runs the plain kernels when every K is 255), K in the entry's pad word.  Every pixel is scaled by export_core.h fade_px
+// (native opacity) or fade_opaque (any other: the stored colour with alpha 255) and then blended by the format's native
+// item body, so a quad that is zero after scaling is neither loaded from the destination nor stored.  Items are
+// overlay_walk's: bands under native opacity with marks, row pairs otherwise; under any other opacity no pixel is zero, so
+// every row of the rectangle is read and written.
+
+// overlay_walk's Body for overlay_frames' destinations (RGBA / BGRA rows, NV12 row pairs), the native blend only
+template <int E>
+struct OverlayFramesBody {
+    const OverlayArgs& a;
+    ExportFmt f;                                            // unused by the native blend: overlay_nv12 takes it
+    bool bgra;
+    __device__ __forceinline__ explicit OverlayFramesBody(const OverlayArgs& a_)
+        : a(a_), f{ a_.format, 1, 0, 0u }, bgra(a_.format == GLAVA_B200_EXPORT_BGRA) {}
+    static __device__ __forceinline__ uint8_t* dst(const ExportEntryUV* e) {
+        return reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst)));
+    }
+    __device__ __forceinline__ bool pairs() const { return a.format == GLAVA_B200_EXPORT_NV12; }
+    __device__ __forceinline__ uint8_t* chroma(const ExportEntryUV* e) const {
+        return reinterpret_cast<uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&e->dst_uv)));
+    }
+    __device__ __forceinline__ void row(const ExportEntryUV*, uint8_t* dst, int r, int x, const uint32_t q[4]) const {
+        overlay_rgba(dst + (size_t) r * a.pitch, x, a.w, bgra, q);
+    }
+    __device__ __forceinline__ void pair(uint8_t* dst, uint8_t* uv, int j, int x, const uint32_t top[4], const uint32_t bot[4]) const {
+        overlay_nv12<E>(f, true, dst + (size_t) (2 * j) * a.pitch, uv + (size_t) j * a.pitch, a.pitch, x, a.w, top, bot);
+    }
+};
+
+// overlay_walk's Body that scales every pixel by its entry's K and hands it to Inner's native row / pair
+template <typename Args, typename Entry, typename Inner>
+struct OverlayFadeBody {
+    template <typename C> struct Faded { C c; uint32_t k; };
+    const Args& a;
+    Inner in;
+    __device__ __forceinline__ explicit OverlayFadeBody(const Args& a_) : a(a_), in(a_) {}
+    static __device__ __forceinline__ uint32_t k_of(const Entry* e) { return (uint32_t) __ldg(&e->pad); }
+    static __device__ __forceinline__ uint8_t* dst(const Entry* e) { return Inner::dst(e); }
+    __device__ __forceinline__ bool pairs() const { return in.pairs(); }
+    __device__ __forceinline__ auto chroma(const Entry* e) const { return Faded<decltype(in.chroma(e))>{ in.chroma(e), k_of(e) }; }
+    static __device__ __forceinline__ void scale(bool native, uint32_t k, const uint32_t q[4], uint32_t out[4]) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) out[i] = native ? fade_px(q[i], k) : fade_opaque(q[i], k);
+    }
+    // native, band items
+    __device__ __forceinline__ void row(const Entry* e, uint8_t* dst, int r, int x, const uint32_t q[4]) const {
+        uint32_t s[4];
+        scale(true, k_of(e), q, s);
+        in.row(e, dst, r, x, s);
+    }
+    template <typename C>
+    __device__ __forceinline__ void pair(uint8_t* dst, const Faded<C>& c, int j, int x, const uint32_t top[4], const uint32_t bot[4]) const {
+        uint32_t t[4], b[4];
+        scale(true, c.k, top, t);
+        scale(true, c.k, bot, b);
+        in.pair(dst, c.c, j, x, t, b);
+    }
+    // row-pair items, any opacity
+    __device__ __forceinline__ void item(const Entry* e, uint8_t* dst, int u, int x, const uint32_t top[4], const uint32_t bot[4],
+                                         int y1) const {
+        const uint32_t k = k_of(e);
+        uint32_t t[4], b[4];
+        scale(a.native, k, top, t);
+        scale(a.native, k, bot, b);
+        if (in.pairs()) {
+            in.pair(dst, in.chroma(e), u, x, t, b);
+        } else {
+            in.row(e, dst, 2 * u, x, t);
+            if (y1 >= 0) in.row(e, dst, 2 * u + 1, x, b);
+        }
+    }
+};
+
+template <typename Index, bool Band, int E>
+__global__ void __launch_bounds__(256) overlay_fade_kernel(const __grid_constant__ OverlayArgs a) {
+    overlay_walk<Index, Band>(OverlayFadeBody<OverlayArgs, ExportEntryUV, OverlayFramesBody<E>>(a));
+}
+
+template <typename Index, bool Band, int Fmt, int E>
+__global__ void __launch_bounds__(256) overlay_planes_fade_kernel(const __grid_constant__ OverlayPlanesArgs a) {
+    overlay_walk<Index, Band>(OverlayFadeBody<OverlayPlanesArgs, OverlayPlanesEntry, OverlayPlanesBody<Fmt, E>>(a));
+}
+
+static void launch_overlay_fade(const OverlayArgs& a, const ExportGrid& g, cudaStream_t st) {
+    for_any_enc(a.enc, [&](auto e) {
+        constexpr int E = decltype(e)::value;
+        if (a.band) {
+            if (g.narrow) overlay_fade_kernel<uint32_t, true, E><<<g.blocks, 256, 0, st>>>(a);
+            else overlay_fade_kernel<uint64_t, true, E><<<g.blocks, 256, 0, st>>>(a);
+        } else {
+            if (g.narrow) overlay_fade_kernel<uint32_t, false, E><<<g.blocks, 256, 0, st>>>(a);
+            else overlay_fade_kernel<uint64_t, false, E><<<g.blocks, 256, 0, st>>>(a);
+        }
+    });
+}
+
+template <int Fmt>
+static void launch_planes_fade(const OverlayPlanesArgs& a, const ExportGrid& g, cudaStream_t st) {
+    for_any_enc(a.enc, [&](auto e) {
+        constexpr int E = decltype(e)::value;
+        if (a.band) {
+            if (g.narrow) overlay_planes_fade_kernel<uint32_t, true, Fmt, E><<<g.blocks, 256, 0, st>>>(a);
+            else overlay_planes_fade_kernel<uint64_t, true, Fmt, E><<<g.blocks, 256, 0, st>>>(a);
+        } else {
+            if (g.narrow) overlay_planes_fade_kernel<uint32_t, false, Fmt, E><<<g.blocks, 256, 0, st>>>(a);
+            else overlay_planes_fade_kernel<uint64_t, false, Fmt, E><<<g.blocks, 256, 0, st>>>(a);
+        }
+    });
 }
 
 }  // namespace glb

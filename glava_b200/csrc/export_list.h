@@ -45,13 +45,25 @@ bool rects_meet(const Rect& a, const Rect& b, size_t P, size_t B);
 // whether rows of r meet the byte range [f0, f1)
 bool rect_meets_range(const Rect& r, size_t P, size_t B, uintptr_t f0, uintptr_t f1);
 
+// whether an overlay's opacity list ([count] K, null: all 255) needs the fade kernels (DESIGN 4.20): some K is not 255
+inline bool opacity_fades(const uint8_t* opacity, int count) {
+    for (int i = 0; opacity && i < count; ++i)
+        if (opacity[i] != 255) return true;
+    return false;
+}
+
 // The enqueue every call shares, on the raster stream: wait for after_event, copy the list out of the pinned buffer the
-// caller filled (h[cur]) and record its event, launch(device list), then done_event
+// caller filled (h[cur]) and record its event, launch(device list), then done_event.  An empty list (an overlay whose every
+// entry is at opacity 0) copies and launches nothing: the stream still waits for after_event and records done_event.
 template <typename Launch>
 int list_enqueue(const RendererView& v, ExportList* L, size_t bytes, void* after_event, void* done_event, Launch launch) {
     cudaStream_t st = (cudaStream_t) v.stream;
     const int k = L->cur;
     if (after_event) CU(cudaStreamWaitEvent(st, (cudaEvent_t) after_event, 0));
+    if (!bytes) {
+        if (done_event) CU(cudaEventRecord((cudaEvent_t) done_event, st));
+        return 0;
+    }
     CU(cudaMemcpyAsync(L->d, L->h[k], bytes, cudaMemcpyHostToDevice, st));
     CU(cudaEventRecord(L->ev[k], st));
     L->cur = (k + 1) & 3;

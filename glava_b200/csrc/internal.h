@@ -218,7 +218,7 @@ struct alignas(8) ExportEntryUV {
     uint8_t* dst;               // output row 0 (RGBA / BGRA pixels, or Y samples)
     uint8_t* dst_uv;            // NV12 / P010: CbCr row 0; planar formats: Cb row 0 (unused for RGBA / BGRA)
     int      slot;              // framebuffer slot of the listed stream
-    int      pad;
+    int      pad;               // the overlay's fade kernel (DESIGN 4.20): the entry's opacity K, 1..255; else 0
 };
 // export_kernels.cu: glava_b200_export_scaled (DESIGN 4.11), one launch for the whole list, its own argument struct and
 // ExportEntryUV entries so that export_kernel keeps its machine code.  Crop and output size are common to the list; d = src_w * src_h is
@@ -254,6 +254,7 @@ struct OverlayArgs {
     int    format, native, band;
     size_t pitch;
     int    enc;                 // NV12: the destination's encoding, as ExportArgs (enc != 0 runs overlay_enc_kernel)
+    int    fade;                // DESIGN 4.20: 1 runs overlay_fade_kernel, each entry's pad its opacity K (in what was padding)
 };
 int launch_overlay(const OverlayArgs& a, void* stream);
 // export_kernels.cu: glava_b200_overlay_planes (DESIGN 4.17), one launch for the whole list.  Items as OverlayArgs'; an
@@ -261,7 +262,7 @@ int launch_overlay(const OverlayArgs& a, void* stream);
 struct alignas(16) OverlayPlanesEntry {
     uint8_t* plane[3];
     int      slot;              // framebuffer slot of the listed stream
-    int      pad;
+    int      pad;               // as ExportEntryUV's: the fade kernel's opacity K
 };
 struct OverlayPlanesArgs {
     const uint8_t*  fb;         // [slots][h][w] RGBA8
@@ -272,8 +273,9 @@ struct OverlayPlanesArgs {
     int    format, native, band;   // format: NV12, I420, YUV444, P010, YUV420P10 or YUV444P10
     size_t pitch, chroma_pitch;    // bytes between luma rows, between rows of every chroma plane
     int    enc;                 // the picture's encoding, as ExportArgs
+    int    fade;                // as OverlayArgs: 1 runs overlay_planes_fade_kernel (in what was padding)
 };
-// overlay_planes_kernel, instantiated per format, encoding, item kind and index width
+// overlay_planes_kernel (fade: overlay_planes_fade_kernel), instantiated per format, encoding, item kind and index width
 int launch_overlay_planes(const OverlayPlanesArgs& a, void* stream);
 // export_kernels.cu: glava_b200_export_ladder (DESIGN 4.13), one launch for every rung of every entry.  Per rung what a
 // standalone call would take: the whole frame at its own size (whole = 1) runs export_kernel's items, every other rung
@@ -327,9 +329,12 @@ int export_check(ExportKind kind, glava_b200* r, const int* streams, int count, 
                  const glava_b200_export* desc, const glava_b200_export_scale* scale, const char* who,
                  glava_b200_export_scale* q = nullptr);
 // The call of `kind` on one renderer (glava_b200_export_frames / _export_scaled / glava_b200_overlay_frames): every check,
-// then the list copy and the kernel on the raster stream behind `after_event` (or nothing), then `done_event` (or nothing)
+// then the list copy and the kernel on the raster stream behind `after_event` (or nothing), then `done_event` (or nothing).
+// The overlay's `opacity` ([count] K, DESIGN 4.20; null: all 255) drops K = 0 entries and runs the fade kernel unless every K
+// is 255; `who` (null: the plain call's name) names the call in its messages.
 int export_run(ExportKind kind, glava_b200* r, const int* streams, int count, void* const* dst, void* const* dst_uv,
-               const glava_b200_export* desc, const glava_b200_export_scale* scale, void* after_event, void* done_event);
+               const glava_b200_export* desc, const glava_b200_export_scale* scale, void* after_event, void* done_event,
+               const uint8_t* opacity = nullptr, const char* who = nullptr);
 // export_ladder.cpp, glava_b200_export_ladder: `rungs` non-null and 1 <= nrungs <= GLAVA_B200_LADDER_MAX (checked first, also by the sharded form
 // before it splits the list); then export_check of the scaled kind once per rung, `who` extended by the rung's index; dst and
 // dst_uv are [count][nrungs].  q (if non-null): [nrungs] rectangles with their defaults applied.
@@ -355,7 +360,7 @@ bool plane_rects_meet(const PlaneRect& a, const PlaneRect& b);
 int planes_geometry_check(int w, int h, int count, const glava_b200_picture* pics, const glava_b200_overlay_planes_desc& desc,
                           const uint8_t* const* fb, const size_t* fb_bytes, int nfb, const char* who);
 int planes_run(glava_b200* r, const int* streams, int count, const glava_b200_picture* pics, const glava_b200_overlay_planes_desc* desc,
-               void* after_event, void* done_event, const char* who);
+               void* after_event, void* done_event, const char* who, const uint8_t* opacity = nullptr);
 // capi.cu, for sharded.cpp: the blob checks of glava_b200_load_streams (nothing is touched), and save / load with one
 // host pointer per listed stream (the blobs of one shard's streams are not contiguous in the caller's array)
 int state_check_blobs(const glava_b200* r, const void* const* blobs, int count, const char* who);

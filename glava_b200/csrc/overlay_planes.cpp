@@ -152,7 +152,7 @@ int planes_geometry_check(int w, int h, int count, const glava_b200_picture* pic
 
 // On the handle's stream, where readback copies: after the latest raster pass, before the next one can overwrite a slot
 int planes_run(glava_b200* r, const int* streams, int count, const glava_b200_picture* pics, const glava_b200_overlay_planes_desc* desc,
-               void* after_event, void* done_event, const char* who) {
+               void* after_event, void* done_event, const char* who, const uint8_t* opacity) {
     clear_error();
     if (!r || !desc) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
     int rc = planes_check(r, streams, count, pics, desc, who);
@@ -161,13 +161,20 @@ int planes_run(glava_b200* r, const int* streams, int count, const glava_b200_pi
     const size_t fb_bytes = (size_t) v.slots * (size_t) v.h * (size_t) v.w * 4;
     if ((rc = planes_geometry_check(v.w, v.h, count, pics, *desc, &v.fb, &fb_bytes, 1, who)) != 0) return rc;
     CU(cudaSetDevice(v.device));
-    const size_t bytes = (size_t) count * sizeof(OverlayPlanesEntry);
+    // opacity (DESIGN 4.20) as overlay_frames': the fade kernel unless every K is 255, K = 0 entries left out of the list
+    const bool fade = opacity_fades(opacity, count);
+    int n = 0;
+    for (int i = 0; i < count; ++i) n += !fade || opacity[i] ? 1 : 0;
+    const size_t bytes = (size_t) n * sizeof(OverlayPlanesEntry);
     ExportList* L = nullptr;
     if ((rc = list_room(v, bytes, &L)) != 0) return rc;
     CU(cudaEventSynchronize(L->ev[L->cur]));                // the copy that last read h[cur] (four calls ago)
     OverlayPlanesEntry* const host = reinterpret_cast<OverlayPlanesEntry*>((uint8_t*) L->h[L->cur]);
-    for (int i = 0; i < count; ++i)
-        host[i] = { { (uint8_t*) pics[i].plane[0], (uint8_t*) pics[i].plane[1], (uint8_t*) pics[i].plane[2] }, streams[i] % v.slots, 0 };
+    for (int i = 0, k = 0; i < count; ++i)
+        if (!fade || opacity[i])
+            host[k++] = { { (uint8_t*) pics[i].plane[0], (uint8_t*) pics[i].plane[1], (uint8_t*) pics[i].plane[2] }, streams[i] % v.slots,
+                          fade ? opacity[i] : 0 };
+    count = n;
     return list_enqueue(v, L, bytes, after_event, done_event, [&](const void* d_list) {
         OverlayPlanesArgs a = {};
         a.fb = v.fb;
@@ -179,6 +186,7 @@ int planes_run(glava_b200* r, const int* streams, int count, const glava_b200_pi
         a.band = a.native && a.marks && a.mark_rows > 0 ? 1 : 0;   // band items wherever marks exist, as overlay_frames
         a.pitch = desc->pitch; a.chroma_pitch = desc->chroma_pitch;
         a.enc = export_enc(desc->flags);
+        a.fade = fade ? 1 : 0;
         return launch_overlay_planes(a, v.stream);
     });
 }
@@ -188,4 +196,9 @@ int planes_run(glava_b200* r, const int* streams, int count, const glava_b200_pi
 extern "C" int glava_b200_overlay_planes(glava_b200* r, const int* streams, int count, const glava_b200_picture* pics,
                                          const glava_b200_overlay_planes_desc* desc, void* after_event, void* done_event) {
     return glb::planes_run(r, streams, count, pics, desc, after_event, done_event, "glava_b200_overlay_planes");
+}
+extern "C" int glava_b200_overlay_planes_opacity(glava_b200* r, const int* streams, int count, const glava_b200_picture* pics,
+                                                 const glava_b200_overlay_planes_desc* desc, const uint8_t* opacity,
+                                                 void* after_event, void* done_event) {
+    return glb::planes_run(r, streams, count, pics, desc, after_event, done_event, "glava_b200_overlay_planes_opacity", opacity);
 }

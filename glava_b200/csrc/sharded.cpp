@@ -310,10 +310,11 @@ int glava_b200_sharded_get_stream_styles(const glava_b200_sharded* g, const int*
 // The caller-buffer exports (DESIGN 4.10–4.12), global stream indices (repeats allowed): the list is split by shard, dst[i]
 // and dst_uv[i] travelling with streams[i].  Every shard's part passes the single-renderer checks, and for an overlay the
 // whole list the overlap test against itself and every shard's framebuffer (shards may share a device), before any shard
-// starts; the shards then issue at once.  A ladder (rungs non-null) carries nrungs destinations per entry.
+// starts; the shards then issue at once.  A ladder (rungs non-null) carries nrungs destinations per entry; an overlay's
+// opacity (DESIGN 4.20, null: all 255) travels with its entry.
 static int sharded_export(glava_b200_sharded* g, ExportKind kind, const int* streams, int count, void* const* dst,
                           void* const* dst_uv, const glava_b200_export* desc, const glava_b200_export_scale* scale, const char* who,
-                          const glava_b200_export_rung* rungs = nullptr, int nrungs = 1) {
+                          const glava_b200_export_rung* rungs = nullptr, int nrungs = 1, const uint8_t* opacity = nullptr) {
     clear_error();
     const bool ladder = kind == ExportKind::ladder;
     if (!g || (!ladder && !desc)) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
@@ -323,6 +324,7 @@ static int sharded_export(glava_b200_sharded* g, ExportKind kind, const int* str
     const size_t per = ladder ? (size_t) nrungs : 1;
     std::vector<std::vector<int>> idx(g->shards.size());
     std::vector<std::vector<void*>> ptr(g->shards.size()), uv(g->shards.size());
+    std::vector<std::vector<uint8_t>> op(g->shards.size());
     for (int i = 0; i < count; ++i) {
         const int s = streams[i];
         if (s < 0 || s >= g->batch) return fail(GLAVA_B200_EINVAL, "%s: stream %d out of range (batch %d)", who, s, g->batch);
@@ -330,6 +332,7 @@ static int sharded_export(glava_b200_sharded* g, ExportKind kind, const int* str
             const Shard* sh = g->shards[k];
             if (s >= sh->first && s < sh->first + sh->count) {
                 idx[k].push_back(s - sh->first);
+                if (opacity) op[k].push_back(opacity[i]);
                 for (size_t j = 0; j < per; ++j) {
                     ptr[k].push_back(dst[i * per + j]); uv[k].push_back(dst_uv ? dst_uv[i * per + j] : nullptr);
                 }
@@ -361,7 +364,7 @@ static int sharded_export(glava_b200_sharded* g, ExportKind kind, const int* str
             return ladder_run(s.r, idx[k].data(), (int) idx[k].size(), rungs, nrungs, ptr[k].data(), dst_uv ? uv[k].data() : nullptr,
                               nullptr, nullptr, who);
         return export_run(kind, s.r, idx[k].data(), (int) idx[k].size(), ptr[k].data(), dst_uv ? uv[k].data() : nullptr, desc,
-                          scale, nullptr, nullptr);
+                          scale, nullptr, nullptr, opacity ? op[k].data() : nullptr, opacity ? who : nullptr);
     });
 }
 
@@ -376,23 +379,29 @@ int glava_b200_sharded_overlay_frames(glava_b200_sharded* g, const int* streams,
                                       const glava_b200_export* desc) {
     return sharded_export(g, ExportKind::overlay, streams, count, dst, dst_uv, desc, nullptr, "glava_b200_sharded_overlay_frames");
 }
+int glava_b200_sharded_overlay_frames_opacity(glava_b200_sharded* g, const int* streams, int count, void* const* dst,
+                                              void* const* dst_uv, const glava_b200_export* desc, const uint8_t* opacity) {
+    return sharded_export(g, ExportKind::overlay, streams, count, dst, dst_uv, desc, nullptr, "glava_b200_sharded_overlay_frames_opacity",
+                          nullptr, 1, opacity);
+}
 int glava_b200_sharded_export_ladder(glava_b200_sharded* g, const int* streams, int count, const glava_b200_export_rung* rungs,
                                      int nrungs, void* const* dst, void* const* dst_uv) {
     return sharded_export(g, ExportKind::ladder, streams, count, dst, dst_uv, nullptr, nullptr, "glava_b200_sharded_export_ladder",
                           rungs, nrungs);
 }
 
-// glava_b200_overlay_planes with global stream indices: the list split by shard (pics[i] travelling with streams[i]), every
-// shard's part checked as one renderer, then the whole list's overlap and every shard's framebuffer, before any shard starts
-int glava_b200_sharded_overlay_planes(glava_b200_sharded* g, const int* streams, int count, const glava_b200_picture* pics,
-                                      const glava_b200_overlay_planes_desc* desc) {
+// glava_b200_overlay_planes with global stream indices: the list split by shard (pics[i] and opacity[i] travelling with
+// streams[i]), every shard's part checked as one renderer, then the whole list's overlap and every shard's framebuffer, before
+// any shard starts
+static int sharded_planes(glava_b200_sharded* g, const int* streams, int count, const glava_b200_picture* pics,
+                          const glava_b200_overlay_planes_desc* desc, const uint8_t* opacity, const char* who) {
     clear_error();
-    const char* who = "glava_b200_sharded_overlay_planes";
     if (!g || !desc) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
     if (count < 1) return fail(GLAVA_B200_EINVAL, "%s: count %d < 1", who, count);
     if (!streams || !pics) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
     std::vector<std::vector<int>> idx(g->shards.size());
     std::vector<std::vector<glava_b200_picture>> part(g->shards.size());
+    std::vector<std::vector<uint8_t>> op(g->shards.size());
     for (int i = 0; i < count; ++i) {
         const int s = streams[i];
         if (s < 0 || s >= g->batch) return fail(GLAVA_B200_EINVAL, "%s: stream %d out of range (batch %d)", who, s, g->batch);
@@ -401,6 +410,7 @@ int glava_b200_sharded_overlay_planes(glava_b200_sharded* g, const int* streams,
             if (s >= sh->first && s < sh->first + sh->count) {
                 idx[k].push_back(s - sh->first);
                 part[k].push_back(pics[i]);
+                if (opacity) op[k].push_back(opacity[i]);
                 break;
             }
         }
@@ -420,8 +430,17 @@ int glava_b200_sharded_overlay_planes(glava_b200_sharded* g, const int* streams,
     return broadcast(g, [&](Shard& s) {
         const size_t k = (size_t) (std::find(g->shards.begin(), g->shards.end(), &s) - g->shards.begin());
         if (idx[k].empty()) return 0;
-        return planes_run(s.r, idx[k].data(), (int) idx[k].size(), part[k].data(), desc, nullptr, nullptr, who);
+        return planes_run(s.r, idx[k].data(), (int) idx[k].size(), part[k].data(), desc, nullptr, nullptr, who,
+                          opacity ? op[k].data() : nullptr);
     });
+}
+int glava_b200_sharded_overlay_planes(glava_b200_sharded* g, const int* streams, int count, const glava_b200_picture* pics,
+                                      const glava_b200_overlay_planes_desc* desc) {
+    return sharded_planes(g, streams, count, pics, desc, nullptr, "glava_b200_sharded_overlay_planes");
+}
+int glava_b200_sharded_overlay_planes_opacity(glava_b200_sharded* g, const int* streams, int count, const glava_b200_picture* pics,
+                                              const glava_b200_overlay_planes_desc* desc, const uint8_t* opacity) {
+    return sharded_planes(g, streams, count, pics, desc, opacity, "glava_b200_sharded_overlay_planes_opacity");
 }
 
 int glava_b200_sharded_textures(glava_b200_sharded* g, uint16_t* out_l, uint16_t* out_r) {

@@ -614,6 +614,27 @@ typedef struct {
 int glava_b200_overlay_planes(glava_b200* r, const int* streams, int count, const glava_b200_picture* pics,
                               const glava_b200_overlay_planes_desc* desc, void* after_event, void* done_event);
 
+/* Overlay at a per-entry opacity (DESIGN.md §4.20), for fading a visualiser in and out and running it translucent over video:
+ *   glava_b200_overlay_frames_opacity / glava_b200_overlay_planes_opacity  the plain calls with one more argument,
+ *     opacity                  [count] opacities K, 0..255, of the entries (read during the call, as streams); NULL: all 255
+ *   Entry i composites a pixel scaled by K_i / 255 in all four channels with the blend path's unorm8 product (mul_norm8, so
+ *   premultiplied colour stays at or below alpha) through the format's native blend.  Under setopacity "native" the pixel
+ *   is the stored premultiplied one; under any other opacity GLava's window is opaque and it is the stored colour with
+ *   alpha 255, which at K = 255 gives exactly the plain call's bytes.  K = 255 is the plain call bit for bit, K = 0 leaves
+ *   the picture untouched; against the float64 composite c K / 255 + D (1 - a K / 255^2) the result stays within the
+ *   bounds DESIGN.md §4.20 records per format and encoding.  Every refusal of the plain call applies unchanged, to every
+ *   entry (K = 0 ones included), and names the _opacity call.  A list whose K are all 255 (or NULL) runs the plain
+ *   kernel; K = 0 entries are left out of the device list, and a list of only those enqueues no kernel (the stream still
+ *   waits for after_event and records done_event).
+ *   glava_b200_sharded_overlay_frames_opacity / glava_b200_sharded_overlay_planes_opacity  the sharded forms, opacity[i]
+ *                              travelling with streams[i]. */
+int glava_b200_overlay_frames_opacity(glava_b200* r, const int* streams, int count, void* const* dst, void* const* dst_uv,
+                                      const glava_b200_export* desc, const uint8_t* opacity /* [count], NULL = all 255 */,
+                                      void* after_event, void* done_event);
+int glava_b200_overlay_planes_opacity(glava_b200* r, const int* streams, int count, const glava_b200_picture* pics,
+                                      const glava_b200_overlay_planes_desc* desc, const uint8_t* opacity /* [count], NULL = all 255 */,
+                                      void* after_event, void* done_event);
+
 /* ---- one handle for a batch spread over several GPUs of a node (csrc/sharded.cpp) -------------------------------------
  * The streams of a batch are independent (one GLava process each, in the reference), so the batch is cut into contiguous
  * blocks, one per device — glava_b200_shard_range: counts differ by at most one — and nothing crosses between devices (no
@@ -647,6 +668,12 @@ int  glava_b200_sharded_overlay_frames(glava_b200_sharded* s, const int* streams
                                        void* const* dst_uv, const glava_b200_export* desc);   /* see glava_b200_overlay_frames */
 int  glava_b200_sharded_overlay_planes(glava_b200_sharded* s, const int* streams, int count, const glava_b200_picture* pics,
                                        const glava_b200_overlay_planes_desc* desc);   /* see glava_b200_overlay_planes */
+int  glava_b200_sharded_overlay_frames_opacity(glava_b200_sharded* s, const int* streams, int count, void* const* dst,
+                                               void* const* dst_uv, const glava_b200_export* desc,
+                                               const uint8_t* opacity);   /* see glava_b200_overlay_frames_opacity */
+int  glava_b200_sharded_overlay_planes_opacity(glava_b200_sharded* s, const int* streams, int count, const glava_b200_picture* pics,
+                                               const glava_b200_overlay_planes_desc* desc,
+                                               const uint8_t* opacity);   /* see glava_b200_overlay_planes_opacity */
 int  glava_b200_sharded_export_ladder(glava_b200_sharded* s, const int* streams, int count,
                                       const glava_b200_export_rung* rungs, int nrungs, void* const* dst,
                                       void* const* dst_uv);   /* global indices; see glava_b200_export_ladder */
