@@ -352,6 +352,10 @@ def lib():
     L.glava_b200_sharded_overlay_frames_opacity.argtypes = [vp, vp, i32, vp, vp, C.POINTER(Export), vp]
     L.glava_b200_overlay_planes_opacity.argtypes = [vp, vp, i32, C.POINTER(Picture), C.POINTER(OverlayPlanesDesc), vp, vp, vp]
     L.glava_b200_sharded_overlay_planes_opacity.argtypes = [vp, vp, i32, C.POINTER(Picture), C.POINTER(OverlayPlanesDesc), vp]
+    L.glava_b200_overlay_scaled.argtypes = [vp, vp, i32, C.POINTER(Picture), C.POINTER(OverlayPlanesDesc), C.POINTER(ExportScale),
+                                            vp, vp, vp]
+    L.glava_b200_sharded_overlay_scaled.argtypes = [vp, vp, i32, C.POINTER(Picture), C.POINTER(OverlayPlanesDesc),
+                                                    C.POINTER(ExportScale), vp]
     _lib = L
     # errors surface as Python exceptions; keep stderr quiet
     _quiet = C.CFUNCTYPE(None, cp)(lambda msg: None)
@@ -614,13 +618,43 @@ class _FrameExport:
             raise ValueError(f"opacity: values must lie in [0, 1] (got {o.min()} .. {o.max()})")
         return np.ascontiguousarray(np.floor(255.0 * o + 0.5), dtype=np.uint8)
 
-    def _overlay_plan(self, streams, images, at, fmt, matrix="bt709", full_range=False):
+    @staticmethod
+    def _overlay_scale(size, crop):
+        """-> (None, None) when size and crop are None (the overlay at the frame's own size), else (rectangle size (w, h),
+        ExportScale) of an overlay of the downscaled, cropped frame (DESIGN 4.21): size = (w, h), None: the crop's size; crop
+        = (x, y, w, h) in top-down coordinates, None: the whole frame.  Raises ValueError for a size that is not two
+        positive integers or a crop that is not four integers (the library refuses a crop that leaves the frame and
+        upscaling)."""
+        if size is None and crop is None:
+            return None, None
+        if crop is not None:
+            crop = tuple(int(v) for v in crop)
+            if len(crop) != 4:
+                raise ValueError(f"crop: (x, y, w, h), got {crop}")
+        size = crop[2:] if size is None else tuple(int(v) for v in size)
+        if len(size) != 2 or min(size) < 1:
+            raise ValueError(f"size: (w, h) of positive integers, got {size}")
+        return size, _export_scale(size, crop)
+
+    @staticmethod
+    def _frames_pictures(desc, dst, uv, count):
+        """overlay_frames' (Export, dst, dst_uv) as glava_b200_overlay_scaled's (OverlayPlanesDesc, Picture array): RGBA /
+        BGRA one plane, NV12 its Y and CbCr planes at one pitch"""
+        pd = OverlayPlanesDesc()
+        pd.format, pd.flags, pd.pitch = desc.format, desc.flags, desc.pitch
+        pd.chroma_pitch = desc.pitch if uv is not None else 0
+        arr = (Picture * max(count, 1))()
+        for i in range(count):
+            arr[i].plane = (C.c_void_p * 3)(dst[i], uv[i] if uv is not None else None, None)
+        return pd, arr
+
+    def _overlay_plan(self, streams, images, at, fmt, matrix="bt709", full_range=False, size=None):
         """-> (stream list, Export, dst pointers, dst_uv pointers or None) of an overlay (DESIGN 4.12).  images: one uint8
         CUDA tensor per entry (one may repeat) or one [count, ...] tensor, each [H, W, 4] (RGBA / BGRA) or [H * 3 / 2, W]
         (NV12, CbCr rows from row H) with contiguous rows and one pitch for all; at: (x, y) of each frame's top-left
         corner in its image (None: (0, 0)).  Raises ValueError for a rectangle that leaves its image or whose rows do
         not start at multiples of 16 bytes (the device refuses the rest).  matrix / full_range: the encoding of an NV12
-        picture (_export_desc)."""
+        picture (_export_desc).  size: the rectangle's (w, h), None: the frame's."""
         import torch
         s = np.ascontiguousarray(np.asarray(streams, dtype=np.int64).reshape(-1), dtype=np.int32)
         count = int(s.shape[0])
@@ -657,7 +691,7 @@ class _FrameExport:
         at = [(0, 0)] * count if at is None else [(int(x), int(y)) for x, y in at]
         if len(at) != count:
             raise ValueError(f"at: {count} positions, got {len(at)}")
-        w, h = self.params.w, self.params.h
+        w, h = size or (self.params.w, self.params.h)
         px = 1 if nv12 else 4
         dst, uv, pitch = [], [], None
         for i, ((base, H, W, ip), (x, y)) in enumerate(zip(ents, at)):
@@ -679,7 +713,7 @@ class _FrameExport:
         arr = (C.c_void_p * max(count, 1))(*dst)
         return s, desc, arr, (C.c_void_p * max(count, 1))(*uv) if nv12 else None
 
-    def _planes_plan(self, streams, pictures, at, fmt, matrix="bt709", full_range=False):
+    def _planes_plan(self, streams, pictures, at, fmt, matrix="bt709", full_range=False, size=None):
         """-> (stream list, OverlayPlanesDesc, Picture array) of an overlay onto decoded pictures (DESIGN 4.17).  pictures:
         one tuple of plane tensors per entry (a tuple may repeat), or one tuple of batched [count, rows, cols] plane tensors;
         a tuple is (Y, CbCr) for NV12 and P010, (Y, Cb, Cr) otherwise, each CUDA, uint8 (the 8-bit formats) or uint16 or
@@ -688,7 +722,8 @@ class _FrameExport:
         YUV422P10 Cb and Cr [H, W / 2] (export_frames' plane views); UYVY is one plane [H, 2 W] of bytes, given as a tensor
         or a 1-tuple (one [count, H, 2 W] tensor for a batch), and a 4:2:2 frame starts at an even x.  Every luma plane has one pitch and every chroma plane one pitch.  at: (x, y) of each frame's top-left
         in luma samples (None: (0, 0)).  Raises ValueError for a rectangle that leaves its picture, mixed pitches within a
-        plane kind, or a plane start that is not 16-byte aligned (the library refuses the rest)."""
+        plane kind, or a plane start that is not 16-byte aligned (the library refuses the rest).  size: the rectangle's (w, h),
+        None: the frame's."""
         import torch
         if fmt not in PLANES_FORMATS:
             raise ValueError(f"format {fmt!r}: overlay_planes takes one of {list(PLANES_FORMATS)} "
@@ -752,7 +787,7 @@ class _FrameExport:
         at = [(0, 0)] * count if at is None else [(int(x), int(y)) for x, y in at]
         if len(at) != count:
             raise ValueError(f"at: {count} positions, got {len(at)}")
-        w, h = self.params.w, self.params.h
+        w, h = size or (self.params.w, self.params.h)
         arr = (Picture * max(count, 1))()
         pitch = cpitch = None
         for i, ((bases, H, W, P, CP), (x, y)) in enumerate(zip(ents, at)):
@@ -1138,17 +1173,25 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
         return results
 
     def overlay_frames(self, streams, images, at=None, fmt="nv12", after=None, done=None, matrix="bt709", full_range=False,
-                       opacity=None):
+                       opacity=None, size=None, crop=None):
         """The current frames of `streams` composited in place onto the caller's images (glava_b200_overlay_frames): under
         native opacity premultiplied "over" the image's pixels, blended in Y'CbCr for NV12; under any other opacity the
         opaque bytes export_frames writes.  images and at: see _overlay_plan; rectangles of one call must not overlap.
         after / done and the ordering against torch's current stream as export_frames.  matrix / full_range: the encoding
         of NV12 pictures, which the blend works in (DESIGN 4.15).  opacity: None, or one float in [0, 1] for every entry or
         one per entry, each frame composited at that strength (glava_b200_overlay_frames_opacity, DESIGN 4.20; under
-        any other opacity than native the opaque frame is faded over the image).  Returns images."""
-        s, desc, dst, uv = self._overlay_plan(streams, images, at, fmt, matrix, full_range)
+        any other opacity than native the opaque frame is faded over the image).  size / crop: None, or the frame shrunk
+        to size = (w, h) from crop = (x, y, w, h) as export_scaled takes them, composited into a w x h rectangle
+        (glava_b200_overlay_scaled, DESIGN 4.21).  Returns images."""
+        rect, sc = self._overlay_scale(size, crop)
+        s, desc, dst, uv = self._overlay_plan(streams, images, at, fmt, matrix, full_range, rect)
         k = self._opacity(opacity, s.shape[0])
-        if k is None:
+        if sc is not None:
+            pd, arr = self._frames_pictures(desc, dst, uv, s.shape[0])
+            self._ordered(lambda a, d: self._L.glava_b200_overlay_scaled(self._h, s.ctypes.data, s.shape[0], arr, C.byref(pd),
+                                                                         C.byref(sc), None if k is None else k.ctypes.data,
+                                                                         a, d), after, done)
+        elif k is None:
             self._ordered(lambda a, d: self._L.glava_b200_overlay_frames(self._h, s.ctypes.data, s.shape[0], dst, uv, C.byref(desc),
                                                                          a, d), after, done)
         else:
@@ -1157,17 +1200,23 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
         return images
 
     def overlay_planes(self, streams, pictures, at=None, fmt="i420", matrix="bt709", full_range=False, after=None, done=None,
-                       opacity=None):
+                       opacity=None, size=None, crop=None):
         """The current frames of `streams` composited in place onto decoded pictures, one tensor per plane
         (glava_b200_overlay_planes): NV12, I420, YUV444, P010, YUV420P10, YUV444P10, YUV422P, YUV422P10 or UYVY, the planes of each picture at their
         own addresses with one luma and one chroma pitch per call — ffmpeg's AVFrame planes, NVDEC surfaces, or what
         export_frames returns.  Native opacity blends in Y'CbCr in the picture's encoding (matrix / full_range) as
         overlay_frames blends NV12; any other opacity writes export_frames' bytes.  pictures and at: see _planes_plan;
         rectangles of one call must not overlap in any plane.  after / done and the ordering against torch's current
-        stream as export_frames.  opacity: as overlay_frames (glava_b200_overlay_planes_opacity).  Returns pictures."""
-        s, desc, arr = self._planes_plan(streams, pictures, at, fmt, matrix, full_range)
+        stream as export_frames.  opacity: as overlay_frames (glava_b200_overlay_planes_opacity).  size / crop: as
+        overlay_frames (glava_b200_overlay_scaled).  Returns pictures."""
+        rect, sc = self._overlay_scale(size, crop)
+        s, desc, arr = self._planes_plan(streams, pictures, at, fmt, matrix, full_range, rect)
         k = self._opacity(opacity, s.shape[0])
-        if k is None:
+        if sc is not None:
+            self._ordered(lambda a, d: self._L.glava_b200_overlay_scaled(self._h, s.ctypes.data, s.shape[0], arr, C.byref(desc),
+                                                                         C.byref(sc), None if k is None else k.ctypes.data,
+                                                                         a, d), after, done)
+        elif k is None:
             self._ordered(lambda a, d: self._L.glava_b200_overlay_planes(self._h, s.ctypes.data, s.shape[0], arr, C.byref(desc), a, d),
                           after, done)
         else:
@@ -1382,34 +1431,45 @@ class ShardedRenderer(_StreamState, _StreamStyles, _FrameExport):
         _check(self._L.glava_b200_sharded_export_ladder(self._h, s.ctypes.data, s.shape[0], arr, n, dst, None))
         return results
 
-    def overlay_frames(self, streams, images, at=None, fmt="nv12", matrix="bt709", full_range=False, opacity=None):
+    def overlay_frames(self, streams, images, at=None, fmt="nv12", matrix="bt709", full_range=False, opacity=None, size=None,
+                       crop=None):
         """Renderer.overlay_frames with global stream indices (glava_b200_sharded_overlay_frames), each image on the device
         of the shard that owns its stream.  Work queued on torch's current streams of those devices is waited for first;
-        the images are complete after sync().  matrix / full_range / opacity as Renderer.overlay_frames."""
+        the images are complete after sync().  matrix / full_range / opacity / size / crop as Renderer.overlay_frames."""
         import torch
         device_of = self._device_of()
-        s, desc, dst, uv = self._overlay_plan(streams, images, at, fmt, matrix, full_range)
+        rect, sc = self._overlay_scale(size, crop)
+        s, desc, dst, uv = self._overlay_plan(streams, images, at, fmt, matrix, full_range, rect)
         k = self._opacity(opacity, s.shape[0])
         for d in sorted({device_of(int(x)) for x in s if 0 <= int(x) < self.batch}):
             torch.cuda.current_stream(d).synchronize()
-        if k is None:
+        if sc is not None:
+            pd, arr = self._frames_pictures(desc, dst, uv, s.shape[0])
+            _check(self._L.glava_b200_sharded_overlay_scaled(self._h, s.ctypes.data, s.shape[0], arr, C.byref(pd), C.byref(sc),
+                                                             None if k is None else k.ctypes.data))
+        elif k is None:
             _check(self._L.glava_b200_sharded_overlay_frames(self._h, s.ctypes.data, s.shape[0], dst, uv, C.byref(desc)))
         else:
             _check(self._L.glava_b200_sharded_overlay_frames_opacity(self._h, s.ctypes.data, s.shape[0], dst, uv, C.byref(desc),
                                                                      k.ctypes.data))
         return images
 
-    def overlay_planes(self, streams, pictures, at=None, fmt="i420", matrix="bt709", full_range=False, opacity=None):
+    def overlay_planes(self, streams, pictures, at=None, fmt="i420", matrix="bt709", full_range=False, opacity=None, size=None,
+                       crop=None):
         """Renderer.overlay_planes with global stream indices (glava_b200_sharded_overlay_planes), each picture on the device
         of the shard that owns its stream.  Work queued on torch's current streams of those devices is waited for first;
-        the pictures are complete after sync().  opacity as Renderer.overlay_frames."""
+        the pictures are complete after sync().  opacity / size / crop as Renderer.overlay_frames."""
         import torch
         device_of = self._device_of()
-        s, desc, arr = self._planes_plan(streams, pictures, at, fmt, matrix, full_range)
+        rect, sc = self._overlay_scale(size, crop)
+        s, desc, arr = self._planes_plan(streams, pictures, at, fmt, matrix, full_range, rect)
         k = self._opacity(opacity, s.shape[0])
         for d in sorted({device_of(int(x)) for x in s if 0 <= int(x) < self.batch}):
             torch.cuda.current_stream(d).synchronize()
-        if k is None:
+        if sc is not None:
+            _check(self._L.glava_b200_sharded_overlay_scaled(self._h, s.ctypes.data, s.shape[0], arr, C.byref(desc), C.byref(sc),
+                                                             None if k is None else k.ctypes.data))
+        elif k is None:
             _check(self._L.glava_b200_sharded_overlay_planes(self._h, s.ctypes.data, s.shape[0], arr, C.byref(desc)))
         else:
             _check(self._L.glava_b200_sharded_overlay_planes_opacity(self._h, s.ctypes.data, s.shape[0], arr, C.byref(desc),

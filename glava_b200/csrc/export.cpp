@@ -103,17 +103,8 @@ int desc_check(ExportKind kind, int w, int h, const glava_b200_export& d, const 
                     export_ycbcr(d.format) ? " but EXPORT_FULL_RANGE and EXPORT_BT601" : "");
     *q = { 0, 0, w, h, w, h };
     if (kind != ExportKind::scaled) return desc_size(w, h, d, "frame", who);
-    if (!s) return fail(GLAVA_B200_EINVAL, "%s: null scale", who);
-    *q = *s;
-    if (!q->src_x && !q->src_y && !q->src_w && !q->src_h) { q->src_w = w; q->src_h = h; }
-    if (q->src_x < 0 || q->src_y < 0 || q->src_w < 1 || q->src_h < 1 || (int64_t) q->src_x + q->src_w > w ||
-        (int64_t) q->src_y + q->src_h > h)
-        return fail(GLAVA_B200_EINVAL, "%s: source rectangle (%d, %d) %dx%d is empty or leaves the %dx%d frame", who, q->src_x,
-                    q->src_y, q->src_w, q->src_h, w, h);
-    if (q->out_w < 1 || q->out_h < 1 || q->out_w > q->src_w || q->out_h > q->src_h)
-        return fail(GLAVA_B200_EINVAL, "%s: output %dx%d must be at least 1x1 and at most the %dx%d source (no upscaling)", who,
-                    q->out_w, q->out_h, q->src_w, q->src_h);
-    return desc_size(q->out_w, q->out_h, d, "output", who);
+    const int rc = scale_check(w, h, s, q, who);
+    return rc ? rc : desc_size(q->out_w, q->out_h, d, "output", who);
 }
 
 // the byte count of one destination of a call of `kind`
@@ -151,6 +142,20 @@ void common_args(Args& a, const RendererView& v, const void* d_list, int count, 
 }  // namespace
 
 namespace glb {
+int scale_check(int w, int h, const glava_b200_export_scale* s, glava_b200_export_scale* q, const char* who) {
+    if (!s) return fail(GLAVA_B200_EINVAL, "%s: null scale", who);
+    *q = *s;
+    if (!q->src_x && !q->src_y && !q->src_w && !q->src_h) { q->src_w = w; q->src_h = h; }
+    if (q->src_x < 0 || q->src_y < 0 || q->src_w < 1 || q->src_h < 1 || (int64_t) q->src_x + q->src_w > w ||
+        (int64_t) q->src_y + q->src_h > h)
+        return fail(GLAVA_B200_EINVAL, "%s: source rectangle (%d, %d) %dx%d is empty or leaves the %dx%d frame", who, q->src_x,
+                    q->src_y, q->src_w, q->src_h, w, h);
+    if (q->out_w < 1 || q->out_h < 1 || q->out_w > q->src_w || q->out_h > q->src_h)
+        return fail(GLAVA_B200_EINVAL, "%s: output %dx%d must be at least 1x1 and at most the %dx%d source (no upscaling)", who,
+                    q->out_w, q->out_h, q->src_w, q->src_h);
+    return 0;
+}
+
 // a destination pointer: null, alignment, device memory, device (export_list.h)
 int dst_check(const RendererView& v, const void* p, const char* name, int i, const char* who) {
     if (!p || ((uintptr_t) p & 15))

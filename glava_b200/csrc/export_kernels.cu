@@ -2031,4 +2031,99 @@ static void launch_planes_fade(const OverlayPlanesArgs& a, const ExportGrid& g, 
     });
 }
 
+// ---- glava_b200_overlay_scaled (DESIGN 4.21) ---------------------------------------------------------------------------------
+// The overlay of a downscaled, cropped frame.  Items are export_scaled_kernel's: (entry, output row — 4:2:0: row pair —, run
+// of 32 output columns), one warp each, lane = output column, every pixel scaled_px's exact area average with its mark-aware
+// footprint reads (native: of the stored pixels, zc 0; any other opacity: of the pixels made opaque, zc opaque black).  Each
+// pixel is scaled by the entry's K through fade_px / fade_opaque (K = 255 is the identity, so there is no separate plain
+// kernel), lanes past out_w hold zero, and the quad at X = 0 mod 4 is gathered by __shfl_down_sync into the lane that owns
+// it, which runs the format's native body: overlay_rgba for RGBA / BGRA, OverlayPlanesBody's row / pair otherwise.  The
+// bodies read the rectangle's width from their argument struct, so they get a view whose w is out_w.  An all-zero quad
+// under native opacity is neither loaded from the picture nor stored.
+template <typename Index, int Fmt, int E>
+__global__ void __launch_bounds__(256) overlay_scaled_kernel(const __grid_constant__ OverlayScaledArgs a) {
+    using Body = OverlayPlanesBody<Fmt, E>;
+    constexpr bool rgba = Fmt == GLAVA_B200_EXPORT_RGBA;    // RGBA and BGRA (a.format says which)
+    OverlayPlanesArgs view = {};                            // what the body reads: the rectangle's width and the pitches
+    view.w = a.out_w; view.h = a.out_h; view.format = Fmt; view.native = 1;
+    view.pitch = a.pitch; view.chroma_pitch = a.chroma_pitch;
+    const Body body(view);
+    const bool bgra = a.format == GLAVA_B200_EXPORT_BGRA;
+    const ExportFmt f = { a.format, a.native ? 0 : 1, a.native, 0u };
+    const ExportRecip rcp = { a.div_mul, a.div_shift };
+    const uint32_t zc = a.native ? 0u : export_over(0u, 0u, 0);   // what a zero pixel becomes
+    const Index runs = (Index) ((a.out_w + 31) >> 5), per = runs * (Index) (Body::k420 ? a.out_h >> 1 : a.out_h);
+    const Index items = (Index) a.count * per;
+    const Index warps = (Index) (((size_t) gridDim.x * blockDim.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    for (Index it = (Index) (((size_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5); it < items; it += warps) {
+        const Index k = it / per, rem = it - k * per;
+        const int u = (int) (rem / runs), X = (int) (rem - (Index) u * runs) * 32 + lane;
+        const bool active = X < a.out_w;
+        const OverlayPlanesEntry* e = a.list + k;
+        const int slot = __ldg(&e->slot);
+        const uint32_t K = (uint32_t) __ldg(&e->pad);
+        const uint32_t* frame = reinterpret_cast<const uint32_t*>(a.fb) + (size_t) slot * a.h * a.w;
+        const ExportSpan sx = export_span(active ? X : 0, a.src_w, a.out_w);
+        uint8_t* const dst = Body::dst(e);
+        if constexpr (Body::k420) {
+            uint32_t top = scaled_px<false>(a, f, frame, slot, 2 * u, active, sx, rcp, zc);
+            uint32_t bot = scaled_px<false>(a, f, frame, slot, 2 * u + 1, active, sx, rcp, zc);
+            top = !active ? 0u : a.native ? fade_px(top, K) : fade_opaque(top, K);
+            bot = !active ? 0u : a.native ? fade_px(bot, K) : fade_opaque(bot, K);
+            uint32_t t[4] = { top, 0u, 0u, 0u }, b[4] = { bot, 0u, 0u, 0u };
+#pragma unroll
+            for (int i = 1; i < 4; ++i) {
+                t[i] = __shfl_down_sync(0xffffffffu, top, i);
+                b[i] = __shfl_down_sync(0xffffffffu, bot, i);
+            }
+            if ((lane & 3) || !active) continue;
+            body.pair(dst, body.chroma(e), u, X, t, b);
+        } else {
+            uint32_t px = scaled_px<false>(a, f, frame, slot, u, active, sx, rcp, zc);
+            px = !active ? 0u : a.native ? fade_px(px, K) : fade_opaque(px, K);
+            uint32_t q[4] = { px, 0u, 0u, 0u };
+#pragma unroll
+            for (int i = 1; i < 4; ++i) q[i] = __shfl_down_sync(0xffffffffu, px, i);
+            if ((lane & 3) || !active) continue;
+            if constexpr (rgba) overlay_rgba(dst + (size_t) u * a.pitch, X, a.out_w, bgra, q);
+            else body.row(e, dst, u, X, q);
+        }
+    }
+}
+
+template <int Fmt>
+static void launch_scaled_overlay(const OverlayScaledArgs& a, const ExportGrid& g, cudaStream_t st) {
+    for_any_enc(a.enc, [&](auto e) {
+        constexpr int E = decltype(e)::value;
+        if (g.narrow) overlay_scaled_kernel<uint32_t, Fmt, E><<<g.blocks, 256, 0, st>>>(a);
+        else overlay_scaled_kernel<uint64_t, Fmt, E><<<g.blocks, 256, 0, st>>>(a);
+    });
+}
+
+int launch_overlay_scaled(const OverlayScaledArgs& a, void* stream) {
+    const bool pairs = export_420(a.format);
+    const ExportGrid g = export_grid((uint64_t) a.count * (uint64_t) ((a.out_w + 31) >> 5) *
+                                     (uint64_t) (pairs ? a.out_h >> 1 : a.out_h));
+    cudaStream_t st = (cudaStream_t) stream;
+    switch (a.format) {
+    case GLAVA_B200_EXPORT_RGBA:
+    case GLAVA_B200_EXPORT_BGRA:
+        if (g.narrow) overlay_scaled_kernel<uint32_t, GLAVA_B200_EXPORT_RGBA, 0><<<g.blocks, 256, 0, st>>>(a);
+        else overlay_scaled_kernel<uint64_t, GLAVA_B200_EXPORT_RGBA, 0><<<g.blocks, 256, 0, st>>>(a);
+        break;
+    case GLAVA_B200_EXPORT_NV12: launch_scaled_overlay<GLAVA_B200_EXPORT_NV12>(a, g, st); break;
+    case GLAVA_B200_EXPORT_I420: launch_scaled_overlay<GLAVA_B200_EXPORT_I420>(a, g, st); break;
+    case GLAVA_B200_EXPORT_YUV444: launch_scaled_overlay<GLAVA_B200_EXPORT_YUV444>(a, g, st); break;
+    case GLAVA_B200_EXPORT_P010: launch_scaled_overlay<GLAVA_B200_EXPORT_P010>(a, g, st); break;
+    case GLAVA_B200_EXPORT_YUV420P10: launch_scaled_overlay<GLAVA_B200_EXPORT_YUV420P10>(a, g, st); break;
+    case GLAVA_B200_EXPORT_YUV444P10: launch_scaled_overlay<GLAVA_B200_EXPORT_YUV444P10>(a, g, st); break;
+    case GLAVA_B200_EXPORT_YUV422P: launch_scaled_overlay<GLAVA_B200_EXPORT_YUV422P>(a, g, st); break;
+    case GLAVA_B200_EXPORT_YUV422P10: launch_scaled_overlay<GLAVA_B200_EXPORT_YUV422P10>(a, g, st); break;
+    case GLAVA_B200_EXPORT_UYVY: launch_scaled_overlay<GLAVA_B200_EXPORT_UYVY>(a, g, st); break;
+    default: return fail(GLAVA_B200_EINVAL, "scaled overlay launch: format %d", a.format);
+    }
+    return launch_status("scaled overlay");
+}
+
 }  // namespace glb

@@ -32,6 +32,12 @@ struct ExportList {
 // room for `bytes` of list (the buffers are replaced only once the raster stream has drained); *out: the renderer's list
 int list_room(const RendererView& v, size_t bytes, ExportList** out);
 
+// overlay_planes.cpp: the list of an overlay onto pictures (overlay_planes, DESIGN 4.17; overlay_scaled, 4.21) in the pinned
+// buffer h[cur] of the renderer's list: one OverlayPlanesEntry (plane pointers, slot) per entry whose K is not 0, K in its pad
+// word; k null: every entry, pad `pad`.  *bytes: the list's size.
+int planes_list(const RendererView& v, const int* streams, int count, const glava_b200_picture* pics, const uint8_t* k, int pad,
+                ExportList** L, size_t* bytes);
+
 // the background of a descriptor as 0x00BBGGRR
 uint32_t background(const glava_b200_export& d);
 

@@ -277,6 +277,25 @@ struct OverlayPlanesArgs {
 };
 // overlay_planes_kernel (fade: overlay_planes_fade_kernel), instantiated per format, encoding, item kind and index width
 int launch_overlay_planes(const OverlayPlanesArgs& a, void* stream);
+// export_kernels.cu: glava_b200_overlay_scaled (DESIGN 4.21), one launch for the whole list: each entry's out_w x out_h
+// rectangle gets export_scaled's pixel of the source rectangle (native: the premultiplied average; any other opacity: of
+// opaque pixels), scaled by the entry's K (pad) and blended by the format's native body.  Entries as overlay_planes'
+// (RGBA / BGRA: plane[0] only); w, h, marks and mark_rows describe the framebuffer as ScaledArgs' do.
+struct OverlayScaledArgs {
+    const uint8_t*  fb;         // [slots][h][w] RGBA8
+    const uint32_t* marks;      // as ExportArgs
+    int             mark_rows;
+    const OverlayPlanesEntry* list;
+    int    count, w, h;
+    int    format, native;      // format: RGBA, BGRA or one of overlay_planes'
+    size_t pitch, chroma_pitch;    // as OverlayPlanesArgs (RGBA / BGRA: chroma_pitch 0)
+    int    src_x, src_y, src_w, src_h, out_w, out_h;   // as ScaledArgs
+    uint64_t div_mul;
+    int    div_shift;
+    int    enc;                 // as ExportArgs
+};
+// overlay_scaled_kernel, instantiated per format (RGBA and BGRA share one), encoding and index width
+int launch_overlay_scaled(const OverlayScaledArgs& a, void* stream);
 // export_kernels.cu: glava_b200_export_ladder (DESIGN 4.13), one launch for every rung of every entry.  Per rung what a
 // standalone call would take: the whole frame at its own size (whole = 1) runs export_kernel's items, every other rung
 // export_scaled_kernel's; z*: what a zero pixel becomes under the rung's format (export_core.h, filled on the host).
@@ -351,16 +370,30 @@ int overlay_geometry_check(int w, int h, int count, void* const* dst, void* cons
 // flags, even 4:2:0 sizes, both pitches) and the planes' shapes; planes_check: every refusal that depends on this renderer
 // alone (the overlap and framebuffer tests are planes_geometry_check's, over rectangles each with its own pitch P and row
 // bytes B); planes_run: the call on one renderer.
+// The scaled overlay (glava_b200_overlay_scaled, DESIGN 4.21) passes `q`, its rectangle with the defaults applied: the
+// descriptor is then checked against q->out_w x q->out_h, and RGBA / BGRA are one plane of 4 bytes per pixel (chroma_pitch 0).
 struct PlanesGeom { int planes; size_t luma_row, chroma_row; int chroma_rows; };
 struct PlaneRect { uintptr_t p; size_t rows, P, B; int entry, plane; };
-int planes_geometry(int w, int h, const glava_b200_overlay_planes_desc& d, PlanesGeom* g, const char* who);
+int planes_geometry(int w, int h, const glava_b200_overlay_planes_desc& d, PlanesGeom* g, const char* who, bool rgba = false);
 int planes_check(glava_b200* r, const int* streams, int count, const glava_b200_picture* pics,
-                 const glava_b200_overlay_planes_desc* desc, const char* who);
+                 const glava_b200_overlay_planes_desc* desc, const char* who, const glava_b200_export_scale* q = nullptr);
 bool plane_rects_meet(const PlaneRect& a, const PlaneRect& b);
 int planes_geometry_check(int w, int h, int count, const glava_b200_picture* pics, const glava_b200_overlay_planes_desc& desc,
-                          const uint8_t* const* fb, const size_t* fb_bytes, int nfb, const char* who);
+                          const uint8_t* const* fb, const size_t* fb_bytes, int nfb, const char* who, bool rgba = false);
 int planes_run(glava_b200* r, const int* streams, int count, const glava_b200_picture* pics, const glava_b200_overlay_planes_desc* desc,
                void* after_event, void* done_event, const char* who, const uint8_t* opacity = nullptr);
+// export.cpp: the scale rectangle of export_scaled against a w x h frame (null, empty or leaving the frame, upscaling); *q
+// receives it with the whole-frame default applied
+int scale_check(int w, int h, const glava_b200_export_scale* s, glava_b200_export_scale* q, const char* who);
+// overlay_scaled.cpp, glava_b200_overlay_scaled (DESIGN 4.21): the call on one renderer.  The whole frame at its own size runs
+// export_run's / planes_run's overlay (its plain or fade kernel); any other rectangle overlay_scaled_kernel.
+int scaled_overlay_run(glava_b200* r, const int* streams, int count, const glava_b200_picture* pics,
+                       const glava_b200_overlay_planes_desc* desc, const glava_b200_export_scale* scale, const uint8_t* opacity,
+                       void* after_event, void* done_event, const char* who);
+// the scaled overlay's checks that depend on one renderer alone (*q: the rectangle with its defaults applied)
+int scaled_overlay_check(glava_b200* r, const int* streams, int count, const glava_b200_picture* pics,
+                         const glava_b200_overlay_planes_desc* desc, const glava_b200_export_scale* scale,
+                         glava_b200_export_scale* q, const char* who);
 // capi.cu, for sharded.cpp: the blob checks of glava_b200_load_streams (nothing is touched), and save / load with one
 // host pointer per listed stream (the blobs of one shard's streams are not contiguous in the caller's array)
 int state_check_blobs(const glava_b200* r, const void* const* blobs, int count, const char* who);

@@ -27,6 +27,8 @@ const char* planes_format_name(int format) {
     case GLAVA_B200_EXPORT_YUV422P: return "YUV422P";
     case GLAVA_B200_EXPORT_YUV422P10: return "YUV422P10";
     case GLAVA_B200_EXPORT_UYVY: return "UYVY";
+    case GLAVA_B200_EXPORT_RGBA: return "RGBA";             // the scaled overlay's (DESIGN 4.21)
+    case GLAVA_B200_EXPORT_BGRA: return "BGRA";
     default: return nullptr;
     }
 }
@@ -36,9 +38,10 @@ const char* plane_name(int planes, int p) { return p == 0 ? "Y" : p == 2 ? "Cr" 
 
 }  // namespace
 
-int planes_geometry(int w, int h, const glava_b200_overlay_planes_desc& d, PlanesGeom* g, const char* who) {
+int planes_geometry(int w, int h, const glava_b200_overlay_planes_desc& d, PlanesGeom* g, const char* who, bool rgba) {
     const int fmt = d.format;
-    if (fmt == GLAVA_B200_EXPORT_RGBA || fmt == GLAVA_B200_EXPORT_BGRA)
+    const bool packed = fmt == GLAVA_B200_EXPORT_RGBA || fmt == GLAVA_B200_EXPORT_BGRA;
+    if (packed && !rgba)
         return fail(GLAVA_B200_EINVAL, "%s: format %s: RGBA and BGRA images go to glava_b200_overlay_frames", who,
                     fmt == GLAVA_B200_EXPORT_RGBA ? "RGBA" : "BGRA");
     if (export_yuva(fmt))                                   // DESIGN 4.19: a transparent layer is exported, not blended onto
@@ -51,14 +54,17 @@ int planes_geometry(int w, int h, const glava_b200_overlay_planes_desc& d, Plane
         return fail(GLAVA_B200_EINVAL, "%s: flags 0x%x: EXPORT_STRAIGHT is for the exports; the overlay composites", who, d.flags);
     if (d.flags & ~colour)
         return fail(GLAVA_B200_EINVAL, "%s: flags 0x%x: the overlay takes none but EXPORT_FULL_RANGE and EXPORT_BT601", who, d.flags);
-    const bool c420 = export_420(fmt), uyvy = fmt == GLAVA_B200_EXPORT_UYVY;
+    if (packed && (d.flags & colour))
+        return fail(GLAVA_B200_EINVAL, "%s: flags 0x%x: %s has no matrix or range (EXPORT_FULL_RANGE and EXPORT_BT601 are for the "
+                    "Y'CbCr formats)", who, d.flags, name);
+    const bool c420 = export_420(fmt), uyvy = fmt == GLAVA_B200_EXPORT_UYVY || packed;   // RGBA / BGRA: one plane, as UYVY
     const bool wide = fmt == GLAVA_B200_EXPORT_P010 || export_p10(fmt) || fmt == GLAVA_B200_EXPORT_YUV422P10 || uyvy;
     if (c420 && ((w | h) & 1))
         return fail(GLAVA_B200_EINVAL, "%s: %s needs an even width and height, the frame is %dx%d", who, name, w, h);
     if (export_422(fmt) && (w & 1))
         return fail(GLAVA_B200_EINVAL, "%s: %s needs an even width, the frame is %dx%d", who, name, w, h);
     g->planes = uyvy ? 1 : export_planar(fmt) ? 3 : 2;
-    g->luma_row = (size_t) w * (wide ? 2 : 1);                // UYVY: its one plane, 2 bytes per pixel
+    g->luma_row = (size_t) w * (packed ? 4 : wide ? 2 : 1);   // UYVY: its one plane, 2 bytes per pixel
     g->chroma_row = fmt == GLAVA_B200_EXPORT_I420 || fmt == GLAVA_B200_EXPORT_YUV422P ? (size_t) w / 2
                     : fmt == GLAVA_B200_EXPORT_P010 || fmt == GLAVA_B200_EXPORT_YUV444P10 ? (size_t) w * 2
                     : uyvy ? 0 : (size_t) w;
@@ -67,7 +73,7 @@ int planes_geometry(int w, int h, const glava_b200_overlay_planes_desc& d, Plane
         return fail(GLAVA_B200_EINVAL, "%s: pitch %zu must be a multiple of 16 and at least %zu", who, d.pitch, g->luma_row);
     if (uyvy) {
         if (d.chroma_pitch)
-            return fail(GLAVA_B200_EINVAL, "%s: UYVY chroma_pitch %zu must be 0: UYVY has no chroma plane", who, d.chroma_pitch);
+            return fail(GLAVA_B200_EINVAL, "%s: %s chroma_pitch %zu must be 0: %s has no chroma plane", who, name, d.chroma_pitch, name);
         return 0;
     }
     if (d.chroma_pitch % 16 || d.chroma_pitch < g->chroma_row)
@@ -77,11 +83,11 @@ int planes_geometry(int w, int h, const glava_b200_overlay_planes_desc& d, Plane
 }
 
 int planes_check(glava_b200* r, const int* streams, int count, const glava_b200_picture* pics,
-                 const glava_b200_overlay_planes_desc* desc, const char* who) {
+                 const glava_b200_overlay_planes_desc* desc, const char* who, const glava_b200_export_scale* q) {
     const RendererView v = renderer_view(r);
     if (!v.built) return fail(GLAVA_B200_EINVAL, "%s: the renderer has no tables: a reconfigure or resize failed and must be repeated", who);
     PlanesGeom g;
-    int rc = planes_geometry(v.w, v.h, *desc, &g, who);
+    int rc = q ? planes_geometry(q->out_w, q->out_h, *desc, &g, who, true) : planes_geometry(v.w, v.h, *desc, &g, who);
     if (rc) return rc;
     if (count < 1) return fail(GLAVA_B200_EINVAL, "%s: count %d < 1", who, count);
     if (!streams || !pics) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
@@ -97,8 +103,8 @@ int planes_check(glava_b200* r, const int* streams, int count, const glava_b200_
             return fail(GLAVA_B200_EINVAL, "%s: pics[%d].plane[2] must be NULL: %s has one interleaved chroma plane", who, i,
                         planes_format_name(desc->format));
         if (g.planes == 1 && (pics[i].plane[1] || pics[i].plane[2]))
-            return fail(GLAVA_B200_EINVAL, "%s: pics[%d].plane[%d] must be NULL: UYVY has one packed plane", who, i,
-                        pics[i].plane[1] ? 1 : 2);
+            return fail(GLAVA_B200_EINVAL, "%s: pics[%d].plane[%d] must be NULL: %s has one packed plane", who, i,
+                        pics[i].plane[1] ? 1 : 2, planes_format_name(desc->format));
     }
     return 0;
 }
@@ -116,9 +122,9 @@ bool plane_rects_meet(const PlaneRect& a, const PlaneRect& b) {
 }
 
 int planes_geometry_check(int w, int h, int count, const glava_b200_picture* pics, const glava_b200_overlay_planes_desc& desc,
-                          const uint8_t* const* fb, const size_t* fb_bytes, int nfb, const char* who) {
+                          const uint8_t* const* fb, const size_t* fb_bytes, int nfb, const char* who, bool rgba) {
     PlanesGeom g;
-    int rc = planes_geometry(w, h, desc, &g, who);
+    int rc = planes_geometry(w, h, desc, &g, who, rgba);
     if (rc) return rc;
     std::vector<PlaneRect> rs;
     rs.reserve((size_t) count * (size_t) g.planes);
@@ -150,6 +156,22 @@ int planes_geometry_check(int w, int h, int count, const glava_b200_picture* pic
     return 0;
 }
 
+int planes_list(const RendererView& v, const int* streams, int count, const glava_b200_picture* pics, const uint8_t* k, int pad,
+                ExportList** L, size_t* bytes) {
+    int n = 0;
+    for (int i = 0; i < count; ++i) n += !k || k[i] ? 1 : 0;
+    *bytes = (size_t) n * sizeof(OverlayPlanesEntry);
+    int rc;
+    if ((rc = list_room(v, *bytes, L)) != 0) return rc;
+    CU(cudaEventSynchronize((*L)->ev[(*L)->cur]));          // the copy that last read h[cur] (four calls ago)
+    OverlayPlanesEntry* const host = reinterpret_cast<OverlayPlanesEntry*>((uint8_t*) (*L)->h[(*L)->cur]);
+    for (int i = 0, j = 0; i < count; ++i)
+        if (!k || k[i])
+            host[j++] = { { (uint8_t*) pics[i].plane[0], (uint8_t*) pics[i].plane[1], (uint8_t*) pics[i].plane[2] }, streams[i] % v.slots,
+                          k ? k[i] : pad };
+    return 0;
+}
+
 // On the handle's stream, where readback copies: after the latest raster pass, before the next one can overwrite a slot
 int planes_run(glava_b200* r, const int* streams, int count, const glava_b200_picture* pics, const glava_b200_overlay_planes_desc* desc,
                void* after_event, void* done_event, const char* who, const uint8_t* opacity) {
@@ -163,18 +185,10 @@ int planes_run(glava_b200* r, const int* streams, int count, const glava_b200_pi
     CU(cudaSetDevice(v.device));
     // opacity (DESIGN 4.20) as overlay_frames': the fade kernel unless every K is 255, K = 0 entries left out of the list
     const bool fade = opacity_fades(opacity, count);
-    int n = 0;
-    for (int i = 0; i < count; ++i) n += !fade || opacity[i] ? 1 : 0;
-    const size_t bytes = (size_t) n * sizeof(OverlayPlanesEntry);
     ExportList* L = nullptr;
-    if ((rc = list_room(v, bytes, &L)) != 0) return rc;
-    CU(cudaEventSynchronize(L->ev[L->cur]));                // the copy that last read h[cur] (four calls ago)
-    OverlayPlanesEntry* const host = reinterpret_cast<OverlayPlanesEntry*>((uint8_t*) L->h[L->cur]);
-    for (int i = 0, k = 0; i < count; ++i)
-        if (!fade || opacity[i])
-            host[k++] = { { (uint8_t*) pics[i].plane[0], (uint8_t*) pics[i].plane[1], (uint8_t*) pics[i].plane[2] }, streams[i] % v.slots,
-                          fade ? opacity[i] : 0 };
-    count = n;
+    size_t bytes = 0;
+    if ((rc = planes_list(v, streams, count, pics, fade ? opacity : nullptr, 0, &L, &bytes)) != 0) return rc;
+    count = (int) (bytes / sizeof(OverlayPlanesEntry));
     return list_enqueue(v, L, bytes, after_event, done_event, [&](const void* d_list) {
         OverlayPlanesArgs a = {};
         a.fb = v.fb;

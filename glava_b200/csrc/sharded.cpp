@@ -392,9 +392,10 @@ int glava_b200_sharded_export_ladder(glava_b200_sharded* g, const int* streams, 
 
 // glava_b200_overlay_planes with global stream indices: the list split by shard (pics[i] and opacity[i] travelling with
 // streams[i]), every shard's part checked as one renderer, then the whole list's overlap and every shard's framebuffer, before
-// any shard starts
+// any shard starts.  scale non-null: glava_b200_overlay_scaled's (DESIGN 4.21), the rectangles out_w x out_h.
 static int sharded_planes(glava_b200_sharded* g, const int* streams, int count, const glava_b200_picture* pics,
-                          const glava_b200_overlay_planes_desc* desc, const uint8_t* opacity, const char* who) {
+                          const glava_b200_overlay_planes_desc* desc, const uint8_t* opacity, const char* who,
+                          const glava_b200_export_scale* scale = nullptr) {
     clear_error();
     if (!g || !desc) return fail(GLAVA_B200_EINVAL, "%s: null argument", who);
     if (count < 1) return fail(GLAVA_B200_EINVAL, "%s: count %d < 1", who, count);
@@ -417,19 +418,26 @@ static int sharded_planes(glava_b200_sharded* g, const int* streams, int count, 
     }
     std::vector<const uint8_t*> fb;
     std::vector<size_t> fb_bytes;
+    const RendererView v0 = renderer_view(g->shards[0]->r);
+    glava_b200_export_scale q = { 0, 0, v0.w, v0.h, v0.w, v0.h };   // every shard has the same frame size
     for (size_t k = 0; k < g->shards.size(); ++k) {
         const RendererView v = renderer_view(g->shards[k]->r);
         fb.push_back(v.fb); fb_bytes.push_back((size_t) v.slots * (size_t) v.h * (size_t) v.w * 4);
         if (idx[k].empty()) continue;
-        const int rc = planes_check(g->shards[k]->r, idx[k].data(), (int) idx[k].size(), part[k].data(), desc, who);
+        const int rc = scale ? scaled_overlay_check(g->shards[k]->r, idx[k].data(), (int) idx[k].size(), part[k].data(), desc, scale,
+                                                    &q, who)
+                             : planes_check(g->shards[k]->r, idx[k].data(), (int) idx[k].size(), part[k].data(), desc, who);
         if (rc) return rc;
     }
-    const RendererView v0 = renderer_view(g->shards[0]->r);
-    const int rc = planes_geometry_check(v0.w, v0.h, count, pics, *desc, fb.data(), fb_bytes.data(), (int) fb.size(), who);
+    const int rc = planes_geometry_check(q.out_w, q.out_h, count, pics, *desc, fb.data(), fb_bytes.data(), (int) fb.size(), who,
+                                         scale != nullptr);
     if (rc) return rc;
     return broadcast(g, [&](Shard& s) {
         const size_t k = (size_t) (std::find(g->shards.begin(), g->shards.end(), &s) - g->shards.begin());
         if (idx[k].empty()) return 0;
+        if (scale)
+            return scaled_overlay_run(s.r, idx[k].data(), (int) idx[k].size(), part[k].data(), desc, scale,
+                                      opacity ? op[k].data() : nullptr, nullptr, nullptr, who);
         return planes_run(s.r, idx[k].data(), (int) idx[k].size(), part[k].data(), desc, nullptr, nullptr, who,
                           opacity ? op[k].data() : nullptr);
     });
@@ -441,6 +449,15 @@ int glava_b200_sharded_overlay_planes(glava_b200_sharded* g, const int* streams,
 int glava_b200_sharded_overlay_planes_opacity(glava_b200_sharded* g, const int* streams, int count, const glava_b200_picture* pics,
                                               const glava_b200_overlay_planes_desc* desc, const uint8_t* opacity) {
     return sharded_planes(g, streams, count, pics, desc, opacity, "glava_b200_sharded_overlay_planes_opacity");
+}
+int glava_b200_sharded_overlay_scaled(glava_b200_sharded* g, const int* streams, int count, const glava_b200_picture* pics,
+                                      const glava_b200_overlay_planes_desc* desc, const glava_b200_export_scale* scale,
+                                      const uint8_t* opacity) {
+    if (!scale) {                                           // refused here: sharded_planes reads null as overlay_planes
+        clear_error();
+        return fail(GLAVA_B200_EINVAL, "glava_b200_sharded_overlay_scaled: null scale");
+    }
+    return sharded_planes(g, streams, count, pics, desc, opacity, "glava_b200_sharded_overlay_scaled", scale);
 }
 
 int glava_b200_sharded_textures(glava_b200_sharded* g, uint16_t* out_l, uint16_t* out_r) {

@@ -635,6 +635,34 @@ int glava_b200_overlay_planes_opacity(glava_b200* r, const int* streams, int cou
                                       const glava_b200_overlay_planes_desc* desc, const uint8_t* opacity /* [count], NULL = all 255 */,
                                       void* after_event, void* done_event);
 
+/* Overlay a downscaled, cropped frame (DESIGN.md §4.21), for picture-in-picture and for the same visualiser on every rendition
+ * of an overlaid video:
+ *   glava_b200_overlay_scaled  streams, pics and desc as glava_b200_overlay_planes, with the formats RGBA and BGRA added (only
+ *                              plane[0], chroma_pitch 0, flags 0); scale as glava_b200_export_scaled (a source rectangle, top-down,
+ *                              all zero = the whole frame; out_w x out_h, downscale only); opacity as
+ *                              glava_b200_overlay_planes_opacity; after_event / done_event as glava_b200_export_frames.
+ *   The rectangle in pics[i] is out_w x out_h.  Entry i leaves there exactly what glava_b200_overlay_planes_opacity (RGBA /
+ *   BGRA: glava_b200_overlay_frames_opacity) would leave with opacity[i] if the stream's frame were S_i, the out_w x out_h
+ *   RGBA image glava_b200_export_scaled of streams[i] with this scale writes at this point in call order: under setopacity
+ *   "native" with flags 0 (the premultiplied exact area average), under any other opacity with EXPORT_OVER (each pixel made
+ *   opaque before the average).  Ordered on the raster stream as the other overlays; streams may repeat.  Hence, bit for bit:
+ *   the whole frame at its own size is glava_b200_overlay_planes_opacity / _overlay_frames_opacity (whose kernels it runs);
+ *   under any other opacity at K = 255 the rectangle holds glava_b200_export_scaled's bytes of the format and encoding
+ *   (RGBA / BGRA: with EXPORT_OVER); a frame of zero pixels under native opacity, and K = 0 in any mode, leave the picture
+ *   untouched (an all-zero quad of S_i is neither read nor written, and a 10-bit sample no non-zero pixel covers keeps all
+ *   16 bits).  K = 0 entries are left out of the device list; a list of only those enqueues no kernel, but the stream
+ *   still waits for after_event and records done_event.
+ *   GLAVA_B200_EINVAL, with nothing enqueued and the message naming the call, for: every refusal of glava_b200_overlay_planes
+ *   measured against out_w x out_h (parity, pitches, plane pointers, stream range, count, an unbuilt renderer, overlap with
+ *   the framebuffer array or between any two plane rectangles of the call); a null scale, a source rectangle that is empty or
+ *   leaves the frame, an output larger than the source; EXPORT_STRAIGHT, EXPORT_OVER or any other flag (RGBA / BGRA: any
+ *   flag), the YUVA formats; for RGBA / BGRA a non-null plane[1] or plane[2] or a non-zero chroma_pitch.
+ *   glava_b200_sharded_overlay_scaled  the same with global stream indices, each picture on the device of the shard that
+ *                              owns streams[i]; every entry and the overlap of the whole list are checked before any shard starts. */
+int glava_b200_overlay_scaled(glava_b200* r, const int* streams, int count, const glava_b200_picture* pics,
+                              const glava_b200_overlay_planes_desc* desc, const glava_b200_export_scale* scale,
+                              const uint8_t* opacity /* [count], NULL = all 255 */, void* after_event, void* done_event);
+
 /* ---- one handle for a batch spread over several GPUs of a node (csrc/sharded.cpp) -------------------------------------
  * The streams of a batch are independent (one GLava process each, in the reference), so the batch is cut into contiguous
  * blocks, one per device — glava_b200_shard_range: counts differ by at most one — and nothing crosses between devices (no
@@ -674,6 +702,9 @@ int  glava_b200_sharded_overlay_frames_opacity(glava_b200_sharded* s, const int*
 int  glava_b200_sharded_overlay_planes_opacity(glava_b200_sharded* s, const int* streams, int count, const glava_b200_picture* pics,
                                                const glava_b200_overlay_planes_desc* desc,
                                                const uint8_t* opacity);   /* see glava_b200_overlay_planes_opacity */
+int  glava_b200_sharded_overlay_scaled(glava_b200_sharded* s, const int* streams, int count, const glava_b200_picture* pics,
+                                       const glava_b200_overlay_planes_desc* desc, const glava_b200_export_scale* scale,
+                                       const uint8_t* opacity);   /* see glava_b200_overlay_scaled */
 int  glava_b200_sharded_export_ladder(glava_b200_sharded* s, const int* streams, int count,
                                       const glava_b200_export_rung* rungs, int nrungs, void* const* dst,
                                       void* const* dst_uv);   /* global indices; see glava_b200_export_ladder */
