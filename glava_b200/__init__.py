@@ -18,7 +18,7 @@ from .api import (Params, Color, Renderer, GlavaError, default_params, load_conf
                   Export, ExportScale, ExportRung, LADDER_MAX, EXPORT_RGBA, EXPORT_BGRA, EXPORT_NV12, EXPORT_I420,
                   EXPORT_YUV444, EXPORT_P010, EXPORT_YUV420P10, EXPORT_YUV444P10, EXPORT_YUV422P, EXPORT_YUV422P10,
                   EXPORT_UYVY, EXPORT_YUVA420P, EXPORT_YUVA444P10, EXPORT_OVER, EXPORT_STRAIGHT, EXPORT_FULL_RANGE,
-                  EXPORT_BT601, Picture, OverlayPlanesDesc, PLANES_FORMATS)
+                  EXPORT_BT601, EXPORT_PQ, EXPORT_HLG, Picture, OverlayPlanesDesc, PLANES_FORMATS)
 from . import audio
 from .synth import synth_pcm_int16, fifo_to_float, StreamRings
 
@@ -28,6 +28,6 @@ __all__ = ["audio", "Params", "Color", "Renderer", "GlavaError", "default_params
            "Export", "ExportScale", "ExportRung", "LADDER_MAX", "EXPORT_RGBA", "EXPORT_BGRA", "EXPORT_NV12", "EXPORT_I420",
            "EXPORT_YUV444", "EXPORT_P010", "EXPORT_YUV420P10", "EXPORT_YUV444P10", "EXPORT_YUV422P",
            "EXPORT_YUV422P10", "EXPORT_UYVY", "EXPORT_YUVA420P", "EXPORT_YUVA444P10", "EXPORT_OVER", "EXPORT_STRAIGHT",
-           "EXPORT_FULL_RANGE", "EXPORT_BT601",
+           "EXPORT_FULL_RANGE", "EXPORT_BT601", "EXPORT_PQ", "EXPORT_HLG",
            "Picture", "OverlayPlanesDesc", "PLANES_FORMATS", "synth_pcm_int16",
            "fifo_to_float", "StreamRings"]

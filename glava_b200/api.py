@@ -153,6 +153,24 @@ EXPORT_OVER = 1
 EXPORT_STRAIGHT = 4                                     # RGBA / BGRA with straight (unassociated) alpha (DESIGN 4.19)
 EXPORT_FULL_RANGE, EXPORT_BT601 = 0x100, 0x200          # the Y'CbCr encoding (DESIGN 4.15); neither: BT.709 limited range
 EXPORT_MATRICES = {"bt709": 0, "bt601": EXPORT_BT601}
+EXPORT_PQ, EXPORT_HLG = 0x800, 0x1000                   # BT.2020 HDR, limited range, 10-bit formats only (DESIGN 4.22)
+EXPORT_TRANSFERS = {"pq": EXPORT_PQ, "hlg": EXPORT_HLG}
+
+
+def _colour_flags(matrix="bt709", full_range=False, transfer=None):
+    """The colour flags of a Y'CbCr encoding: matrix "bt709" / "bt601" with full_range (DESIGN 4.15), or matrix "bt2020"
+    with transfer "pq" / "hlg" (DESIGN 4.22: BT.2020 limited range HDR, P010 / YUV420P10 / YUV444P10 / YUV422P10; other
+    formats reach the library's refusal).  Either of "bt2020" and transfer alone, and full_range with a transfer, raise
+    ValueError"""
+    if matrix == "bt2020" or transfer is not None:
+        if matrix != "bt2020" or transfer not in EXPORT_TRANSFERS:
+            raise ValueError(f"matrix {matrix!r}, transfer {transfer!r}: HDR is matrix='bt2020' with transfer 'pq' or 'hlg'")
+        if full_range:
+            raise ValueError(f"transfer {transfer!r}: HDR is limited range, full_range=True does not apply")
+        return EXPORT_TRANSFERS[transfer]
+    if matrix not in EXPORT_MATRICES:
+        raise ValueError(f"matrix {matrix!r}: one of {sorted(EXPORT_MATRICES) + ['bt2020']}")
+    return EXPORT_MATRICES[matrix] | (EXPORT_FULL_RANGE if full_range else 0)
 EXPORT_FORMATS = {"rgba": EXPORT_RGBA, "bgra": EXPORT_BGRA, "nv12": EXPORT_NV12, "i420": EXPORT_I420,
                   "yuv444": EXPORT_YUV444, "p010": EXPORT_P010, "yuv420p10": EXPORT_YUV420P10,
                   "yuv444p10": EXPORT_YUV444P10, "yuv422p": EXPORT_YUV422P, "yuv422p10": EXPORT_YUV422P10,
@@ -516,7 +534,7 @@ class _FrameExport:
     """export_frames over the handle's C entry point: destinations as torch tensors (DESIGN 4.10)"""
 
     def _export_plan(self, streams, fmt, over, background, out, device_of, size=None, matrix="bt709", full_range=False,
-                     straight=False):
+                     straight=False, transfer=None):
         """-> (stream list, Export, [dst pointers], what to return).  device_of(stream): the CUDA device of a stream's
         frame.  size: (w, h) of each output, None: the frame's.  out: None (allocate), one uint8 tensor [count, rows, ...]
         whose dim 1 steps by the pitch, or a list of count tensors [rows, ...] with one common pitch; rows as
@@ -530,7 +548,7 @@ class _FrameExport:
         devices = [device_of(int(x)) for x in s]
         p = self.params
         w, h = (p.w, p.h) if size is None else (int(size[0]), int(size[1]))
-        desc = _export_desc(fmt, over, background, matrix, full_range, straight)
+        desc = _export_desc(fmt, over, background, matrix, full_range, straight, transfer)
         rows, row_bytes, align = _export_layout(fmt, w, h)
         dtypes = (torch.uint8, torch.uint16) if fmt in WIDE_FORMATS else (torch.uint8,)
 
@@ -583,14 +601,15 @@ class _FrameExport:
         arr = (ExportRung * max(len(rungs), 1))()
         ptrs, results = [], []
         for j, (rung, o) in enumerate(zip(rungs, outs)):
-            unknown = set(rung) - {"size", "crop", "fmt", "over", "background", "matrix", "full_range", "straight"}
+            unknown = set(rung) - {"size", "crop", "fmt", "over", "background", "matrix", "full_range", "straight",
+                                   "transfer"}
             if unknown:
                 raise ValueError(f"rungs[{j}]: unknown keys {sorted(unknown)}")
             size = rung.get("size") or (p.w, p.h)
             _, desc, dst, result = self._export_plan(s, rung.get("fmt", "nv12"), rung.get("over", False),
                                                      rung.get("background", (0, 0, 0)), o, device_of, size,
                                                      rung.get("matrix", "bt709"), rung.get("full_range", False),
-                                                     rung.get("straight", False))
+                                                     rung.get("straight", False), rung.get("transfer"))
             arr[j].desc, arr[j].scale = desc, _export_scale(size, rung.get("crop"))
             ptrs.append(dst)
             results.append(result)
@@ -713,7 +732,7 @@ class _FrameExport:
         arr = (C.c_void_p * max(count, 1))(*dst)
         return s, desc, arr, (C.c_void_p * max(count, 1))(*uv) if nv12 else None
 
-    def _planes_plan(self, streams, pictures, at, fmt, matrix="bt709", full_range=False, size=None):
+    def _planes_plan(self, streams, pictures, at, fmt, matrix="bt709", full_range=False, size=None, transfer=None):
         """-> (stream list, OverlayPlanesDesc, Picture array) of an overlay onto decoded pictures (DESIGN 4.17).  pictures:
         one tuple of plane tensors per entry (a tuple may repeat), or one tuple of batched [count, rows, cols] plane tensors;
         a tuple is (Y, CbCr) for NV12 and P010, (Y, Cb, Cr) otherwise, each CUDA, uint8 (the 8-bit formats) or uint16 or
@@ -812,28 +831,24 @@ class _FrameExport:
             arr[i].plane = (C.c_void_p * 3)(*(ptrs + [None] * (3 - nplanes)))
         desc = OverlayPlanesDesc()
         desc.format = EXPORT_FORMATS[fmt]
-        if matrix not in EXPORT_MATRICES:
-            raise ValueError(f"matrix {matrix!r}: one of {sorted(EXPORT_MATRICES)}")
-        desc.flags = EXPORT_MATRICES[matrix] | (EXPORT_FULL_RANGE if full_range else 0)
+        desc.flags = _colour_flags(matrix, full_range, transfer)
         desc.pitch, desc.chroma_pitch = pitch or 0, cpitch or 0
         return s, desc, arr
 
 
-def _export_desc(fmt, over, background, matrix="bt709", full_range=False, straight=False):
+def _export_desc(fmt, over, background, matrix="bt709", full_range=False, straight=False, transfer=None):
     """the Export descriptor of a format name, the composite flag, an RGB(A) background (pitch and uv_offset 0), the
     Y'CbCr encoding: matrix "bt709" or "bt601", full_range (DESIGN 4.15; the defaults set no flag, and a matrix or range
-    on RGBA / BGRA reaches the library's refusal) and straight alpha (DESIGN 4.19; on a Y'CbCr format it reaches the
-    library's refusal)"""
+    on RGBA / BGRA reaches the library's refusal), or matrix "bt2020" with transfer "pq" / "hlg" (DESIGN 4.22), and straight
+    alpha (DESIGN 4.19; on a Y'CbCr format it reaches the library's refusal)"""
     if fmt not in EXPORT_FORMATS:
         raise ValueError(f"format {fmt!r}: one of {sorted(EXPORT_FORMATS)}")
-    if matrix not in EXPORT_MATRICES:
-        raise ValueError(f"matrix {matrix!r}: one of {sorted(EXPORT_MATRICES)}")
+    colour = _colour_flags(matrix, full_range, transfer)
     if straight and over:
         raise ValueError("straight and over exclude each other: a composite is opaque")
     desc = Export()
     desc.format = EXPORT_FORMATS[fmt]
-    desc.flags = ((EXPORT_OVER if over else 0) | (EXPORT_STRAIGHT if straight else 0) | EXPORT_MATRICES[matrix]
-                  | (EXPORT_FULL_RANGE if full_range else 0))
+    desc.flags = (EXPORT_OVER if over else 0) | (EXPORT_STRAIGHT if straight else 0) | colour
     bg = [int(v) for v in background]
     assert len(bg) in (3, 4), background
     desc.background = (C.c_uint8 * 4)(*bg[:3], 0)
@@ -1112,7 +1127,7 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
         return self._L.glava_b200_framebuffer_device(self._h)
 
     def export_frames(self, streams, fmt="rgba", over=False, background=(0, 0, 0), out=None, after=None, done=None,
-                      matrix="bt709", full_range=False, straight=False):
+                      matrix="bt709", full_range=False, straight=False, transfer=None):
         """The current frames of `streams` (repeats allowed) top-down in the caller's device memory (glava_b200_export_frames):
         fmt "rgba" / "bgra" ([h, w, 4] per frame; over=True composites over `background` as GLava's window shows it) or
         "nv12" ([h * 3 / 2, w]: Y rows, then interleaved CbCr rows), "p010" (the same as uint16 samples, 10-bit code << 6),
@@ -1128,9 +1143,11 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
         `done` behind itself.  Left None, the export is ordered after the work already queued on torch's current stream,
         and that stream waits for the export (the tensors can be used right away).
         matrix ("bt709" / "bt601") and full_range: the Y'CbCr encoding of every YUV format (DESIGN 4.15; the
-        default is BT.709 limited range; matrix="bt601", full_range=True is JPEG's)."""
+        default is BT.709 limited range; matrix="bt601", full_range=True is JPEG's).  matrix="bt2020" with transfer="pq" or
+        "hlg": BT.2020 HDR10 / HLG limited range on p010, yuv420p10, yuv444p10 and yuv422p10, SDR graphics white at 203 cd/m^2
+        (DESIGN 4.22)."""
         s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, lambda stream: self.device, None, matrix,
-                                                 full_range, straight)
+                                                 full_range, straight, transfer)
         self._ordered(lambda a, d: self._L.glava_b200_export_frames(self._h, s.ctypes.data, s.shape[0], dst, C.byref(desc), a, d),
                       after, done)
         return result
@@ -1149,13 +1166,13 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
             cur.wait_stream(own)
 
     def export_scaled(self, streams, size, crop=None, fmt="rgba", over=False, background=(0, 0, 0), out=None, after=None,
-                      done=None, matrix="bt709", full_range=False, straight=False):
+                      done=None, matrix="bt709", full_range=False, straight=False, transfer=None):
         """export_frames of a source rectangle shrunk to size = (w, h) by the exact area average (glava_b200_export_scaled):
         crop = (x, y, w, h) in top-down coordinates (y = 0 is the top row), None: the whole frame.  Downscale only; NV12,
-        I420, P010 and YUV420P10 need an even w and h, YUV422P, YUV422P10 and UYVY an even w.  Shapes, out, after, done, matrix and full_range as export_frames, with the output
+        I420, P010 and YUV420P10 need an even w and h, YUV422P, YUV422P10 and UYVY an even w.  Shapes, out, after, done, matrix, full_range and transfer as export_frames, with the output
         size in place of the frame's; straight as export_frames (the stored channels averaged, then un-premultiplied)."""
         s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, lambda stream: self.device, size, matrix,
-                                                 full_range, straight)
+                                                 full_range, straight, transfer)
         sc = _export_scale(size, crop)
         self._ordered(lambda a, d: self._L.glava_b200_export_scaled(self._h, s.ctypes.data, s.shape[0], dst, None, C.byref(desc),
                                                                     C.byref(sc), a, d), after, done)
@@ -1164,7 +1181,8 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
     def export_ladder(self, streams, rungs, out=None, after=None, done=None):
         """Several sizes of each frame in one launch that reads each source row about once (glava_b200_export_ladder), for
         an encoder ladder: rungs = [dict(size=(w, h) or None for the frame's, crop=None, fmt="nv12", over=False,
-        background=(0, 0, 0), matrix="bt709", full_range=False, straight=False), ...], at most LADDER_MAX; rungs may mix encodings.  Rung j is exactly export_scaled(streams, **rungs[j]) at this
+        background=(0, 0, 0), matrix="bt709", full_range=False, straight=False, transfer=None), ...], at most LADDER_MAX; rungs may
+        mix encodings, HDR and SDR included.  Rung j is exactly export_scaled(streams, **rungs[j]) at this
         point in call order.  out: None or one entry per rung in any form export_scaled takes.  Returns one result per rung,
         shaped as export_scaled returns it; after / done and the ordering against torch's current stream as export_frames."""
         s, arr, n, dst, results = self._ladder_plan(streams, rungs, out, lambda stream: self.device)
@@ -1200,7 +1218,7 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
         return images
 
     def overlay_planes(self, streams, pictures, at=None, fmt="i420", matrix="bt709", full_range=False, after=None, done=None,
-                       opacity=None, size=None, crop=None):
+                       opacity=None, size=None, crop=None, transfer=None):
         """The current frames of `streams` composited in place onto decoded pictures, one tensor per plane
         (glava_b200_overlay_planes): NV12, I420, YUV444, P010, YUV420P10, YUV444P10, YUV422P, YUV422P10 or UYVY, the planes of each picture at their
         own addresses with one luma and one chroma pitch per call — ffmpeg's AVFrame planes, NVDEC surfaces, or what
@@ -1208,9 +1226,10 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
         overlay_frames blends NV12; any other opacity writes export_frames' bytes.  pictures and at: see _planes_plan;
         rectangles of one call must not overlap in any plane.  after / done and the ordering against torch's current
         stream as export_frames.  opacity: as overlay_frames (glava_b200_overlay_planes_opacity).  size / crop: as
-        overlay_frames (glava_b200_overlay_scaled).  Returns pictures."""
+        overlay_frames (glava_b200_overlay_scaled).  matrix="bt2020" with transfer="pq" / "hlg": an HDR picture (p010,
+        yuv420p10, yuv444p10, yuv422p10), the graphics blended at 203 cd/m^2 (DESIGN 4.22).  Returns pictures."""
         rect, sc = self._overlay_scale(size, crop)
-        s, desc, arr = self._planes_plan(streams, pictures, at, fmt, matrix, full_range, rect)
+        s, desc, arr = self._planes_plan(streams, pictures, at, fmt, matrix, full_range, rect, transfer)
         k = self._opacity(opacity, s.shape[0])
         if sc is not None:
             self._ordered(lambda a, d: self._L.glava_b200_overlay_scaled(self._h, s.ctypes.data, s.shape[0], arr, C.byref(desc),
@@ -1224,7 +1243,8 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
                                                                                  C.byref(desc), k.ctypes.data, a, d), after, done)
         return pictures
 
-    def export_mosaic(self, streams, cols, tile, fmt="nv12", background=(0, 0, 0), out=None, matrix="bt709", full_range=False):
+    def export_mosaic(self, streams, cols, tile, fmt="nv12", background=(0, 0, 0), out=None, matrix="bt709", full_range=False,
+                      transfer=None):
         """The frames of `streams` shrunk to tile = (w, h) and laid out row-major, `cols` tiles per row, in one picture, by
         one export_scaled call with a destination and a chroma destination per tile.  W = cols * w, H = rows * h; returns
         [H * 3 / 2, W] for NV12 (uint8) and P010 (uint16), Y rows then CbCr rows, the plane views (Y, Cb, Cr) for I420 and
@@ -1234,7 +1254,7 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
         BGRA).  out: a CUDA tensor [rows, pitch] whose rows hold the picture's row bytes, rows as
         _export_layout gives them for W x H (planar formats: the chroma planes back to back from row H); tiles past the last
         stream keep its bytes (out None: black).  Ordered against torch's current stream as export_frames without events.
-        matrix / full_range as export_frames (black: Y 0 in full range)."""
+        matrix / full_range / transfer as export_frames (black: Y 0 in full range, 64 in limited range and HDR)."""
         import torch
         s = np.ascontiguousarray(np.asarray(streams, dtype=np.int64).reshape(-1), dtype=np.int32)
         count, cols = int(s.shape[0]), int(cols)
@@ -1243,7 +1263,7 @@ class Renderer(_StreamState, _StreamStyles, _FrameExport):
             raise ValueError("export_mosaic: at least one stream and one column")
         if fmt in ALPHA_FORMATS:
             raise ValueError(f"export_mosaic: format {fmt!r}: a mosaic is one opaque picture, it takes no alpha format")
-        desc = _export_desc(fmt, False, background, matrix, full_range)
+        desc = _export_desc(fmt, False, background, matrix, full_range, transfer=transfer)
         W, H = cols * tw, (count + cols - 1) // cols * th
         rows, row_bytes, align = _export_layout(fmt, W, H)
         px = {"rgba": 4, "bgra": 4, "uyvy": 2}.get(fmt, 2 if fmt in WIDE_FORMATS else 1)
@@ -1393,27 +1413,29 @@ class ShardedRenderer(_StreamState, _StreamStyles, _FrameExport):
         return l, r
 
     def export_frames(self, streams, fmt="rgba", over=False, background=(0, 0, 0), out=None, matrix="bt709", full_range=False,
-                      straight=False):
+                      straight=False, transfer=None):
         """Renderer.export_frames with global stream indices (glava_b200_sharded_export_frames): each destination on the
         device of the shard that owns its stream (out None: one tensor when every listed stream lives on one device, else
         a list of per-frame tensors).  Work queued on torch's current streams of those devices is waited for first; the
-        frames are complete after sync().  matrix / full_range / straight as Renderer.export_frames."""
+        frames are complete after sync().  matrix / full_range / straight / transfer as Renderer.export_frames."""
         import torch
         device_of = self._device_of()
-        s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, device_of, None, matrix, full_range, straight)
+        s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, device_of, None, matrix, full_range, straight,
+                                                 transfer)
         for d in sorted({device_of(int(x)) for x in s}):
             torch.cuda.current_stream(d).synchronize()
         _check(self._L.glava_b200_sharded_export_frames(self._h, s.ctypes.data, s.shape[0], dst, C.byref(desc)))
         return result
 
     def export_scaled(self, streams, size, crop=None, fmt="rgba", over=False, background=(0, 0, 0), out=None, matrix="bt709",
-                      full_range=False, straight=False):
+                      full_range=False, straight=False, transfer=None):
         """Renderer.export_scaled with global stream indices (glava_b200_sharded_export_scaled), destinations placed as
         export_frames places them; the frames are complete after sync().  matrix / full_range / straight as
         Renderer.export_frames."""
         import torch
         device_of = self._device_of()
-        s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, device_of, size, matrix, full_range, straight)
+        s, desc, dst, result = self._export_plan(streams, fmt, over, background, out, device_of, size, matrix, full_range, straight,
+                                                 transfer)
         sc = _export_scale(size, crop)
         for d in sorted({device_of(int(x)) for x in s}):
             torch.cuda.current_stream(d).synchronize()
@@ -1455,14 +1477,14 @@ class ShardedRenderer(_StreamState, _StreamStyles, _FrameExport):
         return images
 
     def overlay_planes(self, streams, pictures, at=None, fmt="i420", matrix="bt709", full_range=False, opacity=None, size=None,
-                       crop=None):
+                       crop=None, transfer=None):
         """Renderer.overlay_planes with global stream indices (glava_b200_sharded_overlay_planes), each picture on the device
         of the shard that owns its stream.  Work queued on torch's current streams of those devices is waited for first;
         the pictures are complete after sync().  opacity / size / crop as Renderer.overlay_frames."""
         import torch
         device_of = self._device_of()
         rect, sc = self._overlay_scale(size, crop)
-        s, desc, arr = self._planes_plan(streams, pictures, at, fmt, matrix, full_range, rect)
+        s, desc, arr = self._planes_plan(streams, pictures, at, fmt, matrix, full_range, rect, transfer)
         k = self._opacity(opacity, s.shape[0])
         for d in sorted({device_of(int(x)) for x in s if 0 <= int(x) < self.batch}):
             torch.cuda.current_stream(d).synchronize()

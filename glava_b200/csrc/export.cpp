@@ -81,8 +81,16 @@ int desc_check(ExportKind kind, int w, int h, const glava_b200_export& d, const 
         return fail(GLAVA_B200_EINVAL, "%s: format %s: the overlay takes RGBA, BGRA or NV12", who, format_name(d.format));
     // the colour bits (DESIGN 4.15) are flags of the Y'CbCr formats only
     const uint32_t colour = GLAVA_B200_EXPORT_FULL_RANGE | GLAVA_B200_EXPORT_BT601;
-    if (d.flags & ~(GLAVA_B200_EXPORT_OVER | GLAVA_B200_EXPORT_STRAIGHT | colour))
+    const uint32_t hdr = GLAVA_B200_EXPORT_PQ | GLAVA_B200_EXPORT_HLG;
+    if (d.flags & ~(GLAVA_B200_EXPORT_OVER | GLAVA_B200_EXPORT_STRAIGHT | colour | hdr))
         return fail(GLAVA_B200_EINVAL, "%s: unknown flags 0x%x", who, d.flags);
+    if (d.flags & hdr) {                                    // DESIGN 4.22
+        if (kind == ExportKind::overlay)
+            return fail(GLAVA_B200_EINVAL, "%s: flags 0x%x: the overlay of RGBA, BGRA and NV12 takes no HDR bit (EXPORT_PQ, "
+                        "EXPORT_HLG); HDR pictures go to glava_b200_overlay_planes", who, d.flags);
+        const int rc = hdr_flags_check(d.format, d.flags, who);
+        if (rc) return rc;
+    }
     // transparency (DESIGN 4.19): straight alpha is RGBA / BGRA's alone, and never composited; the YUVA formats never are
     if (kind == ExportKind::overlay && (d.flags & GLAVA_B200_EXPORT_STRAIGHT))
         return fail(GLAVA_B200_EINVAL, "%s: flags 0x%x: EXPORT_STRAIGHT is for the exports; the overlay composites", who, d.flags);
@@ -142,6 +150,23 @@ void common_args(Args& a, const RendererView& v, const void* d_list, int count, 
 }  // namespace
 
 namespace glb {
+// The HDR bits (DESIGN 4.22) of an export or a picture: one of them, alone among the colour bits, without EXPORT_STRAIGHT,
+// on P010, YUV420P10, YUV444P10 or YUV422P10
+int hdr_flags_check(int format, uint32_t flags, const char* who) {
+    const uint32_t hdr = GLAVA_B200_EXPORT_PQ | GLAVA_B200_EXPORT_HLG;
+    if ((flags & hdr) == hdr)
+        return fail(GLAVA_B200_EINVAL, "%s: flags 0x%x: EXPORT_PQ and EXPORT_HLG exclude each other", who, flags);
+    if (flags & (GLAVA_B200_EXPORT_FULL_RANGE | GLAVA_B200_EXPORT_BT601))
+        return fail(GLAVA_B200_EINVAL, "%s: flags 0x%x: EXPORT_PQ / EXPORT_HLG are BT.2020 limited range (no EXPORT_FULL_RANGE or "
+                    "EXPORT_BT601)", who, flags);
+    if (flags & GLAVA_B200_EXPORT_STRAIGHT)
+        return fail(GLAVA_B200_EINVAL, "%s: flags 0x%x: EXPORT_PQ / EXPORT_HLG carry no alpha (no EXPORT_STRAIGHT)", who, flags);
+    if (!export_hdr_format(format))
+        return fail(GLAVA_B200_EINVAL, "%s: flags 0x%x: EXPORT_PQ / EXPORT_HLG are for P010, YUV420P10, YUV444P10 and YUV422P10, "
+                    "not format %d", who, flags, format);
+    return 0;
+}
+
 int scale_check(int w, int h, const glava_b200_export_scale* s, glava_b200_export_scale* q, const char* who) {
     if (!s) return fail(GLAVA_B200_EINVAL, "%s: null scale", who);
     *q = *s;

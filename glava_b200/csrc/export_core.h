@@ -88,8 +88,12 @@ constexpr bool yuv_same(const YuvCoef& a, int yr, int yg, int yb, int cbr, int c
            a.crb == crb && a.crr == -(crg + crb);
 }
 static_assert(yuv_same(yuv_enc(0, 8), GLB_Y_R, GLB_Y_G, GLB_Y_B, GLB_CB_R, GLB_CB_G, GLB_CR_G, GLB_CR_B), "BT.709 limited 8-bit");
-// the encoding index of a descriptor's flags
-GLB_HD int export_enc(uint32_t flags) { return (int) ((flags >> 8) & 3u); }
+// the encoding index of a descriptor's flags: 0..3 as above, 4 for GLAVA_B200_EXPORT_PQ and 5 for GLAVA_B200_EXPORT_HLG
+// (DESIGN 4.22; the host refuses either with the other bits)
+GLB_HD int export_enc(uint32_t flags) {
+    const uint32_t hdr = (flags >> 11) & 3u;
+    return hdr ? (int) (3u + hdr) : (int) ((flags >> 8) & 3u);
+}
 // a code of set S from its accumulator (scaled by 2^shift, rounding included): full range clamps to the top code
 template <int E, int Bits>
 GLB_HD uint32_t yuv_code(int acc, int shift) {
@@ -97,6 +101,123 @@ GLB_HD uint32_t yuv_code(int acc, int shift) {
     const int v = acc >> shift;
     if constexpr (S.full) return (uint32_t) (v > S.top ? S.top : v);
     return (uint32_t) v;
+}
+
+// ---- BT.2020 HDR: PQ and HLG at 10 bits (DESIGN 4.22) --------------------------------------------------------------------
+// GLAVA_B200_EXPORT_PQ (0x800) and GLAVA_B200_EXPORT_HLG (0x1000) select encodings E = 4 and 5: BT.2020 non-constant-
+// luminance Y'CbCr, limited range, with that transfer function, on P010, YUV420P10, YUV444P10 and YUV422P10 only.  An
+// 8-bit R'G'B' triple v (BT.709 primaries) is shown as SDR graphics at BT.2408's 203 cd/m^2, display-referred:
+//   L = (v / 255)^2.4 (BT.1886, L_B = 0; hdr_lin's table of float64 rounded to float32),
+//   F = 203 M L, M the BT.709 -> BT.2020 matrix from the primaries and D65 (BT.2087's to 4 decimals),
+//   PQ: E' = PQ^-1(F / 10000) (ST 2084); HLG: BT.2100's inverse OOTF for a 1000 cd/m^2 display (gamma 1.2, L_B = 0), then
+//   its OETF; Y' = 0.2627 R' + 0.6780 G' + 0.0593 B', Y = 64 + 876 Y', Cb = 512 + 896 (B' - Y') / 1.8814, Cr = 512 + 896
+//   (R' - Y') / 1.4746, rounded half up.  Subsampled chroma is that of the mean of the pixels' E' (hdr_mean4, a fixed order).
+// Only correctly rounded float32 operations and gl_math.h's glm_log / glm_exp / glm_pow, so the host build and the kernels
+// (--fmad=false) agree bit for bit.  No channel passes 203 cd/m^2, so MaxCLL <= 203.  These encodings run only in
+// instantiations E = 4, 5 of the 10-bit items (export_y10 and the quads branch on E at compile time).
+#define GLB_ENC_PQ 4
+#define GLB_ENC_HLG 5
+GLB_HD bool export_hdr_format(int format) {             // the formats the HDR bits apply to
+    return format == GLAVA_B200_EXPORT_P010 || format == GLAVA_B200_EXPORT_YUV420P10 || format == GLAVA_B200_EXPORT_YUV444P10 ||
+           format == GLAVA_B200_EXPORT_YUV422P10;
+}
+#define GLB_HDR_LIN_TABLE { \
+    0.0f, 1.67611404e-06f, 8.84658311e-06f, 2.34096315e-05f, 4.66925449e-05f, 7.97685279e-05f, 0.000123556776f, 0.000178870556f, \
+    0.000246444717f, 0.000326953188f, 0.000421020814f, 0.000529231911f, 0.000652136572f, 0.000790255668f, 0.000944084488f, 0.00111409591f, \
+    0.00130074308f, 0.00150446116f, 0.00172566937f, 0.00196477212f, 0.00222216127f, 0.0024982153f, 0.00279330276f, 0.00310778082f, \
+    0.00344199757f, 0.00379629177f, 0.00417099427f, 0.00456642779f, 0.00498290779f, 0.00542074209f, 0.00588023337f, 0.00636167731f, \
+    0.0068653631f, 0.00739157572f, 0.00794059318f, 0.00851269066f, 0.00910813734f, 0.00972719677f, 0.0103701297f, 0.0110371923f, \
+    0.0117286369f, 0.0124447113f, 0.0131856594f, 0.0139517235f, 0.01474314f, 0.0155601436f, 0.0164029654f, 0.0172718335f, \
+    0.0181669723f, 0.0190886036f, 0.0200369488f, 0.0210122224f, 0.0220146403f, 0.023044413f, 0.0241017509f, 0.0251868591f, \
+    0.0262999441f, 0.0274412073f, 0.0286108498f, 0.029809067f, 0.0310360584f, 0.0322920159f, 0.033577133f, 0.0348916017f, \
+    0.0362356044f, 0.0376093313f, 0.0390129685f, 0.0404466987f, 0.0419107042f, 0.043405164f, 0.0449302532f, 0.0464861542f, \
+    0.0480730385f, 0.049691081f, 0.0513404533f, 0.0530213267f, 0.0547338724f, 0.0564782582f, 0.0582546517f, 0.0600632168f, \
+    0.0619041175f, 0.0637775213f, 0.0656835809f, 0.0676224604f, 0.0695943311f, 0.0715993345f, 0.0736376345f, 0.0757093951f, \
+    0.0778147578f, 0.0799538866f, 0.0821269304f, 0.0843340382f, 0.0865753666f, 0.0888510644f, 0.0911612809f, 0.0935061574f, \
+    0.0958858505f, 0.0983005017f, 0.100750253f, 0.103235252f, 0.10575565f, 0.108311571f, 0.110903174f, 0.113530591f, \
+    0.116193965f, 0.118893437f, 0.121629141f, 0.124401219f, 0.127209798f, 0.130055025f, 0.132937044f, 0.135855973f, \
+    0.138811946f, 0.141805097f, 0.144835562f, 0.147903472f, 0.151008964f, 0.15415217f, 0.15733321f, 0.160552204f, \
+    0.163809299f, 0.167104617f, 0.17043829f, 0.173810437f, 0.177221179f, 0.180670649f, 0.184158966f, 0.187686265f, \
+    0.191252664f, 0.194858283f, 0.198503241f, 0.202187672f, 0.205911696f, 0.209675416f, 0.213478968f, 0.217322454f, \
+    0.221206024f, 0.225129768f, 0.22909382f, 0.233098283f, 0.237143293f, 0.241228953f, 0.245355383f, 0.249522701f, \
+    0.253731012f, 0.257980436f, 0.262271076f, 0.266603082f, 0.270976543f, 0.275391549f, 0.279848248f, 0.28434673f, \
+    0.288887113f, 0.293469518f, 0.298094034f, 0.30276081f, 0.307469904f, 0.312221438f, 0.317015558f, 0.321852326f, \
+    0.32673189f, 0.33165434f, 0.336619765f, 0.341628283f, 0.346680015f, 0.35177505f, 0.356913507f, 0.362095475f, \
+    0.367321074f, 0.372590393f, 0.377903551f, 0.383260638f, 0.388661772f, 0.394107074f, 0.399596572f, 0.405130446f, \
+    0.410708755f, 0.416331619f, 0.421999156f, 0.427711427f, 0.43346855f, 0.439270616f, 0.445117742f, 0.451010019f, \
+    0.456947535f, 0.462930411f, 0.468958735f, 0.475032598f, 0.481152117f, 0.487317383f, 0.493528455f, 0.499785483f, \
+    0.506088555f, 0.512437761f, 0.51883316f, 0.525274873f, 0.531763017f, 0.538297653f, 0.54487896f, 0.551506877f, \
+    0.558181643f, 0.564903319f, 0.571671903f, 0.578487635f, 0.585350454f, 0.592260599f, 0.599218071f, 0.606222987f, \
+    0.613275409f, 0.620375514f, 0.627523303f, 0.634718955f, 0.641962469f, 0.649253964f, 0.656593561f, 0.663981318f, \
+    0.671417356f, 0.678901732f, 0.686434567f, 0.69401592f, 0.701645911f, 0.709324598f, 0.717052102f, 0.724828482f, \
+    0.732653797f, 0.740528226f, 0.748451769f, 0.756424546f, 0.764446676f, 0.772518218f, 0.780639231f, 0.788809836f, \
+    0.797030091f, 0.805300117f, 0.813620031f, 0.821989834f, 0.830409646f, 0.838879526f, 0.847399592f, 0.855969965f, \
+    0.864590704f, 0.873261809f, 0.881983459f, 0.890755713f, 0.899578691f, 0.908452392f, 0.917376935f, 0.926352441f, \
+    0.935378969f, 0.944456577f, 0.953585386f, 0.962765455f, 0.971996844f, 0.981279731f, 0.990614057f, 1.0f \
+}
+#ifdef __CUDACC__
+__device__ static const float glb_hdr_lin_dev[256] = GLB_HDR_LIN_TABLE;
+#endif
+static const float glb_hdr_lin_host[256] = GLB_HDR_LIN_TABLE;
+// (v / 255)^2.4 of an 8-bit code
+GLB_HD float hdr_lin(uint32_t v) {
+#ifdef __CUDA_ARCH__
+    return __ldg(glb_hdr_lin_dev + v);
+#else
+    return glb_hdr_lin_host[v];
+#endif
+}
+// 203 M / 10000 (PQ's F / 10000) and 203 M / 1000 (HLG's F / 1000), float64 rounded to float32, row-major
+#define GLB_HDR_M_PQ { 0.0127362991f, 0.00668444578f, 0.00087925524f, 0.00140267494f, 0.0186666697f, 0.000230655001f, \
+                       0.000332746218f, 0.00178667018f, 0.0181805845f }
+#define GLB_HDR_M_HLG { 0.127362996f, 0.0668444559f, 0.00879255217f, 0.0140267499f, 0.186666697f, 0.00230655004f, \
+                        0.00332746212f, 0.0178667009f, 0.181805834f }
+struct HdrRgb { float r, g, b; };                           // E' = (R', G', B')
+struct HdrM { float rr, rg, rb, gr, gg, gb, br, bg, bb; };
+// ST 2084's inverse EOTF of y = F / 10000 >= 0; m1, m2, c1, c2, c3 are exact in float32
+GLB_HD float hdr_pq(float y) {
+    const float p = glm_pow(y, 0.1593017578125f);
+    return glm_pow(glm_div(glm_fma(18.8515625f, p, 0.8359375f), glm_fma(18.6875f, p, 1.0f)), 78.84375f);
+}
+// BT.2100's HLG OETF of scene light e >= 0 (a = 0.17883277, b = 1 - 4a, c = 0.5 - a ln 4a)
+GLB_HD float hdr_hlg(float e) {
+    if (e <= 1.0f / 12.0f) return glm_sqrt(glm_mul(3.0f, e));
+    return glm_fma(0.17883277f, glm_log(glm_fma(12.0f, e, -0.28466892f)), 0.55991073f);
+}
+// E' of an 8-bit triple c (R low; the top byte is ignored) under E = 4 (PQ) or 5 (HLG)
+template <int E>
+GLB_HD HdrRgb hdr_rgb(uint32_t c) {
+    constexpr HdrM m = E == GLB_ENC_PQ ? HdrM GLB_HDR_M_PQ : HdrM GLB_HDR_M_HLG;
+    const float lr = hdr_lin(c & 255u), lg = hdr_lin((c >> 8) & 255u), lb = hdr_lin((c >> 16) & 255u);
+    const float fr = glm_fma(m.rb, lb, glm_fma(m.rg, lg, glm_mul(m.rr, lr)));
+    const float fg = glm_fma(m.gb, lb, glm_fma(m.gg, lg, glm_mul(m.gr, lr)));
+    const float fb = glm_fma(m.bb, lb, glm_fma(m.bg, lg, glm_mul(m.br, lr)));
+    if constexpr (E == GLB_ENC_PQ) {
+        return { hdr_pq(fr), hdr_pq(fg), hdr_pq(fb) };
+    } else {
+        // inverse OOTF: E = (F / 1000) (Y_D / 1000)^(-1/6), E = 0 where Y_D = 0 (black: every F is 0)
+        const float yd = glm_fma(0.0593f, fb, glm_fma(0.6780f, fg, glm_mul(0.2627f, fr)));
+        if (yd <= 0.0f) return { 0.0f, 0.0f, 0.0f };
+        const float s = glm_pow(yd, -1.0f / 6.0f);
+        return { hdr_hlg(glm_mul(fr, s)), hdr_hlg(glm_mul(fg, s)), hdr_hlg(glm_mul(fb, s)) };
+    }
+}
+// BT.2020's Y' of E'
+GLB_HD float hdr_luma(const HdrRgb& e) { return glm_fma(0.0593f, e.b, glm_fma(0.6780f, e.g, glm_mul(0.2627f, e.r))); }
+// the unrounded 10-bit codes: Y, and Cb / Cr (896 / 1.8814 and 896 / 1.4746 folded)
+GLB_HD float hdr_yf(const HdrRgb& e) { return glm_fma(876.0f, hdr_luma(e), 64.0f); }
+GLB_HD float hdr_cbf(const HdrRgb& e) { return glm_fma(476.241097f, glm_add(e.b, -hdr_luma(e)), 512.0f); }
+GLB_HD float hdr_crf(const HdrRgb& e) { return glm_fma(607.622406f, glm_add(e.r, -hdr_luma(e)), 512.0f); }
+// a code rounded half up; every value passed lies in [0, 1023]
+GLB_HD uint32_t hdr_code(float x) { return (uint32_t) glm_add(x, 0.5f); }
+GLB_HD uint32_t hdr_y10(const HdrRgb& e) { return hdr_code(hdr_yf(e)); }
+// (Cb, Cr) codes of E', Cb in the low 16 bits (as export_cbcr10)
+GLB_HD uint32_t hdr_cbcr10(const HdrRgb& e) { return hdr_code(hdr_cbf(e)) | (hdr_code(hdr_crf(e)) << 16); }
+// the mean E' of a 2x2 block (a, b the top row) in a fixed order; a 4:2:2 pair (a, b) is the block (a, b, a, b), whose mean
+// is exactly (a + b) / 2, and one pixel the block (a, a, a, a), whose mean is exactly a
+GLB_HD HdrRgb hdr_mean4(const HdrRgb& a, const HdrRgb& b, const HdrRgb& c, const HdrRgb& d) {
+    return { glm_mul(glm_add(glm_add(a.r, b.r), glm_add(c.r, d.r)), 0.25f), glm_mul(glm_add(glm_add(a.g, b.g), glm_add(c.g, d.g)), 0.25f),
+             glm_mul(glm_add(glm_add(a.b, b.b), glm_add(c.b, d.b)), 0.25f) };
 }
 
 // the Y code of a composited pixel under encoding E (E = 0: the BT.709 limited byte above)
@@ -222,9 +343,13 @@ static_assert(yuv_same(yuv_enc(0, 10), GLB_Y10_R, GLB_Y10_G, GLB_Y10_B, GLB_CB10
 // the 10-bit Y code of a composited pixel
 template <int E = 0>
 GLB_HD uint32_t export_y10(uint32_t c) {
-    constexpr YuvCoef S = yuv_enc(E, 10);
-    const int r = (int) (c & 255u), g = (int) ((c >> 8) & 255u), b = (int) ((c >> 16) & 255u);
-    return yuv_code<E, 10>(S.yr * r + S.yg * g + S.yb * b + (S.yoff << GLB_YUV_SHIFT) + GLB_YUV_HALF, GLB_YUV_SHIFT);
+    if constexpr (E >= GLB_ENC_PQ) {
+        return hdr_y10(hdr_rgb<E>(c));
+    } else {
+        constexpr YuvCoef S = yuv_enc(E, 10);
+        const int r = (int) (c & 255u), g = (int) ((c >> 8) & 255u), b = (int) ((c >> 16) & 255u);
+        return yuv_code<E, 10>(S.yr * r + S.yg * g + S.yb * b + (S.yoff << GLB_YUV_SHIFT) + GLB_YUV_HALF, GLB_YUV_SHIFT);
+    }
 }
 // The per-channel sums (0..1020) of a 2x2 block's four composited pixels, 10 bits each (R low).  P010 chroma takes these
 // exact sums, not NV12's (s + 2) >> 2 byte: the two bits that average rounds away are what 10 bits carry.
@@ -245,22 +370,44 @@ GLB_HD uint32_t export_cbcr10(uint32_t s) {
     const uint32_t cr = yuv_code<E, 10>(S.crr * r + S.crg * g + S.crb * b + (S.coff << 18) + (1 << 17), 18);
     return cb | (cr << 16);
 }
+// The 10-bit (Cb, Cr) codes of the 2x2 block of composited pixels a, b (top row), c, d, Cb low: export_cbcr10 of their sums,
+// or under an HDR encoding the chroma of their mean E' (the scaled items, which hold one pixel per lane, take this)
+template <int E = 0>
+GLB_HD uint32_t export_block10(uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+    if constexpr (E >= GLB_ENC_PQ) return hdr_cbcr10(hdr_mean4(hdr_rgb<E>(a), hdr_rgb<E>(b), hdr_rgb<E>(c), hdr_rgb<E>(d)));
+    else return export_cbcr10<E>(export_sum4(a, b, c, d));
+}
 // P010 of a quad of output rows 2j (top) and 2j + 1 (bot): per row its four Y samples as two words (little-endian uint16,
 // code << 6), and the (Cb, Cr) sample pairs of the quad's two 2x2 blocks, one word each
 template <int E = 0>
 GLB_HD void export_p010_quad(const ExportFmt& f, const uint32_t top[4], const uint32_t bot[4], uint32_t yt[2], uint32_t yb[2],
                              uint32_t uv[2]) {
-    uint32_t t[4], b[4];
+    if constexpr (E >= GLB_ENC_PQ) {                        // DESIGN 4.22: each pixel's E' once, the block's mean for chroma
+        HdrRgb t[4], b[4];
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        t[k] = export_over(top[k], f.bg, f.native);
-        b[k] = export_over(bot[k], f.bg, f.native);
-    }
+        for (int k = 0; k < 4; ++k) {
+            t[k] = hdr_rgb<E>(export_over(top[k], f.bg, f.native));
+            b[k] = hdr_rgb<E>(export_over(bot[k], f.bg, f.native));
+        }
 #pragma unroll
-    for (int k = 0; k < 2; ++k) {
-        yt[k] = (export_y10<E>(t[2 * k]) << 6) | (export_y10<E>(t[2 * k + 1]) << 22);
-        yb[k] = (export_y10<E>(b[2 * k]) << 6) | (export_y10<E>(b[2 * k + 1]) << 22);
-        uv[k] = export_cbcr10<E>(export_sum4(t[2 * k], t[2 * k + 1], b[2 * k], b[2 * k + 1])) << 6;
+        for (int k = 0; k < 2; ++k) {
+            yt[k] = (hdr_y10(t[2 * k]) << 6) | (hdr_y10(t[2 * k + 1]) << 22);
+            yb[k] = (hdr_y10(b[2 * k]) << 6) | (hdr_y10(b[2 * k + 1]) << 22);
+            uv[k] = hdr_cbcr10(hdr_mean4(t[2 * k], t[2 * k + 1], b[2 * k], b[2 * k + 1])) << 6;
+        }
+    } else {
+        uint32_t t[4], b[4];
+    #pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            t[k] = export_over(top[k], f.bg, f.native);
+            b[k] = export_over(bot[k], f.bg, f.native);
+        }
+    #pragma unroll
+        for (int k = 0; k < 2; ++k) {
+            yt[k] = (export_y10<E>(t[2 * k]) << 6) | (export_y10<E>(t[2 * k + 1]) << 22);
+            yb[k] = (export_y10<E>(b[2 * k]) << 6) | (export_y10<E>(b[2 * k + 1]) << 22);
+            uv[k] = export_cbcr10<E>(export_sum4(t[2 * k], t[2 * k + 1], b[2 * k], b[2 * k + 1])) << 6;
+        }
     }
 }
 
@@ -292,40 +439,72 @@ GLB_HD ExportZero export_zero(const ExportFmt& f) {
 // per-pixel 10-bit code, so no new rounding enters.
 template <int E = 0>
 GLB_HD uint32_t export_cbcr10_px(uint32_t c) {
-    const uint32_t s = (c & 255u) | (((c >> 8) & 255u) << 10) | (((c >> 16) & 255u) << 20);
-    return export_cbcr10<E>(s << 2);
+    if constexpr (E >= GLB_ENC_PQ) {
+        return hdr_cbcr10(hdr_rgb<E>(c));
+    } else {
+        const uint32_t s = (c & 255u) | (((c >> 8) & 255u) << 10) | (((c >> 16) & 255u) << 20);
+        return export_cbcr10<E>(s << 2);
+    }
 }
 // yuv420p10le of a quad of output rows 2j (top) and 2j + 1 (bot): per row its four Y samples as two words (two uint16
 // each), and the Cb samples and the Cr samples of the quad's two 2x2 blocks, one word each
 template <int E = 0>
 GLB_HD void export_i010_quad(const ExportFmt& f, const uint32_t top[4], const uint32_t bot[4], uint32_t yt[2], uint32_t yb[2],
                              uint32_t* cb, uint32_t* cr) {
-    uint32_t t[4], b[4];
+    if constexpr (E >= GLB_ENC_PQ) {                        // as export_p010_quad's, in the planar layout
+        HdrRgb t[4], b[4];
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        t[k] = export_over(top[k], f.bg, f.native);
-        b[k] = export_over(bot[k], f.bg, f.native);
-    }
+        for (int k = 0; k < 4; ++k) {
+            t[k] = hdr_rgb<E>(export_over(top[k], f.bg, f.native));
+            b[k] = hdr_rgb<E>(export_over(bot[k], f.bg, f.native));
+        }
 #pragma unroll
-    for (int k = 0; k < 2; ++k) {
-        yt[k] = export_y10<E>(t[2 * k]) | (export_y10<E>(t[2 * k + 1]) << 16);
-        yb[k] = export_y10<E>(b[2 * k]) | (export_y10<E>(b[2 * k + 1]) << 16);
+        for (int k = 0; k < 2; ++k) {
+            yt[k] = hdr_y10(t[2 * k]) | (hdr_y10(t[2 * k + 1]) << 16);
+            yb[k] = hdr_y10(b[2 * k]) | (hdr_y10(b[2 * k + 1]) << 16);
+        }
+        const uint32_t c0 = hdr_cbcr10(hdr_mean4(t[0], t[1], b[0], b[1])), c1 = hdr_cbcr10(hdr_mean4(t[2], t[3], b[2], b[3]));
+        *cb = (c0 & 0xffffu) | (c1 << 16);
+        *cr = (c0 >> 16) | (c1 & 0xffff0000u);
+    } else {
+        uint32_t t[4], b[4];
+    #pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            t[k] = export_over(top[k], f.bg, f.native);
+            b[k] = export_over(bot[k], f.bg, f.native);
+        }
+    #pragma unroll
+        for (int k = 0; k < 2; ++k) {
+            yt[k] = export_y10<E>(t[2 * k]) | (export_y10<E>(t[2 * k + 1]) << 16);
+            yb[k] = export_y10<E>(b[2 * k]) | (export_y10<E>(b[2 * k + 1]) << 16);
+        }
+        const uint32_t c0 = export_cbcr10<E>(export_sum4(t[0], t[1], b[0], b[1]));
+        const uint32_t c1 = export_cbcr10<E>(export_sum4(t[2], t[3], b[2], b[3]));
+        *cb = (c0 & 0xffffu) | (c1 << 16);
+        *cr = (c0 >> 16) | (c1 & 0xffff0000u);
     }
-    const uint32_t c0 = export_cbcr10<E>(export_sum4(t[0], t[1], b[0], b[1]));
-    const uint32_t c1 = export_cbcr10<E>(export_sum4(t[2], t[3], b[2], b[3]));
-    *cb = (c0 & 0xffffu) | (c1 << 16);
-    *cr = (c0 >> 16) | (c1 & 0xffff0000u);
 }
 // yuv444p10le of one row's quad: the Y, Cb and Cr samples of each composited pixel, two words each
 template <int E = 0>
 GLB_HD void export_444p10_quad(const ExportFmt& f, const uint32_t in[4], uint32_t y[2], uint32_t cb[2], uint32_t cr[2]) {
+    if constexpr (E >= GLB_ENC_PQ) {                        // DESIGN 4.22: each pixel's E' once
 #pragma unroll
-    for (int k = 0; k < 2; ++k) {
-        const uint32_t c0 = export_over(in[2 * k], f.bg, f.native), c1 = export_over(in[2 * k + 1], f.bg, f.native);
-        const uint32_t uv0 = export_cbcr10_px<E>(c0), uv1 = export_cbcr10_px<E>(c1);
-        y[k] = export_y10<E>(c0) | (export_y10<E>(c1) << 16);
-        cb[k] = (uv0 & 0xffffu) | (uv1 << 16);
-        cr[k] = (uv0 >> 16) | (uv1 & 0xffff0000u);
+        for (int k = 0; k < 2; ++k) {
+            const HdrRgb e0 = hdr_rgb<E>(export_over(in[2 * k], f.bg, f.native)), e1 = hdr_rgb<E>(export_over(in[2 * k + 1], f.bg, f.native));
+            const uint32_t uv0 = hdr_cbcr10(e0), uv1 = hdr_cbcr10(e1);
+            y[k] = hdr_y10(e0) | (hdr_y10(e1) << 16);
+            cb[k] = (uv0 & 0xffffu) | (uv1 << 16);
+            cr[k] = (uv0 >> 16) | (uv1 & 0xffff0000u);
+        }
+    } else {
+    #pragma unroll
+        for (int k = 0; k < 2; ++k) {
+            const uint32_t c0 = export_over(in[2 * k], f.bg, f.native), c1 = export_over(in[2 * k + 1], f.bg, f.native);
+            const uint32_t uv0 = export_cbcr10_px<E>(c0), uv1 = export_cbcr10_px<E>(c1);
+            y[k] = export_y10<E>(c0) | (export_y10<E>(c1) << 16);
+            cb[k] = (uv0 & 0xffffu) | (uv1 << 16);
+            cr[k] = (uv0 >> 16) | (uv1 & 0xffff0000u);
+        }
     }
 }
 // export_zero of the planar 10-bit formats: y, one of a row's two equal luma words; u and v, the Cb and Cr words (YUV420P10:
@@ -374,15 +553,26 @@ GLB_HD void export_uyvy_split(const uint32_t w[2], uint32_t* y, uint32_t* uv) {
 // pairs, one word each
 template <int E = 0>
 GLB_HD void export_422p10_quad(const ExportFmt& f, const uint32_t in[4], uint32_t y[2], uint32_t* cb, uint32_t* cr) {
-    uint32_t c[4];
+    if constexpr (E >= GLB_ENC_PQ) {                        // DESIGN 4.22: each pixel's E' once, a pair's chroma its block's
+        HdrRgb e[4];
 #pragma unroll
-    for (int k = 0; k < 4; ++k) c[k] = export_over(in[k], f.bg, f.native);
+        for (int k = 0; k < 4; ++k) e[k] = hdr_rgb<E>(export_over(in[k], f.bg, f.native));
 #pragma unroll
-    for (int k = 0; k < 2; ++k) y[k] = export_y10<E>(c[2 * k]) | (export_y10<E>(c[2 * k + 1]) << 16);
-    const uint32_t c0 = export_cbcr10<E>(export_sum4(c[0], c[1], c[0], c[1]));
-    const uint32_t c1 = export_cbcr10<E>(export_sum4(c[2], c[3], c[2], c[3]));
-    *cb = (c0 & 0xffffu) | (c1 << 16);
-    *cr = (c0 >> 16) | (c1 & 0xffff0000u);
+        for (int k = 0; k < 2; ++k) y[k] = hdr_y10(e[2 * k]) | (hdr_y10(e[2 * k + 1]) << 16);
+        const uint32_t c0 = hdr_cbcr10(hdr_mean4(e[0], e[1], e[0], e[1])), c1 = hdr_cbcr10(hdr_mean4(e[2], e[3], e[2], e[3]));
+        *cb = (c0 & 0xffffu) | (c1 << 16);
+        *cr = (c0 >> 16) | (c1 & 0xffff0000u);
+    } else {
+        uint32_t c[4];
+    #pragma unroll
+        for (int k = 0; k < 4; ++k) c[k] = export_over(in[k], f.bg, f.native);
+    #pragma unroll
+        for (int k = 0; k < 2; ++k) y[k] = export_y10<E>(c[2 * k]) | (export_y10<E>(c[2 * k + 1]) << 16);
+        const uint32_t c0 = export_cbcr10<E>(export_sum4(c[0], c[1], c[0], c[1]));
+        const uint32_t c1 = export_cbcr10<E>(export_sum4(c[2], c[3], c[2], c[3]));
+        *cb = (c0 & 0xffffu) | (c1 << 16);
+        *cr = (c0 >> 16) | (c1 & 0xffff0000u);
+    }
 }
 // export_zero of the 4:2:2 formats: YUV422P y the Y word, u and v the Cb and Cr pairs; YUV422P10 y one of the two equal Y
 // words, u and v the Cb and Cr words; UYVY y the word of a pixel pair (u, v unused)
@@ -623,10 +813,13 @@ GLB_HD int ladder_unit_col(uint64_t u) { return (int) (u & 0xfffffffu); }
 // The kernel a ladder launches, from its rungs' formats (kernel format codes) and encodings (host code):
 // export_ladder_yuva_kernel when a rung is YUVA or straight RGBA / BGRA, else export_ladder_422_kernel when one is 4:2:2,
 // else export_ladder_p10_kernel when one is planar 10-bit, else export_ladder_enc_kernel when one has an encoding other
-// than 0, else export_ladder_yuv_kernel when one is I420, YUV444 or P010, else export_ladder_kernel
-enum LadderKernel { ladder_plain = 0, ladder_yuv = 1, ladder_enc = 2, ladder_p10 = 3, ladder_422 = 4, ladder_yuva = 5 };
+// than 0, else export_ladder_yuv_kernel when one is I420, YUV444 or P010, else export_ladder_kernel; before all of them
+// export_ladder_hdr_kernel when a rung has an HDR encoding (DESIGN 4.22)
+enum LadderKernel { ladder_plain = 0, ladder_yuv = 1, ladder_enc = 2, ladder_p10 = 3, ladder_422 = 4, ladder_yuva = 5, ladder_hdr = 6 };
 inline int ladder_kernel(const int* format, const int* enc, int n) {
     bool yuv = false, e = false, p10 = false, k422 = false, alpha = false;
+    for (int j = 0; j < n; ++j)
+        if (enc[j] >= GLB_ENC_PQ) return ladder_hdr;
     for (int j = 0; j < n; ++j) {
         yuv |= format[j] != GLAVA_B200_EXPORT_NV12 && export_yuv(format[j]);
         e |= enc[j] != 0;
@@ -797,6 +990,38 @@ GLB_HD uint32_t overlay_block10(uint32_t p0, uint32_t p1, uint32_t p2, uint32_t 
 template <int E, bool Msb>
 GLB_HD uint32_t overlay_px10(uint32_t px, uint32_t cb, uint32_t cr) { return overlay_block10<E, Msb>(px, px, px, px, cb, cr); }
 
+// ---- overlay onto HDR pictures (DESIGN 4.22) ------------------------------------------------------------------------------
+// The blend happens in the picture's code domain, as at SDR, from each pixel's straight colour S (export_straight_px) and its
+// alpha a: Y = round((a Y_f(S) + (255 - a) Y_D) / 255), Y_f the unrounded code; the chroma of n pixels (a 2x2 block, a
+// pair as the block (p0, p1, p0, p1), one pixel as the block of four) with A = sum a_i is round(512 + sum a_i (C_f(S_i) -
+// 512) / (255 n) + (1 - A / (255 n)) (C_D - 512)), taken as the chroma of the weighted mean P = sum (a_i / 255) E'_i / n
+// (linear in E') plus (1 - A / (255 n)) (C_D - 512).  An opaque pixel (block) has weights 1 and 0 exactly, so it gives the
+// HDR export's codes bit for bit; zero pixels and blocks are left to the callers, which keep their samples.
+struct HdrPx { HdrRgb e; float w; };                        // E' of the straight colour, and a / 255
+template <int E>
+GLB_HD HdrPx hdr_px(uint32_t px) { return { hdr_rgb<E>(export_straight_px(px)), glm_div((float) (px >> 24), 255.0f) }; }
+// the Y code of pixel p over the code yd
+GLB_HD uint32_t hdr_over_y(const HdrPx& p, uint32_t yd) {
+    const uint32_t v = hdr_code(glm_add(glm_mul(hdr_yf(p.e), p.w), glm_mul((float) yd, glm_add(1.0f, -p.w))));
+    return v > 1023u ? 1023u : v;
+}
+// the (Cb, Cr) codes, Cb low, of the block a, b (top row), c, d over the codes cbd, crd
+GLB_HD uint32_t hdr_over_cbcr(const HdrPx& a, const HdrPx& b, const HdrPx& c, const HdrPx& d, uint32_t cbd, uint32_t crd) {
+    const HdrRgb m = hdr_mean4({ glm_mul(a.e.r, a.w), glm_mul(a.e.g, a.w), glm_mul(a.e.b, a.w) },
+                               { glm_mul(b.e.r, b.w), glm_mul(b.e.g, b.w), glm_mul(b.e.b, b.w) },
+                               { glm_mul(c.e.r, c.w), glm_mul(c.e.g, c.w), glm_mul(c.e.b, c.w) },
+                               { glm_mul(d.e.r, d.w), glm_mul(d.e.g, d.w), glm_mul(d.e.b, d.w) });
+    const float k = glm_add(1.0f, -glm_mul(glm_add(glm_add(a.w, b.w), glm_add(c.w, d.w)), 0.25f));
+    const uint32_t cb = hdr_code(glm_add(hdr_cbf(m), glm_mul(k, glm_add((float) cbd, -512.0f))));
+    const uint32_t cr = hdr_code(glm_add(hdr_crf(m), glm_mul(k, glm_add((float) crd, -512.0f))));
+    return (cb > 1023u ? 1023u : cb) | ((cr > 1023u ? 1023u : cr) << 16);
+}
+// Y of pixel px (E' and weight p) over sample v: a zero pixel keeps all 16 bits
+template <bool Msb>
+GLB_HD uint32_t hdr_over_y_sample(uint32_t px, const HdrPx& p, uint32_t v) {
+    return px ? overlay_sample10<Msb>(hdr_over_y(p, overlay_code10<Msb>(v))) : v & 0xffffu;
+}
+
 // I420 of a quad (rows 2j and 2j + 1) over the Y words yt / yb and the Cb and Cr pairs cb / cr (two bytes each): NV12's
 // overlay_nv12_quad on the interleaved pairs, so I420 is NV12 deinterleaved bit for bit
 template <int E = 0>
@@ -822,53 +1047,101 @@ GLB_HD void overlay_444_quad(const uint32_t in[4], uint32_t* y, uint32_t* cb, ui
 // P010 uv[2], one (Cb, Cr) word per block; YUV420P10 uv[0] the two Cb samples, uv[1] the two Cr samples
 template <int E, bool Msb>
 GLB_HD void overlay_p10_quad(const uint32_t top[4], const uint32_t bot[4], uint32_t yt[2], uint32_t yb[2], uint32_t uv[2]) {
+    if constexpr (E >= GLB_ENC_PQ) {                        // DESIGN 4.22: each pixel's E' once
+        HdrPx t[4], b[4];
 #pragma unroll
-    for (int k = 0; k < 2; ++k) {
-        yt[k] = overlay_y10_word<E, Msb>(top[2 * k], top[2 * k + 1], yt[k]);
-        yb[k] = overlay_y10_word<E, Msb>(bot[2 * k], bot[2 * k + 1], yb[k]);
-    }
-    if (Msb) {
+        for (int k = 0; k < 4; ++k) { t[k] = hdr_px<E>(top[k]); b[k] = hdr_px<E>(bot[k]); }
 #pragma unroll
-        for (int k = 0; k < 2; ++k) uv[k] = overlay_block10<E, true>(top[2 * k], top[2 * k + 1], bot[2 * k], bot[2 * k + 1], uv[k], uv[k] >> 16);
-    } else {
-        // sample by sample: packing both blocks' results through overlay_block10's words let nvcc 12.9 (sm_90a) merge a
-        // kept Cr sample's bits into the blended one; tests/test_gpu_overlay_planes.py pins the result on the device
+        for (int k = 0; k < 2; ++k) {
+            yt[k] = hdr_over_y_sample<Msb>(top[2 * k], t[2 * k], yt[k]) | (hdr_over_y_sample<Msb>(top[2 * k + 1], t[2 * k + 1], yt[k] >> 16) << 16);
+            yb[k] = hdr_over_y_sample<Msb>(bot[2 * k], b[2 * k], yb[k]) | (hdr_over_y_sample<Msb>(bot[2 * k + 1], b[2 * k + 1], yb[k] >> 16) << 16);
+        }
+        // sample by sample, as the planar chroma below: P010 uv[k] is block k's (Cb, Cr) word, YUV420P10 uv[0] / uv[1] the
+        // two Cb / Cr samples
         uint32_t cb[2], cr[2];
 #pragma unroll
         for (int k = 0; k < 2; ++k) {
-            cb[k] = (uv[0] >> (16 * k)) & 0xffffu;
-            cr[k] = (uv[1] >> (16 * k)) & 0xffffu;
+            cb[k] = Msb ? uv[k] & 0xffffu : (uv[0] >> (16 * k)) & 0xffffu;
+            cr[k] = Msb ? uv[k] >> 16 : (uv[1] >> (16 * k)) & 0xffffu;
             if ((top[2 * k] | top[2 * k + 1] | bot[2 * k] | bot[2 * k + 1]) != 0u) {
-                const uint32_t c = overlay_cbcr10<E>(export_sum4(top[2 * k], top[2 * k + 1], bot[2 * k], bot[2 * k + 1]),
-                                                     overlay_asum4(top[2 * k], top[2 * k + 1], bot[2 * k], bot[2 * k + 1]),
-                                                     cb[k] & 1023u, cr[k] & 1023u);
-                cb[k] = c & 0xffffu;
-                cr[k] = c >> 16;
+                const uint32_t c = hdr_over_cbcr(t[2 * k], t[2 * k + 1], b[2 * k], b[2 * k + 1], overlay_code10<Msb>(cb[k]),
+                                                 overlay_code10<Msb>(cr[k]));
+                cb[k] = overlay_sample10<Msb>(c & 0xffffu);
+                cr[k] = overlay_sample10<Msb>(c >> 16);
             }
         }
-        uv[0] = cb[0] | (cb[1] << 16);
-        uv[1] = cr[0] | (cr[1] << 16);
+        if (Msb) { uv[0] = cb[0] | (cr[0] << 16); uv[1] = cb[1] | (cr[1] << 16); }
+        else { uv[0] = cb[0] | (cb[1] << 16); uv[1] = cr[0] | (cr[1] << 16); }
+    } else {
+    #pragma unroll
+        for (int k = 0; k < 2; ++k) {
+            yt[k] = overlay_y10_word<E, Msb>(top[2 * k], top[2 * k + 1], yt[k]);
+            yb[k] = overlay_y10_word<E, Msb>(bot[2 * k], bot[2 * k + 1], yb[k]);
+        }
+        if (Msb) {
+    #pragma unroll
+            for (int k = 0; k < 2; ++k) uv[k] = overlay_block10<E, true>(top[2 * k], top[2 * k + 1], bot[2 * k], bot[2 * k + 1], uv[k], uv[k] >> 16);
+        } else {
+            // sample by sample: packing both blocks' results through overlay_block10's words let nvcc 12.9 (sm_90a) merge a
+            // kept Cr sample's bits into the blended one; tests/test_gpu_overlay_planes.py pins the result on the device
+            uint32_t cb[2], cr[2];
+    #pragma unroll
+            for (int k = 0; k < 2; ++k) {
+                cb[k] = (uv[0] >> (16 * k)) & 0xffffu;
+                cr[k] = (uv[1] >> (16 * k)) & 0xffffu;
+                if ((top[2 * k] | top[2 * k + 1] | bot[2 * k] | bot[2 * k + 1]) != 0u) {
+                    const uint32_t c = overlay_cbcr10<E>(export_sum4(top[2 * k], top[2 * k + 1], bot[2 * k], bot[2 * k + 1]),
+                                                         overlay_asum4(top[2 * k], top[2 * k + 1], bot[2 * k], bot[2 * k + 1]),
+                                                         cb[k] & 1023u, cr[k] & 1023u);
+                    cb[k] = c & 0xffffu;
+                    cr[k] = c >> 16;
+                }
+            }
+            uv[0] = cb[0] | (cb[1] << 16);
+            uv[1] = cr[0] | (cr[1] << 16);
+        }
     }
 }
 // YUV444P10 of one row's quad over the Y, Cb and Cr words y[2], cb[2], cr[2] (two samples each)
 template <int E = 0>
 GLB_HD void overlay_444p10_quad(const uint32_t in[4], uint32_t y[2], uint32_t cb[2], uint32_t cr[2]) {
+    if constexpr (E >= GLB_ENC_PQ) {                        // DESIGN 4.22: each pixel's chroma its own block of four
+        uint32_t oy[4], u[4], v[4];
 #pragma unroll
-    for (int k = 0; k < 2; ++k) y[k] = overlay_y10_word<E, false>(in[2 * k], in[2 * k + 1], y[k]);
-    // sample by sample, as overlay_p10_quad's planar chroma
-    uint32_t u[4], v[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        u[k] = (cb[k >> 1] >> (16 * (k & 1))) & 0xffffu;
-        v[k] = (cr[k >> 1] >> (16 * (k & 1))) & 0xffffu;
-        if (in[k]) {
-            const uint32_t c = overlay_cbcr10<E>(export_sum4(in[k], in[k], in[k], in[k]), 4u * (in[k] >> 24), u[k] & 1023u, v[k] & 1023u);
-            u[k] = c & 0xffffu;
-            v[k] = c >> 16;
+        for (int k = 0; k < 4; ++k) {
+            const uint32_t ys = (y[k >> 1] >> (16 * (k & 1))) & 0xffffu;
+            u[k] = (cb[k >> 1] >> (16 * (k & 1))) & 0xffffu;
+            v[k] = (cr[k >> 1] >> (16 * (k & 1))) & 0xffffu;
+            oy[k] = ys;
+            if (in[k]) {
+                const HdrPx p = hdr_px<E>(in[k]);
+                oy[k] = hdr_over_y(p, ys & 1023u);
+                const uint32_t c = hdr_over_cbcr(p, p, p, p, u[k] & 1023u, v[k] & 1023u);
+                u[k] = c & 0xffffu;
+                v[k] = c >> 16;
+            }
         }
+        y[0] = oy[0] | (oy[1] << 16); y[1] = oy[2] | (oy[3] << 16);
+        cb[0] = u[0] | (u[1] << 16); cb[1] = u[2] | (u[3] << 16);
+        cr[0] = v[0] | (v[1] << 16); cr[1] = v[2] | (v[3] << 16);
+    } else {
+    #pragma unroll
+        for (int k = 0; k < 2; ++k) y[k] = overlay_y10_word<E, false>(in[2 * k], in[2 * k + 1], y[k]);
+        // sample by sample, as overlay_p10_quad's planar chroma
+        uint32_t u[4], v[4];
+    #pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            u[k] = (cb[k >> 1] >> (16 * (k & 1))) & 0xffffu;
+            v[k] = (cr[k >> 1] >> (16 * (k & 1))) & 0xffffu;
+            if (in[k]) {
+                const uint32_t c = overlay_cbcr10<E>(export_sum4(in[k], in[k], in[k], in[k]), 4u * (in[k] >> 24), u[k] & 1023u, v[k] & 1023u);
+                u[k] = c & 0xffffu;
+                v[k] = c >> 16;
+            }
+        }
+        cb[0] = u[0] | (u[1] << 16); cb[1] = u[2] | (u[3] << 16);
+        cr[0] = v[0] | (v[1] << 16); cr[1] = v[2] | (v[3] << 16);
     }
-    cb[0] = u[0] | (u[1] << 16); cb[1] = u[2] | (u[3] << 16);
-    cr[0] = v[0] | (v[1] << 16); cr[1] = v[2] | (v[3] << 16);
 }
 
 // ---- overlay onto 4:2:2 pictures (DESIGN 4.18) ----------------------------------------------------------------------------
@@ -889,22 +1162,44 @@ GLB_HD void overlay_422_quad(const uint32_t in[4], uint32_t* y, uint32_t* uv) {
 // sample, as overlay_p10_quad's planar chroma
 template <int E = 0>
 GLB_HD void overlay_422p10_quad(const uint32_t in[4], uint32_t y[2], uint32_t* cb, uint32_t* cr) {
+    if constexpr (E >= GLB_ENC_PQ) {                        // DESIGN 4.22: each pixel's E' once, a pair's chroma its block's
+        HdrPx p[4];
 #pragma unroll
-    for (int k = 0; k < 2; ++k) y[k] = overlay_y10_word<E, false>(in[2 * k], in[2 * k + 1], y[k]);
-    uint32_t u[2], v[2];
+        for (int k = 0; k < 4; ++k) p[k] = hdr_px<E>(in[k]);
 #pragma unroll
-    for (int k = 0; k < 2; ++k) {
-        const uint32_t p0 = in[2 * k], p1 = in[2 * k + 1];
-        u[k] = (*cb >> (16 * k)) & 0xffffu;
-        v[k] = (*cr >> (16 * k)) & 0xffffu;
-        if ((p0 | p1) != 0u) {
-            const uint32_t c = overlay_cbcr10<E>(export_sum4(p0, p1, p0, p1), overlay_asum4(p0, p1, p0, p1), u[k] & 1023u, v[k] & 1023u);
-            u[k] = c & 0xffffu;
-            v[k] = c >> 16;
+        for (int k = 0; k < 2; ++k)
+            y[k] = hdr_over_y_sample<false>(in[2 * k], p[2 * k], y[k]) | (hdr_over_y_sample<false>(in[2 * k + 1], p[2 * k + 1], y[k] >> 16) << 16);
+        uint32_t u[2], v[2];
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+            u[k] = (*cb >> (16 * k)) & 0xffffu;
+            v[k] = (*cr >> (16 * k)) & 0xffffu;
+            if ((in[2 * k] | in[2 * k + 1]) != 0u) {
+                const uint32_t c = hdr_over_cbcr(p[2 * k], p[2 * k + 1], p[2 * k], p[2 * k + 1], u[k] & 1023u, v[k] & 1023u);
+                u[k] = c & 0xffffu;
+                v[k] = c >> 16;
+            }
         }
+        *cb = u[0] | (u[1] << 16);
+        *cr = v[0] | (v[1] << 16);
+    } else {
+    #pragma unroll
+        for (int k = 0; k < 2; ++k) y[k] = overlay_y10_word<E, false>(in[2 * k], in[2 * k + 1], y[k]);
+        uint32_t u[2], v[2];
+    #pragma unroll
+        for (int k = 0; k < 2; ++k) {
+            const uint32_t p0 = in[2 * k], p1 = in[2 * k + 1];
+            u[k] = (*cb >> (16 * k)) & 0xffffu;
+            v[k] = (*cr >> (16 * k)) & 0xffffu;
+            if ((p0 | p1) != 0u) {
+                const uint32_t c = overlay_cbcr10<E>(export_sum4(p0, p1, p0, p1), overlay_asum4(p0, p1, p0, p1), u[k] & 1023u, v[k] & 1023u);
+                u[k] = c & 0xffffu;
+                v[k] = c >> 16;
+            }
+        }
+        *cb = u[0] | (u[1] << 16);
+        *cr = v[0] | (v[1] << 16);
     }
-    *cb = u[0] | (u[1] << 16);
-    *cr = v[0] | (v[1] << 16);
 }
 
 }  // namespace glb

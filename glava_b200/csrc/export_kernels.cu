@@ -333,6 +333,14 @@ static void for_any_enc(int enc, F&& f) {
     else for_enc(enc, f);
 }
 
+// f(std::integral_constant<int, E>()) for the HDR encoding E = enc, 4 (PQ) or 5 (HLG) (DESIGN 4.22): the launchers route
+// these to new instantiations of the 10-bit kernels before for_enc / for_any_enc, so no existing kernel sees them
+template <typename F>
+static void for_hdr(int enc, F&& f) {
+    if (enc == GLB_ENC_PQ) f(std::integral_constant<int, GLB_ENC_PQ>());
+    else f(std::integral_constant<int, GLB_ENC_HLG>());
+}
+
 // the first n (1..4) uint16 samples of the words v[0], v[1] at p (n == 4: p is 8-byte aligned); the tail is written out,
 // since indexing v by a run-time sample number puts the words on the stack
 __device__ __forceinline__ void store_u16(uint8_t* p, const uint32_t v[2], int n) {
@@ -636,9 +644,27 @@ static void launch_yuva(const ExportArgs& a, unsigned blocks, cudaStream_t st) {
     });
 }
 
+// ---- BT.2020 HDR (DESIGN 4.22): P010, YUV420P10, YUV444P10 and YUV422P10 under E = 4 / 5 -------------------------------
+// The 10-bit kernels' own items, instantiated for the HDR encodings (export_core.h's quads branch on E at compile time)
+template <typename Index, int E>
+static void launch_hdr(const ExportArgs& a, unsigned blocks, cudaStream_t st) {
+    if (a.format == GLAVA_B200_EXPORT_P010) export_yuv_enc_kernel<Index, GLAVA_B200_EXPORT_P010, E><<<blocks, 256, 0, st>>>(a);
+    else if (a.format == GLAVA_B200_EXPORT_YUV420P10) export_p10_kernel<Index, GLAVA_B200_EXPORT_YUV420P10, E><<<blocks, 256, 0, st>>>(a);
+    else if (a.format == GLAVA_B200_EXPORT_YUV444P10) export_p10_kernel<Index, GLAVA_B200_EXPORT_YUV444P10, E><<<blocks, 256, 0, st>>>(a);
+    else export_422_kernel<Index, GLAVA_B200_EXPORT_YUV422P10, E><<<blocks, 256, 0, st>>>(a);
+}
+
 int launch_export(const ExportArgs& a, void* stream) {
     const ExportGrid g = export_grid((uint64_t) a.count * (uint64_t) ((a.w + 127) >> 7) * (uint64_t) ((a.h + 1) >> 1));
     cudaStream_t st = (cudaStream_t) stream;
+    if (a.enc >= GLB_ENC_PQ) {
+        for_hdr(a.enc, [&](auto e) {
+            constexpr int E = decltype(e)::value;
+            if (g.narrow) launch_hdr<uint32_t, E>(a, g.blocks, st);
+            else launch_hdr<uint64_t, E>(a, g.blocks, st);
+        });
+        return launch_status("export");
+    }
     if (export_alpha(a.format)) {
         if (g.narrow) launch_yuva<uint32_t>(a, g.blocks, st);
         else launch_yuva<uint64_t>(a, g.blocks, st);
@@ -810,7 +836,7 @@ __device__ __forceinline__ void scaled_yuv_item(const A& a, const ExportFmt& f, 
         __stcs(reinterpret_cast<unsigned short*>(r0), (unsigned short) (export_y10<E>(top) << 6));
         __stcs(reinterpret_cast<unsigned short*>(r0 + a.pitch), (unsigned short) (export_y10<E>(bot) << 6));
         if (!(lane & 1))
-            __stcs(reinterpret_cast<uint32_t*>(cb + (size_t) u * a.pitch + 2 * X), export_cbcr10<E>(export_sum4(top, top1, bot, bot1)) << 6);
+            __stcs(reinterpret_cast<uint32_t*>(cb + (size_t) u * a.pitch + 2 * X), export_block10<E>(top, top1, bot, bot1) << 6);
     }
 }
 
@@ -883,7 +909,7 @@ __device__ __forceinline__ void scaled_p10_item(const A& a, const ExportFmt& f, 
     __stcs(reinterpret_cast<unsigned short*>(r0), (unsigned short) export_y10<E>(top));
     __stcs(reinterpret_cast<unsigned short*>(r0 + a.pitch), (unsigned short) export_y10<E>(bot));
     if (!(lane & 1)) {
-        const uint32_t uv = export_cbcr10<E>(export_sum4(top, top1, bot, bot1));
+        const uint32_t uv = export_block10<E>(top, top1, bot, bot1);
         uint8_t* const pu = cb + (size_t) u * (a.pitch >> 1) + X;   // X / 2 samples of 2 bytes
         __stcs(reinterpret_cast<unsigned short*>(pu), (unsigned short) uv);
         __stcs(reinterpret_cast<unsigned short*>(pu + cr), (unsigned short) (uv >> 16));
@@ -950,7 +976,7 @@ __device__ __forceinline__ void scaled_422_item(const A& a, const ExportFmt& f, 
     } else {                                                // YUV422P10
         __stcs(reinterpret_cast<unsigned short*>(dst + (size_t) u * a.pitch + 2 * (size_t) X), (unsigned short) export_y10<E>(px));
         if (!(lane & 1)) {
-            const uint32_t uv = export_cbcr10<E>(export_sum4(px, px1, px, px1));
+            const uint32_t uv = export_block10<E>(px, px1, px, px1);
             uint8_t* const pu = cb + (size_t) u * (a.pitch >> 1) + X;   // X / 2 samples of 2 bytes
             __stcs(reinterpret_cast<unsigned short*>(pu), (unsigned short) uv);
             __stcs(reinterpret_cast<unsigned short*>(pu + cr), (unsigned short) (uv >> 16));
@@ -1064,10 +1090,27 @@ static void launch_scaled_yuva(const ScaledArgs& a, unsigned blocks, cudaStream_
     });
 }
 
+// the scaled 10-bit kernels under an HDR encoding (DESIGN 4.22), as launch_hdr
+template <typename Index, int E>
+static void launch_scaled_hdr(const ScaledArgs& a, unsigned blocks, cudaStream_t st) {
+    if (a.format == GLAVA_B200_EXPORT_P010) export_scaled_yuv_enc_kernel<Index, GLAVA_B200_EXPORT_P010, E><<<blocks, 256, 0, st>>>(a);
+    else if (a.format == GLAVA_B200_EXPORT_YUV420P10) export_scaled_p10_kernel<Index, GLAVA_B200_EXPORT_YUV420P10, E><<<blocks, 256, 0, st>>>(a);
+    else if (a.format == GLAVA_B200_EXPORT_YUV444P10) export_scaled_p10_kernel<Index, GLAVA_B200_EXPORT_YUV444P10, E><<<blocks, 256, 0, st>>>(a);
+    else export_scaled_422_kernel<Index, GLAVA_B200_EXPORT_YUV422P10, E><<<blocks, 256, 0, st>>>(a);
+}
+
 int launch_export_scaled(const ScaledArgs& a, void* stream) {
     const uint64_t units = export_420(a.format) ? (uint64_t) (a.out_h >> 1) : (uint64_t) a.out_h;
     const ExportGrid g = export_grid((uint64_t) a.count * (uint64_t) ((a.out_w + 31) >> 5) * units);
     cudaStream_t st = (cudaStream_t) stream;
+    if (a.enc >= GLB_ENC_PQ) {
+        for_hdr(a.enc, [&](auto e) {
+            constexpr int E = decltype(e)::value;
+            if (g.narrow) launch_scaled_hdr<uint32_t, E>(a, g.blocks, st);
+            else launch_scaled_hdr<uint64_t, E>(a, g.blocks, st);
+        });
+        return launch_status("scaled export");
+    }
     if (export_alpha(a.format)) {
         if (g.narrow) launch_scaled_yuva<uint32_t>(a, g.blocks, st);
         else launch_scaled_yuva<uint64_t>(a, g.blocks, st);
@@ -1381,13 +1424,65 @@ __global__ void __launch_bounds__(256) export_ladder_yuva_kernel(const __grid_co
     }
 }
 
+// One unit of export_ladder_hdr_kernel under the HDR encoding E (DESIGN 4.22): the item of its rung's standalone kernel
+// (P010: export_yuv_enc_kernel's; the planar 10-bit formats: export_p10_kernel's; YUV422P10: export_422_kernel's, or their
+// scaled forms) in that kernel's HDR instantiation
+template <int E>
+__device__ __forceinline__ void ladder_hdr_item(const LadderArgs& a, const LadderRung& g, const ExportEntryUV* e, int rung, int row,
+                                                int col, int lane) {
+    if (export_422(g.format)) ladder_422_item<E>(a, g, e, rung, row, col, lane);
+    else if (export_p10(g.format)) ladder_p10_item<E>(a, g, e, rung, row, col, lane);
+    else ladder_item<true, E>(a, g, e, rung, row, col, lane);
+}
+
+// Any format and encoding per rung, launched only when a rung is HDR (DESIGN 4.22): HDR units run ladder_hdr_item, every
+// other unit what export_ladder_yuva_kernel runs for it, so that HDR and SDR rungs mix in one launch and the older ladder
+// kernels keep their machine code
+template <typename Index>
+__global__ void __launch_bounds__(256) export_ladder_hdr_kernel(const __grid_constant__ LadderArgs a) {
+    const Index units = (Index) a.units, items = (Index) a.count * units;
+    const Index warps = (Index) (((size_t) gridDim.x * blockDim.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    for (Index it = (Index) (((size_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5); it < items; it += warps) {
+        const Index k = it / units;
+        const uint64_t unit = __ldg(reinterpret_cast<const unsigned long long*>(a.sched) + (it - k * units));
+        const int rung = ladder_unit_rung(unit), row = ladder_unit_row(unit), col = ladder_unit_col(unit);
+        const LadderRung& g = a.rung[rung];
+        const ExportEntryUV* e = a.list + (size_t) k * a.nrungs + rung;
+        if (g.enc == GLB_ENC_PQ) ladder_hdr_item<GLB_ENC_PQ>(a, g, e, rung, row, col, lane);
+        else if (g.enc == GLB_ENC_HLG) ladder_hdr_item<GLB_ENC_HLG>(a, g, e, rung, row, col, lane);
+        else if (export_alpha(g.format)) {
+            if (g.enc == 1) ladder_yuva_item<1>(a, g, e, rung, row, col, lane);
+            else if (g.enc == 2) ladder_yuva_item<2>(a, g, e, rung, row, col, lane);
+            else if (g.enc == 3) ladder_yuva_item<3>(a, g, e, rung, row, col, lane);
+            else ladder_yuva_item<0>(a, g, e, rung, row, col, lane);
+        } else if (export_422(g.format)) {
+            if (g.enc == 1) ladder_422_item<1>(a, g, e, rung, row, col, lane);
+            else if (g.enc == 2) ladder_422_item<2>(a, g, e, rung, row, col, lane);
+            else if (g.enc == 3) ladder_422_item<3>(a, g, e, rung, row, col, lane);
+            else ladder_422_item<0>(a, g, e, rung, row, col, lane);
+        } else if (export_p10(g.format)) {
+            if (g.enc == 1) ladder_p10_item<1>(a, g, e, rung, row, col, lane);
+            else if (g.enc == 2) ladder_p10_item<2>(a, g, e, rung, row, col, lane);
+            else if (g.enc == 3) ladder_p10_item<3>(a, g, e, rung, row, col, lane);
+            else ladder_p10_item<0>(a, g, e, rung, row, col, lane);
+        } else if (g.enc == 1) ladder_item<true, 1>(a, g, e, rung, row, col, lane);
+        else if (g.enc == 2) ladder_item<true, 2>(a, g, e, rung, row, col, lane);
+        else if (g.enc == 3) ladder_item<true, 3>(a, g, e, rung, row, col, lane);
+        else ladder_item<true, 0>(a, g, e, rung, row, col, lane);
+    }
+}
+
 int launch_export_ladder(const LadderArgs& a, void* stream) {
     const ExportGrid g = export_grid((uint64_t) a.count * (uint64_t) a.units);
     int format[GLAVA_B200_LADDER_MAX], enc[GLAVA_B200_LADDER_MAX];
     for (int j = 0; j < a.nrungs; ++j) { format[j] = a.rung[j].format; enc[j] = a.rung[j].enc; }
     const int kind = ladder_kernel(format, enc, a.nrungs);
     cudaStream_t st = (cudaStream_t) stream;
-    if (kind == ladder_yuva) {
+    if (kind == ladder_hdr) {
+        if (g.narrow) export_ladder_hdr_kernel<uint32_t><<<g.blocks, 256, 0, st>>>(a);
+        else export_ladder_hdr_kernel<uint64_t><<<g.blocks, 256, 0, st>>>(a);
+    } else if (kind == ladder_yuva) {
         if (g.narrow) export_ladder_yuva_kernel<uint32_t><<<g.blocks, 256, 0, st>>>(a);
         else export_ladder_yuva_kernel<uint64_t><<<g.blocks, 256, 0, st>>>(a);
     } else if (kind == ladder_422) {
@@ -1900,10 +1995,23 @@ static void launch_planes(const OverlayPlanesArgs& a, const ExportGrid& g, cudaS
     });
 }
 
+template <int Fmt>
+static void launch_planes_hdr(const OverlayPlanesArgs& a, const ExportGrid& g, cudaStream_t st);   // DESIGN 4.22, below
+
 int launch_overlay_planes(const OverlayPlanesArgs& a, void* stream) {
     const int rows = a.band ? a.mark_rows : 2;
     const ExportGrid g = export_grid((uint64_t) a.count * (uint64_t) ((a.w + 127) >> 7) * (uint64_t) ((a.h + rows - 1) / rows));
     cudaStream_t st = (cudaStream_t) stream;
+    if (a.enc >= GLB_ENC_PQ) {
+        switch (a.format) {
+        case GLAVA_B200_EXPORT_P010: launch_planes_hdr<GLAVA_B200_EXPORT_P010>(a, g, st); break;
+        case GLAVA_B200_EXPORT_YUV420P10: launch_planes_hdr<GLAVA_B200_EXPORT_YUV420P10>(a, g, st); break;
+        case GLAVA_B200_EXPORT_YUV444P10: launch_planes_hdr<GLAVA_B200_EXPORT_YUV444P10>(a, g, st); break;
+        case GLAVA_B200_EXPORT_YUV422P10: launch_planes_hdr<GLAVA_B200_EXPORT_YUV422P10>(a, g, st); break;
+        default: return fail(GLAVA_B200_EINVAL, "planes overlay launch: HDR on format %d", a.format);
+        }
+        return launch_status("planes overlay");
+    }
     switch (a.format) {
     case GLAVA_B200_EXPORT_NV12: launch_planes<GLAVA_B200_EXPORT_NV12>(a, g, st); break;
     case GLAVA_B200_EXPORT_I420: launch_planes<GLAVA_B200_EXPORT_I420>(a, g, st); break;
@@ -2031,6 +2139,29 @@ static void launch_planes_fade(const OverlayPlanesArgs& a, const ExportGrid& g, 
     });
 }
 
+// the 10-bit formats' plain and fade kernels under an HDR encoding (DESIGN 4.22)
+template <int Fmt>
+static void launch_planes_hdr(const OverlayPlanesArgs& a, const ExportGrid& g, cudaStream_t st) {
+    for_hdr(a.enc, [&](auto e) {
+        constexpr int E = decltype(e)::value;
+        if (a.fade) {
+            if (a.band) {
+                if (g.narrow) overlay_planes_fade_kernel<uint32_t, true, Fmt, E><<<g.blocks, 256, 0, st>>>(a);
+                else overlay_planes_fade_kernel<uint64_t, true, Fmt, E><<<g.blocks, 256, 0, st>>>(a);
+            } else {
+                if (g.narrow) overlay_planes_fade_kernel<uint32_t, false, Fmt, E><<<g.blocks, 256, 0, st>>>(a);
+                else overlay_planes_fade_kernel<uint64_t, false, Fmt, E><<<g.blocks, 256, 0, st>>>(a);
+            }
+        } else if (a.band) {
+            if (g.narrow) overlay_planes_kernel<uint32_t, true, Fmt, E><<<g.blocks, 256, 0, st>>>(a);
+            else overlay_planes_kernel<uint64_t, true, Fmt, E><<<g.blocks, 256, 0, st>>>(a);
+        } else {
+            if (g.narrow) overlay_planes_kernel<uint32_t, false, Fmt, E><<<g.blocks, 256, 0, st>>>(a);
+            else overlay_planes_kernel<uint64_t, false, Fmt, E><<<g.blocks, 256, 0, st>>>(a);
+        }
+    });
+}
+
 // ---- glava_b200_overlay_scaled (DESIGN 4.21) ---------------------------------------------------------------------------------
 // The overlay of a downscaled, cropped frame.  Items are export_scaled_kernel's: (entry, output row — 4:2:0: row pair —, run
 // of 32 output columns), one warp each, lane = output column, every pixel scaled_px's exact area average with its mark-aware
@@ -2101,11 +2232,31 @@ static void launch_scaled_overlay(const OverlayScaledArgs& a, const ExportGrid& 
     });
 }
 
+// the 10-bit formats' kernels under an HDR encoding (DESIGN 4.22)
+template <int Fmt>
+static void launch_scaled_overlay_hdr(const OverlayScaledArgs& a, const ExportGrid& g, cudaStream_t st) {
+    for_hdr(a.enc, [&](auto e) {
+        constexpr int E = decltype(e)::value;
+        if (g.narrow) overlay_scaled_kernel<uint32_t, Fmt, E><<<g.blocks, 256, 0, st>>>(a);
+        else overlay_scaled_kernel<uint64_t, Fmt, E><<<g.blocks, 256, 0, st>>>(a);
+    });
+}
+
 int launch_overlay_scaled(const OverlayScaledArgs& a, void* stream) {
     const bool pairs = export_420(a.format);
     const ExportGrid g = export_grid((uint64_t) a.count * (uint64_t) ((a.out_w + 31) >> 5) *
                                      (uint64_t) (pairs ? a.out_h >> 1 : a.out_h));
     cudaStream_t st = (cudaStream_t) stream;
+    if (a.enc >= GLB_ENC_PQ) {
+        switch (a.format) {
+        case GLAVA_B200_EXPORT_P010: launch_scaled_overlay_hdr<GLAVA_B200_EXPORT_P010>(a, g, st); break;
+        case GLAVA_B200_EXPORT_YUV420P10: launch_scaled_overlay_hdr<GLAVA_B200_EXPORT_YUV420P10>(a, g, st); break;
+        case GLAVA_B200_EXPORT_YUV444P10: launch_scaled_overlay_hdr<GLAVA_B200_EXPORT_YUV444P10>(a, g, st); break;
+        case GLAVA_B200_EXPORT_YUV422P10: launch_scaled_overlay_hdr<GLAVA_B200_EXPORT_YUV422P10>(a, g, st); break;
+        default: return fail(GLAVA_B200_EINVAL, "scaled overlay launch: HDR on format %d", a.format);
+        }
+        return launch_status("scaled overlay");
+    }
     switch (a.format) {
     case GLAVA_B200_EXPORT_RGBA:
     case GLAVA_B200_EXPORT_BGRA:

@@ -151,6 +151,8 @@ int ladder_run(glava_b200* r, const int* streams, int count, const glava_b200_ex
             case 1: z = rung_zero<1>(f, &g); break;
             case 2: z = rung_zero<2>(f, &g); break;
             case 3: z = rung_zero<3>(f, &g); break;
+            case GLB_ENC_PQ: z = rung_zero<GLB_ENC_PQ>(f, &g); break;
+            case GLB_ENC_HLG: z = rung_zero<GLB_ENC_HLG>(f, &g); break;
             default: z = rung_zero<0>(f, &g); break;
             }
             a.yuv[j] = { planes[j].cr, z.y, z.u, z.v, z.a };

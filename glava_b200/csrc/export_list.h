@@ -44,6 +44,8 @@ uint32_t background(const glava_b200_export& d);
 // (export.cpp, shared with overlay_planes.cpp) a destination pointer: null, 16-byte alignment, device memory, the
 // renderer's device; `name`[i] names it in the message
 int dst_check(const RendererView& v, const void* p, const char* name, int i, const char* who);
+// the HDR bits of a descriptor that has one (export.cpp, DESIGN 4.22)
+int hdr_flags_check(int format, uint32_t flags, const char* who);
 // One plane of one entry's rectangle: `rows` rows of the common row bytes, the common pitch apart, from byte address p
 struct Rect { uintptr_t p; size_t rows; int entry; bool uv; };
 // Two rectangles of one pitch P and row bytes B, a starting first (a.p <= b.p): whether any rows meet

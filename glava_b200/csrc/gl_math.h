@@ -55,6 +55,14 @@ GLM_FN float glm_div(float a, float b) {
     return a / b;
 #endif
 }
+/* correctly rounded square root (IEEE-754 requires it of both) */
+GLM_FN float glm_sqrt(float x) {
+#if defined(__CUDA_ARCH__)
+    return __fsqrt_rn(x);
+#else
+    return sqrtf(x);
+#endif
+}
 GLM_FN uint32_t glm_f2u(float f) {
 #if defined(__CUDA_ARCH__)
     return __float_as_uint(f);

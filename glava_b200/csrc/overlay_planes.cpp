@@ -50,9 +50,14 @@ int planes_geometry(int w, int h, const glava_b200_overlay_planes_desc& d, Plane
     const char* name = planes_format_name(fmt);
     if (!name) return fail(GLAVA_B200_EINVAL, "%s: unknown format %d", who, fmt);
     const uint32_t colour = GLAVA_B200_EXPORT_FULL_RANGE | GLAVA_B200_EXPORT_BT601;
+    const uint32_t hdr = GLAVA_B200_EXPORT_PQ | GLAVA_B200_EXPORT_HLG;   // the picture's HDR encoding (DESIGN 4.22)
     if (d.flags & GLAVA_B200_EXPORT_STRAIGHT)
         return fail(GLAVA_B200_EINVAL, "%s: flags 0x%x: EXPORT_STRAIGHT is for the exports; the overlay composites", who, d.flags);
-    if (d.flags & ~colour)
+    if (d.flags & hdr) {
+        const int rc = hdr_flags_check(fmt, d.flags, who);
+        if (rc) return rc;
+    }
+    if (d.flags & ~(colour | hdr))
         return fail(GLAVA_B200_EINVAL, "%s: flags 0x%x: the overlay takes none but EXPORT_FULL_RANGE and EXPORT_BT601", who, d.flags);
     if (packed && (d.flags & colour))
         return fail(GLAVA_B200_EINVAL, "%s: flags 0x%x: %s has no matrix or range (EXPORT_FULL_RANGE and EXPORT_BT601 are for the "

@@ -421,6 +421,14 @@ int   glava_b200_framebuffer_ipc(glava_b200* r, void* handle, size_t handle_byte
  *                              (64 + 876/255 Y', 512 + 896/255 P).  Both: the JFIF encoding JPEG encoders take (nvJPEG's
  *                              YUV input, libjpeg-turbo's raw data, ffmpeg's yuvj420p).  Every grey has Cb = Cr = 128
  *                              (512).  RGBA / BGRA with either bit are GLAVA_B200_EINVAL (no matrix or range).
+ *   GLAVA_B200_EXPORT_PQ, GLAVA_B200_EXPORT_HLG   (P010, YUV420P10, YUV444P10 and YUV422P10 only) BT.2020 non-constant-
+ *                              luminance Y'CbCr, limited range, with the PQ (SMPTE ST 2084, HDR10) or HLG (ITU-R BT.2100)
+ *                              transfer: each R'G'B' colour is shown as SDR graphics at BT.2408's 203 cd/m^2 (BT.1886
+ *                              linearisation, BT.709 -> BT.2020 primaries, HLG through the inverse OOTF of a 1000 cd/m^2
+ *                              display), so white is Y 573 (PQ) or 721 (HLG) and no channel exceeds 203 cd/m^2: MaxCLL
+ *                              <= 203 for the stream's HDR10 metadata (DESIGN.md §4.22).  Both bits together, either with
+ *                              EXPORT_FULL_RANGE, EXPORT_BT601 or EXPORT_STRAIGHT, or on any other format are
+ *                              GLAVA_B200_EINVAL.  Byte counts do not depend on them.
  *   dst[i], pitch and uv_offset are multiples of 16, pitch >= the row bytes, uv_offset (when set) >= pitch * h (planar
  *   formats: >= one chroma plane).  An unknown format or flag, odd NV12 / I420 / P010 / YUV420P10 dimensions, an odd
  *   YUV422P / YUV422P10 / UYVY width, a misaligned or short pitch (I420, YUV420P10, YUV422P, YUV422P10: not a multiple of
@@ -456,11 +464,13 @@ int   glava_b200_framebuffer_ipc(glava_b200* r, void* handle, size_t handle_byte
 #define GLAVA_B200_EXPORT_STRAIGHT 0x4u
 #define GLAVA_B200_EXPORT_FULL_RANGE 0x100u
 #define GLAVA_B200_EXPORT_BT601 0x200u
+#define GLAVA_B200_EXPORT_PQ 0x800u
+#define GLAVA_B200_EXPORT_HLG 0x1000u
 typedef struct {
     int      format;            /* GLAVA_B200_EXPORT_RGBA / _BGRA / _NV12 / _I420 / _YUV444 / _P010 / _YUV420P10 /
                                    _YUV444P10 / _YUV422P / _YUV422P10 / _UYVY / _YUVA420P / _YUVA444P10 */
     uint32_t flags;             /* GLAVA_B200_EXPORT_OVER or (RGBA / BGRA) _STRAIGHT, and for the Y'CbCr formats
-                                   _FULL_RANGE / _BT601 */
+                                   _FULL_RANGE / _BT601, or for the 10-bit ones _PQ / _HLG */
     uint8_t  background[4];     /* R, G, B of the opaque background the composite uses; byte 3 unused */
     size_t   pitch;             /* bytes from one output row to the next (every plane; I420 / YUV420P10 / YUV422P /
                                    YUV422P10 chroma rows: pitch / 2) */
@@ -592,6 +602,12 @@ int glava_b200_overlay_frames(glava_b200* r, const int* streams, int count, void
  *   sample is written with its other bits zero; a sample no non-zero pixel covers (a luma sample under a zero pixel, a chroma
  *   sample whose pixel or 2x2 block is all zero) keeps all 16 bits, and rows the marks skip and all-zero quads are neither
  *   read nor written.  Under any other opacity every sample of the rectangle gets glava_b200_export_frames' bytes.
+ *   HDR pictures (DESIGN.md §4.22): EXPORT_PQ or EXPORT_HLG on P010, YUV420P10, YUV444P10 or YUV422P10 says the picture is
+ *   BT.2020 PQ / HLG limited range; the blend then takes each pixel's straight colour S in the HDR export's arithmetic, Y =
+ *   round((a Y_f(S) + (255 - a) Y_D) / 255) and chroma round(512 + sum a_i (C_f(S_i) - 512) / (255 n) + (1 - A / (255 n))
+ *   (C_D - 512)) over the n pixels of a block / pair / pixel, so graphics land at 203 cd/m^2, an opaque pixel gives the HDR
+ *   export's codes and zero pixels keep every bit.  Either bit on another format, both, or with EXPORT_FULL_RANGE /
+ *   EXPORT_BT601 is GLAVA_B200_EINVAL; glava_b200_overlay_frames takes neither.
  *   GLAVA_B200_EINVAL, with nothing enqueued, for: a null argument, count < 1, an unbuilt renderer; RGBA, BGRA (those go to
  *   glava_b200_overlay_frames) or an unknown format; any other flag; odd w or h for the 4:2:0 formats, odd w for the 4:2:2
  *   ones; a pitch or chroma_pitch that is not a multiple of 16 or below the plane's row bytes (luma w, 2w at 10 bits and
@@ -607,7 +623,8 @@ typedef struct { void* plane[3]; } glava_b200_picture;
 typedef struct {
     int      format;        /* GLAVA_B200_EXPORT_NV12, _I420, _YUV444, _P010, _YUV420P10, _YUV444P10, _YUV422P,
                                _YUV422P10, _UYVY */
-    uint32_t flags;         /* 0, or GLAVA_B200_EXPORT_FULL_RANGE / GLAVA_B200_EXPORT_BT601 */
+    uint32_t flags;         /* 0, or GLAVA_B200_EXPORT_FULL_RANGE / GLAVA_B200_EXPORT_BT601, or (10-bit formats)
+                               GLAVA_B200_EXPORT_PQ / GLAVA_B200_EXPORT_HLG */
     size_t   pitch;         /* bytes between luma rows */
     size_t   chroma_pitch;  /* bytes between rows of every chroma plane */
 } glava_b200_overlay_planes_desc;
